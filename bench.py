@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py -- BBBAlexNet forward + KL images/sec on B200 (BASELINE.json metric).
+"""bench.py -- BBBAlexNet forward + KL images/sec on H100 (BASELINE.json metric).
 
-    python bench.py [--gpus N --steps K --warmup W] [--impl reference]
+    python bench.py [--gpus N --steps K --warmup W] [--impl reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 One "step" = one pass of the hot path over one synthetic batch: BBBAlexNet
@@ -12,8 +12,14 @@ is the shard axis: rank r runs sample r of the SAME batch and one NCCL all-reduc
 combines sum_j softmax_j and the KL (SURVEY.md 8e) -> weak scaling, value =
 B * N * K / t.
 
-Printed JSON (rank 0, one line): the driver contract + `roofline`, `cpu_baseline`,
-`e2e`, `clocks`, `gpu_launches`, `per_layer`.
+Printed JSON (rank 0, one line): metric, value, unit, steps + `roofline`, `cpu_baseline`,
+`e2e`, `clocks`, `gpu_launches`, `per_layer`.  Every timed figure is one window of
+exactly --steps steps unless --windows asks for more.
+
+--dump-outputs DIR writes what the last timed step of the headline arm returned
+(mc.MCForward's outputs: log_outputs [B, C], kl, ...) as DIR/<name>.npy in float32.
+Inputs, parameters and noise seeds are fixed, so two builds run with the same
+arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -43,7 +49,8 @@ def peaks():
         d = json.load(open(p))
         return {"hbm_gbs": d["hbm_gbs"], "tf_burst": d["bf16_tflops"], "tf_sustained": d["bf16_tflops_sustained"],
                 "source": "measured (MEASURED_PEAKS.json)"}
-    return {"hbm_gbs": 6650.0, "tf_burst": 1590.0, "tf_sustained": 1400.0, "source": "fallback (B200_PROFILING.md)"}
+    return {"hbm_gbs": 3350.0, "tf_burst": 989.0, "tf_sustained": 989.0,
+            "source": "NVIDIA H100 SXM data sheet (700 W, dense bf16): not measured"}
 
 
 # --------------------------------------------------------------------------- #
@@ -186,9 +193,8 @@ def run_ours(args):
         if world == 1 and args.gpus > 1:
             raise SystemExit("launch with torch.distributed.run for --gpus > 1")
     numa = pin_to_gpu_numa_node(local)
-    # The GPU arms do no CPU math: keep the OpenMP pool at one thread, as torch.distributed.run does for N > 1.  Measured
-    # (tools/e2e_probe.py, profiles/r2_e2e_probe.txt): with 64 idle-spinning OpenMP workers the pinned H2D path dropped from
-    # 53.5 to 17-26 GB/s and the N=1 end-to-end figure was half of one rank's at N=2.  The CPU baseline leg sets its own count.
+    # The GPU arms do no CPU math: keep the OpenMP pool at one thread, as torch.distributed.run does for N > 1 -- idle-spinning
+    # OpenMP workers slow the pinned H2D path of the end-to-end arm (tools/e2e_probe.py).  The CPU baseline leg sets its own count.
     torch.set_num_threads(1)
     torch.cuda.set_device(local)
     dev = torch.device("cuda", local)
@@ -223,10 +229,10 @@ def run_ours(args):
     in_shape = (B, cfg["inputs"], 32, 32)
     in_bytes = B * cfg["inputs"] * 32 * 32 * 4
     n_inputs = 4                                 # pinned host batches (e2e arm)
-    n_dev_inputs = max(2, -(-(160 << 20) // in_bytes))   # device-resident arm rotates through > 126 MB (L2) of inputs
+    n_dev_inputs = max(2, -(-(160 << 20) // in_bytes))   # device-resident arm rotates through > 50 MB (L2) of inputs
     x_host = [torch.randn(*in_shape, generator=gx).pin_memory() for _ in range(n_inputs)]
     x_dev = [torch.randn(*in_shape, device=dev) for _ in range(n_dev_inputs)]
-    # The step = the package's public MC step (mc.MCForward): this rank's samples through the engine (fused tcgen05 chain),
+    # The step = the package's public MC step (mc.MCForward): this rank's samples through the engine (fused wgmma chain),
     # then ONE kernel that combines them, exchanges the partials with the other ranks over NVLink and finishes
     # logmeanexp / KL (/ uncertainty) on the device -- all in one captured CUDA graph per resident input batch.
     # overlap=True: the exchange kernel of step t runs on its own stream beside the first kernels of step t+1 (the windows
@@ -278,6 +284,8 @@ def run_ours(args):
     wall0 = time.perf_counter()
     wins = [window(resident, args.steps) for _ in range(args.windows)]
     wall = time.perf_counter() - wall0
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, eng.out)
     total_ms = statistics.median(wins)
     images_per_step = B * S_total                # image-samples of the whole job per step (SURVEY 8d: B*S/t)
     value = images_per_step * args.steps / (total_ms * 1e-3)
@@ -316,7 +324,7 @@ def run_ours(args):
             main.wait_stream(eng_e2e.result_stream)
 
     window(e2e_steps, max(3, args.warmup))
-    e2e_wins = [window(e2e_steps, args.steps) for _ in range(max(5, args.windows // 3))]
+    e2e_wins = [window(e2e_steps, args.steps) for _ in range(args.windows)]
     e2e_ms = statistics.median(e2e_wins)
     e2e_value = images_per_step * args.steps / (e2e_ms * 1e-3)
     clocks = sampler.stop() if rank == 0 else None
@@ -333,7 +341,7 @@ def run_ours(args):
                 counter[0] += 1
 
         window(resident_serial, args.warmup)
-        s_wins = [window(resident_serial, args.steps) for _ in range(max(5, args.windows // 3))]
+        s_wins = [window(resident_serial, args.steps) for _ in range(args.windows)]
         s_ms = statistics.median(s_wins)
         serial = {"ms_per_step": s_ms / args.steps, "value": images_per_step * args.steps / (s_ms * 1e-3), "unit": "images/s",
                   "note": "one step in flight, exchange kernel inside the step's graph (the step latency); the headline value "
@@ -428,8 +436,8 @@ def run_ours(args):
         tw = [window(tsteps, args.train_steps) for _ in range(3)]
         tms = statistics.median(tw) / args.train_steps
         train = {"value": images_per_step / (tms * 1e-3), "unit": "images/s", "ms_per_step": tms,
-                 "what": "forward (tcgen05 layer kernels, autograd on: no fused chain) + backward (wgrad / dgrad as role-swapped "
-                         "tcgen05 layer calls, eps regenerated from Philox; BBB_B200_BWD=simt selects the fp32 CUDA-core "
+                 "what": "forward (wgmma layer kernels, autograd on: no fused chain) + backward (wgrad / dgrad as role-swapped "
+                         "wgmma layer calls, eps regenerated from Philox; BBB_B200_BWD=simt selects the fp32 CUDA-core "
                          "kernels) + MC exchange/ELBO kernel + one gradient all-reduce + Adam; eager launches (no graph)"}
         ts.close()
 
@@ -449,7 +457,7 @@ def run_ours(args):
                                         "single-launch S=10 figure is under mc_batched"),
                        "batch": B, "variant": cfg["variant"], "math": args.math, "mc_samples_total": S_total,
                        "parallelism": f"mc{world}", "steps_in_flight": infl, "exchange_overlapped": ovl,
-                       "l2": f"no flush: inputs rotate through {n_dev_inputs} resident batches = {n_dev_inputs * in_bytes >> 20} MB > 126 MB L2",
+                       "l2": f"no flush: inputs rotate through {n_dev_inputs} resident batches = {n_dev_inputs * in_bytes >> 20} MB > 50 MB L2",
                        "launch": ("two CUDA graph replays per step (layer chain: noise advance, per-layer prep + GEMM kernels; then the MC "
                                   "exchange kernel over NVLink peer memory on its own stream, beside the next step's chain)" if ovl else
                                   "one CUDA graph replay per step (noise advance, per-layer prep + GEMM kernels, MC exchange kernel over "
@@ -523,7 +531,7 @@ def in_chain_kernels(net, x, dev, reps=20):
 
 
 def gpu_eager_incumbent(args, dev, reps=12):
-    """SURVEY 8d's same-box incumbent: the reference's op sequence in stock PyTorch eager ON THE B200 (the oracle port's
+    """SURVEY 8d's same-box incumbent: the reference's op sequence in stock PyTorch eager ON THE SAME GPU (the oracle port's
     aten calls with CUDA tensors -- cuDNN conv (TF32 by default, SURVEY D9) + elementwise launches), including what the
     reference does every forward: eps drawn on the CPU generator and copied host->device (BBB/BBBConv.py:63,68)."""
     try:
@@ -546,7 +554,7 @@ def gpu_eager_incumbent(args, dev, reps=12):
             ts.append(time.perf_counter() - t0)
         med = statistics.median(ts)
         return {"value": args.batch / med, "unit": "images/s", "ms_per_step": med * 1e3, "min_ms": min(ts) * 1e3,
-                "what": "oracle port's aten ops on the same B200, eager, incl. per-forward CPU eps draw + H2D copy and the "
+                "what": "oracle port's aten ops on the same GPU, eager, incl. per-forward CPU eps draw + H2D copy and the "
                         "kl.item() sync (reference semantics); wall clock around synchronize"}
     except Exception as e:
         return {"value": None, "note": f"failed: {e}"[:200]}
@@ -630,12 +638,6 @@ def layer_rooflines(net, x, args, pk, flush, reps=20):
                 "unit": "GB/s", "frac": top["mbytes"] / 1e3 / t_k / pk["hbm_gbs"], "traffic": None,
                 "peak_source": pk["source"],
                 "kernel_us": t_k * 1e6, "layer_us_prep_plus_gemm": top["ms"] * 1e3, "layer_frac": top["frac"]}
-    tp = os.path.join(ROOT, "profiles", "r2_ncu_full_traffic.json")      # dram__bytes_read+write of that kernel, one ncu --set full capture
-    if os.path.exists(tp):
-        tj = json.load(open(tp))
-        if tj.get("variant") == args.variant and tj.get("batch") == args.batch and top["name"] in tj["layers"]:
-            roof["traffic"] = tj["layers"][top["name"]]["dram_bytes"]
-            roof["traffic_source"] = tj["source"]
     t_roof = sum(max(algorithmic(r, args.variant, act_b)[0] / (pk["tf_burst"] * 1e12),
                      algorithmic(r, args.variant, act_b)[1] / (pk["hbm_gbs"] * 1e9)) for r in rows)
     roof["net_t_roof_us"] = t_roof * 1e6
@@ -732,6 +734,16 @@ def run_reference(args):
     print(json.dumps(out), flush=True)
 
 
+def dump_outputs(path, outs):
+    """The arrays a caller of the timed step receives, as float32 .npy files (<= 64 MB in all at any batch the bench runs:
+    the largest is log_outputs, B x C)."""
+    import numpy as np
+    os.makedirs(path, exist_ok=True)
+    torch.cuda.synchronize()
+    for name, t in outs.items():
+        np.save(os.path.join(path, f"{name}.npy"), t.detach().float().cpu().numpy())
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -746,7 +758,9 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--mc-batch", type=int, default=10, help="also report S MC samples folded into one launch (LRT; 0 = skip)")
     ap.add_argument("--train-steps", type=int, default=5, help="steps per window of the sharded training-step figure (0 = skip)")
-    ap.add_argument("--windows", type=int, default=25, help="timed windows of --steps steps; the median window is reported")
+    ap.add_argument("--windows", type=int, default=1, help="timed windows of --steps steps; the median window is reported")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's outputs as DIR/<name>.npy (float32)")
     ap.add_argument("--config", default="headline", choices=list(CONFIGS),
                     help="headline (default: BBBAlexNet-10 B=512, one MC sample per GPU per step) or one of BASELINE.json's configs restated")
     args = ap.parse_args()

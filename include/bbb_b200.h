@@ -1,5 +1,5 @@
 /*
- * bbb_b200.h -- C ABI of the B200-native Bayes-by-Backprop layer engine.
+ * bbb_b200.h -- C ABI of the H100-native Bayes-by-Backprop layer engine.
  *
  * The reference (kumar-shridhar/PyTorch-BayesianCNN) has no FFI / plugin layer:
  * its boundary for this path is the Python class surface of layers/ (SURVEY.md
@@ -39,9 +39,9 @@ enum { BBB_VARIANT_BBB = 0,   /* weight-space sampling   (layers/BBB/...)      *
        BBB_VARIANT_LRT = 1 }; /* local reparameterisation (layers/BBB_LRT/...) */
 enum { BBB_DTYPE_F32 = 0, BBB_DTYPE_BF16 = 1 };
 enum { BBB_MATH_FP32 = 0,      /* CUDA-core FFMA, IEEE fp32 accumulate          */
-       BBB_MATH_BF16_TC = 1,   /* tcgen05 bf16 x bf16 -> fp32 in TMEM           */
+       BBB_MATH_BF16_TC = 1,   /* wgmma bf16 x bf16 -> fp32                     */
        BBB_MATH_AUTO = 2,      /* engine picks per layer shape                  */
-       BBB_MATH_TF32_TC = 3 }; /* tcgen05 tf32 x tf32 -> fp32 in TMEM (operands rounded to tf32, 10-bit mantissa: what the
+       BBB_MATH_TF32_TC = 3 }; /* wgmma tf32 x tf32 -> fp32 (operands rounded to tf32, 10-bit mantissa: what the
                                   reference's own GPU conv computes by default, SURVEY D9); per-layer calls only */
 enum { BBB_KL_REFERENCE = 0,   /* as executed by the reference: KL(prior||post) */
        BBB_KL_TEXTBOOK = 1 };  /* KL(q||p)                                      */
@@ -112,7 +112,7 @@ int bbb_linear_forward(const bbb_layer_desc* desc, const void* x,
                        uint64_t seed, uint64_t stream_id, const uint64_t* stream_base,
                        void* workspace, size_t workspace_bytes, void* cuda_stream);
 
-/* Activation layouts of the fused tcgen05 chain (bbb_layer_forward_fused). */
+/* Activation layouts of the fused tensor-core chain (bbb_layer_forward_fused). */
 enum { BBB_LAYOUT_NCHW_F32 = 0,      /* reference layout: [B, C, H, W] fp32                       */
        BBB_LAYOUT_PACKED_BF16 = 1,   /* "tiled packed" bf16: the [B, F] matrix, F = H*W*C, column = (h*W + w)*C + c,
                                         C % 64 == 0, stored as [ceil(B/128)][F/64][128 rows x 128 B] with every 16 KB
@@ -257,8 +257,8 @@ uint64_t bbb_launch_count(void);
 /* Tile policy of the fused chain's tap-GEMM layers (bbb_layer_forward_fused), read at launch (= graph capture) time:
  * 0 (default) = 128-column tiles only where the grid still covers most of the SMs (best latency of ONE step);
  * 1 = 128-column tiles wherever Cout allows (fewer operand bytes per MAC; best throughput when several independent
- * steps are in flight and fill the SMs a narrow grid leaves idle -- measured 63.8 -> 59.5 us per BBBAlexNet step
- * with four steps in flight, 92 -> 97 us for a single step).  Returns the previous value. */
+ * steps are in flight and fill the SMs a narrow grid leaves idle; slower for a single step).  Returns the previous
+ * value. */
 int32_t bbb_set_wide_tiles(int32_t prefer_wide);
 
 #ifdef __cplusplus

@@ -11,7 +11,7 @@ product package never does.
 Parity pin: the reference has NO golden vectors and its only test file does not
 collect (SURVEY.md D4).  The oracle is therefore pinned against outputs of the
 reference itself, run in the build container by ``tests/golden/make_golden.py``
-(imports /root/reference unmodified, replays its CPU-generator eps draws) and
+(imports the original project unmodified, replays its CPU-generator eps draws) and
 committed as ``tests/golden/*.npz``.  ``tests/test_oracle_golden.py`` checks the
 oracle against those fixtures bit-for-bit in fp32.
 
@@ -20,7 +20,7 @@ the restatement uses the same aten calls in the same order so that, given the
 same eps, it is bitwise equal on the same torch build.  A float64 mode is
 offered for tolerance budgeting.
 
-Every function cites the reference file:line (relative to /root/reference).
+Every function cites the reference file:line (relative to the original project's root).
 """
 from __future__ import annotations
 

@@ -1,4 +1,4 @@
-"""B200-native Bayes-by-Backprop layer engine (hot path of kumar-shridhar/PyTorch-BayesianCNN).
+"""H100-native Bayes-by-Backprop layer engine (hot path of kumar-shridhar/PyTorch-BayesianCNN).
 
 Public surface = the reference's ``layers`` exports (layers/__init__.py:1-7) plus the
 engine controls.  The compute lives in libbbb_b200.so (csrc/, C ABI in include/bbb_b200.h).

@@ -42,13 +42,13 @@ int cuda_fail(cudaError_t e, const char* what) {
 constexpr size_t kCounterBytes = 64;
 constexpr size_t kMaxKlSlots = 4096;
 constexpr size_t kBaseWorkspace = kCounterBytes + kMaxKlSlots * sizeof(double);
-constexpr size_t kTcOffset = (kBaseWorkspace + 1023) / 1024 * 1024;   // prepared-operand region (tcgen05 path)
+constexpr size_t kTcOffset = (kBaseWorkspace + 1023) / 1024 * 1024;   // prepared-operand region (tensor-core path)
 
 int sm_count() {
     static int n = 0;
     if (n == 0) {
         int dev = 0; cudaGetDevice(&dev);
-        if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+        if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
     }
     return n;
 }
@@ -80,9 +80,9 @@ int forward_impl(const bbb_layer_desc* d, bool linear, const void* x, const floa
     int math = d->math;
     if (math == BBB_MATH_AUTO) math = bbb::tc_supported(*d, g) ? BBB_MATH_BF16_TC : BBB_MATH_FP32;
     if (math == BBB_MATH_BF16_TC || math == BBB_MATH_TF32_TC) {
-        if (!bbb::tc_supported(*d, g)) return fail(BBB_E_UNSUPPORTED, "tcgen05 math mode: shape not supported by the tcgen05 path");
+        if (!bbb::tc_supported(*d, g)) return fail(BBB_E_UNSUPPORTED, "tensor-core math mode: shape not supported by the tensor-core path");
         const size_t need = kTcOffset + bbb::tc_workspace_bytes(g);
-        if (!ws || ws_bytes < need) return fail(BBB_E_WORKSPACE, "workspace too small for the tcgen05 path: need %zu bytes", need);
+        if (!ws || ws_bytes < need) return fail(BBB_E_WORKSPACE, "workspace too small for the tensor-core path: need %zu bytes", need);
         bbb::TcArgs a;
         a.wtiles = (__nv_bfloat16*)((char*)ws + kTcOffset);
         a.tf32 = math == BBB_MATH_TF32_TC;
@@ -204,7 +204,7 @@ int bbb_linear_backward(const bbb_layer_desc* desc, const void* x, const void* g
 static int fused_check(const bbb_layer_desc* d, bbb::Geom& g, int32_t in_layout, int32_t in_pitch, int32_t prev_hw,
                        int32_t out_layout, int32_t out_pitch) {
     if (int rc = check_desc(d, g, false)) return rc;
-    if (d->math == BBB_MATH_FP32 || d->math == BBB_MATH_TF32_TC) return fail(BBB_E_UNSUPPORTED, "the fused chain exists on the tcgen05 (bf16) path only");
+    if (d->math == BBB_MATH_FP32 || d->math == BBB_MATH_TF32_TC) return fail(BBB_E_UNSUPPORTED, "the fused chain exists on the tensor-core (bf16) path only");
     const int pool = d->pool_k != 0;
     if (pool && !(d->pool_k == 2 && d->pool_s == 2)) return fail(BBB_E_UNSUPPORTED, "only a 2x2 stride-2 max-pool can be fused");
     if (pool && ((g.OH | g.OW) & 1)) return fail(BBB_E_UNSUPPORTED, "fused pool needs even output height/width");
@@ -212,7 +212,7 @@ static int fused_check(const bbb_layer_desc* d, bbb::Geom& g, int32_t in_layout,
         return fail(BBB_E_INVALID, "tiled packed output needs Cout %% 64 == 0 and out_pitch == pixels*Cout (got %d)", out_pitch);
     const int out_mode = out_layout == BBB_LAYOUT_PACKED_BF16 ? 0 : (out_layout == BBB_LAYOUT_ROWMAJOR_F32 ? 1 : 2);
     if (in_layout == BBB_LAYOUT_NCHW_F32) {
-        if (!bbb::tc_supported(*d, g)) return fail(BBB_E_UNSUPPORTED, "shape not supported by the tcgen05 gather path");
+        if (!bbb::tc_supported(*d, g)) return fail(BBB_E_UNSUPPORTED, "shape not supported by the tensor-core gather path");
         if (out_mode == 1 && (pool ? g.OHW / 4 : g.OHW) != 1) return fail(BBB_E_UNSUPPORTED, "row-major fp32 output needs a 1x1 map on the gather path");
     } else if (in_layout == BBB_LAYOUT_PACKED_BF16) {
         if (!bbb::fused_supported(g, pool)) return fail(BBB_E_UNSUPPORTED, "shape not supported by the fused tap-GEMM path");

@@ -98,8 +98,7 @@ __device__ __forceinline__ float4 normal4(uint64_t grp, const NoiseKey& k) {
 
 // the normal of one element (tiling independent: same value whoever asks).
 // Deliberately NOT inlined: ~110 SASS instructions per copy, and the kernels that call it
-// are instruction-cache bound when it is replicated at every unrolled call site (ncu:
-// stall_no_instructions dominated the first tcgen05 kernels).
+// are instruction-cache bound when it is replicated at every unrolled call site.
 __device__ __noinline__ float normal1(uint64_t idx, const NoiseKey k) {
     const uint4 r = philox4x32_10(make_uint4((uint32_t)(idx >> 2), (uint32_t)(idx >> 34), k.stream_lo, k.stream_hi),
                                   make_uint2(k.seed_lo, k.seed_hi));

@@ -9,25 +9,25 @@
 // K-major SWIZZLE_32B canonical layout, so an M=128 x K=16 operand (16 images x 8 output columns; 4 input pixels x 4
 // channels) is ONE shared-memory descriptor: start = (kernel row, 4-pixel group), 8-row-group stride = image pitch.
 // The windows of neighbouring output pixels overlap in memory; that is fine because the hardware applies the swizzle
-// XOR to the absolute shared-memory address (measured: tools/sw32_probe.cu, 66/66 window positions exact), so the image
+// XOR to the absolute shared-memory address (the bf16 parity tests of the fused chain check it), so the image
 // is simply stored at swizzle(address).  K order = (kernel row r, window pixel j = s+1, channel c): per kernel row 12
 // pixels x 4 channels = 48 = three K16 MMAs, the padding slots (s = -1, c = 3) carry zero weights.
 //
 //   CTA  = 16 images x one PAIR of output rows (2*ohp, 2*ohp+1) x all 8 output columns x 64 output channels:
-//          four TMEM accumulators [row of the pair][mean | variance] x 64 columns; both rows of a pool window live in
+//          four accumulators [row of the pair][mean | variance] x 64 columns; both rows of a pool window live in
 //          the same CTA, and the weight stages are used twice.  grid = ceil(B/16) x OH/2 (AlexNet B=512: 128 CTAs).
-//   warps 0-7 : stage the images (coalesced float4 loads, bf16 x and x^2, swizzled 16-byte stores), then draw the
-//               tile's LRT noise (Philox, 64 normals per thread, registers) WHILE the tensor core works, then the
-//               epilogue: tcgen05.ld, bias, sqrt(var)*eps, 2x2 max (registers + one lane shuffle), activation, stores
-//   warp 8    : tcgen05.mma issuer (12 MMAs per kernel row), tcgen05.commit
-//   warp 9    : weight producer: one 6/12 KB cp.async.bulk per kernel row into a 4-stage mbarrier ring
+//   warps 0-7 : stage the images (coalesced float4 loads, bf16 x and x^2, swizzled 16-byte stores); then warpgroup h
+//               issues the wgmma of tile rows [64h, 64h + 64) = images [8h, 8h + 8) (12 per kernel row, fp32
+//               accumulators in registers); then the epilogue through shared memory: bias, sqrt(var)*eps with the
+//               LRT noise drawn in place, 2x2 max (one lane shuffle), activation, stores
+//   warp 8    : weight producer: one 6/12 KB cp.async.bulk per kernel row into a 3-stage mbarrier ring
 // The parameter-only half (sigma, eps, bf16 operand tiles in the K order above, KL) is conv_s4_prep_kernel.
 #pragma once
 #include "fused_tc.cuh"      // bf16x2_sq, tiled activation format
 
 namespace bbb {
 
-constexpr int S4_IMGS = 16, S4_WIN_PX = 12, S4_KROW = 48, S4_THREADS = 320;
+constexpr int S4_IMGS = 16, S4_WIN_PX = 12, S4_KROW = 48, S4_THREADS = 288;
 // weight ring depth: three 12 KB stages keep the CTA at ~193 KB, so that one weight-prep CTA of a later layer (<= 26 KB,
 // launch_fused) can share the SM -- with four stages every prep CTA kept a conv_s4 CTA off its SM until it had drained
 constexpr int S4_STAGES = 3;
@@ -131,15 +131,18 @@ conv_s4_prep_kernel(const S4Args p) {
 
 // ------------------------------------------------------------------ (G) conv
 struct S4Smem {
-    unsigned long long full[S4_STAGES], empty[S4_STAGES], accum, img_ready[2];
-    uint32_t tmem_base, pad;
+    unsigned long long full[S4_STAGES], empty[S4_STAGES], img_ready[2];
     float bias[64], bvar[64];
 };
 
-// K-major SWIZZLE_32B descriptor: rows 32 B apart, 8-row groups `sbo` bytes apart (layout type 6, version 1)
+// K-major SWIZZLE_32B wgmma descriptor: rows 32 B apart, 8-row groups `sbo` bytes apart (layout type 3 at [62,64))
 __device__ __forceinline__ uint64_t make_smem_desc_sw32(uint32_t saddr, uint32_t sbo_bytes) {
-    return (uint64_t)((saddr & 0x3FFFFu) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)(sbo_bytes >> 4) << 32) | (1ull << 46) | (6ull << 61);
+    return (uint64_t)((saddr & 0x3FFFFu) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)(sbo_bytes >> 4) << 32) | (3ull << 62);
 }
+// shared memory of the four accumulator tiles ([row of the pair][mean | variance], 128 rows of 64 + 4 floats), staged
+// over the weight ring and the images once the main loop is done
+constexpr int S4_AP = 64 + 4;
+__host__ __device__ constexpr size_t s4_acc_bytes(int planes) { return (size_t)2 * planes * 128 * S4_AP * 4; }
 __device__ __forceinline__ uint32_t sw32(uint32_t addr) { return addr ^ (((addr >> 7) & 1u) << 4); }
 template <int VARIANT>
 __global__ void __launch_bounds__(S4_THREADS, 1)
@@ -167,57 +170,29 @@ conv_s4_kernel(const S4Args p) {
     tl_enter(p.tl_gemm);
     pdl_trigger();
     if (threadIdx.x == 0) {
-        for (int s = 0; s < S4_STAGES; ++s) { mbar_init(smem_u32(&ctl->full[s]), 1); mbar_init(smem_u32(&ctl->empty[s]), 1); }
-        mbar_init(smem_u32(&ctl->accum), 1);
+        for (int s = 0; s < S4_STAGES; ++s) { mbar_init(smem_u32(&ctl->full[s]), 1); mbar_init(smem_u32(&ctl->empty[s]), 8); }
         mbar_init(smem_u32(&ctl->img_ready[0]), 256);
         mbar_init(smem_u32(&ctl->img_ready[1]), 256);
         fence_barrier_init();
     }
-    const uint32_t tmem_cols = (two && !p.eps_a) ? 512u : (two ? 256u : 128u);      // accumulators (+ the LRT noise tile)
-    if (warp == 8) tmem_alloc(smem_u32(&ctl->tmem_base), tmem_cols);
     // No CTA-wide griddepcontrol.wait: the programmatic predecessor is this layer's weight-prep kernel (which has itself
-    // waited for everything before it), and staging the images needs nothing it writes.  Only the weight producer (warp 9:
+    // waited for everything before it), and staging the images needs nothing it writes.  Only the weight producer (warp 8:
     // operand tiles, bias) and the workers' noise/epilogue (Philox base, output buffers) wait -- the image staging of all
     // CTAs overlaps the prep kernel.
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = ctl->tmem_base;
     if (tr && threadIdx.x == 0) tr[1] = clock64();
 
     if (warp < 8) {
-        // ================= (1) stage the images, (2) draw the LRT noise -- interleaved =============================
-        // Both are latency problems (global loads / the serial Philox rounds), so each staging batch issues its loads,
-        // then a slice of the noise is computed while they are in flight, then the batch is converted and stored.
+        // ================= (1) stage the images ====================================================================
+        // Each staging batch issues its loads for several (image, row) pairs at once, then converts and stores them.
+        // The LRT noise is drawn later, in the epilogue (4).
         const int t = threadIdx.x;
-        const int m = (warp & 3) * 32 + lane, half = warp >> 2;            // TMEM lane == tile row; 32 of the 64 columns
+        const int m = (warp & 3) * 32 + lane, half = warp >> 2;            // tile row; 32 of the 64 columns
         const int mi = m >> 3, ow = m & 7, b = img0 + mi;
         const bool bvalid = b < g.B;
         const bool philox = two && !p.eps_a;
-        // Noise goes to TENSOR MEMORY (columns behind the accumulators, this thread's lane): 64 values per thread would
-        // otherwise pin 64 registers and force the epilogue to be fully unrolled (register arrays cannot be indexed by a
-        // loop counter) -- straight-line code executed once per CTA, which is what the cold instruction cache punishes.
-        const uint32_t lane_base = tmem + ((uint32_t)((warp & 3) * 32) << 16) + (uint32_t)(half * 32);
-        const uint32_t noise_col = 256u;
         int b_s = b;                                                        // image index inside its MC sample
         NoiseKey nkey = p.key;                                              // completed after griddepcontrol.wait (reads the stream base)
-        auto noise_slice = [&](int it) {                                    // 16 of this thread's 64 normals: 4 independent Philox chains
-            const int ohl = it >> 1, k16 = it & 1;
-            float z[16];
-            if (bvalid) {
-                const uint64_t g0 = (((uint64_t)b_s * g.OHW + (uint64_t)((2 * ohp + ohl) * g.OW + ow)) * g.N + half * 32 + k16 * 16) >> 2;
-                const float4 za = normal4(g0, nkey), zb = normal4(g0 + 1, nkey), zc = normal4(g0 + 2, nkey), zd = normal4(g0 + 3, nkey);
-                z[0] = za.x; z[1] = za.y; z[2] = za.z; z[3] = za.w; z[4] = zb.x; z[5] = zb.y; z[6] = zb.z; z[7] = zb.w;
-                z[8] = zc.x; z[9] = zc.y; z[10] = zc.z; z[11] = zc.w; z[12] = zd.x; z[13] = zd.y; z[14] = zd.z; z[15] = zd.w;
-            } else {
-#pragma unroll
-                for (int j = 0; j < 16; ++j) z[j] = 0.0f;
-            }
-            const float (&lo)[8] = *reinterpret_cast<const float (*)[8]>(&z[0]);
-            const float (&hi)[8] = *reinterpret_cast<const float (*)[8]>(&z[8]);
-            tmem_st8(lane_base + noise_col + (uint32_t)(ohl * 64 + k16 * 16), lo);
-            tmem_st8(lane_base + noise_col + (uint32_t)(ohl * 64 + k16 * 16 + 8), hi);
-        };
 
         const int groups = g.W >> 2;                                        // float4 groups per input row
         const int n_rows = S4_IMGS * p.rows;                                // staged rows of the tile (image-major)
@@ -241,7 +216,7 @@ conv_s4_kernel(const S4Args p) {
         const size_t chw = (size_t)g.Cin * g.HW;
         const int split = min(p.rows, 2 * g.SH);
         constexpr int SB = 4;                                               // (image, row) pairs in flight per thread: 12 independent 16-byte loads
-        int nit = 0, nslice = 0;
+        int nit = 0;
 #pragma unroll 1
         for (int batch = 0; batch < 2; ++batch) {
             const int lr0 = batch ? split : 0, nb = batch ? p.rows - split : split;   // rows of this batch
@@ -290,16 +265,63 @@ conv_s4_kernel(const S4Args p) {
         if (tr && threadIdx.x == 0) tr[2] = clock64();
         pdl_wait();                                                         // Philox base / output buffers: everything before this launch is complete
         nkey = fold_key(effective_key(p.key, p.stream_base), p.fold, b, b_s);
-        if (philox) {
-#pragma unroll 1
-            for (; nslice < 4; ++nslice) noise_slice(nslice);                        // the rest, while the tensor core works
-            tmem_st_wait();
-        }
         if (tr && threadIdx.x == 0) tr[3] = clock64();
 
-        // ================= (3) epilogue ===========================================================================
-        mbar_wait(smem_u32(&ctl->accum), 0u);
-        tc_fence_after();
+        // ================= (3) MMA: warpgroup `half` owns tile rows [64 half, 64 half + 64) = images [8 half, 8 half + 8)
+        // Descriptors are linear in their 16-byte address field: build the four A bases and the B base once, step them
+        // by constants per kernel row, and add immediates per MMA.
+        float acc[2][2][32];                                                 // [output row of the pair][mean | variance]
+#pragma unroll
+        for (int i = 0; i < 32; ++i) { acc[0][0][i] = 0.0f; acc[0][1][i] = 0.0f; acc[1][0][i] = 0.0f; acc[1][1][i] = 0.0f; }
+        {
+            const uint32_t arow_step = rowb >> 4;                            // one kernel row further down the staged image
+            const uint32_t wg_off = (uint32_t)half * 8u * imgb;              // 8 images = 8 core-matrix row groups
+            uint64_t dA[2][2];                                               // [output row of the pair][x | x^2], kernel row 0
+#pragma unroll
+            for (int ohl = 0; ohl < 2; ++ohl) {
+                dA[ohl][0] = make_smem_desc_sw32(imgx + wg_off + (uint32_t)(ohl * g.SH) * rowb, imgb);
+                dA[ohl][1] = make_smem_desc_sw32(imgx2 + wg_off + (uint32_t)(ohl * g.SH) * rowb, imgb);
+            }
+            const uint64_t dB0 = make_smem_desc(ring, 1024u, 128u);
+            const int split = min(p.rows, 2 * g.SH);
+            mbar_wait(smem_u32(&ctl->img_ready[0]), 0u);
+#pragma unroll 1
+            for (int r = 0; r < g.KH; ++r) {
+                const int s = r % S4_STAGES;
+                if (r + g.SH == split) mbar_wait(smem_u32(&ctl->img_ready[1]), 0u);   // staged row r + 4 belongs to the second batch
+                mbar_wait(smem_u32(&ctl->full[s]), (uint32_t)(r / S4_STAGES) & 1u);
+                if (tr && threadIdx.x == 0) tr[8 + r] = clock64();
+                const uint64_t db = dB0 + (uint64_t)(((uint32_t)s * stage_bytes) >> 4);
+                const uint32_t acc_on = r ? 1u : 0u;
+                wgmma_fence();
+#pragma unroll
+                for (int kc = 0; kc < 3; ++kc) {
+                    wgmma_m64n64k16_bf16(acc[0][0], dA[0][0] + 2 * kc, db + 128 * kc, acc_on | kc);
+                    wgmma_m64n64k16_bf16(acc[1][0], dA[1][0] + 2 * kc, db + 128 * kc, acc_on | kc);
+                    if (two) {
+                        wgmma_m64n64k16_bf16(acc[0][1], dA[0][1] + 2 * kc, db + (S4_BPLANE >> 4) + 128 * kc, acc_on | kc);
+                        wgmma_m64n64k16_bf16(acc[1][1], dA[1][1] + 2 * kc, db + (S4_BPLANE >> 4) + 128 * kc, acc_on | kc);
+                    }
+                }
+                wgmma_commit();
+                wgmma_wait<1>();                                             // kernel row r - 1 retired: its stage may be refilled
+                if (r > 0 && lane == 0) mbar_arrive(smem_u32(&ctl->empty[(r - 1) % S4_STAGES]));
+                dA[0][0] += arow_step; dA[0][1] += arow_step; dA[1][0] += arow_step; dA[1][1] += arow_step;
+            }
+            wgmma_wait<0>();
+        }
+        if (tr && threadIdx.x == 0) tr[4] = clock64();
+
+        // ================= (4) epilogue ===========================================================================
+        // accumulators -> shared memory over the ring and the images (both consumed), then one tile row per thread
+        float* accs = reinterpret_cast<float*>(sm + (ring - base));
+        bar_sync(1, 256);
+#pragma unroll
+        for (int ohl = 0; ohl < 2; ++ohl) {
+            acc_to_smem(acc[ohl][0], accs + ((ohl * p.planes) * 128 + half * 64) * S4_AP, S4_AP);
+            if (two) acc_to_smem(acc[ohl][1], accs + ((ohl * 2 + 1) * 128 + half * 64) * S4_AP, S4_AP);
+        }
+        bar_sync(1, 256);
         if (tr && threadIdx.x == 0) tr[5] = clock64();
         // the other column of the 2x2 window lives in the neighbouring lane; after the shuffle both lanes hold the pooled
         // value: the even lane stores y, the odd lane y^2 (act is monotone: act(max) == max(act))
@@ -313,13 +335,18 @@ conv_s4_kernel(const S4Args p) {
 #pragma unroll
             for (int ohl = 0; ohl < 2; ++ohl) {
                 float am[8];
-                tmem_ld8_nowait(lane_base + (uint32_t)(ohl * p.planes * 64 + c8 * 8), am);
+                ld_row8(accs + ((ohl * p.planes) * 128 + m) * S4_AP + n0, am);
                 if (two) {
                     float av[8], e8[8];
-                    tmem_ld8_nowait(lane_base + (uint32_t)(ohl * 128 + 64 + c8 * 8), av);
-                    if (philox) tmem_ld8_nowait(lane_base + noise_col + (uint32_t)(ohl * 64 + c8 * 8), e8);
-                    tmem_ld_wait();
-                    if (!philox) {
+                    ld_row8(accs + ((ohl * 2 + 1) * 128 + m) * S4_AP + n0, av);
+                    if (philox) {
+                        float4 za = make_float4(0.f, 0.f, 0.f, 0.f), zb = za;
+                        if (bvalid) {
+                            const uint64_t g0 = (((uint64_t)b_s * g.OHW + (uint64_t)((2 * ohp + ohl) * g.OW + ow)) * g.N + n0) >> 2;
+                            za = normal4(g0, nkey); zb = normal4(g0 + 1, nkey);
+                        }
+                        e8[0] = za.x; e8[1] = za.y; e8[2] = za.z; e8[3] = za.w; e8[4] = zb.x; e8[5] = zb.y; e8[6] = zb.z; e8[7] = zb.w;
+                    } else {
 #pragma unroll
                         for (int j = 0; j < 8; ++j)
                             e8[j] = bvalid ? __ldg(p.eps_a + ((size_t)b * g.N + n0 + j) * g.OHW + (2 * ohp + ohl) * g.OW + ow) : 0.0f;
@@ -330,7 +357,6 @@ conv_s4_kernel(const S4Args p) {
                         am[j] = am[j] + ctl->bias[n0 + j] + fast_sqrt(var) * e8[j];
                     }
                 } else {
-                    tmem_ld_wait();
 #pragma unroll
                     for (int j = 0; j < 8; ++j) am[j] += ctl->bias[n0 + j];
                 }
@@ -352,64 +378,10 @@ conv_s4_kernel(const S4Args p) {
             }
         }
         if (tr && threadIdx.x == 0) tr[6] = clock64();
-        tc_fence_before();
-    } else if (warp == 8) {
-        // ================= MMA issuer ================================================================================
-        // One thread issues every MMA, so the instructions BETWEEN two tcgen05.mma are the main loop's critical path
-        // (measured: ~20 dependent ALU instructions per MMA for descriptor arithmetic = ~115 cycles per 32-cycle MMA).
-        // Descriptors are linear in their 16-byte address field: build the four A bases and the B base once, step them
-        // by constants per kernel row, and add immediates per MMA.
-        constexpr uint32_t idesc = make_idesc_bf16(128, 64);
-        const uint32_t arow_step = rowb >> 4;                                // one kernel row further down the staged image
-        uint64_t dA[2][2];                                                   // [output row of the pair][x | x^2], kernel row 0
-#pragma unroll
-        for (int ohl = 0; ohl < 2; ++ohl) {
-            dA[ohl][0] = make_smem_desc_sw32(imgx + (uint32_t)(ohl * g.SH) * rowb, imgb);
-            dA[ohl][1] = make_smem_desc_sw32(imgx2 + (uint32_t)(ohl * g.SH) * rowb, imgb);
-        }
-        const uint64_t dB0 = make_smem_desc(ring, 1024u, 128u);
-        const uint32_t acc1 = (uint32_t)(p.planes * 64);                     // accumulators of the second output row
-        const int split = min(p.rows, 2 * g.SH);
-        __syncwarp();
-        mbar_wait(smem_u32(&ctl->img_ready[0]), 0u);
-        tc_fence_after();
-#pragma unroll 1
-        for (int r = 0; r < g.KH; ++r) {
-            const int s = r % S4_STAGES;
-            if (r + g.SH == split) {                                        // staged row r + 4 belongs to the second batch
-                __syncwarp();
-                mbar_wait(smem_u32(&ctl->img_ready[1]), 0u);
-                tc_fence_after();
-            }
-            __syncwarp();                                                   // converged whole-warp wait (DESIGN.md: single-lane waits wake late)
-            mbar_wait(smem_u32(&ctl->full[s]), (uint32_t)(r / S4_STAGES) & 1u);
-            tc_fence_after();
-            if (tr && lane == 0) tr[8 + r] = clock64();
-            if (lane == 0) {
-                const uint64_t db = dB0 + (uint64_t)(((uint32_t)s * stage_bytes) >> 4);
-                const uint32_t acc = r ? 1u : 0u;
-#pragma unroll
-                for (int kc = 0; kc < 3; ++kc) {
-                    umma_bf16(tmem, dA[0][0] + 2 * kc, db + 128 * kc, idesc, (acc | kc) ? 1u : 0u);
-                    umma_bf16(tmem + acc1, dA[1][0] + 2 * kc, db + 128 * kc, idesc, (acc | kc) ? 1u : 0u);
-                    if (two) {
-                        umma_bf16(tmem + 64u, dA[0][1] + 2 * kc, db + (S4_BPLANE >> 4) + 128 * kc, idesc, (acc | kc) ? 1u : 0u);
-                        umma_bf16(tmem + 192u, dA[1][1] + 2 * kc, db + (S4_BPLANE >> 4) + 128 * kc, idesc, (acc | kc) ? 1u : 0u);
-                    }
-                }
-                umma_commit(smem_u32(&ctl->empty[s]));
-                if (r == g.KH - 1) umma_commit(smem_u32(&ctl->accum));
-                if (tr) tr[24 + r] = clock64();
-                dA[0][0] += arow_step; dA[0][1] += arow_step; dA[1][0] += arow_step; dA[1][1] += arow_step;
-            }
-            __syncwarp();
-        }
-        if (tr && lane == 0) tr[4] = clock64();
-        tc_fence_before();
     } else {
         // ================= weight producer ============================================================================
         pdl_wait();                                                         // the prep kernel's tiles and bias
-        tl_dep(p.tl_gemm, 288);
+        tl_dep(p.tl_gemm, 256);
         for (int c = lane; c < 64; c += 32) {
             ctl->bias[c] = p.bias_ws[c];
             ctl->bvar[c] = p.bias_ws[64 + c];
@@ -428,8 +400,6 @@ conv_s4_kernel(const S4Args p) {
         }
     }
     __syncthreads();
-    tc_fence_after();
-    if (warp == 8) tmem_dealloc(tmem, tmem_cols);
     if (tr && threadIdx.x == 256) tr[7] = clock64();
     tl_exit(p.tl_gemm, 256);
 }
@@ -460,7 +430,7 @@ inline cudaError_t launch_conv_s4(S4Args a, cudaStream_t st, bool do_prep, bool 
     }
     if (!do_gemm) return cudaSuccess;
     const size_t imgb = (size_t)a.rows * a.wp * 8, img_plane = (S4_IMGS * imgb + 127) / 128 * 128;
-    const size_t smem = 1023 + 1024 + (size_t)S4_STAGES * a.planes * S4_BPLANE + a.planes * img_plane + 256;
+    const size_t smem = 1023 + 1024 + std::max((size_t)S4_STAGES * a.planes * S4_BPLANE + a.planes * img_plane + 256, s4_acc_bytes(a.planes));
     dim3 grid((unsigned)((g.B + S4_IMGS - 1) / S4_IMGS) * (g.OH >> 1));
     auto launch = [&](auto kernel) {
         cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);

@@ -1,4 +1,4 @@
-// Fused tcgen05 pipeline for chains of Bayesian layers on small feature maps.
+// Fused tensor-core (wgmma) pipeline for chains of Bayesian layers on small feature maps.
 //
 // Between fused layers the activation lives in HBM "tiled packed": [B/128][F/64][planes] blocks of
 // 128 rows x 128 B (64 bf16 of the NHWC-flattened (pixel, channel) axis), each block already in the
@@ -16,13 +16,14 @@
 //      tap that links the group's output pixel to the input pixel is computed; if
 //      it falls outside the kernel window the MMA (and the weight copy) is skipped
 //      -- zero padding costs nothing (AlexNet conv3-5: 4 of 9 taps are live).
-//        warps 9-12 : producers (each owns ring stages): cp.async.bulk of A / A^2 blocks and of the
+//        warps 8-11 : producers (each owns ring stages): cp.async.bulk of A / A^2 blocks and of the
 //                     live weight sub-tiles, mbarrier complete_tx
-//        warp 8     : tcgen05.mma issuer (M=128, N=64, bf16 -> fp32 TMEM; LRT: 2nd accumulator)
-//        warps 0-7  : LRT noise tile (Philox) during the main loop, then the epilogue -- tcgen05.ld,
-//                     bias, sqrt(var)*eps, 2x2 max-pool across the four column groups, activation,
+//        warps 0-7  : two warpgroups issuing wgmma (64 tile rows each, N = 64 or 128, bf16 -> fp32 in
+//                     registers; LRT: 2nd accumulator), then the epilogue -- bias, sqrt(var)*eps with the
+//                     LRT noise drawn in place, 2x2 max-pool across the four column groups, activation,
 //                     tiled-packed bf16 (+square) or fp32 store
 #pragma once
+#include <algorithm>
 #include "fwd_tc.cuh"
 
 namespace bbb {
@@ -43,7 +44,7 @@ struct FusedArgs {
     int out_mode, out_pitch, pool, in_pitch;   // pitches = F (columns) of the tiled packed matrices
     long long* trace;            // debug: per-CTA clock64 checkpoints (nullptr in production)
     long long* tl_prep; long long* tl_gemm;   // debug: timeline slots of the two launches (nullptr in production)
-    int units;                   // K blocks per pipeline step (TAP_UNITS, or 1 in the two-CTAs-per-SM LRT configuration)
+    int units;                   // K blocks per pipeline step (TAP_UNITS, or 1 for the 128-column LRT tile)
     McFold fold;                 // MC samples folded into the batch (rows = 0: off)
 };
 
@@ -136,8 +137,8 @@ tap_prep_kernel(const FusedArgs p) {
 // Same outputs as tap_prep_kernel for layers with a real kernel window (KHW > 1, prev_hw == 1), but reading the
 // parameters the way they lie in memory.  tap_prep_kernel's work item is one 16-byte output chunk = 8 input
 // channels of ONE tap, i.e. eight 4-byte loads KHW floats apart per thread and a different row per lane: every
-// warp load touches 32 lines and every 32-byte sector is fetched KHW times (by KHW different CTAs).  That made the
-// preps LSU-bound (17-32 us per AlexNet layer for 0.3-0.9 M weights) and they share the machine with the first
+// warp load touches 32 lines and every 32-byte sector is fetched KHW times (by KHW different CTAs).  That makes the
+// preps LSU-bound, and they share the machine with the first
 // GEMMs.  Here a CTA owns R output channels x one 64-input-channel block: each row's 64*KHW floats are contiguous
 // in OIHW order and are read with consecutive lanes on consecutive floats; softplus / eps / KL are element-wise, so
 // they are applied right there; the bf16 results go through shared memory ([plane][tap][row][cin]) and leave as the
@@ -245,29 +246,28 @@ tap_prep_conv_kernel(const FusedArgs p, const int R) {
     tl_exit(p.tl_prep);
 }
 
-// ------------------------------------------------------------- UMMA helpers
+// ------------------------------------------------------------ wgmma helpers
 // two packed bf16 -> their squares (exact product, one rounding: same value as bf16(float(x) * float(x)))
 __device__ __forceinline__ uint32_t bf16x2_sq(uint32_t v) {
     __nv_bfloat162 h = *reinterpret_cast<__nv_bfloat162*>(&v);
     h = __hmul2(h, h);
     return *reinterpret_cast<uint32_t*>(&h);
 }
-// K-major SWIZZLE_128B descriptor: 8-row groups 1024 B apart, layout_type = 2 at [61,64)
+// K-major SWIZZLE_128B wgmma descriptor: 8-row groups 1024 B apart, layout_type = 1 at [62,64)
 __device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t saddr) {
-    return (uint64_t)((saddr & 0x3FFFFu) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) |
-           (1ull << 46) | (2ull << 61);
+    return (uint64_t)((saddr & 0x3FFFFu) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 62);
 }
 
 constexpr int TAP_MAX_ITEMS = 64;       // live (input pixel, 64-channel block) pairs per tile (control block must stay < 2 KB)
 constexpr int TAP_UNITS = 2;            // K blocks handled per pipeline step (one mbarrier phase)
 static_assert(true, "");
 struct FusedSmem {
-    unsigned long long full[4], empty[4], accum;
-    uint32_t tmem_base, n_items;
+    unsigned long long full[4], empty[4];
+    uint32_t n_items, pad;
     float bias[128], bvar[128];     // this tile's output columns (BN <= 128)
     // K-loop schedule, built once per CTA: x = ipix | kb << 16, y = the four column groups' taps (0xFF = outside the
     // kernel window -> zero sub-tile).  A pipeline step covers TAP_UNITS consecutive items: the fixed cost of a stage
-    // hand-off (~500-900 cycles measured: barrier round trip + TMA issue + first-MMA start-up) is paid per STEP.
+    // hand-off (barrier round trip + TMA issue + first-MMA start-up) is paid per STEP.
     int2 items[TAP_MAX_ITEMS];
     int taps_px[64];                // per input pixel: packed taps (staging for the schedule build)
 };
@@ -277,14 +277,6 @@ __device__ __forceinline__ int tap_of(const Geom& g, int oh, int ow, int ih, int
     const int r = ih - oh * g.SH + g.PH, s = iw - ow * g.SW + g.PW;
     if ((unsigned)r < (unsigned)g.KH && (unsigned)s < (unsigned)g.KW) return r * g.KW + s;
     return -1;
-}
-
-__device__ __forceinline__ void tmem_ld4(uint32_t taddr, float (&v)[4]) {
-    uint32_t r0, r1, r2, r3;
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x4.b32 {%0,%1,%2,%3}, [%4];"
-                 : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3) : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-    v[0] = __uint_as_float(r0); v[1] = __uint_as_float(r1); v[2] = __uint_as_float(r2); v[3] = __uint_as_float(r3);
 }
 
 // LRT activation noise of image b, output pixel pix, channels [n, n+4): Philox element index is
@@ -297,37 +289,27 @@ __device__ __forceinline__ float4 act_noise4(const NoiseKey& k, int b, int pix, 
     return z;
 }
 
-// Thread roles (416 threads): warps 0-7 epilogue (two groups of four; group h owns half of the tile's 64
-// columns; warps w and w+4 read the same TMEM lanes), warp 8 MMA issuer, warps 9-12 TMA producers (one
-// elected thread each; the copies of a stage are dealt round-robin so their ~100-cycle issue costs overlap).
-constexpr int TAP_THREADS = 416, TAP_NPROD = 4;
+// Thread roles (384 threads): warps 0-7 = two warpgroups; warpgroup h issues the wgmma of tile rows [64h, 64h + 64)
+// (fp32 accumulators in registers), then the pair runs the epilogue; warps 8-11 TMA producers (one elected thread each;
+// the copies of a stage are dealt round-robin so their ~100-cycle issue costs overlap).
+constexpr int TAP_THREADS = 384, TAP_NPROD = 4;
 
-__device__ __forceinline__ void tmem_st8(uint32_t taddr, const float (&v)[8]) {
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};"
-                 ::"r"(taddr), "r"(__float_as_uint(v[0])), "r"(__float_as_uint(v[1])), "r"(__float_as_uint(v[2])), "r"(__float_as_uint(v[3])),
-                   "r"(__float_as_uint(v[4])), "r"(__float_as_uint(v[5])), "r"(__float_as_uint(v[6])), "r"(__float_as_uint(v[7])) : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
+// Accumulators leave the registers through shared memory (the operand ring, free after the main loop): rows of BN + 4
+// floats, [mean | variance] planes.  The epilogue stays a short rolled loop over 8-column chunks with one thread per
+// image row -- a register-indexed epilogue would force full unrolling, and straight-line code that runs once per CTA is
+// what the cold instruction cache punishes.  The LRT noise is drawn chunk by chunk in the epilogue.
+__host__ __device__ constexpr size_t tap_acc_bytes(int bn, int planes) { return (size_t)planes * TC_BM * (bn + 4) * 4; }
 
-// TMEM columns of a tile (BN = tile width, 64 or 128): [0,BN) mean accumulator, [BN,2BN) variance accumulator (LRT),
-// [2BN,3BN) the tile's LRT noise.  The noise tile is drawn (Philox) by the epilogue warps WHILE the main loop runs and
-// parked in tensor memory: no shared memory, no registers held across the main loop, and the epilogue stays a short rolled
-// loop with static register indices (a 64-value register array would force full unrolling; straight-line code that runs
-// once per CTA is what the cold instruction cache punishes -- DESIGN.md 5).
-//
-// BN: every SS-mode tcgen05.mma pulls (128 + BN) * 32 B of operands out of shared memory at 64 B/clk (measured, DESIGN.md
-// 5), i.e. 96 cycles for the 32 cycles of math of an N=64 MMA, 128 for the 64 cycles of an N=128 one: the wider tile
-// raises the tensor-pipe ceiling from 1/3 to 1/2 and is used whenever it still leaves enough CTAs for the machine.
-// MINB = resident CTAs per SM the register allocation is sized for (1: configuration A, 2: configuration B)
-template <int MINB, int BN>
-__global__ void __launch_bounds__(TAP_THREADS, MINB)
+// TWO: LRT variance plane (planes == 2), compile-time for the same reason as in gemm_tc_kernel
+template <int BN, bool TWO>
+__global__ void __launch_bounds__(TAP_THREADS, 1)
 tap_gemm_kernel(const FusedArgs p, const int stages) {
     extern __shared__ uint8_t smem_raw[];
     constexpr uint32_t TB = BN * 128;                   // bytes of one B plane of a K block (BN rows x 64 bf16)
     const Geom& g = p.g;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int planes = p.planes;
-    const bool two = planes == 2;
+    const int planes = TWO ? 2 : 1;                    // == p.planes
+    constexpr bool two = TWO;
     const int ng = p.ng, groups = BN / ng;
 
     const uint32_t raw = smem_u32(smem_raw);
@@ -359,9 +341,8 @@ tap_gemm_kernel(const FusedArgs p, const int stages) {
     if (threadIdx.x == 0) {
         for (int s = 0; s < stages; ++s) {
             mbar_init(smem_u32(&ctl->full[s]), 1);
-            mbar_init(smem_u32(&ctl->empty[s]), 1);
+            mbar_init(smem_u32(&ctl->empty[s]), 8);           // lane 0 of each MMA warp once its wgmma retired
         }
-        mbar_init(smem_u32(&ctl->accum), 1);
         fence_barrier_init();
     }
     // K-loop schedule: one thread per input pixel works out the taps (integer divisions), thread 64 compacts
@@ -388,32 +369,25 @@ tap_gemm_kernel(const FusedArgs p, const int stages) {
         ctl->n_items = (uint32_t)n;
     }
     const bool philox = two && !p.eps_a;
-    const uint32_t tmem_cols = philox ? 4u * BN : (two ? 2u * BN : (uint32_t)BN);     // power of two >= 3 BN when the noise tile lives there
-    constexpr uint32_t NOISE_COL = 2u * BN;
-    if (warp == 8) tmem_alloc(smem_u32(&ctl->tmem_base), tmem_cols);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = ctl->tmem_base;
     if (tr && threadIdx.x == 0) tr[1] = clock64();
 
     const int n_items = (int)ctl->n_items;
     const int n_steps = (n_items + units - 1) / units;
 
-    if (warp >= 9) {
+    if (warp >= 8) {
         // ======================= TMA producers ==================================
         // The WHOLE warp executes the loop and the mbarrier waits; only the copies are issued by one lane.
-        // (tools/pipe_probe.cu: a try_wait that blocks with a single active lane is woken ~750 cycles late --
-        //  apparently by a time-out poll -- while a fully converged warp is woken as soon as the phase flips.)
-        // Issuing a stage costs one thread several hundred cycles of dependent latency (tools/tma_probe.cu: ~350
-        // cycles per expect_tx + cp.async.bulk pair) while the data lands ~250 cycles later, so the STEPS are dealt
-        // round-robin to the four producer warps: four issue chains run concurrently.
+        // (a try_wait that blocks with a single active lane can be woken late, while a fully converged warp is woken
+        //  as soon as the phase flips.)
+        // Issuing a stage costs one thread a chain of dependent latency (expect_tx + one cp.async.bulk per copy), so the
+        // STEPS are dealt round-robin to the four producer warps: four issue chains run concurrently.
         // A producer must see EVERY phase of the stage it fills (parity waits alias after two phases), so at most
         // `stages` producers take part and producer p owns stage p (mod nprod).
-        const int pid = warp - 9;
+        const int pid = warp - 8;
         const int nprod = min(TAP_NPROD, stages);
         pdl_wait();                                      // A / A^2 are the previous layer's output
-        tl_dep(p.tl_gemm, 288);
+        tl_dep(p.tl_gemm, 256);
         const size_t sub_elems = (size_t)planes * ng * 64;
         const __nv_bfloat16* zero_tile = p.wtiles + (size_t)p.taps * p.n_cblk * p.n_kblk * sub_elems;
         const uint32_t gbytes = (uint32_t)ng * 128;                     // one group, one plane
@@ -455,41 +429,8 @@ tap_gemm_kernel(const FusedArgs p, const int stages) {
             }
             __syncwarp();                                // stay converged: the next blocking wait must be a whole-warp wait
         }
-    } else if (warp == 8) {
-        // ======================= MMA issuer =====================================
-        const uint32_t idesc = make_idesc_bf16(TC_BM, BN);
-        // descriptors are linear in the (address >> 4) field: build them once, add offsets per MMA
-        const uint64_t dA0 = make_smem_desc_sw128(base + tiles_off);
-        const uint64_t dB0 = make_smem_desc_sw128(base + tiles_off + b_off);
-#pragma unroll 1
-        for (int it = 0; it < n_steps; ++it) {
-            const int s = it % stages;
-            __syncwarp();                                // converged whole-warp wait (see the producer comment)
-            mbar_wait(smem_u32(&ctl->full[s]), (uint32_t)(it / stages) & 1u);
-            tc_fence_after();
-            if (tr && it == 0 && lane == 0) tr[3] = clock64();
-            if (tr && it < 32 && lane == 0) tr[8 + it] = clock64();
-            if (lane == 0) {
-                const int nu = min(units, n_items - it * units);
-#pragma unroll 1
-                for (int u = 0; u < nu; ++u) {
-                    const uint32_t so = ((uint32_t)s * stage_bytes + (uint32_t)u * unit_bytes) >> 4;
-                    const uint64_t da = dA0 + so, db = dB0 + so;
-#pragma unroll
-                    for (int j = 0; j < 4; ++j) {
-                        umma_bf16(tmem, da + 2 * j, db + 2 * j, idesc, (it | u | j) ? 1u : 0u);
-                        if (two) umma_bf16(tmem + (uint32_t)BN, da + (a2_off >> 4) + 2 * j, db + (TB >> 4) + 2 * j, idesc, (it | u | j) ? 1u : 0u);
-                    }
-                }
-                umma_commit(smem_u32(&ctl->empty[s]));
-            }
-            __syncwarp();
-        }
-        if (lane == 0) { umma_commit(smem_u32(&ctl->accum)); if (tr) tr[4] = clock64(); }
-        __syncwarp();
-        tc_fence_before();
     } else {
-        // ======================= epilogue (warps 0-7) ===========================
+        // ======================= MMA + epilogue (warps 0-7) =====================
         // thread = (tile row t = image, half h).  Its columns, in chunks of 8:
         //   pool: the tile holds ng channels x the 4 pixels of a 2x2 window (column = q*ng + channel); half h owns ng/2
         //         channels = NC chunks, each present once per pixel q
@@ -497,7 +438,6 @@ tap_gemm_kernel(const FusedArgs p, const int stages) {
         constexpr int NCH = BN / 16;                      // 8-column chunks per thread
         const int t = threadIdx.x & 127, h = threadIdx.x >> 7, b = m0 + t;
         const bool bvalid = b < g.B;
-        const uint32_t lane_base = tmem + ((uint32_t)((warp & 3) * 32) << 16);
         const int nc = p.pool ? NCH / 4 : NCH;            // channel chunks this thread owns
         // chunk index k -> (channel chunk cc, pixel group q): pool: k = cc*4 + q (the four pixels of a chunk are consecutive)
         auto chunk_col = [&](int k, int& q, int& n0) {
@@ -505,28 +445,47 @@ tap_gemm_kernel(const FusedArgs p, const int stages) {
             q = 0; n0 = cb * BN + h * (BN / 2) + k * 8;
             return h * (BN / 2) + k * 8;
         };
-        // (1) while the main loop runs: draw this row's LRT noise and park it in tensor memory
-        if (philox) {
-            int b_s = b;                                 // image index inside its MC sample
-            const NoiseKey nkey = fold_key(effective_key(p.key, p.stream_base), p.fold, b, b_s);
-#pragma unroll 1
-            for (int k = 0; k < NCH; ++k) {
-                int q, n0, oh, ow;
-                const int c0 = chunk_col(k, q, n0);
-                group_pix(q, oh, ow);
-                float z8[8];
+        // (1) main loop: warpgroup h multiplies tile rows [64h, 64h + 64)
+        float acc[BN / 2], acc2[BN / 2];
 #pragma unroll
-                for (int hh = 0; hh < 2; ++hh) {
-                    float4 z = make_float4(0.f, 0.f, 0.f, 0.f);
-                    if (bvalid && n0 + 4 * hh < g.N) z = act_noise4(nkey, b_s, oh * g.OW + ow, n0 + 4 * hh, g.OHW, g.N);
-                    z8[4 * hh] = z.x; z8[4 * hh + 1] = z.y; z8[4 * hh + 2] = z.z; z8[4 * hh + 3] = z.w;
+        for (int i = 0; i < BN / 2; ++i) { acc[i] = 0.0f; acc2[i] = 0.0f; }
+        {
+            // descriptors are linear in the (address >> 4) field: build them once, add offsets per MMA
+            const uint64_t dA0 = make_smem_desc_sw128(base + tiles_off + (uint32_t)h * 64u * 128u);
+            const uint64_t dB0 = make_smem_desc_sw128(base + tiles_off + b_off);
+            // One wgmma group per K block (item), one loop level: a runtime loop over the items of a step nested inside
+            // the fence ... commit bracket makes ptxas serialize every wgmma.  After committing the first item of step
+            // it, wait_group<1> leaves only that item in flight, so all of step it - 1 has retired: release its stage.
+#pragma unroll 1
+            for (int i = 0; i < n_items; ++i) {
+                const int it = i / units, u = i - it * units, s = it % stages;
+                if (u == 0) {
+                    mbar_wait(smem_u32(&ctl->full[s]), (uint32_t)(it / stages) & 1u);
+                    if (tr && it == 0 && threadIdx.x == 0) tr[3] = clock64();
+                    if (tr && it < 32 && threadIdx.x == 0) tr[8 + it] = clock64();
                 }
-                tmem_st8(lane_base + NOISE_COL + (uint32_t)c0, z8);
+                const uint32_t so = ((uint32_t)s * stage_bytes + (uint32_t)u * unit_bytes) >> 4;
+                const uint64_t da = dA0 + so, db = dB0 + so;
+                wgmma_fence();
+#pragma unroll
+                for (int j = 0; j < 4; ++j) {
+                    const uint32_t acc_on = (i | j) ? 1u : 0u;
+                    if (BN == 128) {
+                        wgmma_m64n128k16_bf16(*reinterpret_cast<float (*)[64]>(acc), da + 2 * j, db + 2 * j, acc_on);
+                        if (two) wgmma_m64n128k16_bf16(*reinterpret_cast<float (*)[64]>(acc2), da + (a2_off >> 4) + 2 * j, db + (TB >> 4) + 2 * j, acc_on);
+                    } else {
+                        wgmma_m64n64k16_bf16(*reinterpret_cast<float (*)[32]>(acc), da + 2 * j, db + 2 * j, acc_on);
+                        if (two) wgmma_m64n64k16_bf16(*reinterpret_cast<float (*)[32]>(acc2), da + (a2_off >> 4) + 2 * j, db + (TB >> 4) + 2 * j, acc_on);
+                    }
+                }
+                wgmma_commit();
+                wgmma_wait<1>();
+                if (u == 0 && it > 0 && lane == 0) mbar_arrive(smem_u32(&ctl->empty[(it - 1) % stages]));
             }
-            tmem_st_wait();
+            wgmma_wait<0>();
+            if (tr && threadIdx.x == 0) tr[4] = clock64();
         }
-        const bool any_mma = n_items > 0;  // did the schedule of warp 8 contain at least one step?
-        // (2) accumulator ready
+        // (2) accumulators -> shared memory (the ring is free: every step was consumed), bias of this tile
         pdl_wait();                                      // our output buffers may still be read by the previous step's consumer
         if (threadIdx.x < BN) {                          // bias / bias variance of this tile's columns (written by the prep
             const int c = threadIdx.x;                   // kernel, which may be the programmatic predecessor: after the wait)
@@ -534,10 +493,15 @@ tap_gemm_kernel(const FusedArgs p, const int stages) {
             ctl->bias[c] = p.bias_ws[n];
             ctl->bvar[c] = p.bias_ws[p.n_cblk * ng + n];
         }
-        asm volatile("bar.sync 1, 256;" ::: "memory");   // the eight epilogue warps only
-        mbar_wait(smem_u32(&ctl->accum), 0u);
-        tc_fence_after();
+        constexpr int AP = BN + 4;                       // row pitch in floats
+        float* accs = reinterpret_cast<float*>(sm + tiles_off);
+        bar_sync(1, 256);                                // both warpgroups' wgmma retired before the ring is overwritten
+        acc_to_smem(acc, accs + h * 64 * AP, AP);
+        if (two) acc_to_smem(acc2, accs + (TC_BM + h * 64) * AP, AP);
+        bar_sync(1, 256);
         if (tr && threadIdx.x == 0) tr[5] = clock64();
+        int b_s = b;                                     // image index inside its MC sample
+        const NoiseKey nkey = fold_key(effective_key(p.key, p.stream_base), p.fold, b, b_s);
         const int ohw_out = p.pool ? (g.OHW >> 2) : g.OHW;
         (void)nc;
         float r[8];
@@ -546,28 +510,32 @@ tap_gemm_kernel(const FusedArgs p, const int stages) {
             int q, n0;
             const int c0 = chunk_col(k, q, n0);           // tile column / first output channel of this chunk
             float am[8];
-            tmem_ld8_nowait(lane_base + (uint32_t)c0, am);
+            ld_row8(accs + t * AP + c0, am);
             if (two) {
                 float av[8], e8[8];
-                tmem_ld8_nowait(lane_base + (uint32_t)BN + (uint32_t)c0, av);
-                if (philox) tmem_ld8_nowait(lane_base + NOISE_COL + (uint32_t)c0, e8);
-                tmem_ld_wait();
-                if (!philox) {
-                    int oh, ow;
-                    group_pix(q, oh, ow);
+                ld_row8(accs + (TC_BM + t) * AP + c0, av);
+                int oh, ow;
+                group_pix(q, oh, ow);
+                if (philox) {
+#pragma unroll
+                    for (int hh = 0; hh < 2; ++hh) {
+                        float4 z = make_float4(0.f, 0.f, 0.f, 0.f);
+                        if (bvalid && n0 + 4 * hh < g.N) z = act_noise4(nkey, b_s, oh * g.OW + ow, n0 + 4 * hh, g.OHW, g.N);
+                        e8[4 * hh] = z.x; e8[4 * hh + 1] = z.y; e8[4 * hh + 2] = z.z; e8[4 * hh + 3] = z.w;
+                    }
+                } else {
 #pragma unroll
                     for (int u = 0; u < 8; ++u)
                         e8[u] = (bvalid && n0 + u < g.N) ? __ldg(p.eps_a + ((size_t)b * g.N + n0 + u) * g.OHW + oh * g.OW + ow) : 0.0f;
                 }
 #pragma unroll
                 for (int u = 0; u < 8; ++u) {
-                    const float var = 1e-16f + ((any_mma ? av[u] : 0.0f) + ctl->bvar[c0 + u]);
-                    am[u] = (any_mma ? am[u] : 0.0f) + ctl->bias[c0 + u] + fast_sqrt(var) * e8[u];
+                    const float var = 1e-16f + (av[u] + ctl->bvar[c0 + u]);
+                    am[u] = am[u] + ctl->bias[c0 + u] + fast_sqrt(var) * e8[u];
                 }
             } else {
-                tmem_ld_wait();
 #pragma unroll
-                for (int u = 0; u < 8; ++u) am[u] = (any_mma ? am[u] : 0.0f) + ctl->bias[c0 + u];
+                for (int u = 0; u < 8; ++u) am[u] = am[u] + ctl->bias[c0 + u];
             }
             if (p.pool) {                                 // 2x2 max over the chunk's four pixels, store after the last
 #pragma unroll
@@ -601,11 +569,8 @@ tap_gemm_kernel(const FusedArgs p, const int stages) {
             }
         }
         if (tr && threadIdx.x == 0) tr[6] = clock64();
-        tc_fence_before();
     }
     __syncthreads();
-    tc_fence_after();
-    if (warp == 8) tmem_dealloc(tmem, tmem_cols);
     if (tr && threadIdx.x == 256) tr[7] = clock64();
     tl_exit(p.tl_gemm, 256);
 }
@@ -621,7 +586,7 @@ inline bool fused_supported(const Geom& g, int pool) {
 }
 
 inline cudaError_t launch_fused(FusedArgs a, const void* x, const void* x_sq, cudaStream_t st, int* n_launch, const char** why,
-                                bool do_prep = true, bool do_gemm = true, int n_sm = 148, bool prefer_wide = false) {
+                                bool do_prep = true, bool do_gemm = true, int n_sm = 132, bool prefer_wide = false) {
     const Geom& g = a.g;
     *n_launch = 0;
     a.planes = tc_planes(a.variant, a.sample);
@@ -668,7 +633,7 @@ inline cudaError_t launch_fused(FusedArgs a, const void* x, const void* x_sq, cu
         // <= 26 KB of staging per CTA: the preps run beside the GEMM chain (side streams) and must fit next to its CTAs
         constexpr size_t kPrepSmem = 26 * 1024;
         // (smaller CTAs -- >= 4 per SM -- were tried for more loads in flight: the preps then lose the scheduling race against
-        //  the high-priority GEMM chain and the third layer's prep finished at 61 us instead of 21 us: 123 vs 107 us per step)
+        //  the high-priority GEMM chain, and a late prep delays the whole step)
         while (R > 2 && ((long)(npad / R) * a.n_kblk < n_sm || need(R) > kPrepSmem)) R >>= 1;
         const bool prep2 = prep2_on && g.KHW > 1 && a.prev_hw == 1 && g.Cin % 64 == 0 && a.taps == g.KHW && need(R) <= 48 * 1024;
         if (prep2) {
@@ -692,19 +657,16 @@ inline cudaError_t launch_fused(FusedArgs a, const void* x, const void* x_sq, cu
         *n_launch += 1;
     }
     if (!do_gemm) return cudaSuccess;
-    // Configurations.  BN = 64: (A) one CTA per SM, stage = 2 K blocks, deep ring; (B) two CTAs per SM (~99 KB each) when
-    // the grid has more CTAs than SMs, so that all tiles run in ONE wave and one CTA's epilogue overlaps the other's main
-    // loop.  BN = 128: one CTA per SM, 64 KB (LRT) / 32 KB K blocks, three stages.  The LRT noise tile always lives in
-    // tensor memory and is drawn during the main loop.
-    const long n_ctas = (long)psets * a.n_cblk * row_tiles;
-    const bool two_per_sm = bn == 64 && n_ctas > n_sm;
+    // Configurations, one CTA per SM: two 384-thread CTAs would leave 85 registers per thread, fewer than the wgmma
+    // accumulators of an LRT tile need.  BN = 64: stage = 2 K blocks, deep ring.  BN = 128: 64 KB (LRT) / 32 KB K
+    // blocks, three stages.
     int stages;
-    if (bn == 128)       { stages = 3; a.units = a.planes == 2 ? 1 : 2; }
-    else if (two_per_sm) { stages = 2; a.units = a.planes == 2 ? 1 : 2; }
-    else                 { stages = a.planes == 2 ? 2 : 4; a.units = TAP_UNITS; }
+    if (bn == 128) { stages = 3; a.units = a.planes == 2 ? 1 : 2; }
+    else           { stages = a.planes == 2 ? 2 : 4; a.units = TAP_UNITS; }
     if (const char* e = getenv("BBB_B200_STAGES")) { const int v = atoi(e); if (v >= 2 && v <= stages) stages = v; }
     const size_t unit_bytes = (size_t)a.planes * (TC_A_BYTES + (size_t)bn * 128);
-    const size_t smem = 1023 + 2048 + (size_t)stages * a.units * unit_bytes;   // align slack + control/schedule + ring
+    // align slack + control/schedule + ring (which also holds the accumulators once the main loop is done)
+    const size_t smem = 1023 + 2048 + std::max((size_t)stages * a.units * unit_bytes, tap_acc_bytes(bn, a.planes));
     dim3 grid(psets * a.n_cblk, row_tiles);
     cudaError_t e;
     auto launch = [&](auto kernel) {
@@ -713,7 +675,8 @@ inline cudaError_t launch_fused(FusedArgs a, const void* x, const void* x_sq, cu
         if (e2 != cudaSuccess) return e2;
         return launch_pdl(kernel, grid, dim3(TAP_THREADS), smem, st, a, stages);
     };
-    e = bn == 128 ? launch(tap_gemm_kernel<1, 128>) : (two_per_sm ? launch(tap_gemm_kernel<2, 64>) : launch(tap_gemm_kernel<1, 64>));
+    if (a.planes == 2) e = bn == 128 ? launch(tap_gemm_kernel<128, true>) : launch(tap_gemm_kernel<64, true>);
+    else               e = bn == 128 ? launch(tap_gemm_kernel<128, false>) : launch(tap_gemm_kernel<64, false>);
     if (e != cudaSuccess) return e;
     e = cudaGetLastError();
     if (e == cudaSuccess) *n_launch += 1;

@@ -1,5 +1,5 @@
 // Fused Bayesian layer forward on CUDA cores (IEEE fp32): the exact-arithmetic
-// path (BBB_MATH_FP32) and the path for shapes too small for a UMMA tile.
+// path (BBB_MATH_FP32) and the path for shapes too small for a wgmma tile.
 //
 // One kernel per layer call does everything the reference spreads over ~15-40
 // aten launches (SURVEY.md 2a): sigma = log1p(exp(rho)), eps (external or

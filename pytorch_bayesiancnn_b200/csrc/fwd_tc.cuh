@@ -1,11 +1,11 @@
-// Bayesian layer forward on the 5th-gen tensor cores (BBB_MATH_BF16_TC).
+// Bayesian layer forward on the Hopper tensor cores (BBB_MATH_BF16_TC / BBB_MATH_TF32_TC).
 //
 // Two kernels per layer call:
 //
 //  (P) weight_prep_kernel  -- HBM-bound, touches every parameter exactly once:
 //      sigma = log1p(exp(rho)); closed-form KL reduced to one scalar; BBB: draws eps
 //      (external or Philox) and forms W = mu + eps*sigma, LRT: forms (mu, sigma^2);
-//      writes bf16 operand tiles to the workspace ALREADY IN the canonical UMMA
+//      writes bf16 operand tiles to the workspace ALREADY IN the canonical wgmma
 //      K-major core-matrix order, one contiguous 8 KB (BBB) / 16 KB (LRT) block per
 //      (n-tile, k-block), so the GEMM kernel stages them with a single bulk-TMA copy.
 //      Doing this once per weight instead of once per M-tile CTA removes a
@@ -13,15 +13,14 @@
 //      depends on the parameters only, so in a captured graph it runs on a side
 //      branch, off the activation critical path.
 //
-//  (G) gemm_tc_kernel  -- implicit-GEMM conv / linear on tcgen05:
-//      warps 0-3 : A producers -- gather the im2col rows of x (fp32 NCHW), convert to
-//                  bf16 (LRT: also x^2), st.shared into the canonical K-major layout,
-//                  fence.proxy.async, mbarrier arrive; afterwards the same warps run
-//                  the epilogue (tcgen05.ld -> bias / sqrt(var)*eps -> NCHW store)
-//      warp 4    : one elected thread issues tcgen05.mma (M=128, N=64, K=16, bf16 ->
-//                  fp32 in TMEM; LRT: second accumulator for the variance path) and
-//                  tcgen05.commit to release smem stages / publish the accumulator
-//      warp 5    : one elected thread stages the prepared weight tiles with
+//  (G) gemm_tc_kernel  -- implicit-GEMM conv / linear on wgmma (M=128 tile, N=64):
+//      warps 0-7 : gather the im2col rows of x (fp32 NCHW), convert to bf16 (LRT: also
+//                  x^2), st.shared into the canonical K-major layout, fence.proxy.async,
+//                  mbarrier arrive; then each warpgroup issues wgmma for its 64 rows
+//                  (fp32 accumulators in registers; LRT: second accumulator for the
+//                  variance path) and gathers the next k-block while it runs; finally
+//                  the same warps run the epilogue (bias / sqrt(var)*eps -> store)
+//      warp 8    : one elected thread stages the prepared weight tiles with
 //                  cp.async.bulk (TMA, mbarrier complete_tx)
 //
 // Replaces layers/BBB/BBBConv.py:61-83, BBB/BBBLinear.py:54-76,
@@ -61,7 +60,8 @@ constexpr int TC_BM = 128, TC_BN = 64, TC_BK = 64;
 constexpr int TC_TILE_ELEMS = TC_BN * TC_BK;                 // 4096 bf16 = 8 KB
 constexpr int TC_A_BYTES = TC_BM * TC_BK * 2;                // 16 KB
 constexpr int TC_B_BYTES = TC_BN * TC_BK * 2;                // 8 KB
-constexpr int TC_SMEM_LIMIT = 227 * 1024;
+constexpr int TC_SMEM_LIMIT = 227 * 1024;            // H100: opt-in shared memory per block
+constexpr int TC_THREADS = 288;                    // 8 A-producer / MMA / epilogue warps + 1 weight-TMA warp
 
 inline int tc_planes(int variant, int sample) { return (variant == BBB_VARIANT_LRT && sample) ? 2 : 1; }
 inline size_t tc_stage_bytes(int planes) { return (size_t)planes * (TC_A_BYTES + TC_B_BYTES); }
@@ -114,52 +114,63 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
 }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
 __device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                  ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
 }
-__device__ __forceinline__ void tmem_alloc(uint32_t dst_smem, uint32_t cols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "r"(cols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t cols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(cols) : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem], tf32 x tf32 -> fp32 (operands: fp32 words, the low 13 mantissa bits ignored)
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
+
+// ---- Hopper warpgroup MMA (wgmma): D[registers of the 128 threads of a warpgroup] (+)= A[smem] * B[smem], M = 64.
+// Accumulator fragment of thread (warp w of the warpgroup, lane l): d[4i + {0,1}] = row 16w + l/4, columns
+// 8i + 2(l%4) + {0,1}; d[4i + {2,3}] = the same columns of row 16w + l/4 + 8.
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// bf16 x bf16 -> fp32, K = 16; tf32 x tf32 -> fp32, K = 8 (operands: fp32 words, the low 13 mantissa bits ignored).
+// Both read two 16-byte K chunks per row: the operand byte geometry is the same for both types.
+__device__ __forceinline__ void wgmma_m64n64k16_bf16(float (&d)[32], uint64_t da, uint64_t db, uint32_t accumulate) {
     asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t"
-        "}" ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate) : "memory");
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(da), "l"(db), "r"(accumulate));
 }
-// D[tmem] (+)= A[smem] * B[smem], bf16 x bf16 -> fp32
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
+
+__device__ __forceinline__ void wgmma_m64n128k16_bf16(float (&d)[64], uint64_t da, uint64_t db, uint32_t accumulate) {
     asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}" ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate) : "memory");
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(da), "l"(db), "r"(accumulate));
 }
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float (&v)[16]) {
-    uint32_t r[16];
+
+__device__ __forceinline__ void wgmma_m64n64k8_tf32(float (&d)[32], uint64_t da, uint64_t db, uint32_t accumulate) {
     asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(da), "l"(db), "r"(accumulate));
+}
+
+// Park a warpgroup's m64 x (2 * NR) accumulator fragment in shared memory: `tile` = row 0 of the warpgroup's 64 rows,
+// rows `pitch` floats apart.  The epilogues then read whole rows (one thread per output row).
+template <int NR>
+__device__ __forceinline__ void acc_to_smem(const float (&d)[NR], float* tile, int pitch) {
+    const int w = (threadIdx.x >> 5) & 3, l = threadIdx.x & 31;
+    float* r0 = tile + (16 * w + (l >> 2)) * pitch + 2 * (l & 3);
+    float* r8 = r0 + 8 * pitch;
 #pragma unroll
-    for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
+    for (int i = 0; i < NR / 4; ++i) {
+        *reinterpret_cast<float2*>(r0 + 8 * i) = make_float2(d[4 * i], d[4 * i + 1]);
+        *reinterpret_cast<float2*>(r8 + 8 * i) = make_float2(d[4 * i + 2], d[4 * i + 3]);
+    }
 }
+__device__ __forceinline__ void ld_row8(const float* p, float (&v)[8]) {
+    const float4 a = *reinterpret_cast<const float4*>(p), b = *reinterpret_cast<const float4*>(p + 4);
+    v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
+}
+// named barrier over the first `n` threads of the CTA (id 0 is __syncthreads)
+__device__ __forceinline__ void bar_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
 
 // Programmatic dependent launch: a kernel launched with the programmatic-serialization attribute may start
 // while its predecessor in the stream is still running; it must execute pdl_wait() before touching anything
@@ -170,8 +181,8 @@ __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.lau
 inline bool pdl_enabled() {
     static int v = -1;
     // on by default: inside the captured chain the next GEMM's CTAs start on idle SMs while the previous GEMM is
-    // still in its epilogue, so its prologue (barriers, TMEM, K schedule, LRT noise tile) is done by the time its
-    // inputs are: -5 us (LRT) / -10 us (BBB) per BBBAlexNet forward (tools/timeline.py).  BBB_B200_PDL=0 turns it off.
+    // still in its epilogue, so its prologue (barriers, K schedule) is done by the time its inputs are.
+    // BBB_B200_PDL=0 turns it off.
     if (v < 0) { const char* e = getenv("BBB_B200_PDL"); v = (e && e[0] == '0') ? 0 : 1; }
     return v == 1;
 }
@@ -187,23 +198,13 @@ inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, s
     return cudaLaunchKernelEx(&cfg, kernel, KArgs(args)...);
 }
 
-// K-major, SWIZZLE_NONE ("interleave") shared-memory matrix descriptor (sm_100):
+// K-major, SWIZZLE_NONE ("interleave") wgmma shared-memory matrix descriptor (sm_90):
 //   [0,14)  start address >> 4        [16,30) leading-dim byte offset >> 4 (stride between
 //   the two 16-byte K chunks of one MMA)  [32,46) stride-dim byte offset >> 4 (stride between
-//   8-row core-matrix groups)          [46,48) version = 1            [61,64) layout = 0
+//   8-row core-matrix groups)          [49,52) base offset = 0    [62,64) layout = 0
 __device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
     return (uint64_t)((saddr & 0x3FFFFu) >> 4) | ((uint64_t)(lbo_bytes >> 4) << 16) |
-           ((uint64_t)(sbo_bytes >> 4) << 32) | (1ull << 46);
-}
-// kind::f16 instruction descriptor: c_format=F32 [4,6), a/b_format=BF16 [7,10)/[10,13), K-major A and B,
-// N>>3 at [17,23), M>>4 at [24,29).
-__host__ __device__ constexpr uint32_t make_idesc_bf16(int M, int N) {
-    return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-
-// kind::tf32: a/b_format = TF32 (2)
-__host__ __device__ constexpr uint32_t make_idesc_tf32(int M, int N) {
-    return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+           ((uint64_t)(sbo_bytes >> 4) << 32);
 }
 // round-to-nearest tf32 (10-bit mantissa) kept in an fp32 word: the tensor core would otherwise truncate
 __device__ __forceinline__ uint32_t to_tf32(float x) {
@@ -231,9 +232,9 @@ enum { OUT_PACKED_BF16 = 0, OUT_ROWMAJOR_F32 = 1, OUT_NCHW_F32 = 2 };
 // "Tiled packed" inter-layer activation: the [B, F] bf16 matrix (F = pixels x channels, F % 64 == 0) is stored as
 // [B/128 row tiles][F/64 column blocks][128 rows x 128 B], every 16 KB block already in the K-major SWIZZLE_128B
 // smem image -- the consumer stages an A tile with ONE 16 KB cp.async.bulk instead of a 128-row tensor-map box
-// (measured: the strided box costs ~900 cycles per stage regardless of bytes, stages or CTA count).
+// (a strided box costs a fixed latency per stage regardless of bytes).
 // When a following LRT layer also needs x^2, the two planes of a block are interleaved ([block][x | x^2], 32 KB),
-// so the consumer stages both with ONE bulk copy (every cp.async.bulk costs ~200 issue cycles, DESIGN.md 5).
+// so the consumer stages both with ONE bulk copy (every cp.async.bulk has a fixed issue cost).
 // Offset (in elements) of the 8-element chunk holding columns [col, col+8) of row b in plane 0:
 __device__ __forceinline__ size_t tiled_chunk_offset(int b, int col, int kb_total, int planes) {
     const int r = b & 127, kb = col >> 6, ch = (col & 63) >> 3;
@@ -253,25 +254,6 @@ __device__ __forceinline__ float fast_sqrt(float x) {
     asm("sqrt.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x));
     return r;
 }
-__device__ __forceinline__ void tmem_ld8(uint32_t taddr, float (&v)[8]) {
-    uint32_t r[8];
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]) : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-    for (int i = 0; i < 8; ++i) v[i] = __uint_as_float(r[i]);
-}
-
-// issue-only variant + one wait: several TMEM loads in flight instead of one round trip each
-__device__ __forceinline__ void tmem_ld8_nowait(uint32_t taddr, float (&v)[8]) {
-    uint32_t r[8];
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]) : "r"(taddr));
-#pragma unroll
-    for (int i = 0; i < 8; ++i) v[i] = __uint_as_float(r[i]);
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
 // Apply the fused activation to 16 consecutive output channels [n0, n0+16) of image b at
 // output position `pos` (pixel, or pooled window) and store them in the requested layout.
 struct StoreCfg { void* y; void* y_sq; int out_mode, out_pitch, N, act; };
@@ -378,8 +360,7 @@ weight_prep_kernel(const TcArgs p) {
 
 // ----------------------------------------------------------------- (G) GEMM
 struct TcSmem {      // barrier block at the start of dynamic smem (after 1024-alignment)
-    unsigned long long full[4], empty[4], accum;
-    uint32_t tmem_base, pad;
+    unsigned long long full[4], empty[4];
     float bias[64], bvar[64];
 };
 
@@ -389,16 +370,19 @@ __host__ __device__ inline int tc_tile_images(int OHW) {
     return OHW >= TC_BM ? 2 : (TC_BM + OHW - 1) / OHW + 1;
 }
 
-template <int VARIANT, bool TF32>
-__global__ void __launch_bounds__(320, 2)
+// TWO: the LRT variance plane (x^2 against sigma^2) is multiplied as well (planes == 2).  A compile-time flag: a runtime
+// branch around the second wgmma makes ptxas serialize every wgmma of the loop.
+template <int VARIANT, bool TF32, bool TWO>
+__global__ void __launch_bounds__(TC_THREADS, 2)
 gemm_tc_kernel(const TcArgs p, const int stages) {
     constexpr bool LRT = VARIANT == BBB_VARIANT_LRT;
+    static_assert(LRT || !TWO, "only the LRT variant has a variance plane");
     constexpr int CE = TF32 ? 4 : 8, BKE = 8 * CE;                  // elements per 16-byte chunk / per K block
     extern __shared__ uint8_t smem_raw[];
     const Geom& g = p.g;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int planes = p.planes;                       // 2 only for LRT && sample
-    const bool two = LRT && planes == 2;
+    const int planes = TWO ? 2 : 1;                    // == p.planes
+    constexpr bool two = TWO;
 
     const uint32_t raw = smem_u32(smem_raw);
     const uint32_t base = (raw + 1023u) & ~1023u;
@@ -466,24 +450,19 @@ gemm_tc_kernel(const TcArgs p, const int stages) {
     if (threadIdx.x == 0) {
         for (int s = 0; s < stages; ++s) {
             mbar_init(smem_u32(&ctl->full[s]), 256 + 1);      // 256 A-producer threads + the TMA thread
-            mbar_init(smem_u32(&ctl->empty[s]), 1);           // one tcgen05.commit
+            mbar_init(smem_u32(&ctl->empty[s]), 8);           // lane 0 of each MMA warp once its wgmma retired
         }
-        mbar_init(smem_u32(&ctl->accum), 1);
         fence_barrier_init();
     }
-    const uint32_t tmem_cols = two ? 128u : 64u;
-    if (warp == 8) tmem_alloc(smem_u32(&ctl->tmem_base), tmem_cols);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = ctl->tmem_base;
     if (tr && threadIdx.x == 0) tr[1] = clock64();
 
     if (warp < 8) {
-        // ================= A producers (then epilogue) =========================
+        // ================= A producers, MMA (then epilogue) ===================
         // 8 warps: thread -> (row = t & 127, half = t >> 7); a half owns 4 of the 8 K-chunks of every k-block in the
-        // main loop and 32 of the 64 output columns in the epilogue (warps w and w+4 share TMEM lanes 32*(w&3)..)
-        const int t = threadIdx.x & 127, half = threadIdx.x >> 7;   // row of the tile == TMEM lane
+        // main loop and 32 of the 64 output columns in the epilogue.  Warpgroup wg (== half) multiplies tile rows
+        // [64 wg, 64 wg + 64): its wgmma of k-block kb runs while the same threads gather k-block kb + 1.
+        const int t = threadIdx.x & 127, half = threadIdx.x >> 7;   // row of the tile
         const int m = m0 + t;
         const bool mvalid = m < g.M;
         int ih0 = 0, iw0 = 0; long xb = 0;
@@ -502,6 +481,9 @@ gemm_tc_kernel(const TcArgs p, const int stages) {
             xb = (long)(p.stage_x ? bimg - img0 : bimg) * chw + (long)ih0 * g.W + iw0;
         }
         const float* __restrict__ xp = p.stage_x ? xs : reinterpret_cast<const float*>(p.x);
+        float acc[32], acc2[32];
+#pragma unroll
+        for (int i = 0; i < 32; ++i) { acc[i] = 0.0f; acc2[i] = 0.0f; }
         for (int kb = 0; kb < p.k_blocks; ++kb) {
             const int s = kb % stages;
             const uint32_t ph = (uint32_t)(kb / stages) & 1u;
@@ -529,25 +511,52 @@ gemm_tc_kernel(const TcArgs p, const int stages) {
             fence_proxy_async();                        // generic-proxy stores -> visible to the tensor core
             mbar_arrive(smem_u32(&ctl->full[s]));
             if (tr && threadIdx.x == 0 && kb == 0) tr[2] = clock64();
+            mbar_wait(smem_u32(&ctl->full[s]), ph);     // both halves of A and the weight tile have landed
+            // one MMA = two 16-byte K chunks per row (K = 16 bf16 or 8 tf32): the byte geometry is the same for both types
+            const uint32_t sa = base + tiles_off + (uint32_t)s * stage_bytes + (uint32_t)half * 64u * 16u;
+            const uint32_t sb = base + tiles_off + (uint32_t)s * stage_bytes + b_off;
+            wgmma_fence();
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+                const uint32_t acc_on = (kb | j) ? 1u : 0u;
+                const uint64_t da = make_smem_desc(sa + a_off + j * 2 * (TC_BM * 16), TC_BM * 16, 128);
+                const uint64_t db = make_smem_desc(sb + j * 2 * (TC_BN * 16), TC_BN * 16, 128);
+                if (TF32) wgmma_m64n64k8_tf32(acc, da, db, acc_on);
+                else wgmma_m64n64k16_bf16(acc, da, db, acc_on);
+                if (two) {
+                    const uint64_t da2 = make_smem_desc(sa + a2_off + j * 2 * (TC_BM * 16), TC_BM * 16, 128);
+                    const uint64_t db2 = make_smem_desc(sb + TC_B_BYTES + j * 2 * (TC_BN * 16), TC_BN * 16, 128);
+                    if (TF32) wgmma_m64n64k8_tf32(acc2, da2, db2, acc_on);
+                    else wgmma_m64n64k16_bf16(acc2, da2, db2, acc_on);
+                }
+            }
+            wgmma_commit();
+            wgmma_wait<1>();                            // k-block kb - 1 retired: its stage may be refilled
+            if (kb > 0 && lane == 0) mbar_arrive(smem_u32(&ctl->empty[(kb - 1) % stages]));
         }
+        wgmma_wait<0>();
         if (tr && threadIdx.x == 0) tr[3] = clock64();
+        // accumulators -> shared memory (the operand ring is free now), one row per thread from here on
+        bar_sync(1, 256);
+        constexpr int AP = TC_BN + 4;                   // row pitch in floats
+        float* accs = reinterpret_cast<float*>(sm + tiles_off);
+        acc_to_smem(acc, accs + half * 64 * AP, AP);
+        if (two) acc_to_smem(acc2, accs + (TC_BM + half * 64) * AP, AP);
+        bar_sync(1, 256);
 
         // ================= epilogue ============================================
         // (1) LRT noise for this row, 8 columns at a time, drawn while the last MMAs drain
         const bool philox = two && !p.eps_a;
         const NoiseKey nkey = effective_key(p.key, p.stream_base);
-        mbar_wait(smem_u32(&ctl->accum), 0u);
-        tc_fence_after();
         if (tr && threadIdx.x == 0) tr[5] = clock64();
-        const uint32_t lane_base = tmem + ((uint32_t)((warp & 3) * 32) << 16);
         const int ohw_out = p.pool ? (g.OHW >> 2) : g.OHW;
         const int opix = p.pool ? pwin : pix;
         const bool writer = mvalid && !(p.pool && (threadIdx.x & 3));
 #pragma unroll 1
         for (int c0 = half * 32; c0 < half * 32 + 32; c0 += 8) {
             float am[8], av[8], ez[8];
-            tmem_ld8(lane_base + (uint32_t)c0, am);
-            if (two) tmem_ld8(lane_base + 64u + (uint32_t)c0, av);
+            ld_row8(accs + t * AP + c0, am);
+            if (two) ld_row8(accs + (TC_BM + t) * AP + c0, av);
             const int nb = n0 + c0;
             if (philox) {
 #pragma unroll
@@ -603,41 +612,9 @@ gemm_tc_kernel(const TcArgs p, const int stages) {
             }
         }
         if (tr && threadIdx.x == 0) tr[6] = clock64();
-        tc_fence_before();
-    } else if (warp == 8) {
-        // ================= MMA issuer ==========================================
-        // one MMA = two 16-byte K chunks per row (K = 16 bf16 or 8 tf32): the byte geometry is the same for both types
-        constexpr uint32_t idesc = TF32 ? make_idesc_tf32(TC_BM, TC_BN) : make_idesc_bf16(TC_BM, TC_BN);
-        for (int kb = 0; kb < p.k_blocks; ++kb) {
-            const int s = kb % stages;
-            const uint32_t ph = (uint32_t)(kb / stages) & 1u;
-            __syncwarp();
-            mbar_wait(smem_u32(&ctl->full[s]), ph);
-            tc_fence_after();
-            if (lane == 0) {
-                const uint32_t st = base + tiles_off + (uint32_t)s * stage_bytes;
-#pragma unroll
-                for (int j = 0; j < 4; ++j) {
-                    const uint64_t da = make_smem_desc(st + a_off + j * 2 * (TC_BM * 16), TC_BM * 16, 128);
-                    const uint64_t db = make_smem_desc(st + b_off + j * 2 * (TC_BN * 16), TC_BN * 16, 128);
-                    if (TF32) umma_tf32(tmem, da, db, idesc, (kb | j) ? 1u : 0u);
-                    else umma_bf16(tmem, da, db, idesc, (kb | j) ? 1u : 0u);
-                    if (two) {
-                        const uint64_t da2 = make_smem_desc(st + a2_off + j * 2 * (TC_BM * 16), TC_BM * 16, 128);
-                        const uint64_t db2 = make_smem_desc(st + b_off + TC_B_BYTES + j * 2 * (TC_BN * 16), TC_BN * 16, 128);
-                        if (TF32) umma_tf32(tmem + 64u, da2, db2, idesc, (kb | j) ? 1u : 0u);
-                        else umma_bf16(tmem + 64u, da2, db2, idesc, (kb | j) ? 1u : 0u);
-                    }
-                }
-                umma_commit(smem_u32(&ctl->empty[s]));            // frees the smem stage when the MMAs retire
-                if (kb == p.k_blocks - 1) umma_commit(smem_u32(&ctl->accum));
-            }
-            __syncwarp();
-        }
-        tc_fence_before();
     } else {
         // ================= weight-tile TMA ======================================
-        // whole warp waits (a blocking try_wait with one active lane is woken ~750 cycles late), lane 0 issues
+        // whole warp waits (a blocking try_wait with one active lane can be woken late), lane 0 issues
         {
             const uint32_t bytes = (uint32_t)planes * TC_B_BYTES;
             const uint8_t* src0 = reinterpret_cast<const uint8_t*>(p.wtiles) + (size_t)n_tile * p.k_blocks * planes * TC_B_BYTES;
@@ -656,8 +633,6 @@ gemm_tc_kernel(const TcArgs p, const int stages) {
         }
     }
     __syncthreads();
-    tc_fence_after();
-    if (warp == 8) tmem_dealloc(tmem, tmem_cols);
     if (tr && threadIdx.x == 256) tr[7] = clock64();
     tl_exit(p.tl_gemm, 256);
 }
@@ -671,7 +646,7 @@ inline cudaError_t launch_fwd_tc_t(TcArgs a, cudaStream_t st, int* n_launch) {
         if (grid > 2048) grid = 2048;
         // Same shared-memory carve-out as the GEMM kernels: an SM only changes its L1/smem split when idle, so prep
         // CTAs running at the default (small-smem) split kept the first GEMM's CTAs off every SM they touched until
-        // their grids drained (tools/timeline.py: first GEMM 8 us after its own prep had finished).
+        // their grids drained (tools/timeline.py shows the start of each GEMM).
         static const bool carve = [] {
             const char* e = getenv("BBB_B200_PREP_CARVEOUT");
             if (e && e[0] == '0') return false;
@@ -704,10 +679,11 @@ inline cudaError_t launch_fwd_tc_t(TcArgs a, cudaStream_t st, int* n_launch) {
         smem += xs_elems * (a.stage_x == 2 ? 2 : 4);
     }
     dim3 grid((g.M + TC_BM - 1) / TC_BM, a.n_tiles);
-    cudaFuncSetAttribute(gemm_tc_kernel<VARIANT, TF32>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-    cudaError_t e = cudaFuncSetAttribute(gemm_tc_kernel<VARIANT, TF32>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    auto* kernel = a.planes == 2 ? gemm_tc_kernel<VARIANT, TF32, VARIANT == BBB_VARIANT_LRT> : gemm_tc_kernel<VARIANT, TF32, false>;
+    cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
-    e = launch_pdl(gemm_tc_kernel<VARIANT, TF32>, grid, dim3(320), smem, st, a, stages);
+    e = launch_pdl(kernel, grid, dim3(TC_THREADS), smem, st, a, stages);
     if (e != cudaSuccess) return e;
     e = cudaGetLastError();
     if (e == cudaSuccess) *n_launch += 1;

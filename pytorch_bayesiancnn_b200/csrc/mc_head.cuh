@@ -19,8 +19,8 @@
 //   [4096, ...)                     u64 data[2 slots][world][n_planes * B * C + 2]
 // Every float travels as ONE 8-byte store {value bits, sequence number} (the "LL" idea of NCCL's low-latency protocol):
 // 8-byte stores are single-copy atomic over NVLink, so the receiver simply polls each word until its tag equals the
-// launch's sequence number -- no fence, no separate flag, no CTA barrier between the push and the finish.  (Measured
-// with a fence.sys + st.release.sys flag per CTA instead: 3.0 + 3.4 us of fences per step on the critical path.)
+// launch's sequence number -- no fence, no separate flag, no CTA barrier between the push and the finish.  (A fence.sys +
+// st.release.sys flag per CTA instead would put two system-scope fences per step on the critical path.)
 // Tags make the buffer reusable without a reset: launch k of a rank uses slot k & 1; a peer can be at most one launch
 // ahead (it cannot finish launch k+1 before it has OUR launch k+1 words, which we send after we finished reading k).
 #pragma once
@@ -267,7 +267,7 @@ mc_exchange_kernel(const McxArgs p) {
         __syncthreads();                 // the last CTA's bookkeeping below must follow every thread's reads of this launch's slot
     }
     if (threadIdx.x == 0) {
-        // (a fence here also waits for the acknowledgements of this CTA's NVLink stores, ~3 us: only where something is published)
+        // (a fence here also waits for the acknowledgements of this CTA's NVLink stores: only where something is published)
         if (want_head) { p.head_partials[2 * blockIdx.x] = nll_cta; p.head_partials[2 * blockIdx.x + 1] = hit_cta; __threadfence(); }
         const unsigned int prev = atomicAdd(p.done, 1u);
         if (prev == gridDim.x - 1) {

@@ -188,7 +188,7 @@ def _stream(device):
 def _require_cuda(t: torch.Tensor, what: str):
     if not t.is_cuda:
         raise L.EngineError(
-            f"{what}: tensor is on {t.device}; the Bayesian layer engine runs on CUDA (sm_100a) only "
+            f"{what}: tensor is on {t.device}; the Bayesian layer engine runs on CUDA (sm_90a) only "
             "and has no CPU fallback")
 
 
@@ -218,7 +218,7 @@ def workspace(device, desc=None, owner=None) -> torch.Tensor:
     """Zero-initialised scratch.  Without `owner`: one per (device, stream) -- calls on
     one stream are ordered, so sharing is safe and the kernels leave the counters
     zeroed.  With `owner` (a layer module): a private buffer sized by bbb_workspace_bytes(desc),
-    which on the tcgen05 path also holds that layer's prepared bf16 operand tiles; it is held
+    which on the tensor-core path also holds that layer's prepared bf16 operand tiles; it is held
     through a weak reference to the layer, so it is freed with it and never re-bound to another one."""
     n = int(L.lib().bbb_workspace_bytes(C.byref(desc) if desc is not None else None))
     if owner is None:
@@ -262,7 +262,7 @@ def out_hw(h, w, kh, kw, conv):
 
 
 # --------------------------------------------------------------------------- #
-# tensor-core backward: wgrad / dgrad as role-swapped calls of the tcgen05 layer kernel
+# tensor-core backward: wgrad / dgrad as role-swapped calls of the tensor-core layer kernel
 # --------------------------------------------------------------------------- #
 _TC_K_MAX = 8192          # the gather kernel keeps an 8-byte table entry per reduction index in shared memory
 
@@ -271,8 +271,8 @@ _tc_math = L.MATH_BF16_TC          # operand type of the backward contractions (
 
 
 def _tc_contract(x, w, conv):
-    """Plain (mean-only, bias-free) conv2d / linear of fp32 `x` with the fp32 tensor `w` on the tcgen05 layer kernel
-    (bf16 or tf32 operands like the layer's forward, fp32 TMEM accumulators): the engine's forward with sample=0, no KL."""
+    """Plain (mean-only, bias-free) conv2d / linear of fp32 `x` with the fp32 tensor `w` on the tensor-core layer kernel
+    (bf16 or tf32 operands like the layer's forward, fp32 accumulators): the engine's forward with sample=0, no KL."""
     lib = L.lib()
     x, w = x.contiguous(), w.contiguous()
     d = make_desc(tuple(x.shape), tuple(w.shape), conv, L.VARIANT_BBB, False, False, 0.0, 1.0, _tc_math)
@@ -286,13 +286,13 @@ def _tc_contract(x, w, conv):
     ws = workspace(x.device, d)
     rc = fn(C.byref(d), _ptr(x), _ptr(w), _ptr(w), None, None, _ptr(y), None, None, None, None,
             C.c_uint64(0), C.c_uint64(0), None, _ptr(ws), C.c_size_t(ws.numel()), _stream(x.device))
-    L.check(rc, "tcgen05 contraction (backward)")
+    L.check(rc, "tensor-core contraction (backward)")
     return y
 
 
 def _tc_dgrad(g, w, conv, x_shape):
     """d x of y = conv(x, w): the full correlation of (zero-inserted) g with the flipped, channel-transposed kernel --
-    itself a stride-1 convolution, so it runs on the same tcgen05 layer kernel."""
+    itself a stride-1 convolution, so it runs on the same tensor-core layer kernel."""
     if conv is None:
         return _tc_contract(g, w.t(), None)                               # [B,N] x [K,N]^T -> [B,K]
     (sh, sw), (ph, pw), (dh, dw) = conv
@@ -314,7 +314,7 @@ def _tc_dgrad(g, w, conv, x_shape):
 
 def _tc_wgrad(x, g, conv, w_shape):
     """d w of y = conv(x, w): a convolution with the batch as the reduction ("channel") axis -- input x^T [C,B,H,W],
-    kernel g^T [N,B,OH,OW], stride <-> dilation swapped -- on the tcgen05 layer kernel.  Deterministic (no atomics);
+    kernel g^T [N,B,OH,OW], stride <-> dilation swapped -- on the tensor-core layer kernel.  Deterministic (no atomics);
     the batch is cut so that the reduction index fits the kernel's shared-memory table and the partial results summed."""
     if conv is None:
         out = _tc_contract(x.t(), g.t(), None)                             # [K,B] x [N,B]^T -> [K,N]
@@ -418,7 +418,7 @@ class BayesLayerFn(torch.autograd.Function):
             try:
                 out = BayesLayerFn._backward_tc(ctx, gy.contiguous().float())
             except L.EngineError as e:
-                if "code -2" not in str(e):                # BBB_E_UNSUPPORTED: a shape the tcgen05 kernel does not take
+                if "code -2" not in str(e):                # BBB_E_UNSUPPORTED: a shape the tensor-core kernel does not take
                     raise
                 out = None
             if out is not None:
@@ -460,7 +460,7 @@ class BayesLayerFn(torch.autograd.Function):
     @staticmethod
     def _backward_tc(ctx, gy):
         """SURVEY.md Appendix A on the tensor cores: every contraction of the backward (wgrad of the mean and of the
-        variance path, dgrad of both) is a call of the tcgen05 layer kernel with the operands' roles swapped; eps is
+        variance path, dgrad of both) is a call of the tensor-core layer kernel with the operands' roles swapped; eps is
         regenerated from the forward's Philox stream; the element-wise chain rule through sigma = softplus(rho) is
         parameter-sized glue.  Returns None when a shape does not fit (the caller then uses the CUDA-core kernels)."""
         x, W_mu, W_rho, bias_mu, bias_rho, act_std, eps_a, eps_b = ctx.saved_tensors

@@ -5,7 +5,7 @@ The reference's model files interleave the Bayesian layers with ``nn.Softplus`` 
 (BayesianAlexNet.py:34-53).  ``ModuleWrapper.forward`` (layers/misc.py:16-18) just
 calls them in order; here the same child list is pattern-matched into runs of
 ``[Bayesian layer, activation?, 2x2 max-pool?, flatten*]`` and each run becomes ONE
-``bbb_layer_forward_fused`` call (weight-prep kernel + tcgen05 GEMM kernel whose
+``bbb_layer_forward_fused`` call (weight-prep kernel + tensor-core GEMM kernel whose
 epilogue applies the activation and the pool and writes the packed bf16 format the
 next layer's TMA loads).  The model files stay unmodified; anything that does not
 match (other pools, other modules, autograd needed) falls back to the plain
@@ -213,7 +213,7 @@ def _run(steps, x, overlap_prep, out, terms, owner, fold=None, kls_out=None):
     first layer's prep is on the activation critical path.  The preps are issued in layer order over
     a few serial chains (default 3: layers 1,4 / 2,5 / 3) rather than all at once: six concurrent prep
     grids fill the machine and the first layer's prep -- the one the GEMM chain is waiting for -- was
-    scheduled last (measured with tools/timeline.py: first GEMM at 24 us instead of ~20).  The KL sum
+    scheduled last (tools/timeline.py shows the start of each GEMM).  The KL sum
     depends on the preps only and runs on the side as well."""
     dev = x.device
     kls = kls_out[:len(steps)] if kls_out is not None else torch.empty(len(steps), dtype=torch.float32, device=dev)

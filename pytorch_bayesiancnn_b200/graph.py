@@ -1,7 +1,7 @@
 """CUDA-graph capture of a whole forward(+KL): the six layer kernels and the
 interleaved aten activation/pool kernels become one graph launch, which is what
-the problem size needs (SURVEY.md H1: the whole BBBAlexNet forward is ~10-20 us of
-roofline time, i.e. the cost of its own kernel launches).
+the problem size needs (SURVEY.md H1: the whole BBBAlexNet forward is ~18-29 us of
+roofline time on an H100, i.e. the cost of its own kernel launches).
 
 Noise under replay: kernel arguments are frozen at capture, so the Philox stream
 is taken relative to a device scalar that a captured bbb_noise_advance kernel

@@ -8,7 +8,7 @@ results do not depend on R) and ONE exchange carries the per-(image, class) part
 Two implementations of the same contract:
 
 * ``MCForward`` / ``mc_forward(net, ...)`` -- the product path on the CUDA engine: the local samples run through the
-  engine (fused tcgen05 chain where the net allows), then ONE kernel (``bbb_mc_exchange``, csrc/mc_head.cuh) reduces
+  engine (fused tensor-core chain where the net allows), then ONE kernel (``bbb_mc_exchange``, csrc/mc_head.cuh) reduces
   them, pushes the partials into every peer's receive buffer over NVLink (CUDA-IPC peer-mapped memory, no NCCL on the
   data path), waits for the peers and finishes logmeanexp, KL/num_ens, the ELBO head (metrics.py:12-14, 23-24) and the
   uncertainty outputs (uncertainty_estimation.py:80-96, softmax or softplus-normalised :73-77) on the device.  The whole
@@ -207,11 +207,10 @@ class MCForward:
         kl_buf = self.kl_terms_all[par] if self.overlap else None
         inc = _STRIDE * self.inflight
         with torch.no_grad(), Fn.workspace_slot(par if self.inflight > 1 else Fn.current_workspace_slot()):
-            # The Philox base moves at the HEAD of a captured step, BEFORE the prep streams fork.  Measured (B200, captured
-            # step, tools/quick_step.py): with this one-thread kernel as the single root of the graph every GEMM kernel of
-            # the chain is launched programmatically behind its predecessor (100 us per step); with the fork in front of it
-            # (prep kernels as further root nodes) or with no plain kernel at the head, the programmatic edges of the whole
-            # chain are lost -- every GEMM then starts ~3 us after its predecessor ends (132 us per step).
+            # The Philox base moves at the HEAD of a captured step, BEFORE the prep streams fork: with this one-thread
+            # kernel as the single root of the graph every GEMM kernel of the chain is launched programmatically behind
+            # its predecessor; with the fork in front of it (prep kernels as further root nodes) or with no plain kernel
+            # at the head, the programmatic edges of the whole chain are lost and every GEMM waits for its predecessor.
             if advance:
                 Fn.noise_advance(base, inc)
             kl_ptr, n_kl = None, 0

@@ -9,8 +9,8 @@ models/BayesianModels/*.py import and train unchanged.  The bodies are new: one
 fused CUDA kernel per forward (through the C ABI), KL computed in that kernel.
 
 Engine knobs ride on ``set_flag`` (never on the constructor):
-  math           'fp32' | 'bf16' | 'tf32' | 'auto'   arithmetic path (default from $BBB_B200_MATH or 'auto': the tcgen05 tensor-core
-                                            path wherever the shape fits a UMMA tile, IEEE-fp32 CUDA cores otherwise;
+  math           'fp32' | 'bf16' | 'tf32' | 'auto'   arithmetic path (default from $BBB_B200_MATH or 'auto': the tensor-core
+                                            path wherever the shape fits a wgmma tile, IEEE-fp32 CUDA cores otherwise;
                                             'fp32' forces the exact-arithmetic kernels everywhere)
   kl_convention  'reference' | 'textbook'   default 'reference' = the formula as executed (SURVEY D1)
 """
@@ -55,7 +55,7 @@ class ModuleWrapper(nn.Module):
                 child.set_flag(flag_name, value)
 
     def _try_fused(self, x):
-        """Run the children as a fused tcgen05 chain if they match (see fused.py); None = not fusable."""
+        """Run the children as a fused tensor-core chain if they match (see fused.py); None = not fusable."""
         if not (torch.is_tensor(x) and x.is_cuda and x.dim() == 4) or not getattr(self, "fuse", _default_fuse()):
             return None
         if torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for p in self.parameters())):

@@ -1,11 +1,11 @@
-"""Generate golden fixtures by running the UNMODIFIED reference in this container.
+"""Generate golden fixtures by running the UNMODIFIED reference on the CPU.
 
-    PYTHONDONTWRITEBYTECODE=1 python tests/golden/make_golden.py
+    PYTHONDONTWRITEBYTECODE=1 python tests/golden/make_golden.py /path/to/PyTorch-BayesianCNN
 
-Imports /root/reference (read-only) -- never copied into the repo -- runs its
+Imports the original project (read-only) -- never copied into the repo -- runs its
 layers / models on seeded inputs, recovers the eps it drew by seed-replay of the
 global CPU generator (SURVEY.md 8c), and writes small ``.npz`` files next to
-this script.  /root/reference does not exist on the GPU box, so nothing in the
+this script.  The suite never needs the original project, so nothing in the
 test-suite calls this script; it is committed so the fixtures are reproducible.
 
 Fixtures
@@ -18,7 +18,7 @@ import os
 import sys
 
 sys.dont_write_bytecode = True
-REF = "/root/reference"
+REF = sys.argv[1] if len(sys.argv) > 1 else "."
 HERE = os.path.dirname(os.path.abspath(__file__))
 # the reference's layer files do `sys.path.append("..")` and import top-level
 # `metrics`; run with the reference root first on sys.path, like `cd reference`.

@@ -1,61 +1,50 @@
-"""The reference's UNMODIFIED model files on top of this repo's `layers` package.
-Runs only where /root/reference exists (the build container); the GPU box uses models.py."""
-import importlib
+"""The original project's model files on top of this repo's `layers` package.
+
+tests/golden/dropin.json records what models/BayesianModels/*.py of the original project build when this
+repository's `layers` resolves first (tests/golden/make_dropin.py): state_dict keys and shapes and child module
+types.  Our own model classes must build the same, so checkpoints are interchangeable and the original model
+files run unchanged on the engine."""
+import json
 import os
-import sys
 
 import pytest
 import torch
 
-from tests.conftest import ROOT
+from tests.conftest import GOLDEN
 from tests.util import CFG_PRIORS
 
-REF = "/root/reference"
-pytestmark = pytest.mark.skipif(not os.path.isdir(os.path.join(REF, "models")), reason="reference tree not present")
+
+@pytest.fixture(scope="module")
+def dropin():
+    with open(os.path.join(GOLDEN, "dropin.json")) as f:
+        return json.load(f)
 
 
-@pytest.fixture()
-def ref_models():
-    """Import models.BayesianModels.* from the reference with OUR `layers` resolving first."""
-    saved_path, saved_mods = list(sys.path), dict(sys.modules)
-    for k in [k for k in sys.modules if k == "models" or k.startswith("models.")]:
-        del sys.modules[k]
-    sys.path[:] = [ROOT] + [p for p in sys.path if p not in (ROOT, REF)] + [REF]
-    sys.dont_write_bytecode = True
-    try:
-        import layers
-        assert os.path.dirname(os.path.abspath(layers.__file__)) == os.path.join(ROOT, "layers")
-        mods = {n: importlib.import_module(f"models.BayesianModels.{m}") for n, m in
-                (("alexnet", "BayesianAlexNet"), ("lenet", "BayesianLeNet"), ("3conv3fc", "Bayesian3Conv3FC"))}
-        assert all(m.__file__.startswith(REF) for m in mods.values())
-        yield mods
-    finally:
-        sys.path[:] = saved_path
-        for k in [k for k in sys.modules if k == "models" or k.startswith("models.")]:
-            del sys.modules[k]
-
-
-def test_reference_model_files_build_on_our_layers(ref_models):
+def test_reference_model_files_build_on_our_layers(dropin):
     import pytorch_bayesiancnn_b200 as bbb
     from pytorch_bayesiancnn_b200 import models as ours
-    pairs = [(ref_models["alexnet"].BBBAlexNet, ours.BBBAlexNet, 3), (ref_models["lenet"].BBBLeNet, ours.BBBLeNet, 3),
-             (ref_models["3conv3fc"].BBB3Conv3FC, ours.BBB3Conv3FC, 1)]
-    for ref_cls, our_cls, cin in pairs:
-        for lt in ("lrt", "bbb"):
-            net = ref_cls(10, cin, CFG_PRIORS, lt, "softplus")          # reference constructor, our layers
-            mine = our_cls(10, cin, CFG_PRIORS, lt, "softplus")
-            assert isinstance(net, bbb.ModuleWrapper)
-            assert list(net.state_dict().keys()) == list(mine.state_dict().keys())
-            assert [type(m).__name__ for m in net.children()] == [type(m).__name__ for m in mine.children()]
-            mine.load_state_dict(net.state_dict())                       # checkpoints are interchangeable
+    assert sorted(dropin) == sorted(f"{m}/{lt}" for m in ("alexnet", "lenet", "3conv3fc") for lt in ("lrt", "bbb"))
+    for key, rec in dropin.items():
+        lt = key.split("/")[1]
+        our_cls = getattr(ours, rec["cls"])
+        mine = our_cls(10, rec["inputs"], CFG_PRIORS, lt, "softplus")
+        assert isinstance(mine, bbb.ModuleWrapper)
+        assert [[k, list(v.shape)] for k, v in mine.state_dict().items()] == rec["state_dict"], key
+        assert [type(m).__name__ for m in mine.children()] == rec["children"], key
+        state = {k: torch.randn(shape) for k, shape in rec["state_dict"]}
+        mine.load_state_dict(state)                                      # checkpoints are interchangeable
         with pytest.raises(ValueError):
-            ref_cls(10, cin, CFG_PRIORS, "nope")
+            our_cls(10, rec["inputs"], CFG_PRIORS, "nope")
 
 
 @pytest.mark.gpu
-def test_reference_model_files_run_on_the_engine(ref_models):
-    import pytorch_bayesiancnn_b200 as bbb
-    net = ref_models["lenet"].BBBLeNet(10, 3, CFG_PRIORS, "bbb", "relu").cuda().train()
+def test_reference_model_files_run_on_the_engine(dropin):
+    """Runs this package's restated BBBLeNet (models.py), not the original model file: the stored record ties the two
+    together (same state_dict layout), and the run checks that a ReLU BBB net goes through the engine end to end."""
+    from pytorch_bayesiancnn_b200 import models as ours
+    rec = dropin["lenet/bbb"]
+    net = getattr(ours, rec["cls"])(10, 3, CFG_PRIORS, "bbb", "relu").cuda().train()
+    assert [[k, list(v.shape)] for k, v in net.state_dict().items()] == rec["state_dict"]
     with torch.no_grad():
         out, kl = net(torch.randn(5, 3, 32, 32, device="cuda"))
     assert out.shape == (5, 10) and kl.dim() == 0 and torch.isfinite(out).all()

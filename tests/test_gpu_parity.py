@@ -226,7 +226,7 @@ def test_errors_are_loud(dev):
 
 
 # --------------------------------------------------------------------------- #
-# tcgen05 path (math='bf16'): bf16 operands, fp32 accumulate -> 1e-2 bar
+# tensor-core path (math='bf16'): bf16 operands, fp32 accumulate -> 1e-2 bar
 # --------------------------------------------------------------------------- #
 BF16_TOL = 1e-2
 
@@ -255,7 +255,7 @@ def test_tc_layer_cases_external_eps(golden_layers, dev):
 
 def test_tc_alexnet_layer_shapes_b512(dev):
     """Every BBBAlexNet layer geometry at the BASELINE batch (512), both variants,
-    tcgen05 path vs the oracle on identical eps."""
+    tensor-core path vs the oracle on identical eps."""
     import pytorch_bayesiancnn_b200 as bbb
     from oracle import bbb_oracle as O
     torch.set_num_threads(max(1, (torch.get_num_threads())))
@@ -345,7 +345,7 @@ def _alexnet(variant, classes, dev, act="softplus"):
 
 
 def test_fused_chain_vs_oracle_external_eps(dev):
-    """Whole BBBAlexNet through the fused tcgen05 chain vs the oracle on identical eps,
+    """Whole BBBAlexNet through the fused tensor-core chain vs the oracle on identical eps,
     at a batch that is not a multiple of the 128-row tile and at the BASELINE batch."""
     import pytorch_bayesiancnn_b200 as bbb
     from oracle import bbb_oracle as O
@@ -453,7 +453,7 @@ def test_backward_matches_oracle_autograd(dev):
 
 
 def test_backward_tensor_core_path_matches_oracle_autograd(dev):
-    """math='auto': forward AND backward contractions on tcgen05 (wgrad / dgrad as role-swapped calls of the layer
+    """math='auto': forward AND backward contractions on tensor-core (wgrad / dgrad as role-swapped calls of the layer
     kernel, bf16 operands, fp32 accumulate) against torch autograd through the oracle: the bf16 bar."""
     for variant in ("bbb", "lrt"):
         for conv in (True, False):

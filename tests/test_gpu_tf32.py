@@ -1,4 +1,4 @@
-"""math='tf32': the tcgen05 layer kernel with tf32 operands (fp32 storage rounded to a 10-bit mantissa, fp32 TMEM
+"""math='tf32': the tensor-core layer kernel with tf32 operands (fp32 storage rounded to a 10-bit mantissa, fp32
 accumulators) -- what the reference's own GPU conv computes by default (SURVEY D9) -- against the oracle and the
 reference-generated golden fixtures.  Bar: 1e-3 of the output scale per layer (north_star's fp32 bar), KL 1e-5."""
 import pytest

@@ -1,4 +1,5 @@
-"""A small run of every tcgen05 / mbarrier / TMEM kernel for compute-sanitizer (racecheck, synccheck, memcheck):
+"""A small run of every wgmma / mbarrier / TMA kernel for compute-sanitizer (racecheck, synccheck, memcheck) -- the
+empty/full barrier rings and the accumulators staged over the operand ring and the staged images:
     compute-sanitizer --tool racecheck python tools/sanitize_fwd.py
 BBBAlexNet, batch 48 (ragged tiles), LRT and BBB, fused chain (conv_s4 + tap-GEMMs) + the MC exchange kernel, no graphs."""
 import os, sys
