@@ -75,7 +75,8 @@ typedef struct bbb_layer_desc {
 
 /* Bytes of caller-allocated scratch a forward/KL call on `desc` needs.  The
  * scratch must be zero-filled ONCE when allocated; calls leave it zeroed where
- * that matters (self-resetting counters). */
+ * that matters (self-resetting counters).  A desc that folds the MC samples of a BBB layer
+ * (bbb_layer_forward_fused, reserved[1]) needs one operand set per sample. */
 size_t bbb_workspace_bytes(const bbb_layer_desc* desc);
 
 /* Replaces BBBConv2d.forward + .kl_loss:
@@ -136,11 +137,15 @@ enum { BBB_LAYOUT_NCHW_F32 = 0,      /* reference layout: [B, C, H, W] fp32     
  * the activation critical path: BBB_FUSED_PREP_ONLY launches just the weight-prep kernel
  * (sigma, eps, bf16 operand tiles, KL -> kl_out; x/y unused), BBB_FUSED_SKIP_PREP just the GEMM
  * kernel (the caller orders it after the prep, e.g. with an event).  0 = both, in order.
- * desc->reserved[1] > 0 folds Monte-Carlo samples into the batch (LRT + Philox only; what
+ * desc->reserved[1] > 0 folds Monte-Carlo samples into the batch (in-kernel Philox noise only; what
  * uncertainty_estimation.py:38-41 does by repeating the input): row b of the batch is image b % reserved[1] of sample
- * b / reserved[1], whose noise comes from Philox stream stream_id + (b / reserved[1]) * stride, stride = the uint64
- * in reserved[2] (low) / reserved[3] (high) -- bit-identical to separate calls per sample.  The NCHW input of the
- * first layer then holds reserved[1] images (it is not repeated). */
+ * s = b / reserved[1], whose noise comes from Philox stream stream_id + s * stride, stride = the uint64 in reserved[2]
+ * (low) / reserved[3] (high) -- bit-identical to separate calls per sample.  LRT: the activation noise of row b.  BBB:
+ * sample s multiplies by its own weights and bias, W_mu + softplus(W_rho) * eps with eps drawn from that stream (same
+ * element index as an unfolded call); needs reserved[1] % 128 == 0 (else BBB_E_UNSUPPORTED) and batch / reserved[1]
+ * times the operand workspace (bbb_workspace_bytes of the folding desc).  Either way the KL is computed once, as by an
+ * unfolded call.  The gather path (an NCHW input the stride-4 kernel does not take) does not fold.  The NCHW input of
+ * the first layer then holds reserved[1] images (it is not repeated). */
 enum { BBB_FUSED_PREP_ONLY = 1, BBB_FUSED_SKIP_PREP = 2 };
 int bbb_layer_forward_fused(const bbb_layer_desc* desc,
                             const void* x, const void* x_sq, int32_t in_layout, int32_t in_pitch, int32_t prev_hw,

@@ -53,6 +53,22 @@ int sm_count() {
     return n;
 }
 
+// Bytes of one set of prepared operands (tiles, zero sub-tile, bias rows) of whichever tensor-core path takes the layer.
+size_t tc_set_bytes(const bbb::Geom& g) {
+    return std::max({bbb::tc_workspace_bytes(g), bbb::fused_workspace_bytes(g), bbb::conv_s4_workspace_bytes(g)});
+}
+// Operand sets a call prepares: batch / rows for a BBB fold (one weight draw per MC sample), else 1.
+int weight_sets(const bbb_layer_desc& d, const bbb::Geom& g) {
+    const int rows = d.reserved[1];
+    return (d.variant == BBB_VARIANT_BBB && rows > 0 && g.B % rows == 0) ? g.B / rows : 1;
+}
+size_t set_stride(const bbb::Geom& g) { return (tc_set_bytes(g) + 1023) / 1024 * 1024; }
+
+bool s4_enabled() {
+    static const bool on = [] { const char* e = getenv("BBB_B200_CONV1_DIRECT"); return !(e && e[0] == '0'); }();
+    return on;
+}
+
 int check_desc(const bbb_layer_desc* d, bbb::Geom& g, bool linear) {
     if (!d) return fail(BBB_E_INVALID, "desc is NULL");
     if (!bbb::make_geom(*d, g)) return fail(BBB_E_INVALID, "invalid layer geometry");
@@ -157,11 +173,8 @@ size_t bbb_workspace_bytes(const bbb_layer_desc* desc) {
     if (!desc || desc->math == BBB_MATH_FP32) return kBaseWorkspace;
     bbb::Geom g;
     if (!bbb::make_geom(*desc, g)) return kBaseWorkspace;
-    size_t a = bbb::tc_workspace_bytes(g);
-    const size_t b = bbb::fused_workspace_bytes(g), c = bbb::conv_s4_workspace_bytes(g);
-    if (b > a) a = b;
-    if (c > a) a = c;
-    return kTcOffset + a;
+    const int sets = weight_sets(*desc, g);
+    return kTcOffset + (sets > 1 ? sets * set_stride(g) : tc_set_bytes(g));
 }
 
 int bbb_conv2d_forward(const bbb_layer_desc* desc, const void* x, const float* W_mu, const float* W_rho,
@@ -200,9 +213,11 @@ int bbb_linear_backward(const bbb_layer_desc* desc, const void* x, const void* g
                          cuda_stream);
 }
 
-/* shape / layout checks of bbb_layer_forward_fused, callable without a GPU (host logic only) */
+/* shape / layout / MC-fold checks of bbb_layer_forward_fused, callable without a GPU (host logic only); `s4` tells
+ * whether an NCHW input goes to the stride-4 first-layer kernel rather than the gather path */
 static int fused_check(const bbb_layer_desc* d, bbb::Geom& g, int32_t in_layout, int32_t in_pitch, int32_t prev_hw,
-                       int32_t out_layout, int32_t out_pitch) {
+                       int32_t out_layout, int32_t out_pitch, bool& s4) {
+    s4 = false;
     if (int rc = check_desc(d, g, false)) return rc;
     if (d->math == BBB_MATH_FP32 || d->math == BBB_MATH_TF32_TC) return fail(BBB_E_UNSUPPORTED, "the fused chain exists on the tensor-core (bf16) path only");
     const int pool = d->pool_k != 0;
@@ -211,6 +226,15 @@ static int fused_check(const bbb_layer_desc* d, bbb::Geom& g, int32_t in_layout,
     if (out_layout == BBB_LAYOUT_PACKED_BF16 && (g.N % 64 || out_pitch != (pool ? g.OHW / 4 : g.OHW) * g.N))
         return fail(BBB_E_INVALID, "tiled packed output needs Cout %% 64 == 0 and out_pitch == pixels*Cout (got %d)", out_pitch);
     const int out_mode = out_layout == BBB_LAYOUT_PACKED_BF16 ? 0 : (out_layout == BBB_LAYOUT_ROWMAJOR_F32 ? 1 : 2);
+    s4 = in_layout == BBB_LAYOUT_NCHW_F32 && s4_enabled() && bbb::conv_s4_supported(*d, g, pool, out_mode == 0);
+    if (const int rows = d->reserved[1]; rows > 0) {   // MC samples folded into the batch
+        if (!d->sample) return fail(BBB_E_UNSUPPORTED, "MC-sample folding needs a sampling call");
+        if (g.B % rows) return fail(BBB_E_INVALID, "batch %d is not a multiple of the rows per MC sample %d", g.B, rows);
+        // a row tile (128 rows; 16 images in the stride-4 kernel) must not straddle two weight samples
+        if (d->variant == BBB_VARIANT_BBB && rows % 128)
+            return fail(BBB_E_UNSUPPORTED, "BBB MC-sample folding needs a multiple of 128 rows per sample (got %d)", rows);
+        if (in_layout == BBB_LAYOUT_NCHW_F32 && !s4) return fail(BBB_E_UNSUPPORTED, "MC-sample folding is not available on the gather path");
+    }
     if (in_layout == BBB_LAYOUT_NCHW_F32) {
         if (!bbb::tc_supported(*d, g)) return fail(BBB_E_UNSUPPORTED, "shape not supported by the tensor-core gather path");
         if (out_mode == 1 && (pool ? g.OHW / 4 : g.OHW) != 1) return fail(BBB_E_UNSUPPORTED, "row-major fp32 output needs a 1x1 map on the gather path");
@@ -227,7 +251,8 @@ static int fused_check(const bbb_layer_desc* d, bbb::Geom& g, int32_t in_layout,
 int bbb_fused_supported(const bbb_layer_desc* d, int32_t in_layout, int32_t in_pitch, int32_t prev_hw,
                         int32_t out_layout, int32_t out_pitch) {
     bbb::Geom g;
-    return fused_check(d, g, in_layout, in_pitch, prev_hw, out_layout, out_pitch);
+    bool s4;
+    return fused_check(d, g, in_layout, in_pitch, prev_hw, out_layout, out_pitch, s4);
 }
 
 int bbb_layer_forward_fused(const bbb_layer_desc* d, const void* x, const void* x_sq, int32_t in_layout,
@@ -236,19 +261,20 @@ int bbb_layer_forward_fused(const bbb_layer_desc* d, const void* x, const void* 
                             int32_t out_pitch, float* kl_out, const float* eps_a, const float* eps_b, uint64_t seed,
                             uint64_t stream_id, const uint64_t* stream_base, void* ws, size_t ws_bytes, void* stream) {
     bbb::Geom g;
-    if (int rc = fused_check(d, g, in_layout, in_pitch, prev_hw, out_layout, out_pitch)) return rc;
+    bool s4;
+    if (int rc = fused_check(d, g, in_layout, in_pitch, prev_hw, out_layout, out_pitch, s4)) return rc;
     const bool prep_only = (d->reserved[0] & BBB_FUSED_PREP_ONLY) != 0, skip_prep = (d->reserved[0] & BBB_FUSED_SKIP_PREP) != 0;
     if (prep_only && skip_prep) return fail(BBB_E_INVALID, "PREP_ONLY and SKIP_PREP are exclusive");
     if (!W_mu || !W_rho || (!prep_only && (!x || !y))) return fail(BBB_E_INVALID, "NULL tensor pointer");
     if (d->has_bias && (!bias_mu || !bias_rho)) return fail(BBB_E_INVALID, "has_bias set but bias pointers NULL");
     const int pool = d->pool_k != 0;
-    bbb::McFold fold; fold.rows = 0; fold.stride = 0;
-    if (d->reserved[1] > 0) {           // MC samples folded into the batch
-        if (d->variant != BBB_VARIANT_LRT || !d->sample || eps_a)
-            return fail(BBB_E_UNSUPPORTED, "MC-sample folding needs the LRT variant with in-kernel Philox noise");
-        if (g.B % d->reserved[1]) return fail(BBB_E_INVALID, "batch %d is not a multiple of the rows per MC sample %d", g.B, d->reserved[1]);
+    bbb::McFold fold; fold.rows = 0; fold.stride = 0; fold.sets = 1; fold.set_bytes = 0;
+    if (d->reserved[1] > 0) {           // MC samples folded into the batch (checked by fused_check)
+        if (eps_a || eps_b) return fail(BBB_E_UNSUPPORTED, "MC-sample folding draws its noise in-kernel (no external eps)");
         fold.rows = d->reserved[1];
         fold.stride = ((unsigned long long)(uint32_t)d->reserved[3] << 32) | (uint32_t)d->reserved[2];
+        fold.sets = weight_sets(*d, g);
+        fold.set_bytes = set_stride(g);
     }
     const size_t need = bbb_workspace_bytes(d);
     if (!ws || ws_bytes < need) return fail(BBB_E_WORKSPACE, "workspace too small for the fused path: need %zu bytes", need);
@@ -257,8 +283,7 @@ int bbb_layer_forward_fused(const bbb_layer_desc* d, const void* x, const void* 
     cudaStream_t st = (cudaStream_t)stream;
     const int out_mode = out_layout == BBB_LAYOUT_PACKED_BF16 ? 0 : (out_layout == BBB_LAYOUT_ROWMAJOR_F32 ? 1 : 2);
     int nl = 0;
-    static const bool s4_on = [] { const char* e = getenv("BBB_B200_CONV1_DIRECT"); return !(e && e[0] == '0'); }();
-    if (in_layout == BBB_LAYOUT_NCHW_F32 && s4_on && bbb::conv_s4_supported(*d, g, pool, out_mode == 0)) {
+    if (s4) {
         // stride-4 first layer: the tensor core reads its A operand straight from the staged image (conv_s4_tc.cuh)
         bbb::S4Args a;
         a.g = g; a.x = (const float*)x; a.w_mu = W_mu; a.w_rho = W_rho; a.b_mu = bias_mu; a.b_rho = bias_rho;
@@ -275,7 +300,6 @@ int bbb_layer_forward_fused(const bbb_layer_desc* d, const void* x, const void* 
         cudaError_t e = bbb::launch_conv_s4(a, st, !skip_prep, !prep_only, &nl);
         if (e != cudaSuccess) return cuda_fail(e, "conv_s4 launch");
     } else if (in_layout == BBB_LAYOUT_NCHW_F32) {
-        if (fold.rows) return fail(BBB_E_UNSUPPORTED, "MC-sample folding is not available on the gather path");
         bbb::TcArgs a;
         a.g = g; a.x = x; a.w_mu = W_mu; a.w_rho = W_rho; a.b_mu = bias_mu; a.b_rho = bias_rho;
         a.y = y; a.kl_out = kl_out; a.act_std = nullptr; a.eps_a = eps_a; a.eps_b = eps_b;

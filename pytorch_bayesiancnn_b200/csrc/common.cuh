@@ -71,19 +71,30 @@ __device__ __forceinline__ NoiseKey effective_key(NoiseKey k, const unsigned lon
     return k;
 }
 
-// Monte-Carlo samples folded into the batch (LRT: samples differ only in their per-activation noise, so S samples of a
-// batch are one launch over S*rows rows): row b of the folded batch is image b % rows of sample b / rows, drawn from the
-// stream of that sample = stream + (b / rows) * stride -- bit-identical to S separate launches.
-struct McFold { int rows; unsigned long long stride; };
+// Monte-Carlo samples folded into the batch (S samples of a batch are one launch over S*rows rows): row b of the folded
+// batch is image b % rows of sample b / rows, drawn from the stream of that sample = stream + (b / rows) * stride --
+// bit-identical to S separate launches.  LRT samples differ only in their per-activation noise.  A BBB sample draws a
+// whole weight tensor: the prep writes `sets` = S operand sets (tiles + bias) `set_bytes` apart in the workspace, and a
+// row tile, which never straddles two samples, multiplies by the set of its sample.  LRT: sets = 1.
+struct McFold { int rows; unsigned long long stride; int sets; size_t set_bytes; };
+__device__ __forceinline__ NoiseKey sample_key(NoiseKey k, const McFold& f, int j) {
+    const unsigned long long s = (((unsigned long long)k.stream_hi << 32) | k.stream_lo) + (unsigned long long)j * f.stride;
+    k.stream_lo = (uint32_t)s; k.stream_hi = (uint32_t)(s >> 32);
+    return k;
+}
 __device__ __forceinline__ NoiseKey fold_key(NoiseKey k, const McFold& f, int b, int& b_in_sample) {
     b_in_sample = b;
     if (f.rows > 0) {
         const int j = b / f.rows;
         b_in_sample = b - j * f.rows;
-        const unsigned long long s = (((unsigned long long)k.stream_hi << 32) | k.stream_lo) + (unsigned long long)j * f.stride;
-        k.stream_lo = (uint32_t)s; k.stream_hi = (uint32_t)(s >> 32);
+        k = sample_key(k, f, j);
     }
     return k;
+}
+// operand set `j` of a BBB fold (j = 0: the set an unfolded call uses)
+template <class T>
+__host__ __device__ __forceinline__ T* fold_set(T* p, const McFold& f, int j) {
+    return reinterpret_cast<T*>(reinterpret_cast<uintptr_t>(p) + (size_t)j * f.set_bytes);
 }
 
 // four normals of group g (elements 4g .. 4g+3)

@@ -65,7 +65,8 @@ inline size_t conv_s4_workspace_bytes(const Geom& g) { return (size_t)g.KH * 2 *
 
 // ------------------------------------------------------------------ (P) prep
 // item = (kernel row r, 8-wide K chunk, output channel): K' = chunk*8 + e -> window pixel j = K'/4 (s = j - 1), channel K'%4
-template <int VARIANT>
+// FOLD: BBB fold, one operand set per weight sample (a separate instantiation keeps the other preps as they were)
+template <int VARIANT, bool FOLD = false>
 __global__ void __launch_bounds__(256)
 conv_s4_prep_kernel(const S4Args p) {
     __shared__ double red[32];
@@ -81,13 +82,15 @@ conv_s4_prep_kernel(const S4Args p) {
     pdl_wait();
     pdl_trigger();
     const NoiseKey nkey = effective_key(p.key, p.stream_base);
+    const int sets = FOLD ? p.fold.sets : 1;
     for (int gi = blockIdx.x * blockDim.x + threadIdx.x; gi < n_items; gi += gridDim.x * blockDim.x) {
         const int row = gi & 63, chunk = (gi >> 6) % 6, r = gi / (6 * 64);
-        float w[8], s2[8];
+        float w[8], s2[8], mu8[8], sg8[8];                          // mu8 / sg8: kept for the other samples of a fold
 #pragma unroll
         for (int e = 0; e < 8; ++e) {
             const int kq = chunk * 8 + e, s = (kq >> 2) - 1, c = kq & 3;
             float wv = 0.0f, sv = 0.0f;
+            mu8[e] = sg8[e] = 0.0f;
             if (s >= 0 && s < g.KW && c < g.Cin) {
                 const size_t wi = (((size_t)row * g.Cin + c) * g.KH + r) * g.KW + s;
                 const float mu = __ldg(p.w_mu + wi);
@@ -99,13 +102,26 @@ conv_s4_prep_kernel(const S4Args p) {
                     wv = mu + e_ * sigma;
                 } else wv = mu;
                 if (do_kl) kl_acc += (double)kl_term_fast(mu, sigma, p.prior_mu, p.prior_sigma, p.kl_convention);
+                mu8[e] = mu; sg8[e] = sigma;
             }
             w[e] = wv; s2[e] = sv;
         }
-        __nv_bfloat16* dst = p.wtiles + (size_t)r * p.planes * (S4_BPLANE / 2) + chunk * 512 + row * 8;   // canonical K-major, no swizzle
+        const size_t off = (size_t)r * p.planes * (S4_BPLANE / 2) + chunk * 512 + row * 8;   // canonical K-major, no swizzle
+        __nv_bfloat16* dst = p.wtiles + off;
         *reinterpret_cast<uint4*>(dst) = make_uint4(pack_bf16(w[0], w[1]), pack_bf16(w[2], w[3]), pack_bf16(w[4], w[5]), pack_bf16(w[6], w[7]));
         if (p.planes == 2)
             *reinterpret_cast<uint4*>(dst + S4_BPLANE / 2) = make_uint4(pack_bf16(s2[0], s2[1]), pack_bf16(s2[2], s2[3]), pack_bf16(s2[4], s2[5]), pack_bf16(s2[6], s2[7]));
+        for (int j = 1; j < sets; ++j) {                            // the other samples' weights from the same mu / sigma
+            const NoiseKey kj = sample_key(nkey, p.fold, j);
+#pragma unroll
+            for (int e = 0; e < 8; ++e) {
+                const int kq = chunk * 8 + e, s = (kq >> 2) - 1, c = kq & 3;
+                const size_t wi = (((size_t)row * g.Cin + c) * g.KH + r) * g.KW + s;
+                w[e] = (s >= 0 && s < g.KW && c < g.Cin) ? mu8[e] + normal1(wi, kj) * sg8[e] : 0.0f;
+            }
+            *reinterpret_cast<uint4*>(fold_set(p.wtiles, p.fold, j) + off) =
+                make_uint4(pack_bf16(w[0], w[1]), pack_bf16(w[2], w[3]), pack_bf16(w[4], w[5]), pack_bf16(w[6], w[7]));
+        }
     }
     for (int n = blockIdx.x * blockDim.x + threadIdx.x; n < 64; n += gridDim.x * blockDim.x) {   // bias
         float bm = 0.0f, bv = 0.0f;
@@ -118,6 +134,8 @@ conv_s4_prep_kernel(const S4Args p) {
                 bm = mu + e_ * sigma;
             } else bm = mu;
             if (do_kl) kl_acc += (double)kl_term_fast(mu, sigma, p.prior_mu, p.prior_sigma, p.kl_convention);
+            for (int j = 1; j < sets; ++j)
+                fold_set(p.bias_ws, p.fold, j)[n] = mu + normal1((uint64_t)g.N * g.K + n, sample_key(nkey, p.fold, j)) * sigma;
         }
         p.bias_ws[n] = bm;
         p.bias_ws[64 + n] = bv;
@@ -382,9 +400,13 @@ conv_s4_kernel(const S4Args p) {
         // ================= weight producer ============================================================================
         pdl_wait();                                                         // the prep kernel's tiles and bias
         tl_dep(p.tl_gemm, 256);
+        // BBB fold: the weight sample of this CTA's images (16 | rows, so the CTA lies inside one sample)
+        const int set = p.fold.sets > 1 ? img0 / p.fold.rows : 0;
+        const float* bias_ws = fold_set(p.bias_ws, p.fold, set);
+        const __nv_bfloat16* wtiles = fold_set(p.wtiles, p.fold, set);
         for (int c = lane; c < 64; c += 32) {
-            ctl->bias[c] = p.bias_ws[c];
-            ctl->bvar[c] = p.bias_ws[64 + c];
+            ctl->bias[c] = bias_ws[c];
+            ctl->bvar[c] = bias_ws[64 + c];
         }
         __syncwarp();                                                       // bias stores ordered before lane 0's first mbarrier arrive
         for (int r = 0; r < g.KH; ++r) {
@@ -394,7 +416,7 @@ conv_s4_kernel(const S4Args p) {
             if (lane == 0) {
                 const uint32_t bar = smem_u32(&ctl->full[s]);
                 mbar_arrive_expect_tx(bar, stage_bytes);
-                bulk_g2s(ring + (uint32_t)s * stage_bytes, p.wtiles + (size_t)r * (stage_bytes / 2), stage_bytes, bar);
+                bulk_g2s(ring + (uint32_t)s * stage_bytes, wtiles + (size_t)r * (stage_bytes / 2), stage_bytes, bar);
             }
             __syncwarp();
         }
@@ -418,12 +440,14 @@ inline cudaError_t launch_conv_s4(S4Args a, cudaStream_t st, bool do_prep, bool 
             if (e && e[0] == '0') return false;
             cudaFuncSetAttribute(conv_s4_prep_kernel<BBB_VARIANT_LRT>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
             cudaFuncSetAttribute(conv_s4_prep_kernel<BBB_VARIANT_BBB>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+            cudaFuncSetAttribute(conv_s4_prep_kernel<BBB_VARIANT_BBB, true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
             return true;
         }();
         (void)carve;
         const int grid = (g.KH * 6 * 64 + 255) / 256;
         cudaError_t e = lrt ? launch_pdl(conv_s4_prep_kernel<BBB_VARIANT_LRT>, dim3(grid), dim3(256), 0, st, a)
-                            : launch_pdl(conv_s4_prep_kernel<BBB_VARIANT_BBB>, dim3(grid), dim3(256), 0, st, a);
+                      : a.fold.sets > 1 ? launch_pdl(conv_s4_prep_kernel<BBB_VARIANT_BBB, true>, dim3(grid), dim3(256), 0, st, a)
+                                        : launch_pdl(conv_s4_prep_kernel<BBB_VARIANT_BBB>, dim3(grid), dim3(256), 0, st, a);
         if (e == cudaSuccess) e = cudaGetLastError();
         if (e != cudaSuccess) return e;
         *n_launch += 1;

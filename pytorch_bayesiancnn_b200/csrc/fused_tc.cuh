@@ -56,7 +56,47 @@ inline size_t fused_workspace_bytes(const Geom& g) {
 }
 
 // ------------------------------------------------------------- (P) tap prep
-template <int VARIANT>
+// Tail of both tap preps, per operand set: one all-zero sub-tile behind the real ones (staged for pool-window pixels
+// whose tap is outside the kernel) and the bias rows, prepared (and their KL counted once) by the first CTAs, one thread
+// per channel; then the KL publish.
+template <bool LRT, bool FOLD>
+__device__ __forceinline__ void tap_prep_tail(const FusedArgs& p, const NoiseKey& nkey, bool stoch, bool do_kl,
+                                              double kl_acc, double* red) {
+    const Geom& g = p.g;
+    const int sets = FOLD ? p.fold.sets : 1;
+    const size_t sub = fused_wtile_elems(p);
+    for (int j = 0; j < sets; ++j) {
+        uint4* zero = reinterpret_cast<uint4*>(fold_set(p.wtiles, p.fold, j) + (size_t)p.taps * p.n_cblk * p.n_kblk * sub);
+        for (long gi = (long)blockIdx.x * blockDim.x + threadIdx.x; gi < (long)(sub / 8); gi += (long)gridDim.x * blockDim.x)
+            zero[gi] = make_uint4(0u, 0u, 0u, 0u);
+    }
+    const int npad = p.n_cblk * p.ng;
+    for (int n = blockIdx.x * blockDim.x + threadIdx.x; n < npad; n += gridDim.x * blockDim.x) {
+        float bm = 0.0f, bv = 0.0f;
+        if (p.has_bias && n < g.N) {
+            const float mu = __ldg(p.b_mu + n);
+            const float sigma = (stoch || do_kl) ? softplus_sigma_fast(__ldg(p.b_rho + n)) : 0.0f;
+            if (LRT) { bm = mu; bv = sigma * sigma; }
+            else if (stoch) {
+                const float e_ = p.eps_b ? __ldg(p.eps_b + n) : normal1((uint64_t)g.N * g.K + n, nkey);
+                bm = mu + e_ * sigma;
+            } else bm = mu;
+            if (do_kl) kl_acc += (double)kl_term_fast(mu, sigma, p.prior_mu, p.prior_sigma, p.kl_convention);
+            for (int j = 1; j < sets; ++j)
+                fold_set(p.bias_ws, p.fold, j)[n] = mu + normal1((uint64_t)g.N * g.K + n, sample_key(nkey, p.fold, j)) * sigma;
+        }
+        p.bias_ws[n] = bm;
+        p.bias_ws[npad + n] = bv;
+    }
+    if (do_kl) {
+        const double tot = block_sum(kl_acc, red);
+        if (threadIdx.x == 0) kl_publish(tot, blockIdx.x, gridDim.x, p.kl_partials, p.kl_counter, p.kl_out);
+    }
+    tl_exit(p.tl_prep);
+}
+
+// FOLD: BBB fold, one operand set per weight sample (a separate instantiation keeps the other preps as they were)
+template <int VARIANT, bool FOLD = false>
 __global__ void __launch_bounds__(256)
 tap_prep_kernel(const FusedArgs p) {
     __shared__ double red[32];
@@ -68,6 +108,7 @@ tap_prep_kernel(const FusedArgs p) {
     const size_t sub = fused_wtile_elems(p);
     const int per_sub = p.ng * 8;                                  // (row, 8-wide K chunk) items per sub-tile
     const long n_items = (long)p.taps * p.n_cblk * p.n_kblk * per_sub;
+    const int sets = FOLD ? p.fold.sets : 1;
     double kl_acc = 0.0;
     tl_enter(p.tl_prep);
     for (long gi = (long)blockIdx.x * blockDim.x + threadIdx.x; gi < n_items; gi += (long)gridDim.x * blockDim.x) {
@@ -76,11 +117,12 @@ tap_prep_kernel(const FusedArgs p) {
         __nv_bfloat16* dst = p.wtiles + (size_t)st * sub;          // st == (tap*n_cblk + cb)*n_kblk + kb
         const int row = item % p.ng, chunk = item / p.ng;
         const int n = cb * p.ng + row;
-        float w[8], s2[8];
+        float w[8], s2[8], mu8[8], sg8[8];                         // mu8 / sg8: kept for the other samples of a fold
 #pragma unroll
         for (int e = 0; e < 8; ++e) {
             const int kq = kb * 64 + chunk * 8 + e;                // packed input-channel index
             float wv = 0.0f, sv = 0.0f;
+            mu8[e] = sg8[e] = 0.0f;
             if (n < g.N && kq < g.Cin) {
                 const int cin = (p.prev_hw > 1) ? ((kq % cprev) * p.prev_hw + kq / cprev) : kq;
                 const size_t wi = (size_t)n * g.K + (size_t)cin * g.KHW + tap;
@@ -93,6 +135,7 @@ tap_prep_kernel(const FusedArgs p) {
                     wv = mu + e_ * sigma;
                 } else wv = mu;
                 if (do_kl) kl_acc += (double)kl_term_fast(mu, sigma, p.prior_mu, p.prior_sigma, p.kl_convention);
+                mu8[e] = mu; sg8[e] = sigma;
             }
             w[e] = wv; s2[e] = sv;
         }
@@ -104,33 +147,20 @@ tap_prep_kernel(const FusedArgs p) {
             const uint4 o2 = make_uint4(pack_bf16(s2[0], s2[1]), pack_bf16(s2[2], s2[3]), pack_bf16(s2[4], s2[5]), pack_bf16(s2[6], s2[7]));
             *reinterpret_cast<uint4*>(dst + p.ng * 64 + sw) = o2;
         }
-    }
-    // one all-zero sub-tile behind the real ones: staged for pool-window pixels whose tap is outside the kernel
-    for (long gi = (long)blockIdx.x * blockDim.x + threadIdx.x; gi < (long)(sub / 8); gi += (long)gridDim.x * blockDim.x)
-        reinterpret_cast<uint4*>(p.wtiles + (size_t)p.taps * p.n_cblk * p.n_kblk * sub)[gi] = make_uint4(0u, 0u, 0u, 0u);
-    {   // bias: prepared (and its KL counted) by the first CTAs, one thread per channel
-        const int npad = p.n_cblk * p.ng;
-        for (int n = blockIdx.x * blockDim.x + threadIdx.x; n < npad; n += gridDim.x * blockDim.x) {
-            float bm = 0.0f, bv = 0.0f;
-            if (p.has_bias && n < g.N) {
-                const float mu = __ldg(p.b_mu + n);
-                const float sigma = (stoch || do_kl) ? softplus_sigma_fast(__ldg(p.b_rho + n)) : 0.0f;
-                if (LRT) { bm = mu; bv = sigma * sigma; }
-                else if (stoch) {
-                    const float e_ = p.eps_b ? __ldg(p.eps_b + n) : normal1((uint64_t)g.N * g.K + n, nkey);
-                    bm = mu + e_ * sigma;
-                } else bm = mu;
-                if (do_kl) kl_acc += (double)kl_term_fast(mu, sigma, p.prior_mu, p.prior_sigma, p.kl_convention);
+        for (int j = 1; j < sets; ++j) {                           // the other samples' weights from the same mu / sigma
+            const NoiseKey kj = sample_key(nkey, p.fold, j);
+#pragma unroll
+            for (int e = 0; e < 8; ++e) {
+                const int kq = kb * 64 + chunk * 8 + e;
+                const int cin = (p.prev_hw > 1) ? ((kq % cprev) * p.prev_hw + kq / cprev) : kq;
+                const size_t wi = (size_t)n * g.K + (size_t)cin * g.KHW + tap;
+                w[e] = (n < g.N && kq < g.Cin) ? mu8[e] + normal1(wi, kj) * sg8[e] : 0.0f;
             }
-            p.bias_ws[n] = bm;
-            p.bias_ws[npad + n] = bv;
+            *reinterpret_cast<uint4*>(fold_set(dst, p.fold, j) + sw) =
+                make_uint4(pack_bf16(w[0], w[1]), pack_bf16(w[2], w[3]), pack_bf16(w[4], w[5]), pack_bf16(w[6], w[7]));
         }
     }
-    if (do_kl) {
-        const double tot = block_sum(kl_acc, red);
-        if (threadIdx.x == 0) kl_publish(tot, blockIdx.x, gridDim.x, p.kl_partials, p.kl_counter, p.kl_out);
-    }
-    tl_exit(p.tl_prep);
+    tap_prep_tail<LRT, FOLD>(p, nkey, stoch, do_kl, kl_acc, red);
 }
 
 // ------------------------------------------------- (P2) tap prep, conv layers
@@ -143,19 +173,23 @@ tap_prep_kernel(const FusedArgs p) {
 // in OIHW order and are read with consecutive lanes on consecutive floats; softplus / eps / KL are element-wise, so
 // they are applied right there; the bf16 results go through shared memory ([plane][tap][row][cin]) and leave as the
 // same pre-swizzled 16-byte chunks, 1 KB contiguous per (tap, plane).
+// A BBB fold keeps the work split (so the KL sums in the same order as an unfolded call): phase 1 parks the fp32
+// (mu, sigma) pairs in shared memory instead, and phase 2 draws every sample's weights from them, chunk by chunk.
 constexpr int PREP2_BATCH = 4;                                     // loads in flight per thread
 __host__ __device__ inline int prep2_slab(int R) { return R * 64 + 8; }   // bf16 per (plane, tap) slab; +8 keeps 16 B alignment, skews banks
 
-template <int VARIANT>
+template <int VARIANT, bool FOLD = false>
 __global__ void __launch_bounds__(256)
 tap_prep_conv_kernel(const FusedArgs p, const int R) {
     extern __shared__ __align__(16) uint8_t prep2_smem[];
     __shared__ double red[32];
     constexpr bool LRT = VARIANT == BBB_VARIANT_LRT;
     __nv_bfloat16* sm = reinterpret_cast<__nv_bfloat16*>(prep2_smem);
+    float2* smf = reinterpret_cast<float2*>(prep2_smem);           // BBB fold: (mu, sigma) per element, same indexing
     const Geom& g = p.g;
     const NoiseKey nkey = effective_key(p.key, p.stream_base);
     const bool stoch = p.sample != 0, do_kl = p.kl_out != nullptr;
+    constexpr bool fold = FOLD;
     const int KHW = g.KHW, L = 64 * KHW, PS = prep2_slab(R);
     const size_t sub = fused_wtile_elems(p);
     const int n_units = (p.n_cblk * p.ng / R) * p.n_kblk;
@@ -194,17 +228,43 @@ tap_prep_conv_kernel(const FusedArgs p, const int R) {
                 if (ok[u]) {
                     const float sigma = (stoch || do_kl) ? softplus_sigma_fast(rho[u]) : 0.0f;
                     if (LRT) { wv = mu[u]; sv = sigma * sigma; }
+                    else if (fold) smf[so[u]] = make_float2(mu[u], sigma);   // every sample's weight is drawn in phase 2
                     else if (stoch) {
                         const float e_ = p.eps_a ? __ldg(p.eps_a + wi[u]) : normal1(wi[u], nkey);
                         wv = mu[u] + e_ * sigma;
                     } else wv = mu[u];
                     if (do_kl) kl_acc += (double)kl_term_fast(mu[u], sigma, p.prior_mu, p.prior_sigma, p.kl_convention);
                 }
+                if (fold) continue;
                 sm[so[u]] = __float2bfloat16_rn(wv);
                 if (p.planes == 2) sm[KHW * PS + so[u]] = __float2bfloat16_rn(sv);
             }
         }
         __syncthreads();
+        if (fold) {
+            // ---- phase 2, BBB fold: every sample's chunk from the same (mu, sigma) ----
+            for (int it = threadIdx.x; it < KHW * R * 8; it += 256) {
+                const int chunk = it & 7, rr = (it >> 3) % R, tp = it / (8 * R);
+                const float2* src = smf + (size_t)tp * PS + rr * 64 + chunk * 8;
+                const int n = n0 + rr, cb = n / p.ng, row = n - cb * p.ng, c0 = cin0 + chunk * 8;
+                const size_t st = ((size_t)tp * p.n_cblk + cb) * p.n_kblk + kb;
+                const size_t wi0 = (size_t)n * g.K + (size_t)c0 * KHW + tp;
+                __nv_bfloat16* dst = p.wtiles + st * sub + row * 64 + ((chunk ^ (row & 7)) << 3);
+                for (int j = 0; j < p.fold.sets; ++j) {
+                    const NoiseKey kj = sample_key(nkey, p.fold, j);
+                    float w[8];
+#pragma unroll
+                    for (int e = 0; e < 8; ++e) {
+                        const float2 ms = src[e];
+                        w[e] = (n < g.N && c0 + e < g.Cin) ? ms.x + normal1(wi0 + (size_t)e * KHW, kj) * ms.y : 0.0f;
+                    }
+                    *reinterpret_cast<uint4*>(fold_set(dst, p.fold, j)) =
+                        make_uint4(pack_bf16(w[0], w[1]), pack_bf16(w[2], w[3]), pack_bf16(w[4], w[5]), pack_bf16(w[6], w[7]));
+                }
+            }
+            __syncthreads();
+            continue;
+        }
         // ---- phase 2: 16-byte chunks (8 input channels of one tap) out, in the SW128 image order ----
         const int items = p.planes * KHW * R * 8;
         for (int it = threadIdx.x; it < items; it += 256) {
@@ -218,32 +278,7 @@ tap_prep_conv_kernel(const FusedArgs p, const int R) {
         }
         __syncthreads();
     }
-    // one all-zero sub-tile behind the real ones: staged for pool-window pixels whose tap is outside the kernel
-    for (long gi = (long)blockIdx.x * blockDim.x + threadIdx.x; gi < (long)(sub / 8); gi += (long)gridDim.x * blockDim.x)
-        reinterpret_cast<uint4*>(p.wtiles + (size_t)p.taps * p.n_cblk * p.n_kblk * sub)[gi] = make_uint4(0u, 0u, 0u, 0u);
-    {   // bias: prepared (and its KL counted) by the first CTAs, one thread per channel
-        const int npad = p.n_cblk * p.ng;
-        for (int n = blockIdx.x * blockDim.x + threadIdx.x; n < npad; n += gridDim.x * blockDim.x) {
-            float bm = 0.0f, bv = 0.0f;
-            if (p.has_bias && n < g.N) {
-                const float mu = __ldg(p.b_mu + n);
-                const float sigma = (stoch || do_kl) ? softplus_sigma_fast(__ldg(p.b_rho + n)) : 0.0f;
-                if (LRT) { bm = mu; bv = sigma * sigma; }
-                else if (stoch) {
-                    const float e_ = p.eps_b ? __ldg(p.eps_b + n) : normal1((uint64_t)g.N * g.K + n, nkey);
-                    bm = mu + e_ * sigma;
-                } else bm = mu;
-                if (do_kl) kl_acc += (double)kl_term_fast(mu, sigma, p.prior_mu, p.prior_sigma, p.kl_convention);
-            }
-            p.bias_ws[n] = bm;
-            p.bias_ws[npad + n] = bv;
-        }
-    }
-    if (do_kl) {
-        const double tot = block_sum(kl_acc, red);
-        if (threadIdx.x == 0) kl_publish(tot, blockIdx.x, gridDim.x, p.kl_partials, p.kl_counter, p.kl_out);
-    }
-    tl_exit(p.tl_prep);
+    tap_prep_tail<LRT, FOLD>(p, nkey, stoch, do_kl, kl_acc, red);
 }
 
 // ------------------------------------------------------------ wgmma helpers
@@ -389,7 +424,9 @@ tap_gemm_kernel(const FusedArgs p, const int stages) {
         pdl_wait();                                      // A / A^2 are the previous layer's output
         tl_dep(p.tl_gemm, 256);
         const size_t sub_elems = (size_t)planes * ng * 64;
-        const __nv_bfloat16* zero_tile = p.wtiles + (size_t)p.taps * p.n_cblk * p.n_kblk * sub_elems;
+        // BBB fold: the operand set of this row tile's weight sample (128 | rows, so the tile lies inside one sample)
+        const __nv_bfloat16* wtiles = fold_set(p.wtiles, p.fold, p.fold.sets > 1 ? m0 / p.fold.rows : 0);
+        const __nv_bfloat16* zero_tile = wtiles + (size_t)p.taps * p.n_cblk * p.n_kblk * sub_elems;
         const uint32_t gbytes = (uint32_t)ng * 128;                     // one group, one plane
         const uint32_t a_copy = (uint32_t)planes * TC_A_BYTES;
         const uint32_t unit_tx = a_copy + (uint32_t)(groups * planes) * gbytes;
@@ -416,7 +453,7 @@ tap_gemm_kernel(const FusedArgs p, const int stages) {
 #pragma unroll 1
                     for (int q = 0; q < groups; ++q) {
                         const int tp = (item.y >> (8 * q)) & 0xFF;
-                        const __nv_bfloat16* sp = tp != 0xFF ? p.wtiles + ((size_t)(tp * p.n_cblk + cb) * p.n_kblk + kb) * sub_elems : zero_tile;
+                        const __nv_bfloat16* sp = tp != 0xFF ? wtiles + ((size_t)(tp * p.n_cblk + cb) * p.n_kblk + kb) * sub_elems : zero_tile;
                         if (groups == 1) {           // [mu | sigma^2] of the sub-tile are contiguous here and in the stage
                             bulk_g2s(st + b_off, sp, (uint32_t)planes * gbytes, bar);
                         } else {
@@ -490,8 +527,9 @@ tap_gemm_kernel(const FusedArgs p, const int stages) {
         if (threadIdx.x < BN) {                          // bias / bias variance of this tile's columns (written by the prep
             const int c = threadIdx.x;                   // kernel, which may be the programmatic predecessor: after the wait)
             const int n = p.pool ? (cb * ng + (c % ng)) : (cb * BN + c);
-            ctl->bias[c] = p.bias_ws[n];
-            ctl->bvar[c] = p.bias_ws[p.n_cblk * ng + n];
+            const float* bias_ws = fold_set(p.bias_ws, p.fold, p.fold.sets > 1 ? m0 / p.fold.rows : 0);
+            ctl->bias[c] = bias_ws[n];
+            ctl->bvar[c] = bias_ws[p.n_cblk * ng + n];
         }
         constexpr int AP = BN + 4;                       // row pitch in floats
         float* accs = reinterpret_cast<float*>(sm + tiles_off);
@@ -612,6 +650,7 @@ inline cudaError_t launch_fused(FusedArgs a, const void* x, const void* x_sq, cu
         return cudaErrorInvalidValue;
     }
     if (do_prep) {
+        const bool fold = !lrt && a.fold.sets > 1;    // one operand set per weight sample: same grid / R, so the same KL sum
         const long items = (long)a.taps * a.n_cblk * a.n_kblk * a.ng * 8;
         int grid = (int)((items + 255) / 256);
         if (grid > 2048) grid = 2048;
@@ -621,6 +660,7 @@ inline cudaError_t launch_fused(FusedArgs a, const void* x, const void* x_sq, cu
             if (e && e[0] == '0') return false;
             cudaFuncSetAttribute(tap_prep_kernel<BBB_VARIANT_LRT>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
             cudaFuncSetAttribute(tap_prep_kernel<BBB_VARIANT_BBB>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+            cudaFuncSetAttribute(tap_prep_kernel<BBB_VARIANT_BBB, true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
             return true;
         }();
         (void)carve;
@@ -642,16 +682,26 @@ inline cudaError_t launch_fused(FusedArgs a, const void* x, const void* x_sq, cu
                 if (e && e[0] == '0') return false;
                 cudaFuncSetAttribute(tap_prep_conv_kernel<BBB_VARIANT_LRT>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
                 cudaFuncSetAttribute(tap_prep_conv_kernel<BBB_VARIANT_BBB>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+                cudaFuncSetAttribute(tap_prep_conv_kernel<BBB_VARIANT_BBB, true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
                 return true;
             }();
             (void)carve2;
             int grid2 = (npad / R) * a.n_kblk;
             if (grid2 > 2048) grid2 = 2048;
-            if (lrt) tap_prep_conv_kernel<BBB_VARIANT_LRT><<<grid2, 256, need(R), st>>>(a, R);
-            else     tap_prep_conv_kernel<BBB_VARIANT_BBB><<<grid2, 256, need(R), st>>>(a, R);
+            // a BBB fold stages fp32 (mu, sigma) pairs: 4x the bf16 slab, same R and grid as the unfolded call
+            if (fold) {
+                const size_t smem2 = (size_t)g.KHW * prep2_slab(R) * 8;
+                const cudaError_t e2 = cudaFuncSetAttribute(tap_prep_conv_kernel<BBB_VARIANT_BBB, true>,
+                                                            cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem2);
+                if (e2 != cudaSuccess) return e2;
+                tap_prep_conv_kernel<BBB_VARIANT_BBB, true><<<grid2, 256, smem2, st>>>(a, R);
+            }
+            else if (lrt) tap_prep_conv_kernel<BBB_VARIANT_LRT><<<grid2, 256, need(R), st>>>(a, R);
+            else          tap_prep_conv_kernel<BBB_VARIANT_BBB><<<grid2, 256, need(R), st>>>(a, R);
         }
-        else if (lrt) tap_prep_kernel<BBB_VARIANT_LRT><<<grid, 256, 0, st>>>(a);
-        else          tap_prep_kernel<BBB_VARIANT_BBB><<<grid, 256, 0, st>>>(a);
+        else if (fold) tap_prep_kernel<BBB_VARIANT_BBB, true><<<grid, 256, 0, st>>>(a);
+        else if (lrt)  tap_prep_kernel<BBB_VARIANT_LRT><<<grid, 256, 0, st>>>(a);
+        else           tap_prep_kernel<BBB_VARIANT_BBB><<<grid, 256, 0, st>>>(a);
         cudaError_t e = cudaGetLastError();
         if (e != cudaSuccess) return e;
         *n_launch += 1;

@@ -230,6 +230,8 @@ def workspace(device, desc=None, owner=None) -> torch.Tensor:
         key = (device.index, _ws_slot)
     ws = cache.get(key)
     if ws is None or ws.numel() < n:
+        if ws is not None:                        # a larger call (a BBB MC-sample fold) grows it: a graph captured on
+            cache.setdefault("retired", []).append(ws)   # the old buffer still writes there, so it stays allocated
         ws = torch.zeros(n, dtype=torch.uint8, device=device)
         cache[key] = ws
     return ws

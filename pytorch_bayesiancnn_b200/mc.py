@@ -131,17 +131,18 @@ class MCForward:
             ptrs = self._open_peers(nbytes)
         self.peers = (C.c_void_p * self.world)(*ptrs)
         self.base = torch.zeros(1, dtype=torch.int64, device=dev)
-        # LRT nets: the local samples differ only in their per-activation noise, so they FOLD into the batch -- one pass
-        # of the fused chain over S_local*B rows (what uncertainty_estimation.py:38-41 does by repeating the input), each
-        # row drawing from its own sample's Philox stream; the KL is computed once.  BBB nets (a weight draw per sample)
-        # and nets the chain cannot take run sample by sample.
+        # The local samples FOLD into the batch -- one pass of the fused chain over S_local*B rows (what
+        # uncertainty_estimation.py:38-41 does by repeating the input), each row drawing from its own sample's Philox
+        # stream; the KL is computed once.  LRT samples differ only in their per-activation noise; a BBB layer prepares one
+        # weight draw per sample and each row tile multiplies by its sample's draw.  Nets whose layers are all LRT or all
+        # BBB fold when the engine accepts the folded chain (BBB: B a multiple of 128); the rest run sample by sample.
         self.fold_steps = None
         from . import fused
         from .modules import _BayesLayer
         kids = list(net.children())
         layers = [m_ for m_ in kids if isinstance(m_, _BayesLayer)]
-        all_lrt = bool(layers) and all(m_._variant == L.VARIANT_LRT for m_ in layers) and getattr(net, "fuse", True)
-        if fold and len(self.ids) > 1 and all_lrt:
+        one_variant = bool(layers) and len({m_._variant for m_ in layers}) == 1 and getattr(net, "fuse", True)
+        if fold and len(self.ids) > 1 and one_variant:
             self.fold = (self.B, self.world << 40)
             self.fold_steps = fused.plan(kids, (len(self.ids) * self.B,) + tuple(example_x.shape[1:]), self.fold)
         self.graph, self.graphs = None, []
