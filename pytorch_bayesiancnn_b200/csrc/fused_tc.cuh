@@ -21,7 +21,8 @@
 //        warps 0-7  : two warpgroups issuing wgmma (64 tile rows each, N = 64 or 128, bf16 -> fp32 in
 //                     registers; LRT: 2nd accumulator), then the epilogue -- bias, sqrt(var)*eps with the
 //                     LRT noise drawn in place, 2x2 max-pool across the four column groups, activation,
-//                     tiled-packed bf16 (+square) or fp32 store
+//                     tiled-packed bf16 (+square) or fp32 store (unpooled tiled-packed tiles: one bulk copy
+//                     of the tile's shared-memory image, see tap_out_stage_bytes)
 #pragma once
 #include <algorithm>
 #include "fwd_tc.cuh"
@@ -335,6 +336,15 @@ constexpr int TAP_THREADS = 384, TAP_NPROD = 4;
 // what the cold instruction cache punishes.  The LRT noise is drawn chunk by chunk in the epilogue.
 __host__ __device__ constexpr size_t tap_acc_bytes(int bn, int planes) { return (size_t)planes * TC_BM * (bn + 4) * 4; }
 
+// Unpooled tiled-packed output: the tile's BN/64 column blocks, each [x | x^2 for an LRT consumer] x 16 KB, are one
+// contiguous stretch of y, and each block IS its shared-memory image.  The epilogue builds that image behind the staged
+// accumulators and one thread writes it with a single bulk copy.  Thread-per-row 16-byte stores put every lane of a
+// warp on a different 128-byte line, which made the stores the largest part of these layers' epilogue.
+// Ragged last row tiles keep the direct stores (rows past the batch are never written).
+inline size_t tap_out_stage_bytes(int bn, int pool, int out_mode, bool squares) {
+    return (!pool && out_mode == OUT_PACKED_BF16) ? (size_t)(bn / 64) * (squares ? 2 : 1) * 16384 : 0;
+}
+
 // TWO: LRT variance plane (planes == 2), compile-time for the same reason as in gemm_tc_kernel
 template <int BN, bool TWO>
 __global__ void __launch_bounds__(TAP_THREADS, 1)
@@ -542,6 +552,10 @@ tap_gemm_kernel(const FusedArgs p, const int stages) {
         const NoiseKey nkey = fold_key(effective_key(p.key, p.stream_base), p.fold, b, b_s);
         const int ohw_out = p.pool ? (g.OHW >> 2) : g.OHW;
         (void)nc;
+        const int planes_o = p.y_sq ? 2 : 1;
+        // see tap_out_stage_bytes: the output image goes behind the staged accumulators
+        const bool bulk_out = !p.pool && p.out_mode == OUT_PACKED_BF16 && m0 + TC_BM <= g.B;
+        uint8_t* ostage = sm + tiles_off + tap_acc_bytes(BN, planes);
         float r[8];
 #pragma unroll 1
         for (int k = 0; k < NCH; ++k) {
@@ -587,13 +601,20 @@ tap_gemm_kernel(const FusedArgs p, const int stages) {
 #pragma unroll
             for (int u = 0; u < 8; ++u) r[u] = fast_act(r[u], p.act);       // act is monotone: act(max) == max(act)
             if (p.out_mode == OUT_PACKED_BF16) {          // tiled packed (N % 64 == 0 guaranteed by the host)
-                const size_t off = tiled_chunk_offset(b, pset * g.N + n0, p.out_pitch >> 6, p.y_sq ? 2 : 1);
-                *reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(p.y) + off) =
-                    make_uint4(pack_bf16(r[0], r[1]), pack_bf16(r[2], r[3]), pack_bf16(r[4], r[5]), pack_bf16(r[6], r[7]));
+                const uint4 v = make_uint4(pack_bf16(r[0], r[1]), pack_bf16(r[2], r[3]), pack_bf16(r[4], r[5]), pack_bf16(r[6], r[7]));
+                uint4 v2 = v;
                 if (p.y_sq)
-                    *reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(p.y_sq) + off) =
-                        make_uint4(pack_bf16(r[0] * r[0], r[1] * r[1]), pack_bf16(r[2] * r[2], r[3] * r[3]),
-                                   pack_bf16(r[4] * r[4], r[5] * r[5]), pack_bf16(r[6] * r[6], r[7] * r[7]));
+                    v2 = make_uint4(pack_bf16(r[0] * r[0], r[1] * r[1]), pack_bf16(r[2] * r[2], r[3] * r[3]),
+                                    pack_bf16(r[4] * r[4], r[5] * r[5]), pack_bf16(r[6] * r[6], r[7] * r[7]));
+                if (bulk_out) {                           // block c0 / 64 of the tile, row t, 16-byte chunk swizzled as in HBM
+                    uint8_t* d = ostage + (size_t)(c0 >> 6) * planes_o * 16384 + t * 128 + ((((c0 & 63) >> 3) ^ (t & 7)) << 4);
+                    *reinterpret_cast<uint4*>(d) = v;
+                    if (p.y_sq) *reinterpret_cast<uint4*>(d + 16384) = v2;
+                    continue;
+                }
+                const size_t off = tiled_chunk_offset(b, pset * g.N + n0, p.out_pitch >> 6, planes_o);
+                *reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(p.y) + off) = v;
+                if (p.y_sq) *reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(p.y_sq) + off) = v2;
             } else {
                 float* yo = reinterpret_cast<float*>(p.y);
 #pragma unroll
@@ -604,6 +625,16 @@ tap_gemm_kernel(const FusedArgs p, const int stages) {
                         else yo[((size_t)b * g.N + n) * ohw_out + pset] = r[u];
                     }
                 }
+            }
+        }
+        if (bulk_out) {
+            fence_proxy_async();                          // this thread's image writes -> visible to the bulk copy
+            bar_sync(1, 256);
+            if (threadIdx.x == 0) {
+                const size_t g0 = tiled_chunk_offset(m0, pset * g.N + cb * BN, p.out_pitch >> 6, planes_o);
+                bulk_s2g(reinterpret_cast<__nv_bfloat16*>(p.y) + g0, smem_u32(ostage), (uint32_t)(BN / 64) * planes_o * 16384u);
+                bulk_commit();
+                bulk_wait_read();                         // the image must outlive the copy's reads
             }
         }
         if (tr && threadIdx.x == 0) tr[6] = clock64();
@@ -715,8 +746,10 @@ inline cudaError_t launch_fused(FusedArgs a, const void* x, const void* x_sq, cu
     else           { stages = a.planes == 2 ? 2 : 4; a.units = TAP_UNITS; }
     if (const char* e = getenv("BBB_B200_STAGES")) { const int v = atoi(e); if (v >= 2 && v <= stages) stages = v; }
     const size_t unit_bytes = (size_t)a.planes * (TC_A_BYTES + (size_t)bn * 128);
-    // align slack + control/schedule + ring (which also holds the accumulators once the main loop is done)
-    const size_t smem = 1023 + 2048 + std::max((size_t)stages * a.units * unit_bytes, tap_acc_bytes(bn, a.planes));
+    // align slack + control/schedule + ring (which also holds the accumulators and the output image once the main loop
+    // is done; BN = 128 LRT: 203,775 B, under the 227 KB limit)
+    const size_t smem = 1023 + 2048 + std::max((size_t)stages * a.units * unit_bytes,
+                                               tap_acc_bytes(bn, a.planes) + tap_out_stage_bytes(bn, a.pool, a.out_mode, a.y_sq != nullptr));
     dim3 grid(psets * a.n_cblk, row_tiles);
     cudaError_t e;
     auto launch = [&](auto kernel) {

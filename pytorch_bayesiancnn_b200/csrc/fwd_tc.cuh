@@ -118,6 +118,12 @@ __device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                  ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
 }
+// shared -> global bulk copy (bulk-group completion); the source must stay untouched until bulk_wait_read()
+__device__ __forceinline__ void bulk_s2g(void* dst, uint32_t src, uint32_t bytes) {
+    asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(dst), "r"(src), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
 
 // ---- Hopper warpgroup MMA (wgmma): D[registers of the 128 threads of a warpgroup] (+)= A[smem] * B[smem], M = 64.
 // Accumulator fragment of thread (warp w of the warpgroup, lane l): d[4i + {0,1}] = row 16w + l/4, columns
