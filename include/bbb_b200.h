@@ -76,7 +76,7 @@ typedef struct bbb_layer_desc {
 /* Bytes of caller-allocated scratch a forward/KL call on `desc` needs.  The
  * scratch must be zero-filled ONCE when allocated; calls leave it zeroed where
  * that matters (self-resetting counters).  A desc that folds the MC samples of a BBB layer
- * (bbb_layer_forward_fused, reserved[1]) needs one operand set per sample. */
+ * (reserved[1], on bbb_layer_forward_fused or the per-layer forward) needs one operand set per sample. */
 size_t bbb_workspace_bytes(const bbb_layer_desc* desc);
 
 /* Replaces BBBConv2d.forward + .kl_loss:
@@ -93,7 +93,15 @@ size_t bbb_workspace_bytes(const bbb_layer_desc* desc);
  *                       consecutive channels share one Philox call in every kernel.
  * stream_base: nullable DEVICE pointer; when set the effective Philox stream is
  *          stream_id + *stream_base, read by the kernel at run time -- this is how a
- *          captured CUDA graph draws fresh noise on every replay (bbb_noise_advance). */
+ *          captured CUDA graph draws fresh noise on every replay (bbb_noise_advance).
+ * desc->reserved[1] > 0 folds Monte-Carlo samples into the batch, as on bbb_layer_forward_fused: row (image) b is image
+ *          b % reserved[1] of sample s = b / reserved[1], drawn from Philox stream stream_id + s * stride (stride = the
+ *          uint64 in reserved[2] (low) / reserved[3] (high)), with the element index of an unfolded call on that image
+ *          -- bit-identical to one call per sample.  LRT: the activation noise of row b.  BBB: sample s multiplies by its
+ *          own weight draw; needs (reserved[1] * OH * OW) % 128 == 0 and the workspace of the folding desc.  The KL is
+ *          computed once, bit-identical to an unfolded call.  Needs sample == 1, in-kernel noise (eps_a / eps_b NULL,
+ *          else BBB_E_UNSUPPORTED), batch % reserved[1] == 0 (else BBB_E_INVALID) and a tensor-core math mode (bf16 /
+ *          tf32, or auto resolving to one; else BBB_E_UNSUPPORTED).  reserved[] all zero: no fold. */
 int bbb_conv2d_forward(const bbb_layer_desc* desc, const void* x,
                        const float* W_mu, const float* W_rho,
                        const float* bias_mu, const float* bias_rho,
@@ -104,7 +112,7 @@ int bbb_conv2d_forward(const bbb_layer_desc* desc, const void* x,
 
 /* Replaces BBBLinear.forward + .kl_loss:
  *   layers/BBB/BBBLinear.py:54-76, layers/BBB_LRT/BBBLinear.py:56-79.
- * Same arguments; desc must be the degenerate (1x1) geometry. */
+ * Same arguments; desc must be the degenerate (1x1) geometry (a BBB fold then needs reserved[1] % 128 == 0). */
 int bbb_linear_forward(const bbb_layer_desc* desc, const void* x,
                        const float* W_mu, const float* W_rho,
                        const float* bias_mu, const float* bias_rho,
@@ -112,6 +120,12 @@ int bbb_linear_forward(const bbb_layer_desc* desc, const void* x,
                        const float* eps_a, const float* eps_b,
                        uint64_t seed, uint64_t stream_id, const uint64_t* stream_base,
                        void* workspace, size_t workspace_bytes, void* cuda_stream);
+
+/* Host-only query (no GPU work, no GPU needed): would bbb_conv2d_forward / bbb_linear_forward accept this desc, its
+ * MC-sample fold (reserved[1..3]) included?  Returns BBB_OK or the error code the call would return
+ * (bbb_last_error() says why); pointer, external-eps and workspace checks are the call's own.  The host side asks
+ * before it folds a net's samples on the per-layer path. */
+int bbb_forward_supported(const bbb_layer_desc* desc);
 
 /* Activation layouts of the fused tensor-core chain (bbb_layer_forward_fused). */
 enum { BBB_LAYOUT_NCHW_F32 = 0,      /* reference layout: [B, C, H, W] fp32                       */

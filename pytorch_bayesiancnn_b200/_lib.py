@@ -27,7 +27,7 @@ ACT_BY_NAME = {None: ACT_NONE, "none": ACT_NONE, "softplus": ACT_SOFTPLUS, "relu
 
 SYMBOLS = (
     "bbb_workspace_bytes", "bbb_conv2d_forward", "bbb_linear_forward", "bbb_layer_forward_fused", "bbb_fused_supported",
-    "bbb_kl_forward",
+    "bbb_forward_supported", "bbb_kl_forward",
     "bbb_kl_backward", "bbb_conv2d_backward", "bbb_linear_backward", "bbb_philox_normal_fill",
     "bbb_mc_combine", "bbb_noise_advance", "bbb_last_error", "bbb_abi_version", "bbb_launch_count",
     "bbb_mc_buffer_bytes", "bbb_mc_state_bytes", "bbb_mc_exchange",
@@ -71,6 +71,8 @@ def _bind(lib):
     lib.bbb_layer_forward_fused.restype = C.c_int
     lib.bbb_fused_supported.argtypes = [dp, i32, i32, i32, i32, i32]
     lib.bbb_fused_supported.restype = C.c_int
+    lib.bbb_forward_supported.argtypes = [dp]
+    lib.bbb_forward_supported.restype = C.c_int
     lib.bbb_kl_forward.argtypes = [fp, fp, u64, fp, fp, u64, C.c_float, C.c_float, i32, fp, vp, sz, vp]
     lib.bbb_kl_forward.restype = C.c_int
     lib.bbb_kl_backward.argtypes = [fp, fp, u64, C.c_float, C.c_float, i32, fp, fp, fp, vp]

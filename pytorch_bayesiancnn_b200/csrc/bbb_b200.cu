@@ -80,6 +80,35 @@ int check_desc(const bbb_layer_desc* d, bbb::Geom& g, bool linear) {
     return BBB_OK;
 }
 
+// Pool, math-mode and shape checks of the per-layer forward (host logic only); `math` = the resolved BBB_MATH_*.
+int layer_math(const bbb_layer_desc* d, const bbb::Geom& g, int& math) {
+    if (d->pool_k != 0) return fail(BBB_E_UNSUPPORTED, "fused max-pool epilogue is not available on this path");
+    math = d->math;
+    if (math == BBB_MATH_AUTO) math = bbb::tc_supported(*d, g) ? BBB_MATH_BF16_TC : BBB_MATH_FP32;
+    if (math == BBB_MATH_BF16_TC || math == BBB_MATH_TF32_TC) {
+        if (!bbb::tc_supported(*d, g)) return fail(BBB_E_UNSUPPORTED, "tensor-core math mode: shape not supported by the tensor-core path");
+        return BBB_OK;
+    }
+    if (math != BBB_MATH_FP32) return fail(BBB_E_INVALID, "bad math mode %d", d->math);
+    if (d->act_dtype != BBB_DTYPE_F32) return fail(BBB_E_UNSUPPORTED, "BBB_MATH_FP32 path takes fp32 activations only");
+    if ((size_t)bbb::simt_kl_slots(g) > kMaxKlSlots || bbb::simt_kl_slots(g) > 65535)
+        return fail(BBB_E_UNSUPPORTED, "out_channels too large for the CUDA-core path (%d column tiles)", bbb::simt_kl_slots(g));
+    return BBB_OK;
+}
+
+// MC-sample fold checks of the per-layer forward (desc->reserved[1..3], include/bbb_b200.h); a no-op when reserved[1] == 0
+int layer_fold_check(const bbb_layer_desc* d, const bbb::Geom& g, int math) {
+    const int rows = d->reserved[1];
+    if (rows <= 0) return BBB_OK;
+    if (!d->sample) return fail(BBB_E_UNSUPPORTED, "MC-sample folding needs a sampling call");
+    if (g.B % rows) return fail(BBB_E_INVALID, "batch %d is not a multiple of the rows per MC sample %d", g.B, rows);
+    if (math == BBB_MATH_FP32) return fail(BBB_E_UNSUPPORTED, "MC-sample folding needs a tensor-core math mode");
+    // a 128-row GEMM tile multiplies by ONE weight sample's operand set
+    if (d->variant == BBB_VARIANT_BBB && ((long)rows * g.OHW) % bbb::TC_BM)
+        return fail(BBB_E_UNSUPPORTED, "BBB MC-sample folding needs rows x OH x OW %% %d == 0 (got %d x %d)", bbb::TC_BM, rows, g.OHW);
+    return BBB_OK;
+}
+
 int forward_impl(const bbb_layer_desc* d, bool linear, const void* x, const float* W_mu, const float* W_rho,
                  const float* bias_mu, const float* bias_rho, void* y, float* kl_out, float* act_std,
                  const float* eps_a, const float* eps_b, uint64_t seed, uint64_t stream_id, const uint64_t* stream_base, void* ws,
@@ -90,16 +119,24 @@ int forward_impl(const bbb_layer_desc* d, bool linear, const void* x, const floa
     if (d->has_bias && (!bias_mu || !bias_rho)) return fail(BBB_E_INVALID, "has_bias set but bias pointers NULL");
     if (kl_out && (!ws || ws_bytes < bbb_workspace_bytes(d)))
         return fail(BBB_E_WORKSPACE, "workspace too small: need %zu bytes", bbb_workspace_bytes(d));
-    if (d->pool_k != 0) return fail(BBB_E_UNSUPPORTED, "fused max-pool epilogue is not available on this path");
     cudaStream_t st = (cudaStream_t)stream;
 
-    int math = d->math;
-    if (math == BBB_MATH_AUTO) math = bbb::tc_supported(*d, g) ? BBB_MATH_BF16_TC : BBB_MATH_FP32;
+    int math = BBB_MATH_FP32;
+    if (int rc = layer_math(d, g, math)) return rc;
+    if (int rc = layer_fold_check(d, g, math)) return rc;
+    bbb::McFold fold; fold.rows = 0; fold.stride = 0; fold.sets = 1; fold.set_bytes = 0;
+    if (d->reserved[1] > 0) {
+        if (eps_a || eps_b) return fail(BBB_E_UNSUPPORTED, "MC-sample folding draws its noise in-kernel (no external eps)");
+        fold.rows = d->reserved[1];
+        fold.stride = ((unsigned long long)(uint32_t)d->reserved[3] << 32) | (uint32_t)d->reserved[2];
+        fold.sets = weight_sets(*d, g);
+        fold.set_bytes = set_stride(g);
+    }
     if (math == BBB_MATH_BF16_TC || math == BBB_MATH_TF32_TC) {
-        if (!bbb::tc_supported(*d, g)) return fail(BBB_E_UNSUPPORTED, "tensor-core math mode: shape not supported by the tensor-core path");
-        const size_t need = kTcOffset + bbb::tc_workspace_bytes(g);
+        const size_t need = fold.sets > 1 ? bbb_workspace_bytes(d) : kTcOffset + bbb::tc_workspace_bytes(g);
         if (!ws || ws_bytes < need) return fail(BBB_E_WORKSPACE, "workspace too small for the tensor-core path: need %zu bytes", need);
         bbb::TcArgs a;
+        a.fold = fold;
         a.wtiles = (__nv_bfloat16*)((char*)ws + kTcOffset);
         a.tf32 = math == BBB_MATH_TF32_TC;
         // operand tiles: 2 planes x npad rows x (kpad * 2 bytes of bf16 | kpad32 * 4 bytes of tf32), then the bias rows
@@ -119,10 +156,6 @@ int forward_impl(const bbb_layer_desc* d, bool linear, const void* x, const floa
         g_launches += nl;
         return BBB_OK;
     }
-    if (math != BBB_MATH_FP32) return fail(BBB_E_INVALID, "bad math mode %d", d->math);
-    if (d->act_dtype != BBB_DTYPE_F32) return fail(BBB_E_UNSUPPORTED, "BBB_MATH_FP32 path takes fp32 activations only");
-    if ((size_t)bbb::simt_kl_slots(g) > kMaxKlSlots || bbb::simt_kl_slots(g) > 65535)
-        return fail(BBB_E_UNSUPPORTED, "out_channels too large for the CUDA-core path (%d column tiles)", bbb::simt_kl_slots(g));
 
     bbb::FwdArgs a;
     a.g = g; a.x = (const float*)x; a.w_mu = W_mu; a.w_rho = W_rho; a.b_mu = bias_mu; a.b_rho = bias_rho;
@@ -248,6 +281,14 @@ static int fused_check(const bbb_layer_desc* d, bbb::Geom& g, int32_t in_layout,
     return BBB_OK;
 }
 
+int bbb_forward_supported(const bbb_layer_desc* d) {
+    bbb::Geom g;
+    int math = BBB_MATH_FP32;
+    if (int rc = check_desc(d, g, false)) return rc;
+    if (int rc = layer_math(d, g, math)) return rc;
+    return layer_fold_check(d, g, math);
+}
+
 int bbb_fused_supported(const bbb_layer_desc* d, int32_t in_layout, int32_t in_pitch, int32_t prev_hw,
                         int32_t out_layout, int32_t out_pitch) {
     bbb::Geom g;
@@ -311,6 +352,7 @@ int bbb_layer_forward_fused(const bbb_layer_desc* d, const void* x, const void* 
         a.wtiles = (__nv_bfloat16*)((char*)ws + kTcOffset);
         a.bias_ws = (float*)((char*)ws + kTcOffset + (size_t)bbb::tc_npad(g) * bbb::tc_kpad(g) * 4);
         a.tf32 = 0;
+        a.fold = fold;                  // rows = 0: fused_check refuses a fold on the gather path
         a.trace = g_trace; a.skip_prep = skip_prep; a.prep_only = prep_only; a.y_sq = y_sq; a.out_mode = out_mode == 1 ? 2 : out_mode; a.out_pitch = out_pitch; a.pool = pool;
         a.tl_prep = tl_slot(!skip_prep, "weight_prep", g); a.tl_gemm = tl_slot(!prep_only, "gemm_tc", g);
         cudaError_t e = bbb::launch_fwd_tc(a, st, sm_count(), &nl);

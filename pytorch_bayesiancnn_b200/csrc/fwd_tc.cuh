@@ -54,6 +54,7 @@ struct TcArgs {
     void* y_sq; int out_mode, out_pitch, pool;     // out_mode: 0 packed bf16 [B,(pix,c)], 2 NCHW fp32 (default)
     long long* trace;                              // debug: per-CTA clock64 checkpoints (nullptr in production)
     long long* tl_prep; long long* tl_gemm;        // debug: timeline slots of the two launches (nullptr in production)
+    McFold fold;                                   // MC samples folded into the batch (rows = 0: off; common.cuh)
 };
 
 constexpr int TC_BM = 128, TC_BN = 64, TC_BK = 64;
@@ -298,7 +299,9 @@ __device__ __noinline__ void store_row16(const StoreCfg p, int b, int pos, int n
 // ------------------------------------------------------------ (P) weight prep
 // One CTA per (n-tile, k-block) 64x64 tile (grid-stride).  256 threads: item = (row, 8-wide
 // K chunk); consecutive threads take consecutive rows so the 16-byte writes are contiguous.
-template <int VARIANT, bool TF32>
+// FOLD: BBB fold, one operand set per weight sample, all drawn from the same (mu, sigma) in the same work split as an
+// unfolded call, so the KL sums in the same order (a separate instantiation keeps the unfolded prep as it was).
+template <int VARIANT, bool TF32, bool FOLD = false>
 __global__ void __launch_bounds__(256)
 weight_prep_kernel(const TcArgs p) {
     __shared__ double red[32];
@@ -320,10 +323,12 @@ weight_prep_kernel(const TcArgs p) {
         const int row = item & (TC_BN - 1), chunk = item >> 6;
         const int n = nt * TC_BN + row, k0 = kb * BKE + chunk * CE;
         float w[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f}, s2[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+        float mu8[CE], sg8[CE];                                     // FOLD: kept for the other samples' weights
 #pragma unroll
         for (int e = 0; e < CE; ++e) {
             const int k = k0 + e;
             float wv = 0.0f, sv = 0.0f;
+            mu8[e] = sg8[e] = 0.0f;
             if (n < g.N && k < g.K) {
                 const size_t wi = (size_t)n * g.K + k;
                 const float mu = __ldg(p.w_mu + wi);
@@ -335,15 +340,27 @@ weight_prep_kernel(const TcArgs p) {
                     wv = mu + e_ * sigma;
                 } else wv = mu;
                 if (do_kl) kl_acc += (double)kl_term_fast(mu, sigma, p.prior_mu, p.prior_sigma, p.kl_convention);
+                mu8[e] = mu; sg8[e] = sigma;
             }
             w[e] = wv; s2[e] = sv;
         }
         // canonical K-major core-matrix order inside the 8 KB tile: chunk*1024 + row*16 bytes
         *reinterpret_cast<uint4*>(dst + chunk * (TC_BN * 16) + row * 16) = pack_chunk<TF32>(w);
         if (p.planes == 2) *reinterpret_cast<uint4*>(dst + TC_B_BYTES + chunk * (TC_BN * 16) + row * 16) = pack_chunk<TF32>(s2);
+        if (FOLD) {
+            for (int j = 1; j < p.fold.sets; ++j) {                // sample j: the same element's draw on its own stream
+                const NoiseKey kj = sample_key(nkey, p.fold, j);
+#pragma unroll
+                for (int e = 0; e < CE; ++e) {
+                    const int k = k0 + e;
+                    w[e] = (n < g.N && k < g.K) ? mu8[e] + normal1((size_t)n * g.K + k, kj) * sg8[e] : 0.0f;
+                }
+                *reinterpret_cast<uint4*>(fold_set(dst, p.fold, j) + chunk * (TC_BN * 16) + row * 16) = pack_chunk<TF32>(w);
+            }
+        }
     }
     for (int n = blockIdx.x * blockDim.x + threadIdx.x; n < npad; n += gridDim.x * blockDim.x) {   // bias
-        float bm = 0.0f, bv = 0.0f;
+        float bm = 0.0f, bv = 0.0f, bmu = 0.0f, bsg = 0.0f;
         if (p.has_bias && n < g.N) {
             const float mu = __ldg(p.b_mu + n);
             const float sigma = (stoch || do_kl) ? softplus_sigma_fast(__ldg(p.b_rho + n)) : 0.0f;
@@ -353,9 +370,17 @@ weight_prep_kernel(const TcArgs p) {
                 bm = mu + e_ * sigma;
             } else bm = mu;
             if (do_kl) kl_acc += (double)kl_term_fast(mu, sigma, p.prior_mu, p.prior_sigma, p.kl_convention);
+            bmu = mu; bsg = sigma;
         }
         p.bias_ws[n] = bm;
         p.bias_ws[npad + n] = bv;
+        if (FOLD) {
+            for (int j = 1; j < p.fold.sets; ++j) {
+                float* bj = fold_set(p.bias_ws, p.fold, j);
+                bj[n] = (p.has_bias && n < g.N) ? bmu + normal1((uint64_t)g.N * g.K + n, sample_key(nkey, p.fold, j)) * bsg : 0.0f;
+                bj[npad + n] = 0.0f;
+            }
+        }
     }
     if (do_kl) {
         const double tot = block_sum(kl_acc, red);
@@ -405,8 +430,11 @@ gemm_tc_kernel(const TcArgs p, const int stages) {
 
     const int n_tile = blockIdx.y, m_tile = blockIdx.x;     // M tiles on x: gridDim.x has no 65535 limit
     const int m0 = m_tile * TC_BM, n0 = n_tile * TC_BN;
+    const int rows_here = min(TC_BM, g.M - m0);             // rows of this tile (no m0 + TC_BM: M may lie near 2^31)
     const int chw = g.Cin * g.HW;
     const int img0 = m0 / g.OHW;
+    // BBB fold: the operand set of this tile's weight sample ((rows * OHW) % TC_BM == 0: the tile lies inside one sample)
+    const int wset = p.fold.sets > 1 ? img0 / p.fold.rows : 0;
 
     long long* tr = p.trace ? p.trace + (size_t)(blockIdx.y * gridDim.x + blockIdx.x) * 128 : nullptr;
     if (tr && threadIdx.x == 0) tr[0] = clock64();
@@ -428,7 +456,7 @@ gemm_tc_kernel(const TcArgs p, const int stages) {
     if (p.stage_x) {
         // the tile's input images, loaded once and coalesced; the im2col gather then reads shared memory
         // (LDS latency ~30 cycles) instead of issuing 64 dependent-latency global loads per thread and k-block
-        const int last = min(m0 + TC_BM - 1, g.M - 1) / g.OHW;
+        const int last = (m0 + rows_here - 1) / g.OHW;
         const int nflt = (last - img0 + 1) * chw;
         const float* src = reinterpret_cast<const float*>(p.x) + (size_t)img0 * chw;
         const bool vec = ((reinterpret_cast<uintptr_t>(src) | (uintptr_t)(nflt * 4)) & 15u) == 0;
@@ -450,8 +478,9 @@ gemm_tc_kernel(const TcArgs p, const int stages) {
     }
     if (threadIdx.x < 64) {
         const int npad_ = p.n_tiles * TC_BN;
-        ctl->bias[threadIdx.x] = p.bias_ws[n0 + threadIdx.x];
-        ctl->bvar[threadIdx.x] = p.bias_ws[npad_ + n0 + threadIdx.x];
+        const float* bias_ws = fold_set(p.bias_ws, p.fold, wset);
+        ctl->bias[threadIdx.x] = bias_ws[n0 + threadIdx.x];
+        ctl->bvar[threadIdx.x] = bias_ws[npad_ + n0 + threadIdx.x];
     }
     if (threadIdx.x == 0) {
         for (int s = 0; s < stages; ++s) {
@@ -469,8 +498,8 @@ gemm_tc_kernel(const TcArgs p, const int stages) {
         // main loop and 32 of the 64 output columns in the epilogue.  Warpgroup wg (== half) multiplies tile rows
         // [64 wg, 64 wg + 64): its wgmma of k-block kb runs while the same threads gather k-block kb + 1.
         const int t = threadIdx.x & 127, half = threadIdx.x >> 7;   // row of the tile
-        const int m = m0 + t;
-        const bool mvalid = m < g.M;
+        const bool mvalid = t < rows_here;
+        const int m = m0 + (mvalid ? t : 0);
         int ih0 = 0, iw0 = 0; long xb = 0;
         int bimg = 0, pix = 0;
         int pwin = 0;                                  // pooled-window index (pool mode)
@@ -553,7 +582,8 @@ gemm_tc_kernel(const TcArgs p, const int stages) {
         // ================= epilogue ============================================
         // (1) LRT noise for this row, 8 columns at a time, drawn while the last MMAs drain
         const bool philox = two && !p.eps_a;
-        const NoiseKey nkey = effective_key(p.key, p.stream_base);
+        int b_s;                                        // image index within its MC sample (== bimg unless folded)
+        const NoiseKey nkey = fold_key(effective_key(p.key, p.stream_base), p.fold, bimg, b_s);
         if (tr && threadIdx.x == 0) tr[5] = clock64();
         const int ohw_out = p.pool ? (g.OHW >> 2) : g.OHW;
         const int opix = p.pool ? pwin : pix;
@@ -569,7 +599,7 @@ gemm_tc_kernel(const TcArgs p, const int stages) {
                 for (int h = 0; h < 2; ++h) {
                     float4 z = make_float4(0.f, 0.f, 0.f, 0.f);
                     if (mvalid && nb + 4 * h < g.N) {
-                        const uint64_t o4 = ((uint64_t)bimg * g.OHW + pix) * g.N + nb + 4 * h;   // NHWC-flat element index
+                        const uint64_t o4 = ((uint64_t)b_s * g.OHW + pix) * g.N + nb + 4 * h;   // NHWC-flat element index
                         if ((g.N & 3) == 0) z = normal4(o4 >> 2, nkey);
                         else { z.x = normal1(o4, nkey); z.y = normal1(o4 + 1, nkey); z.z = normal1(o4 + 2, nkey); z.w = normal1(o4 + 3, nkey); }
                     }
@@ -623,7 +653,7 @@ gemm_tc_kernel(const TcArgs p, const int stages) {
         // whole warp waits (a blocking try_wait with one active lane can be woken late), lane 0 issues
         {
             const uint32_t bytes = (uint32_t)planes * TC_B_BYTES;
-            const uint8_t* src0 = reinterpret_cast<const uint8_t*>(p.wtiles) + (size_t)n_tile * p.k_blocks * planes * TC_B_BYTES;
+            const uint8_t* src0 = reinterpret_cast<const uint8_t*>(fold_set(p.wtiles, p.fold, wset)) + (size_t)n_tile * p.k_blocks * planes * TC_B_BYTES;
             for (int kb = 0; kb < p.k_blocks; ++kb) {
                 const int s = kb % stages;
                 const uint32_t ph = (uint32_t)(kb / stages) & 1u;
@@ -653,14 +683,18 @@ inline cudaError_t launch_fwd_tc_t(TcArgs a, cudaStream_t st, int* n_launch) {
         // Same shared-memory carve-out as the GEMM kernels: an SM only changes its L1/smem split when idle, so prep
         // CTAs running at the default (small-smem) split kept the first GEMM's CTAs off every SM they touched until
         // their grids drained (tools/timeline.py shows the start of each GEMM).
+        // A BBB fold (one operand set per weight sample) keeps the grid, so its KL sums in the unfolded call's order.
+        const bool fold = VARIANT == BBB_VARIANT_BBB && a.fold.sets > 1;
+        auto* prep = fold ? weight_prep_kernel<VARIANT, TF32, true> : weight_prep_kernel<VARIANT, TF32, false>;
         static const bool carve = [] {
             const char* e = getenv("BBB_B200_PREP_CARVEOUT");
             if (e && e[0] == '0') return false;
-            cudaFuncSetAttribute(weight_prep_kernel<VARIANT, TF32>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+            cudaFuncSetAttribute(weight_prep_kernel<VARIANT, TF32, false>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+            cudaFuncSetAttribute(weight_prep_kernel<VARIANT, TF32, true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
             return true;
         }();
         (void)carve;
-        weight_prep_kernel<VARIANT, TF32><<<grid, 256, 0, st>>>(a);
+        prep<<<grid, 256, 0, st>>>(a);
         cudaError_t e = cudaGetLastError();
         if (e != cudaSuccess) return e;
         *n_launch += 1;
@@ -684,7 +718,7 @@ inline cudaError_t launch_fwd_tc_t(TcArgs a, cudaStream_t st, int* n_launch) {
         if (!TF32 && 2 * (smem + xs_elems * 4 + 1024) > per_sm && 2 * ((smem + xs_elems * 2 + 127) / 128 * 128 + 1024) <= per_sm) a.stage_x = 2;
         smem += xs_elems * (a.stage_x == 2 ? 2 : 4);
     }
-    dim3 grid((g.M + TC_BM - 1) / TC_BM, a.n_tiles);
+    dim3 grid((g.M - 1) / TC_BM + 1, a.n_tiles);       // not (M + TC_BM - 1): M may lie near 2^31
     auto* kernel = a.planes == 2 ? gemm_tc_kernel<VARIANT, TF32, VARIANT == BBB_VARIANT_LRT> : gemm_tc_kernel<VARIANT, TF32, false>;
     cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
     cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);

@@ -53,6 +53,7 @@ class _Noise(threading.local):
         self.counter = 0
         self.queue = None          # external-eps queue (parity mode)
         self.base = None           # device int64[1] stream base (CUDA-graph capture mode)
+        self.fold = None           # (rows per MC sample, Philox stream stride) of layer_fold
 
     def current_seed(self) -> int:
         if not self.explicit:
@@ -118,6 +119,25 @@ def stream_base(base: Optional[torch.Tensor]):
         yield
     finally:
         _noise.base, _noise.counter = prev, prev_ctr
+
+
+@contextlib.contextmanager
+def layer_fold(rows: int, stride: int):
+    """Layer calls inside fold Monte-Carlo samples into the batch (include/bbb_b200.h, bbb_conv2d_forward): image b of
+    the batch is image b % rows of sample b // rows, which draws from Philox stream stream_id + (b // rows) * stride --
+    the same numbers as one call per sample.  What uncertainty_estimation.py:38-41 does by repeating the input, with
+    each repeat its own sample.  Forward only, in-kernel noise only: a layer call under autograd or with external eps
+    raises EngineError."""
+    prev = _noise.fold
+    _noise.fold = (int(rows), int(stride))
+    try:
+        yield
+    finally:
+        _noise.fold = prev
+
+
+def layer_fold_active() -> bool:
+    return _noise.fold is not None
 
 
 def noise_advance(base: torch.Tensor, inc: int):
@@ -239,7 +259,8 @@ def workspace(device, desc=None, owner=None) -> torch.Tensor:
 
 def make_desc(x_shape, w_shape, conv, variant, sample, has_bias, prior_mu, prior_sigma,
               math=L.MATH_FP32, kl_convention=L.KL_REFERENCE, act=L.ACT_NONE,
-              act_dtype=L.DTYPE_F32) -> L.LayerDesc:
+              act_dtype=L.DTYPE_F32, fold=None) -> L.LayerDesc:
+    """``fold`` = (rows per MC sample, Philox stream stride): the desc folds MC samples into its batch (layer_fold)."""
     d = L.LayerDesc()
     if conv is None:
         d.batch, d.in_channels, d.in_h, d.in_w = x_shape[0], x_shape[1], 1, 1
@@ -255,6 +276,11 @@ def make_desc(x_shape, w_shape, conv, variant, sample, has_bias, prior_mu, prior
     d.act_dtype, d.math, d.kl_convention, d.epilogue_act = act_dtype, math, kl_convention, act
     d.pool_k = d.pool_s = 0
     d.prior_mu, d.prior_sigma = float(prior_mu), float(prior_sigma)
+    if fold is not None:
+        rows, stride = fold
+        d.reserved[1] = int(rows)
+        d.reserved[2] = C.c_int32(stride & 0xFFFFFFFF).value
+        d.reserved[3] = C.c_int32((stride >> 32) & 0xFFFFFFFF).value
     return d
 
 
@@ -358,8 +384,14 @@ class BayesLayerFn(torch.autograd.Function):
             x = x.float()
         W_mu_c, W_rho_c = W_mu.contiguous(), W_rho.contiguous()
         has_bias = bias_mu is not None
+        need_grad = any(ctx.needs_input_grad[:5])      # grad mode is off inside Function.forward
+        fold = _noise.fold
+        if fold is not None and need_grad and cfg.get("grad_enabled", True):
+            raise L.EngineError("layer_fold: MC-sample folding is forward-only (call under torch.no_grad())")
+        if fold is not None and external_eps_active():
+            raise L.EngineError("layer_fold: MC-sample folding draws its noise in-kernel (no external eps)")
         d = make_desc(tuple(x.shape), tuple(W_mu.shape), conv, variant, sample, has_bias,
-                      cfg["prior_mu"], cfg["prior_sigma"], cfg["math"], cfg["kl_convention"], cfg["act"])
+                      cfg["prior_mu"], cfg["prior_sigma"], cfg["math"], cfg["kl_convention"], cfg["act"], fold=fold)
         if conv is None:
             if x.dim() != 2 or x.shape[1] != W_mu.shape[1]:
                 raise L.EngineError(f"linear: x {tuple(x.shape)} vs weight {tuple(W_mu.shape)}")
@@ -385,7 +417,6 @@ class BayesLayerFn(torch.autograd.Function):
             else:
                 seed, stream_id = next_stream()
                 base = _noise.base
-        need_grad = any(ctx.needs_input_grad[:5])      # grad mode is off inside Function.forward
         act_std = None
         if variant == L.VARIANT_LRT and sample and need_grad:
             act_std = torch.empty(yshape, dtype=torch.float32, device=dev)

@@ -48,6 +48,72 @@ def get_beta(batch_idx, m, beta_type, epoch=None, num_epochs=None):
     return 0
 
 
+# Memory budget of one folded pass on the per-layer path (MCForward, nets the fused chain does not take): G samples share
+# a pass while G times the bytes one sample's pass holds at once stays within it.  Chosen from tools/mc_layer_fold_bench.py
+# on C5 (one H100 80GB HBM3, 400 W power limit; README, Status): one step at a time G = 2 / 4 / 8 / 15 took 483 / 477 /
+# 473 / 475 ms against 496 ms sample by sample, but with four steps in flight G = 4 / 8 took 470 / 478 ms against 466 ms.
+# 2 GiB (G = 4 for C5) keeps most of the first gain and stays near even in flight.
+LAYER_FOLD_BUDGET = 2 << 30
+_INT32_MAX = (1 << 31) - 1
+
+
+def layer_fold_groups(n_local: int, pass_bytes: int, max_elems: int, budget: int = LAYER_FOLD_BUDGET,
+                      fold_group: Optional[int] = None):
+    """How the per-layer fold groups a rank's ``n_local`` samples: a list of (first local index, size), consecutive and
+    covering every local index once, in order, with sizes as equal as possible; None when no group would hold two samples.
+    ``pass_bytes``: what one sample's pass holds at once (the largest fp32 input + output of any of its modules; aten ops
+    between the layers are not in place).  ``max_elems``: the largest element count of one sample's activations -- a
+    layer call keeps its counts in int32, so a group never exceeds 2^31 - 1 elements.  ``fold_group`` (> 0) replaces the
+    byte budget as the largest group size."""
+    cap = _INT32_MAX // max(1, int(max_elems))
+    want = int(fold_group) if fold_group is not None else int(budget) // max(1, int(pass_bytes))
+    g = min(int(n_local), want, cap)
+    if g < 2:
+        return None
+    n = -(-int(n_local) // g)
+    q, r = divmod(int(n_local), n)
+    groups, start = [], 0
+    for i in range(n):
+        size = q + (1 if i < r else 0)
+        groups.append((start, size))
+        start += size
+    return groups
+
+
+def _per_image_chain(kids, x_shape):
+    """What the children of a ModuleWrapper do, run one after another on a batch of ``x_shape``: (the Bayesian layers
+    with their input shapes, pass bytes, largest element count) -- or None when a child is not known to treat every image
+    on its own (then folding samples into the batch could change a result)."""
+    import math
+    from torch import nn
+    from .modules import FlattenLayer, _BayesLayer
+    shape, layers, pass_bytes, big = tuple(x_shape), [], 0, 0
+    for m in kids:
+        if isinstance(m, _BayesLayer):
+            conv = m._conv_geometry()
+            if conv is None:
+                if len(shape) != 2 or shape[1] != m.in_features:
+                    return None
+                out = (shape[0], m.out_features)
+            else:
+                if len(shape) != 4 or shape[1] != m.in_channels:
+                    return None
+                out = (shape[0], m.out_channels) + Fn.out_hw(shape[2], shape[3], *m.kernel_size, conv)
+            layers.append((m, shape))
+        elif isinstance(m, FlattenLayer):
+            if math.prod(shape[1:]) != m.num_features:
+                return None                                  # view(-1, F) would mix the images of the batch
+            out = (shape[0], m.num_features)
+        elif isinstance(m, (nn.Softplus, nn.ReLU, nn.MaxPool2d)):
+            out = tuple(m(torch.empty(shape, device="meta")).shape)
+        else:
+            return None
+        a, b = math.prod(shape), math.prod(out)
+        pass_bytes, big = max(pass_bytes, 4 * (a + b)), max(big, a, b)
+        shape = out
+    return layers, pass_bytes, big
+
+
 def _dist_info(group):
     import torch.distributed as dist
     on = dist.is_available() and dist.is_initialized()
@@ -65,7 +131,8 @@ class MCForward:
     def __init__(self, net, example_x: torch.Tensor, num_ens: int, group=None, want_uncertainty: bool = False,
                  normalized: bool = False, with_labels: bool = False, train_size: float = 1.0, beta: float = 0.0,
                  seed: Optional[int] = None, graph: bool = True, num_classes: Optional[int] = None,
-                 static_inputs=None, first_replay: int = 0, fold: bool = True, overlap: bool = False, inflight: int = 1):
+                 static_inputs=None, first_replay: int = 0, fold: bool = True, overlap: bool = False, inflight: int = 1,
+                 fold_group: Optional[int] = None, fold_budget: int = LAYER_FOLD_BUDGET):
         """``static_inputs``: device tensors the caller fills in place (e.g. targets of its host->device copies, or a
         rotation of resident batches); one graph is captured per tensor and ``self(slot=k)`` runs the step on
         ``static_inputs[k]`` with no staging copy.  ``first_replay``: index of the first replay's noise block.
@@ -75,7 +142,9 @@ class MCForward:
         current stream (a device synchronize covers it too).  ``inflight=k`` (with ``overlap``): consecutive steps are
         independent, so steps t, t+1, .. t+k-1 run on k streams with their own layer workspaces and Philox counters -- the
         head of step t+1 (parameter preps, first layers) fills the SMs the tail of step t leaves idle.  Results are
-        identical to the serial engine; ``wait()`` also covers the inputs (they may be rewritten afterwards)."""
+        identical to the serial engine; ``wait()`` also covers the inputs (they may be rewritten afterwards).
+        ``fold_group``: the largest number of samples one pass of the per-layer fold takes (nets the fused chain does not
+        take); None = as many as ``fold_budget`` bytes of activations allow (layer_fold_groups)."""
         Fn._require_cuda(example_x, "MCForward")
         lib = L.lib()
         self.net, self.group = net, group
@@ -145,12 +214,55 @@ class MCForward:
         if fold and len(self.ids) > 1 and one_variant:
             self.fold = (self.B, self.world << 40)
             self.fold_steps = fused.plan(kids, (len(self.ids) * self.B,) + tuple(example_x.shape[1:]), self.fold)
+        # Nets the fused chain does not take (BBBLeNet, BBB3Conv3FC) fold on the per-layer path instead: groups of G
+        # consecutive local samples, one pass of the tensor-core layer kernels over G x B rows each (Fn.layer_fold), with
+        # the aten activations / pools between them -- per-image ops, so every output equals the sample loop's bit for bit.
+        # layer_fold = (G, number of groups) when it does.
+        self.layer_fold, self._groups = None, None
+        if self.fold_steps is None and fold and len(self.ids) > 1:
+            self._groups = self._plan_layer_fold(net, kids, example_x, fold_group, fold_budget)
+        if self._groups is not None:
+            G = max(n for _, n in self._groups)
+            self.layer_fold = (G, len(self._groups))
+            # the first layer's input: x repeated G times, one buffer per concurrently running step
+            self.xrep_all = [torch.empty((G * B,) + tuple(example_x.shape[1:]), dtype=example_x.dtype, device=dev)
+                             for _ in range(nbuf)]
         self.graph, self.graphs = None, []
         self.result_stream = None                 # overlap mode: the stream the results are complete on
         self.replays = 0
         self.kernels_per_step = None
         if graph:
             self._capture()
+
+    def _plan_layer_fold(self, net, kids, example_x, fold_group, budget):
+        """The groups of the per-layer fold (layer_fold_groups), or None: the net runs on the fused chain unfolded (it
+        then keeps the fused fold or the sample loop), a child is not a per-image op, or the engine would refuse a
+        Bayesian layer's folded call (bbb_forward_supported: e.g. math='fp32', or a BBB layer whose 128-row tiles would
+        straddle two samples)."""
+        from . import fused
+        from .modules import ModuleWrapper, _default_fuse
+        if not kids or type(net).forward is not ModuleWrapper.forward:
+            return None
+        shape = tuple(example_x.shape)
+        if getattr(net, "fuse", _default_fuse()) and fused.plan(kids, shape) is not None:
+            return None
+        chain = _per_image_chain(kids, shape)
+        if chain is None:
+            return None
+        layers, pass_bytes, big = chain
+        groups = layer_fold_groups(len(self.ids), pass_bytes, big, budget, fold_group)
+        if groups is None:
+            return None
+        lib = L.lib()
+        for n in sorted({n for _, n in groups}):
+            for m, xs in layers:
+                cfg = m._cfg(True)
+                d = Fn.make_desc((n * xs[0],) + tuple(xs[1:]), tuple(m.W_mu.shape), cfg["conv"], cfg["variant"], True,
+                                 m.bias_mu is not None, cfg["prior_mu"], cfg["prior_sigma"], cfg["math"],
+                                 cfg["kl_convention"], cfg["act"], fold=(self.B, self.world << 40))
+                if lib.bbb_forward_supported(C.byref(d)) != 0:
+                    return None
+        return groups
 
     # -- peer-mapped receive buffers (CUDA IPC; handles travel over torch.distributed) -----------------------
     def _open_peers(self, nbytes):
@@ -221,7 +333,22 @@ class MCForward:
                                         fold=self.fold, kls_out=kl_buf)
                 self._kl_terms = kls
                 kl_ptr, n_kl = Fn._ptr(kls), kls.numel()
-            for k, j in enumerate(self.ids if self.fold_steps is None else ()):
+            if self._groups is not None:
+                # group (s0, n): local samples s0 .. s0+n-1 in one pass over n x B rows; row block k is global sample
+                # ids[s0] + k * world (stream stride world << 40, as in the fused fold) and lands in logits_buf[s0 + k]
+                xr = self.xrep_all[par]
+                G = self.layer_fold[0]
+                xr.view((G,) + tuple(x.shape)).copy_(x.unsqueeze(0).expand((G,) + tuple(x.shape)))
+                for gi, (s0, n) in enumerate(self._groups):
+                    with Fn.stream_base(base), Fn.mc_sample(self.ids[s0], self.seed), \
+                            Fn.layer_fold(self.B, self.world << 40):
+                        logits, kl = self.net(xr[:n * self.B])
+                    logits_buf[s0:s0 + n].view(n * self.B, self.C).copy_(logits.reshape(n * self.B, self.C))
+                    if gi == 0:                               # every sample has the same KL, computed once per pass
+                        one = self.kl_one_all[par:par + 1]
+                        one.copy_(torch.as_tensor(kl, dtype=torch.float32, device=self.dev).reshape(1))
+                        kl_ptr, n_kl = Fn._ptr(one), 1
+            for k, j in enumerate(self.ids if self.fold_steps is None and self._groups is None else ()):
                 with Fn.stream_base(base), Fn.mc_sample(j, self.seed), \
                         fused.direct_output(logits_buf[k], kl_buf if k == 0 else None) as hook:
                     logits, kl = self.net(x)
@@ -277,6 +404,17 @@ class MCForward:
         # GEMM chain on a HIGH-priority stream, parameter preps on the (default-priority) side streams: when both have CTAs
         # pending, the chain's go first -- the preps of later layers no longer keep the first GEMM's CTAs off the SMs
         cap = torch.cuda.Stream(device=dev, priority=-1)
+        # A folded pass of the per-layer path holds up to fold_budget bytes of activations, which a captured graph keeps in
+        # its memory pool: the chain graphs that never run at the same time (one per resident input, same buffer parity)
+        # share one pool instead of one each.
+        pools = {}
+
+        def pool_kw(par):
+            return {"pool": pools.get(par)} if self._groups is not None else {}
+
+        def keep_pool(par, g):
+            if self._groups is not None:
+                pools.setdefault(par, g.pool())
         if self.overlap:
             # two graphs per step: the layer chain (per resident input and buffer parity) and the exchange kernel (per
             # parity); __call__ replays the second on its own stream so that it runs beside the next step's chain
@@ -288,8 +426,9 @@ class MCForward:
                 for xin in self.inputs:
                     g = torch.cuda.CUDAGraph()
                     n0 = L.launch_count()
-                    with torch.cuda.graph(g, stream=cap):
+                    with torch.cuda.graph(g, stream=cap, **pool_kw(par)):
                         kl_ptr, n_kl = self._chain(xin, self._bases[par], advance=True, par=par)
+                    keep_pool(par, g)
                     n_chain = L.launch_count() - n0
                     self.chain_graphs[par].append(g)
                 g = torch.cuda.CUDAGraph()
@@ -311,8 +450,9 @@ class MCForward:
         for xin in (() if self.overlap else self.inputs):
             g = torch.cuda.CUDAGraph()
             n0 = L.launch_count()
-            with torch.cuda.graph(g, stream=cap):
+            with torch.cuda.graph(g, stream=cap, **pool_kw(0)):
                 self._step(xin, self.base, advance=True)
+            keep_pool(0, g)
             self.kernels_per_step = L.launch_count() - n0          # engine kernels captured in one step
             self.graphs.append(g)
         self.graph = self.graphs[0]

@@ -58,6 +58,8 @@ class ModuleWrapper(nn.Module):
         """Run the children as a fused tensor-core chain if they match (see fused.py); None = not fusable."""
         if not (torch.is_tensor(x) and x.is_cuda and x.dim() == 4) or not getattr(self, "fuse", _default_fuse()):
             return None
+        if Fn.layer_fold_active():
+            return None                                    # MC samples folded on the per-layer path (Fn.layer_fold)
         if torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for p in self.parameters())):
             return None                                    # the fused chain is forward-only
         from . import fused
@@ -169,8 +171,9 @@ class _BayesLayer(ModuleWrapper):
 
     def forward(self, x, sample=True):
         stochastic = bool(self.training or sample)      # BBB/BBBConv.py:62, BBB_LRT/BBBConv.py:77
-        y, kl = Fn.BayesLayerFn.apply(x, self.W_mu, self.W_rho, self.bias_mu, self.bias_rho,
-                                      self._cfg(stochastic))
+        cfg = self._cfg(stochastic)
+        cfg["grad_enabled"] = torch.is_grad_enabled()  # grad mode is always off inside Function.forward
+        y, kl = Fn.BayesLayerFn.apply(x, self.W_mu, self.W_rho, self.bias_mu, self.bias_rho, cfg)
         self._kl_cache = (kl, self._versions(), torch.is_grad_enabled())
         return y
 
