@@ -250,8 +250,10 @@ int bbb_mc_combine(const float* logits, int32_t S, int32_t B, int32_t C,
  * kl: n_kl device floats whose SUM is one sample's KL (e.g. the per-layer scalars the layer calls wrote: the sum over
  *   layers of ModuleWrapper.forward, layers/misc.py:21-23, happens here); n_kl <= 0 means 1.
  * noise_base (nullable): *noise_base += noise_inc when the launch has finished -- the last kernel of a captured step
- *   moves the Philox stream base for the next replay (replaces a leading bbb_noise_advance launch). */
-enum { BBB_MC_MOMENTS = 1, BBB_MC_NORMALIZED = 2 };
+ *   moves the Philox stream base for the next replay (replaces a leading bbb_noise_advance launch).
+ * BBB_MC_INFO (needs BBB_MC_MOMENTS; see bbb_mc_exchange_info) adds one [B] plane per rank to the receive buffer:
+ *   bbb_mc_buffer_bytes grows only when the flag is set, and returns 0 for BBB_MC_INFO without BBB_MC_MOMENTS. */
+enum { BBB_MC_MOMENTS = 1, BBB_MC_NORMALIZED = 2, BBB_MC_INFO = 4 };
 size_t bbb_mc_buffer_bytes(int32_t B, int32_t C, int32_t flags, int32_t world);
 size_t bbb_mc_state_bytes(void);
 int bbb_mc_exchange(const float* logits, int32_t S_local, int32_t S_total, int32_t B, int32_t C, const float* kl,
@@ -259,6 +261,24 @@ int bbb_mc_exchange(const float* logits, int32_t S_local, int32_t S_total, int32
                     int32_t world, void* const* peer_buffers, void* state, float* log_outputs, float* kl_out, float* pred,
                     float* epistemic, float* aleatoric, float* entropy, float* head, uint64_t* noise_base,
                     uint64_t noise_inc, void* cuda_stream);
+/* bbb_mc_exchange plus the rest of the entropy decomposition  H[p_bar] = E_s H[p_hat_s] + I(y; w)  (total = expected
+ * entropy, the aleatoric part + mutual information / BALD, the epistemic part), for each image b:
+ *   p_hat_s            the per-sample probabilities the moments use: softmax(logits_s), or with BBB_MC_NORMALIZED
+ *                      softplus(logits_s) / sum softplus (uncertainty_estimation.py:73-77)
+ *   H[p]               = -sum_c p_c log p_c with 0 log 0 = 0 (a class whose probability underflows to 0 adds nothing)
+ *   expected_entropy[b] = (1/S_total) sum_{s over all ranks} H[p_hat_s]
+ *   mutual_info[b]     = entropy[b] - expected_entropy[b], in fp32 and NOT clamped: rounding may leave it slightly
+ *                        negative where the samples agree
+ * expected_entropy / mutual_info: [B] fp32 each, nullable.  They need flags & BBB_MC_INFO, which needs
+ * BBB_MC_MOMENTS (H[p_bar] comes from the sum-p plane); otherwise BBB_E_INVALID.  Each rank pushes one more word per
+ * image (the sum of H[p_hat_s] over its samples; 0 without samples); the sums are finished in rank order, so the outputs
+ * are bitwise identical on every rank.  Without BBB_MC_INFO this is bbb_mc_exchange: the same kernel and results. */
+int bbb_mc_exchange_info(const float* logits, int32_t S_local, int32_t S_total, int32_t B, int32_t C, const float* kl,
+                         int32_t n_kl, int32_t flags, const int64_t* labels, float train_size, float beta, int32_t rank,
+                         int32_t world, void* const* peer_buffers, void* state, float* log_outputs, float* kl_out,
+                         float* pred, float* epistemic, float* aleatoric, float* entropy, float* head,
+                         uint64_t* noise_base, uint64_t noise_inc, float* expected_entropy, float* mutual_info,
+                         void* cuda_stream);
 
 /* Peer-mapped receive buffers for bbb_mc_exchange (one process per GPU, same node): allocate locally, export a
  * 64-byte CUDA-IPC handle, ship it to the peers by any host channel (the Python side uses torch.distributed),

@@ -445,15 +445,16 @@ int bbb_mc_combine(const float* logits, int32_t S, int32_t B, int32_t C, float* 
 
 size_t bbb_mc_buffer_bytes(int32_t B, int32_t C, int32_t flags, int32_t world) {
     if (B <= 0 || C <= 0 || world <= 0 || world > bbb::MCX_MAX_RANKS) return 0;
-    return bbb::mcx_buffer_bytes(B, C, flags & BBB_MC_MOMENTS, world);
+    if ((flags & BBB_MC_INFO) && !(flags & BBB_MC_MOMENTS)) return 0;
+    return bbb::mcx_buffer_bytes(B, C, flags & BBB_MC_MOMENTS, world, (flags & BBB_MC_INFO) != 0);
 }
 size_t bbb_mc_state_bytes(void) { return 64 + (size_t)bbb::MCX_MAX_CTAS * 2 * sizeof(double); }
 
-int bbb_mc_exchange(const float* logits, int32_t S_local, int32_t S_total, int32_t B, int32_t C, const float* kl,
-                    int32_t n_kl, int32_t flags, const int64_t* labels, float train_size, float beta, int32_t rank, int32_t world,
-                    void* const* peer_buffers, void* state, float* log_outputs, float* kl_out, float* pred,
-                    float* epistemic, float* aleatoric, float* entropy, float* head, uint64_t* noise_base,
-                    uint64_t noise_inc, void* cuda_stream) {
+int bbb_mc_exchange_info(const float* logits, int32_t S_local, int32_t S_total, int32_t B, int32_t C, const float* kl,
+                         int32_t n_kl, int32_t flags, const int64_t* labels, float train_size, float beta, int32_t rank,
+                         int32_t world, void* const* peer_buffers, void* state, float* log_outputs, float* kl_out, float* pred,
+                         float* epistemic, float* aleatoric, float* entropy, float* head, uint64_t* noise_base,
+                         uint64_t noise_inc, float* expected_entropy, float* mutual_info, void* cuda_stream) {
     if (!log_outputs || !peer_buffers || !state) return fail(BBB_E_INVALID, "NULL pointer");
     if (S_local < 0 || S_total <= 0 || B <= 0 || C <= 0) return fail(BBB_E_INVALID, "bad S/B/C");
     if (S_local > 0 && !logits) return fail(BBB_E_INVALID, "S_local > 0 but logits is NULL");
@@ -461,6 +462,10 @@ int bbb_mc_exchange(const float* logits, int32_t S_local, int32_t S_total, int32
     if (world < 1 || world > bbb::MCX_MAX_RANKS || rank < 0 || rank >= world) return fail(BBB_E_INVALID, "bad rank/world %d/%d", rank, world);
     if ((pred || epistemic || aleatoric || entropy) && !(flags & BBB_MC_MOMENTS))
         return fail(BBB_E_INVALID, "uncertainty outputs need BBB_MC_MOMENTS");
+    const bool info = (flags & BBB_MC_INFO) != 0;
+    if (info && !(flags & BBB_MC_MOMENTS)) return fail(BBB_E_INVALID, "BBB_MC_INFO needs BBB_MC_MOMENTS");
+    if ((expected_entropy || mutual_info) && !info)
+        return fail(BBB_E_INVALID, "expected_entropy / mutual_info need BBB_MC_INFO");
     bbb::McxArgs a;
     a.logits = logits; a.kl = kl; a.n_kl = kl ? (n_kl > 0 ? n_kl : 1) : 0; a.S_local = S_local; a.S_total = S_total; a.B = B; a.C = C;
     a.want_moments = (flags & BBB_MC_MOMENTS) ? 1 : 0; a.normalized = (flags & BBB_MC_NORMALIZED) ? 1 : 0;
@@ -475,17 +480,28 @@ int bbb_mc_exchange(const float* logits, int32_t S_local, int32_t S_total, int32
     a.head_partials = (double*)((char*)state + 64);
     a.log_outputs = log_outputs; a.kl_out = kl_out; a.pred = pred; a.epistemic = epistemic; a.aleatoric = aleatoric;
     a.entropy = entropy; a.head = head; a.trace = g_mcx_trace;
+    a.expected_entropy = expected_entropy; a.mutual_info = mutual_info;
     { bbb::Geom tg = {}; tg.M = B; tg.N = C; tg.K = S_local; a.tl = tl_slot(true, "mc_exchange", tg); }
     // the grid depends on B only: CTA c of every rank owns the same images, so flags pair up CTA by CTA.  At most
     // MCX_MAX_CTAS CTAs: all co-resident, so a CTA spinning on a peer's flag never keeps that peer's producer off an SM.
     int grid = (B + bbb::MCX_THREADS / 32 - 1) / (bbb::MCX_THREADS / 32);
     if (grid > bbb::MCX_MAX_CTAS) grid = bbb::MCX_MAX_CTAS;
-    cudaError_t e = bbb::launch_pdl(bbb::mc_exchange_kernel, dim3(grid), dim3(bbb::MCX_THREADS),
-                                     (size_t)(bbb::MCX_THREADS / 32) * S_local * sizeof(float), (cudaStream_t)cuda_stream, a);
+    cudaError_t e = bbb::launch_pdl(info ? bbb::mc_exchange_kernel<true> : bbb::mc_exchange_kernel<false>, dim3(grid),
+                                     dim3(bbb::MCX_THREADS), (size_t)(bbb::MCX_THREADS / 32) * S_local * sizeof(float),
+                                     (cudaStream_t)cuda_stream, a);
     if (e == cudaSuccess) e = cudaGetLastError();
     if (e != cudaSuccess) return cuda_fail(e, "mc_exchange launch");
     g_launches += 1;
     return BBB_OK;
+}
+int bbb_mc_exchange(const float* logits, int32_t S_local, int32_t S_total, int32_t B, int32_t C, const float* kl,
+                    int32_t n_kl, int32_t flags, const int64_t* labels, float train_size, float beta, int32_t rank, int32_t world,
+                    void* const* peer_buffers, void* state, float* log_outputs, float* kl_out, float* pred,
+                    float* epistemic, float* aleatoric, float* entropy, float* head, uint64_t* noise_base,
+                    uint64_t noise_inc, void* cuda_stream) {
+    return bbb_mc_exchange_info(logits, S_local, S_total, B, C, kl, n_kl, flags, labels, train_size, beta, rank, world,
+                                peer_buffers, state, log_outputs, kl_out, pred, epistemic, aleatoric, entropy, head,
+                                noise_base, noise_inc, nullptr, nullptr, cuda_stream);
 }
 
 int bbb_comm_alloc(size_t bytes, void** dev_ptr) {

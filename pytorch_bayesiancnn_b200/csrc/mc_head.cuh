@@ -16,7 +16,15 @@
 //
 // Receive buffer of one rank (all ranks use the same layout):
 //   [0, 4096)                       reserved
-//   [4096, ...)                     u64 data[2 slots][world][n_planes * B * C + 2]
+//   [4096, ...)                     u64 data[2 slots][world][n_planes * B * C + 2 (+ B with INFO)]
+// Per sending rank: the n_planes [B, C] planes, the KL word at n_planes * B * C, a spare word, and -- only in the INFO
+// instantiation -- a plane of B words behind them: sum over the rank's samples of H[p_hat_s] per image.
+//
+// INFO (BBB_MC_INFO) adds the two other terms of the entropy decomposition H[p_bar] = E_s H[p_hat_s] + I(y; w):
+//   H[p]                   = -sum_c p_c log p_c, with 0 log 0 = 0 (a class whose probability underflows adds nothing)
+//   expected_entropy[b]    = (1/S_total) sum_{s over all ranks} H[p_hat_s[b]]      (aleatoric)
+//   mutual_info[b]         = entropy[b] - expected_entropy[b]  in fp32, not clamped: rounding may leave it slightly < 0
+// p_hat_s is the same softmax (or softplus-normalised) row the moments use.
 // Every float travels as ONE 8-byte store {value bits, sequence number} (the "LL" idea of NCCL's low-latency protocol):
 // 8-byte stores are single-copy atomic over NVLink, so the receiver simply polls each word until its tag equals the
 // launch's sequence number -- no fence, no separate flag, no CTA barrier between the push and the finish.  (A fence.sys +
@@ -53,12 +61,16 @@ struct McxArgs {
     float* head;                  // [4]: loss, nll, accuracy, beta*kl; nullable (needs labels)
     long long* tl;                // debug timeline slot (nullptr in production)
     long long* trace;             // debug: [CTA][8] %globaltimer stamps of the handshake (nullptr in production)
+    float* expected_entropy; float* mutual_info;   // [B] each; nullable; written by the INFO instantiation only
 };
 
 __host__ __device__ inline int mcx_planes(int want_moments) { return want_moments ? 5 : 2; }
-__host__ __device__ inline size_t mcx_rank_floats(int B, int C, int want_moments) { return (size_t)mcx_planes(want_moments) * B * C + 2; }
-__host__ inline size_t mcx_buffer_bytes(int B, int C, int want_moments, int world) {
-    return MCX_CTRL_BYTES + 2 * (size_t)world * mcx_rank_floats(B, C, want_moments) * sizeof(unsigned long long);
+__host__ __device__ inline size_t mcx_info_off(int B, int C, int want_moments) { return (size_t)mcx_planes(want_moments) * B * C + 2; }
+__host__ __device__ inline size_t mcx_rank_floats(int B, int C, int want_moments, bool info = false) {
+    return mcx_info_off(B, C, want_moments) + (info ? (size_t)B : 0);
+}
+__host__ inline size_t mcx_buffer_bytes(int B, int C, int want_moments, int world, bool info = false) {
+    return MCX_CTRL_BYTES + 2 * (size_t)world * mcx_rank_floats(B, C, want_moments, info) * sizeof(unsigned long long);
 }
 
 __device__ __forceinline__ void st_ll(unsigned long long* p, float v, unsigned int seq) {
@@ -72,7 +84,9 @@ __device__ __forceinline__ unsigned long long ld_ll(const unsigned long long* p)
 }
 __device__ __forceinline__ float softplus_f(float v) { return v > 20.0f ? v : log1pf(expf(v)); }   // F.softplus(beta=1, threshold=20)
 
-// <= 51 registers: an exchange CTA has to fit beside a GEMM CTA (320 x ~120 registers) and a prep CTA of the next step
+// <= 51 registers: an exchange CTA has to fit beside a GEMM CTA (320 x ~120 registers) and a prep CTA of the next step.
+// INFO: also expected_entropy / mutual_info (the extra plane of the receive buffer); INFO == false is the default kernel.
+template <bool INFO>
 __global__ void __launch_bounds__(MCX_THREADS, 5)
 mc_exchange_kernel(const McxArgs p) {
     // per warp: log-sum-exp (or softplus sum) of each local sample's row -- dynamic, 32 * S_local bytes: next to a 193 KB
@@ -93,7 +107,7 @@ mc_exchange_kernel(const McxArgs p) {
     if (threadIdx.x == 0) seq_sh = *p.seq + 1u;
     __syncthreads();
     const unsigned int seq = seq_sh;
-    const size_t rank_floats = mcx_rank_floats(B, C, p.want_moments);
+    const size_t rank_floats = mcx_rank_floats(B, C, p.want_moments, INFO);
     const size_t slot_off = (size_t)(seq & 1u) * p.world * rank_floats;     // in words, behind the control block
     const float inv_S = 1.0f / (float)p.S_total;
 
@@ -115,8 +129,9 @@ mc_exchange_kernel(const McxArgs p) {
             rf.ent -= pbar > 0.0f ? pbar * logf(pbar) : 0.0f;             // H[p_bar] (no reference, SURVEY D3)
         }
     };
-    // row reductions: entropy, the label's log-probability, argmax (first maximal class, like torch.argmax on ties)
-    auto fin_row = [&](RowFin& rf, int b) {
+    // row reductions: entropy, the label's log-probability, argmax (first maximal class, like torch.argmax on ties);
+    // hsum (INFO): sum over all S_total samples of H[p_hat_s] of this image
+    auto fin_row = [&](RowFin& rf, int b, float hsum) {
         float ent = warp_sum(rf.ent), lab_lp = warp_sum(rf.lab_lp), best = rf.best;
         int best_c = rf.best_c;
 #pragma unroll
@@ -127,6 +142,11 @@ mc_exchange_kernel(const McxArgs p) {
         }
         if (lane == 0) {
             if (p.entropy && p.want_moments) p.entropy[b] = ent;
+            if constexpr (INFO) {
+                const float ee = __fmul_rn(hsum, inv_S);   // not fused into the subtraction: mutual_info == entropy - ee exactly
+                if (p.expected_entropy) p.expected_entropy[b] = ee;
+                if (p.mutual_info) p.mutual_info[b] = ent - ee;
+            }
             if (p.labels) { nll_acc -= (double)lab_lp; hit_acc += (best_c == (int)rf.lab) ? 1.0 : 0.0; }
         }
     };
@@ -166,6 +186,7 @@ mc_exchange_kernel(const McxArgs p) {
         }
         __syncwarp();
         RowFin rf{-INFINITY, 0x7fffffff, 0.0f, 0.0f, (solo && p.labels) ? p.labels[b] : -1};
+        float hl = 0.0f;                                         // INFO: sum over local samples and this lane's classes of -p log p
         for (int c = lane; c < C; c += 32) {
             float mx = -INFINITY, acc = 0.0f, sp = 0.0f, sp2 = 0.0f, sl = 0.0f;
             for (int s = 0; s < p.S_local; ++s) {
@@ -176,6 +197,7 @@ mc_exchange_kernel(const McxArgs p) {
                 if (lp > mx) { acc = acc * expf(mx - lp) + 1.0f; mx = lp; }  // online logsumexp over the samples
                 else if (lp > -INFINITY) acc += expf(lp - mx);               // lp == -inf: a probability of exactly 0 adds nothing
                 sp += pr; sp2 += pr * pr; sl += l;
+                if constexpr (INFO) hl -= pr > 0.0f ? pr * lp : 0.0f;       // 0 log 0 = 0, not 0 * -inf
             }
             const size_t e = (size_t)b * C + c;
             if (solo) { fin_elem(rf, e, c, mx, acc, sp, sp2, sl); continue; }
@@ -185,7 +207,14 @@ mc_exchange_kernel(const McxArgs p) {
                 if (p.want_moments) { st_ll(dst + 2 * (size_t)BC + e, sp, seq); st_ll(dst + 3 * (size_t)BC + e, sp2, seq); st_ll(dst + 4 * (size_t)BC + e, sl, seq); }
             }
         }
-        if (solo) fin_row(rf, b);
+        float hloc = 0.0f;                                       // INFO: sum over the local samples of H[p_hat_s]
+        if constexpr (INFO) {
+            hloc = warp_sum(hl);
+            if (!solo && lane < p.world)                         // a rank without samples pushes 0
+                st_ll(reinterpret_cast<unsigned long long*>(p.peer[lane] + MCX_CTRL_BYTES) + slot_off + (size_t)p.rank * rank_floats +
+                          mcx_info_off(B, C, p.want_moments) + b, hloc, seq);
+        }
+        if (solo) fin_row(rf, b, hloc);
         __syncwarp();
     }
     float kl_solo = 0.0f;
@@ -243,7 +272,16 @@ mc_exchange_kernel(const McxArgs p) {
                 const float sp = mom[0], sp2 = mom[1], sl = mom[2];
                 fin_elem(rf, e, c, M, tot, sp, sp2, sl);
             }
-            fin_row(rf, b);
+            float hsum = 0.0f;
+            if constexpr (INFO) {       // lane q fetches rank q's word (one round trip); every lane adds them in rank order
+                float hq = 0.0f;
+                if (lane < p.world) {
+                    const unsigned long long* w = rx + (size_t)lane * rank_floats + mcx_info_off(B, C, p.want_moments) + b;
+                    hq = ll_value(ld_ll(w), w);
+                }
+                for (int q = 0; q < p.world; ++q) hsum += __shfl_sync(0xffffffffu, hq, q);
+            }
+            fin_row(rf, b, hsum);
         }
     }
     // ---- (5) cross-CTA finish (deterministic order), KL, ELBO head, sequence number ------------------------

@@ -125,14 +125,16 @@ class MCForward:
 
     Returns a dict of device tensors (the same objects every call; identical on all ranks):
       log_outputs [B,C], kl (= sum_j kl_j / num_ens), and with ``want_uncertainty`` pred / epistemic / aleatoric [B,C]
-      and entropy [B]; with ``with_labels`` head = [loss, nll, accuracy, beta*kl] (metrics.py:12-14, 23-24).
+      and entropy [B]; with ``with_labels`` head = [loss, nll, accuracy, beta*kl] (metrics.py:12-14, 23-24); with
+      ``want_information`` (needs ``want_uncertainty``) expected_entropy = mean_s H[p_hat_s] and mutual_info = entropy -
+      expected_entropy [B] (include/bbb_b200.h, bbb_mc_exchange_info).
     """
 
     def __init__(self, net, example_x: torch.Tensor, num_ens: int, group=None, want_uncertainty: bool = False,
                  normalized: bool = False, with_labels: bool = False, train_size: float = 1.0, beta: float = 0.0,
                  seed: Optional[int] = None, graph: bool = True, num_classes: Optional[int] = None,
                  static_inputs=None, first_replay: int = 0, fold: bool = True, overlap: bool = False, inflight: int = 1,
-                 fold_group: Optional[int] = None, fold_budget: int = LAYER_FOLD_BUDGET):
+                 fold_group: Optional[int] = None, fold_budget: int = LAYER_FOLD_BUDGET, want_information: bool = False):
         """``static_inputs``: device tensors the caller fills in place (e.g. targets of its host->device copies, or a
         rotation of resident batches); one graph is captured per tensor and ``self(slot=k)`` runs the step on
         ``static_inputs[k]`` with no staging copy.  ``first_replay``: index of the first replay's noise block.
@@ -145,6 +147,8 @@ class MCForward:
         identical to the serial engine; ``wait()`` also covers the inputs (they may be rewritten afterwards).
         ``fold_group``: the largest number of samples one pass of the per-layer fold takes (nets the fused chain does not
         take); None = as many as ``fold_budget`` bytes of activations allow (layer_fold_groups)."""
+        if want_information and not want_uncertainty:
+            raise L.EngineError("MCForward: want_information needs want_uncertainty")
         Fn._require_cuda(example_x, "MCForward")
         lib = L.lib()
         self.net, self.group = net, group
@@ -156,7 +160,8 @@ class MCForward:
         self.ids = local_samples(self.num_ens, self.world, self.rank)
         self.B = int(example_x.shape[0])
         self.C = int(num_classes if num_classes is not None else net.num_classes)
-        self.flags = (L.MC_MOMENTS if want_uncertainty else 0) | (L.MC_NORMALIZED if normalized else 0)
+        self.flags = (L.MC_MOMENTS if want_uncertainty else 0) | (L.MC_NORMALIZED if normalized else 0) | \
+            (L.MC_INFO if want_information else 0)
         self.want_uncertainty, self.with_labels = want_uncertainty, with_labels
         self.train_size, self.beta = float(train_size), float(beta)
         # every rank must draw sample j from the same (seed, stream): share rank 0's seed unless one is given
@@ -188,6 +193,9 @@ class MCForward:
             for k in ("pred", "epistemic", "aleatoric"):
                 self.out[k] = torch.empty(B, Cc, **f32)
             self.out["entropy"] = torch.empty(B, **f32)
+        if want_information:
+            self.out["expected_entropy"] = torch.empty(B, **f32)
+            self.out["mutual_info"] = torch.empty(B, **f32)
         if with_labels:
             self.out["head"] = torch.empty(4, **f32)
         self.state = torch.zeros(int(lib.bbb_mc_state_bytes()), dtype=torch.uint8, device=dev)
@@ -367,16 +375,17 @@ class MCForward:
         return kl_ptr, n_kl
 
     def _exchange(self, kl_ptr, n_kl, advance_base=None, par=0):
-        """The one kernel behind the samples: combine + exchange + heads (bbb_mc_exchange)."""
+        """The one kernel behind the samples: combine + exchange + heads (bbb_mc_exchange_info)."""
         from .graph import _STRIDE
         o = self.out
-        rc = L.lib().bbb_mc_exchange(
+        rc = L.lib().bbb_mc_exchange_info(
             Fn._ptr(self.logits_all[par]), len(self.ids), self.num_ens, self.B, self.C, kl_ptr, n_kl, self.flags,
             Fn._ptr(self.labels_all[par] if self.labels_all is not None else None), C.c_float(self.train_size), C.c_float(self.beta), self.rank, self.world, self.peers,
             Fn._ptr(self.state), Fn._ptr(o["log_outputs"]), Fn._ptr(o["kl"]), Fn._ptr(o.get("pred")),
             Fn._ptr(o.get("epistemic")), Fn._ptr(o.get("aleatoric")), Fn._ptr(o.get("entropy")), Fn._ptr(o.get("head")),
-            Fn._ptr(advance_base), C.c_uint64(_STRIDE if advance_base is not None else 0), Fn._stream(self.dev))
-        L.check(rc, "bbb_mc_exchange")
+            Fn._ptr(advance_base), C.c_uint64(_STRIDE if advance_base is not None else 0),
+            Fn._ptr(o.get("expected_entropy")), Fn._ptr(o.get("mutual_info")), Fn._stream(self.dev))
+        L.check(rc, "bbb_mc_exchange_info")
 
     def _capture(self, warmup: int = 2):
         from .graph import _STRIDE
@@ -510,9 +519,12 @@ class MCForward:
         return self._chain_done[self._last] if (self.overlap and self.replays) else None
 
 
-def _generic_mc_forward(forward_fn: Callable, x: torch.Tensor, num_ens: int, group=None, want_uncertainty: bool = False):
+def _generic_mc_forward(forward_fn: Callable, x: torch.Tensor, num_ens: int, group=None, want_uncertainty: bool = False,
+                        information: bool = False):
     """Backend-agnostic restatement (any device, any torch.distributed backend): the exact (max, sum-exp) partials of
-    logmeanexp per rank and ONE all-gather; returns (log_outputs, kl[, (pred, epistemic, aleatoric, entropy)])."""
+    logmeanexp per rank and ONE all-gather; returns (log_outputs, kl[, (pred, epistemic, aleatoric, entropy)]) --
+    with ``information`` the tuple also holds expected_entropy and mutual_info (each rank's sum of H[p_hat_s] over its
+    samples travels as one more [B] plane of the same all-gather)."""
     dist, world, rank = _dist_info(group)
     ids = local_samples(num_ens, world, rank)
     parts, shape, dev = None, None, x.device
@@ -523,13 +535,19 @@ def _generic_mc_forward(forward_fn: Callable, x: torch.Tensor, num_ens: int, gro
         lsm = torch.log_softmax(logits, dim=1)
         p = lsm.exp()
         klv = torch.as_tensor(kl, dtype=torch.float32, device=dev).reshape(1)
+        if information:
+            h = -torch.where(p > 0, p * lsm, torch.zeros_like(p)).sum(1)   # H[p_hat_j], 0 log 0 = 0
         if parts is None:
             parts = [lsm.clone(), torch.ones_like(lsm), p.clone(), p * p, logits.clone(), klv.clone()]
+            if information:
+                parts.append(h)
         else:
             m = torch.maximum(parts[0], lsm)
             parts[1] = parts[1] * (parts[0] - m).exp() + (lsm - m).exp()
             parts[0] = m
             parts[2] += p; parts[3] += p * p; parts[4] += logits; parts[5] += klv
+            if information:
+                parts[6] += h
     if world > 1:
         meta = [tuple(shape) if shape is not None else None]
         metas = [None] * world
@@ -539,6 +557,8 @@ def _generic_mc_forward(forward_fn: Callable, x: torch.Tensor, num_ens: int, gro
     if parts is None:                                 # a rank with no sample (num_ens < world) still joins the collective
         z = torch.zeros(shape, dtype=torch.float32, device=dev)
         parts = [torch.full(shape, -float("inf"), device=dev), z, z.clone(), z.clone(), z.clone(), torch.zeros(1, device=dev)]
+        if information:
+            parts.append(torch.zeros(shape[0], device=dev))
     vec = torch.cat([t.reshape(-1) for t in parts])
     if world > 1:
         allv = [torch.empty_like(vec) for _ in range(world)]
@@ -560,34 +580,42 @@ def _generic_mc_forward(forward_fn: Callable, x: torch.Tensor, num_ens: int, gro
     epistemic = p2 - p_bar * p_bar                    # diag((p-pbar)^T (p-pbar))/T  (uncertainty_estimation.py:89-91)
     aleatoric = p_bar - p2                            # diag(diag(pbar) - p^T p / T)  (:94-95)
     entropy = -(p_bar * torch.log(p_bar.clamp_min(1e-38))).sum(1)      # H[pbar]; no reference (SURVEY D3)
-    return log_outputs, kl, (pred, epistemic, aleatoric, entropy)
+    if not information:
+        return log_outputs, kl, (pred, epistemic, aleatoric, entropy)
+    expected_entropy = sum(v[5 * n + 1:5 * n + 1 + shape[0]] for v in allv) / S      # E_j H[p_hat_j], rank order
+    return log_outputs, kl, (pred, epistemic, aleatoric, entropy, expected_entropy, entropy - expected_entropy)
 
 
 def mc_forward(net_or_fn, x: torch.Tensor, num_ens: int, group=None, want_uncertainty: bool = False,
                normalized: bool = False, labels: Optional[torch.Tensor] = None, train_size: float = 1.0,
-               beta: float = 0.0, seed: Optional[int] = None):
+               beta: float = 0.0, seed: Optional[int] = None, information: bool = False):
     """(log_outputs [B,C], kl) like main_bayesian.py:46-53 -- plus (pred, epistemic, aleatoric, entropy) like
     uncertainty_estimation.py:70-96 with ``want_uncertainty`` and the ELBO head [loss, nll, acc, beta*kl] when
-    ``labels`` are given.  ``net_or_fn``: a net built on the engine with CUDA input -> the device path (MCForward,
-    cached on the net per shape/options); any ``forward_fn(x, sample_id) -> (logits, kl)`` -> the generic path."""
+    ``labels`` are given.  ``information`` (needs ``want_uncertainty``) extends that tuple to (pred, epistemic, aleatoric,
+    entropy, expected_entropy, mutual_info).  ``net_or_fn``: a net built on the engine with CUDA input -> the device path
+    (MCForward, cached on the net per shape/options); any ``forward_fn(x, sample_id) -> (logits, kl)`` -> the generic
+    path."""
     from .modules import ModuleWrapper
+    if information and not want_uncertainty:
+        raise L.EngineError("mc_forward: information needs want_uncertainty")
     if isinstance(net_or_fn, ModuleWrapper) and x.is_cuda:
         net = net_or_fn
         key = (tuple(x.shape), int(num_ens), bool(want_uncertainty), bool(normalized), labels is not None,
-               float(train_size), float(beta), seed, id(group))
+               float(train_size), float(beta), seed, id(group), bool(information))
         cache = net.__dict__.setdefault("_mc_engines", {})
         eng = cache.get(key)
         if eng is None:
             eng = cache[key] = MCForward(net, x, num_ens, group, want_uncertainty, normalized, labels is not None,
-                                         train_size, beta, seed)
+                                         train_size, beta, seed, want_information=information)
         out = eng(x, labels)
         res = [out["log_outputs"], out["kl"]]
         if want_uncertainty:
-            res.append((out["pred"], out["epistemic"], out["aleatoric"], out["entropy"]))
+            res.append(tuple(out[k] for k in ("pred", "epistemic", "aleatoric", "entropy") +
+                             (("expected_entropy", "mutual_info") if information else ())))
         if labels is not None:
             res.append(out["head"])
         return tuple(res)
-    return _generic_mc_forward(net_or_fn, x, num_ens, group, want_uncertainty)
+    return _generic_mc_forward(net_or_fn, x, num_ens, group, want_uncertainty, information)
 
 
 def engine_forward_fn(net) -> Callable:
