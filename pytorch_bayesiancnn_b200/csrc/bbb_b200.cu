@@ -109,6 +109,39 @@ int layer_fold_check(const bbb_layer_desc* d, const bbb::Geom& g, int math) {
     return BBB_OK;
 }
 
+// The MC-sample fold of a tensor-core call (desc->reserved[1..3], include/bbb_b200.h; rows = 0: none).  A fold draws its
+// noise in-kernel, so it takes no external eps.
+int layer_fold(const bbb_layer_desc* d, const bbb::Geom& g, const float* eps_a, const float* eps_b, bbb::McFold& fold) {
+    fold.rows = 0; fold.stride = 0; fold.sets = 1; fold.set_bytes = 0;
+    if (d->reserved[1] <= 0) return BBB_OK;
+    if (eps_a || eps_b) return fail(BBB_E_UNSUPPORTED, "MC-sample folding draws its noise in-kernel (no external eps)");
+    fold.rows = d->reserved[1];
+    fold.stride = ((unsigned long long)(uint32_t)d->reserved[3] << 32) | (uint32_t)d->reserved[2];
+    fold.sets = weight_sets(*d, g);
+    fold.set_bytes = set_stride(g);
+    return BBB_OK;
+}
+
+// The parameter half of a tensor-core call: desc, parameters, noise, KL workspace, operand region (tiles at kTcOffset,
+// bias rows `bias_offset` bytes behind them), fold and debug slots.  The timeline slots are taken in launch order.
+void layer_args(bbb::LayerArgs& a, const bbb_layer_desc* d, const bbb::Geom& g, const float* W_mu, const float* W_rho,
+                const float* bias_mu, const float* bias_rho, float* kl_out, const float* eps_a, const float* eps_b,
+                uint64_t seed, uint64_t stream_id, const uint64_t* stream_base, void* ws, size_t bias_offset,
+                const bbb::McFold& fold, const char* prep_name, bool do_prep, const char* gemm_name, bool do_gemm) {
+    a.g = g; a.w_mu = W_mu; a.w_rho = W_rho; a.b_mu = bias_mu; a.b_rho = bias_rho; a.eps_a = eps_a; a.eps_b = eps_b;
+    a.key = bbb::make_key(seed, stream_id); a.stream_base = (const unsigned long long*)stream_base;
+    a.kl_counter = (unsigned int*)ws; a.kl_partials = (double*)((char*)ws + kCounterBytes); a.kl_out = kl_out;
+    a.prior_mu = d->prior_mu; a.prior_sigma = d->prior_sigma;
+    a.sample = d->sample; a.kl_convention = d->kl_convention; a.has_bias = d->has_bias; a.act = d->epilogue_act;
+    a.variant = d->variant;
+    a.wtiles = (__nv_bfloat16*)((char*)ws + kTcOffset);
+    a.bias_ws = (float*)((char*)ws + kTcOffset + bias_offset);
+    a.fold = fold;
+    a.trace = g_trace;
+    a.tl_prep = tl_slot(do_prep, prep_name, g);
+    a.tl_gemm = tl_slot(do_gemm, gemm_name, g);
+}
+
 int forward_impl(const bbb_layer_desc* d, bool linear, const void* x, const float* W_mu, const float* W_rho,
                  const float* bias_mu, const float* bias_rho, void* y, float* kl_out, float* act_std,
                  const float* eps_a, const float* eps_b, uint64_t seed, uint64_t stream_id, const uint64_t* stream_base, void* ws,
@@ -124,32 +157,18 @@ int forward_impl(const bbb_layer_desc* d, bool linear, const void* x, const floa
     int math = BBB_MATH_FP32;
     if (int rc = layer_math(d, g, math)) return rc;
     if (int rc = layer_fold_check(d, g, math)) return rc;
-    bbb::McFold fold; fold.rows = 0; fold.stride = 0; fold.sets = 1; fold.set_bytes = 0;
-    if (d->reserved[1] > 0) {
-        if (eps_a || eps_b) return fail(BBB_E_UNSUPPORTED, "MC-sample folding draws its noise in-kernel (no external eps)");
-        fold.rows = d->reserved[1];
-        fold.stride = ((unsigned long long)(uint32_t)d->reserved[3] << 32) | (uint32_t)d->reserved[2];
-        fold.sets = weight_sets(*d, g);
-        fold.set_bytes = set_stride(g);
-    }
+    bbb::McFold fold;
+    if (int rc = layer_fold(d, g, eps_a, eps_b, fold)) return rc;
     if (math == BBB_MATH_BF16_TC || math == BBB_MATH_TF32_TC) {
         const size_t need = fold.sets > 1 ? bbb_workspace_bytes(d) : kTcOffset + bbb::tc_workspace_bytes(g);
         if (!ws || ws_bytes < need) return fail(BBB_E_WORKSPACE, "workspace too small for the tensor-core path: need %zu bytes", need);
+        const bool tf32 = math == BBB_MATH_TF32_TC;
         bbb::TcArgs a;
-        a.fold = fold;
-        a.wtiles = (__nv_bfloat16*)((char*)ws + kTcOffset);
-        a.tf32 = math == BBB_MATH_TF32_TC;
-        // operand tiles: 2 planes x npad rows x (kpad * 2 bytes of bf16 | kpad32 * 4 bytes of tf32), then the bias rows
-        a.bias_ws = (float*)((char*)ws + kTcOffset + (size_t)bbb::tc_npad(g) * bbb::tc_kpad(g, a.tf32) * (a.tf32 ? 8 : 4));
-        a.skip_prep = 0; a.prep_only = 0; a.y_sq = nullptr; a.out_mode = 2; a.out_pitch = 0; a.pool = 0; a.trace = g_trace;
-        a.tl_prep = tl_slot(true, "weight_prep", g); a.tl_gemm = tl_slot(true, "gemm_tc", g);
-        a.g = g; a.x = x; a.w_mu = W_mu; a.w_rho = W_rho; a.b_mu = bias_mu; a.b_rho = bias_rho;
-        a.y = y; a.kl_out = kl_out; a.act_std = act_std; a.eps_a = eps_a; a.eps_b = eps_b;
-        a.key = bbb::make_key(seed, stream_id); a.stream_base = (const unsigned long long*)stream_base;
-        a.kl_counter = (unsigned int*)ws; a.kl_partials = (double*)((char*)ws + kCounterBytes);
-        a.prior_mu = d->prior_mu; a.prior_sigma = d->prior_sigma;
-        a.sample = d->sample; a.kl_convention = d->kl_convention; a.has_bias = d->has_bias; a.act = d->epilogue_act;
-        a.act_dtype = d->act_dtype; a.variant = d->variant;
+        layer_args(a, d, g, W_mu, W_rho, bias_mu, bias_rho, kl_out, eps_a, eps_b, seed, stream_id, stream_base, ws,
+                   bbb::tc_bias_offset(g, tf32), fold, "weight_prep", true, "gemm_tc", true);
+        a.tf32 = tf32;
+        a.skip_prep = 0; a.prep_only = 0; a.y_sq = nullptr; a.out_mode = 2; a.out_pitch = 0; a.pool = 0;
+        a.x = x; a.y = y; a.act_std = act_std; a.act_dtype = d->act_dtype;
         int nl = 0;
         cudaError_t e = bbb::launch_fwd_tc(a, st, sm_count(), &nl);
         if (e != cudaSuccess) return cuda_fail(e, "fwd_tc launch");
@@ -309,14 +328,8 @@ int bbb_layer_forward_fused(const bbb_layer_desc* d, const void* x, const void* 
     if (!W_mu || !W_rho || (!prep_only && (!x || !y))) return fail(BBB_E_INVALID, "NULL tensor pointer");
     if (d->has_bias && (!bias_mu || !bias_rho)) return fail(BBB_E_INVALID, "has_bias set but bias pointers NULL");
     const int pool = d->pool_k != 0;
-    bbb::McFold fold; fold.rows = 0; fold.stride = 0; fold.sets = 1; fold.set_bytes = 0;
-    if (d->reserved[1] > 0) {           // MC samples folded into the batch (checked by fused_check)
-        if (eps_a || eps_b) return fail(BBB_E_UNSUPPORTED, "MC-sample folding draws its noise in-kernel (no external eps)");
-        fold.rows = d->reserved[1];
-        fold.stride = ((unsigned long long)(uint32_t)d->reserved[3] << 32) | (uint32_t)d->reserved[2];
-        fold.sets = weight_sets(*d, g);
-        fold.set_bytes = set_stride(g);
-    }
+    bbb::McFold fold;                   // rows, samples and path checked by fused_check
+    if (int rc = layer_fold(d, g, eps_a, eps_b, fold)) return rc;
     const size_t need = bbb_workspace_bytes(d);
     if (!ws || ws_bytes < need) return fail(BBB_E_WORKSPACE, "workspace too small for the fused path: need %zu bytes", need);
     if (out_layout == BBB_LAYOUT_PACKED_BF16 && y_sq && y_sq != (void*)((__nv_bfloat16*)y + 128 * 64))
@@ -327,49 +340,25 @@ int bbb_layer_forward_fused(const bbb_layer_desc* d, const void* x, const void* 
     if (s4) {
         // stride-4 first layer: the tensor core reads its A operand straight from the staged image (conv_s4_tc.cuh)
         bbb::S4Args a;
-        a.g = g; a.x = (const float*)x; a.w_mu = W_mu; a.w_rho = W_rho; a.b_mu = bias_mu; a.b_rho = bias_rho;
-        a.y = y; a.y_sq = y_sq; a.kl_out = kl_out; a.eps_a = eps_a; a.eps_b = eps_b;
-        a.key = bbb::make_key(seed, stream_id); a.stream_base = (const unsigned long long*)stream_base;
-        a.kl_counter = (unsigned int*)ws; a.kl_partials = (double*)((char*)ws + kCounterBytes);
-        a.prior_mu = d->prior_mu; a.prior_sigma = d->prior_sigma;
-        a.sample = d->sample; a.kl_convention = d->kl_convention; a.has_bias = d->has_bias; a.act = d->epilogue_act;
-        a.variant = d->variant; a.out_pitch = out_pitch;
-        a.wtiles = (__nv_bfloat16*)((char*)ws + kTcOffset);
-        a.bias_ws = (float*)((char*)ws + kTcOffset + (size_t)g.KH * 2 * bbb::S4_BPLANE);
-        a.trace = g_trace; a.fold = fold;
-        a.tl_prep = tl_slot(!skip_prep, "conv_s4_prep", g); a.tl_gemm = tl_slot(!prep_only, "conv_s4", g);
+        layer_args(a, d, g, W_mu, W_rho, bias_mu, bias_rho, kl_out, eps_a, eps_b, seed, stream_id, stream_base, ws,
+                   bbb::conv_s4_bias_offset(g), fold, "conv_s4_prep", !skip_prep, "conv_s4", !prep_only);
+        a.x = (const float*)x; a.y = y; a.y_sq = y_sq; a.out_pitch = out_pitch;
         cudaError_t e = bbb::launch_conv_s4(a, st, !skip_prep, !prep_only, &nl);
         if (e != cudaSuccess) return cuda_fail(e, "conv_s4 launch");
     } else if (in_layout == BBB_LAYOUT_NCHW_F32) {
-        bbb::TcArgs a;
-        a.g = g; a.x = x; a.w_mu = W_mu; a.w_rho = W_rho; a.b_mu = bias_mu; a.b_rho = bias_rho;
-        a.y = y; a.kl_out = kl_out; a.act_std = nullptr; a.eps_a = eps_a; a.eps_b = eps_b;
-        a.key = bbb::make_key(seed, stream_id); a.stream_base = (const unsigned long long*)stream_base;
-        a.kl_counter = (unsigned int*)ws; a.kl_partials = (double*)((char*)ws + kCounterBytes);
-        a.prior_mu = d->prior_mu; a.prior_sigma = d->prior_sigma;
-        a.sample = d->sample; a.kl_convention = d->kl_convention; a.has_bias = d->has_bias; a.act = d->epilogue_act;
-        a.act_dtype = d->act_dtype; a.variant = d->variant;
-        a.wtiles = (__nv_bfloat16*)((char*)ws + kTcOffset);
-        a.bias_ws = (float*)((char*)ws + kTcOffset + (size_t)bbb::tc_npad(g) * bbb::tc_kpad(g) * 4);
-        a.tf32 = 0;
-        a.fold = fold;                  // rows = 0: fused_check refuses a fold on the gather path
-        a.trace = g_trace; a.skip_prep = skip_prep; a.prep_only = prep_only; a.y_sq = y_sq; a.out_mode = out_mode == 1 ? 2 : out_mode; a.out_pitch = out_pitch; a.pool = pool;
-        a.tl_prep = tl_slot(!skip_prep, "weight_prep", g); a.tl_gemm = tl_slot(!prep_only, "gemm_tc", g);
+        bbb::TcArgs a;                  // fold.rows = 0: fused_check refuses a fold on the gather path
+        layer_args(a, d, g, W_mu, W_rho, bias_mu, bias_rho, kl_out, eps_a, eps_b, seed, stream_id, stream_base, ws,
+                   bbb::tc_bias_offset(g, false), fold, "weight_prep", !skip_prep, "gemm_tc", !prep_only);
+        a.x = x; a.y = y; a.act_std = nullptr; a.act_dtype = d->act_dtype; a.tf32 = 0;
+        a.skip_prep = skip_prep; a.prep_only = prep_only; a.y_sq = y_sq; a.out_mode = out_mode == 1 ? 2 : out_mode; a.out_pitch = out_pitch; a.pool = pool;
         cudaError_t e = bbb::launch_fwd_tc(a, st, sm_count(), &nl);
         if (e != cudaSuccess) return cuda_fail(e, "fused gather launch");
     } else if (in_layout == BBB_LAYOUT_PACKED_BF16) {
         bbb::FusedArgs a;
-        a.g = g; a.variant = d->variant; a.sample = d->sample; a.has_bias = d->has_bias; a.act = d->epilogue_act;
-        a.kl_convention = d->kl_convention; a.prior_mu = d->prior_mu; a.prior_sigma = d->prior_sigma;
-        a.w_mu = W_mu; a.w_rho = W_rho; a.b_mu = bias_mu; a.b_rho = bias_rho; a.eps_a = eps_a; a.eps_b = eps_b;
-        a.key = bbb::make_key(seed, stream_id); a.stream_base = (const unsigned long long*)stream_base;
-        a.kl_counter = (unsigned int*)ws; a.kl_partials = (double*)((char*)ws + kCounterBytes); a.kl_out = kl_out;
-        const size_t cpad = (size_t)(g.N + 63) / 64 * 64, kpad = (size_t)(g.Cin + 63) / 64 * 64;
-        a.wtiles = (__nv_bfloat16*)((char*)ws + kTcOffset);
-        a.bias_ws = (float*)((char*)ws + kTcOffset + cpad * kpad * g.KHW * 4 + 32768);   // behind the zero sub-tile
+        layer_args(a, d, g, W_mu, W_rho, bias_mu, bias_rho, kl_out, eps_a, eps_b, seed, stream_id, stream_base, ws,
+                   bbb::fused_bias_offset(g), fold, "tap_prep", !skip_prep, "tap_gemm", !prep_only);
         a.prev_hw = prev_hw; a.y = y; a.y_sq = y_sq; a.out_mode = out_mode; a.out_pitch = out_pitch; a.pool = pool;
-        a.in_pitch = in_pitch; a.trace = g_trace; a.fold = fold;
-        a.tl_prep = tl_slot(!skip_prep, "tap_prep", g); a.tl_gemm = tl_slot(!prep_only, "tap_gemm", g);
+        a.in_pitch = in_pitch;
         const char* why = "";
         cudaError_t e = bbb::launch_fused(a, x, x_sq, st, &nl, &why, !skip_prep, !prep_only, sm_count(), g_wide_tiles.load() != 0);
         if (e != cudaSuccess) return fail(BBB_E_CUDA, "fused tap-GEMM launch: %s %s", cudaGetErrorString(e), why);

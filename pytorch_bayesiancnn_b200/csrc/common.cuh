@@ -1,6 +1,7 @@
 // Shared device helpers: geometry, Philox4x32-10 noise, softplus, KL terms.
 #pragma once
 #include <cuda_runtime.h>
+#include <cuda_bf16.h>
 #include <stdint.h>
 #include "../../include/bbb_b200.h"
 
@@ -96,6 +97,25 @@ template <class T>
 __host__ __device__ __forceinline__ T* fold_set(T* p, const McFold& f, int j) {
     return reinterpret_cast<T*>(reinterpret_cast<uintptr_t>(p) + (size_t)j * f.set_bytes);
 }
+
+// The parameter half of a tensor-core layer call, common to its three kernel pairs (TcArgs, FusedArgs, S4Args derive
+// from it): what the weight-prep kernel reads and writes, and what the GEMM kernel needs of the prepared operands.
+struct LayerArgs {
+    Geom g;
+    const float* w_mu; const float* w_rho; const float* b_mu; const float* b_rho;
+    const float* eps_a; const float* eps_b;        // external eps (nullptr: in-kernel Philox)
+    NoiseKey key; const unsigned long long* stream_base;
+    double* kl_partials; unsigned int* kl_counter; float* kl_out;
+    float prior_mu, prior_sigma;
+    int sample, kl_convention, has_bias, act, variant;
+    // prepared-operand workspace: operand tiles in the path's own layout, then the bias rows
+    // [2][npad]: row 0 = bias (BBB: sampled; LRT: mu), row 1 = LRT sigma_b^2
+    __nv_bfloat16* wtiles; float* bias_ws;
+    int planes;                                    // operand planes: 2 = LRT (mu, sigma^2), else 1
+    McFold fold;                                   // MC samples folded into the batch (rows = 0: off)
+    long long* trace;                              // debug: per-CTA clock64 checkpoints (nullptr in production)
+    long long* tl_prep; long long* tl_gemm;        // debug: timeline slots of the two launches (nullptr in production)
+};
 
 // four normals of group g (elements 4g .. 4g+3)
 __device__ __forceinline__ float4 normal4(uint64_t grp, const NoiseKey& k) {

@@ -33,20 +33,11 @@ constexpr int S4_IMGS = 16, S4_WIN_PX = 12, S4_KROW = 48, S4_THREADS = 288;
 constexpr int S4_STAGES = 3;
 constexpr int S4_BPLANE = 64 * S4_KROW * 2;                // one plane of one kernel row: 6 chunks x 64 rows x 16 B = 6144 B
 
-struct S4Args {
-    Geom g;
-    const float* x; const float* w_mu; const float* w_rho; const float* b_mu; const float* b_rho;
-    void* y; void* y_sq; float* kl_out;
-    const float* eps_a; const float* eps_b;
-    NoiseKey key; const unsigned long long* stream_base;
-    double* kl_partials; unsigned int* kl_counter;
-    float prior_mu, prior_sigma;
-    int sample, kl_convention, has_bias, act, variant;
-    __nv_bfloat16* wtiles; float* bias_ws;
-    int planes, out_pitch;
+struct S4Args : LayerArgs {
+    const float* x;                // a fold's x holds fold.rows images
+    void* y; void* y_sq;
+    int out_pitch;
     int lpad, wp, rows;            // left zero pad in pixels (PW + 1), staged row width in pixels, staged rows per image (4 + KH)
-    McFold fold;                   // MC samples folded into the batch (rows = 0: off); x then holds fold.rows images
-    long long* trace; long long* tl_prep; long long* tl_gemm;
 };
 
 inline bool conv_s4_supported(const bbb_layer_desc& d, const Geom& g, int pool, int out_packed) {
@@ -61,7 +52,9 @@ inline bool conv_s4_supported(const bbb_layer_desc& d, const Geom& g, int pool, 
     const size_t img = (size_t)S4_IMGS * (4 + g.KH) * ((wp + 1) & ~1) * 8;
     return 2 * img + S4_STAGES * 2 * S4_BPLANE + 4096 <= (size_t)TC_SMEM_LIMIT;
 }
-inline size_t conv_s4_workspace_bytes(const Geom& g) { return (size_t)g.KH * 2 * S4_BPLANE + 2 * 64 * 4 + 256; }
+// operand tiles (one 2-plane stage per kernel row), then the bias rows
+inline size_t conv_s4_bias_offset(const Geom& g) { return (size_t)g.KH * 2 * S4_BPLANE; }
+inline size_t conv_s4_workspace_bytes(const Geom& g) { return conv_s4_bias_offset(g) + 2 * 64 * 4 + 256; }
 
 // ------------------------------------------------------------------ (P) prep
 // item = (kernel row r, 8-wide K chunk, output channel): K' = chunk*8 + e -> window pixel j = K'/4 (s = j - 1), channel K'%4
@@ -69,10 +62,8 @@ inline size_t conv_s4_workspace_bytes(const Geom& g) { return (size_t)g.KH * 2 *
 template <int VARIANT, bool FOLD = false>
 __global__ void __launch_bounds__(256)
 conv_s4_prep_kernel(const S4Args p) {
-    __shared__ double red[32];
     constexpr bool LRT = VARIANT == BBB_VARIANT_LRT;
     const Geom& g = p.g;
-    const bool stoch = p.sample != 0, do_kl = p.kl_out != nullptr;
     const int n_items = g.KH * 6 * 64;
     double kl_acc = 0.0;
     tl_enter(p.tl_prep);
@@ -85,66 +76,34 @@ conv_s4_prep_kernel(const S4Args p) {
     const int sets = FOLD ? p.fold.sets : 1;
     for (int gi = blockIdx.x * blockDim.x + threadIdx.x; gi < n_items; gi += gridDim.x * blockDim.x) {
         const int row = gi & 63, chunk = (gi >> 6) % 6, r = gi / (6 * 64);
-        float w[8], s2[8], mu8[8], sg8[8];                          // mu8 / sg8: kept for the other samples of a fold
+        // weight index of element e of this chunk: window pixel s = kq / 4 - 1 (s = -1 and channel 3 are padding slots)
+        auto w_ok = [&](int e) { const int kq = chunk * 8 + e, s = (kq >> 2) - 1; return s >= 0 && s < g.KW && (kq & 3) < g.Cin; };
+        auto w_index = [&](int e) { const int kq = chunk * 8 + e; return (((size_t)row * g.Cin + (kq & 3)) * g.KH + r) * g.KW + (kq >> 2) - 1; };
+        float w[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f}, s2[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+        float mu8[8], sg8[8];                                       // kept for the other samples of a fold
 #pragma unroll
         for (int e = 0; e < 8; ++e) {
-            const int kq = chunk * 8 + e, s = (kq >> 2) - 1, c = kq & 3;
-            float wv = 0.0f, sv = 0.0f;
             mu8[e] = sg8[e] = 0.0f;
-            if (s >= 0 && s < g.KW && c < g.Cin) {
-                const size_t wi = (((size_t)row * g.Cin + c) * g.KH + r) * g.KW + s;
+            if (w_ok(e)) {
+                const size_t wi = w_index(e);
                 const float mu = __ldg(p.w_mu + wi);
-                float sigma = 0.0f;
-                if (stoch || do_kl) sigma = softplus_sigma_fast(__ldg(p.w_rho + wi));
-                if (LRT) { wv = mu; sv = sigma * sigma; }
-                else if (stoch) {
-                    const float e_ = p.eps_a ? __ldg(p.eps_a + wi) : normal1(wi, nkey);
-                    wv = mu + e_ * sigma;
-                } else wv = mu;
-                if (do_kl) kl_acc += (double)kl_term_fast(mu, sigma, p.prior_mu, p.prior_sigma, p.kl_convention);
-                mu8[e] = mu; sg8[e] = sigma;
+                const PrepElem o = prep_elem<LRT>(p, mu, RhoAt{p.w_rho, wi}, p.eps_a, wi, wi, nkey, kl_acc);
+                w[e] = o.w; s2[e] = o.s2; mu8[e] = mu; sg8[e] = o.sigma;
             }
-            w[e] = wv; s2[e] = sv;
         }
         const size_t off = (size_t)r * p.planes * (S4_BPLANE / 2) + chunk * 512 + row * 8;   // canonical K-major, no swizzle
         __nv_bfloat16* dst = p.wtiles + off;
-        *reinterpret_cast<uint4*>(dst) = make_uint4(pack_bf16(w[0], w[1]), pack_bf16(w[2], w[3]), pack_bf16(w[4], w[5]), pack_bf16(w[6], w[7]));
-        if (p.planes == 2)
-            *reinterpret_cast<uint4*>(dst + S4_BPLANE / 2) = make_uint4(pack_bf16(s2[0], s2[1]), pack_bf16(s2[2], s2[3]), pack_bf16(s2[4], s2[5]), pack_bf16(s2[6], s2[7]));
+        *reinterpret_cast<uint4*>(dst) = pack_chunk<false>(w);
+        if (p.planes == 2) *reinterpret_cast<uint4*>(dst + S4_BPLANE / 2) = pack_chunk<false>(s2);
         for (int j = 1; j < sets; ++j) {                            // the other samples' weights from the same mu / sigma
             const NoiseKey kj = sample_key(nkey, p.fold, j);
 #pragma unroll
-            for (int e = 0; e < 8; ++e) {
-                const int kq = chunk * 8 + e, s = (kq >> 2) - 1, c = kq & 3;
-                const size_t wi = (((size_t)row * g.Cin + c) * g.KH + r) * g.KW + s;
-                w[e] = (s >= 0 && s < g.KW && c < g.Cin) ? mu8[e] + normal1(wi, kj) * sg8[e] : 0.0f;
-            }
-            *reinterpret_cast<uint4*>(fold_set(p.wtiles, p.fold, j) + off) =
-                make_uint4(pack_bf16(w[0], w[1]), pack_bf16(w[2], w[3]), pack_bf16(w[4], w[5]), pack_bf16(w[6], w[7]));
+            for (int e = 0; e < 8; ++e) w[e] = w_ok(e) ? fold_draw(mu8[e], sg8[e], w_index(e), kj) : 0.0f;
+            *reinterpret_cast<uint4*>(fold_set(p.wtiles, p.fold, j) + off) = pack_chunk<false>(w);
         }
     }
-    for (int n = blockIdx.x * blockDim.x + threadIdx.x; n < 64; n += gridDim.x * blockDim.x) {   // bias
-        float bm = 0.0f, bv = 0.0f;
-        if (p.has_bias && n < g.N) {
-            const float mu = __ldg(p.b_mu + n);
-            const float sigma = (stoch || do_kl) ? softplus_sigma_fast(__ldg(p.b_rho + n)) : 0.0f;
-            if (LRT) { bm = mu; bv = sigma * sigma; }
-            else if (stoch) {
-                const float e_ = p.eps_b ? __ldg(p.eps_b + n) : normal1((uint64_t)g.N * g.K + n, nkey);
-                bm = mu + e_ * sigma;
-            } else bm = mu;
-            if (do_kl) kl_acc += (double)kl_term_fast(mu, sigma, p.prior_mu, p.prior_sigma, p.kl_convention);
-            for (int j = 1; j < sets; ++j)
-                fold_set(p.bias_ws, p.fold, j)[n] = mu + normal1((uint64_t)g.N * g.K + n, sample_key(nkey, p.fold, j)) * sigma;
-        }
-        p.bias_ws[n] = bm;
-        p.bias_ws[64 + n] = bv;
-    }
-    if (do_kl) {
-        const double tot = block_sum(kl_acc, red);
-        if (threadIdx.x == 0) kl_publish(tot, blockIdx.x, gridDim.x, p.kl_partials, p.kl_counter, p.kl_out);
-    }
-    tl_exit(p.tl_prep);
+    prep_bias<LRT, FOLD>(p, nkey, 64, kl_acc);
+    prep_finish(p, kl_acc);
 }
 
 // ------------------------------------------------------------------ (G) conv
@@ -435,15 +394,8 @@ inline cudaError_t launch_conv_s4(S4Args a, cudaStream_t st, bool do_prep, bool 
     a.rows = 4 + g.KH;
     const bool lrt = a.variant == BBB_VARIANT_LRT;
     if (do_prep) {
-        static const bool carve = [] {               // keep every kernel of the chain on one shared-memory carve-out (see launch_fwd_tc)
-            const char* e = getenv("BBB_B200_PREP_CARVEOUT");
-            if (e && e[0] == '0') return false;
-            cudaFuncSetAttribute(conv_s4_prep_kernel<BBB_VARIANT_LRT>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-            cudaFuncSetAttribute(conv_s4_prep_kernel<BBB_VARIANT_BBB>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-            cudaFuncSetAttribute(conv_s4_prep_kernel<BBB_VARIANT_BBB, true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-            return true;
-        }();
-        (void)carve;
+        prep_carveout<conv_s4_prep_kernel<BBB_VARIANT_LRT>, conv_s4_prep_kernel<BBB_VARIANT_BBB>,
+                      conv_s4_prep_kernel<BBB_VARIANT_BBB, true>>();
         const int grid = (g.KH * 6 * 64 + 255) / 256;
         cudaError_t e = lrt ? launch_pdl(conv_s4_prep_kernel<BBB_VARIANT_LRT>, dim3(grid), dim3(256), 0, st, a)
                       : a.fold.sets > 1 ? launch_pdl(conv_s4_prep_kernel<BBB_VARIANT_BBB, true>, dim3(grid), dim3(256), 0, st, a)

@@ -30,40 +30,29 @@
 namespace bbb {
 
 
-struct FusedArgs {
-    Geom g;
-    int variant, sample, has_bias, act, kl_convention;
-    float prior_mu, prior_sigma;
-    const float *w_mu, *w_rho, *b_mu, *b_rho, *eps_a, *eps_b;
-    NoiseKey key; const unsigned long long* stream_base;
-    double* kl_partials; unsigned int* kl_counter; float* kl_out;
-    __nv_bfloat16* wtiles; float* bias_ws;
-    int planes, ng, n_cblk, n_kblk, taps;
+struct FusedArgs : LayerArgs {
+    int ng, n_cblk, n_kblk, taps;
     int prev_hw;                 // linear fed by a flattened HxW map: k' = pix*C + c  <->  ref k = c*HW + pix
     const void* x; const void* x_sq;   // tiled packed input (and its square)
     void* y; void* y_sq;
     int out_mode, out_pitch, pool, in_pitch;   // pitches = F (columns) of the tiled packed matrices
-    long long* trace;            // debug: per-CTA clock64 checkpoints (nullptr in production)
-    long long* tl_prep; long long* tl_gemm;   // debug: timeline slots of the two launches (nullptr in production)
     int units;                   // K blocks per pipeline step (TAP_UNITS, or 1 for the 128-column LRT tile)
-    McFold fold;                 // MC samples folded into the batch (rows = 0: off)
 };
 
 __host__ __device__ inline size_t fused_wtile_elems(const FusedArgs& a) { return (size_t)a.planes * a.ng * 64; }
-inline size_t fused_workspace_bytes(const Geom& g) {
-    // worst case NG=16 padding of Cout, 2 planes
+// operand sub-tiles (worst case NG=16 padding of Cout, 2 planes), the zero sub-tile (<= 2 planes x 128 rows x 128 B),
+// then the bias rows
+inline size_t fused_bias_offset(const Geom& g) {
     const size_t cpad = (size_t)(g.N + 63) / 64 * 64, kpad = (size_t)(g.Cin + 63) / 64 * 64;
-    return cpad * kpad * g.KHW * 2 * 2 + 32768 /* zero sub-tile (<= 2 planes x 128 rows x 128 B) */ + 2 * cpad * 4;
+    return cpad * kpad * g.KHW * 2 * 2 + 32768;
 }
+inline size_t fused_workspace_bytes(const Geom& g) { return fused_bias_offset(g) + 2 * ((size_t)(g.N + 63) / 64 * 64) * 4; }
 
 // ------------------------------------------------------------- (P) tap prep
 // Tail of both tap preps, per operand set: one all-zero sub-tile behind the real ones (staged for pool-window pixels
-// whose tap is outside the kernel) and the bias rows, prepared (and their KL counted once) by the first CTAs, one thread
-// per channel; then the KL publish.
+// whose tap is outside the kernel), then the bias rows and the KL publish.
 template <bool LRT, bool FOLD>
-__device__ __forceinline__ void tap_prep_tail(const FusedArgs& p, const NoiseKey& nkey, bool stoch, bool do_kl,
-                                              double kl_acc, double* red) {
-    const Geom& g = p.g;
+__device__ __forceinline__ void tap_prep_tail(const FusedArgs& p, const NoiseKey& nkey, double kl_acc) {
     const int sets = FOLD ? p.fold.sets : 1;
     const size_t sub = fused_wtile_elems(p);
     for (int j = 0; j < sets; ++j) {
@@ -71,40 +60,20 @@ __device__ __forceinline__ void tap_prep_tail(const FusedArgs& p, const NoiseKey
         for (long gi = (long)blockIdx.x * blockDim.x + threadIdx.x; gi < (long)(sub / 8); gi += (long)gridDim.x * blockDim.x)
             zero[gi] = make_uint4(0u, 0u, 0u, 0u);
     }
-    const int npad = p.n_cblk * p.ng;
-    for (int n = blockIdx.x * blockDim.x + threadIdx.x; n < npad; n += gridDim.x * blockDim.x) {
-        float bm = 0.0f, bv = 0.0f;
-        if (p.has_bias && n < g.N) {
-            const float mu = __ldg(p.b_mu + n);
-            const float sigma = (stoch || do_kl) ? softplus_sigma_fast(__ldg(p.b_rho + n)) : 0.0f;
-            if (LRT) { bm = mu; bv = sigma * sigma; }
-            else if (stoch) {
-                const float e_ = p.eps_b ? __ldg(p.eps_b + n) : normal1((uint64_t)g.N * g.K + n, nkey);
-                bm = mu + e_ * sigma;
-            } else bm = mu;
-            if (do_kl) kl_acc += (double)kl_term_fast(mu, sigma, p.prior_mu, p.prior_sigma, p.kl_convention);
-            for (int j = 1; j < sets; ++j)
-                fold_set(p.bias_ws, p.fold, j)[n] = mu + normal1((uint64_t)g.N * g.K + n, sample_key(nkey, p.fold, j)) * sigma;
-        }
-        p.bias_ws[n] = bm;
-        p.bias_ws[npad + n] = bv;
-    }
-    if (do_kl) {
-        const double tot = block_sum(kl_acc, red);
-        if (threadIdx.x == 0) kl_publish(tot, blockIdx.x, gridDim.x, p.kl_partials, p.kl_counter, p.kl_out);
-    }
-    tl_exit(p.tl_prep);
+    prep_bias<LRT, FOLD>(p, nkey, p.n_cblk * p.ng, kl_acc);
+    prep_finish(p, kl_acc);
 }
 
 // FOLD: BBB fold, one operand set per weight sample (a separate instantiation keeps the other preps as they were)
+// Resident CTAs per SM: left to itself ptxas gives the LRT instantiation 54 registers (4 CTAs); the bound keeps it at 48
+// (5 CTAs).  The other two are given the occupancy they reach anyway (40 and 64 registers): any explicit bound changes
+// ptxas's register target for every instantiation of the template.
 template <int VARIANT, bool FOLD = false>
-__global__ void __launch_bounds__(256)
+__global__ void __launch_bounds__(256, VARIANT == BBB_VARIANT_LRT ? 5 : FOLD ? 4 : 6)
 tap_prep_kernel(const FusedArgs p) {
-    __shared__ double red[32];
     constexpr bool LRT = VARIANT == BBB_VARIANT_LRT;
     const Geom& g = p.g;
     const NoiseKey nkey = effective_key(p.key, p.stream_base);
-    const bool stoch = p.sample != 0, do_kl = p.kl_out != nullptr;
     const int cprev = g.Cin / p.prev_hw;
     const size_t sub = fused_wtile_elems(p);
     const int per_sub = p.ng * 8;                                  // (row, 8-wide K chunk) items per sub-tile
@@ -118,50 +87,37 @@ tap_prep_kernel(const FusedArgs p) {
         __nv_bfloat16* dst = p.wtiles + (size_t)st * sub;          // st == (tap*n_cblk + cb)*n_kblk + kb
         const int row = item % p.ng, chunk = item / p.ng;
         const int n = cb * p.ng + row;
-        float w[8], s2[8], mu8[8], sg8[8];                         // mu8 / sg8: kept for the other samples of a fold
+        // element e of this chunk: packed input channel kq and its weight index (prev_hw > 1: reorder to the reference's)
+        auto w_ok = [&](int e) { return n < g.N && kb * 64 + chunk * 8 + e < g.Cin; };
+        auto w_index = [&](int e) {
+            const int kq = kb * 64 + chunk * 8 + e;
+            const int cin = (p.prev_hw > 1) ? ((kq % cprev) * p.prev_hw + kq / cprev) : kq;
+            return (size_t)n * g.K + (size_t)cin * g.KHW + tap;
+        };
+        float w[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f}, s2[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+        float mu8[8], sg8[8];                                      // kept for the other samples of a fold
 #pragma unroll
         for (int e = 0; e < 8; ++e) {
-            const int kq = kb * 64 + chunk * 8 + e;                // packed input-channel index
-            float wv = 0.0f, sv = 0.0f;
             mu8[e] = sg8[e] = 0.0f;
-            if (n < g.N && kq < g.Cin) {
-                const int cin = (p.prev_hw > 1) ? ((kq % cprev) * p.prev_hw + kq / cprev) : kq;
-                const size_t wi = (size_t)n * g.K + (size_t)cin * g.KHW + tap;
+            if (w_ok(e)) {
+                const size_t wi = w_index(e);
                 const float mu = __ldg(p.w_mu + wi);
-                float sigma = 0.0f;
-                if (stoch || do_kl) sigma = softplus_sigma_fast(__ldg(p.w_rho + wi));
-                if (LRT) { wv = mu; sv = sigma * sigma; }
-                else if (stoch) {
-                    const float e_ = p.eps_a ? __ldg(p.eps_a + wi) : normal1(wi, nkey);
-                    wv = mu + e_ * sigma;
-                } else wv = mu;
-                if (do_kl) kl_acc += (double)kl_term_fast(mu, sigma, p.prior_mu, p.prior_sigma, p.kl_convention);
-                mu8[e] = mu; sg8[e] = sigma;
+                const PrepElem o = prep_elem<LRT>(p, mu, RhoAt{p.w_rho, wi}, p.eps_a, wi, wi, nkey, kl_acc);
+                w[e] = o.w; s2[e] = o.s2; mu8[e] = mu; sg8[e] = o.sigma;
             }
-            w[e] = wv; s2[e] = sv;
         }
         // K-major SWIZZLE_128B image: row r = 128 contiguous bytes, its 16-byte chunk c stored at chunk (c ^ (r & 7))
         const int sw = row * 64 + ((chunk ^ (row & 7)) << 3);
-        const uint4 o = make_uint4(pack_bf16(w[0], w[1]), pack_bf16(w[2], w[3]), pack_bf16(w[4], w[5]), pack_bf16(w[6], w[7]));
-        *reinterpret_cast<uint4*>(dst + sw) = o;
-        if (p.planes == 2) {
-            const uint4 o2 = make_uint4(pack_bf16(s2[0], s2[1]), pack_bf16(s2[2], s2[3]), pack_bf16(s2[4], s2[5]), pack_bf16(s2[6], s2[7]));
-            *reinterpret_cast<uint4*>(dst + p.ng * 64 + sw) = o2;
-        }
+        *reinterpret_cast<uint4*>(dst + sw) = pack_chunk<false>(w);
+        if (p.planes == 2) *reinterpret_cast<uint4*>(dst + p.ng * 64 + sw) = pack_chunk<false>(s2);
         for (int j = 1; j < sets; ++j) {                           // the other samples' weights from the same mu / sigma
             const NoiseKey kj = sample_key(nkey, p.fold, j);
 #pragma unroll
-            for (int e = 0; e < 8; ++e) {
-                const int kq = kb * 64 + chunk * 8 + e;
-                const int cin = (p.prev_hw > 1) ? ((kq % cprev) * p.prev_hw + kq / cprev) : kq;
-                const size_t wi = (size_t)n * g.K + (size_t)cin * g.KHW + tap;
-                w[e] = (n < g.N && kq < g.Cin) ? mu8[e] + normal1(wi, kj) * sg8[e] : 0.0f;
-            }
-            *reinterpret_cast<uint4*>(fold_set(dst, p.fold, j) + sw) =
-                make_uint4(pack_bf16(w[0], w[1]), pack_bf16(w[2], w[3]), pack_bf16(w[4], w[5]), pack_bf16(w[6], w[7]));
+            for (int e = 0; e < 8; ++e) w[e] = w_ok(e) ? fold_draw(mu8[e], sg8[e], w_index(e), kj) : 0.0f;
+            *reinterpret_cast<uint4*>(fold_set(dst, p.fold, j) + sw) = pack_chunk<false>(w);
         }
     }
-    tap_prep_tail<LRT, FOLD>(p, nkey, stoch, do_kl, kl_acc, red);
+    tap_prep_tail<LRT, FOLD>(p, nkey, kl_acc);
 }
 
 // ------------------------------------------------- (P2) tap prep, conv layers
@@ -183,13 +139,11 @@ template <int VARIANT, bool FOLD = false>
 __global__ void __launch_bounds__(256)
 tap_prep_conv_kernel(const FusedArgs p, const int R) {
     extern __shared__ __align__(16) uint8_t prep2_smem[];
-    __shared__ double red[32];
     constexpr bool LRT = VARIANT == BBB_VARIANT_LRT;
     __nv_bfloat16* sm = reinterpret_cast<__nv_bfloat16*>(prep2_smem);
     float2* smf = reinterpret_cast<float2*>(prep2_smem);           // BBB fold: (mu, sigma) per element, same indexing
     const Geom& g = p.g;
     const NoiseKey nkey = effective_key(p.key, p.stream_base);
-    const bool stoch = p.sample != 0, do_kl = p.kl_out != nullptr;
     constexpr bool fold = FOLD;
     const int KHW = g.KHW, L = 64 * KHW, PS = prep2_slab(R);
     const size_t sub = fused_wtile_elems(p);
@@ -217,7 +171,7 @@ tap_prep_conv_kernel(const FusedArgs p, const int R) {
                 wi[u] = (size_t)n * g.K + (size_t)(cin0 + cin) * KHW + tap;
                 so[u] = in ? tap * PS + r * 64 + cin : -1;
                 mu[u] = ok[u] ? __ldg(p.w_mu + wi[u]) : 0.0f;
-                rho[u] = (ok[u] && (stoch || do_kl)) ? __ldg(p.w_rho + wi[u]) : 0.0f;
+                rho[u] = (ok[u] && (p.sample || p.kl_out)) ? __ldg(p.w_rho + wi[u]) : 0.0f;
                 tap += dq; cin += dc;
                 if (tap >= KHW) { tap -= KHW; ++cin; }
                 while (cin >= 64) { cin -= 64; ++r; }
@@ -225,20 +179,14 @@ tap_prep_conv_kernel(const FusedArgs p, const int R) {
 #pragma unroll
             for (int u = 0; u < PREP2_BATCH; ++u) {
                 if (so[u] < 0) continue;
-                float wv = 0.0f, sv = 0.0f;
+                PrepElem o = {0.0f, 0.0f, 0.0f};
                 if (ok[u]) {
-                    const float sigma = (stoch || do_kl) ? softplus_sigma_fast(rho[u]) : 0.0f;
-                    if (LRT) { wv = mu[u]; sv = sigma * sigma; }
-                    else if (fold) smf[so[u]] = make_float2(mu[u], sigma);   // every sample's weight is drawn in phase 2
-                    else if (stoch) {
-                        const float e_ = p.eps_a ? __ldg(p.eps_a + wi[u]) : normal1(wi[u], nkey);
-                        wv = mu[u] + e_ * sigma;
-                    } else wv = mu[u];
-                    if (do_kl) kl_acc += (double)kl_term_fast(mu[u], sigma, p.prior_mu, p.prior_sigma, p.kl_convention);
+                    o = prep_elem<LRT, !fold>(p, mu[u], rho[u], p.eps_a, wi[u], wi[u], nkey, kl_acc);
+                    if (fold) smf[so[u]] = make_float2(mu[u], o.sigma);   // every sample's weight is drawn in phase 2
                 }
                 if (fold) continue;
-                sm[so[u]] = __float2bfloat16_rn(wv);
-                if (p.planes == 2) sm[KHW * PS + so[u]] = __float2bfloat16_rn(sv);
+                sm[so[u]] = __float2bfloat16_rn(o.w);
+                if (p.planes == 2) sm[KHW * PS + so[u]] = __float2bfloat16_rn(o.s2);
             }
         }
         __syncthreads();
@@ -257,10 +205,9 @@ tap_prep_conv_kernel(const FusedArgs p, const int R) {
 #pragma unroll
                     for (int e = 0; e < 8; ++e) {
                         const float2 ms = src[e];
-                        w[e] = (n < g.N && c0 + e < g.Cin) ? ms.x + normal1(wi0 + (size_t)e * KHW, kj) * ms.y : 0.0f;
+                        w[e] = (n < g.N && c0 + e < g.Cin) ? fold_draw(ms.x, ms.y, wi0 + (size_t)e * KHW, kj) : 0.0f;
                     }
-                    *reinterpret_cast<uint4*>(fold_set(dst, p.fold, j)) =
-                        make_uint4(pack_bf16(w[0], w[1]), pack_bf16(w[2], w[3]), pack_bf16(w[4], w[5]), pack_bf16(w[6], w[7]));
+                    *reinterpret_cast<uint4*>(fold_set(dst, p.fold, j)) = pack_chunk<false>(w);
                 }
             }
             __syncthreads();
@@ -279,7 +226,7 @@ tap_prep_conv_kernel(const FusedArgs p, const int R) {
         }
         __syncthreads();
     }
-    tap_prep_tail<LRT, FOLD>(p, nkey, stoch, do_kl, kl_acc, red);
+    tap_prep_tail<LRT, FOLD>(p, nkey, kl_acc);
 }
 
 // ------------------------------------------------------------ wgmma helpers
@@ -686,15 +633,7 @@ inline cudaError_t launch_fused(FusedArgs a, const void* x, const void* x_sq, cu
         int grid = (int)((items + 255) / 256);
         if (grid > 2048) grid = 2048;
         if (grid < 1) grid = 1;
-        static const bool carve = [] {           // see launch_fwd_tc: keep every kernel of the chain on one smem carve-out
-            const char* e = getenv("BBB_B200_PREP_CARVEOUT");
-            if (e && e[0] == '0') return false;
-            cudaFuncSetAttribute(tap_prep_kernel<BBB_VARIANT_LRT>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-            cudaFuncSetAttribute(tap_prep_kernel<BBB_VARIANT_BBB>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-            cudaFuncSetAttribute(tap_prep_kernel<BBB_VARIANT_BBB, true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-            return true;
-        }();
-        (void)carve;
+        prep_carveout<tap_prep_kernel<BBB_VARIANT_LRT>, tap_prep_kernel<BBB_VARIANT_BBB>, tap_prep_kernel<BBB_VARIANT_BBB, true>>();
         // conv layers: the coalesced variant (rows x 64-channel block per CTA); R = rows per CTA, shrunk until the
         // grid covers the SMs and the staging tile fits 48 KB
         static const bool prep2_on = [] { const char* e = getenv("BBB_B200_PREP2"); return !(e && e[0] == '0'); }();
@@ -708,15 +647,8 @@ inline cudaError_t launch_fused(FusedArgs a, const void* x, const void* x_sq, cu
         while (R > 2 && ((long)(npad / R) * a.n_kblk < n_sm || need(R) > kPrepSmem)) R >>= 1;
         const bool prep2 = prep2_on && g.KHW > 1 && a.prev_hw == 1 && g.Cin % 64 == 0 && a.taps == g.KHW && need(R) <= 48 * 1024;
         if (prep2) {
-            static const bool carve2 = [] {
-                const char* e = getenv("BBB_B200_PREP_CARVEOUT");
-                if (e && e[0] == '0') return false;
-                cudaFuncSetAttribute(tap_prep_conv_kernel<BBB_VARIANT_LRT>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-                cudaFuncSetAttribute(tap_prep_conv_kernel<BBB_VARIANT_BBB>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-                cudaFuncSetAttribute(tap_prep_conv_kernel<BBB_VARIANT_BBB, true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-                return true;
-            }();
-            (void)carve2;
+            prep_carveout<tap_prep_conv_kernel<BBB_VARIANT_LRT>, tap_prep_conv_kernel<BBB_VARIANT_BBB>,
+                          tap_prep_conv_kernel<BBB_VARIANT_BBB, true>>();
             int grid2 = (npad / R) * a.n_kblk;
             if (grid2 > 2048) grid2 = 2048;
             // a BBB fold stages fp32 (mu, sigma) pairs: 4x the bf16 slab, same R and grid as the unfolded call

@@ -33,28 +33,17 @@
 
 namespace bbb {
 
-struct TcArgs {
-    Geom g;
-    const void* x; const float* w_mu; const float* w_rho; const float* b_mu; const float* b_rho;
-    void* y; float* kl_out; float* act_std;
-    const float* eps_a; const float* eps_b;
-    NoiseKey key; const unsigned long long* stream_base;
-    double* kl_partials; unsigned int* kl_counter;
-    float prior_mu, prior_sigma;
-    int sample, kl_convention, has_bias, act, act_dtype, variant;
-    // prepared-operand workspace
-    __nv_bfloat16* wtiles;   // [n_tiles][k_blocks][planes][8 KB tile]  (64 rows x 8 K chunks of 16 bytes: 64 bf16 or 32 tf32 of K)
-    float* bias_ws;          // [2][Npad]: row 0 = bias (BBB: sampled; LRT: mu), row 1 = LRT sigma_b^2
-    int n_tiles, k_blocks, planes;
+// wtiles: [n_tiles][k_blocks][planes][8 KB tile]  (64 rows x 8 K chunks of 16 bytes: 64 bf16 or 32 tf32 of K)
+struct TcArgs : LayerArgs {
+    const void* x; void* y; float* act_std;
+    int act_dtype;
+    int n_tiles, k_blocks;
     int skip_prep, prep_only;
     int tf32;                // operands as tf32 (fp32 storage, 4 elements per 16-byte K chunk, kind::tf32) instead of bf16
     int stage_x;             // stage the tile's input images in shared memory: 0 no, 1 as fp32, 2 as bf16 (half the
                              // footprint: lets two LRT CTAs share an SM; x^2 is then formed from the bf16 value)
     // fused epilogue (first layer of a fused chain): 2x2 max-pool + packed bf16 output
     void* y_sq; int out_mode, out_pitch, pool;     // out_mode: 0 packed bf16 [B,(pix,c)], 2 NCHW fp32 (default)
-    long long* trace;                              // debug: per-CTA clock64 checkpoints (nullptr in production)
-    long long* tl_prep; long long* tl_gemm;        // debug: timeline slots of the two launches (nullptr in production)
-    McFold fold;                                   // MC samples folded into the batch (rows = 0: off; common.cuh)
 };
 
 constexpr int TC_BM = 128, TC_BN = 64, TC_BK = 64;
@@ -77,9 +66,11 @@ inline int tc_stages(const Geom& g, int planes) {
     if (s > 4) s = 4;
     return (int)s;
 }
+// operand tiles: 2 planes x npad rows x (kpad * 2 bytes of bf16 | kpad32 * 4 bytes of tf32), then the bias rows
+inline size_t tc_bias_offset(const Geom& g, bool tf32) { return (size_t)tc_npad(g) * tc_kpad(g, tf32) * (tf32 ? 8 : 4); }
 inline size_t tc_workspace_bytes(const Geom& g) {
-    // 2 planes of operand tiles (bf16: kpad * 2 bytes per row, tf32: kpad32 * 4 -- never less) + bias rows
-    return (size_t)tc_npad(g) * tc_kpad(g, true) * 2 /*planes*/ * 4 /*tf32*/ + (size_t)2 * tc_npad(g) * 4;
+    // the tf32 layout, never smaller than the bf16 one
+    return tc_bias_offset(g, true) + (size_t)2 * tc_npad(g) * 4;
 }
 inline bool tc_supported(const bbb_layer_desc& d, const Geom& g) {
     if (d.act_dtype != BBB_DTYPE_F32) return false;
@@ -296,6 +287,93 @@ __device__ __noinline__ void store_row16(const StoreCfg p, int b, int pos, int n
     }
 }
 
+// ------------------------------------------------ (P) shared by every prep kernel
+// The parameter math of the weight-prep kernels (weight_prep_kernel here, tap_prep_kernel / tap_prep_conv_kernel in
+// fused_tc.cuh, conv_s4_prep_kernel in conv_s4_tc.cuh); each kernel adds only its index mapping and tile layout.
+// The KL is a per-thread double sum in the kernel's own loop order, then prep_finish: keep both, or the KL bits move.
+
+// rho of one element: the value a kernel already loaded, or where to read it (RhoAt).  Either way it is only used, and
+// a RhoAt only read, when sigma is needed: a sampling call or one that computes the KL.
+struct RhoAt { const float* rho; size_t i; };
+__device__ __forceinline__ float rho_of(float rho) { return rho; }
+__device__ __forceinline__ float rho_of(const RhoAt& r) { return __ldg(r.rho + r.i); }
+
+// One parameter element: sigma = softplus(rho); plane 0 = BBB mu + eps*sigma when sampling (eps: `eps[ei]` if given,
+// else Philox element i), otherwise mu; plane 1 = LRT sigma^2; and its KL term added to `kl`.
+// DRAW = false leaves plane 0 at mu: a BBB fold that draws every sample later with fold_draw.
+struct PrepElem { float w, s2, sigma; };
+template <bool LRT, bool DRAW = true, class Rho>
+__device__ __forceinline__ PrepElem prep_elem(const LayerArgs& p, float mu, const Rho& rho, const float* eps, size_t ei,
+                                              uint64_t i, const NoiseKey& nkey, double& kl) {
+    const bool stoch = p.sample != 0, do_kl = p.kl_out != nullptr;
+    PrepElem o = {mu, 0.0f, 0.0f};
+    if (stoch || do_kl) o.sigma = softplus_sigma_fast(rho_of(rho));
+    if (LRT) o.s2 = o.sigma * o.sigma;
+    else if (DRAW && stoch) {
+        const float e_ = eps ? __ldg(eps + ei) : normal1(i, nkey);
+        o.w = mu + e_ * o.sigma;
+    }
+    if (do_kl) kl += (double)kl_term_fast(mu, o.sigma, p.prior_mu, p.prior_sigma, p.kl_convention);
+    return o;
+}
+
+// Weight sample j of a BBB fold: the same element drawn on sample j's stream, kj = sample_key(nkey, fold, j)
+__device__ __forceinline__ float fold_draw(float mu, float sigma, uint64_t i, const NoiseKey& kj) {
+    return mu + normal1(i, kj) * sigma;
+}
+
+// Bias rows of every operand set: bias_ws[n] (BBB: sampled, LRT: mu) and bias_ws[npad + n] (LRT: sigma_b^2) for all npad
+// padded columns, zero past N or without a bias; one thread per column, each bias KL term counted once.  Bias element n
+// is Philox element N*K + n, behind the weights.
+template <bool LRT, bool FOLD>
+__device__ __forceinline__ void prep_bias(const LayerArgs& p, const NoiseKey& nkey, int npad, double& kl) {
+    const Geom& g = p.g;
+    const uint64_t i0 = (uint64_t)g.N * g.K;
+    for (int n = blockIdx.x * blockDim.x + threadIdx.x; n < npad; n += gridDim.x * blockDim.x) {
+        const bool real = p.has_bias && n < g.N;
+        float mu = 0.0f;
+        PrepElem o = {0.0f, 0.0f, 0.0f};
+        if (real) {
+            mu = __ldg(p.b_mu + n);
+            o = prep_elem<LRT>(p, mu, RhoAt{p.b_rho, (size_t)n}, p.eps_b, n, i0 + n, nkey, kl);
+        }
+        p.bias_ws[n] = o.w;
+        p.bias_ws[npad + n] = o.s2;
+        if (FOLD) {
+            for (int j = 1; j < p.fold.sets; ++j) {
+                float* bj = fold_set(p.bias_ws, p.fold, j);
+                bj[n] = real ? fold_draw(mu, o.sigma, i0 + n, sample_key(nkey, p.fold, j)) : 0.0f;
+                bj[npad + n] = 0.0f;
+            }
+        }
+    }
+}
+
+// End of a prep kernel: the CTA's KL partial, published in CTA order (kl_publish), then the timeline exit
+__device__ __forceinline__ void prep_finish(const LayerArgs& p, double kl) {
+    __shared__ double red[32];
+    if (p.kl_out) {
+        const double tot = block_sum(kl, red);
+        if (threadIdx.x == 0) kl_publish(tot, blockIdx.x, gridDim.x, p.kl_partials, p.kl_counter, p.kl_out);
+    }
+    tl_exit(p.tl_prep);
+}
+
+// Prep kernels run on the same shared-memory carve-out as the GEMM kernels: an SM only changes its L1/smem split when
+// idle, so prep CTAs running at the default (small-smem) split kept the first GEMM's CTAs off every SM they touched until
+// their grids drained (tools/timeline.py shows the start of each GEMM).  Set once per process for the listed kernels;
+// BBB_B200_PREP_CARVEOUT=0 leaves the default split.
+template <auto... Kernels>
+inline void prep_carveout() {
+    static const bool on = [] {
+        const char* e = getenv("BBB_B200_PREP_CARVEOUT");
+        if (e && e[0] == '0') return false;
+        (cudaFuncSetAttribute(Kernels, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared), ...);
+        return true;
+    }();
+    (void)on;
+}
+
 // ------------------------------------------------------------ (P) weight prep
 // One CTA per (n-tile, k-block) 64x64 tile (grid-stride).  256 threads: item = (row, 8-wide
 // K chunk); consecutive threads take consecutive rows so the 16-byte writes are contiguous.
@@ -304,14 +382,11 @@ __device__ __noinline__ void store_row16(const StoreCfg p, int b, int pos, int n
 template <int VARIANT, bool TF32, bool FOLD = false>
 __global__ void __launch_bounds__(256)
 weight_prep_kernel(const TcArgs p) {
-    __shared__ double red[32];
     constexpr bool LRT = VARIANT == BBB_VARIANT_LRT;
+    static_assert(!(LRT && FOLD), "a fold prep draws BBB weight samples");
     constexpr int CE = TF32 ? 4 : 8, BKE = 8 * CE;                  // elements per 16-byte chunk / per K block
     const Geom& g = p.g;
     const NoiseKey nkey = effective_key(p.key, p.stream_base);
-    const bool stoch = p.sample != 0;
-    const bool do_kl = p.kl_out != nullptr;
-    const int npad = p.n_tiles * TC_BN;
     constexpr int PER_TILE = TC_BN * (TC_BK / 8);                   // (row, 8-wide K chunk) items per tile
     const long n_items = (long)p.n_tiles * p.k_blocks * PER_TILE;
     double kl_acc = 0.0;
@@ -327,66 +402,31 @@ weight_prep_kernel(const TcArgs p) {
 #pragma unroll
         for (int e = 0; e < CE; ++e) {
             const int k = k0 + e;
-            float wv = 0.0f, sv = 0.0f;
             mu8[e] = sg8[e] = 0.0f;
             if (n < g.N && k < g.K) {
                 const size_t wi = (size_t)n * g.K + k;
                 const float mu = __ldg(p.w_mu + wi);
-                float sigma = 0.0f;
-                if (stoch || do_kl) sigma = softplus_sigma_fast(__ldg(p.w_rho + wi));
-                if (LRT) { wv = mu; sv = sigma * sigma; }
-                else if (stoch) {
-                    const float e_ = p.eps_a ? __ldg(p.eps_a + wi) : normal1(wi, nkey);
-                    wv = mu + e_ * sigma;
-                } else wv = mu;
-                if (do_kl) kl_acc += (double)kl_term_fast(mu, sigma, p.prior_mu, p.prior_sigma, p.kl_convention);
-                mu8[e] = mu; sg8[e] = sigma;
+                const PrepElem o = prep_elem<LRT>(p, mu, RhoAt{p.w_rho, wi}, p.eps_a, wi, wi, nkey, kl_acc);
+                w[e] = o.w; s2[e] = o.s2; mu8[e] = mu; sg8[e] = o.sigma;
             }
-            w[e] = wv; s2[e] = sv;
         }
         // canonical K-major core-matrix order inside the 8 KB tile: chunk*1024 + row*16 bytes
         *reinterpret_cast<uint4*>(dst + chunk * (TC_BN * 16) + row * 16) = pack_chunk<TF32>(w);
         if (p.planes == 2) *reinterpret_cast<uint4*>(dst + TC_B_BYTES + chunk * (TC_BN * 16) + row * 16) = pack_chunk<TF32>(s2);
         if (FOLD) {
-            for (int j = 1; j < p.fold.sets; ++j) {                // sample j: the same element's draw on its own stream
+            for (int j = 1; j < p.fold.sets; ++j) {
                 const NoiseKey kj = sample_key(nkey, p.fold, j);
 #pragma unroll
                 for (int e = 0; e < CE; ++e) {
                     const int k = k0 + e;
-                    w[e] = (n < g.N && k < g.K) ? mu8[e] + normal1((size_t)n * g.K + k, kj) * sg8[e] : 0.0f;
+                    w[e] = (n < g.N && k < g.K) ? fold_draw(mu8[e], sg8[e], (size_t)n * g.K + k, kj) : 0.0f;
                 }
                 *reinterpret_cast<uint4*>(fold_set(dst, p.fold, j) + chunk * (TC_BN * 16) + row * 16) = pack_chunk<TF32>(w);
             }
         }
     }
-    for (int n = blockIdx.x * blockDim.x + threadIdx.x; n < npad; n += gridDim.x * blockDim.x) {   // bias
-        float bm = 0.0f, bv = 0.0f, bmu = 0.0f, bsg = 0.0f;
-        if (p.has_bias && n < g.N) {
-            const float mu = __ldg(p.b_mu + n);
-            const float sigma = (stoch || do_kl) ? softplus_sigma_fast(__ldg(p.b_rho + n)) : 0.0f;
-            if (LRT) { bm = mu; bv = sigma * sigma; }
-            else if (stoch) {
-                const float e_ = p.eps_b ? __ldg(p.eps_b + n) : normal1((uint64_t)g.N * g.K + n, nkey);
-                bm = mu + e_ * sigma;
-            } else bm = mu;
-            if (do_kl) kl_acc += (double)kl_term_fast(mu, sigma, p.prior_mu, p.prior_sigma, p.kl_convention);
-            bmu = mu; bsg = sigma;
-        }
-        p.bias_ws[n] = bm;
-        p.bias_ws[npad + n] = bv;
-        if (FOLD) {
-            for (int j = 1; j < p.fold.sets; ++j) {
-                float* bj = fold_set(p.bias_ws, p.fold, j);
-                bj[n] = (p.has_bias && n < g.N) ? bmu + normal1((uint64_t)g.N * g.K + n, sample_key(nkey, p.fold, j)) * bsg : 0.0f;
-                bj[npad + n] = 0.0f;
-            }
-        }
-    }
-    if (do_kl) {
-        const double tot = block_sum(kl_acc, red);
-        if (threadIdx.x == 0) kl_publish(tot, blockIdx.x, gridDim.x, p.kl_partials, p.kl_counter, p.kl_out);
-    }
-    tl_exit(p.tl_prep);
+    prep_bias<LRT, FOLD>(p, nkey, p.n_tiles * TC_BN, kl_acc);
+    prep_finish(p, kl_acc);
 }
 
 // ----------------------------------------------------------------- (G) GEMM
@@ -680,20 +720,11 @@ inline cudaError_t launch_fwd_tc_t(TcArgs a, cudaStream_t st, int* n_launch) {
         const long items = (long)a.n_tiles * a.k_blocks * TC_BN * 8;
         int grid = (int)((items + 255) / 256);
         if (grid > 2048) grid = 2048;
-        // Same shared-memory carve-out as the GEMM kernels: an SM only changes its L1/smem split when idle, so prep
-        // CTAs running at the default (small-smem) split kept the first GEMM's CTAs off every SM they touched until
-        // their grids drained (tools/timeline.py shows the start of each GEMM).
         // A BBB fold (one operand set per weight sample) keeps the grid, so its KL sums in the unfolded call's order.
-        const bool fold = VARIANT == BBB_VARIANT_BBB && a.fold.sets > 1;
-        auto* prep = fold ? weight_prep_kernel<VARIANT, TF32, true> : weight_prep_kernel<VARIANT, TF32, false>;
-        static const bool carve = [] {
-            const char* e = getenv("BBB_B200_PREP_CARVEOUT");
-            if (e && e[0] == '0') return false;
-            cudaFuncSetAttribute(weight_prep_kernel<VARIANT, TF32, false>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-            cudaFuncSetAttribute(weight_prep_kernel<VARIANT, TF32, true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-            return true;
-        }();
-        (void)carve;
+        // (For LRT both names below are the unfolded prep: only BBB has a fold instantiation.)
+        constexpr bool BBB = VARIANT == BBB_VARIANT_BBB;
+        prep_carveout<weight_prep_kernel<VARIANT, TF32, false>, weight_prep_kernel<VARIANT, TF32, BBB>>();
+        auto* prep = BBB && a.fold.sets > 1 ? weight_prep_kernel<VARIANT, TF32, BBB> : weight_prep_kernel<VARIANT, TF32, false>;
         prep<<<grid, 256, 0, st>>>(a);
         cudaError_t e = cudaGetLastError();
         if (e != cudaSuccess) return e;
