@@ -101,7 +101,17 @@ size_t bbb_workspace_bytes(const bbb_layer_desc* desc);
  *          own weight draw; needs (reserved[1] * OH * OW) % 128 == 0 and the workspace of the folding desc.  The KL is
  *          computed once, bit-identical to an unfolded call.  Needs sample == 1, in-kernel noise (eps_a / eps_b NULL,
  *          else BBB_E_UNSUPPORTED), batch % reserved[1] == 0 (else BBB_E_INVALID) and a tensor-core math mode (bf16 /
- *          tf32, or auto resolving to one; else BBB_E_UNSUPPORTED).  reserved[] all zero: no fold. */
+ *          tf32, or auto resolving to one; else BBB_E_UNSUPPORTED).  reserved[] all zero: no fold.
+ * desc->reserved[0] bits 8..30 (BBB_FIRST_IMAGE_*): the FIRST IMAGE, the global index of image 0 of this call (of each
+ *          sample block when folded) when a batch is split into row blocks over several calls or ranks
+ *          (bbb_mc_exchange_sharded).  LRT: image b draws its activation noise at element index
+ *          (((first_image + b)*OH*OW + pixel)*Cout + c) -- what an unsplit call draws at its rows, bit for bit.  Only the
+ *          Philox counter moves; x, y, eps_a and act_std stay indexed by the call's own rows.  BBB weight noise does not
+ *          depend on rows.  Accepted by every forward, both backwards and the support queries; a negative reserved[0]
+ *          or a first image whose last image would pass int32 element counts ((first_image + rows)*OH*OW*Cout, rows =
+ *          reserved[1] when folded, else batch) is BBB_E_INVALID.  0 = the batch starts at image 0 (unsplit). */
+#define BBB_FIRST_IMAGE_SHIFT 8
+#define BBB_FIRST_IMAGE_MASK 0x7fffff00u
 int bbb_conv2d_forward(const bbb_layer_desc* desc, const void* x,
                        const float* W_mu, const float* W_rho,
                        const float* bias_mu, const float* bias_rho,
@@ -150,7 +160,8 @@ enum { BBB_LAYOUT_NCHW_F32 = 0,      /* reference layout: [B, C, H, W] fp32     
  * desc->reserved[0] splits the call so the parameter-only half can run on a side stream, off
  * the activation critical path: BBB_FUSED_PREP_ONLY launches just the weight-prep kernel
  * (sigma, eps, bf16 operand tiles, KL -> kl_out; x/y unused), BBB_FUSED_SKIP_PREP just the GEMM
- * kernel (the caller orders it after the prep, e.g. with an event).  0 = both, in order.
+ * kernel (the caller orders it after the prep, e.g. with an event).  0 = both, in order.  Bits 8..30 of reserved[0]
+ * carry the first image of a row block, as on bbb_conv2d_forward (the phase stays in bits 0..1).
  * desc->reserved[1] > 0 folds Monte-Carlo samples into the batch (in-kernel Philox noise only; what
  * uncertainty_estimation.py:38-41 does by repeating the input): row b of the batch is image b % reserved[1] of sample
  * s = b / reserved[1], whose noise comes from Philox stream stream_id + s * stride, stride = the uint64 in reserved[2]
@@ -192,7 +203,7 @@ int bbb_kl_backward(const float* mu, const float* rho, uint64_t n,
 
 /* Backward of bbb_conv2d_forward / bbb_linear_forward (SURVEY.md Appendix A).
  * Regenerates eps from (seed, stream_id) or reads eps_a/eps_b exactly like the
- * forward.  grad_x nullable.  g_* are ACCUMULATED into (caller zeroes).
+ * forward (the first image of desc->reserved[0] included).  grad_x nullable.  g_* are ACCUMULATED into (caller zeroes).
  * act_std: LRT only, the tensor the forward saved.                            */
 int bbb_conv2d_backward(const bbb_layer_desc* desc, const void* x, const void* grad_y,
                         const float* W_mu, const float* W_rho,
@@ -279,6 +290,23 @@ int bbb_mc_exchange_info(const float* logits, int32_t S_local, int32_t S_total, 
                          float* pred, float* epistemic, float* aleatoric, float* entropy, float* head,
                          uint64_t* noise_base, uint64_t noise_inc, float* expected_entropy, float* mutual_info,
                          void* cuda_stream);
+/* bbb_mc_exchange_info with the batch split into row blocks as well as the samples into groups, so that every rank works
+ * when there are fewer samples than ranks (or they do not divide evenly).  world = Rs x Rb, Rb = batch_shards (world %
+ * batch_shards != 0 or batch_shards > B: BBB_E_INVALID).  Rank r is sample group g = r % Rs (it holds the samples
+ * {j : j mod Rs == g}) and row block k = r / Rs: images [b0, b1), the blocks as equal as possible, the first B % Rb one
+ * image longer.  logits: [S_local, b1 - b0, C] (its rows only); labels: all [B].  Every rank returns the same full
+ * [B, C] / [B] outputs and head as bbb_mc_exchange_info, and they are bitwise equal to that call on Rs ranks holding
+ * the same samples: the receive buffer is [2 slots][Rs][...] -- bbb_mc_buffer_bytes(B, C, flags, Rs) -- rank (g, k)
+ * pushes the words of its rows into slot g of every peer, the block-0 rank of each group its KL word, and the Rs groups
+ * are merged in ascending order.  peer_buffers still holds all `world` buffers.  batch_shards == 1 is
+ * bbb_mc_exchange_info (the same kernel).  The callers' layer calls draw the rows of a block with the first image b0
+ * (desc->reserved[0]), so per-sample logits do not depend on (Rs, Rb). */
+int bbb_mc_exchange_sharded(const float* logits, int32_t S_local, int32_t S_total, int32_t B, int32_t C, const float* kl,
+                            int32_t n_kl, int32_t flags, const int64_t* labels, float train_size, float beta,
+                            int32_t rank, int32_t world, void* const* peer_buffers, void* state, float* log_outputs,
+                            float* kl_out, float* pred, float* epistemic, float* aleatoric, float* entropy, float* head,
+                            uint64_t* noise_base, uint64_t noise_inc, float* expected_entropy, float* mutual_info,
+                            int32_t batch_shards, void* cuda_stream);
 
 /* Peer-mapped receive buffers for bbb_mc_exchange (one process per GPU, same node): allocate locally, export a
  * 64-byte CUDA-IPC handle, ship it to the peers by any host channel (the Python side uses torch.distributed),

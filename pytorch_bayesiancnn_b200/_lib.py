@@ -30,7 +30,7 @@ SYMBOLS = (
     "bbb_forward_supported", "bbb_kl_forward",
     "bbb_kl_backward", "bbb_conv2d_backward", "bbb_linear_backward", "bbb_philox_normal_fill",
     "bbb_mc_combine", "bbb_noise_advance", "bbb_last_error", "bbb_abi_version", "bbb_launch_count",
-    "bbb_mc_buffer_bytes", "bbb_mc_state_bytes", "bbb_mc_exchange", "bbb_mc_exchange_info",
+    "bbb_mc_buffer_bytes", "bbb_mc_state_bytes", "bbb_mc_exchange", "bbb_mc_exchange_info", "bbb_mc_exchange_sharded",
     "bbb_comm_alloc", "bbb_comm_free", "bbb_comm_export", "bbb_comm_import", "bbb_comm_unimport", "bbb_set_wide_tiles",
 )
 MC_MOMENTS, MC_NORMALIZED, MC_INFO = 1, 2, 4
@@ -90,6 +90,8 @@ def _bind(lib):
     lib.bbb_mc_exchange.restype = C.c_int
     lib.bbb_mc_exchange_info.argtypes = lib.bbb_mc_exchange.argtypes[:-1] + [fp, fp, vp]
     lib.bbb_mc_exchange_info.restype = C.c_int
+    lib.bbb_mc_exchange_sharded.argtypes = lib.bbb_mc_exchange_info.argtypes[:-1] + [i32, vp]
+    lib.bbb_mc_exchange_sharded.restype = C.c_int
     lib.bbb_comm_alloc.argtypes = [sz, C.POINTER(C.c_void_p)]
     lib.bbb_comm_export.argtypes = [vp, vp]
     lib.bbb_comm_import.argtypes = [vp, C.POINTER(C.c_void_p)]

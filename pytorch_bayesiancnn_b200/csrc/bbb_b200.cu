@@ -69,6 +69,8 @@ bool s4_enabled() {
     return on;
 }
 
+int first_image_of(const bbb_layer_desc& d) { return (int)(((uint32_t)d.reserved[0] & BBB_FIRST_IMAGE_MASK) >> BBB_FIRST_IMAGE_SHIFT); }
+
 int check_desc(const bbb_layer_desc* d, bbb::Geom& g, bool linear) {
     if (!d) return fail(BBB_E_INVALID, "desc is NULL");
     if (!bbb::make_geom(*d, g)) return fail(BBB_E_INVALID, "invalid layer geometry");
@@ -77,6 +79,13 @@ int check_desc(const bbb_layer_desc* d, bbb::Geom& g, bool linear) {
     if (d->kl_convention != BBB_KL_REFERENCE && d->kl_convention != BBB_KL_TEXTBOOK) return fail(BBB_E_INVALID, "bad kl_convention");
     if (d->epilogue_act < BBB_ACT_NONE || d->epilogue_act > BBB_ACT_RELU) return fail(BBB_E_INVALID, "bad epilogue_act");
     if (!(d->prior_sigma > 0.0f)) return fail(BBB_E_INVALID, "prior_sigma must be > 0");
+    // first image of a row block (reserved[0] bits 8..30, include/bbb_b200.h): the noise index of its last image must
+    // still be an int32 element count, as that of an unsplit batch is
+    if (d->reserved[0] < 0) return fail(BBB_E_INVALID, "negative first image (desc->reserved[0] = %d)", d->reserved[0]);
+    const long images = (long)first_image_of(*d) + (d->reserved[1] > 0 ? d->reserved[1] : g.B);
+    if (images * g.OHW * g.N > 0x7fffffffL)
+        return fail(BBB_E_INVALID, "first image %d: image %ld x %d x %d outputs passes int32 element counts",
+                    first_image_of(*d), images, g.OHW, g.N);
     return BBB_OK;
 }
 
@@ -113,6 +122,7 @@ int layer_fold_check(const bbb_layer_desc* d, const bbb::Geom& g, int math) {
 // noise in-kernel, so it takes no external eps.
 int layer_fold(const bbb_layer_desc* d, const bbb::Geom& g, const float* eps_a, const float* eps_b, bbb::McFold& fold) {
     fold.rows = 0; fold.stride = 0; fold.sets = 1; fold.set_bytes = 0;
+    fold.first_image = first_image_of(*d);
     if (d->reserved[1] <= 0) return BBB_OK;
     if (eps_a || eps_b) return fail(BBB_E_UNSUPPORTED, "MC-sample folding draws its noise in-kernel (no external eps)");
     fold.rows = d->reserved[1];
@@ -183,6 +193,7 @@ int forward_impl(const bbb_layer_desc* d, bool linear, const void* x, const floa
     a.kl_counter = (unsigned int*)ws; a.kl_partials = (double*)((char*)ws + kCounterBytes);
     a.prior_mu = d->prior_mu; a.prior_sigma = d->prior_sigma;
     a.sample = d->sample; a.kl_convention = d->kl_convention; a.has_bias = d->has_bias; a.act = d->epilogue_act;
+    a.first_image = first_image_of(*d);
     cudaError_t e = d->variant == BBB_VARIANT_LRT ? bbb::launch_fwd_simt<BBB_VARIANT_LRT>(a, st)
                                                   : bbb::launch_fwd_simt<BBB_VARIANT_BBB>(a, st);
     if (e != cudaSuccess) return cuda_fail(e, "fwd_simt launch");
@@ -210,6 +221,7 @@ int backward_impl(const bbb_layer_desc* d, bool linear, const void* x, const voi
     a.key = bbb::make_key(seed, stream_id); a.stream_base = (const unsigned long long*)stream_base;
     a.gx = (float*)grad_x; a.g_w_mu = g_W_mu; a.g_w_rho = g_W_rho; a.g_b_mu = g_bias_mu; a.g_b_rho = g_bias_rho;
     a.sample = d->sample; a.has_bias = d->has_bias; a.variant = d->variant;
+    a.first_image = first_image_of(*d);
     int nl = 0;
     cudaError_t e = bbb::launch_bwd_simt(a, (cudaStream_t)stream, sm_count(), &nl);
     if (e != cudaSuccess) return cuda_fail(e, "bwd_simt launch");
@@ -439,12 +451,16 @@ size_t bbb_mc_buffer_bytes(int32_t B, int32_t C, int32_t flags, int32_t world) {
 }
 size_t bbb_mc_state_bytes(void) { return 64 + (size_t)bbb::MCX_MAX_CTAS * 2 * sizeof(double); }
 
-int bbb_mc_exchange_info(const float* logits, int32_t S_local, int32_t S_total, int32_t B, int32_t C, const float* kl,
-                         int32_t n_kl, int32_t flags, const int64_t* labels, float train_size, float beta, int32_t rank,
-                         int32_t world, void* const* peer_buffers, void* state, float* log_outputs, float* kl_out, float* pred,
-                         float* epistemic, float* aleatoric, float* entropy, float* head, uint64_t* noise_base,
-                         uint64_t noise_inc, float* expected_entropy, float* mutual_info, void* cuda_stream) {
+// bbb_mc_exchange_info and bbb_mc_exchange_sharded: batch_shards == 1 launches the default kernels
+static int mc_exchange_impl(const float* logits, int32_t S_local, int32_t S_total, int32_t B, int32_t C, const float* kl,
+                            int32_t n_kl, int32_t flags, const int64_t* labels, float train_size, float beta, int32_t rank,
+                            int32_t world, void* const* peer_buffers, void* state, float* log_outputs, float* kl_out,
+                            float* pred, float* epistemic, float* aleatoric, float* entropy, float* head,
+                            uint64_t* noise_base, uint64_t noise_inc, float* expected_entropy, float* mutual_info,
+                            int32_t batch_shards, void* cuda_stream) {
     if (!log_outputs || !peer_buffers || !state) return fail(BBB_E_INVALID, "NULL pointer");
+    if (batch_shards < 1 || world % batch_shards) return fail(BBB_E_INVALID, "world %d is not a multiple of batch_shards %d", world, batch_shards);
+    if (batch_shards > B) return fail(BBB_E_INVALID, "batch_shards %d > B %d: a row block would be empty", batch_shards, B);
     if (S_local < 0 || S_total <= 0 || B <= 0 || C <= 0) return fail(BBB_E_INVALID, "bad S/B/C");
     if (S_local > 0 && !logits) return fail(BBB_E_INVALID, "S_local > 0 but logits is NULL");
     if (S_local > bbb::MCX_MAX_SLOCAL) return fail(BBB_E_UNSUPPORTED, "more than %d local samples per call", bbb::MCX_MAX_SLOCAL);
@@ -470,18 +486,43 @@ int bbb_mc_exchange_info(const float* logits, int32_t S_local, int32_t S_total, 
     a.log_outputs = log_outputs; a.kl_out = kl_out; a.pred = pred; a.epistemic = epistemic; a.aleatoric = aleatoric;
     a.entropy = entropy; a.head = head; a.trace = g_mcx_trace;
     a.expected_entropy = expected_entropy; a.mutual_info = mutual_info;
+    // row blocks: rank r = sample group r % Rs, row block r / Rs; blocks as equal as possible, the first B % Rb one longer
+    const int Rs = world / batch_shards, blk = rank / Rs, per = B / batch_shards, rem = B % batch_shards;
+    a.groups = Rs; a.group = rank % Rs; a.block = blk;
+    a.row0 = blk * per + (blk < rem ? blk : rem); a.rows = per + (blk < rem ? 1 : 0);
     { bbb::Geom tg = {}; tg.M = B; tg.N = C; tg.K = S_local; a.tl = tl_slot(true, "mc_exchange", tg); }
-    // the grid depends on B only: CTA c of every rank owns the same images, so flags pair up CTA by CTA.  At most
-    // MCX_MAX_CTAS CTAs: all co-resident, so a CTA spinning on a peer's flag never keeps that peer's producer off an SM.
+    // the grid depends on B only: CTA c of every rank finishes the same images.  At most MCX_MAX_CTAS CTAs: all
+    // co-resident, so a CTA spinning on a peer's word never keeps that peer's producer off an SM.
     int grid = (B + bbb::MCX_THREADS / 32 - 1) / (bbb::MCX_THREADS / 32);
     if (grid > bbb::MCX_MAX_CTAS) grid = bbb::MCX_MAX_CTAS;
-    cudaError_t e = bbb::launch_pdl(info ? bbb::mc_exchange_kernel<true> : bbb::mc_exchange_kernel<false>, dim3(grid),
-                                     dim3(bbb::MCX_THREADS), (size_t)(bbb::MCX_THREADS / 32) * S_local * sizeof(float),
+    const bool shard = batch_shards > 1;
+    cudaError_t e = bbb::launch_pdl(shard ? (info ? bbb::mc_exchange_kernel<true, true> : bbb::mc_exchange_kernel<false, true>)
+                                          : (info ? bbb::mc_exchange_kernel<true> : bbb::mc_exchange_kernel<false>),
+                                     dim3(grid), dim3(bbb::MCX_THREADS), (size_t)(bbb::MCX_THREADS / 32) * S_local * sizeof(float),
                                      (cudaStream_t)cuda_stream, a);
     if (e == cudaSuccess) e = cudaGetLastError();
     if (e != cudaSuccess) return cuda_fail(e, "mc_exchange launch");
     g_launches += 1;
     return BBB_OK;
+}
+int bbb_mc_exchange_info(const float* logits, int32_t S_local, int32_t S_total, int32_t B, int32_t C, const float* kl,
+                         int32_t n_kl, int32_t flags, const int64_t* labels, float train_size, float beta, int32_t rank,
+                         int32_t world, void* const* peer_buffers, void* state, float* log_outputs, float* kl_out, float* pred,
+                         float* epistemic, float* aleatoric, float* entropy, float* head, uint64_t* noise_base,
+                         uint64_t noise_inc, float* expected_entropy, float* mutual_info, void* cuda_stream) {
+    return mc_exchange_impl(logits, S_local, S_total, B, C, kl, n_kl, flags, labels, train_size, beta, rank, world,
+                            peer_buffers, state, log_outputs, kl_out, pred, epistemic, aleatoric, entropy, head, noise_base,
+                            noise_inc, expected_entropy, mutual_info, 1, cuda_stream);
+}
+int bbb_mc_exchange_sharded(const float* logits, int32_t S_local, int32_t S_total, int32_t B, int32_t C, const float* kl,
+                            int32_t n_kl, int32_t flags, const int64_t* labels, float train_size, float beta, int32_t rank,
+                            int32_t world, void* const* peer_buffers, void* state, float* log_outputs, float* kl_out,
+                            float* pred, float* epistemic, float* aleatoric, float* entropy, float* head,
+                            uint64_t* noise_base, uint64_t noise_inc, float* expected_entropy, float* mutual_info,
+                            int32_t batch_shards, void* cuda_stream) {
+    return mc_exchange_impl(logits, S_local, S_total, B, C, kl, n_kl, flags, labels, train_size, beta, rank, world,
+                            peer_buffers, state, log_outputs, kl_out, pred, epistemic, aleatoric, entropy, head, noise_base,
+                            noise_inc, expected_entropy, mutual_info, batch_shards, cuda_stream);
 }
 int bbb_mc_exchange(const float* logits, int32_t S_local, int32_t S_total, int32_t B, int32_t C, const float* kl,
                     int32_t n_kl, int32_t flags, const int64_t* labels, float train_size, float beta, int32_t rank, int32_t world,

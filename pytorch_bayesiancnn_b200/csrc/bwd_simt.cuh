@@ -26,13 +26,14 @@ struct BwdArgs {
     float* gx; float* g_w_mu; float* g_w_rho; float* g_b_mu; float* g_b_rho;
     int sample, has_bias, variant;
     int m_chunk;        // rows of M per wgrad split
+    int first_image;    // as in the forward (FwdArgs): LRT noise of image b is drawn at image first_image + b
 };
 
 __device__ __forceinline__ float sigmoidf_(float r) { return 1.0f / (1.0f + expf(-r)); }
 
 // g_v = gy * eps / (2 sqrt(v)) at flat NCHW output index o = ((b*N + n)*OHW + pix)
 __device__ __forceinline__ float lrt_gv(const BwdArgs& p, const NoiseKey& k, float gy, size_t o, int b, int n, int pix) {
-    const float e = p.eps_a ? __ldg(p.eps_a + o) : normal1(((uint64_t)b * p.g.OHW + pix) * p.g.N + n, k);
+    const float e = p.eps_a ? __ldg(p.eps_a + o) : normal1(((uint64_t)(b + p.first_image) * p.g.OHW + pix) * p.g.N + n, k);
     return gy * e / (2.0f * __ldg(p.act_std + o));
 }
 

@@ -77,7 +77,10 @@ __device__ __forceinline__ NoiseKey effective_key(NoiseKey k, const unsigned lon
 // bit-identical to S separate launches.  LRT samples differ only in their per-activation noise.  A BBB sample draws a
 // whole weight tensor: the prep writes `sets` = S operand sets (tiles + bias) `set_bytes` apart in the workspace, and a
 // row tile, which never straddles two samples, multiplies by the set of its sample.  LRT: sets = 1.
-struct McFold { int rows; unsigned long long stride; int sets; size_t set_bytes; };
+// first_image: the global index of row 0 (of each sample block when folded) in a batch that is split over calls (row
+// blocks of a sharded MC step): the LRT noise index counts images from there, so a block draws what the whole batch
+// draws at its rows.  It moves the Philox element index only; x, y, eps and workspace indexing stay local.
+struct McFold { int rows; int first_image; unsigned long long stride; int sets; size_t set_bytes; };
 __device__ __forceinline__ NoiseKey sample_key(NoiseKey k, const McFold& f, int j) {
     const unsigned long long s = (((unsigned long long)k.stream_hi << 32) | k.stream_lo) + (unsigned long long)j * f.stride;
     k.stream_lo = (uint32_t)s; k.stream_hi = (uint32_t)(s >> 32);
@@ -90,6 +93,7 @@ __device__ __forceinline__ NoiseKey fold_key(NoiseKey k, const McFold& f, int b,
         b_in_sample = b - j * f.rows;
         k = sample_key(k, f, j);
     }
+    b_in_sample += f.first_image;
     return k;
 }
 // operand set `j` of a BBB fold (j = 0: the set an unfolded call uses)

@@ -23,6 +23,7 @@ struct FwdArgs {
     double* kl_partials; unsigned int* kl_counter;
     float prior_mu, prior_sigma;
     int sample, kl_convention, has_bias, act;
+    int first_image;    // global index of image 0: LRT noise of image b is drawn at image first_image + b (McFold)
 };
 
 __device__ __noinline__ float apply_act(float v, int act) {
@@ -214,8 +215,9 @@ fwd_simt_kernel(const FwdArgs p) {
             if (need_var) {
                 const float var = 1e-16f + (accv[i][j] + bias_v[j]);   // BBB_LRT/BBBConv.py:73-74
                 const float sd = sqrtf(var);
-                // Philox element index of the activation noise: NHWC-flat ((b*OHW + pix)*N + n)
-                const float e = p.eps_a ? __ldg(p.eps_a + o) : normal1(((uint64_t)b * g.OHW + pix) * g.N + n, nkey);
+                // Philox element index of the activation noise: NHWC-flat ((b*OHW + pix)*N + n), b counted from first_image
+                const float e = p.eps_a ? __ldg(p.eps_a + o)
+                                        : normal1(((uint64_t)(b + p.first_image) * g.OHW + pix) * g.N + n, nkey);
                 v = v + sd * e;                                       // BBB_LRT/BBBConv.py:79
                 if (p.act_std) p.act_std[o] = sd;
             }

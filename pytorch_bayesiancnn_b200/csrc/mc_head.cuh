@@ -19,6 +19,9 @@
 //   [4096, ...)                     u64 data[2 slots][world][n_planes * B * C + 2 (+ B with INFO)]
 // Per sending rank: the n_planes [B, C] planes, the KL word at n_planes * B * C, a spare word, and -- only in the INFO
 // instantiation -- a plane of B words behind them: sum over the rank's samples of H[p_hat_s] per image.
+// Row blocks (bbb_mc_exchange_sharded, world = Rs sample groups x Rb row blocks): [2 slots][Rs][...] of the same layout,
+// one sender slot per sample group; rank (g, k) writes the words of its rows [b0, b1) into slot g, the group's block-0
+// rank also the KL word.  Every row of a slot then comes from exactly one rank of its group.
 //
 // INFO (BBB_MC_INFO) adds the two other terms of the entropy decomposition H[p_bar] = E_s H[p_hat_s] + I(y; w):
 //   H[p]                   = -sum_c p_c log p_c, with 0 log 0 = 0 (a class whose probability underflows adds nothing)
@@ -62,6 +65,10 @@ struct McxArgs {
     long long* tl;                // debug timeline slot (nullptr in production)
     long long* trace;             // debug: [CTA][8] %globaltimer stamps of the handshake (nullptr in production)
     float* expected_entropy; float* mutual_info;   // [B] each; nullable; written by the INFO instantiation only
+    // row blocks (the SHARD instantiation only, bbb_mc_exchange_sharded): this rank is row block `block` of sample group
+    // `group` of `groups`; its logits are [S_local, rows, C] for images [row0, row0 + rows); the receive buffer has one
+    // slot per group, which the group's row blocks fill together
+    int groups, group, block, row0, rows;
 };
 
 __host__ __device__ inline int mcx_planes(int want_moments) { return want_moments ? 5 : 2; }
@@ -86,7 +93,10 @@ __device__ __forceinline__ float softplus_f(float v) { return v > 20.0f ? v : lo
 
 // <= 51 registers: an exchange CTA has to fit beside a GEMM CTA (320 x ~120 registers) and a prep CTA of the next step.
 // INFO: also expected_entropy / mutual_info (the extra plane of the receive buffer); INFO == false is the default kernel.
-template <bool INFO>
+// SHARD: row blocks (bbb_mc_exchange_sharded).  The rank pushes the partials of ITS rows into slot `group` of every peer
+// (the group's block-0 rank also its KL word), and every rank finishes all B rows from the `groups` slots, in ascending
+// group order -- with groups == world and one block per group that is exactly the default kernel's work.
+template <bool INFO, bool SHARD = false>
 __global__ void __launch_bounds__(MCX_THREADS, 5)
 mc_exchange_kernel(const McxArgs p) {
     // per warp: log-sum-exp (or softplus sum) of each local sample's row -- dynamic, 32 * S_local bytes: next to a 193 KB
@@ -108,7 +118,17 @@ mc_exchange_kernel(const McxArgs p) {
     __syncthreads();
     const unsigned int seq = seq_sh;
     const size_t rank_floats = mcx_rank_floats(B, C, p.want_moments, INFO);
-    const size_t slot_off = (size_t)(seq & 1u) * p.world * rank_floats;     // in words, behind the control block
+    // senders of one launch: ranks, or sample groups in row-block mode; this rank's partials go to sender slot `src`
+    auto nsrc = [&] { return SHARD ? p.groups : p.world; };
+    auto src = [&] { return SHARD ? p.group : p.rank; };
+    // the images [pb0, pb1) this CTA reduces and pushes: the images it finishes, unless the rank holds a row block
+    const int nrows = SHARD ? p.rows : B, rowoff = SHARD ? p.row0 : 0;
+    int pb0 = b0, pb1 = b1;
+    if constexpr (SHARD) {
+        const int rpc = (nrows + gridDim.x - 1) / gridDim.x;
+        pb0 = rowoff + blockIdx.x * rpc; pb1 = min(rowoff + nrows, pb0 + rpc);
+    }
+    const size_t slot_off = (size_t)(seq & 1u) * nsrc() * rank_floats;        // in words, behind the control block
     const float inv_S = 1.0f / (float)p.S_total;
 
     const unsigned long long* rx = reinterpret_cast<const unsigned long long*>(p.peer[p.rank] + MCX_CTRL_BYTES) + slot_off;
@@ -165,9 +185,10 @@ mc_exchange_kernel(const McxArgs p) {
     };
 
     // ---- (1) local partials of this CTA's images, pushed to every rank's receive buffer ---------------------
-    for (int b = b0 + warp; b < b1; b += nwarp) {
+    for (int b = pb0 + warp; b < pb1; b += nwarp) {
+        const int bl = b - rowoff;                               // local row of image b
         for (int s = 0; s < p.S_local; ++s) {                   // row normaliser of every local sample
-            const float* row = p.logits + ((size_t)s * B + b) * C;
+            const float* row = p.logits + ((size_t)s * nrows + bl) * C;
             float r;
             if (p.normalized) {
                 float acc = 0.0f;
@@ -190,7 +211,7 @@ mc_exchange_kernel(const McxArgs p) {
         for (int c = lane; c < C; c += 32) {
             float mx = -INFINITY, acc = 0.0f, sp = 0.0f, sp2 = 0.0f, sl = 0.0f;
             for (int s = 0; s < p.S_local; ++s) {
-                const float l = p.logits[((size_t)s * B + b) * C + c];
+                const float l = p.logits[((size_t)s * nrows + bl) * C + c];
                 float pr, lp;
                 if (p.normalized) { pr = softplus_f(l) / norm_dyn[warp * p.S_local + s]; lp = logf(pr); }
                 else { lp = l - norm_dyn[warp * p.S_local + s]; pr = expf(lp); }            // log_softmax (main_bayesian.py:49)
@@ -202,7 +223,7 @@ mc_exchange_kernel(const McxArgs p) {
             const size_t e = (size_t)b * C + c;
             if (solo) { fin_elem(rf, e, c, mx, acc, sp, sp2, sl); continue; }
             for (int q = 0; q < p.world; ++q) {
-                unsigned long long* dst = reinterpret_cast<unsigned long long*>(p.peer[q] + MCX_CTRL_BYTES) + slot_off + (size_t)p.rank * rank_floats;
+                unsigned long long* dst = reinterpret_cast<unsigned long long*>(p.peer[q] + MCX_CTRL_BYTES) + slot_off + (size_t)src() * rank_floats;
                 st_ll(dst + e, mx, seq); st_ll(dst + BC + e, acc, seq);
                 if (p.want_moments) { st_ll(dst + 2 * (size_t)BC + e, sp, seq); st_ll(dst + 3 * (size_t)BC + e, sp2, seq); st_ll(dst + 4 * (size_t)BC + e, sl, seq); }
             }
@@ -211,7 +232,7 @@ mc_exchange_kernel(const McxArgs p) {
         if constexpr (INFO) {
             hloc = warp_sum(hl);
             if (!solo && lane < p.world)                         // a rank without samples pushes 0
-                st_ll(reinterpret_cast<unsigned long long*>(p.peer[lane] + MCX_CTRL_BYTES) + slot_off + (size_t)p.rank * rank_floats +
+                st_ll(reinterpret_cast<unsigned long long*>(p.peer[lane] + MCX_CTRL_BYTES) + slot_off + (size_t)src() * rank_floats +
                           mcx_info_off(B, C, p.want_moments) + b, hloc, seq);
         }
         if (solo) fin_row(rf, b, hloc);
@@ -222,14 +243,15 @@ mc_exchange_kernel(const McxArgs p) {
         if (blockIdx.x == 0 && threadIdx.x == 0) for (int i = 0; p.kl && i < p.n_kl; ++i) kl_solo += __ldg(p.kl + i);
         kl_solo *= (float)p.S_local;
     } else {
-        if (blockIdx.x == 0 && threadIdx.x < p.world) {             // this rank's KL contribution: S_local * kl
-            unsigned long long* dst = reinterpret_cast<unsigned long long*>(p.peer[threadIdx.x] + MCX_CTRL_BYTES) + slot_off + (size_t)p.rank * rank_floats;
+        // this rank's KL contribution: S_local * kl (row blocks: the group's block-0 rank, so each group counts once)
+        if (blockIdx.x == 0 && threadIdx.x < p.world && (!SHARD || p.block == 0)) {
+            unsigned long long* dst = reinterpret_cast<unsigned long long*>(p.peer[threadIdx.x] + MCX_CTRL_BYTES) + slot_off + (size_t)src() * rank_floats;
             float one = 0.0f;
             for (int i = 0; p.kl && i < p.n_kl; ++i) one += __ldg(p.kl + i);
             st_ll(dst + (size_t)mcx_planes(p.want_moments) * BC, (float)p.S_local * one, seq);
         }
         if (tracer) tr[1] = (long long)globaltimer_ns();
-        // ---- (4) finish: fixed rank order => bitwise identical on every rank ----------------------------------
+        // ---- (4) finish: fixed rank (row blocks: group) order => bitwise identical on every rank --------------
         for (int b = b0 + warp; b < b1; b += nwarp) {
             RowFin rf{-INFINITY, 0x7fffffff, 0.0f, 0.0f, p.labels ? p.labels[b] : -1};
             for (int c = lane; c < C; c += 32) {
@@ -237,17 +259,17 @@ mc_exchange_kernel(const McxArgs p) {
                 // the words of this element from up to 8 ranks in flight at once (one L2 round trip), stragglers polled;
                 // ranks merged in ascending order with the online logsumexp update: same operations on every rank
                 float M = -INFINITY, tot = 0.0f, mom[3] = {0.0f, 0.0f, 0.0f};
-                for (int q0 = 0; q0 < p.world; q0 += 8) {
+                for (int q0 = 0; q0 < nsrc(); q0 += 8) {
                     unsigned long long wm[8], wa[8];
 #pragma unroll
                     for (int j = 0; j < 8; ++j) {
-                        if (q0 + j >= p.world) continue;
+                        if (q0 + j >= nsrc()) continue;
                         const unsigned long long* r = rx + (size_t)(q0 + j) * rank_floats + e;
                         wm[j] = ld_ll(r); wa[j] = ld_ll(r + BC);
                     }
 #pragma unroll
                     for (int j = 0; j < 8; ++j) {
-                        if (q0 + j >= p.world) continue;
+                        if (q0 + j >= nsrc()) continue;
                         const unsigned long long* r = rx + (size_t)(q0 + j) * rank_floats + e;
                         const float mq = ll_value(wm[j], r), aq = ll_value(wa[j], r + BC);
                         if (aq > 0.0f) {
@@ -259,14 +281,14 @@ mc_exchange_kernel(const McxArgs p) {
                 if (p.want_moments) {
 #pragma unroll
                     for (int pl = 0; pl < 3; ++pl)
-                        for (int q0 = 0; q0 < p.world; q0 += 8) {
+                        for (int q0 = 0; q0 < nsrc(); q0 += 8) {
                             unsigned long long w[8];
 #pragma unroll
                             for (int j = 0; j < 8; ++j)
-                                if (q0 + j < p.world) w[j] = ld_ll(rx + (size_t)(q0 + j) * rank_floats + (size_t)(2 + pl) * BC + e);
+                                if (q0 + j < nsrc()) w[j] = ld_ll(rx + (size_t)(q0 + j) * rank_floats + (size_t)(2 + pl) * BC + e);
 #pragma unroll
                             for (int j = 0; j < 8; ++j)
-                                if (q0 + j < p.world) mom[pl] += ll_value(w[j], rx + (size_t)(q0 + j) * rank_floats + (size_t)(2 + pl) * BC + e);
+                                if (q0 + j < nsrc()) mom[pl] += ll_value(w[j], rx + (size_t)(q0 + j) * rank_floats + (size_t)(2 + pl) * BC + e);
                         }
                 }
                 const float sp = mom[0], sp2 = mom[1], sl = mom[2];
@@ -275,11 +297,11 @@ mc_exchange_kernel(const McxArgs p) {
             float hsum = 0.0f;
             if constexpr (INFO) {       // lane q fetches rank q's word (one round trip); every lane adds them in rank order
                 float hq = 0.0f;
-                if (lane < p.world) {
+                if (lane < nsrc()) {
                     const unsigned long long* w = rx + (size_t)lane * rank_floats + mcx_info_off(B, C, p.want_moments) + b;
                     hq = ll_value(ld_ll(w), w);
                 }
-                for (int q = 0; q < p.world; ++q) hsum += __shfl_sync(0xffffffffu, hq, q);
+                for (int q = 0; q < nsrc(); ++q) hsum += __shfl_sync(0xffffffffu, hq, q);
             }
             fin_row(rf, b, hsum);
         }
@@ -315,7 +337,7 @@ mc_exchange_kernel(const McxArgs p) {
                 for (int i = 0; p.kl && i < p.n_kl; ++i) klsum += __ldg(p.kl + i);
                 klsum *= (float)p.S_local;
             } else {
-                for (int q = 0; q < p.world; ++q) { const unsigned long long* w = rx + (size_t)q * rank_floats + (size_t)mcx_planes(p.want_moments) * BC; klsum += ll_value(ld_ll(w), w); }
+                for (int q = 0; q < nsrc(); ++q) { const unsigned long long* w = rx + (size_t)q * rank_floats + (size_t)mcx_planes(p.want_moments) * BC; klsum += ll_value(ld_ll(w), w); }
             }
             const float kl = klsum * inv_S;                               // main_bayesian.py:51  (kl / num_ens)
             if (p.kl_out) *p.kl_out = kl;

@@ -54,6 +54,7 @@ class _Noise(threading.local):
         self.queue = None          # external-eps queue (parity mode)
         self.base = None           # device int64[1] stream base (CUDA-graph capture mode)
         self.fold = None           # (rows per MC sample, Philox stream stride) of layer_fold
+        self.first_image = 0       # global index of image 0 of the layer calls (first_image)
 
     def current_seed(self) -> int:
         if not self.explicit:
@@ -134,6 +135,35 @@ def layer_fold(rows: int, stride: int):
         yield
     finally:
         _noise.fold = prev
+
+
+@contextlib.contextmanager
+def first_image(b0: int):
+    """Layer calls inside hold images [b0, b0 + batch) of a larger batch (a row block of a sharded Monte-Carlo step,
+    mc.MCForward(batch_shards=...)): the LRT activation noise of image b is drawn at image b0 + b, so a block's outputs
+    equal the whole batch's outputs at its rows bit for bit -- on every forward path and the backward.  BBB weight noise
+    does not depend on rows.  Only the Philox element index moves (include/bbb_b200.h, desc->reserved[0])."""
+    b0 = int(b0)
+    if not 0 <= b0 <= FIRST_IMAGE_MAX:
+        raise L.EngineError(f"first_image: {b0} is outside [0, {FIRST_IMAGE_MAX}]")
+    prev = _noise.first_image
+    _noise.first_image = b0
+    try:
+        yield
+    finally:
+        _noise.first_image = prev
+
+
+def current_first_image() -> int:
+    return _noise.first_image
+
+
+FIRST_IMAGE_MAX = (1 << 23) - 1       # bits 8..30 of desc->reserved[0]
+
+
+def first_image_word(b0: int) -> int:
+    """desc->reserved[0] bits of first image b0 (an int32; a value the engine refuses when b0 is out of range)."""
+    return C.c_int32((int(b0) << 8) & 0xFFFFFFFF).value if 0 <= int(b0) <= FIRST_IMAGE_MAX else -1
 
 
 def layer_fold_active() -> bool:
@@ -259,8 +289,9 @@ def workspace(device, desc=None, owner=None) -> torch.Tensor:
 
 def make_desc(x_shape, w_shape, conv, variant, sample, has_bias, prior_mu, prior_sigma,
               math=L.MATH_FP32, kl_convention=L.KL_REFERENCE, act=L.ACT_NONE,
-              act_dtype=L.DTYPE_F32, fold=None) -> L.LayerDesc:
-    """``fold`` = (rows per MC sample, Philox stream stride): the desc folds MC samples into its batch (layer_fold)."""
+              act_dtype=L.DTYPE_F32, fold=None, first_image: int = 0) -> L.LayerDesc:
+    """``fold`` = (rows per MC sample, Philox stream stride): the desc folds MC samples into its batch (layer_fold).
+    ``first_image``: global index of image 0 (of each sample block when folded), in reserved[0] bits 8..30."""
     d = L.LayerDesc()
     if conv is None:
         d.batch, d.in_channels, d.in_h, d.in_w = x_shape[0], x_shape[1], 1, 1
@@ -281,6 +312,8 @@ def make_desc(x_shape, w_shape, conv, variant, sample, has_bias, prior_mu, prior
         d.reserved[1] = int(rows)
         d.reserved[2] = C.c_int32(stride & 0xFFFFFFFF).value
         d.reserved[3] = C.c_int32((stride >> 32) & 0xFFFFFFFF).value
+    if first_image:
+        d.reserved[0] = first_image_word(first_image)
     return d
 
 
@@ -391,7 +424,8 @@ class BayesLayerFn(torch.autograd.Function):
         if fold is not None and external_eps_active():
             raise L.EngineError("layer_fold: MC-sample folding draws its noise in-kernel (no external eps)")
         d = make_desc(tuple(x.shape), tuple(W_mu.shape), conv, variant, sample, has_bias,
-                      cfg["prior_mu"], cfg["prior_sigma"], cfg["math"], cfg["kl_convention"], cfg["act"], fold=fold)
+                      cfg["prior_mu"], cfg["prior_sigma"], cfg["math"], cfg["kl_convention"], cfg["act"], fold=fold,
+                      first_image=_noise.first_image)
         if conv is None:
             if x.dim() != 2 or x.shape[1] != W_mu.shape[1]:
                 raise L.EngineError(f"linear: x {tuple(x.shape)} vs weight {tuple(W_mu.shape)}")
@@ -429,6 +463,7 @@ class BayesLayerFn(torch.autograd.Function):
         ctx.cfg = cfg
         ctx.desc = d
         ctx.noise = (seed, stream_id, base)
+        ctx.first_image = _noise.first_image
         ctx.has_bias = has_bias
         ctx.save_for_backward(x, W_mu_c, W_rho_c, bias_mu, bias_rho, act_std, eps_a, eps_b)
         return y, kl
@@ -514,7 +549,8 @@ class BayesLayerFn(torch.autograd.Function):
             gw_mu = _tc_wgrad(x, gy, conv, W_mu.shape)
             if sample:
                 if eps_a is None:
-                    z = philox_normal(gy.numel(), seed, stream_id, 0, device=dev)
+                    # element index of image b is counted from the call's first image, as in the forward
+                    z = philox_normal(gy.numel(), seed, stream_id, ctx.first_image * (gy.numel() // gy.shape[0]), device=dev)
                     eps = z.view(gy.shape) if conv is None else z.view(gy.shape[0], gy.shape[2], gy.shape[3], gy.shape[1]).permute(0, 3, 1, 2)
                 else:
                     eps = eps_a

@@ -153,7 +153,7 @@ def _step_desc(st, phase, fold=None):
     d.kl_convention = L.KL_BY_NAME[m.kl_convention]
     d.epilogue_act = st.act
     d.pool_k = d.pool_s = 2 if st.pool else 0
-    d.reserved[0] = phase
+    d.reserved[0] = phase | (Fn.first_image_word(Fn.current_first_image()) if Fn.current_first_image() else 0)
     if fold is not None:                    # MC samples folded into the batch (include/bbb_b200.h)
         rows, stride = fold
         d.reserved[1] = int(rows)

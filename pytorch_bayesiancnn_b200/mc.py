@@ -33,6 +33,24 @@ def local_samples(num_ens: int, world: int, rank: int):
     return list(range(rank, num_ens, world))
 
 
+def row_block(B: int, batch_shards: int, block: int):
+    """Images [b0, b1) of row block `block` of `batch_shards`: blocks as equal as possible, the first B % batch_shards one
+    image longer (include/bbb_b200.h, bbb_mc_exchange_sharded)."""
+    q, r = divmod(int(B), int(batch_shards))
+    b0 = block * q + min(block, r)
+    return b0, b0 + q + (1 if block < r else 0)
+
+
+def shard_layout(world: int, rank: int, batch_shards: int = 1):
+    """(sample_shards Rs, sample group g, row block k) of `rank` when `world` = Rs x batch_shards ranks split the samples
+    into Rs groups and the batch into batch_shards row blocks: g = rank % Rs, k = rank // Rs."""
+    rb = int(batch_shards)
+    if rb < 1 or world % rb:
+        raise L.EngineError(f"batch_shards={rb}: the world size {world} must be a multiple of it")
+    rs = world // rb
+    return rs, rank % rs, rank // rs
+
+
 def get_beta(batch_idx, m, beta_type, epoch=None, num_epochs=None):
     """metrics.py:32-46 (host scalar; it only feeds the `beta` argument of the ELBO head)."""
     if isinstance(beta_type, (int, float)):
@@ -128,13 +146,20 @@ class MCForward:
       and entropy [B]; with ``with_labels`` head = [loss, nll, accuracy, beta*kl] (metrics.py:12-14, 23-24); with
       ``want_information`` (needs ``want_uncertainty``) expected_entropy = mean_s H[p_hat_s] and mutual_info = entropy -
       expected_entropy [B] (include/bbb_b200.h, bbb_mc_exchange_info).
+
+    ``batch_shards=Rb`` splits the batch as well as the samples: world = Rs x Rb ranks, rank r is sample group
+    g = r % Rs (samples local_samples(num_ens, Rs, g)) and row block k = r // Rs (images ``rows`` = [b0, b1), row_block).
+    Every rank is given the full x (and labels) and runs its samples on its rows only, with the LRT noise of image b drawn
+    at b (Fn.first_image): the per-sample logits do not depend on (Rs, Rb), and every rank returns the same full
+    outputs (bbb_mc_exchange_sharded).  Rb = 1 (default) is the sample-only split.
     """
 
     def __init__(self, net, example_x: torch.Tensor, num_ens: int, group=None, want_uncertainty: bool = False,
                  normalized: bool = False, with_labels: bool = False, train_size: float = 1.0, beta: float = 0.0,
                  seed: Optional[int] = None, graph: bool = True, num_classes: Optional[int] = None,
                  static_inputs=None, first_replay: int = 0, fold: bool = True, overlap: bool = False, inflight: int = 1,
-                 fold_group: Optional[int] = None, fold_budget: int = LAYER_FOLD_BUDGET, want_information: bool = False):
+                 fold_group: Optional[int] = None, fold_budget: int = LAYER_FOLD_BUDGET, want_information: bool = False,
+                 batch_shards: int = 1):
         """``static_inputs``: device tensors the caller fills in place (e.g. targets of its host->device copies, or a
         rotation of resident batches); one graph is captured per tensor and ``self(slot=k)`` runs the step on
         ``static_inputs[k]`` with no staging copy.  ``first_replay``: index of the first replay's noise block.
@@ -157,8 +182,14 @@ class MCForward:
             raise L.EngineError("MCForward: at most 16 ranks (one node)")
         dev = self.dev = example_x.device
         self.num_ens = int(num_ens)
-        self.ids = local_samples(self.num_ens, self.world, self.rank)
+        self.sample_shards, self.group_index, self.block = shard_layout(self.world, self.rank, batch_shards)
+        self.batch_shards = int(batch_shards)
+        self.ids = local_samples(self.num_ens, self.sample_shards, self.group_index)
         self.B = int(example_x.shape[0])
+        if self.batch_shards > self.B:
+            raise L.EngineError(f"MCForward: batch_shards={self.batch_shards} > batch {self.B} (a row block would be empty)")
+        self.rows = row_block(self.B, self.batch_shards, self.block)     # this rank's images [b0, b1)
+        self.nb = self.rows[1] - self.rows[0]
         self.C = int(num_classes if num_classes is not None else net.num_classes)
         self.flags = (L.MC_MOMENTS if want_uncertainty else 0) | (L.MC_NORMALIZED if normalized else 0) | \
             (L.MC_INFO if want_information else 0)
@@ -183,7 +214,7 @@ class MCForward:
         nbuf = self.nbuf
         self.labels_all = torch.zeros(nbuf, B, dtype=torch.int64, device=dev) if with_labels else None
         self.labels = self.labels_all[0] if with_labels else None
-        self.logits_all = torch.zeros(nbuf, max(1, len(self.ids)), B, Cc, **f32)
+        self.logits_all = torch.zeros(nbuf, max(1, len(self.ids)), self.nb, Cc, **f32)
         self.logits = self.logits_all[0]
         self.kl_one_all = torch.zeros(nbuf, **f32)
         self.kl_one = self.kl_one_all[0]
@@ -199,7 +230,7 @@ class MCForward:
         if with_labels:
             self.out["head"] = torch.empty(4, **f32)
         self.state = torch.zeros(int(lib.bbb_mc_state_bytes()), dtype=torch.uint8, device=dev)
-        nbytes = int(lib.bbb_mc_buffer_bytes(B, Cc, self.flags, self.world))
+        nbytes = int(lib.bbb_mc_buffer_bytes(B, Cc, self.flags, self.sample_shards))   # one slot per sample group
         self._imported, self._own = [], None
         if self.world == 1:
             self._buf = torch.zeros(nbytes, dtype=torch.uint8, device=dev)
@@ -219,9 +250,12 @@ class MCForward:
         kids = list(net.children())
         layers = [m_ for m_ in kids if isinstance(m_, _BayesLayer)]
         one_variant = bool(layers) and len({m_._variant for m_ in layers}) == 1 and getattr(net, "fuse", True)
+        # Row blocks: everything below runs on this rank's nb rows; a group's local samples are g, g + Rs, .. (stream
+        # stride Rs << 40).
         if fold and len(self.ids) > 1 and one_variant:
-            self.fold = (self.B, self.world << 40)
-            self.fold_steps = fused.plan(kids, (len(self.ids) * self.B,) + tuple(example_x.shape[1:]), self.fold)
+            self.fold = (self.nb, self.sample_shards << 40)
+            with Fn.first_image(self.rows[0]):
+                self.fold_steps = fused.plan(kids, (len(self.ids) * self.nb,) + tuple(example_x.shape[1:]), self.fold)
         # Nets the fused chain does not take (BBBLeNet, BBB3Conv3FC) fold on the per-layer path instead: groups of G
         # consecutive local samples, one pass of the tensor-core layer kernels over G x B rows each (Fn.layer_fold), with
         # the aten activations / pools between them -- per-image ops, so every output equals the sample loop's bit for bit.
@@ -233,7 +267,7 @@ class MCForward:
             G = max(n for _, n in self._groups)
             self.layer_fold = (G, len(self._groups))
             # the first layer's input: x repeated G times, one buffer per concurrently running step
-            self.xrep_all = [torch.empty((G * B,) + tuple(example_x.shape[1:]), dtype=example_x.dtype, device=dev)
+            self.xrep_all = [torch.empty((G * self.nb,) + tuple(example_x.shape[1:]), dtype=example_x.dtype, device=dev)
                              for _ in range(nbuf)]
         self.graph, self.graphs = None, []
         self.result_stream = None                 # overlap mode: the stream the results are complete on
@@ -251,7 +285,7 @@ class MCForward:
         from .modules import ModuleWrapper, _default_fuse
         if not kids or type(net).forward is not ModuleWrapper.forward:
             return None
-        shape = tuple(example_x.shape)
+        shape = (self.nb,) + tuple(example_x.shape[1:])
         if getattr(net, "fuse", _default_fuse()) and fused.plan(kids, shape) is not None:
             return None
         chain = _per_image_chain(kids, shape)
@@ -267,7 +301,8 @@ class MCForward:
                 cfg = m._cfg(True)
                 d = Fn.make_desc((n * xs[0],) + tuple(xs[1:]), tuple(m.W_mu.shape), cfg["conv"], cfg["variant"], True,
                                  m.bias_mu is not None, cfg["prior_mu"], cfg["prior_sigma"], cfg["math"],
-                                 cfg["kl_convention"], cfg["act"], fold=(self.B, self.world << 40))
+                                 cfg["kl_convention"], cfg["act"], fold=(self.nb, self.sample_shards << 40),
+                                 first_image=self.rows[0])
                 if lib.bbb_forward_supported(C.byref(d)) != 0:
                     return None
         return groups
@@ -327,7 +362,10 @@ class MCForward:
         logits_buf = self.logits_all[par]
         kl_buf = self.kl_terms_all[par] if self.overlap else None
         inc = _STRIDE * self.inflight
-        with torch.no_grad(), Fn.workspace_slot(par if self.inflight > 1 else Fn.current_workspace_slot()):
+        b0, nb = self.rows[0], self.nb
+        x = x[b0:b0 + nb]                                 # this rank's row block (a view: NCHW rows are contiguous)
+        with torch.no_grad(), Fn.workspace_slot(par if self.inflight > 1 else Fn.current_workspace_slot()), \
+                Fn.first_image(b0):
             # The Philox base moves at the HEAD of a captured step, BEFORE the prep streams fork: with this one-thread
             # kernel as the single root of the graph every GEMM kernel of the chain is launched programmatically behind
             # its predecessor; with the fork in front of it (prep kernels as further root nodes) or with no plain kernel
@@ -337,21 +375,21 @@ class MCForward:
             kl_ptr, n_kl = None, 0
             if self.fold_steps is not None:
                 with Fn.stream_base(base), Fn.mc_sample(self.ids[0], self.seed):
-                    _, kls = fused._run(self.fold_steps, x, True, logits_buf.view(len(self.ids) * self.B, self.C), True, None,
+                    _, kls = fused._run(self.fold_steps, x, True, logits_buf.view(len(self.ids) * nb, self.C), True, None,
                                         fold=self.fold, kls_out=kl_buf)
                 self._kl_terms = kls
                 kl_ptr, n_kl = Fn._ptr(kls), kls.numel()
             if self._groups is not None:
-                # group (s0, n): local samples s0 .. s0+n-1 in one pass over n x B rows; row block k is global sample
-                # ids[s0] + k * world (stream stride world << 40, as in the fused fold) and lands in logits_buf[s0 + k]
+                # group (s0, n): local samples s0 .. s0+n-1 in one pass over n x nb rows; row block k is global sample
+                # ids[s0] + k * Rs (stream stride Rs << 40, as in the fused fold) and lands in logits_buf[s0 + k]
                 xr = self.xrep_all[par]
                 G = self.layer_fold[0]
                 xr.view((G,) + tuple(x.shape)).copy_(x.unsqueeze(0).expand((G,) + tuple(x.shape)))
                 for gi, (s0, n) in enumerate(self._groups):
                     with Fn.stream_base(base), Fn.mc_sample(self.ids[s0], self.seed), \
-                            Fn.layer_fold(self.B, self.world << 40):
-                        logits, kl = self.net(xr[:n * self.B])
-                    logits_buf[s0:s0 + n].view(n * self.B, self.C).copy_(logits.reshape(n * self.B, self.C))
+                            Fn.layer_fold(nb, self.sample_shards << 40):
+                        logits, kl = self.net(xr[:n * nb])
+                    logits_buf[s0:s0 + n].view(n * nb, self.C).copy_(logits.reshape(n * nb, self.C))
                     if gi == 0:                               # every sample has the same KL, computed once per pass
                         one = self.kl_one_all[par:par + 1]
                         one.copy_(torch.as_tensor(kl, dtype=torch.float32, device=self.dev).reshape(1))
@@ -361,7 +399,7 @@ class MCForward:
                         fused.direct_output(logits_buf[k], kl_buf if k == 0 else None) as hook:
                     logits, kl = self.net(x)
                 if not hook.used:
-                    logits_buf[k].copy_(logits.reshape(self.B, self.C))
+                    logits_buf[k].copy_(logits.reshape(nb, self.C))
                 if k == 0:
                     if hook.used:
                         self._kl_terms = kl                       # per-layer scalars of sample 0 (every sample has the same KL)
@@ -370,22 +408,26 @@ class MCForward:
                         one = self.kl_one_all[par:par + 1]
                         one.copy_(torch.as_tensor(kl, dtype=torch.float32, device=self.dev).reshape(1))
                         kl_ptr, n_kl = Fn._ptr(one), 1
-            if not self.ids and self.rank == 0:
-                raise L.EngineError("MCForward: rank 0 must own a sample")
+            if not self.ids and self.group_index == 0:
+                raise L.EngineError("MCForward: sample group 0 must own a sample")
         return kl_ptr, n_kl
 
     def _exchange(self, kl_ptr, n_kl, advance_base=None, par=0):
         """The one kernel behind the samples: combine + exchange + heads (bbb_mc_exchange_info)."""
         from .graph import _STRIDE
         o = self.out
-        rc = L.lib().bbb_mc_exchange_info(
+        lib = L.lib()
+        args = (
             Fn._ptr(self.logits_all[par]), len(self.ids), self.num_ens, self.B, self.C, kl_ptr, n_kl, self.flags,
             Fn._ptr(self.labels_all[par] if self.labels_all is not None else None), C.c_float(self.train_size), C.c_float(self.beta), self.rank, self.world, self.peers,
             Fn._ptr(self.state), Fn._ptr(o["log_outputs"]), Fn._ptr(o["kl"]), Fn._ptr(o.get("pred")),
             Fn._ptr(o.get("epistemic")), Fn._ptr(o.get("aleatoric")), Fn._ptr(o.get("entropy")), Fn._ptr(o.get("head")),
             Fn._ptr(advance_base), C.c_uint64(_STRIDE if advance_base is not None else 0),
-            Fn._ptr(o.get("expected_entropy")), Fn._ptr(o.get("mutual_info")), Fn._stream(self.dev))
-        L.check(rc, "bbb_mc_exchange_info")
+            Fn._ptr(o.get("expected_entropy")), Fn._ptr(o.get("mutual_info")))
+        if self.batch_shards == 1:
+            L.check(lib.bbb_mc_exchange_info(*args, Fn._stream(self.dev)), "bbb_mc_exchange_info")
+        else:
+            L.check(lib.bbb_mc_exchange_sharded(*args, self.batch_shards, Fn._stream(self.dev)), "bbb_mc_exchange_sharded")
 
     def _capture(self, warmup: int = 2):
         from .graph import _STRIDE
@@ -520,93 +562,118 @@ class MCForward:
 
 
 def _generic_mc_forward(forward_fn: Callable, x: torch.Tensor, num_ens: int, group=None, want_uncertainty: bool = False,
-                        information: bool = False):
+                        information: bool = False, batch_shards: int = 1):
     """Backend-agnostic restatement (any device, any torch.distributed backend): the exact (max, sum-exp) partials of
     logmeanexp per rank and ONE all-gather; returns (log_outputs, kl[, (pred, epistemic, aleatoric, entropy)]) --
     with ``information`` the tuple also holds expected_entropy and mutual_info (each rank's sum of H[p_hat_s] over its
-    samples travels as one more [B] plane of the same all-gather)."""
+    samples travels as one more [B] plane of the same all-gather).  ``batch_shards``: as MCForward -- rank (g, k) calls
+    ``forward_fn`` on its row block x[b0:b1] (under Fn.first_image(b0)), the groups are merged in ascending order and
+    each group's KL is counted once (block 0)."""
     dist, world, rank = _dist_info(group)
-    ids = local_samples(num_ens, world, rank)
+    rs, g, k = shard_layout(world, rank, batch_shards)
+    rb = world // rs
+    B = int(x.shape[0])
+    if rb > B:
+        raise L.EngineError(f"mc_forward: batch_shards={rb} > batch {B} (a row block would be empty)")
+    b0, b1 = row_block(B, rb, k)
+    ids = local_samples(num_ens, rs, g)
     parts, shape, dev = None, None, x.device
-    for j in ids:
-        logits, kl = forward_fn(x, j)
-        logits = logits.float()
-        shape, dev = logits.shape, logits.device
-        lsm = torch.log_softmax(logits, dim=1)
-        p = lsm.exp()
-        klv = torch.as_tensor(kl, dtype=torch.float32, device=dev).reshape(1)
-        if information:
-            h = -torch.where(p > 0, p * lsm, torch.zeros_like(p)).sum(1)   # H[p_hat_j], 0 log 0 = 0
-        if parts is None:
-            parts = [lsm.clone(), torch.ones_like(lsm), p.clone(), p * p, logits.clone(), klv.clone()]
+    with Fn.first_image(b0):
+        for j in ids:
+            logits, kl = forward_fn(x[b0:b1], j)
+            logits = logits.float()
+            shape, dev = logits.shape, logits.device
+            lsm = torch.log_softmax(logits, dim=1)
+            p = lsm.exp()
+            klv = torch.as_tensor(kl, dtype=torch.float32, device=dev).reshape(1)
             if information:
-                parts.append(h)
-        else:
-            m = torch.maximum(parts[0], lsm)
-            parts[1] = parts[1] * (parts[0] - m).exp() + (lsm - m).exp()
-            parts[0] = m
-            parts[2] += p; parts[3] += p * p; parts[4] += logits; parts[5] += klv
-            if information:
-                parts[6] += h
+                h = -torch.where(p > 0, p * lsm, torch.zeros_like(p)).sum(1)   # H[p_hat_j], 0 log 0 = 0
+            if parts is None:
+                parts = [lsm.clone(), torch.ones_like(lsm), p.clone(), p * p, logits.clone(), klv.clone()]
+                if information:
+                    parts.append(h)
+            else:
+                m = torch.maximum(parts[0], lsm)
+                parts[1] = parts[1] * (parts[0] - m).exp() + (lsm - m).exp()
+                parts[0] = m
+                parts[2] += p; parts[3] += p * p; parts[4] += logits; parts[5] += klv
+                if information:
+                    parts[6] += h
     if world > 1:
-        meta = [tuple(shape) if shape is not None else None]
         metas = [None] * world
-        dist.all_gather_object(metas, meta[0], group=group)
-        shape = next(s for s in metas if s is not None)
-    n = shape[0] * shape[1]
-    if parts is None:                                 # a rank with no sample (num_ens < world) still joins the collective
+        dist.all_gather_object(metas, tuple(shape) if shape is not None else None, group=group)
+        ncls = next(s_[1] for s_ in metas if s_ is not None)
+    else:
+        ncls = shape[1]
+    nb, P = b1 - b0, -(-B // rb)                      # rows of this block; rows of the longest block
+    shape = (nb, ncls)
+    if parts is None:                                 # a rank with no sample (num_ens < Rs) still joins the collective
         z = torch.zeros(shape, dtype=torch.float32, device=dev)
         parts = [torch.full(shape, -float("inf"), device=dev), z, z.clone(), z.clone(), z.clone(), torch.zeros(1, device=dev)]
         if information:
             parts.append(torch.zeros(shape[0], device=dev))
+    if nb < P:                                        # ragged blocks: every rank sends the longest block's size
+        pad = lambda t: torch.cat([t, t.new_zeros((P - nb,) + tuple(t.shape[1:]))])
+        parts = [t if i == 5 else pad(t) for i, t in enumerate(parts)]
     vec = torch.cat([t.reshape(-1) for t in parts])
     if world > 1:
         allv = [torch.empty_like(vec) for _ in range(world)]
         dist.all_gather(allv, vec, group=group)       # the ONE collective of the forward path
     else:
         allv = [vec]
+    n, full = P * ncls, (B, ncls)
+
+    def plane(i, width=ncls, off=None):
+        """[Rs] list of plane i of every sample group over all B rows (rank r fills rows row_block(.., r // Rs))."""
+        off = i * n if off is None else off
+        out = [torch.empty((B, width) if width > 1 else (B,), dtype=vec.dtype, device=vec.device) for _ in range(rs)]
+        for r, v in enumerate(allv):
+            c0, c1 = row_block(B, rb, r // rs)
+            out[r % rs][c0:c1] = v[off:off + (c1 - c0) * width].view(out[r % rs][c0:c1].shape)
+        return out
     S = float(num_ens)
-    ms = torch.stack([v[:n] for v in allv])
-    as_ = torch.stack([v[n:2 * n] for v in allv])
+    ms = torch.stack(plane(0))
+    as_ = torch.stack(plane(1))
     M = ms.max(0).values
     tot = (as_ * torch.where(as_ > 0, (ms - M).exp(), torch.zeros_like(ms))).sum(0)
-    log_outputs = (M + torch.log(tot / S)).view(shape)         # == logmeanexp_j log_softmax_j (utils.py:14-22), finite
-    kl = sum(v[5 * n] for v in allv) / S                      # main_bayesian.py:51
+    log_outputs = (M + torch.log(tot / S)).view(full)          # == logmeanexp_j log_softmax_j (utils.py:14-22), finite
+    kl = sum(v[5 * n] for r, v in enumerate(allv) if r // rs == 0) / S      # main_bayesian.py:51; one block per group
     if not want_uncertainty:
         return log_outputs, kl
-    p_bar = (sum(v[2 * n:3 * n] for v in allv) / S).view(shape)
-    p2 = (sum(v[3 * n:4 * n] for v in allv) / S).view(shape)
-    pred = (sum(v[4 * n:5 * n] for v in allv) / S).view(shape)
+    p_bar = (sum(plane(2)) / S).view(full)
+    p2 = (sum(plane(3)) / S).view(full)
+    pred = (sum(plane(4)) / S).view(full)
     epistemic = p2 - p_bar * p_bar                    # diag((p-pbar)^T (p-pbar))/T  (uncertainty_estimation.py:89-91)
     aleatoric = p_bar - p2                            # diag(diag(pbar) - p^T p / T)  (:94-95)
     entropy = -(p_bar * torch.log(p_bar.clamp_min(1e-38))).sum(1)      # H[pbar]; no reference (SURVEY D3)
     if not information:
         return log_outputs, kl, (pred, epistemic, aleatoric, entropy)
-    expected_entropy = sum(v[5 * n + 1:5 * n + 1 + shape[0]] for v in allv) / S      # E_j H[p_hat_j], rank order
+    expected_entropy = sum(plane(6, 1, 5 * n + 1)) / S      # E_j H[p_hat_j], group order
     return log_outputs, kl, (pred, epistemic, aleatoric, entropy, expected_entropy, entropy - expected_entropy)
 
 
 def mc_forward(net_or_fn, x: torch.Tensor, num_ens: int, group=None, want_uncertainty: bool = False,
                normalized: bool = False, labels: Optional[torch.Tensor] = None, train_size: float = 1.0,
-               beta: float = 0.0, seed: Optional[int] = None, information: bool = False):
+               beta: float = 0.0, seed: Optional[int] = None, information: bool = False, batch_shards: int = 1):
     """(log_outputs [B,C], kl) like main_bayesian.py:46-53 -- plus (pred, epistemic, aleatoric, entropy) like
     uncertainty_estimation.py:70-96 with ``want_uncertainty`` and the ELBO head [loss, nll, acc, beta*kl] when
     ``labels`` are given.  ``information`` (needs ``want_uncertainty``) extends that tuple to (pred, epistemic, aleatoric,
     entropy, expected_entropy, mutual_info).  ``net_or_fn``: a net built on the engine with CUDA input -> the device path
     (MCForward, cached on the net per shape/options); any ``forward_fn(x, sample_id) -> (logits, kl)`` -> the generic
-    path."""
+    path.  ``batch_shards``: split the batch into that many row blocks as well (MCForward); 1 = samples only."""
     from .modules import ModuleWrapper
     if information and not want_uncertainty:
         raise L.EngineError("mc_forward: information needs want_uncertainty")
     if isinstance(net_or_fn, ModuleWrapper) and x.is_cuda:
         net = net_or_fn
         key = (tuple(x.shape), int(num_ens), bool(want_uncertainty), bool(normalized), labels is not None,
-               float(train_size), float(beta), seed, id(group), bool(information))
+               float(train_size), float(beta), seed, id(group), bool(information), int(batch_shards))
         cache = net.__dict__.setdefault("_mc_engines", {})
         eng = cache.get(key)
         if eng is None:
             eng = cache[key] = MCForward(net, x, num_ens, group, want_uncertainty, normalized, labels is not None,
-                                         train_size, beta, seed, want_information=information)
+                                         train_size, beta, seed, want_information=information,
+                                         batch_shards=batch_shards)
         out = eng(x, labels)
         res = [out["log_outputs"], out["kl"]]
         if want_uncertainty:
@@ -615,7 +682,7 @@ def mc_forward(net_or_fn, x: torch.Tensor, num_ens: int, group=None, want_uncert
         if labels is not None:
             res.append(out["head"])
         return tuple(res)
-    return _generic_mc_forward(net_or_fn, x, num_ens, group, want_uncertainty, information)
+    return _generic_mc_forward(net_or_fn, x, num_ens, group, want_uncertainty, information, batch_shards)
 
 
 def engine_forward_fn(net) -> Callable:
@@ -635,11 +702,16 @@ class MCTrainStep(MCForward):
     -- plus beta/S of its samples' KL terms, and ONE all-reduce sums the parameter gradients (SURVEY.md 8e "Backward
     sharding").  The caller owns the optimizer: ``out = step(x, labels, beta); optimizer.step()``.
 
-    Noise: sample j of step t draws Philox streams 2^63 + (j << 40) + t * 2^20 + layer, so R ranks == 1 rank."""
+    Noise: sample j of step t draws Philox streams 2^63 + (j << 40) + t * 2^20 + layer, so R ranks == 1 rank.
 
-    def __init__(self, net, example_x, num_ens, train_size, group=None, seed=None):
+    ``batch_shards=Rb`` (MCForward): rank (g, k) back-propagates its samples on its row block only -- d loss / d logits
+    keeps the global B (train_size / B) and uses the combined log_outputs rows of the block, the beta/S KL gradient is
+    added by the block-0 rank of each group -- and the same all-reduce sums the gradients.  With num_ens = 1 (the
+    reference's default) and Rb = world this is a data-parallel step."""
+
+    def __init__(self, net, example_x, num_ens, train_size, group=None, seed=None, batch_shards: int = 1):
         super().__init__(net, example_x, num_ens, group=group, with_labels=True, train_size=train_size, seed=seed,
-                         graph=False, fold=False)
+                         graph=False, fold=False, batch_shards=batch_shards)
         self.params = [p for p in net.parameters() if p.requires_grad]
         self.steps = 0
 
@@ -650,12 +722,14 @@ class MCTrainStep(MCForward):
         for p in self.params:
             p.grad = None
         logits, kls = [], []
+        b0, b1 = self.rows
+        xb = x[b0:b1]                                                  # this rank's row block
         for k, j in enumerate(self.ids):
-            with Fn.mc_sample(j, self.seed, offset=self.steps * _STRIDE):
-                lg, kl = self.net(x)                                   # autograd on: per-layer kernels (no fused chain)
+            with Fn.mc_sample(j, self.seed, offset=self.steps * _STRIDE), Fn.first_image(b0):
+                lg, kl = self.net(xb)                                  # autograd on: per-layer kernels (no fused chain)
             logits.append(lg)
             kls.append(kl)
-            self.logits[k].copy_(lg.detach().reshape(self.B, self.C))
+            self.logits[k].copy_(lg.detach().reshape(self.nb, self.C))
         kl_ptr, n_kl = None, 0
         if self.ids:
             self.kl_one.copy_(kls[0].detach())
@@ -664,16 +738,17 @@ class MCTrainStep(MCForward):
         o = self.out
         if self.ids:
             S = float(self.num_ens)
-            idx = self.labels.view(-1, 1)
-            p_bar_y = o["log_outputs"].gather(1, idx).exp()                 # p_bar[b, y_b]
+            idx = self.labels[b0:b1].view(-1, 1)
+            p_bar_y = o["log_outputs"][b0:b1].gather(1, idx).exp()          # p_bar[b, y_b] of the block's rows
             grads = []
             for lg in logits:
                 sm = torch.softmax(lg.detach().float(), dim=1)
                 w = sm.gather(1, idx) / (S * p_bar_y)
                 onehot = torch.zeros_like(sm).scatter_(1, idx, 1.0)
                 grads.append((-(self.train_size / self.B)) * w * (onehot - sm))
-            kl_g = [torch.full_like(k_, self.beta / S) for k_ in kls if torch.is_tensor(k_) and k_.requires_grad]
-            kl_t = [k_ for k_ in kls if torch.is_tensor(k_) and k_.requires_grad]
+            # the KL does not depend on the rows: one block per sample group adds its gradient
+            kl_t = [k_ for k_ in kls if torch.is_tensor(k_) and k_.requires_grad] if self.block == 0 else []
+            kl_g = [torch.full_like(k_, self.beta / S) for k_ in kl_t]
             torch.autograd.backward(logits + kl_t, grads + kl_g)
         if self.world > 1:                                                  # ONE collective: the summed parameter gradients
             for p in self.params:
