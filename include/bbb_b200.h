@@ -308,6 +308,33 @@ int bbb_mc_exchange_sharded(const float* logits, int32_t S_local, int32_t S_tota
                             uint64_t* noise_base, uint64_t noise_inc, float* expected_entropy, float* mutual_info,
                             int32_t batch_shards, void* cuda_stream);
 
+/* bbb_mc_exchange_sharded that also adds the step to an evaluation accumulator: validate_model's two numbers
+ * (main_bayesian.py:65-86) and calibration over a whole held-out set, with no host read per batch.  batch_shards == 1 is
+ * the sample-only split.  Every output of bbb_mc_exchange_sharded is bitwise the same.  Per image b, on the predictive
+ * distribution p_bar = exp(log_outputs[b]) (the mean of the per-sample p_hat_s, softmax or softplus-normalised):
+ *   conf = p_bar[argmax], correct = (argmax == y) (the first maximal class), nll = -log_outputs[b, y],
+ *   brier = sum_c (p_bar_c - [c == y])^2, calibration bin m = clamp(ceil(conf * BBB_MC_CAL_BINS) - 1, 0, BINS - 1):
+ *   BBB_MC_CAL_BINS equal-width bins (m / BINS, (m + 1) / BINS] (Guo et al. 2017).
+ * metrics: device float64 words, bbb_mc_metrics_bytes() in all, zero-filled by the caller before the first step.  Each
+ * launch adds one step (BINS = BBB_MC_CAL_BINS):
+ *   [0] steps   [1] images   [2] sum_steps nll_step   [3] sum_steps acc_step   (the per-batch means of the head, fp64)
+ *   [4] sum_steps klsum_step, klsum = sum_j kl_j over the S_total samples, NOT divided by S_total (validate_model's kl)
+ *   [5] sum nll   [6] sum correct   [7] sum brier                               (over images)
+ *   [8 + m] count   [8 + BINS + m] sum conf   [8 + 2 BINS + m] sum correct      (images of bin m)
+ * The words behind [8 + 3 BINS] are per-launch scratch.  A loss with a per-batch beta_i is (train_size * [2] +
+ * (sum_i beta_i) * [4] / [0]) / [0]: the KL does not depend on the batch.  Sums are taken per warp, per CTA and over the
+ * CTAs in a fixed order, in double precision: the accumulator is bitwise the same on every rank and from run to run.
+ * Launches that share an accumulator must run one after another (e.g. on one stream); engines of different batch sizes
+ * may share one.  metrics == NULL or labels == NULL: BBB_E_INVALID. */
+enum { BBB_MC_CAL_BINS = 15 };
+size_t bbb_mc_metrics_bytes(void);
+int bbb_mc_exchange_metrics(const float* logits, int32_t S_local, int32_t S_total, int32_t B, int32_t C, const float* kl,
+                            int32_t n_kl, int32_t flags, const int64_t* labels, float train_size, float beta,
+                            int32_t rank, int32_t world, void* const* peer_buffers, void* state, float* log_outputs,
+                            float* kl_out, float* pred, float* epistemic, float* aleatoric, float* entropy, float* head,
+                            uint64_t* noise_base, uint64_t noise_inc, float* expected_entropy, float* mutual_info,
+                            int32_t batch_shards, double* metrics, void* cuda_stream);
+
 /* Peer-mapped receive buffers for bbb_mc_exchange (one process per GPU, same node): allocate locally, export a
  * 64-byte CUDA-IPC handle, ship it to the peers by any host channel (the Python side uses torch.distributed),
  * import theirs.  These five calls are the only ones in this library that allocate or synchronise. */

@@ -32,8 +32,10 @@ SYMBOLS = (
     "bbb_mc_combine", "bbb_noise_advance", "bbb_last_error", "bbb_abi_version", "bbb_launch_count",
     "bbb_mc_buffer_bytes", "bbb_mc_state_bytes", "bbb_mc_exchange", "bbb_mc_exchange_info", "bbb_mc_exchange_sharded",
     "bbb_comm_alloc", "bbb_comm_free", "bbb_comm_export", "bbb_comm_import", "bbb_comm_unimport", "bbb_set_wide_tiles",
+    "bbb_mc_metrics_bytes", "bbb_mc_exchange_metrics",
 )
 MC_MOMENTS, MC_NORMALIZED, MC_INFO = 1, 2, 4
+MC_CAL_BINS = 15                 # BBB_MC_CAL_BINS: calibration bins of the evaluation accumulator
 
 
 class LayerDesc(C.Structure):
@@ -92,6 +94,10 @@ def _bind(lib):
     lib.bbb_mc_exchange_info.restype = C.c_int
     lib.bbb_mc_exchange_sharded.argtypes = lib.bbb_mc_exchange_info.argtypes[:-1] + [i32, vp]
     lib.bbb_mc_exchange_sharded.restype = C.c_int
+    lib.bbb_mc_exchange_metrics.argtypes = lib.bbb_mc_exchange_sharded.argtypes[:-1] + [vp, vp]
+    lib.bbb_mc_exchange_metrics.restype = C.c_int
+    lib.bbb_mc_metrics_bytes.argtypes = []
+    lib.bbb_mc_metrics_bytes.restype = sz
     lib.bbb_comm_alloc.argtypes = [sz, C.POINTER(C.c_void_p)]
     lib.bbb_comm_export.argtypes = [vp, vp]
     lib.bbb_comm_import.argtypes = [vp, C.POINTER(C.c_void_p)]

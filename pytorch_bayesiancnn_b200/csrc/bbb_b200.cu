@@ -457,7 +457,7 @@ static int mc_exchange_impl(const float* logits, int32_t S_local, int32_t S_tota
                             int32_t world, void* const* peer_buffers, void* state, float* log_outputs, float* kl_out,
                             float* pred, float* epistemic, float* aleatoric, float* entropy, float* head,
                             uint64_t* noise_base, uint64_t noise_inc, float* expected_entropy, float* mutual_info,
-                            int32_t batch_shards, void* cuda_stream) {
+                            int32_t batch_shards, double* metrics, void* cuda_stream) {
     if (!log_outputs || !peer_buffers || !state) return fail(BBB_E_INVALID, "NULL pointer");
     if (batch_shards < 1 || world % batch_shards) return fail(BBB_E_INVALID, "world %d is not a multiple of batch_shards %d", world, batch_shards);
     if (batch_shards > B) return fail(BBB_E_INVALID, "batch_shards %d > B %d: a row block would be empty", batch_shards, B);
@@ -485,7 +485,7 @@ static int mc_exchange_impl(const float* logits, int32_t S_local, int32_t S_tota
     a.head_partials = (double*)((char*)state + 64);
     a.log_outputs = log_outputs; a.kl_out = kl_out; a.pred = pred; a.epistemic = epistemic; a.aleatoric = aleatoric;
     a.entropy = entropy; a.head = head; a.trace = g_mcx_trace;
-    a.expected_entropy = expected_entropy; a.mutual_info = mutual_info;
+    a.expected_entropy = expected_entropy; a.mutual_info = mutual_info; a.metrics = metrics;
     // row blocks: rank r = sample group r % Rs, row block r / Rs; blocks as equal as possible, the first B % Rb one longer
     const int Rs = world / batch_shards, blk = rank / Rs, per = B / batch_shards, rem = B % batch_shards;
     a.groups = Rs; a.group = rank % Rs; a.block = blk;
@@ -496,9 +496,12 @@ static int mc_exchange_impl(const float* logits, int32_t S_local, int32_t S_tota
     int grid = (B + bbb::MCX_THREADS / 32 - 1) / (bbb::MCX_THREADS / 32);
     if (grid > bbb::MCX_MAX_CTAS) grid = bbb::MCX_MAX_CTAS;
     const bool shard = batch_shards > 1;
-    cudaError_t e = bbb::launch_pdl(shard ? (info ? bbb::mc_exchange_kernel<true, true> : bbb::mc_exchange_kernel<false, true>)
-                                          : (info ? bbb::mc_exchange_kernel<true> : bbb::mc_exchange_kernel<false>),
-                                     dim3(grid), dim3(bbb::MCX_THREADS), (size_t)(bbb::MCX_THREADS / 32) * S_local * sizeof(float),
+    auto kern = metrics ? (shard ? (info ? bbb::mc_exchange_kernel<true, true, true> : bbb::mc_exchange_kernel<false, true, true>)
+                                 : (info ? bbb::mc_exchange_kernel<true, false, true> : bbb::mc_exchange_kernel<false, false, true>))
+                        : shard ? (info ? bbb::mc_exchange_kernel<true, true> : bbb::mc_exchange_kernel<false, true>)
+                                : (info ? bbb::mc_exchange_kernel<true> : bbb::mc_exchange_kernel<false>);
+    cudaError_t e = bbb::launch_pdl(kern,
+                                     dim3(grid), dim3(bbb::MCX_THREADS), bbb::mcx_smem_bytes(S_local, metrics != nullptr),
                                      (cudaStream_t)cuda_stream, a);
     if (e == cudaSuccess) e = cudaGetLastError();
     if (e != cudaSuccess) return cuda_fail(e, "mc_exchange launch");
@@ -512,7 +515,7 @@ int bbb_mc_exchange_info(const float* logits, int32_t S_local, int32_t S_total, 
                          uint64_t noise_inc, float* expected_entropy, float* mutual_info, void* cuda_stream) {
     return mc_exchange_impl(logits, S_local, S_total, B, C, kl, n_kl, flags, labels, train_size, beta, rank, world,
                             peer_buffers, state, log_outputs, kl_out, pred, epistemic, aleatoric, entropy, head, noise_base,
-                            noise_inc, expected_entropy, mutual_info, 1, cuda_stream);
+                            noise_inc, expected_entropy, mutual_info, 1, nullptr, cuda_stream);
 }
 int bbb_mc_exchange_sharded(const float* logits, int32_t S_local, int32_t S_total, int32_t B, int32_t C, const float* kl,
                             int32_t n_kl, int32_t flags, const int64_t* labels, float train_size, float beta, int32_t rank,
@@ -522,7 +525,21 @@ int bbb_mc_exchange_sharded(const float* logits, int32_t S_local, int32_t S_tota
                             int32_t batch_shards, void* cuda_stream) {
     return mc_exchange_impl(logits, S_local, S_total, B, C, kl, n_kl, flags, labels, train_size, beta, rank, world,
                             peer_buffers, state, log_outputs, kl_out, pred, epistemic, aleatoric, entropy, head, noise_base,
-                            noise_inc, expected_entropy, mutual_info, batch_shards, cuda_stream);
+                            noise_inc, expected_entropy, mutual_info, batch_shards, nullptr, cuda_stream);
+}
+static_assert(BBB_MC_CAL_BINS == bbb::MCM_BINS, "calibration bins: header and kernel disagree");
+size_t bbb_mc_metrics_bytes(void) { return bbb::mcm_bytes(); }
+int bbb_mc_exchange_metrics(const float* logits, int32_t S_local, int32_t S_total, int32_t B, int32_t C, const float* kl,
+                            int32_t n_kl, int32_t flags, const int64_t* labels, float train_size, float beta, int32_t rank,
+                            int32_t world, void* const* peer_buffers, void* state, float* log_outputs, float* kl_out,
+                            float* pred, float* epistemic, float* aleatoric, float* entropy, float* head,
+                            uint64_t* noise_base, uint64_t noise_inc, float* expected_entropy, float* mutual_info,
+                            int32_t batch_shards, double* metrics, void* cuda_stream) {
+    if (!metrics) return fail(BBB_E_INVALID, "metrics is NULL");
+    if (!labels) return fail(BBB_E_INVALID, "metrics need labels");
+    return mc_exchange_impl(logits, S_local, S_total, B, C, kl, n_kl, flags, labels, train_size, beta, rank, world,
+                            peer_buffers, state, log_outputs, kl_out, pred, epistemic, aleatoric, entropy, head, noise_base,
+                            noise_inc, expected_entropy, mutual_info, batch_shards, metrics, cuda_stream);
 }
 int bbb_mc_exchange(const float* logits, int32_t S_local, int32_t S_total, int32_t B, int32_t C, const float* kl,
                     int32_t n_kl, int32_t flags, const int64_t* labels, float train_size, float beta, int32_t rank, int32_t world,

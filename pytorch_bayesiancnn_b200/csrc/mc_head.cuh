@@ -69,7 +69,23 @@ struct McxArgs {
     // `group` of `groups`; its logits are [S_local, rows, C] for images [row0, row0 + rows); the receive buffer has one
     // slot per group, which the group's row blocks fill together
     int groups, group, block, row0, rows;
+    double* metrics;              // the METRICS instantiation only (bbb_mc_exchange_metrics): accumulator + per-CTA scratch
 };
+
+// Evaluation accumulator (METRICS, bbb_mc_exchange_metrics), float64 words; every launch adds one step:
+//   [0] steps  [1] images  [2] sum_steps nll_step  [3] sum_steps acc_step  [4] sum_steps klsum_step
+//   [MCM_HEAD + i] = sum over images of part i, i < MCM_PART:
+//     [0] nll  [1] correct  [2] brier  [3 + m] bin count  [3 + BINS + m] bin sum conf  [3 + 2 BINS + m] bin sum correct
+// and behind the first MCM_SCRATCH words the per-CTA partials [MCX_MAX_CTAS][MCM_PART] of the launch.
+constexpr int MCM_BINS = 15, MCM_HEAD = 5, MCM_PART = 3 + 3 * MCM_BINS, MCM_WORDS = MCM_HEAD + MCM_PART, MCM_SCRATCH = 64;
+static_assert(MCM_WORDS <= MCM_SCRATCH, "accumulator overlaps the per-CTA scratch");
+static_assert(MCM_PART % 2 == 0 && MCM_PART / 2 <= 32, "a warp carries two parts per lane");
+__host__ __device__ inline size_t mcm_bytes() { return ((size_t)MCM_SCRATCH + (size_t)MCX_MAX_CTAS * MCM_PART) * sizeof(double); }
+// dynamic shared memory of a launch: the per-warp row normalisers, then (METRICS) the CTA's partials and the last-CTA flag
+// (392 bytes: the exchange CTA has to fit beside a GEMM and a prep CTA of the next step, see mc_exchange_kernel)
+__host__ inline size_t mcx_smem_bytes(int S_local, bool metrics) {
+    return (size_t)(MCX_THREADS / 32) * S_local * sizeof(float) + (metrics ? (size_t)(MCM_PART + 1) * sizeof(double) : 0);
+}
 
 __host__ __device__ inline int mcx_planes(int want_moments) { return want_moments ? 5 : 2; }
 __host__ __device__ inline size_t mcx_info_off(int B, int C, int want_moments) { return (size_t)mcx_planes(want_moments) * B * C + 2; }
@@ -96,7 +112,13 @@ __device__ __forceinline__ float softplus_f(float v) { return v > 20.0f ? v : lo
 // SHARD: row blocks (bbb_mc_exchange_sharded).  The rank pushes the partials of ITS rows into slot `group` of every peer
 // (the group's block-0 rank also its KL word), and every rank finishes all B rows from the `groups` slots, in ascending
 // group order -- with groups == world and one block per group that is exactly the default kernel's work.
-template <bool INFO, bool SHARD = false>
+// METRICS: also add this step to the evaluation accumulator p.metrics (needs labels).  Per image, on p_bar = exp(log_outputs):
+// nll, correct (argmax == label), brier = sum_c (p_bar_c - [c == y])^2 and the calibration bin m = clamp(ceil(conf * 15) - 1,
+// 0, 14) of conf = p_bar[argmax].  A warp keeps its partials in registers, spread over its lanes (lane l holds parts 2l and
+// 2l + 1); the warps add them into the CTA's shared partials in warp order, and the last CTA sums the CTAs in order
+// (double throughout, no float atomics): bitwise the same on every rank and every run.  Takes the cross-CTA finish even
+// with one rank.
+template <bool INFO, bool SHARD = false, bool METRICS = false>
 __global__ void __launch_bounds__(MCX_THREADS, 5)
 mc_exchange_kernel(const McxArgs p) {
     // per warp: log-sum-exp (or softplus sum) of each local sample's row -- dynamic, 32 * S_local bytes: next to a 193 KB
@@ -115,6 +137,9 @@ mc_exchange_kernel(const McxArgs p) {
     long long* tr = p.trace + blockIdx.x * 8;
     if (tracer) tr[0] = (long long)globaltimer_ns();
     if (threadIdx.x == 0) seq_sh = *p.seq + 1u;
+    double* mcm_cta = reinterpret_cast<double*>(norm_dyn + nwarp * p.S_local);     // METRICS: [MCM_PART]
+    if constexpr (METRICS)
+        if (threadIdx.x < MCM_PART) mcm_cta[threadIdx.x] = 0.0;
     __syncthreads();
     const unsigned int seq = seq_sh;
     const size_t rank_floats = mcx_rank_floats(B, C, p.want_moments, INFO);
@@ -133,6 +158,8 @@ mc_exchange_kernel(const McxArgs p) {
 
     const unsigned long long* rx = reinterpret_cast<const unsigned long long*>(p.peer[p.rank] + MCX_CTRL_BYTES) + slot_off;
     const bool solo = p.world == 1;     // one rank: the partials never leave the registers (no buffer round trip, no handshake)
+    // nll and correct count of the head, on lane 0.  METRICS: lane l < MCM_PART / 2 of a warp sums parts 2l and 2l + 1 of
+    // its rows in them (lane 0's are the head's two), so the partials need no registers or shared memory of their own
     double nll_acc = 0.0, hit_acc = 0.0;
     // per-row state of the finish (4): running argmax, entropy, the label's log-probability
     struct RowFin { float best; int best_c; float ent, lab_lp; long long lab; };
@@ -159,6 +186,24 @@ mc_exchange_kernel(const McxArgs p) {
             const float ob = __shfl_xor_sync(0xffffffffu, best, o);
             const int oc = __shfl_xor_sync(0xffffffffu, best_c, o);
             if (ob > best || (ob == best && oc < best_c)) { best = ob; best_c = oc; }
+        }
+        if constexpr (METRICS) {
+            // Brier score from the log_outputs this lane wrote for the row (no extra register state in the class loop);
+            // per element (p - [c == y])^2, never the expanded form, which cancels
+            double br = 0.0;
+            for (int c = lane; c < C; c += 32) {
+                const double d = (double)expf(p.log_outputs[(size_t)b * C + c]) - ((long long)c == rf.lab ? 1.0 : 0.0);
+                br += d * d;
+            }
+            br = warp_sum(br);                      // br, lab_lp, best, best_c: the same on every lane
+            const float conf = expf(best);
+            const int m = min(max((int)ceilf(conf * (float)MCM_BINS) - 1, 0), MCM_BINS - 1);
+            const double hit = (best_c == (int)rf.lab) ? 1.0 : 0.0;
+            auto part = [&](int i) {                // this row's part i; + 0.0 leaves a sum unchanged
+                return i == 0 ? -(double)lab_lp : i == 1 ? hit : i == 2 ? br : i == 3 + m ? 1.0
+                     : i == 3 + MCM_BINS + m ? (double)conf : i == 3 + 2 * MCM_BINS + m ? hit : 0.0;
+            };
+            if (lane > 0 && lane < MCM_PART / 2) { nll_acc += part(2 * lane); hit_acc += part(2 * lane + 1); }
         }
         if (lane == 0) {
             if (p.entropy && p.want_moments) p.entropy[b] = ent;
@@ -307,7 +352,7 @@ mc_exchange_kernel(const McxArgs p) {
         }
     }
     // ---- (5) cross-CTA finish (deterministic order), KL, ELBO head, sequence number ------------------------
-    if (solo && !(p.head && p.labels)) {
+    if (!METRICS && solo && !(p.head && p.labels)) {
         // nothing crosses CTAs: KL / Philox base by one thread; the sequence number (slot choice, handshake) is unused
         if (blockIdx.x == 0 && threadIdx.x == 0) {
             if (p.kl_out) *p.kl_out = kl_solo * inv_S;                    // main_bayesian.py:51  (kl / num_ens)
@@ -320,16 +365,29 @@ mc_exchange_kernel(const McxArgs p) {
     const bool want_head = p.head && p.labels;
     double nll_cta = 0.0, hit_cta = 0.0;
     if (want_head) {
-        nll_cta = block_sum(nll_acc, red);
+        nll_cta = block_sum(METRICS && lane ? 0.0 : nll_acc, red);     // the head: lane 0's only
         __syncthreads();
-        hit_cta = block_sum(hit_acc, red);
+        hit_cta = block_sum(METRICS && lane ? 0.0 : hit_acc, red);
     } else {
         __syncthreads();                 // the last CTA's bookkeeping below must follow every thread's reads of this launch's slot
+    }
+    unsigned int* mcm_last = reinterpret_cast<unsigned int*>(mcm_cta + MCM_PART);
+    if constexpr (METRICS) {             // this CTA's partials: its warps' in warp order (published before the CTA counts in)
+        for (int w = 0; w < nwarp; ++w) {
+            if (warp == w && lane < MCM_PART / 2) { mcm_cta[2 * lane] += nll_acc; mcm_cta[2 * lane + 1] += hit_acc; }
+            __syncthreads();
+        }
+        if (threadIdx.x < MCM_PART) {
+            p.metrics[MCM_SCRATCH + blockIdx.x * MCM_PART + threadIdx.x] = mcm_cta[threadIdx.x];
+            __threadfence();
+        }
+        __syncthreads();
     }
     if (threadIdx.x == 0) {
         // (a fence here also waits for the acknowledgements of this CTA's NVLink stores: only where something is published)
         if (want_head) { p.head_partials[2 * blockIdx.x] = nll_cta; p.head_partials[2 * blockIdx.x + 1] = hit_cta; __threadfence(); }
         const unsigned int prev = atomicAdd(p.done, 1u);
+        if constexpr (METRICS) *mcm_last = prev == gridDim.x - 1;
         if (prev == gridDim.x - 1) {
             if (want_head) __threadfence();
             float klsum = 0.0f;
@@ -350,9 +408,29 @@ mc_exchange_kernel(const McxArgs p) {
                 p.head[2] = (float)(hit / (double)B);                     // metrics.py:23-24
                 p.head[3] = p.beta * kl;
             }
+            if constexpr (METRICS) {
+                __threadfence();                                          // the other CTAs' partials, read below
+                p.metrics[0] += 1.0; p.metrics[1] += (double)B; p.metrics[4] += (double)klsum;   // validate_model's kl: sum_j kl_j
+            }
             if (p.noise_base) *p.noise_base += p.noise_inc;               // the next step's kernels draw fresh Philox streams
             *p.done = 0u;
             *p.seq = seq;
+        }
+    }
+    if constexpr (METRICS) {             // the last CTA: every partial over the CTAs in index order, into the accumulator
+        __syncthreads();
+        if (*mcm_last && threadIdx.x < MCM_PART) {
+            double s = 0.0;
+            for (unsigned int i0 = 0; i0 < gridDim.x; i0 += 8) {      // 8 loads in flight (L2: the other CTAs' fenced stores)
+                double v[8];
+#pragma unroll
+                for (unsigned int j = 0; j < 8; ++j)
+                    v[j] = i0 + j < gridDim.x ? __ldcg(p.metrics + MCM_SCRATCH + (i0 + j) * MCM_PART + threadIdx.x) : 0.0;
+#pragma unroll
+                for (int j = 0; j < 8; ++j) s += v[j];
+            }
+            p.metrics[MCM_HEAD + threadIdx.x] += s;
+            if (threadIdx.x < 2) p.metrics[2 + threadIdx.x] += s / (double)B;   // the step's nll and accuracy means (head)
         }
     }
     tl_exit(p.tl);

@@ -147,6 +147,12 @@ class MCForward:
       ``want_information`` (needs ``want_uncertainty``) expected_entropy = mean_s H[p_hat_s] and mutual_info = entropy -
       expected_entropy [B] (include/bbb_b200.h, bbb_mc_exchange_info).
 
+    ``metrics`` (needs ``with_labels``): an evaluation accumulator from ``new_metrics``; every step adds its validation
+    loss and accuracy inputs and its calibration sums to it on the device (bbb_mc_exchange_metrics), so a held-out set
+    needs one host read at the end (``read_metrics``).  Engines of different batch sizes may share one accumulator as long
+    as their steps run one after another (``wait()`` the last step of one engine before the next engine's first); the
+    warm-up steps the constructor runs do not count.
+
     ``batch_shards=Rb`` splits the batch as well as the samples: world = Rs x Rb ranks, rank r is sample group
     g = r % Rs (samples local_samples(num_ens, Rs, g)) and row block k = r // Rs (images ``rows`` = [b0, b1), row_block).
     Every rank is given the full x (and labels) and runs its samples on its rows only, with the LRT noise of image b drawn
@@ -159,7 +165,7 @@ class MCForward:
                  seed: Optional[int] = None, graph: bool = True, num_classes: Optional[int] = None,
                  static_inputs=None, first_replay: int = 0, fold: bool = True, overlap: bool = False, inflight: int = 1,
                  fold_group: Optional[int] = None, fold_budget: int = LAYER_FOLD_BUDGET, want_information: bool = False,
-                 batch_shards: int = 1):
+                 batch_shards: int = 1, metrics: Optional[torch.Tensor] = None):
         """``static_inputs``: device tensors the caller fills in place (e.g. targets of its host->device copies, or a
         rotation of resident batches); one graph is captured per tensor and ``self(slot=k)`` runs the step on
         ``static_inputs[k]`` with no staging copy.  ``first_replay``: index of the first replay's noise block.
@@ -176,6 +182,15 @@ class MCForward:
             raise L.EngineError("MCForward: want_information needs want_uncertainty")
         Fn._require_cuda(example_x, "MCForward")
         lib = L.lib()
+        if metrics is not None:
+            if not with_labels:
+                raise L.EngineError("MCForward: metrics needs with_labels")
+            n = int(lib.bbb_mc_metrics_bytes()) // 8
+            if not (metrics.device == example_x.device and metrics.dtype == torch.float64 and metrics.is_contiguous()
+                    and metrics.numel() >= n):
+                raise L.EngineError(f"MCForward: metrics must be a contiguous float64 tensor of >= {n} elements on "
+                                    f"{example_x.device} (mc.new_metrics)")
+        self.metrics = self._metrics = metrics      # _metrics: the accumulator the exchange adds to
         self.net, self.group = net, group
         self.dist, self.world, self.rank = _dist_info(group)
         if self.world > 16:
@@ -424,7 +439,10 @@ class MCForward:
             Fn._ptr(o.get("epistemic")), Fn._ptr(o.get("aleatoric")), Fn._ptr(o.get("entropy")), Fn._ptr(o.get("head")),
             Fn._ptr(advance_base), C.c_uint64(_STRIDE if advance_base is not None else 0),
             Fn._ptr(o.get("expected_entropy")), Fn._ptr(o.get("mutual_info")))
-        if self.batch_shards == 1:
+        if self._metrics is not None:
+            L.check(lib.bbb_mc_exchange_metrics(*args, self.batch_shards, Fn._ptr(self._metrics), Fn._stream(self.dev)),
+                    "bbb_mc_exchange_metrics")
+        elif self.batch_shards == 1:
             L.check(lib.bbb_mc_exchange_info(*args, Fn._stream(self.dev)), "bbb_mc_exchange_info")
         else:
             L.check(lib.bbb_mc_exchange_sharded(*args, self.batch_shards, Fn._stream(self.dev)), "bbb_mc_exchange_sharded")
@@ -435,9 +453,18 @@ class MCForward:
         # several steps in flight: the tap-GEMM layers take their 128-column tiles wherever Cout allows (throughput over the
         # latency of one step; the choice is made at launch = capture time, include/bbb_b200.h bbb_set_wide_tiles)
         prev_wide = L.lib().bbb_set_wide_tiles(1 if self.inflight > 1 else 0)
+        # Engines cached on a net (mc_forward, evaluate) form a reference cycle with it.  If the cyclic collector freed a
+        # dropped one in the middle of this capture, destroying its CUDA graphs would invalidate the capture: collect
+        # before, and keep the collector off while capturing.
+        import gc
+        gc.collect()
+        gc_on = gc.isenabled()
+        gc.disable()
         try:
             self._capture_graphs(warmup)
         finally:
+            if gc_on:
+                gc.enable()
             L.lib().bbb_set_wide_tiles(prev_wide)
 
     def _capture_graphs(self, warmup):
@@ -445,6 +472,9 @@ class MCForward:
         dev = self.dev
         side = torch.cuda.Stream(device=dev)
         side.wait_stream(torch.cuda.current_stream(dev))
+        live = self._metrics
+        if live is not None:
+            self._metrics = torch.zeros_like(live)      # the warm-up steps do not count
         with torch.cuda.stream(side):
             for _ in range(warmup):                 # eager: creates plans / workspaces; every rank runs the same exchanges
                 self._step(self.x, self.base)
@@ -452,6 +482,7 @@ class MCForward:
                 self._exchange(*self._chain(self.x, self.base, par=p_), par=p_)
         torch.cuda.current_stream(dev).wait_stream(side)
         torch.cuda.synchronize(dev)
+        self._metrics = live
         # GEMM chain on a HIGH-priority stream, parameter preps on the (default-priority) side streams: when both have CTAs
         # pending, the chain's go first -- the preps of later layers no longer keep the first GEMM's CTAs off the SMs
         cap = torch.cuda.Stream(device=dev, priority=-1)
@@ -683,6 +714,114 @@ def mc_forward(net_or_fn, x: torch.Tensor, num_ens: int, group=None, want_uncert
             res.append(out["head"])
         return tuple(res)
     return _generic_mc_forward(net_or_fn, x, num_ens, group, want_uncertainty, information, batch_shards)
+
+
+def new_metrics(device) -> torch.Tensor:
+    """A zeroed evaluation accumulator for ``MCForward(metrics=...)`` (bbb_mc_metrics_bytes of float64 words)."""
+    return torch.zeros(int(L.lib().bbb_mc_metrics_bytes()) // 8, dtype=torch.float64, device=device)
+
+
+def read_metrics(t: torch.Tensor) -> dict:
+    """One host read of an evaluation accumulator (layout: include/bbb_b200.h, bbb_mc_exchange_metrics).
+
+    ``steps``, ``images``; validate_model's inputs ``sum_nll_step`` / ``sum_acc_step`` (sums of the per-batch means) and
+    ``klsum`` (sum_j kl_j of one step, the mean over steps); over all images ``nll``, ``accuracy``, ``brier`` (mean
+    sum_c (p_bar_c - [c == y])^2) and ``ece`` (sum_m |correct_m - conf_m| / images over the MC_CAL_BINS equal-width
+    confidence bins); per bin ``bin_count``, ``bin_confidence`` and ``bin_accuracy`` (means; nan for an empty bin) -- a
+    reliability diagram."""
+    nb = L.MC_CAL_BINS
+    a = t[:8 + 3 * nb].cpu().tolist()
+    steps, images = a[0], a[1]
+    div = lambda x, n: x / n if n else float("nan")
+    cnt, conf, cor = a[8:8 + nb], a[8 + nb:8 + 2 * nb], a[8 + 2 * nb:8 + 3 * nb]
+    return {"steps": int(steps), "images": int(images), "sum_nll_step": a[2], "sum_acc_step": a[3],
+            "klsum": div(a[4], steps), "nll": div(a[5], images), "accuracy": div(a[6], images), "brier": div(a[7], images),
+            "ece": div(sum(abs(cor[m] - conf[m]) for m in range(nb)), images),
+            "bin_count": [int(c) for c in cnt], "bin_confidence": [div(conf[m], cnt[m]) for m in range(nb)],
+            "bin_accuracy": [div(cor[m], cnt[m]) for m in range(nb)]}
+
+
+def evaluate(net, loader, num_ens: int, train_size: float, beta_type=0.1, epoch=None, num_epochs=None, group=None,
+             seed: Optional[int] = None, inflight: int = 4, batch_shards: int = 1) -> dict:
+    """main_bayesian.validate_model over ``loader`` (batches of (inputs, labels)) on the engine, with calibration.
+
+    Returns read_metrics' dict plus ``valid_loss`` and ``valid_acc`` as validate_model computes them: the mean over
+    batches of nll_loss * train_size + beta_i * kl, with beta_i = get_beta(i - 1, len(loader), ...) for batch i (0-based)
+    and kl = sum_j kl_j (not divided by num_ens); the mean over batches of the batch accuracy.
+
+    Every batch runs through an in-flight engine (``overlap=True, inflight``), one per batch shape, all adding to one
+    device accumulator; the host reads it once, at the end.  Inputs and labels go into rotating device slots (the
+    engine's static_inputs), each rewritten only after the step that last read it has consumed it; host batches that are
+    not pinned are first copied into pinned slots, so the host can run up to ``max(2, inflight)`` batches ahead.  The
+    engines and the accumulator are kept on the net, as mc_forward keeps its engines, for the next call with the same
+    options (the next epoch); each call draws fresh noise.  Every rank must iterate the same loader (as MCForward
+    requires)."""
+    dev = next(net.parameters()).device
+    key = (int(num_ens), float(train_size), seed, id(group), int(inflight), int(batch_shards))
+    ev = net.__dict__.setdefault("_mc_eval", {}).get(key)
+    if ev is None:
+        ev = net.__dict__["_mc_eval"][key] = {"acc": new_metrics(dev), "engines": {}, "seed": seed}
+    acc, engines, nslots = ev["acc"], ev["engines"], max(2, int(inflight))
+    cur = torch.cuda.current_stream(dev)
+    acc.zero_()
+    last, n = None, 0
+    for x, y in loader:
+        shape = (tuple(x.shape), x.dtype)
+        e = engines.get(shape)
+        if e is None:
+            slots = [torch.zeros(x.shape, dtype=x.dtype, device=dev) for _ in range(nslots)]
+            # the k-th engine built draws noise blocks k * 2^16, k * 2^16 + 1, ...: engines do not share noise
+            eng = MCForward(net, slots[0], num_ens, group, with_labels=True, train_size=train_size, seed=ev["seed"],
+                            static_inputs=slots, first_replay=len(engines) << 16, overlap=True, inflight=inflight,
+                            batch_shards=batch_shards, metrics=acc)
+            ev["seed"] = eng.seed               # every engine draws from the same seed
+            e = engines[shape] = {"eng": eng, "slots": slots, "consumed": [None] * nslots, "steps": 0,
+                                  "labels": [torch.zeros(x.shape[0], dtype=torch.int64, device=dev) for _ in range(nslots)],
+                                  "pinned": [None] * nslots}
+        eng = e["eng"]
+        if last is not None and last is not eng:
+            last.wait()                         # the accumulator takes the steps one after another
+        s = e["steps"] % nslots
+        x, y = _pinned(e, s, x, y)
+        if e["consumed"][s] is not None:
+            # the step that last read slot s has consumed it.  The event is the engine's per-parity chain event, which a
+            # later step of the same parity may have recorded again: waiting on it can only wait longer.
+            cur.wait_event(e["consumed"][s])
+        e["slots"][s].copy_(x, non_blocking=True)
+        e["labels"][s].copy_(y, non_blocking=True)  # the step copies them on its own stream: they must outlive the call
+        if e["pinned"][s] is not None:
+            e["pinned"][s][2].record(cur)       # the pinned slot may be refilled once these copies are done
+        eng(labels=e["labels"][s], slot=s)
+        e["consumed"][s] = eng.input_consumed()
+        e["steps"] += 1
+        last, n = eng, n + 1
+    if last is None:
+        raise ValueError("evaluate: the loader yielded no batch")
+    last.wait()
+    m = read_metrics(acc)
+    beta_sum = sum(get_beta(i - 1, n, beta_type, epoch, num_epochs) for i in range(n))
+    m["valid_loss"] = (float(train_size) * m["sum_nll_step"] + beta_sum * m["klsum"]) / n
+    m["valid_acc"] = m["sum_acc_step"] / n
+    return m
+
+
+def _pinned(e, s, x, y):
+    """(x, y), with host tensors that are not pinned copied into pinned slot s of engine entry e (after the previous
+    copies out of that slot have finished), so that the copies to the device do not hold up the host."""
+    if (x.is_cuda or x.is_pinned()) and (y.is_cuda or y.is_pinned()):
+        return x, y
+    if e["pinned"][s] is None:
+        e["pinned"][s] = (torch.empty(x.shape, dtype=x.dtype).pin_memory(),
+                          torch.empty(y.shape, dtype=y.dtype).pin_memory(), torch.cuda.Event())
+    hx, hy, done = e["pinned"][s]
+    done.synchronize()
+    if not (x.is_cuda or x.is_pinned()):
+        hx.copy_(x)
+        x = hx
+    if not (y.is_cuda or y.is_pinned()):
+        hy.copy_(y)
+        y = hy
+    return x, y
 
 
 def engine_forward_fn(net) -> Callable:
