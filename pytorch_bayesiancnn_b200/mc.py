@@ -19,6 +19,7 @@ Two implementations of the same contract:
 from __future__ import annotations
 
 import ctypes as C
+import math
 from typing import Callable, Optional
 
 import os
@@ -102,7 +103,6 @@ def _per_image_chain(kids, x_shape):
     """What the children of a ModuleWrapper do, run one after another on a batch of ``x_shape``: (the Bayesian layers
     with their input shapes, pass bytes, largest element count) -- or None when a child is not known to treat every image
     on its own (then folding samples into the batch could change a result)."""
-    import math
     from torch import nn
     from .modules import FlattenLayer, _BayesLayer
     shape, layers, pass_bytes, big = tuple(x_shape), [], 0, 0
@@ -832,6 +832,12 @@ def engine_forward_fn(net) -> Callable:
     return fn
 
 
+# Below this log p_bar[b, y_b] (p_bar < 1e-26) MCTrainStep forms the loss gradient's softmax / p_bar ratio in log space.
+# Above it both factors are far from fp32 underflow: any loss of precision of softmax_j[b, y_b] then moves the ratio by
+# less than 1e-18.
+_LOG_P_DIRECT_MIN = -60.0
+
+
 class MCTrainStep(MCForward):
     """One SHARDED training step with main_bayesian.train_model's semantics (main_bayesian.py:38-58): every rank runs
     its share of the ``num_ens`` weight samples WITH autograd (layer forward kernels + the engine's backward kernels),
@@ -878,11 +884,18 @@ class MCTrainStep(MCForward):
         if self.ids:
             S = float(self.num_ens)
             idx = self.labels[b0:b1].view(-1, 1)
-            p_bar_y = o["log_outputs"][b0:b1].gather(1, idx).exp()          # p_bar[b, y_b] of the block's rows
+            log_p_bar_y = o["log_outputs"][b0:b1].gather(1, idx)            # log p_bar[b, y_b] of the block's rows
+            p_bar_y = log_p_bar_y.exp()
+            # softmax_j[b,y_b] / (S p_bar[b,y_b]) is a ratio in [0, 1], but both factors underflow fp32 (0 / 0 = NaN) once
+            # the label's log-probability falls below about -100.  Rows with log p_bar below _LOG_P_DIRECT_MIN take the
+            # ratio in log space; the others keep the direct quotient, exact to fp32 rounding there.
+            in_range = log_p_bar_y > _LOG_P_DIRECT_MIN
             grads = []
             for lg in logits:
-                sm = torch.softmax(lg.detach().float(), dim=1)
-                w = sm.gather(1, idx) / (S * p_bar_y)
+                lg = lg.detach().float()
+                sm = torch.softmax(lg, dim=1)
+                w = torch.where(in_range, sm.gather(1, idx) / (S * p_bar_y),
+                                (torch.log_softmax(lg, dim=1).gather(1, idx) - log_p_bar_y - math.log(S)).exp())
                 onehot = torch.zeros_like(sm).scatter_(1, idx, 1.0)
                 grads.append((-(self.train_size / self.B)) * w * (onehot - sm))
             # the KL does not depend on the rows: one block per sample group adds its gradient

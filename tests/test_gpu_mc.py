@@ -329,13 +329,15 @@ def test_mc_sample_folding_equals_sample_loop(dev):
     assert a.kernels_per_step < b.kernels_per_step
 
 
-def _oracle_train_grads(key, params, x, labels, eps_per_sample, variant, classes, train_size, beta):
-    """main_bayesian.py:46-58 through torch autograd on the oracle: grads of every parameter."""
+def _oracle_train_grads(key, params, x, labels, eps_per_sample, variant, classes, train_size, beta, dtype=torch.float32):
+    """main_bayesian.py:46-58 through torch autograd on the oracle, in `dtype` on the device of the tensors given:
+    grads of every parameter."""
     from oracle import bbb_oracle as O
-    P = [{k: v.clone().requires_grad_(True) for k, v in p.items()} for p in params]
+    P = [{k: v.to(dtype).clone().requires_grad_(True) for k, v in p.items()} for p in params]
+    x = x.to(dtype)
     outs, kl = [], 0.0
     for eps in eps_per_sample:
-        lg, _kl = O.net_forward(key, P, x, eps, variant, "softplus", 0.0, 0.1, classes)
+        lg, _kl = O.net_forward(key, P, x, [e.to(dtype) for e in eps], variant, "softplus", 0.0, 0.1, classes)
         outs.append(lg)
         kl = kl + _kl
     kl = kl / len(eps_per_sample)
