@@ -101,7 +101,10 @@ size_t bbb_workspace_bytes(const bbb_layer_desc* desc);
  *          own weight draw; needs (reserved[1] * OH * OW) % 128 == 0 and the workspace of the folding desc.  The KL is
  *          computed once, bit-identical to an unfolded call.  Needs sample == 1, in-kernel noise (eps_a / eps_b NULL,
  *          else BBB_E_UNSUPPORTED), batch % reserved[1] == 0 (else BBB_E_INVALID) and a tensor-core math mode (bf16 /
- *          tf32, or auto resolving to one; else BBB_E_UNSUPPORTED).  reserved[] all zero: no fold.
+ *          tf32, or auto resolving to one; else BBB_E_UNSUPPORTED).  reserved[] all zero: no fold.  A folded LRT call
+ *          can be trained through: act_std is written for every row, and bbb_lrt_noise_grad with the same desc draws
+ *          the noise of the backward row by row from the same streams; the weight and input gradients are plain
+ *          contractions over all rows (the CUDA-core backward, bbb_conv2d_backward, does not fold).
  * desc->reserved[0] bits 8..30 (BBB_FIRST_IMAGE_*): the FIRST IMAGE, the global index of image 0 of this call (of each
  *          sample block when folded) when a batch is split into row blocks over several calls or ranks
  *          (bbb_mc_exchange_sharded).  LRT: image b draws its activation noise at element index
@@ -229,6 +232,20 @@ int bbb_linear_backward(const bbb_layer_desc* desc, const void* x, const void* g
  * Philox4x32-10(counter = ((offset+i)>>2, stream_id), key = seed), Box-Muller. */
 int bbb_philox_normal_fill(float* out, uint64_t n, uint64_t seed, uint64_t stream_id,
                            uint64_t offset, void* cuda_stream);
+
+/* Backward of the LRT noise term (layers/BBB_LRT/BBBConv.py:75-79, BBB_LRT/BBBLinear.py:67-71):
+ *   gv = grad_y * eps / (2 * act_std)   element for element, fp32, the shape of y,
+ * with eps regenerated exactly as bbb_conv2d_forward / bbb_linear_forward of `desc` drew it:
+ * stream stream_id (+ *stream_base when non-NULL, read on the device), NHWC element index, the first image of
+ * reserved[0], and with reserved[1..3] the per-row sample streams of an MC-sample fold.  No eps tensor is made.
+ * grad_y, act_std (what the forward saved) and gv are NCHW [batch, out_channels, OH, OW] (a linear layer: [batch, out]).
+ * The two multiplies and the division are separate IEEE round-to-nearest operations (no FMA, no approximate division),
+ * so gv is bit for bit what the three element-wise ops compute on eps = bbb_philox_normal_fill's numbers.
+ * Refused: a BBB desc (BBB_E_INVALID), sample == 0 (BBB_E_UNSUPPORTED), batch % reserved[1] != 0 (BBB_E_INVALID), a
+ * first image or fold whose counts would pass int32 (BBB_E_INVALID, as the forward). */
+int bbb_lrt_noise_grad(const bbb_layer_desc* desc, const float* grad_y, const float* act_std,
+                       uint64_t seed, uint64_t stream_id, const uint64_t* stream_base,
+                       float* gv, void* cuda_stream);
 
 /* *base += inc on the device (one tiny kernel; put it at the head of a captured
  * graph so each replay moves every layer to a fresh Philox stream). */

@@ -32,7 +32,7 @@ SYMBOLS = (
     "bbb_mc_combine", "bbb_noise_advance", "bbb_last_error", "bbb_abi_version", "bbb_launch_count",
     "bbb_mc_buffer_bytes", "bbb_mc_state_bytes", "bbb_mc_exchange", "bbb_mc_exchange_info", "bbb_mc_exchange_sharded",
     "bbb_comm_alloc", "bbb_comm_free", "bbb_comm_export", "bbb_comm_import", "bbb_comm_unimport", "bbb_set_wide_tiles",
-    "bbb_mc_metrics_bytes", "bbb_mc_exchange_metrics",
+    "bbb_mc_metrics_bytes", "bbb_mc_exchange_metrics", "bbb_lrt_noise_grad",
 )
 MC_MOMENTS, MC_NORMALIZED, MC_INFO = 1, 2, 4
 MC_CAL_BINS = 15                 # BBB_MC_CAL_BINS: calibration bins of the evaluation accumulator
@@ -81,6 +81,8 @@ def _bind(lib):
     lib.bbb_kl_backward.restype = C.c_int
     lib.bbb_philox_normal_fill.argtypes = [fp, u64, u64, u64, u64, vp]
     lib.bbb_philox_normal_fill.restype = C.c_int
+    lib.bbb_lrt_noise_grad.argtypes = [dp, fp, fp, u64, u64, vp, fp, vp]
+    lib.bbb_lrt_noise_grad.restype = C.c_int
     lib.bbb_mc_combine.argtypes = [fp, i32, i32, i32, fp, fp, vp]
     lib.bbb_mc_combine.restype = C.c_int
     lib.bbb_mc_buffer_bytes.argtypes = [i32, i32, i32, i32]

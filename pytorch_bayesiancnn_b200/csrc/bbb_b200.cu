@@ -432,6 +432,36 @@ int bbb_philox_normal_fill(float* out, uint64_t n, uint64_t seed, uint64_t strea
     return BBB_OK;
 }
 
+int bbb_lrt_noise_grad(const bbb_layer_desc* d, const float* grad_y, const float* act_std, uint64_t seed,
+                       uint64_t stream_id, const uint64_t* stream_base, float* gv, void* cuda_stream) {
+    bbb::Geom g;
+    if (int rc = check_desc(d, g, false)) return rc;        // first image and fold within int32 element counts
+    if (d->variant != BBB_VARIANT_LRT) return fail(BBB_E_INVALID, "bbb_lrt_noise_grad: not an LRT layer desc (variant %d)", d->variant);
+    if (!d->sample) return fail(BBB_E_UNSUPPORTED, "bbb_lrt_noise_grad: a mean-only call (sample == 0) draws no noise");
+    const int rows = d->reserved[1];
+    if (rows > 0 && g.B % rows) return fail(BBB_E_INVALID, "batch %d is not a multiple of the rows per MC sample %d", g.B, rows);
+    if (!grad_y || !act_std || !gv) return fail(BBB_E_INVALID, "NULL tensor pointer");
+    bbb::McFold fold;
+    if (int rc = layer_fold(d, g, nullptr, nullptr, fold)) return rc;
+    const bool vec4 = g.N % 4 == 0;
+    const uint64_t work = (uint64_t)g.B * (vec4 ? g.N / 4 : g.N) * g.OHW;
+    uint64_t blocks = (work + 255) / 256;
+    const uint64_t cap = (uint64_t)sm_count() * 8;
+    if (blocks > cap) blocks = cap;
+    const bbb::NoiseKey key = bbb::make_key(seed, stream_id);
+    const auto* base = (const unsigned long long*)stream_base;
+    if (vec4)
+        bbb::lrt_noise_grad_kernel<true><<<(unsigned)blocks, 256, 0, (cudaStream_t)cuda_stream>>>(
+            grad_y, act_std, gv, g.B, g.N, g.OHW, key, base, fold);
+    else
+        bbb::lrt_noise_grad_kernel<false><<<(unsigned)blocks, 256, 0, (cudaStream_t)cuda_stream>>>(
+            grad_y, act_std, gv, g.B, g.N, g.OHW, key, base, fold);
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return cuda_fail(e, "lrt_noise_grad launch");
+    g_launches += 1;
+    return BBB_OK;
+}
+
 int bbb_mc_combine(const float* logits, int32_t S, int32_t B, int32_t C, float* log_outputs, float* moments,
                    void* cuda_stream) {
     if (!logits || !log_outputs) return fail(BBB_E_INVALID, "NULL tensor pointer");

@@ -62,6 +62,42 @@ philox_fill_kernel(float* __restrict__ out, uint64_t n, NoiseKey key, uint64_t o
         out[i] = normal1(offset + i, key);
 }
 
+// Backward of the LRT noise term, gv = grad_y * eps / (2 * act_std) (layers/BBB_LRT/BBBConv.py:75-79), with eps drawn
+// again where the forward drew it: Philox stream of row b's sample (fold_key), NHWC element index
+// ((first_image + b) * OHW + pix) * N + c.  grad_y, act_std and gv are NCHW [B, N, OHW].  The two multiplies and the
+// division are rounded one by one, as the element-wise ops of a tensor library do it.
+// VEC4 (N % 4 == 0): a thread takes the four channels one Philox call draws, at one pixel; consecutive threads take
+// consecutive pixels, so each of its four loads and stores is coalesced.  Otherwise one thread per element, in NCHW order.
+template <bool VEC4>
+__global__ void __launch_bounds__(256)
+lrt_noise_grad_kernel(const float* __restrict__ gy, const float* __restrict__ act_std, float* __restrict__ gv,
+                      int B, int N, int OHW, NoiseKey key, const unsigned long long* stream_base, McFold fold) {
+    const NoiseKey k0 = effective_key(key, stream_base);
+    const unsigned per = VEC4 ? N / 4 : N;
+    const unsigned total = (unsigned)B * per * (unsigned)OHW;           // <= B * N * OHW < 2^31 (make_geom)
+    for (unsigned t = blockIdx.x * blockDim.x + threadIdx.x; t < total; t += gridDim.x * blockDim.x) {
+        const unsigned pix = t % (unsigned)OHW, r = t / (unsigned)OHW;
+        const unsigned c = r % per;
+        const int b = (int)(r / per);
+        int bi;
+        const NoiseKey k = fold_key(k0, fold, b, bi);
+        const uint64_t pos = ((uint64_t)bi * OHW + pix) * N;                // NHWC index of channel 0 at this pixel
+        if constexpr (VEC4) {
+            const float4 z = normal4((pos >> 2) + c, k);                    // channels 4c .. 4c+3 (pos % 4 == 0)
+            const float e[4] = {z.x, z.y, z.z, z.w};
+            const unsigned o = ((unsigned)b * N + 4 * c) * (unsigned)OHW + pix;
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+                const unsigned oj = o + j * (unsigned)OHW;
+                gv[oj] = __fdiv_rn(__fmul_rn(__ldg(gy + oj), e[j]), __fmul_rn(2.0f, __ldg(act_std + oj)));
+            }
+        } else {
+            const float e = normal1(pos + c, k);
+            gv[t] = __fdiv_rn(__fmul_rn(__ldg(gy + t), e), __fmul_rn(2.0f, __ldg(act_std + t)));
+        }
+    }
+}
+
 __global__ void noise_advance_kernel(unsigned long long* base, unsigned long long inc) { *base += inc; }
 
 // main_bayesian.py:46-53 + utils.py:14-22 (+ uncertainty_estimation.py:70-96 moments).

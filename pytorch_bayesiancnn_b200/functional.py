@@ -54,6 +54,7 @@ class _Noise(threading.local):
         self.queue = None          # external-eps queue (parity mode)
         self.base = None           # device int64[1] stream base (CUDA-graph capture mode)
         self.fold = None           # (rows per MC sample, Philox stream stride) of layer_fold
+        self.fold_grad = False     # layer_fold(grad=True): folded LRT calls record autograd
         self.first_image = 0       # global index of image 0 of the layer calls (first_image)
 
     def current_seed(self) -> int:
@@ -123,18 +124,25 @@ def stream_base(base: Optional[torch.Tensor]):
 
 
 @contextlib.contextmanager
-def layer_fold(rows: int, stride: int):
+def layer_fold(rows: int, stride: int, grad: bool = False):
     """Layer calls inside fold Monte-Carlo samples into the batch (include/bbb_b200.h, bbb_conv2d_forward): image b of
     the batch is image b % rows of sample b // rows, which draws from Philox stream stream_id + (b // rows) * stride --
     the same numbers as one call per sample.  What uncertainty_estimation.py:38-41 does by repeating the input, with
-    each repeat its own sample.  Forward only, in-kernel noise only: a layer call under autograd or with external eps
-    raises EngineError."""
-    prev = _noise.fold
-    _noise.fold = (int(rows), int(stride))
+    each repeat its own sample.  In-kernel noise only: a layer call with external eps raises EngineError.
+
+    ``grad=False`` (default): forward only -- a layer call under autograd raises EngineError.
+    ``grad=True``: an LRT layer call on a tensor-core math mode (bf16, tf32, or auto resolving to one) records autograd.
+    Its backward runs the tensor-core contractions over all rows (a weight gradient sums the rows of every sample, an
+    input-gradient row depends on its own row only) and draws the noise term's gradient row by row from the same
+    streams (bbb_lrt_noise_grad); the KL backward runs once.  Refused with EngineError: a BBB layer, math='fp32', external
+    eps, and any geometry whose backward would fall back to the CUDA-core kernels (tc_backward_refusal), which do not
+    know the fold."""
+    prev = _noise.fold, _noise.fold_grad
+    _noise.fold, _noise.fold_grad = (int(rows), int(stride)), bool(grad)
     try:
         yield
     finally:
-        _noise.fold = prev
+        _noise.fold, _noise.fold_grad = prev
 
 
 @contextlib.contextmanager
@@ -331,12 +339,23 @@ _TC_K_MAX = 8192          # the gather kernel keeps an 8-byte table entry per re
 _tc_math = L.MATH_BF16_TC          # operand type of the backward contractions (set per call by _backward_tc)
 
 
+def _tc_operand_math(math):
+    """The operand type of the backward contractions of a layer on math mode `math`: the forward's (tf32, else bf16)."""
+    return L.MATH_TF32_TC if math == L.MATH_TF32_TC else L.MATH_BF16_TC
+
+
+def _tc_contract_desc(x_shape, w_shape, conv, math):
+    """The desc of one contraction of the tensor-core backward (_tc_contract): the engine's forward of an x of
+    `x_shape` with a weight of `w_shape`, sample=0, no bias -- host-only, so that support can be asked ahead."""
+    return make_desc(tuple(x_shape), tuple(w_shape), conv, L.VARIANT_BBB, False, False, 0.0, 1.0, math)
+
+
 def _tc_contract(x, w, conv):
     """Plain (mean-only, bias-free) conv2d / linear of fp32 `x` with the fp32 tensor `w` on the tensor-core layer kernel
     (bf16 or tf32 operands like the layer's forward, fp32 accumulators): the engine's forward with sample=0, no KL."""
     lib = L.lib()
     x, w = x.contiguous(), w.contiguous()
-    d = make_desc(tuple(x.shape), tuple(w.shape), conv, L.VARIANT_BBB, False, False, 0.0, 1.0, _tc_math)
+    d = _tc_contract_desc(x.shape, w.shape, conv, _tc_math)
     if conv is None:
         y = torch.empty(x.shape[0], w.shape[0], dtype=torch.float32, device=x.device)
         fn = lib.bbb_linear_forward
@@ -351,11 +370,13 @@ def _tc_contract(x, w, conv):
     return y
 
 
-def _tc_dgrad(g, w, conv, x_shape):
+def _tc_dgrad(g, w, conv, x_shape, contract=None):
     """d x of y = conv(x, w): the full correlation of (zero-inserted) g with the flipped, channel-transposed kernel --
-    itself a stride-1 convolution, so it runs on the same tensor-core layer kernel."""
+    itself a stride-1 convolution, so it runs on the same tensor-core layer kernel.  ``contract``: what runs each
+    contraction (default _tc_contract)."""
+    contract = contract or _tc_contract
     if conv is None:
-        return _tc_contract(g, w.t(), None)                               # [B,N] x [K,N]^T -> [B,K]
+        return contract(g, w.t(), None)                                   # [B,N] x [K,N]^T -> [B,K]
     (sh, sw), (ph, pw), (dh, dw) = conv
     kh, kw = w.shape[2], w.shape[3]
     H, W = x_shape[2], x_shape[3]
@@ -370,15 +391,17 @@ def _tc_dgrad(g, w, conv, x_shape):
         gu[:, :, 0:(OH - 1) * sh + 1:sh, 0:(OW - 1) * sw + 1:sw] = g
         g = gu
     wt = w.flip(2, 3).transpose(0, 1)
-    return _tc_contract(g, wt, ((1, 1), (qh, qw), (dh, dw)))
+    return contract(g, wt, ((1, 1), (qh, qw), (dh, dw)))
 
 
-def _tc_wgrad(x, g, conv, w_shape):
+def _tc_wgrad(x, g, conv, w_shape, contract=None):
     """d w of y = conv(x, w): a convolution with the batch as the reduction ("channel") axis -- input x^T [C,B,H,W],
     kernel g^T [N,B,OH,OW], stride <-> dilation swapped -- on the tensor-core layer kernel.  Deterministic (no atomics);
-    the batch is cut so that the reduction index fits the kernel's shared-memory table and the partial results summed."""
+    the batch is cut so that the reduction index fits the kernel's shared-memory table and the partial results summed.
+    ``contract``: what runs each contraction (default _tc_contract)."""
+    contract = contract or _tc_contract
     if conv is None:
-        out = _tc_contract(x.t(), g.t(), None)                             # [K,B] x [N,B]^T -> [K,N]
+        out = contract(x.t(), g.t(), None)                                 # [K,B] x [N,B]^T -> [K,N]
         return out.t()
     (sh, sw), (ph, pw), (dh, dw) = conv
     kh, kw = w_shape[2], w_shape[3]
@@ -388,13 +411,64 @@ def _tc_wgrad(x, g, conv, w_shape):
     for b0 in range(0, B, per):
         xt = x[b0:b0 + per].transpose(0, 1)
         gt = g[b0:b0 + per].transpose(0, 1)
-        part = _tc_contract(xt, gt, ((dh, dw), (ph, pw), (sh, sw)))[:, :, :kh, :kw]
+        part = contract(xt, gt, ((dh, dw), (ph, pw), (sh, sw)))[:, :, :kh, :kw]
         acc = part if acc is None else acc + part
     return acc.transpose(0, 1)
 
 
 def _tc_backward_ok(cfg):
     return cfg["math"] in (L.MATH_BF16_TC, L.MATH_AUTO, L.MATH_TF32_TC) and os.environ.get("BBB_B200_BWD", "tc") != "simt"
+
+
+def _tc_backward_contractions(x_shape, w_shape, conv, need_x=True):
+    """(x shape, w shape, conv) of every distinct contraction the tensor-core backward of a layer call on an input of
+    `x_shape` issues (_tc_wgrad, and _tc_dgrad with ``need_x``), recorded on the meta device without computing; None
+    when _tc_dgrad gives up (padding > dilation * (kernel - 1): no stride-1 correlation gives the input gradient)."""
+    calls = {}
+
+    def out_shape(xs, ws, cv):
+        return (xs[0], ws[0]) + (() if cv is None else out_hw(xs[2], xs[3], ws[2], ws[3], cv))
+
+    def record(x, w, cv):
+        calls[(tuple(x.shape), tuple(w.shape), cv)] = None
+        return torch.empty(out_shape(x.shape, w.shape, cv), device="meta")
+
+    x = torch.empty(tuple(x_shape), device="meta")
+    w = torch.empty(tuple(w_shape), device="meta")
+    g = torch.empty(out_shape(x.shape, w.shape, conv), device="meta")
+    _tc_wgrad(x, g, conv, w.shape, contract=record)
+    if need_x and _tc_dgrad(g, w, conv, x.shape, contract=record) is None:
+        return None
+    return list(calls)
+
+
+def tc_backward_refusal(x_shape, w_shape, conv, math, need_x=True) -> Optional[str]:
+    """Why the tensor-core backward of a layer call on an input of `x_shape` (math mode `math`) would not run -- the
+    layer would then fall back to the CUDA-core kernels -- or None when it runs.  Host-only: it asks
+    bbb_forward_supported, the check the kernel itself makes, about every contraction the backward would issue."""
+    calls = _tc_backward_contractions(x_shape, w_shape, conv, need_x)
+    if calls is None:
+        return "the input gradient has no tensor-core contraction (padding > dilation * (kernel - 1))"
+    lib = L.lib()
+    for xs, ws, cv in calls:
+        if lib.bbb_forward_supported(C.byref(_tc_contract_desc(xs, ws, cv, _tc_operand_math(math)))) != 0:
+            return f"the contraction of x {xs} with w {ws} is refused: {lib.bbb_last_error().decode('utf-8', 'replace')}"
+    return None
+
+
+def _fold_grad_refusal(cfg, x_shape, w_shape, need_x) -> Optional[str]:
+    """Why a layer call under layer_fold(grad=True) cannot record autograd, or None.  The CUDA-core backward does not
+    know the fold: a call whose backward would fall back to it is refused here rather than given wrong gradients."""
+    if cfg["variant"] != L.VARIANT_LRT:
+        return "a BBB layer draws one weight sample per MC sample; only LRT layers train folded"
+    if cfg["math"] == L.MATH_FP32:
+        return "math='fp32' does not fold; use a tensor-core math mode (bf16, tf32 or auto)"
+    if not _tc_backward_ok(cfg):
+        return "the CUDA-core backward (BBB_B200_BWD=simt) does not fold"
+    if external_eps_active():
+        return "MC-sample folding draws its noise in-kernel (no external eps)"
+    why = tc_backward_refusal(x_shape, w_shape, cfg["conv"], cfg["math"], need_x)
+    return None if why is None else f"the backward would leave the tensor cores: {why}"
 
 
 # --------------------------------------------------------------------------- #
@@ -420,7 +494,11 @@ class BayesLayerFn(torch.autograd.Function):
         need_grad = any(ctx.needs_input_grad[:5])      # grad mode is off inside Function.forward
         fold = _noise.fold
         if fold is not None and need_grad and cfg.get("grad_enabled", True):
-            raise L.EngineError("layer_fold: MC-sample folding is forward-only (call under torch.no_grad())")
+            if not _noise.fold_grad:
+                raise L.EngineError("layer_fold: MC-sample folding is forward-only (call under torch.no_grad())")
+            why = _fold_grad_refusal(cfg, tuple(x.shape), tuple(W_mu.shape), ctx.needs_input_grad[0])
+            if why is not None:
+                raise L.EngineError(f"layer_fold(grad=True): {why}")
         if fold is not None and external_eps_active():
             raise L.EngineError("layer_fold: MC-sample folding draws its noise in-kernel (no external eps)")
         d = make_desc(tuple(x.shape), tuple(W_mu.shape), conv, variant, sample, has_bias,
@@ -464,6 +542,7 @@ class BayesLayerFn(torch.autograd.Function):
         ctx.desc = d
         ctx.noise = (seed, stream_id, base)
         ctx.first_image = _noise.first_image
+        ctx.fold = fold
         ctx.has_bias = has_bias
         ctx.save_for_backward(x, W_mu_c, W_rho_c, bias_mu, bias_rho, act_std, eps_a, eps_b)
         return y, kl
@@ -489,6 +568,8 @@ class BayesLayerFn(torch.autograd.Function):
                 if "code -2" not in str(e):                # BBB_E_UNSUPPORTED: a shape the tensor-core kernel does not take
                     raise
                 out = None
+            if out is None and ctx.fold is not None:
+                raise L.EngineError("layer_fold(grad=True): the tensor-core backward refused a folded call")
             if out is not None:
                 gx, gw_mu, gw_rho, gb_mu, gb_rho = out
                 g_W_mu += gw_mu.reshape(g_W_mu.shape)
@@ -530,16 +611,16 @@ class BayesLayerFn(torch.autograd.Function):
         """SURVEY.md Appendix A on the tensor cores: every contraction of the backward (wgrad of the mean and of the
         variance path, dgrad of both) is a call of the tensor-core layer kernel with the operands' roles swapped; eps is
         regenerated from the forward's Philox stream; the element-wise chain rule through sigma = softplus(rho) is
-        parameter-sized glue.  Returns None when a shape does not fit (the caller then uses the CUDA-core kernels)."""
+        parameter-sized glue.  Returns None when a shape does not fit (the caller then uses the CUDA-core kernels).
+        LRT: the noise term's gradient gv = gy * eps / (2 act_std) is one kernel (bbb_lrt_noise_grad) on the forward's
+        desc, folded or not, which reads the stream base on the device."""
         x, W_mu, W_rho, bias_mu, bias_rho, act_std, eps_a, eps_b = ctx.saved_tensors
         cfg = ctx.cfg
         conv, variant, sample = cfg["conv"], cfg["variant"], cfg["sample"]
         dev = x.device
         global _tc_math
-        _tc_math = L.MATH_TF32_TC if cfg["math"] == L.MATH_TF32_TC else L.MATH_BF16_TC     # same operand type as the forward
+        _tc_math = _tc_operand_math(cfg["math"])           # same operand type as the forward
         seed, stream_id, base = ctx.noise
-        if base is not None:
-            stream_id = int(stream_id) + int(base.item())
         need_x = ctx.needs_input_grad[0]
         sig = torch.log1p(torch.exp(W_rho))
         dsig = torch.sigmoid(W_rho)
@@ -549,12 +630,9 @@ class BayesLayerFn(torch.autograd.Function):
             gw_mu = _tc_wgrad(x, gy, conv, W_mu.shape)
             if sample:
                 if eps_a is None:
-                    # element index of image b is counted from the call's first image, as in the forward
-                    z = philox_normal(gy.numel(), seed, stream_id, ctx.first_image * (gy.numel() // gy.shape[0]), device=dev)
-                    eps = z.view(gy.shape) if conv is None else z.view(gy.shape[0], gy.shape[2], gy.shape[3], gy.shape[1]).permute(0, 3, 1, 2)
+                    gv = lrt_noise_grad(ctx.desc, gy, act_std, seed, stream_id, base)
                 else:
-                    eps = eps_a
-                gv = gy * eps / (2.0 * act_std)
+                    gv = gy * eps_a / (2.0 * act_std)
                 gw_rho = _tc_wgrad(x * x, gv, conv, W_mu.shape) * (2.0 * sig * dsig)
             else:
                 gv, gw_rho = None, torch.zeros_like(W_rho)
@@ -575,6 +653,8 @@ class BayesLayerFn(torch.autograd.Function):
                     gb_rho = torch.zeros_like(bias_rho)
         else:
             nw = W_mu.numel()
+            if base is not None:
+                stream_id = int(stream_id) + int(base.item())
             if sample:
                 ew = eps_a if eps_a is not None else philox_normal(nw, seed, stream_id, 0, device=dev).view(W_mu.shape)
                 W = W_mu + ew * sig
@@ -647,6 +727,18 @@ def philox_normal(n: int, seed: int, stream_id: int, offset: int = 0, device="cu
                                         C.c_uint64(offset), _stream(out.device))
     L.check(rc, "bbb_philox_normal_fill")
     return out
+
+
+def lrt_noise_grad(desc: L.LayerDesc, gy: torch.Tensor, act_std: torch.Tensor, seed: int, stream_id: int,
+                   base: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """gv = gy * eps / (2 * act_std) of an LRT layer call, with eps drawn again from the streams of the forward of `desc`
+    (its first image and MC-sample fold included; ``base``: the device stream base of a captured call) -- one kernel,
+    no eps tensor (bbb_lrt_noise_grad).  gy and act_std: contiguous fp32 in y's shape."""
+    gv = torch.empty_like(gy)
+    rc = L.lib().bbb_lrt_noise_grad(C.byref(desc), _ptr(gy), _ptr(act_std), C.c_uint64(seed), C.c_uint64(stream_id),
+                                    _ptr(base), _ptr(gv), _stream(gy.device))
+    L.check(rc, "bbb_lrt_noise_grad")
+    return gv
 
 
 def mc_combine(logits: torch.Tensor, want_moments: bool = False):

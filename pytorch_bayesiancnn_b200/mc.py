@@ -838,6 +838,55 @@ def engine_forward_fn(net) -> Callable:
 _LOG_P_DIRECT_MIN = -60.0
 
 
+def train_fold_groups(net, x_shape, n_local: int, stride: int, first_image: int = 0, fold_group: Optional[int] = None,
+                      budget: int = LAYER_FOLD_BUDGET):
+    """How MCTrainStep(fold=True) groups a rank's ``n_local`` samples on a row block of ``x_shape`` (rows, C, H, W):
+    layer_fold_groups, or None for the sample loop.  None unless every Bayesian layer is LRT and every child treats
+    each image on its own.  G is the largest group size -- up to the budget's or ``fold_group``, the int32 element cap and
+    n_local -- at which the engine accepts every layer's folded forward (bbb_forward_supported) and every contraction of
+    its backward (Fn.tc_backward_refusal; e.g. a linear layer's weight gradient takes at most so many rows).  A math mode
+    without tensor cores folds neither.  Unlike MCForward's per-layer fold this does not defer to the fused chain, which
+    never runs under autograd.  Host-only: no GPU work."""
+    from .modules import ModuleWrapper
+    kids = list(net.children())
+    if not kids or type(net).forward is not ModuleWrapper.forward:
+        return None
+    chain = _per_image_chain(kids, tuple(x_shape))
+    if chain is None:
+        return None
+    layers, pass_bytes, big = chain
+    if not layers or any(m._variant != L.VARIANT_LRT for m, _ in layers):
+        return None
+    fold = (int(x_shape[0]), int(stride))
+    groups = layer_fold_groups(n_local, pass_bytes, big, budget, fold_group)
+    while groups is not None and not all(_train_fold_accepted(layers, n, fold, first_image) for n in {n for _, n in groups}):
+        groups = layer_fold_groups(n_local, pass_bytes, big, fold_group=max(n for _, n in groups) - 1)
+    return groups
+
+
+def _train_fold_accepted(layers, n, fold, first_image):
+    """Does the engine take a training pass of n folded samples: every layer's forward and backward?"""
+    lib = L.lib()
+    for i, (m, xs) in enumerate(layers):
+        cfg = m._cfg(True)
+        xs = (n * xs[0],) + tuple(xs[1:])
+        d = Fn.make_desc(xs, tuple(m.W_mu.shape), cfg["conv"], cfg["variant"], True, m.bias_mu is not None,
+                         cfg["prior_mu"], cfg["prior_sigma"], cfg["math"], cfg["kl_convention"], cfg["act"], fold=fold,
+                         first_image=first_image)
+        if lib.bbb_forward_supported(C.byref(d)) != 0:
+            return False
+        # the first layer's input is data (no input gradient); a later layer's input comes out of a layer
+        if Fn._fold_grad_refusal(cfg, xs, tuple(m.W_mu.shape), i > 0) is not None:
+            return False
+    return True
+
+
+def train_fold_kl_weights(groups, beta: float, num_ens: int):
+    """The gradient each group's KL term gets in a folded training step: every sample has the same KL, which a folded
+    pass computes once, so a group of n samples carries n * beta / S (the sample loop gives each sample beta / S)."""
+    return [n * float(beta) / float(num_ens) for _, n in groups]
+
+
 class MCTrainStep(MCForward):
     """One SHARDED training step with main_bayesian.train_model's semantics (main_bayesian.py:38-58): every rank runs
     its share of the ``num_ens`` weight samples WITH autograd (layer forward kernels + the engine's backward kernels),
@@ -852,13 +901,32 @@ class MCTrainStep(MCForward):
     ``batch_shards=Rb`` (MCForward): rank (g, k) back-propagates its samples on its row block only -- d loss / d logits
     keeps the global B (train_size / B) and uses the combined log_outputs rows of the block, the beta/S KL gradient is
     added by the block-0 rank of each group -- and the same all-reduce sums the gradients.  With num_ens = 1 (the
-    reference's default) and Rb = world this is a data-parallel step."""
+    reference's default) and Rb = world this is a data-parallel step.
 
-    def __init__(self, net, example_x, num_ens, train_size, group=None, seed=None, batch_shards: int = 1):
+    ``fold=True`` folds the local samples into grouped passes, forward and backward: groups of G consecutive local
+    samples (layer_fold_groups; ``fold_group`` caps G) each run ONE forward and ONE backward of the per-layer
+    tensor-core kernels over G x rows images (Fn.layer_fold(grad=True)) instead of G of each.  It folds when every
+    Bayesian layer is LRT, the math mode is a tensor-core one, every child treats each image on its own, and the engine
+    accepts every layer's folded forward and every contraction of its backward at the group's row count; otherwise the
+    step runs the sample loop.  ``layer_fold`` = (G, number of groups), or None for the sample loop.  The per-sample
+    logits, log_outputs, kl and head are bitwise those of the sample loop; the gradients differ only in the order their
+    sums are taken.  The input x gets no gradient in a folded step (a pass reads x repeated G times, a copy).  Memory: the budget (LAYER_FOLD_BUDGET) bounds the activations of one pass, not the step's -- the
+    loss gradient needs p_bar, which depends on every sample, so the autograd graph of every group lives until the
+    exchange, and the step holds as much as the sample loop does."""
+
+    def __init__(self, net, example_x, num_ens, train_size, group=None, seed=None, batch_shards: int = 1,
+                 fold: bool = False, fold_group: Optional[int] = None):
         super().__init__(net, example_x, num_ens, group=group, with_labels=True, train_size=train_size, seed=seed,
                          graph=False, fold=False, batch_shards=batch_shards)
         self.params = [p for p in net.parameters() if p.requires_grad]
         self.steps = 0
+        if fold and len(self.ids) > 1:
+            self._groups = train_fold_groups(net, (self.nb,) + tuple(example_x.shape[1:]), len(self.ids),
+                                             self.sample_shards << 40, self.rows[0], fold_group)
+        if self._groups is not None:
+            G = max(n for _, n in self._groups)
+            self.layer_fold = (G, len(self._groups))
+            self.xrep = torch.empty((G * self.nb,) + tuple(example_x.shape[1:]), dtype=example_x.dtype, device=self.dev)
 
     def __call__(self, x, labels, beta: float = 0.0):
         from .graph import _STRIDE
@@ -869,12 +937,26 @@ class MCTrainStep(MCForward):
         logits, kls = [], []
         b0, b1 = self.rows
         xb = x[b0:b1]                                                  # this rank's row block
-        for k, j in enumerate(self.ids):
-            with Fn.mc_sample(j, self.seed, offset=self.steps * _STRIDE), Fn.first_image(b0):
-                lg, kl = self.net(xb)                                  # autograd on: per-layer kernels (no fused chain)
-            logits.append(lg)
-            kls.append(kl)
-            self.logits[k].copy_(lg.detach().reshape(self.nb, self.C))
+        if self._groups is not None:
+            # group (s0, n): local samples s0 .. s0+n-1 in one pass over n x nb rows (stream stride Rs << 40, as in
+            # MCForward's per-layer fold); logits[i] holds the n samples of group i, one nb-row block each
+            G, nb = self.layer_fold[0], self.nb
+            with torch.no_grad():
+                self.xrep.view((G,) + tuple(xb.shape)).copy_(xb.unsqueeze(0).expand((G,) + tuple(xb.shape)))
+            for s0, n in self._groups:
+                with Fn.mc_sample(self.ids[s0], self.seed, offset=self.steps * _STRIDE), Fn.first_image(b0), \
+                        Fn.layer_fold(nb, self.sample_shards << 40, grad=True):
+                    lg, kl = self.net(self.xrep[:n * nb])
+                logits.append(lg)
+                kls.append(kl)
+                self.logits[s0:s0 + n].view(n * nb, self.C).copy_(lg.detach().reshape(n * nb, self.C))
+        else:
+            for k, j in enumerate(self.ids):
+                with Fn.mc_sample(j, self.seed, offset=self.steps * _STRIDE), Fn.first_image(b0):
+                    lg, kl = self.net(xb)                              # autograd on: per-layer kernels (no fused chain)
+                logits.append(lg)
+                kls.append(kl)
+                self.logits[k].copy_(lg.detach().reshape(self.nb, self.C))
         kl_ptr, n_kl = None, 0
         if self.ids:
             self.kl_one.copy_(kls[0].detach())
@@ -891,16 +973,25 @@ class MCTrainStep(MCForward):
             # ratio in log space; the others keep the direct quotient, exact to fp32 rounding there.
             in_range = log_p_bar_y > _LOG_P_DIRECT_MIN
             grads = []
-            for lg in logits:
-                lg = lg.detach().float()
-                sm = torch.softmax(lg, dim=1)
-                w = torch.where(in_range, sm.gather(1, idx) / (S * p_bar_y),
-                                (torch.log_softmax(lg, dim=1).gather(1, idx) - log_p_bar_y - math.log(S)).exp())
-                onehot = torch.zeros_like(sm).scatter_(1, idx, 1.0)
-                grads.append((-(self.train_size / self.B)) * w * (onehot - sm))
-            # the KL does not depend on the rows: one block per sample group adds its gradient
-            kl_t = [k_ for k_ in kls if torch.is_tensor(k_) and k_.requires_grad] if self.block == 0 else []
-            kl_g = [torch.full_like(k_, self.beta / S) for k_ in kl_t]
+            for lg_all in logits:
+                lg_all = lg_all.detach().float()
+                blocks = []
+                for r0 in range(0, lg_all.shape[0], self.nb):              # one sample per block of nb rows
+                    lg = lg_all[r0:r0 + self.nb]
+                    sm = torch.softmax(lg, dim=1)
+                    w = torch.where(in_range, sm.gather(1, idx) / (S * p_bar_y),
+                                    (torch.log_softmax(lg, dim=1).gather(1, idx) - log_p_bar_y - math.log(S)).exp())
+                    onehot = torch.zeros_like(sm).scatter_(1, idx, 1.0)
+                    blocks.append((-(self.train_size / self.B)) * w * (onehot - sm))
+                grads.append(blocks[0] if len(blocks) == 1 else torch.cat(blocks))
+            # the KL does not depend on the rows: one block per sample group adds its gradient, n * beta / S for a
+            # folded group of n samples
+            wkl = train_fold_kl_weights(self._groups, self.beta, self.num_ens) if self._groups is not None else \
+                [self.beta / S] * len(kls)
+            kl_t = [(k_, w_) for k_, w_ in zip(kls, wkl) if torch.is_tensor(k_) and k_.requires_grad] \
+                if self.block == 0 else []
+            kl_g = [torch.full_like(k_, w_) for k_, w_ in kl_t]
+            kl_t = [k_ for k_, _ in kl_t]
             torch.autograd.backward(logits + kl_t, grads + kl_g)
         if self.world > 1:                                                  # ONE collective: the summed parameter gradients
             for p in self.params:
