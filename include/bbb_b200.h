@@ -64,7 +64,9 @@ typedef struct bbb_layer_desc {
     int32_t variant;        /* BBB_VARIANT_*                                          */
     int32_t sample;         /* 1: stochastic (self.training or sample); 0: mean only */
     int32_t has_bias;
-    int32_t act_dtype;      /* BBB_DTYPE_*: dtype of x and y                          */
+    int32_t act_dtype;      /* BBB_DTYPE_*: dtype of x and y.  BF16: per-layer forward on
+                               BBB_MATH_BF16_TC (or AUTO resolving to it) only; act_std,
+                               KL and parameters stay fp32; backward takes F32 only     */
     int32_t math;           /* BBB_MATH_*                                             */
     int32_t kl_convention;  /* BBB_KL_*                                               */
     int32_t epilogue_act;   /* BBB_ACT_*: activation fused after the layer (0 = none) */
@@ -81,7 +83,12 @@ size_t bbb_workspace_bytes(const bbb_layer_desc* desc);
 
 /* Replaces BBBConv2d.forward + .kl_loss:
  *   layers/BBB/BBBConv.py:61-83, layers/BBB_LRT/BBBConv.py:62-87.
- * y      : [batch, out_channels, OH, OW]
+ * x, y   : [batch, in_channels, H, W] / [batch, out_channels, OH, OW], fp32, or bf16 with act_dtype = BBB_DTYPE_BF16.
+ *          bf16 activations need BBB_MATH_BF16_TC (or AUTO resolving to it; BBB_E_UNSUPPORTED on FP32 / TF32_TC): the
+ *          kernel multiplies the bf16 x it reads (x^2 of the LRT variance plane is formed from it) and rounds the fp32
+ *          output it computes once (round to nearest even) into y.  Tile schedule, accumulation order, noise, folds and
+ *          KL are those of the fp32-I/O call, so on a bf16-representable x, y is bf16(y of the fp32-I/O call) bit for bit
+ *          and act_std and the KL are equal.
  * kl_out : nullable; the layer's KL scalar (weights + bias) is WRITTEN here.
  * act_std: nullable, LRT only, fp32 shape of y: sqrt(act_var) (BBB_LRT/BBBConv.py:75)
  *          saved for the backward.
@@ -135,9 +142,10 @@ int bbb_linear_forward(const bbb_layer_desc* desc, const void* x,
                        void* workspace, size_t workspace_bytes, void* cuda_stream);
 
 /* Host-only query (no GPU work, no GPU needed): would bbb_conv2d_forward / bbb_linear_forward accept this desc, its
- * MC-sample fold (reserved[1..3]) included?  Returns BBB_OK or the error code the call would return
- * (bbb_last_error() says why); pointer, external-eps and workspace checks are the call's own.  The host side asks
- * before it folds a net's samples on the per-layer path. */
+ * MC-sample fold (reserved[1..3]) and activation dtype included?  Returns BBB_OK or the error code the call would return
+ * (bbb_last_error() says why); pointer, external-eps and workspace checks are the call's own.  A bf16 desc gets the
+ * answer of the fp32 one on BBB_MATH_BF16_TC and on AUTO resolving to it, BBB_E_UNSUPPORTED otherwise.  The host side
+ * asks before it folds a net's samples on the per-layer path, and before it sends a bf16 input as bf16. */
 int bbb_forward_supported(const bbb_layer_desc* desc);
 
 /* Activation layouts of the fused tensor-core chain (bbb_layer_forward_fused). */

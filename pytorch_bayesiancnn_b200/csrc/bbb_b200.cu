@@ -92,10 +92,13 @@ int check_desc(const bbb_layer_desc* d, bbb::Geom& g, bool linear) {
 // Pool, math-mode and shape checks of the per-layer forward (host logic only); `math` = the resolved BBB_MATH_*.
 int layer_math(const bbb_layer_desc* d, const bbb::Geom& g, int& math) {
     if (d->pool_k != 0) return fail(BBB_E_UNSUPPORTED, "fused max-pool epilogue is not available on this path");
+    if (d->act_dtype != BBB_DTYPE_F32 && d->act_dtype != BBB_DTYPE_BF16) return fail(BBB_E_UNSUPPORTED, "bad act_dtype %d", d->act_dtype);
     math = d->math;
-    if (math == BBB_MATH_AUTO) math = bbb::tc_supported(*d, g) ? BBB_MATH_BF16_TC : BBB_MATH_FP32;
+    if (math == BBB_MATH_AUTO) math = bbb::tc_supported(g) ? BBB_MATH_BF16_TC : BBB_MATH_FP32;
     if (math == BBB_MATH_BF16_TC || math == BBB_MATH_TF32_TC) {
-        if (!bbb::tc_supported(*d, g)) return fail(BBB_E_UNSUPPORTED, "tensor-core math mode: shape not supported by the tensor-core path");
+        if (!bbb::tc_supported(g)) return fail(BBB_E_UNSUPPORTED, "tensor-core math mode: shape not supported by the tensor-core path");
+        if (math == BBB_MATH_TF32_TC && d->act_dtype != BBB_DTYPE_F32)
+            return fail(BBB_E_UNSUPPORTED, "bf16 activations take bf16 operands (BBB_MATH_BF16_TC), not tf32");
         return BBB_OK;
     }
     if (math != BBB_MATH_FP32) return fail(BBB_E_INVALID, "bad math mode %d", d->math);
@@ -300,7 +303,8 @@ static int fused_check(const bbb_layer_desc* d, bbb::Geom& g, int32_t in_layout,
         if (in_layout == BBB_LAYOUT_NCHW_F32 && !s4) return fail(BBB_E_UNSUPPORTED, "MC-sample folding is not available on the gather path");
     }
     if (in_layout == BBB_LAYOUT_NCHW_F32) {
-        if (!bbb::tc_supported(*d, g)) return fail(BBB_E_UNSUPPORTED, "shape not supported by the tensor-core gather path");
+        if (d->act_dtype != BBB_DTYPE_F32) return fail(BBB_E_UNSUPPORTED, "the tensor-core gather path takes fp32 activations only");
+        if (!bbb::tc_supported(g)) return fail(BBB_E_UNSUPPORTED, "shape not supported by the tensor-core gather path");
         if (out_mode == 1 && (pool ? g.OHW / 4 : g.OHW) != 1) return fail(BBB_E_UNSUPPORTED, "row-major fp32 output needs a 1x1 map on the gather path");
     } else if (in_layout == BBB_LAYOUT_PACKED_BF16) {
         if (!bbb::fused_supported(g, pool)) return fail(BBB_E_UNSUPPORTED, "shape not supported by the fused tap-GEMM path");

@@ -36,7 +36,7 @@ namespace bbb {
 // wtiles: [n_tiles][k_blocks][planes][8 KB tile]  (64 rows x 8 K chunks of 16 bytes: 64 bf16 or 32 tf32 of K)
 struct TcArgs : LayerArgs {
     const void* x; void* y; float* act_std;
-    int act_dtype;
+    int act_dtype;           // BBB_DTYPE_BF16: x and y (NCHW) are bf16 (per-layer calls with bf16 operands only)
     int n_tiles, k_blocks;
     int skip_prep, prep_only;
     int tf32;                // operands as tf32 (fp32 storage, 4 elements per 16-byte K chunk, kind::tf32) instead of bf16
@@ -72,8 +72,8 @@ inline size_t tc_workspace_bytes(const Geom& g) {
     // the tf32 layout, never smaller than the bf16 one
     return tc_bias_offset(g, true) + (size_t)2 * tc_npad(g) * 4;
 }
-inline bool tc_supported(const bbb_layer_desc& d, const Geom& g) {
-    if (d.act_dtype != BBB_DTYPE_F32) return false;
+// Shape checks only: the activation dtype does not change the tile schedule (the callers check it).
+inline bool tc_supported(const Geom& g) {
     if (g.M < 1 || g.N < 1) return false;
     if (tc_stages(g, 2) < 2) return false;
     if ((long)tc_npad(g) / TC_BN * (tc_kpad(g, true) / tc_bk(true)) > 1 << 20) return false;
@@ -443,11 +443,14 @@ __host__ __device__ inline int tc_tile_images(int OHW) {
 
 // TWO: the LRT variance plane (x^2 against sigma^2) is multiplied as well (planes == 2).  A compile-time flag: a runtime
 // branch around the second wgmma makes ptxas serialize every wgmma of the loop.
-template <int VARIANT, bool TF32, bool TWO>
+// BF16IO: x and y are bf16 NCHW (act_dtype = BBB_DTYPE_BF16).  The operands are the bf16 values an fp32 x rounds to,
+// and the epilogue rounds the same fp32 value once: everything but the loads and stores is the fp32-I/O kernel's.
+template <int VARIANT, bool TF32, bool TWO, bool BF16IO = false>
 __global__ void __launch_bounds__(TC_THREADS, 2)
 gemm_tc_kernel(const TcArgs p, const int stages) {
     constexpr bool LRT = VARIANT == BBB_VARIANT_LRT;
     static_assert(LRT || !TWO, "only the LRT variant has a variance plane");
+    static_assert(!(TF32 && BF16IO), "bf16 activations are multiplied as bf16 operands");
     constexpr int CE = TF32 ? 4 : 8, BKE = 8 * CE;                  // elements per 16-byte chunk / per K block
     extern __shared__ uint8_t smem_raw[];
     const Geom& g = p.g;
@@ -500,7 +503,15 @@ gemm_tc_kernel(const TcArgs p, const int stages) {
         const int nflt = (last - img0 + 1) * chw;
         const float* src = reinterpret_cast<const float*>(p.x) + (size_t)img0 * chw;
         const bool vec = ((reinterpret_cast<uintptr_t>(src) | (uintptr_t)(nflt * 4)) & 15u) == 0;
-        if (p.stage_x == 2) {
+        if (BF16IO) {                                   // bf16 input (always staged as bf16): a plain copy
+            const __nv_bfloat16* hsrc = reinterpret_cast<const __nv_bfloat16*>(p.x) + (size_t)img0 * chw;
+            if (((reinterpret_cast<uintptr_t>(hsrc) | (uintptr_t)(nflt * 2)) & 15u) == 0) {
+                for (int i = threadIdx.x; i < (nflt >> 3); i += blockDim.x)
+                    reinterpret_cast<uint4*>(xsh)[i] = __ldg(reinterpret_cast<const uint4*>(hsrc) + i);
+            } else {
+                for (int i = threadIdx.x; i < nflt; i += blockDim.x) xsh[i] = hsrc[i];
+            }
+        } else if (p.stage_x == 2) {
             if (vec) {
                 for (int i = threadIdx.x; i < (nflt >> 2); i += blockDim.x) {
                     const float4 v = __ldg(reinterpret_cast<const float4*>(src) + i);
@@ -556,6 +567,11 @@ gemm_tc_kernel(const TcArgs p, const int stages) {
             xb = (long)(p.stage_x ? bimg - img0 : bimg) * chw + (long)ih0 * g.W + iw0;
         }
         const float* __restrict__ xp = p.stage_x ? xs : reinterpret_cast<const float*>(p.x);
+        // BF16IO: one pointer to the staged images or to x.  With it the two-plane (LRT sampling) instantiation spills a few
+        // words inside the K loop (ptxas: 36 B stored, 60 B loaded; the fp32-I/O one spills 16 / 8 B too).  Branching on
+        // stage_x per element instead removes the spills, but the BBB3Conv3FC B = 2048 forward then took 5.74 ms instead of
+        // 3.94-4.00 ms (H100 80GB HBM3, 700 W power limit, tools/bf16_act_bench.py).
+        const __nv_bfloat16* __restrict__ xhp = p.stage_x ? xsh : reinterpret_cast<const __nv_bfloat16*>(p.x);
         float acc[32], acc2[32];
 #pragma unroll
         for (int i = 0; i < 32; ++i) { acc[i] = 0.0f; acc2[i] = 0.0f; }
@@ -572,8 +588,10 @@ gemm_tc_kernel(const TcArgs p, const int stages) {
                     const int2 kt = ktab[kb * BKE + c8 * CE + e];
                     const int ih = ih0 + (kt.y >> 16), iw = iw0 + (kt.y & 0xffff);
                     float val = 0.0f;
-                    if (mvalid && (unsigned)ih < (unsigned)g.H && (unsigned)iw < (unsigned)g.W)
-                        val = (p.stage_x == 2) ? __bfloat162float(xsh[xb + kt.x]) : xp[xb + kt.x];
+                    if (mvalid && (unsigned)ih < (unsigned)g.H && (unsigned)iw < (unsigned)g.W) {
+                        if (BF16IO) val = __bfloat162float(xhp[xb + kt.x]);
+                        else val = (p.stage_x == 2) ? __bfloat162float(xsh[xb + kt.x]) : xp[xb + kt.x];
+                    }
                     v[e] = val;
                 }
                 *reinterpret_cast<uint4*>(st + a_off + c8 * (TC_BM * 16) + t * 16) = pack_chunk<TF32>(v);
@@ -683,7 +701,9 @@ gemm_tc_kernel(const TcArgs p, const int stages) {
                 for (int j = 0; j < 8; ++j) {
                     const int n = nb + j;
                     if (n >= g.N) continue;
-                    reinterpret_cast<float*>(p.y)[((size_t)bimg * g.N + n) * ohw_out + opix] = am[j];
+                    const size_t o = ((size_t)bimg * g.N + n) * ohw_out + opix;
+                    if (BF16IO) reinterpret_cast<__nv_bfloat16*>(p.y)[o] = __float2bfloat16_rn(am[j]);
+                    else reinterpret_cast<float*>(p.y)[o] = am[j];
                 }
             }
         }
@@ -740,6 +760,10 @@ inline cudaError_t launch_fwd_tc_t(TcArgs a, cudaStream_t st, int* n_launch) {
     const size_t tiles_off = (1024 + (size_t)tc_kpad(g, TF32) * 8 + 1023) / 1024 * 1024;
     size_t smem = 1023 + tiles_off + (size_t)stages * tc_stage_bytes(a.planes);
     const size_t xs_elems = (size_t)tc_tile_images(g.OHW) * g.Cin * g.HW;
+    // bf16 activations (never with tf32 operands: the caller refuses them) stage wherever fp32 ones would, always as bf16.
+    // Staging by the bf16 footprint (xs_elems * 2 <= 32 KB) would stage more layers (BBB3Conv3FC conv2); it is not done:
+    // its effect is unmeasured, and this way a bf16 call and an fp32 one gather the same layers from the same memory.
+    const bool bf16io = !TF32 && a.act_dtype == BBB_DTYPE_BF16;
     a.stage_x = 0;
     if (xs_elems * 4 <= 32 * 1024 && smem + xs_elems * 4 <= (size_t)TC_SMEM_LIMIT) {
         a.stage_x = 1;
@@ -747,10 +771,14 @@ inline cudaError_t launch_fwd_tc_t(TcArgs a, cudaStream_t st, int* n_launch) {
         // (never for tf32 operands: the staged copy would already have lost the bits tf32 keeps)
         const size_t per_sm = 228 * 1024;
         if (!TF32 && 2 * (smem + xs_elems * 4 + 1024) > per_sm && 2 * ((smem + xs_elems * 2 + 127) / 128 * 128 + 1024) <= per_sm) a.stage_x = 2;
+        if (bf16io) a.stage_x = 2;
         smem += xs_elems * (a.stage_x == 2 ? 2 : 4);
     }
     dim3 grid((g.M - 1) / TC_BM + 1, a.n_tiles);       // not (M + TC_BM - 1): M may lie near 2^31
-    auto* kernel = a.planes == 2 ? gemm_tc_kernel<VARIANT, TF32, VARIANT == BBB_VARIANT_LRT> : gemm_tc_kernel<VARIANT, TF32, false>;
+    // (!TF32 as BF16IO: a tf32 launcher names the fp32-I/O kernel twice rather than a bf16-I/O tf32 one)
+    constexpr bool LRT = VARIANT == BBB_VARIANT_LRT;
+    auto* kernel = bf16io ? (a.planes == 2 ? gemm_tc_kernel<VARIANT, TF32, LRT, !TF32> : gemm_tc_kernel<VARIANT, TF32, false, !TF32>)
+                          : (a.planes == 2 ? gemm_tc_kernel<VARIANT, TF32, LRT> : gemm_tc_kernel<VARIANT, TF32, false>);
     cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
     cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;

@@ -471,12 +471,30 @@ def _fold_grad_refusal(cfg, x_shape, w_shape, need_x) -> Optional[str]:
     return None if why is None else f"the backward would leave the tensor cores: {why}"
 
 
+def layer_io(d: L.LayerDesc, x_dtype: torch.dtype) -> tuple[bool, torch.dtype]:
+    """(bf16 activations, y dtype) of a layer call of desc ``d`` on an input of ``x_dtype``; sets ``d.act_dtype``.
+    A bf16 input on math 'bf16' or 'auto' keeps its dtype: the engine reads bf16 x and writes bf16 y (act_dtype =
+    BBB_DTYPE_BF16) wherever it accepts that desc (bbb_forward_supported, host-only), and otherwise the call runs on the
+    upcast input and y is rounded to bf16 -- so y is bf16 either way.  Any other input (and a bf16 one on 'fp32' or
+    'tf32') runs as fp32, with an fp32 y."""
+    d.act_dtype = L.DTYPE_F32
+    if x_dtype != torch.bfloat16 or d.math not in (L.MATH_BF16_TC, L.MATH_AUTO):
+        return False, torch.float32
+    d.act_dtype = L.DTYPE_BF16
+    if L.lib().bbb_forward_supported(C.byref(d)) == 0:
+        return True, torch.bfloat16
+    d.act_dtype = L.DTYPE_F32
+    return False, torch.bfloat16
+
+
 # --------------------------------------------------------------------------- #
 # the layer op
 # --------------------------------------------------------------------------- #
 class BayesLayerFn(torch.autograd.Function):
     """(y, kl) = layer(x; W_mu, W_rho, bias_mu, bias_rho).  One fused kernel forward;
-    backward = bbb_*_backward + bbb_kl_backward accumulating into the same grads."""
+    backward = bbb_*_backward + bbb_kl_backward accumulating into the same grads.
+    A bf16 x on math 'bf16' / 'auto' gives a bf16 y (layer_io) and is saved as bf16; the backward runs on it and gy
+    upcast to fp32 (both exact) and returns gx in x's dtype; parameter gradients and KL are fp32."""
 
     @staticmethod
     def forward(ctx, x, W_mu, W_rho, bias_mu, bias_rho, cfg):
@@ -487,8 +505,7 @@ class BayesLayerFn(torch.autograd.Function):
         conv = cfg["conv"]
         variant, sample = cfg["variant"], cfg["sample"]
         x = x.contiguous()
-        if x.dtype != torch.float32:
-            x = x.float()
+        x_dtype = x.dtype
         W_mu_c, W_rho_c = W_mu.contiguous(), W_rho.contiguous()
         has_bias = bias_mu is not None
         need_grad = any(ctx.needs_input_grad[:5])      # grad mode is off inside Function.forward
@@ -504,6 +521,9 @@ class BayesLayerFn(torch.autograd.Function):
         d = make_desc(tuple(x.shape), tuple(W_mu.shape), conv, variant, sample, has_bias,
                       cfg["prior_mu"], cfg["prior_sigma"], cfg["math"], cfg["kl_convention"], cfg["act"], fold=fold,
                       first_image=_noise.first_image)
+        bf16_io, y_dtype = layer_io(d, x_dtype)
+        if not bf16_io and x.dtype != torch.float32:
+            x = x.float()
         if conv is None:
             if x.dim() != 2 or x.shape[1] != W_mu.shape[1]:
                 raise L.EngineError(f"linear: x {tuple(x.shape)} vs weight {tuple(W_mu.shape)}")
@@ -513,7 +533,7 @@ class BayesLayerFn(torch.autograd.Function):
                 raise L.EngineError(f"conv2d: x {tuple(x.shape)} vs weight {tuple(W_mu.shape)}")
             oh, ow = out_hw(x.shape[2], x.shape[3], W_mu.shape[2], W_mu.shape[3], conv)
             yshape = (x.shape[0], W_mu.shape[0], oh, ow)
-        y = torch.empty(yshape, dtype=torch.float32, device=dev)
+        y = torch.empty(yshape, dtype=x.dtype, device=dev)
         kl = torch.empty((), dtype=torch.float32, device=dev)
         eps_a = eps_b = None
         seed = stream_id = 0
@@ -538,8 +558,12 @@ class BayesLayerFn(torch.autograd.Function):
                 _ptr(y), _ptr(kl), _ptr(act_std), _ptr(eps_a), _ptr(eps_b),
                 C.c_uint64(seed), C.c_uint64(stream_id), _ptr(base), _ptr(ws), C.c_size_t(ws.numel()), _stream(dev))
         L.check(rc, "bbb_linear_forward" if conv is None else "bbb_conv2d_forward")
+        if y.dtype != y_dtype:                      # a bf16 input the engine took as fp32
+            y = y.to(y_dtype)
+        d.act_dtype = L.DTYPE_F32                   # the backward runs on x and gy upcast to fp32
         ctx.cfg = cfg
         ctx.desc = d
+        ctx.x_dtype = x_dtype
         ctx.noise = (seed, stream_id, base)
         ctx.first_image = _noise.first_image
         ctx.fold = fold
@@ -580,6 +604,7 @@ class BayesLayerFn(torch.autograd.Function):
                 done = True
         if gy is not None and not done:
             gy = gy.contiguous().float()
+            x = x.float()                                  # a saved bf16 x: exact (_backward_tc upcasts its own)
             if ctx.needs_input_grad[0]:
                 gx = torch.zeros_like(x)
             ws = workspace(dev)
@@ -590,6 +615,8 @@ class BayesLayerFn(torch.autograd.Function):
                     _ptr(gx), _ptr(g_W_mu), _ptr(g_W_rho), _ptr(g_b_mu), _ptr(g_b_rho),
                     _ptr(ws), C.c_size_t(ws.numel()), _stream(dev))
             L.check(rc, "bbb_*_backward")
+        if gx is not None and gx.dtype != ctx.x_dtype:
+            gx = gx.to(ctx.x_dtype)
         if gkl is not None:
             gkl = gkl.contiguous().float()
             rc = lib.bbb_kl_backward(_ptr(W_mu), _ptr(W_rho), C.c_uint64(W_mu.numel()),
@@ -615,6 +642,7 @@ class BayesLayerFn(torch.autograd.Function):
         LRT: the noise term's gradient gv = gy * eps / (2 act_std) is one kernel (bbb_lrt_noise_grad) on the forward's
         desc, folded or not, which reads the stream base on the device."""
         x, W_mu, W_rho, bias_mu, bias_rho, act_std, eps_a, eps_b = ctx.saved_tensors
+        x = x.float()
         cfg = ctx.cfg
         conv, variant, sample = cfg["conv"], cfg["variant"], cfg["sample"]
         dev = x.device

@@ -974,7 +974,7 @@ class MCTrainStep(MCForward):
             in_range = log_p_bar_y > _LOG_P_DIRECT_MIN
             grads = []
             for lg_all in logits:
-                lg_all = lg_all.detach().float()
+                lg_dtype, lg_all = lg_all.dtype, lg_all.detach().float()
                 blocks = []
                 for r0 in range(0, lg_all.shape[0], self.nb):              # one sample per block of nb rows
                     lg = lg_all[r0:r0 + self.nb]
@@ -983,7 +983,8 @@ class MCTrainStep(MCForward):
                                     (torch.log_softmax(lg, dim=1).gather(1, idx) - log_p_bar_y - math.log(S)).exp())
                     onehot = torch.zeros_like(sm).scatter_(1, idx, 1.0)
                     blocks.append((-(self.train_size / self.B)) * w * (onehot - sm))
-                grads.append(blocks[0] if len(blocks) == 1 else torch.cat(blocks))
+                # bf16 logits (bf16 activations) take their gradient in bf16, as autograd would cast it
+                grads.append((blocks[0] if len(blocks) == 1 else torch.cat(blocks)).to(lg_dtype))
             # the KL does not depend on the rows: one block per sample group adds its gradient, n * beta / S for a
             # folded group of n samples
             wkl = train_fold_kl_weights(self._groups, self.beta, self.num_ens) if self._groups is not None else \

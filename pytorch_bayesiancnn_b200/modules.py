@@ -84,6 +84,8 @@ class ModuleWrapper(nn.Module):
         if out is not None:
             # the fused chain already reduced the per-layer KL scalars (each layer's kl_loss() still
             # returns its own term); same value as the loop below, one launch instead of one per layer
+            if x.dtype == torch.bfloat16:                  # the chain upcasts a bf16 input once: bf16 in, bf16 out
+                return out[0].to(torch.bfloat16), out[1]
             return out
         for child in self.children():
             x = child(x)
