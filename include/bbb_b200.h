@@ -75,6 +75,21 @@ typedef struct bbb_layer_desc {
     float prior_mu, prior_sigma;
 } bbb_layer_desc;
 
+/* Per-element Gaussian prior N(mu_p, sigma_p^2) of one layer, for the *_prior entry points below: the KL of each
+ * parameter element is taken against its own (mu_p, sigma_p) instead of (desc->prior_mu, desc->prior_sigma) -- a previous
+ * task's posterior (variational continual learning), or a prior centred on pretrained weights.  fp32 DEVICE pointers,
+ * contiguous, in the layout of W_mu (OIHW / [out, in]) and of bias_mu ([out_channels]).  All four are read only where
+ * a KL is computed (kl_out != NULL); noise, MC-sample folds, operand tiles and outputs do not depend on them.
+ * sigma_p > 0 (and finite) is the caller's contract: the device does not check it.
+ * A prior is all tensors: w_mu and w_sigma are required, b_mu and b_sigma too when the layer has a bias (else
+ * BBB_E_INVALID); a caller with a scalar part fills a tensor with it.  prior == NULL is the scalar call of the
+ * entry point without _prior (the same kernels, the same bits); a tensor prior filled with desc->prior_mu /
+ * desc->prior_sigma gives that call's KL bit for bit (same kernels' summation order). */
+typedef struct bbb_prior {
+    const float* w_mu;  const float* w_sigma;   /* layout of W_mu (OIHW / [out, in]); sigma > 0 */
+    const float* b_mu;  const float* b_sigma;   /* [out_channels]; required iff has_bias      */
+} bbb_prior;
+
 /* Bytes of caller-allocated scratch a forward/KL call on `desc` needs.  The
  * scratch must be zero-filled ONCE when allocated; calls leave it zeroed where
  * that matters (self-resetting counters).  A desc that folds the MC samples of a BBB layer
@@ -141,6 +156,23 @@ int bbb_linear_forward(const bbb_layer_desc* desc, const void* x,
                        uint64_t seed, uint64_t stream_id, const uint64_t* stream_base,
                        void* workspace, size_t workspace_bytes, void* cuda_stream);
 
+/* bbb_conv2d_forward / bbb_linear_forward with the layer's KL (kl_out) taken against the per-element prior `prior`
+ * (bbb_prior; NULL = the scalar call).  y, act_std and every other output are those of the scalar call. */
+int bbb_conv2d_forward_prior(const bbb_layer_desc* desc, const void* x,
+                             const float* W_mu, const float* W_rho,
+                             const float* bias_mu, const float* bias_rho,
+                             void* y, float* kl_out, float* act_std,
+                             const float* eps_a, const float* eps_b,
+                             uint64_t seed, uint64_t stream_id, const uint64_t* stream_base,
+                             void* workspace, size_t workspace_bytes, void* cuda_stream, const bbb_prior* prior);
+int bbb_linear_forward_prior(const bbb_layer_desc* desc, const void* x,
+                             const float* W_mu, const float* W_rho,
+                             const float* bias_mu, const float* bias_rho,
+                             void* y, float* kl_out, float* act_std,
+                             const float* eps_a, const float* eps_b,
+                             uint64_t seed, uint64_t stream_id, const uint64_t* stream_base,
+                             void* workspace, size_t workspace_bytes, void* cuda_stream, const bbb_prior* prior);
+
 /* Host-only query (no GPU work, no GPU needed): would bbb_conv2d_forward / bbb_linear_forward accept this desc, its
  * MC-sample fold (reserved[1..3]) and activation dtype included?  Returns BBB_OK or the error code the call would return
  * (bbb_last_error() says why); pointer, external-eps and workspace checks are the call's own.  A bf16 desc gets the
@@ -191,6 +223,16 @@ int bbb_layer_forward_fused(const bbb_layer_desc* desc,
                             float* kl_out, const float* eps_a, const float* eps_b,
                             uint64_t seed, uint64_t stream_id, const uint64_t* stream_base,
                             void* workspace, size_t workspace_bytes, void* cuda_stream);
+/* bbb_layer_forward_fused with the KL taken against the per-element prior `prior` (bbb_prior; NULL = the scalar call).
+ * Only the weight-prep kernel reads it (a BBB_FUSED_SKIP_PREP call computes no KL and ignores it). */
+int bbb_layer_forward_fused_prior(const bbb_layer_desc* desc,
+                                  const void* x, const void* x_sq, int32_t in_layout, int32_t in_pitch, int32_t prev_hw,
+                                  const float* W_mu, const float* W_rho,
+                                  const float* bias_mu, const float* bias_rho,
+                                  void* y, void* y_sq, int32_t out_layout, int32_t out_pitch,
+                                  float* kl_out, const float* eps_a, const float* eps_b,
+                                  uint64_t seed, uint64_t stream_id, const uint64_t* stream_base,
+                                  void* workspace, size_t workspace_bytes, void* cuda_stream, const bbb_prior* prior);
 
 /* Host-only query (no GPU work, no GPU needed): would bbb_layer_forward_fused accept this layer with these layouts?
  * Returns BBB_OK, or the error code the call would return (bbb_last_error() says why).  The host-side planner
@@ -206,11 +248,26 @@ int bbb_kl_forward(const float* W_mu, const float* W_rho, uint64_t n_w,
                    float prior_mu, float prior_sigma, int32_t kl_convention,
                    float* kl_out, void* workspace, size_t workspace_bytes, void* cuda_stream);
 
+/* bbb_kl_forward against the per-element prior `prior` (bbb_prior over W_mu's n_w and bias_mu's n_b elements; the
+ * bias pointers are required when n_b > 0).  prior_mu / prior_sigma are then not used; NULL = bbb_kl_forward. */
+int bbb_kl_forward_prior(const float* W_mu, const float* W_rho, uint64_t n_w,
+                         const float* bias_mu, const float* bias_rho, uint64_t n_b,
+                         float prior_mu, float prior_sigma, int32_t kl_convention,
+                         float* kl_out, void* workspace, size_t workspace_bytes, void* cuda_stream,
+                         const bbb_prior* prior);
+
 /* d(kl)/d(mu), d(kl)/d(rho), scaled by *grad_kl (device scalar) and ACCUMULATED
  * into g_mu / g_rho (SURVEY.md Appendix A). */
 int bbb_kl_backward(const float* mu, const float* rho, uint64_t n,
                     float prior_mu, float prior_sigma, int32_t kl_convention,
                     const float* grad_kl, float* g_mu, float* g_rho, void* cuda_stream);
+/* bbb_kl_backward of n elements (a weight tensor, or a bias) against the per-element prior prior->w_mu / prior->w_sigma,
+ * laid out like mu (b_mu / b_sigma are not read: for a bias, pass its prior in the w_ fields).  No gradient flows to
+ * the prior.  NULL = bbb_kl_backward. */
+int bbb_kl_backward_prior(const float* mu, const float* rho, uint64_t n,
+                          float prior_mu, float prior_sigma, int32_t kl_convention,
+                          const float* grad_kl, float* g_mu, float* g_rho, void* cuda_stream,
+                          const bbb_prior* prior);
 
 /* Backward of bbb_conv2d_forward / bbb_linear_forward (SURVEY.md Appendix A).
  * Regenerates eps from (seed, stream_id) or reads eps_a/eps_b exactly like the

@@ -33,6 +33,8 @@ SYMBOLS = (
     "bbb_mc_buffer_bytes", "bbb_mc_state_bytes", "bbb_mc_exchange", "bbb_mc_exchange_info", "bbb_mc_exchange_sharded",
     "bbb_comm_alloc", "bbb_comm_free", "bbb_comm_export", "bbb_comm_import", "bbb_comm_unimport", "bbb_set_wide_tiles",
     "bbb_mc_metrics_bytes", "bbb_mc_exchange_metrics", "bbb_lrt_noise_grad",
+    "bbb_conv2d_forward_prior", "bbb_linear_forward_prior", "bbb_layer_forward_fused_prior", "bbb_kl_forward_prior",
+    "bbb_kl_backward_prior",
 )
 MC_MOMENTS, MC_NORMALIZED, MC_INFO = 1, 2, 4
 MC_CAL_BINS = 15                 # BBB_MC_CAL_BINS: calibration bins of the evaluation accumulator
@@ -45,6 +47,11 @@ class LayerDesc(C.Structure):
         "stride_h", "stride_w", "pad_h", "pad_w", "dil_h", "dil_w", "variant", "sample",
         "has_bias", "act_dtype", "math", "kl_convention", "epilogue_act", "pool_k", "pool_s")]
     _fields_ += [("reserved", C.c_int32 * 4), ("prior_mu", C.c_float), ("prior_sigma", C.c_float)]
+
+
+class Prior(C.Structure):
+    """struct bbb_prior (include/bbb_b200.h): per-element Gaussian prior, fp32 device pointers."""
+    _fields_ = [(n, C.c_void_p) for n in ("w_mu", "w_sigma", "b_mu", "b_sigma")]
 
 
 class EngineError(RuntimeError):
@@ -71,6 +78,12 @@ def _bind(lib):
     lib.bbb_layer_forward_fused.argtypes = [dp, vp, vp, i32, i32, i32, fp, fp, fp, fp, vp, vp, i32, i32, fp, fp, fp,
                                             u64, u64, vp, vp, sz, vp]
     lib.bbb_layer_forward_fused.restype = C.c_int
+    pp = C.POINTER(Prior)
+    for name in ("bbb_conv2d_forward_prior", "bbb_linear_forward_prior"):
+        getattr(lib, name).argtypes = fwd + [pp]
+        getattr(lib, name).restype = C.c_int
+    lib.bbb_layer_forward_fused_prior.argtypes = lib.bbb_layer_forward_fused.argtypes + [pp]
+    lib.bbb_layer_forward_fused_prior.restype = C.c_int
     lib.bbb_fused_supported.argtypes = [dp, i32, i32, i32, i32, i32]
     lib.bbb_fused_supported.restype = C.c_int
     lib.bbb_forward_supported.argtypes = [dp]
@@ -79,6 +92,10 @@ def _bind(lib):
     lib.bbb_kl_forward.restype = C.c_int
     lib.bbb_kl_backward.argtypes = [fp, fp, u64, C.c_float, C.c_float, i32, fp, fp, fp, vp]
     lib.bbb_kl_backward.restype = C.c_int
+    lib.bbb_kl_forward_prior.argtypes = lib.bbb_kl_forward.argtypes + [pp]
+    lib.bbb_kl_forward_prior.restype = C.c_int
+    lib.bbb_kl_backward_prior.argtypes = lib.bbb_kl_backward.argtypes + [pp]
+    lib.bbb_kl_backward_prior.restype = C.c_int
     lib.bbb_philox_normal_fill.argtypes = [fp, u64, u64, u64, u64, vp]
     lib.bbb_philox_normal_fill.restype = C.c_int
     lib.bbb_lrt_noise_grad.argtypes = [dp, fp, fp, u64, u64, vp, fp, vp]

@@ -155,14 +155,30 @@ void layer_args(bbb::LayerArgs& a, const bbb_layer_desc* d, const bbb::Geom& g, 
     a.tl_gemm = tl_slot(do_gemm, gemm_name, g);
 }
 
+// A tensor prior (bbb_prior) is all tensors: the weight part always, the bias part with a bias.
+int check_prior(const bbb_prior* q, bool has_bias) {
+    if (!q) return BBB_OK;
+    if (!q->w_mu || !q->w_sigma) return fail(BBB_E_INVALID, "prior: w_mu / w_sigma NULL (a prior is all tensors)");
+    if (has_bias && (!q->b_mu || !q->b_sigma)) return fail(BBB_E_INVALID, "prior: has_bias set but b_mu / b_sigma NULL");
+    return BBB_OK;
+}
+// What the kernels get of a tensor prior: its pointers when the call computes a KL, else none (the scalar kernels run
+// and nothing of the prior is read)
+bbb::PriorPtrs prior_ptrs(const bbb_prior* q, const float* kl_out) {
+    bbb::PriorPtrs t = {nullptr, nullptr, nullptr, nullptr};
+    if (q && kl_out) { t.w_mu = q->w_mu; t.w_sigma = q->w_sigma; t.b_mu = q->b_mu; t.b_sigma = q->b_sigma; }
+    return t;
+}
+
 int forward_impl(const bbb_layer_desc* d, bool linear, const void* x, const float* W_mu, const float* W_rho,
                  const float* bias_mu, const float* bias_rho, void* y, float* kl_out, float* act_std,
                  const float* eps_a, const float* eps_b, uint64_t seed, uint64_t stream_id, const uint64_t* stream_base, void* ws,
-                 size_t ws_bytes, void* stream) {
+                 size_t ws_bytes, void* stream, const bbb_prior* prior) {
     bbb::Geom g;
     if (int rc = check_desc(d, g, linear)) return rc;
     if (!x || !W_mu || !W_rho || !y) return fail(BBB_E_INVALID, "NULL tensor pointer");
     if (d->has_bias && (!bias_mu || !bias_rho)) return fail(BBB_E_INVALID, "has_bias set but bias pointers NULL");
+    if (int rc = check_prior(prior, d->has_bias != 0)) return rc;
     if (kl_out && (!ws || ws_bytes < bbb_workspace_bytes(d)))
         return fail(BBB_E_WORKSPACE, "workspace too small: need %zu bytes", bbb_workspace_bytes(d));
     cudaStream_t st = (cudaStream_t)stream;
@@ -183,7 +199,7 @@ int forward_impl(const bbb_layer_desc* d, bool linear, const void* x, const floa
         a.skip_prep = 0; a.prep_only = 0; a.y_sq = nullptr; a.out_mode = 2; a.out_pitch = 0; a.pool = 0;
         a.x = x; a.y = y; a.act_std = act_std; a.act_dtype = d->act_dtype;
         int nl = 0;
-        cudaError_t e = bbb::launch_fwd_tc(a, st, sm_count(), &nl);
+        cudaError_t e = bbb::launch_fwd_tc(a, st, sm_count(), &nl, prior_ptrs(prior, kl_out));
         if (e != cudaSuccess) return cuda_fail(e, "fwd_tc launch");
         g_launches += nl;
         return BBB_OK;
@@ -197,6 +213,7 @@ int forward_impl(const bbb_layer_desc* d, bool linear, const void* x, const floa
     a.prior_mu = d->prior_mu; a.prior_sigma = d->prior_sigma;
     a.sample = d->sample; a.kl_convention = d->kl_convention; a.has_bias = d->has_bias; a.act = d->epilogue_act;
     a.first_image = first_image_of(*d);
+    a.prior = prior_ptrs(prior, kl_out);
     cudaError_t e = d->variant == BBB_VARIANT_LRT ? bbb::launch_fwd_simt<BBB_VARIANT_LRT>(a, st)
                                                   : bbb::launch_fwd_simt<BBB_VARIANT_BBB>(a, st);
     if (e != cudaSuccess) return cuda_fail(e, "fwd_simt launch");
@@ -249,7 +266,7 @@ int bbb_conv2d_forward(const bbb_layer_desc* desc, const void* x, const float* W
                        const float* eps_a, const float* eps_b, uint64_t seed, uint64_t stream_id, const uint64_t* stream_base,
                        void* workspace, size_t workspace_bytes, void* cuda_stream) {
     return forward_impl(desc, false, x, W_mu, W_rho, bias_mu, bias_rho, y, kl_out, act_std, eps_a, eps_b, seed,
-                        stream_id, stream_base, workspace, workspace_bytes, cuda_stream);
+                        stream_id, stream_base, workspace, workspace_bytes, cuda_stream, nullptr);
 }
 
 int bbb_linear_forward(const bbb_layer_desc* desc, const void* x, const float* W_mu, const float* W_rho,
@@ -257,7 +274,25 @@ int bbb_linear_forward(const bbb_layer_desc* desc, const void* x, const float* W
                        const float* eps_a, const float* eps_b, uint64_t seed, uint64_t stream_id, const uint64_t* stream_base,
                        void* workspace, size_t workspace_bytes, void* cuda_stream) {
     return forward_impl(desc, true, x, W_mu, W_rho, bias_mu, bias_rho, y, kl_out, act_std, eps_a, eps_b, seed,
-                        stream_id, stream_base, workspace, workspace_bytes, cuda_stream);
+                        stream_id, stream_base, workspace, workspace_bytes, cuda_stream, nullptr);
+}
+
+int bbb_conv2d_forward_prior(const bbb_layer_desc* desc, const void* x, const float* W_mu, const float* W_rho,
+                             const float* bias_mu, const float* bias_rho, void* y, float* kl_out, float* act_std,
+                             const float* eps_a, const float* eps_b, uint64_t seed, uint64_t stream_id,
+                             const uint64_t* stream_base, void* workspace, size_t workspace_bytes, void* cuda_stream,
+                             const bbb_prior* prior) {
+    return forward_impl(desc, false, x, W_mu, W_rho, bias_mu, bias_rho, y, kl_out, act_std, eps_a, eps_b, seed,
+                        stream_id, stream_base, workspace, workspace_bytes, cuda_stream, prior);
+}
+
+int bbb_linear_forward_prior(const bbb_layer_desc* desc, const void* x, const float* W_mu, const float* W_rho,
+                             const float* bias_mu, const float* bias_rho, void* y, float* kl_out, float* act_std,
+                             const float* eps_a, const float* eps_b, uint64_t seed, uint64_t stream_id,
+                             const uint64_t* stream_base, void* workspace, size_t workspace_bytes, void* cuda_stream,
+                             const bbb_prior* prior) {
+    return forward_impl(desc, true, x, W_mu, W_rho, bias_mu, bias_rho, y, kl_out, act_std, eps_a, eps_b, seed,
+                        stream_id, stream_base, workspace, workspace_bytes, cuda_stream, prior);
 }
 
 int bbb_conv2d_backward(const bbb_layer_desc* desc, const void* x, const void* grad_y, const float* W_mu,
@@ -336,6 +371,17 @@ int bbb_layer_forward_fused(const bbb_layer_desc* d, const void* x, const void* 
                             const float* bias_mu, const float* bias_rho, void* y, void* y_sq, int32_t out_layout,
                             int32_t out_pitch, float* kl_out, const float* eps_a, const float* eps_b, uint64_t seed,
                             uint64_t stream_id, const uint64_t* stream_base, void* ws, size_t ws_bytes, void* stream) {
+    return bbb_layer_forward_fused_prior(d, x, x_sq, in_layout, in_pitch, prev_hw, W_mu, W_rho, bias_mu, bias_rho, y, y_sq,
+                                         out_layout, out_pitch, kl_out, eps_a, eps_b, seed, stream_id, stream_base, ws,
+                                         ws_bytes, stream, nullptr);
+}
+
+int bbb_layer_forward_fused_prior(const bbb_layer_desc* d, const void* x, const void* x_sq, int32_t in_layout,
+                                  int32_t in_pitch, int32_t prev_hw, const float* W_mu, const float* W_rho,
+                                  const float* bias_mu, const float* bias_rho, void* y, void* y_sq, int32_t out_layout,
+                                  int32_t out_pitch, float* kl_out, const float* eps_a, const float* eps_b, uint64_t seed,
+                                  uint64_t stream_id, const uint64_t* stream_base, void* ws, size_t ws_bytes, void* stream,
+                                  const bbb_prior* prior) {
     bbb::Geom g;
     bool s4;
     if (int rc = fused_check(d, g, in_layout, in_pitch, prev_hw, out_layout, out_pitch, s4)) return rc;
@@ -343,6 +389,7 @@ int bbb_layer_forward_fused(const bbb_layer_desc* d, const void* x, const void* 
     if (prep_only && skip_prep) return fail(BBB_E_INVALID, "PREP_ONLY and SKIP_PREP are exclusive");
     if (!W_mu || !W_rho || (!prep_only && (!x || !y))) return fail(BBB_E_INVALID, "NULL tensor pointer");
     if (d->has_bias && (!bias_mu || !bias_rho)) return fail(BBB_E_INVALID, "has_bias set but bias pointers NULL");
+    if (int rc = check_prior(prior, d->has_bias != 0)) return rc;
     const int pool = d->pool_k != 0;
     bbb::McFold fold;                   // rows, samples and path checked by fused_check
     if (int rc = layer_fold(d, g, eps_a, eps_b, fold)) return rc;
@@ -359,7 +406,7 @@ int bbb_layer_forward_fused(const bbb_layer_desc* d, const void* x, const void* 
         layer_args(a, d, g, W_mu, W_rho, bias_mu, bias_rho, kl_out, eps_a, eps_b, seed, stream_id, stream_base, ws,
                    bbb::conv_s4_bias_offset(g), fold, "conv_s4_prep", !skip_prep, "conv_s4", !prep_only);
         a.x = (const float*)x; a.y = y; a.y_sq = y_sq; a.out_pitch = out_pitch;
-        cudaError_t e = bbb::launch_conv_s4(a, st, !skip_prep, !prep_only, &nl);
+        cudaError_t e = bbb::launch_conv_s4(a, st, !skip_prep, !prep_only, &nl, prior_ptrs(prior, kl_out));
         if (e != cudaSuccess) return cuda_fail(e, "conv_s4 launch");
     } else if (in_layout == BBB_LAYOUT_NCHW_F32) {
         bbb::TcArgs a;                  // fold.rows = 0: fused_check refuses a fold on the gather path
@@ -367,7 +414,7 @@ int bbb_layer_forward_fused(const bbb_layer_desc* d, const void* x, const void* 
                    bbb::tc_bias_offset(g, false), fold, "weight_prep", !skip_prep, "gemm_tc", !prep_only);
         a.x = x; a.y = y; a.act_std = nullptr; a.act_dtype = d->act_dtype; a.tf32 = 0;
         a.skip_prep = skip_prep; a.prep_only = prep_only; a.y_sq = y_sq; a.out_mode = out_mode == 1 ? 2 : out_mode; a.out_pitch = out_pitch; a.pool = pool;
-        cudaError_t e = bbb::launch_fwd_tc(a, st, sm_count(), &nl);
+        cudaError_t e = bbb::launch_fwd_tc(a, st, sm_count(), &nl, prior_ptrs(prior, kl_out));
         if (e != cudaSuccess) return cuda_fail(e, "fused gather launch");
     } else if (in_layout == BBB_LAYOUT_PACKED_BF16) {
         bbb::FusedArgs a;
@@ -376,7 +423,8 @@ int bbb_layer_forward_fused(const bbb_layer_desc* d, const void* x, const void* 
         a.prev_hw = prev_hw; a.y = y; a.y_sq = y_sq; a.out_mode = out_mode; a.out_pitch = out_pitch; a.pool = pool;
         a.in_pitch = in_pitch;
         const char* why = "";
-        cudaError_t e = bbb::launch_fused(a, x, x_sq, st, &nl, &why, !skip_prep, !prep_only, sm_count(), g_wide_tiles.load() != 0);
+        cudaError_t e = bbb::launch_fused(a, x, x_sq, st, &nl, &why, !skip_prep, !prep_only, sm_count(), g_wide_tiles.load() != 0,
+                                          prior_ptrs(prior, kl_out));
         if (e != cudaSuccess) return fail(BBB_E_CUDA, "fused tap-GEMM launch: %s %s", cudaGetErrorString(e), why);
     } else {
         return fail(BBB_E_INVALID, "bad in_layout %d", in_layout);
@@ -388,19 +436,33 @@ int bbb_layer_forward_fused(const bbb_layer_desc* d, const void* x, const void* 
 int bbb_kl_forward(const float* W_mu, const float* W_rho, uint64_t n_w, const float* bias_mu,
                    const float* bias_rho, uint64_t n_b, float prior_mu, float prior_sigma, int32_t kl_convention,
                    float* kl_out, void* workspace, size_t workspace_bytes, void* cuda_stream) {
+    return bbb_kl_forward_prior(W_mu, W_rho, n_w, bias_mu, bias_rho, n_b, prior_mu, prior_sigma, kl_convention, kl_out,
+                                workspace, workspace_bytes, cuda_stream, nullptr);
+}
+
+int bbb_kl_forward_prior(const float* W_mu, const float* W_rho, uint64_t n_w, const float* bias_mu,
+                         const float* bias_rho, uint64_t n_b, float prior_mu, float prior_sigma, int32_t kl_convention,
+                         float* kl_out, void* workspace, size_t workspace_bytes, void* cuda_stream, const bbb_prior* prior) {
     if (!W_mu || !W_rho || !kl_out) return fail(BBB_E_INVALID, "NULL tensor pointer");
     if (n_b && (!bias_mu || !bias_rho)) return fail(BBB_E_INVALID, "n_b > 0 but bias pointers NULL");
+    if (int rc = check_prior(prior, n_b > 0)) return rc;
     if (!workspace || workspace_bytes < kBaseWorkspace) return fail(BBB_E_WORKSPACE, "workspace too small: need %zu bytes", kBaseWorkspace);
-    if (!(prior_sigma > 0.0f)) return fail(BBB_E_INVALID, "prior_sigma must be > 0");
+    if (!prior && !(prior_sigma > 0.0f)) return fail(BBB_E_INVALID, "prior_sigma must be > 0");
     const uint64_t work = (n_w + 3) / 4 + n_b;
     uint64_t blocks = (work + 255) / 256;
     const uint64_t cap = (uint64_t)sm_count() * 8;
     if (blocks > cap) blocks = cap;
     if (blocks < 1) blocks = 1;
     if (blocks > kMaxKlSlots) blocks = kMaxKlSlots;
-    bbb::kl_forward_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)cuda_stream>>>(
-        W_mu, W_rho, n_w, bias_mu, bias_rho, n_b, prior_mu, prior_sigma, kl_convention,
-        (double*)((char*)workspace + kCounterBytes), (unsigned int*)workspace, kl_out);
+    double* partials = (double*)((char*)workspace + kCounterBytes);
+    if (prior)
+        bbb::kl_forward_prior_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)cuda_stream>>>(
+            W_mu, W_rho, n_w, bias_mu, bias_rho, n_b, prior_ptrs(prior, kl_out), kl_convention, partials,
+            (unsigned int*)workspace, kl_out);
+    else
+        bbb::kl_forward_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)cuda_stream>>>(
+            W_mu, W_rho, n_w, bias_mu, bias_rho, n_b, prior_mu, prior_sigma, kl_convention, partials,
+            (unsigned int*)workspace, kl_out);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return cuda_fail(e, "kl_forward launch");
     g_launches += 1;
@@ -409,13 +471,25 @@ int bbb_kl_forward(const float* W_mu, const float* W_rho, uint64_t n_w, const fl
 
 int bbb_kl_backward(const float* mu, const float* rho, uint64_t n, float prior_mu, float prior_sigma,
                     int32_t kl_convention, const float* grad_kl, float* g_mu, float* g_rho, void* cuda_stream) {
+    return bbb_kl_backward_prior(mu, rho, n, prior_mu, prior_sigma, kl_convention, grad_kl, g_mu, g_rho, cuda_stream,
+                                 nullptr);
+}
+
+int bbb_kl_backward_prior(const float* mu, const float* rho, uint64_t n, float prior_mu, float prior_sigma,
+                          int32_t kl_convention, const float* grad_kl, float* g_mu, float* g_rho, void* cuda_stream,
+                          const bbb_prior* prior) {
     if (!mu || !rho || !grad_kl || !g_mu || !g_rho) return fail(BBB_E_INVALID, "NULL tensor pointer");
+    if (int rc = check_prior(prior, false)) return rc;       // the n elements' prior is prior->w_mu / w_sigma
     if (n == 0) return BBB_OK;
     uint64_t blocks = (n + 255) / 256;
     const uint64_t cap = (uint64_t)sm_count() * 8;
     if (blocks > cap) blocks = cap;
-    bbb::kl_backward_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)cuda_stream>>>(
-        mu, rho, n, prior_mu, prior_sigma, kl_convention, grad_kl, g_mu, g_rho);
+    if (prior)
+        bbb::kl_backward_prior_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)cuda_stream>>>(
+            mu, rho, n, prior->w_mu, prior->w_sigma, kl_convention, grad_kl, g_mu, g_rho);
+    else
+        bbb::kl_backward_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)cuda_stream>>>(
+            mu, rho, n, prior_mu, prior_sigma, kl_convention, grad_kl, g_mu, g_rho);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return cuda_fail(e, "kl_backward launch");
     g_launches += 1;

@@ -121,6 +121,41 @@ struct LayerArgs {
     long long* tl_prep; long long* tl_gemm;        // debug: timeline slots of the two launches (nullptr in production)
 };
 
+// Per-element Gaussian prior of a layer (bbb_prior, include/bbb_b200.h): device pointers in the layout of W_mu and of
+// bias_mu.  The weight-prep kernels take it as a parameter of its own behind their argument struct, so the structs (and
+// the parameter offsets of the GEMM kernels that share them) stay as they were; only the tensor-prior instantiations
+// (template flag TP) read it, and only where they compute a KL.
+struct PriorPtrs { const float* w_mu; const float* w_sigma; const float* b_mu; const float* b_sigma; };
+
+// The prior of one KL term, as a compile-time source: the scalar pair of the argument struct (desc->prior_mu /
+// prior_sigma) or element i of the tensors.  prior_of() is called only where the term is computed, so either is read
+// only there (reading the scalars any earlier changes the code of the scalar kernels).
+template <class A> struct PriorScalar { const A& p; };
+struct PriorAt { const float* mu; const float* sigma; size_t i; };
+struct PriorVal { float mu, sigma; };             // tensor values a kernel already loaded (batched with mu / rho)
+template <class A>
+__device__ __forceinline__ float2 prior_of(const PriorScalar<A>& q) { return make_float2(q.p.prior_mu, q.p.prior_sigma); }
+__device__ __forceinline__ float2 prior_of(const PriorAt& q) { return make_float2(__ldg(q.mu + q.i), __ldg(q.sigma + q.i)); }
+__device__ __forceinline__ float2 prior_of(const PriorVal& q) { return make_float2(q.mu, q.sigma); }
+// Weight element i / bias element n: of the tensors q (TP), else the scalar pair of the argument struct `p`
+template <bool TP, class A>
+__device__ __forceinline__ auto w_prior(const A& p, const PriorPtrs& q, size_t i) {
+    if constexpr (TP) return PriorAt{q.w_mu, q.w_sigma, i};
+    else return PriorScalar<A>{p};
+}
+// The same for a weight element, a tensor prior loaded right away (beside the kernel's own load of mu, so the loads are
+// in flight together) instead of where the KL term is computed; nothing is read without a KL (kl_out NULL)
+template <bool TP, class A>
+__device__ __forceinline__ auto w_prior_now(const A& p, const PriorPtrs& q, size_t i) {
+    if constexpr (TP) return p.kl_out ? PriorVal{__ldg(q.w_mu + i), __ldg(q.w_sigma + i)} : PriorVal{0.0f, 1.0f};
+    else return PriorScalar<A>{p};
+}
+template <bool TP, class A>
+__device__ __forceinline__ auto b_prior(const A& p, const PriorPtrs& q, size_t n) {
+    if constexpr (TP) return PriorAt{q.b_mu, q.b_sigma, n};
+    else return PriorScalar<A>{p};
+}
+
 // four normals of group g (elements 4g .. 4g+3)
 __device__ __forceinline__ float4 normal4(uint64_t grp, const NoiseKey& k) {
     const uint4 r = philox4x32_10(make_uint4((uint32_t)grp, (uint32_t)(grp >> 32), k.stream_lo, k.stream_hi),

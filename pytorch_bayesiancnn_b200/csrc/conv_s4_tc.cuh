@@ -59,9 +59,10 @@ inline size_t conv_s4_workspace_bytes(const Geom& g) { return conv_s4_bias_offse
 // ------------------------------------------------------------------ (P) prep
 // item = (kernel row r, 8-wide K chunk, output channel): K' = chunk*8 + e -> window pixel j = K'/4 (s = j - 1), channel K'%4
 // FOLD: BBB fold, one operand set per weight sample (a separate instantiation keeps the other preps as they were)
-template <int VARIANT, bool FOLD = false>
+// TP: the KL is taken against the tensor prior q (bbb_prior), in the same order.
+template <int VARIANT, bool FOLD = false, bool TP = false>
 __global__ void __launch_bounds__(256)
-conv_s4_prep_kernel(const S4Args p) {
+conv_s4_prep_kernel(const S4Args p, const PriorPtrs q) {
     constexpr bool LRT = VARIANT == BBB_VARIANT_LRT;
     const Geom& g = p.g;
     const int n_items = g.KH * 6 * 64;
@@ -87,7 +88,7 @@ conv_s4_prep_kernel(const S4Args p) {
             if (w_ok(e)) {
                 const size_t wi = w_index(e);
                 const float mu = __ldg(p.w_mu + wi);
-                const PrepElem o = prep_elem<LRT>(p, mu, RhoAt{p.w_rho, wi}, p.eps_a, wi, wi, nkey, kl_acc);
+                const PrepElem o = prep_elem<LRT>(p, mu, RhoAt{p.w_rho, wi}, w_prior_now<TP>(p, q, wi), p.eps_a, wi, wi, nkey, kl_acc);
                 w[e] = o.w; s2[e] = o.s2; mu8[e] = mu; sg8[e] = o.sigma;
             }
         }
@@ -102,7 +103,7 @@ conv_s4_prep_kernel(const S4Args p) {
             *reinterpret_cast<uint4*>(fold_set(p.wtiles, p.fold, j) + off) = pack_chunk<false>(w);
         }
     }
-    prep_bias<LRT, FOLD>(p, nkey, 64, kl_acc);
+    prep_bias<LRT, FOLD, TP>(p, q, nkey, 64, kl_acc);
     prep_finish(p, kl_acc);
 }
 
@@ -385,7 +386,8 @@ conv_s4_kernel(const S4Args p) {
     tl_exit(p.tl_gemm, 256);
 }
 
-inline cudaError_t launch_conv_s4(S4Args a, cudaStream_t st, bool do_prep, bool do_gemm, int* n_launch) {
+// q: the tensor prior of the weight-prep kernel (all NULL: the scalar prior of `a`)
+inline cudaError_t launch_conv_s4(S4Args a, cudaStream_t st, bool do_prep, bool do_gemm, int* n_launch, const PriorPtrs& q = PriorPtrs{}) {
     const Geom& g = a.g;
     *n_launch = 0;
     a.planes = tc_planes(a.variant, a.sample);
@@ -394,12 +396,21 @@ inline cudaError_t launch_conv_s4(S4Args a, cudaStream_t st, bool do_prep, bool 
     a.rows = 4 + g.KH;
     const bool lrt = a.variant == BBB_VARIANT_LRT;
     if (do_prep) {
-        prep_carveout<conv_s4_prep_kernel<BBB_VARIANT_LRT>, conv_s4_prep_kernel<BBB_VARIANT_BBB>,
-                      conv_s4_prep_kernel<BBB_VARIANT_BBB, true>>();
         const int grid = (g.KH * 6 * 64 + 255) / 256;
-        cudaError_t e = lrt ? launch_pdl(conv_s4_prep_kernel<BBB_VARIANT_LRT>, dim3(grid), dim3(256), 0, st, a)
-                      : a.fold.sets > 1 ? launch_pdl(conv_s4_prep_kernel<BBB_VARIANT_BBB, true>, dim3(grid), dim3(256), 0, st, a)
-                                        : launch_pdl(conv_s4_prep_kernel<BBB_VARIANT_BBB>, dim3(grid), dim3(256), 0, st, a);
+        cudaError_t e;
+        if (q.w_mu) {                // tensor prior (set only when the call computes a KL): same grid and work split
+            prep_carveout<conv_s4_prep_kernel<BBB_VARIANT_LRT, false, true>, conv_s4_prep_kernel<BBB_VARIANT_BBB, false, true>,
+                          conv_s4_prep_kernel<BBB_VARIANT_BBB, true, true>>();
+            e = lrt ? launch_pdl(conv_s4_prep_kernel<BBB_VARIANT_LRT, false, true>, dim3(grid), dim3(256), 0, st, a, q)
+                : a.fold.sets > 1 ? launch_pdl(conv_s4_prep_kernel<BBB_VARIANT_BBB, true, true>, dim3(grid), dim3(256), 0, st, a, q)
+                                  : launch_pdl(conv_s4_prep_kernel<BBB_VARIANT_BBB, false, true>, dim3(grid), dim3(256), 0, st, a, q);
+        } else {
+            prep_carveout<conv_s4_prep_kernel<BBB_VARIANT_LRT>, conv_s4_prep_kernel<BBB_VARIANT_BBB>,
+                          conv_s4_prep_kernel<BBB_VARIANT_BBB, true>>();
+            e = lrt ? launch_pdl(conv_s4_prep_kernel<BBB_VARIANT_LRT>, dim3(grid), dim3(256), 0, st, a, q)
+                : a.fold.sets > 1 ? launch_pdl(conv_s4_prep_kernel<BBB_VARIANT_BBB, true>, dim3(grid), dim3(256), 0, st, a, q)
+                                  : launch_pdl(conv_s4_prep_kernel<BBB_VARIANT_BBB>, dim3(grid), dim3(256), 0, st, a, q);
+        }
         if (e == cudaSuccess) e = cudaGetLastError();
         if (e != cudaSuccess) return e;
         *n_launch += 1;

@@ -51,8 +51,8 @@ inline size_t fused_workspace_bytes(const Geom& g) { return fused_bias_offset(g)
 // ------------------------------------------------------------- (P) tap prep
 // Tail of both tap preps, per operand set: one all-zero sub-tile behind the real ones (staged for pool-window pixels
 // whose tap is outside the kernel), then the bias rows and the KL publish.
-template <bool LRT, bool FOLD>
-__device__ __forceinline__ void tap_prep_tail(const FusedArgs& p, const NoiseKey& nkey, double kl_acc) {
+template <bool LRT, bool FOLD, bool TP>
+__device__ __forceinline__ void tap_prep_tail(const FusedArgs& p, const PriorPtrs& q, const NoiseKey& nkey, double kl_acc) {
     const int sets = FOLD ? p.fold.sets : 1;
     const size_t sub = fused_wtile_elems(p);
     for (int j = 0; j < sets; ++j) {
@@ -60,7 +60,7 @@ __device__ __forceinline__ void tap_prep_tail(const FusedArgs& p, const NoiseKey
         for (long gi = (long)blockIdx.x * blockDim.x + threadIdx.x; gi < (long)(sub / 8); gi += (long)gridDim.x * blockDim.x)
             zero[gi] = make_uint4(0u, 0u, 0u, 0u);
     }
-    prep_bias<LRT, FOLD>(p, nkey, p.n_cblk * p.ng, kl_acc);
+    prep_bias<LRT, FOLD, TP>(p, q, nkey, p.n_cblk * p.ng, kl_acc);
     prep_finish(p, kl_acc);
 }
 
@@ -68,9 +68,10 @@ __device__ __forceinline__ void tap_prep_tail(const FusedArgs& p, const NoiseKey
 // Resident CTAs per SM: left to itself ptxas gives the LRT instantiation 54 registers (4 CTAs); the bound keeps it at 48
 // (5 CTAs).  The other two are given the occupancy they reach anyway (40 and 64 registers): any explicit bound changes
 // ptxas's register target for every instantiation of the template.
-template <int VARIANT, bool FOLD = false>
+// TP: the KL is taken against the tensor prior q (bbb_prior), in the same order (both tap preps).
+template <int VARIANT, bool FOLD = false, bool TP = false>
 __global__ void __launch_bounds__(256, VARIANT == BBB_VARIANT_LRT ? 5 : FOLD ? 4 : 6)
-tap_prep_kernel(const FusedArgs p) {
+tap_prep_kernel(const FusedArgs p, const PriorPtrs q) {
     constexpr bool LRT = VARIANT == BBB_VARIANT_LRT;
     const Geom& g = p.g;
     const NoiseKey nkey = effective_key(p.key, p.stream_base);
@@ -102,7 +103,7 @@ tap_prep_kernel(const FusedArgs p) {
             if (w_ok(e)) {
                 const size_t wi = w_index(e);
                 const float mu = __ldg(p.w_mu + wi);
-                const PrepElem o = prep_elem<LRT>(p, mu, RhoAt{p.w_rho, wi}, p.eps_a, wi, wi, nkey, kl_acc);
+                const PrepElem o = prep_elem<LRT>(p, mu, RhoAt{p.w_rho, wi}, w_prior_now<TP>(p, q, wi), p.eps_a, wi, wi, nkey, kl_acc);
                 w[e] = o.w; s2[e] = o.s2; mu8[e] = mu; sg8[e] = o.sigma;
             }
         }
@@ -117,7 +118,7 @@ tap_prep_kernel(const FusedArgs p) {
             *reinterpret_cast<uint4*>(fold_set(dst, p.fold, j) + sw) = pack_chunk<false>(w);
         }
     }
-    tap_prep_tail<LRT, FOLD>(p, nkey, kl_acc);
+    tap_prep_tail<LRT, FOLD, TP>(p, q, nkey, kl_acc);
 }
 
 // ------------------------------------------------- (P2) tap prep, conv layers
@@ -135,9 +136,9 @@ tap_prep_kernel(const FusedArgs p) {
 constexpr int PREP2_BATCH = 4;                                     // loads in flight per thread
 __host__ __device__ inline int prep2_slab(int R) { return R * 64 + 8; }   // bf16 per (plane, tap) slab; +8 keeps 16 B alignment, skews banks
 
-template <int VARIANT, bool FOLD = false>
+template <int VARIANT, bool FOLD = false, bool TP = false>
 __global__ void __launch_bounds__(256)
-tap_prep_conv_kernel(const FusedArgs p, const int R) {
+tap_prep_conv_kernel(const FusedArgs p, const int R, const PriorPtrs q) {
     extern __shared__ __align__(16) uint8_t prep2_smem[];
     constexpr bool LRT = VARIANT == BBB_VARIANT_LRT;
     __nv_bfloat16* sm = reinterpret_cast<__nv_bfloat16*>(prep2_smem);
@@ -160,6 +161,7 @@ tap_prep_conv_kernel(const FusedArgs p, const int R) {
         while (cin >= 64) { cin -= 64; ++r; }
         for (int e0 = threadIdx.x; e0 < total; e0 += 256 * PREP2_BATCH) {
             float mu[PREP2_BATCH], rho[PREP2_BATCH];
+            float pmu[PREP2_BATCH], psg[PREP2_BATCH];                 // TP: the prior, loaded in the same batch
             size_t wi[PREP2_BATCH];
             int so[PREP2_BATCH];                                    // smem offset of the element, -1: past the end
             bool ok[PREP2_BATCH];
@@ -172,16 +174,24 @@ tap_prep_conv_kernel(const FusedArgs p, const int R) {
                 so[u] = in ? tap * PS + r * 64 + cin : -1;
                 mu[u] = ok[u] ? __ldg(p.w_mu + wi[u]) : 0.0f;
                 rho[u] = (ok[u] && (p.sample || p.kl_out)) ? __ldg(p.w_rho + wi[u]) : 0.0f;
+                if constexpr (TP) {
+                    pmu[u] = (ok[u] && p.kl_out) ? __ldg(q.w_mu + wi[u]) : 0.0f;
+                    psg[u] = (ok[u] && p.kl_out) ? __ldg(q.w_sigma + wi[u]) : 1.0f;
+                }
                 tap += dq; cin += dc;
                 if (tap >= KHW) { tap -= KHW; ++cin; }
                 while (cin >= 64) { cin -= 64; ++r; }
             }
+            auto prior_u = [&](int u) {
+                if constexpr (TP) return PriorVal{pmu[u], psg[u]};
+                else return w_prior<false>(p, q, wi[u]);
+            };
 #pragma unroll
             for (int u = 0; u < PREP2_BATCH; ++u) {
                 if (so[u] < 0) continue;
                 PrepElem o = {0.0f, 0.0f, 0.0f};
                 if (ok[u]) {
-                    o = prep_elem<LRT, !fold>(p, mu[u], rho[u], p.eps_a, wi[u], wi[u], nkey, kl_acc);
+                    o = prep_elem<LRT, !fold>(p, mu[u], rho[u], prior_u(u), p.eps_a, wi[u], wi[u], nkey, kl_acc);
                     if (fold) smf[so[u]] = make_float2(mu[u], o.sigma);   // every sample's weight is drawn in phase 2
                 }
                 if (fold) continue;
@@ -226,7 +236,7 @@ tap_prep_conv_kernel(const FusedArgs p, const int R) {
         }
         __syncthreads();
     }
-    tap_prep_tail<LRT, FOLD>(p, nkey, kl_acc);
+    tap_prep_tail<LRT, FOLD, TP>(p, q, nkey, kl_acc);
 }
 
 // ------------------------------------------------------------ wgmma helpers
@@ -601,8 +611,55 @@ inline bool fused_supported(const Geom& g, int pool) {
     return true;
 }
 
+// The weight-prep launch of launch_fused (a.planes, ng, n_cblk, n_kblk and taps set); TP: the tensor-prior instantiations.
+template <bool TP>
+inline cudaError_t launch_tap_prep(const FusedArgs& a, const PriorPtrs& q, cudaStream_t st, int n_sm) {
+    const Geom& g = a.g;
+    const bool lrt = a.variant == BBB_VARIANT_LRT;
+    const bool fold = !lrt && a.fold.sets > 1;    // one operand set per weight sample: same grid / R, so the same KL sum
+    const long items = (long)a.taps * a.n_cblk * a.n_kblk * a.ng * 8;
+    int grid = (int)((items + 255) / 256);
+    if (grid > 2048) grid = 2048;
+    if (grid < 1) grid = 1;
+    prep_carveout<tap_prep_kernel<BBB_VARIANT_LRT, false, TP>, tap_prep_kernel<BBB_VARIANT_BBB, false, TP>, tap_prep_kernel<BBB_VARIANT_BBB, true, TP>>();
+    // conv layers: the coalesced variant (rows x 64-channel block per CTA); R = rows per CTA, shrunk until the
+    // grid covers the SMs and the staging tile fits 48 KB
+    static const bool prep2_on = [] { const char* e = getenv("BBB_B200_PREP2"); return !(e && e[0] == '0'); }();
+    int R = 8;
+    const int npad = a.n_cblk * a.ng;
+    auto need = [&](int r) { return (size_t)a.planes * g.KHW * prep2_slab(r) * 2; };
+    // <= 26 KB of staging per CTA: the preps run beside the GEMM chain (side streams) and must fit next to its CTAs
+    constexpr size_t kPrepSmem = 26 * 1024;
+    // (smaller CTAs -- >= 4 per SM -- were tried for more loads in flight: the preps then lose the scheduling race against
+    //  the high-priority GEMM chain, and a late prep delays the whole step)
+    while (R > 2 && ((long)(npad / R) * a.n_kblk < n_sm || need(R) > kPrepSmem)) R >>= 1;
+    const bool prep2 = prep2_on && g.KHW > 1 && a.prev_hw == 1 && g.Cin % 64 == 0 && a.taps == g.KHW && need(R) <= 48 * 1024;
+    if (prep2) {
+        prep_carveout<tap_prep_conv_kernel<BBB_VARIANT_LRT, false, TP>, tap_prep_conv_kernel<BBB_VARIANT_BBB, false, TP>,
+                      tap_prep_conv_kernel<BBB_VARIANT_BBB, true, TP>>();
+        int grid2 = (npad / R) * a.n_kblk;
+        if (grid2 > 2048) grid2 = 2048;
+        // a BBB fold stages fp32 (mu, sigma) pairs: 4x the bf16 slab, same R and grid as the unfolded call
+        if (fold) {
+            const size_t smem2 = (size_t)g.KHW * prep2_slab(R) * 8;
+            const cudaError_t e2 = cudaFuncSetAttribute(tap_prep_conv_kernel<BBB_VARIANT_BBB, true, TP>,
+                                                        cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem2);
+            if (e2 != cudaSuccess) return e2;
+            tap_prep_conv_kernel<BBB_VARIANT_BBB, true, TP><<<grid2, 256, smem2, st>>>(a, R, q);
+        }
+        else if (lrt) tap_prep_conv_kernel<BBB_VARIANT_LRT, false, TP><<<grid2, 256, need(R), st>>>(a, R, q);
+        else          tap_prep_conv_kernel<BBB_VARIANT_BBB, false, TP><<<grid2, 256, need(R), st>>>(a, R, q);
+    }
+    else if (fold) tap_prep_kernel<BBB_VARIANT_BBB, true, TP><<<grid, 256, 0, st>>>(a, q);
+    else if (lrt)  tap_prep_kernel<BBB_VARIANT_LRT, false, TP><<<grid, 256, 0, st>>>(a, q);
+    else           tap_prep_kernel<BBB_VARIANT_BBB, false, TP><<<grid, 256, 0, st>>>(a, q);
+    return cudaGetLastError();
+}
+
+// q: the tensor prior of the weight-prep kernel (all NULL: the scalar prior of `a`)
 inline cudaError_t launch_fused(FusedArgs a, const void* x, const void* x_sq, cudaStream_t st, int* n_launch, const char** why,
-                                bool do_prep = true, bool do_gemm = true, int n_sm = 132, bool prefer_wide = false) {
+                                bool do_prep = true, bool do_gemm = true, int n_sm = 132, bool prefer_wide = false,
+                                const PriorPtrs& q = PriorPtrs{}) {
     const Geom& g = a.g;
     *n_launch = 0;
     a.planes = tc_planes(a.variant, a.sample);
@@ -621,51 +678,14 @@ inline cudaError_t launch_fused(FusedArgs a, const void* x, const void* x_sq, cu
     a.n_cblk = (g.N + a.ng - 1) / a.ng;
     a.n_kblk = (g.Cin + 63) / 64;
     a.taps = g.KHW;
-    const bool lrt = a.variant == BBB_VARIANT_LRT;
     a.x = x; a.x_sq = x_sq;
     if (do_gemm && a.planes == 2 && x_sq != (const void*)((const __nv_bfloat16*)x + 128 * 64)) {
         *why = "LRT fused layer needs the activation with interleaved x / x^2 blocks (x_sq == x + 8192 elements)";
         return cudaErrorInvalidValue;
     }
     if (do_prep) {
-        const bool fold = !lrt && a.fold.sets > 1;    // one operand set per weight sample: same grid / R, so the same KL sum
-        const long items = (long)a.taps * a.n_cblk * a.n_kblk * a.ng * 8;
-        int grid = (int)((items + 255) / 256);
-        if (grid > 2048) grid = 2048;
-        if (grid < 1) grid = 1;
-        prep_carveout<tap_prep_kernel<BBB_VARIANT_LRT>, tap_prep_kernel<BBB_VARIANT_BBB>, tap_prep_kernel<BBB_VARIANT_BBB, true>>();
-        // conv layers: the coalesced variant (rows x 64-channel block per CTA); R = rows per CTA, shrunk until the
-        // grid covers the SMs and the staging tile fits 48 KB
-        static const bool prep2_on = [] { const char* e = getenv("BBB_B200_PREP2"); return !(e && e[0] == '0'); }();
-        int R = 8;
-        const int npad = a.n_cblk * a.ng;
-        auto need = [&](int r) { return (size_t)a.planes * g.KHW * prep2_slab(r) * 2; };
-        // <= 26 KB of staging per CTA: the preps run beside the GEMM chain (side streams) and must fit next to its CTAs
-        constexpr size_t kPrepSmem = 26 * 1024;
-        // (smaller CTAs -- >= 4 per SM -- were tried for more loads in flight: the preps then lose the scheduling race against
-        //  the high-priority GEMM chain, and a late prep delays the whole step)
-        while (R > 2 && ((long)(npad / R) * a.n_kblk < n_sm || need(R) > kPrepSmem)) R >>= 1;
-        const bool prep2 = prep2_on && g.KHW > 1 && a.prev_hw == 1 && g.Cin % 64 == 0 && a.taps == g.KHW && need(R) <= 48 * 1024;
-        if (prep2) {
-            prep_carveout<tap_prep_conv_kernel<BBB_VARIANT_LRT>, tap_prep_conv_kernel<BBB_VARIANT_BBB>,
-                          tap_prep_conv_kernel<BBB_VARIANT_BBB, true>>();
-            int grid2 = (npad / R) * a.n_kblk;
-            if (grid2 > 2048) grid2 = 2048;
-            // a BBB fold stages fp32 (mu, sigma) pairs: 4x the bf16 slab, same R and grid as the unfolded call
-            if (fold) {
-                const size_t smem2 = (size_t)g.KHW * prep2_slab(R) * 8;
-                const cudaError_t e2 = cudaFuncSetAttribute(tap_prep_conv_kernel<BBB_VARIANT_BBB, true>,
-                                                            cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem2);
-                if (e2 != cudaSuccess) return e2;
-                tap_prep_conv_kernel<BBB_VARIANT_BBB, true><<<grid2, 256, smem2, st>>>(a, R);
-            }
-            else if (lrt) tap_prep_conv_kernel<BBB_VARIANT_LRT><<<grid2, 256, need(R), st>>>(a, R);
-            else          tap_prep_conv_kernel<BBB_VARIANT_BBB><<<grid2, 256, need(R), st>>>(a, R);
-        }
-        else if (fold) tap_prep_kernel<BBB_VARIANT_BBB, true><<<grid, 256, 0, st>>>(a);
-        else if (lrt)  tap_prep_kernel<BBB_VARIANT_LRT><<<grid, 256, 0, st>>>(a);
-        else           tap_prep_kernel<BBB_VARIANT_BBB><<<grid, 256, 0, st>>>(a);
-        cudaError_t e = cudaGetLastError();
+        // a tensor prior (set only when the call computes a KL) takes the TP instantiations: same kernels' grids and work split
+        const cudaError_t e = q.w_mu ? launch_tap_prep<true>(a, q, st, n_sm) : launch_tap_prep<false>(a, q, st, n_sm);
         if (e != cudaSuccess) return e;
         *n_launch += 1;
     }

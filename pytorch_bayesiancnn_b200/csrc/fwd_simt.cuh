@@ -24,6 +24,7 @@ struct FwdArgs {
     float prior_mu, prior_sigma;
     int sample, kl_convention, has_bias, act;
     int first_image;    // global index of image 0: LRT noise of image b is drawn at image first_image + b (McFold)
+    PriorPtrs prior;    // tensor prior (TP = true instantiations only)
 };
 
 __device__ __noinline__ float apply_act(float v, int act) {
@@ -32,7 +33,8 @@ __device__ __noinline__ float apply_act(float v, int act) {
     return v;
 }
 
-template <int VARIANT, int BM, int BN, int TM, int TN>
+// TP: the KL terms are taken against the tensor prior p.prior (bbb_prior) instead of (prior_mu, prior_sigma).
+template <int VARIANT, int BM, int BN, int TM, int TN, bool TP = false>
 __global__ void __launch_bounds__((BM / TM) * (BN / TN))
 fwd_simt_kernel(const FwdArgs p) {
     constexpr int BK = 16, NT = (BM / TM) * (BN / TN), PAD = 4;
@@ -116,7 +118,10 @@ fwd_simt_kernel(const FwdArgs p) {
                 } else {
                     w = mu;
                 }
-                if (do_kl) kl_acc += (double)kl_term(mu, sigma, p.prior_mu, p.prior_sigma, p.kl_convention);
+                if (do_kl) {
+                    const float2 q = prior_of(w_prior<TP>(p, p.prior, wi));
+                    kl_acc += (double)kl_term(mu, sigma, q.x, q.y, p.kl_convention);
+                }
             }
             rb[i] = w;
             if (LRT) rv[i] = s2;
@@ -194,7 +199,8 @@ fwd_simt_kernel(const FwdArgs p) {
     if (do_kl) {
         if (p.has_bias && t < BN && n0 + t < g.N) {
             const float mu = __ldg(p.b_mu + n0 + t), sigma = softplus_sigma(__ldg(p.b_rho + n0 + t));
-            kl_acc += (double)kl_term(mu, sigma, p.prior_mu, p.prior_sigma, p.kl_convention);
+            const float2 q = prior_of(b_prior<TP>(p, p.prior, (size_t)(n0 + t)));
+            kl_acc += (double)kl_term(mu, sigma, q.x, q.y, p.kl_convention);
         }
         const double tot = block_sum(kl_acc, red);
         if (t == 0) kl_publish(tot, blockIdx.y, gridDim.y, p.kl_partials, p.kl_counter, p.kl_out);
@@ -226,22 +232,27 @@ fwd_simt_kernel(const FwdArgs p) {
     }
 }
 
-template <int VARIANT, int BM, int BN, int TM, int TN>
+template <int VARIANT, int BM, int BN, int TM, int TN, bool TP>
 inline cudaError_t launch_fwd_simt_cfg(const FwdArgs& a, cudaStream_t st) {
     dim3 grid((a.g.M + BM - 1) / BM, (a.g.N + BN - 1) / BN);
-    fwd_simt_kernel<VARIANT, BM, BN, TM, TN><<<grid, (BM / TM) * (BN / TN), 0, st>>>(a);
+    fwd_simt_kernel<VARIANT, BM, BN, TM, TN, TP><<<grid, (BM / TM) * (BN / TN), 0, st>>>(a);
     return cudaGetLastError();
 }
 
 inline int simt_n_tile(int N) { return N <= 16 ? 16 : (N <= 32 ? 32 : 64); }
 inline int simt_kl_slots(const Geom& g) { const int bn = simt_n_tile(g.N); return (g.N + bn - 1) / bn; }
 
+template <int VARIANT, bool TP>
+inline cudaError_t launch_fwd_simt_tp(const FwdArgs& a, cudaStream_t st) {
+    const int bn = simt_n_tile(a.g.N);
+    if (bn == 16) return launch_fwd_simt_cfg<VARIANT, 128, 16, 4, 2, TP>(a, st);
+    if (bn == 32) return launch_fwd_simt_cfg<VARIANT, 128, 32, 4, 4, TP>(a, st);
+    return launch_fwd_simt_cfg<VARIANT, 64, 64, 4, 4, TP>(a, st);
+}
+// a tensor prior (a.prior.w_mu, set only when the call computes a KL) takes the TP instantiations
 template <int VARIANT>
 inline cudaError_t launch_fwd_simt(const FwdArgs& a, cudaStream_t st) {
-    const int bn = simt_n_tile(a.g.N);
-    if (bn == 16) return launch_fwd_simt_cfg<VARIANT, 128, 16, 4, 2>(a, st);
-    if (bn == 32) return launch_fwd_simt_cfg<VARIANT, 128, 32, 4, 4>(a, st);
-    return launch_fwd_simt_cfg<VARIANT, 64, 64, 4, 4>(a, st);
+    return a.prior.w_mu ? launch_fwd_simt_tp<VARIANT, true>(a, st) : launch_fwd_simt_tp<VARIANT, false>(a, st);
 }
 
 }  // namespace bbb

@@ -299,12 +299,13 @@ __device__ __forceinline__ float rho_of(float rho) { return rho; }
 __device__ __forceinline__ float rho_of(const RhoAt& r) { return __ldg(r.rho + r.i); }
 
 // One parameter element: sigma = softplus(rho); plane 0 = BBB mu + eps*sigma when sampling (eps: `eps[ei]` if given,
-// else Philox element i), otherwise mu; plane 1 = LRT sigma^2; and its KL term added to `kl`.
+// else Philox element i), otherwise mu; plane 1 = LRT sigma^2; and its KL term against `prior` (PriorScalar / PriorAt,
+// read only here) added to `kl`.
 // DRAW = false leaves plane 0 at mu: a BBB fold that draws every sample later with fold_draw.
 struct PrepElem { float w, s2, sigma; };
-template <bool LRT, bool DRAW = true, class Rho>
-__device__ __forceinline__ PrepElem prep_elem(const LayerArgs& p, float mu, const Rho& rho, const float* eps, size_t ei,
-                                              uint64_t i, const NoiseKey& nkey, double& kl) {
+template <bool LRT, bool DRAW = true, class Rho, class Prior>
+__device__ __forceinline__ PrepElem prep_elem(const LayerArgs& p, float mu, const Rho& rho, const Prior& prior,
+                                              const float* eps, size_t ei, uint64_t i, const NoiseKey& nkey, double& kl) {
     const bool stoch = p.sample != 0, do_kl = p.kl_out != nullptr;
     PrepElem o = {mu, 0.0f, 0.0f};
     if (stoch || do_kl) o.sigma = softplus_sigma_fast(rho_of(rho));
@@ -313,7 +314,10 @@ __device__ __forceinline__ PrepElem prep_elem(const LayerArgs& p, float mu, cons
         const float e_ = eps ? __ldg(eps + ei) : normal1(i, nkey);
         o.w = mu + e_ * o.sigma;
     }
-    if (do_kl) kl += (double)kl_term_fast(mu, o.sigma, p.prior_mu, p.prior_sigma, p.kl_convention);
+    if (do_kl) {
+        const float2 q = prior_of(prior);
+        kl += (double)kl_term_fast(mu, o.sigma, q.x, q.y, p.kl_convention);
+    }
     return o;
 }
 
@@ -324,9 +328,9 @@ __device__ __forceinline__ float fold_draw(float mu, float sigma, uint64_t i, co
 
 // Bias rows of every operand set: bias_ws[n] (BBB: sampled, LRT: mu) and bias_ws[npad + n] (LRT: sigma_b^2) for all npad
 // padded columns, zero past N or without a bias; one thread per column, each bias KL term counted once.  Bias element n
-// is Philox element N*K + n, behind the weights.
-template <bool LRT, bool FOLD>
-__device__ __forceinline__ void prep_bias(const LayerArgs& p, const NoiseKey& nkey, int npad, double& kl) {
+// is Philox element N*K + n, behind the weights.  TP: the KL terms take the bias part of the tensor prior q.
+template <bool LRT, bool FOLD, bool TP>
+__device__ __forceinline__ void prep_bias(const LayerArgs& p, const PriorPtrs& q, const NoiseKey& nkey, int npad, double& kl) {
     const Geom& g = p.g;
     const uint64_t i0 = (uint64_t)g.N * g.K;
     for (int n = blockIdx.x * blockDim.x + threadIdx.x; n < npad; n += gridDim.x * blockDim.x) {
@@ -335,7 +339,7 @@ __device__ __forceinline__ void prep_bias(const LayerArgs& p, const NoiseKey& nk
         PrepElem o = {0.0f, 0.0f, 0.0f};
         if (real) {
             mu = __ldg(p.b_mu + n);
-            o = prep_elem<LRT>(p, mu, RhoAt{p.b_rho, (size_t)n}, p.eps_b, n, i0 + n, nkey, kl);
+            o = prep_elem<LRT>(p, mu, RhoAt{p.b_rho, (size_t)n}, b_prior<TP>(p, q, n), p.eps_b, n, i0 + n, nkey, kl);
         }
         p.bias_ws[n] = o.w;
         p.bias_ws[npad + n] = o.s2;
@@ -379,9 +383,10 @@ inline void prep_carveout() {
 // K chunk); consecutive threads take consecutive rows so the 16-byte writes are contiguous.
 // FOLD: BBB fold, one operand set per weight sample, all drawn from the same (mu, sigma) in the same work split as an
 // unfolded call, so the KL sums in the same order (a separate instantiation keeps the unfolded prep as it was).
-template <int VARIANT, bool TF32, bool FOLD = false>
+// TP: the KL is taken against the tensor prior q (bbb_prior), in the same order.
+template <int VARIANT, bool TF32, bool FOLD = false, bool TP = false>
 __global__ void __launch_bounds__(256)
-weight_prep_kernel(const TcArgs p) {
+weight_prep_kernel(const TcArgs p, const PriorPtrs q) {
     constexpr bool LRT = VARIANT == BBB_VARIANT_LRT;
     static_assert(!(LRT && FOLD), "a fold prep draws BBB weight samples");
     constexpr int CE = TF32 ? 4 : 8, BKE = 8 * CE;                  // elements per 16-byte chunk / per K block
@@ -406,7 +411,7 @@ weight_prep_kernel(const TcArgs p) {
             if (n < g.N && k < g.K) {
                 const size_t wi = (size_t)n * g.K + k;
                 const float mu = __ldg(p.w_mu + wi);
-                const PrepElem o = prep_elem<LRT>(p, mu, RhoAt{p.w_rho, wi}, p.eps_a, wi, wi, nkey, kl_acc);
+                const PrepElem o = prep_elem<LRT>(p, mu, RhoAt{p.w_rho, wi}, w_prior_now<TP>(p, q, wi), p.eps_a, wi, wi, nkey, kl_acc);
                 w[e] = o.w; s2[e] = o.s2; mu8[e] = mu; sg8[e] = o.sigma;
             }
         }
@@ -425,7 +430,7 @@ weight_prep_kernel(const TcArgs p) {
             }
         }
     }
-    prep_bias<LRT, FOLD>(p, nkey, p.n_tiles * TC_BN, kl_acc);
+    prep_bias<LRT, FOLD, TP>(p, q, nkey, p.n_tiles * TC_BN, kl_acc);
     prep_finish(p, kl_acc);
 }
 
@@ -734,7 +739,7 @@ gemm_tc_kernel(const TcArgs p, const int stages) {
 }
 
 template <int VARIANT, bool TF32>
-inline cudaError_t launch_fwd_tc_t(TcArgs a, cudaStream_t st, int* n_launch) {
+inline cudaError_t launch_fwd_tc_t(TcArgs a, cudaStream_t st, int* n_launch, const PriorPtrs& q) {
     const Geom& g = a.g;
     if (!a.skip_prep) {
         const long items = (long)a.n_tiles * a.k_blocks * TC_BN * 8;
@@ -742,10 +747,16 @@ inline cudaError_t launch_fwd_tc_t(TcArgs a, cudaStream_t st, int* n_launch) {
         if (grid > 2048) grid = 2048;
         // A BBB fold (one operand set per weight sample) keeps the grid, so its KL sums in the unfolded call's order.
         // (For LRT both names below are the unfolded prep: only BBB has a fold instantiation.)
+        // A tensor prior (set only when the call computes a KL) takes the TP instantiations: same grid, same work split.
         constexpr bool BBB = VARIANT == BBB_VARIANT_BBB;
-        prep_carveout<weight_prep_kernel<VARIANT, TF32, false>, weight_prep_kernel<VARIANT, TF32, BBB>>();
         auto* prep = BBB && a.fold.sets > 1 ? weight_prep_kernel<VARIANT, TF32, BBB> : weight_prep_kernel<VARIANT, TF32, false>;
-        prep<<<grid, 256, 0, st>>>(a);
+        if (q.w_mu) {
+            prep_carveout<weight_prep_kernel<VARIANT, TF32, false, true>, weight_prep_kernel<VARIANT, TF32, BBB, true>>();
+            prep = BBB && a.fold.sets > 1 ? weight_prep_kernel<VARIANT, TF32, BBB, true> : weight_prep_kernel<VARIANT, TF32, false, true>;
+        } else {
+            prep_carveout<weight_prep_kernel<VARIANT, TF32, false>, weight_prep_kernel<VARIANT, TF32, BBB>>();
+        }
+        prep<<<grid, 256, 0, st>>>(a, q);
         cudaError_t e = cudaGetLastError();
         if (e != cudaSuccess) return e;
         *n_launch += 1;
@@ -789,7 +800,8 @@ inline cudaError_t launch_fwd_tc_t(TcArgs a, cudaStream_t st, int* n_launch) {
     return e;
 }
 
-inline cudaError_t launch_fwd_tc(TcArgs a, cudaStream_t st, int n_sm, int* n_launch) {
+// q: the tensor prior of the weight-prep kernel (all NULL: the scalar prior of `a`)
+inline cudaError_t launch_fwd_tc(TcArgs a, cudaStream_t st, int n_sm, int* n_launch, const PriorPtrs& q = PriorPtrs{}) {
     const Geom& g = a.g;
     const bool tf32 = a.tf32 != 0;
     a.planes = tc_planes(a.variant, a.sample);
@@ -798,8 +810,8 @@ inline cudaError_t launch_fwd_tc(TcArgs a, cudaStream_t st, int n_sm, int* n_lau
     *n_launch = 0;
     (void)n_sm;
     const bool lrt = a.variant == BBB_VARIANT_LRT;
-    if (tf32) return lrt ? launch_fwd_tc_t<BBB_VARIANT_LRT, true>(a, st, n_launch) : launch_fwd_tc_t<BBB_VARIANT_BBB, true>(a, st, n_launch);
-    return lrt ? launch_fwd_tc_t<BBB_VARIANT_LRT, false>(a, st, n_launch) : launch_fwd_tc_t<BBB_VARIANT_BBB, false>(a, st, n_launch);
+    if (tf32) return lrt ? launch_fwd_tc_t<BBB_VARIANT_LRT, true>(a, st, n_launch, q) : launch_fwd_tc_t<BBB_VARIANT_BBB, true>(a, st, n_launch, q);
+    return lrt ? launch_fwd_tc_t<BBB_VARIANT_LRT, false>(a, st, n_launch, q) : launch_fwd_tc_t<BBB_VARIANT_BBB, false>(a, st, n_launch, q);
 }
 
 }  // namespace bbb

@@ -239,6 +239,23 @@ def _ptr(t: Optional[torch.Tensor]):
     return None if t is None else C.c_void_p(t.data_ptr())
 
 
+def prior_arg(prior, bias: bool = False):
+    """The ``const bbb_prior*`` argument of a *_prior entry point: None (NULL, the scalar prior of the desc / call) when
+    ``prior`` is None, else a reference to the bbb_prior of ``prior`` = (w_mu, w_sigma, b_mu, b_sigma) -- contiguous fp32
+    CUDA tensors, b_* None without a bias.  ``bias=True``: the bias part in the w_ fields, as bbb_kl_backward_prior reads
+    the prior of the n elements it is called on."""
+    if prior is None:
+        return None
+    w_mu, w_sigma, b_mu, b_sigma = prior
+    if bias:
+        w_mu, w_sigma, b_mu, b_sigma = b_mu, b_sigma, None, None
+    for t in (w_mu, w_sigma, b_mu, b_sigma):
+        if t is not None:
+            _require_cuda(t, "tensor prior")
+    p = lambda t: None if t is None else t.data_ptr()
+    return C.byref(L.Prior(p(w_mu), p(w_sigma), p(b_mu), p(b_sigma)))
+
+
 def _stream(device):
     return C.c_void_p(torch.cuda.current_stream(device).cuda_stream)
 
@@ -553,10 +570,11 @@ class BayesLayerFn(torch.autograd.Function):
         if variant == L.VARIANT_LRT and sample and need_grad:
             act_std = torch.empty(yshape, dtype=torch.float32, device=dev)
         ws = workspace(dev, d, cfg.get("owner"))
-        fn = lib.bbb_linear_forward if conv is None else lib.bbb_conv2d_forward
+        fn = lib.bbb_linear_forward_prior if conv is None else lib.bbb_conv2d_forward_prior
         rc = fn(C.byref(d), _ptr(x), _ptr(W_mu_c), _ptr(W_rho_c), _ptr(bias_mu), _ptr(bias_rho),
                 _ptr(y), _ptr(kl), _ptr(act_std), _ptr(eps_a), _ptr(eps_b),
-                C.c_uint64(seed), C.c_uint64(stream_id), _ptr(base), _ptr(ws), C.c_size_t(ws.numel()), _stream(dev))
+                C.c_uint64(seed), C.c_uint64(stream_id), _ptr(base), _ptr(ws), C.c_size_t(ws.numel()), _stream(dev),
+                prior_arg(cfg.get("prior")))
         L.check(rc, "bbb_linear_forward" if conv is None else "bbb_conv2d_forward")
         if y.dtype != y_dtype:                      # a bf16 input the engine took as fp32
             y = y.to(y_dtype)
@@ -619,17 +637,18 @@ class BayesLayerFn(torch.autograd.Function):
             gx = gx.to(ctx.x_dtype)
         if gkl is not None:
             gkl = gkl.contiguous().float()
-            rc = lib.bbb_kl_backward(_ptr(W_mu), _ptr(W_rho), C.c_uint64(W_mu.numel()),
-                                     C.c_float(cfg["prior_mu"]), C.c_float(cfg["prior_sigma"]),
-                                     C.c_int32(cfg["kl_convention"]), _ptr(gkl), _ptr(g_W_mu), _ptr(g_W_rho),
-                                     _stream(dev))
-            L.check(rc, "bbb_kl_backward")
+            prior = cfg.get("prior")
+            rc = lib.bbb_kl_backward_prior(_ptr(W_mu), _ptr(W_rho), C.c_uint64(W_mu.numel()),
+                                           C.c_float(cfg["prior_mu"]), C.c_float(cfg["prior_sigma"]),
+                                           C.c_int32(cfg["kl_convention"]), _ptr(gkl), _ptr(g_W_mu), _ptr(g_W_rho),
+                                           _stream(dev), prior_arg(prior))
+            L.check(rc, "bbb_kl_backward_prior")
             if ctx.has_bias:
-                rc = lib.bbb_kl_backward(_ptr(bias_mu), _ptr(bias_rho), C.c_uint64(bias_mu.numel()),
-                                         C.c_float(cfg["prior_mu"]), C.c_float(cfg["prior_sigma"]),
-                                         C.c_int32(cfg["kl_convention"]), _ptr(gkl), _ptr(g_b_mu), _ptr(g_b_rho),
-                                         _stream(dev))
-                L.check(rc, "bbb_kl_backward")
+                rc = lib.bbb_kl_backward_prior(_ptr(bias_mu), _ptr(bias_rho), C.c_uint64(bias_mu.numel()),
+                                               C.c_float(cfg["prior_mu"]), C.c_float(cfg["prior_sigma"]),
+                                               C.c_int32(cfg["kl_convention"]), _ptr(gkl), _ptr(g_b_mu), _ptr(g_b_rho),
+                                               _stream(dev), prior_arg(prior, bias=True))
+                L.check(rc, "bbb_kl_backward_prior")
         return gx, g_W_mu, g_W_rho, g_b_mu, g_b_rho, None
 
 
@@ -706,10 +725,11 @@ class BayesLayerFn(torch.autograd.Function):
 
 
 class KLFn(torch.autograd.Function):
-    """kl_loss() with no preceding forward: sigma recomputed from rho in the kernel."""
+    """kl_loss() with no preceding forward: sigma recomputed from rho in the kernel.  ``prior``: None (the scalar
+    prior_mu / prior_sigma) or the tensor prior (w_mu, w_sigma, b_mu, b_sigma) of the layer (no gradient flows to it)."""
 
     @staticmethod
-    def forward(ctx, W_mu, W_rho, bias_mu, bias_rho, prior_mu, prior_sigma, kl_convention):
+    def forward(ctx, W_mu, W_rho, bias_mu, bias_rho, prior_mu, prior_sigma, kl_convention, prior=None):
         lib = L.lib()
         _require_cuda(W_mu, "kl_loss")
         dev = W_mu.device
@@ -717,12 +737,14 @@ class KLFn(torch.autograd.Function):
         kl = torch.empty((), dtype=torch.float32, device=dev)
         ws = workspace(dev)
         nb = 0 if bias_mu is None else bias_mu.numel()
-        rc = lib.bbb_kl_forward(_ptr(W_mu_c), _ptr(W_rho_c), C.c_uint64(W_mu.numel()), _ptr(bias_mu), _ptr(bias_rho),
-                                C.c_uint64(nb), C.c_float(prior_mu), C.c_float(prior_sigma), C.c_int32(kl_convention),
-                                _ptr(kl), _ptr(ws), C.c_size_t(ws.numel()), _stream(dev))
-        L.check(rc, "bbb_kl_forward")
+        rc = lib.bbb_kl_forward_prior(_ptr(W_mu_c), _ptr(W_rho_c), C.c_uint64(W_mu.numel()), _ptr(bias_mu),
+                                      _ptr(bias_rho), C.c_uint64(nb), C.c_float(prior_mu), C.c_float(prior_sigma),
+                                      C.c_int32(kl_convention), _ptr(kl), _ptr(ws), C.c_size_t(ws.numel()), _stream(dev),
+                                      prior_arg(prior))
+        L.check(rc, "bbb_kl_forward_prior")
         ctx.save_for_backward(W_mu_c, W_rho_c, bias_mu, bias_rho)
         ctx.cfg = (float(prior_mu), float(prior_sigma), int(kl_convention))
+        ctx.prior = prior
         return kl
 
     @staticmethod
@@ -733,16 +755,17 @@ class KLFn(torch.autograd.Function):
         dev = W_mu.device
         gkl = gkl.contiguous().float()
         out = []
-        for mu, rho in ((W_mu, W_rho), (bias_mu, bias_rho)):
+        for mu, rho, bias in ((W_mu, W_rho, False), (bias_mu, bias_rho, True)):
             if mu is None:
                 out += [None, None]
                 continue
             g_mu, g_rho = torch.zeros_like(mu), torch.zeros_like(rho)
-            rc = lib.bbb_kl_backward(_ptr(mu), _ptr(rho), C.c_uint64(mu.numel()), C.c_float(pm), C.c_float(ps),
-                                     C.c_int32(conv), _ptr(gkl), _ptr(g_mu), _ptr(g_rho), _stream(dev))
-            L.check(rc, "bbb_kl_backward")
+            rc = lib.bbb_kl_backward_prior(_ptr(mu), _ptr(rho), C.c_uint64(mu.numel()), C.c_float(pm), C.c_float(ps),
+                                           C.c_int32(conv), _ptr(gkl), _ptr(g_mu), _ptr(g_rho), _stream(dev),
+                                           prior_arg(ctx.prior, bias=bias))
+            L.check(rc, "bbb_kl_backward_prior")
             out += [g_mu, g_rho]
-        return out[0], out[1], out[2], out[3], None, None, None
+        return out[0], out[1], out[2], out[3], None, None, None, None
 
 
 # --------------------------------------------------------------------------- #

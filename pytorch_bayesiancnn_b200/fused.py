@@ -335,13 +335,13 @@ def run_step(st, nxt, cur, cur_sq, cur_pitch, kl=None, noise=None, phase=0, y_in
             noise = _draw_noise(st, B, dev)
         eps_a, eps_b, seed, stream_id, base = noise
         ws = Fn.workspace(dev, d, m)
-        rc = lib.bbb_layer_forward_fused(
+        rc = lib.bbb_layer_forward_fused_prior(
             C.byref(d), Fn._ptr(cur), Fn._ptr(cur_sq), st.in_layout, in_pitch, st.prev_hw,
             Fn._ptr(m.W_mu), Fn._ptr(m.W_rho), Fn._ptr(m.bias_mu), Fn._ptr(m.bias_rho),
             Fn._ptr(y), Fn._ptr(y_sq), st.out_layout, pitch, Fn._ptr(kl), Fn._ptr(eps_a), Fn._ptr(eps_b),
             C.c_uint64(seed), C.c_uint64(stream_id), Fn._ptr(base), Fn._ptr(ws), C.c_size_t(ws.numel()),
-            Fn._stream(dev))
-        L.check(rc, "bbb_layer_forward_fused")
+            Fn._stream(dev), Fn.prior_arg(m.prior_tensors()))
+        L.check(rc, "bbb_layer_forward_fused_prior")
         if phase != L.FUSED_SKIP_PREP:
             m._kl_cache = (kl, m._versions(), torch.is_grad_enabled())
         return y, y_sq, pitch

@@ -49,6 +49,8 @@ class GraphedForward:
                     post(*out)
         torch.cuda.current_stream(dev).wait_stream(side)
         torch.cuda.synchronize(dev)
+        from .modules import PriorGuard
+        self.prior_guard = PriorGuard(net)        # the layers' prior buffers as the graphs read them
         self.graphs, self.outputs = [], []
         cap = torch.cuda.Stream(device=dev, priority=-1)     # GEMM chain above the parameter preps on the (default-priority) side streams
         for xin in self.inputs:
@@ -73,6 +75,7 @@ class GraphedForward:
         self.base.fill_(int(first_stream) - _STRIDE)
 
     def __call__(self, x: torch.Tensor | None = None, non_blocking: bool = True, slot: int = 0):
+        self.prior_guard.check("GraphedForward")
         if x is not None:
             self.inputs[slot].copy_(x, non_blocking=non_blocking)
         self.graphs[slot].replay()

@@ -285,6 +285,7 @@ class MCForward:
             self.xrep_all = [torch.empty((G * self.nb,) + tuple(example_x.shape[1:]), dtype=example_x.dtype, device=dev)
                              for _ in range(nbuf)]
         self.graph, self.graphs = None, []
+        self._prior_guard = None                   # set by _capture (modules.PriorGuard)
         self.result_stream = None                 # overlap mode: the stream the results are complete on
         self.replays = 0
         self.kernels_per_step = None
@@ -449,7 +450,9 @@ class MCForward:
 
     def _capture(self, warmup: int = 2):
         from .graph import _STRIDE
+        from .modules import PriorGuard
         dev = self.dev
+        self._prior_guard = PriorGuard(self.net)   # the layers' prior buffers as the graphs read them
         # several steps in flight: the tap-GEMM layers take their 128-column tiles wherever Cout allows (throughput over the
         # latency of one step; the choice is made at launch = capture time, include/bbb_b200.h bbb_set_wide_tiles)
         prev_wide = L.lib().bbb_set_wide_tiles(1 if self.inflight > 1 else 0)
@@ -543,6 +546,8 @@ class MCForward:
     def __call__(self, x: Optional[torch.Tensor] = None, labels: Optional[torch.Tensor] = None, slot: int = 0):
         if labels is not None and self.labels is None:
             raise L.EngineError("MCForward was built without with_labels=True")
+        if self._prior_guard is not None:
+            self._prior_guard.check("MCForward")
         if self.overlap:
             cur = torch.cuda.current_stream(self.dev)
             par = self.replays % self.nbuf
@@ -699,7 +704,7 @@ def mc_forward(net_or_fn, x: torch.Tensor, num_ens: int, group=None, want_uncert
         net = net_or_fn
         key = (tuple(x.shape), int(num_ens), bool(want_uncertainty), bool(normalized), labels is not None,
                float(train_size), float(beta), seed, id(group), bool(information), int(batch_shards))
-        cache = net.__dict__.setdefault("_mc_engines", {})
+        cache = _engine_cache(net, "_mc_engines")
         eng = cache.get(key)
         if eng is None:
             eng = cache[key] = MCForward(net, x, num_ens, group, want_uncertainty, normalized, labels is not None,
@@ -714,6 +719,19 @@ def mc_forward(net_or_fn, x: torch.Tensor, num_ens: int, group=None, want_uncert
             res.append(out["head"])
         return tuple(res)
     return _generic_mc_forward(net_or_fn, x, num_ens, group, want_uncertainty, information, batch_shards)
+
+
+def _engine_cache(net, name):
+    """The engine cache `name` kept on the net (mc_forward: "_mc_engines", evaluate: "_mc_eval").  Both are dropped when a
+    layer's prior was set, cleared, re-allocated or moved since their engines were captured (modules.PriorGuard), so
+    the next call captures engines that read the layers' current priors."""
+    from .modules import PriorGuard
+    guard = net.__dict__.get("_mc_prior_guard")
+    if guard is None or not guard.ok():
+        net.__dict__.pop("_mc_engines", None)
+        net.__dict__.pop("_mc_eval", None)
+        net.__dict__["_mc_prior_guard"] = PriorGuard(net)
+    return net.__dict__.setdefault(name, {})
 
 
 def new_metrics(device) -> torch.Tensor:
@@ -758,7 +776,7 @@ def evaluate(net, loader, num_ens: int, train_size: float, beta_type=0.1, epoch=
     requires)."""
     dev = next(net.parameters()).device
     key = (int(num_ens), float(train_size), seed, id(group), int(inflight), int(batch_shards))
-    ev = net.__dict__.setdefault("_mc_eval", {}).get(key)
+    ev = _engine_cache(net, "_mc_eval").get(key)
     if ev is None:
         ev = net.__dict__["_mc_eval"][key] = {"acc": new_metrics(dev), "engines": {}, "seed": seed}
     acc, engines, nslots = ev["acc"], ev["engines"], max(2, int(inflight))

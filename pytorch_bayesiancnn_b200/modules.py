@@ -13,6 +13,11 @@ Engine knobs ride on ``set_flag`` (never on the constructor):
                                             path wherever the shape fits a wgmma tile, IEEE-fp32 CUDA cores otherwise;
                                             'fp32' forces the exact-arithmetic kernels everywhere)
   kl_convention  'reference' | 'textbook'   default 'reference' = the formula as executed (SURVEY D1)
+
+Per-weight Gaussian priors (``set_prior`` / ``posterior_as_prior``): the KL of every parameter element is taken against
+its own N(mu_p, sigma_p^2), e.g. the posterior of a previous task (variational continual learning) or a prior centred on
+pretrained weights.  The prior lives in four fp32 buffers (``W_prior_mu``, ``W_prior_sigma``, ``bias_prior_mu``,
+``bias_prior_sigma``) that exist only after ``set_prior``: a layer that never had one keeps the reference's state_dict.
 """
 from __future__ import annotations
 
@@ -31,6 +36,13 @@ _DEFAULT_PRIORS = {
     "posterior_mu_initial": (0, 0.1),
     "posterior_rho_initial": (-3, 0.1),
 }
+_PRIOR_BUFFERS = ("W_prior_mu", "W_prior_sigma", "bias_prior_mu", "bias_prior_sigma")
+_prior_epoch = 0          # bumped whenever some layer's prior buffers are created, replaced, moved or removed (PriorGuard)
+
+
+def _prior_moved():
+    global _prior_epoch
+    _prior_epoch += 1
 
 
 def _default_math() -> str:
@@ -153,10 +165,85 @@ class _BayesLayer(ModuleWrapper):
 
     def _versions(self):
         """What a cached KL scalar depends on: the parameters' versions AND the KL settings (changing
-        kl_convention or the prior after a forward must not return the old value)."""
-        ps = (self.W_mu, self.W_rho, self.bias_mu, self.bias_rho)
+        kl_convention or the prior -- scalar or tensor (set_prior) -- after a forward must not return the old value)."""
+        ps = (self.W_mu, self.W_rho, self.bias_mu, self.bias_rho) + tuple(self._buffers.get(n) for n in _PRIOR_BUFFERS)
         return tuple((p._version, p.data_ptr()) if p is not None else None for p in ps) + (
             self.kl_convention, float(self.prior_mu), float(self.prior_sigma))
+
+    # -- per-weight priors ----------------------------------------------------
+    def prior_tensors(self):
+        """(W_prior_mu, W_prior_sigma, bias_prior_mu, bias_prior_sigma) after set_prior (bias ones None without a
+        bias), or None: the KL is taken against the scalar prior_mu / prior_sigma."""
+        if self._buffers.get("W_prior_mu") is None:
+            return None
+        return tuple(self._buffers.get(n) for n in _PRIOR_BUFFERS)
+
+    def set_prior(self, mu=None, sigma=None, bias_mu=None, bias_sigma=None):
+        """Take the KL against a per-element Gaussian prior N(mu, sigma^2) from now on.  Each argument is a number or a
+        tensor that broadcasts to the shape of W_mu (mu, sigma) or bias_mu (bias_mu, bias_sigma); None takes the layer's
+        scalar prior_mu / prior_sigma.  The values are stored as contiguous fp32 buffers on the parameters' device, so
+        they follow .to() / .cuda() and are saved in the state_dict.  sigma must be finite and > 0 (ValueError; checked
+        here, not by the kernels).  Setting again with the same shapes copies in place: the buffers keep their
+        addresses, so an engine captured after the first set_prior (MCForward, GraphedForward) reads the new values on
+        its next replay.  No gradient flows to the prior."""
+        if not self.use_bias and (bias_mu is not None or bias_sigma is not None):
+            raise ValueError("set_prior: the layer has no bias")
+        dev = self.W_mu.device
+        parts = [("W_prior_mu", mu, self.prior_mu, self.W_mu.shape, False),
+                 ("W_prior_sigma", sigma, self.prior_sigma, self.W_mu.shape, True)]
+        if self.use_bias:
+            parts += [("bias_prior_mu", bias_mu, self.prior_mu, self.bias_mu.shape, False),
+                      ("bias_prior_sigma", bias_sigma, self.prior_sigma, self.bias_mu.shape, True)]
+        vals = []
+        for name, v, scalar, shape, is_sigma in parts:
+            t = torch.as_tensor(scalar if v is None else v).detach().to(device=dev, dtype=torch.float32)
+            try:
+                ok = torch.broadcast_shapes(t.shape, shape) == shape
+            except RuntimeError:
+                ok = False
+            if not ok:
+                raise ValueError(f"set_prior: {name} of shape {tuple(t.shape)} does not broadcast to {tuple(shape)}")
+            if not bool(torch.isfinite(t).all()) or (is_sigma and not bool((t > 0).all())):
+                raise ValueError(f"set_prior: {name} must be finite" + (" and > 0" if is_sigma else ""))
+            vals.append((name, t, shape))
+        for name, t, shape in vals:
+            buf = self._buffers.get(name)
+            if buf is not None and buf.shape == shape and buf.device == dev and buf.is_contiguous():
+                with torch.no_grad():
+                    buf.copy_(t)
+            else:
+                self.register_buffer(name, torch.empty(shape, dtype=torch.float32, device=dev).copy_(t))
+                _prior_moved()
+        return self
+
+    def clear_prior(self):
+        """Back to the scalar prior_mu / prior_sigma: removes the prior buffers.  A captured engine that read them
+        refuses its next replay (PriorGuard); mc_forward / evaluate build new engines."""
+        removed = [self._buffers.pop(n, None) for n in _PRIOR_BUFFERS]
+        if any(t is not None for t in removed):
+            _prior_moved()
+        return self
+
+    def _apply(self, fn, *args, **kwargs):
+        # .to() / .cuda() / .float() replace the buffers: engines captured on the old ones must notice
+        out = super()._apply(fn, *args, **kwargs)
+        if self._buffers.get("W_prior_mu") is not None:
+            _prior_moved()
+        return out
+
+    def _load_from_state_dict(self, state_dict, prefix, local_metadata, strict, missing_keys, unexpected_keys,
+                              error_msgs):
+        # a checkpoint saved after set_prior carries the prior: create the buffers so that it loads into a fresh layer.
+        # They take the parameters' shapes, so a checkpoint prior of another shape fails torch's size check.
+        shapes = {"W_prior_mu": self.W_mu.shape, "W_prior_sigma": self.W_mu.shape}
+        if self.use_bias:
+            shapes.update(bias_prior_mu=self.bias_mu.shape, bias_prior_sigma=self.bias_mu.shape)
+        for n, shape in shapes.items():
+            if prefix + n in state_dict and self._buffers.get(n) is None:
+                self.register_buffer(n, torch.zeros(shape, dtype=torch.float32, device=self.W_mu.device))
+                _prior_moved()
+        super()._load_from_state_dict(state_dict, prefix, local_metadata, strict, missing_keys, unexpected_keys,
+                                      error_msgs)
 
     def _cfg(self, sample):
         return {
@@ -169,6 +256,7 @@ class _BayesLayer(ModuleWrapper):
             "kl_convention": L.KL_BY_NAME[self.kl_convention],
             "act": L.ACT_NONE,
             "owner": self,
+            "prior": self.prior_tensors(),
         }
 
     def forward(self, x, sample=True):
@@ -188,7 +276,7 @@ class _BayesLayer(ModuleWrapper):
         if c is not None and c[1] == self._versions() and (c[2] or not torch.is_grad_enabled()):
             return c[0]
         return Fn.KLFn.apply(self.W_mu, self.W_rho, self.bias_mu, self.bias_rho, float(self.prior_mu),
-                             float(self.prior_sigma), L.KL_BY_NAME[self.kl_convention])
+                             float(self.prior_sigma), L.KL_BY_NAME[self.kl_convention], self.prior_tensors())
 
     @property
     def W_sigma(self):
@@ -269,3 +357,50 @@ class BBBLRTLinear(_LinearMixin, _BayesLayer):
     def __init__(self, in_features, out_features, bias=True, priors=None):
         super().__init__()
         self._init_linear(in_features, out_features, bias, priors)
+
+
+def prior_signature(net: nn.Module) -> tuple:
+    """Where every Bayesian layer of `net` keeps its prior: the buffers' addresses, or None for the scalar prior."""
+    return tuple(None if m.prior_tensors() is None else tuple(None if t is None else t.data_ptr() for t in m.prior_tensors())
+                 for m in net.modules() if isinstance(m, _BayesLayer))
+
+
+class PriorGuard:
+    """The layers' priors as a captured CUDA graph of `net` bakes them in: the buffers' addresses, or NULL for a scalar
+    prior.  It holds the buffers, so a replay never reads freed memory, and ``ok()`` tells whether a replay still reads
+    what the layers hold: false once a prior was set for the first time, cleared, re-allocated or moved.  An in-place
+    set_prior keeps the addresses (the next replay reads the new values).  While no layer anywhere changed its prior's
+    identity, ``ok()`` is one integer compare."""
+
+    def __init__(self, net: nn.Module):
+        self.net, self.epoch, self.sig = net, _prior_epoch, prior_signature(net)
+        self.keep = [t for m in net.modules() if isinstance(m, _BayesLayer) for t in (m.prior_tensors() or ())
+                     if t is not None]
+
+    def ok(self) -> bool:
+        if self.epoch == _prior_epoch:
+            return True
+        if prior_signature(self.net) != self.sig:
+            return False
+        self.epoch = _prior_epoch
+        return True
+
+    def check(self, what: str):
+        if not self.ok():
+            raise L.EngineError(f"{what}: a layer's prior was set, cleared, re-allocated or moved since this engine's "
+                                "CUDA graphs were captured; build a new engine (an in-place set_prior of the same shapes "
+                                "is read by the next replay)")
+
+
+def posterior_as_prior(net: nn.Module) -> nn.Module:
+    """The continual-learning step (variational continual learning, Nguyen et al. 2018): every Bayesian layer of `net`
+    takes its current posterior N(W_mu, softplus(W_rho)^2), element by element, as the prior of its KL from now on
+    (set_prior; the bias likewise).  Train task A, call this, then train task B: the KL pulls the weights towards what
+    task A learned, in proportion to how certain it was.  sigma = log1p(exp(rho)), the engine's softplus."""
+    for m in net.modules():
+        if isinstance(m, _BayesLayer):
+            with torch.no_grad():
+                m.set_prior(m.W_mu.detach(), torch.log1p(torch.exp(m.W_rho.detach())),
+                            m.bias_mu.detach() if m.use_bias else None,
+                            torch.log1p(torch.exp(m.bias_rho.detach())) if m.use_bias else None)
+    return net
