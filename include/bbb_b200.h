@@ -269,6 +269,47 @@ int bbb_kl_backward_prior(const float* mu, const float* rho, uint64_t n,
                           const float* grad_kl, float* g_mu, float* g_rho, void* cuda_stream,
                           const bbb_prior* prior);
 
+/* The scale-mixture prior of Bayes by Backprop (Blundell et al. 2015, section 3.3; nothing in the reference):
+ *   p(w) = pi N(w; 0, sigma1^2) + (1 - pi) N(w; 0, sigma2^2),   usually sigma1 > sigma2: a wide slab and a narrow spike.
+ * HOST values.  0 < pi <= 1, sigma1 > 0, sigma2 > 0, all finite and sigma^2 within fp32 range, else BBB_E_INVALID
+ * (pi == 1 is the single Gaussian N(0, sigma1^2)). */
+typedef struct bbb_mixture_prior { float pi, sigma1, sigma2; } bbb_mixture_prior;
+
+/* Monte-Carlo estimate of KL(q || p) of a layer against a mixture prior, which has no closed form.  For a parameter
+ * element with q = N(mu, sigma^2), sigma = log1p(exp(rho)), and one standard normal eps:
+ *   w    = mu + sigma eps
+ *   term = -log sigma - 1/2
+ *          - logsumexp(log pi - log sigma1 - w^2 / (2 sigma1^2), log(1 - pi) - log sigma2 - w^2 / (2 sigma2^2))
+ * kl_out[d] = sum of the terms over W, then the bias.  The entropy half is exact and only -E_q[log p] is sampled (the
+ * 1/2 log 2 pi of the two halves cancel), so pi == 1 converges to the textbook Gaussian KL.  It is always an estimate of
+ * KL(q || p): kl_convention has no meaning here.
+ * Noise: draw d uses Philox stream stream_id (+ *stream_base when not NULL, read on the device) + d * draw_stride of
+ * `seed`; element i of W draws normal(i) of it and bias element n draws normal(n_w + n), whoever computes it.  Draw d
+ * of a call therefore equals, bit for bit, the single-draw call on stream_id + d * draw_stride: with the stride of an
+ * MC-sample fold, one call gives the per-sample estimates of the folded samples.  The layer forwards do not compute this
+ * term: call them with kl_out == NULL and take the layer's KL from here.
+ * workspace: bbb_kl_mc_workspace_bytes(n_draws) bytes, zero-filled once when allocated (self-resetting counters); calls
+ * that may run concurrently need workspaces of their own.  n_draws >= 1, else BBB_E_INVALID. */
+size_t bbb_kl_mc_workspace_bytes(int32_t n_draws);
+int bbb_kl_mc_forward(const float* W_mu, const float* W_rho, uint64_t n_w,
+                      const float* bias_mu, const float* bias_rho, uint64_t n_b,
+                      const bbb_mixture_prior* prior,
+                      uint64_t seed, uint64_t stream_id, const uint64_t* stream_base,
+                      int32_t n_draws, uint64_t draw_stride,
+                      float* kl_out /* [n_draws] */, void* workspace, size_t workspace_bytes, void* cuda_stream);
+
+/* Reparameterisation gradient of bbb_kl_mc_forward for n elements (a weight tensor with first_element = 0, or the bias
+ * with first_element = n_w), eps drawn again from the same streams (element i draws normal(first_element + i)):
+ *   s = w (r1 / sigma1^2 + r2 / sigma2^2)   with r1, r2 the softmax of the two logsumexp arguments  (= -d log p / dw)
+ *   d/dmu = s     d/dsigma = -1/sigma + s eps     d/drho = sigmoid(rho) d/dsigma
+ * g_mu / g_rho are ACCUMULATED into: += sum_d grad_kl[d] * (...), draws in ascending order (grad_kl: n_draws device
+ * floats). */
+int bbb_kl_mc_backward(const float* mu, const float* rho, uint64_t n, uint64_t first_element,
+                       const bbb_mixture_prior* prior,
+                       uint64_t seed, uint64_t stream_id, const uint64_t* stream_base,
+                       int32_t n_draws, uint64_t draw_stride,
+                       const float* grad_kl /* [n_draws] */, float* g_mu, float* g_rho, void* cuda_stream);
+
 /* Backward of bbb_conv2d_forward / bbb_linear_forward (SURVEY.md Appendix A).
  * Regenerates eps from (seed, stream_id) or reads eps_a/eps_b exactly like the
  * forward (the first image of desc->reserved[0] included).  grad_x nullable.  g_* are ACCUMULATED into (caller zeroes).

@@ -34,7 +34,7 @@ SYMBOLS = (
     "bbb_comm_alloc", "bbb_comm_free", "bbb_comm_export", "bbb_comm_import", "bbb_comm_unimport", "bbb_set_wide_tiles",
     "bbb_mc_metrics_bytes", "bbb_mc_exchange_metrics", "bbb_lrt_noise_grad",
     "bbb_conv2d_forward_prior", "bbb_linear_forward_prior", "bbb_layer_forward_fused_prior", "bbb_kl_forward_prior",
-    "bbb_kl_backward_prior",
+    "bbb_kl_backward_prior", "bbb_kl_mc_workspace_bytes", "bbb_kl_mc_forward", "bbb_kl_mc_backward",
 )
 MC_MOMENTS, MC_NORMALIZED, MC_INFO = 1, 2, 4
 MC_CAL_BINS = 15                 # BBB_MC_CAL_BINS: calibration bins of the evaluation accumulator
@@ -52,6 +52,11 @@ class LayerDesc(C.Structure):
 class Prior(C.Structure):
     """struct bbb_prior (include/bbb_b200.h): per-element Gaussian prior, fp32 device pointers."""
     _fields_ = [(n, C.c_void_p) for n in ("w_mu", "w_sigma", "b_mu", "b_sigma")]
+
+
+class MixturePrior(C.Structure):
+    """struct bbb_mixture_prior (include/bbb_b200.h): the scale-mixture prior's host values."""
+    _fields_ = [(n, C.c_float) for n in ("pi", "sigma1", "sigma2")]
 
 
 class EngineError(RuntimeError):
@@ -96,6 +101,13 @@ def _bind(lib):
     lib.bbb_kl_forward_prior.restype = C.c_int
     lib.bbb_kl_backward_prior.argtypes = lib.bbb_kl_backward.argtypes + [pp]
     lib.bbb_kl_backward_prior.restype = C.c_int
+    mp = C.POINTER(MixturePrior)
+    lib.bbb_kl_mc_workspace_bytes.argtypes = [i32]
+    lib.bbb_kl_mc_workspace_bytes.restype = sz
+    lib.bbb_kl_mc_forward.argtypes = [fp, fp, u64, fp, fp, u64, mp, u64, u64, vp, i32, u64, fp, vp, sz, vp]
+    lib.bbb_kl_mc_forward.restype = C.c_int
+    lib.bbb_kl_mc_backward.argtypes = [fp, fp, u64, u64, mp, u64, u64, vp, i32, u64, fp, fp, fp, vp]
+    lib.bbb_kl_mc_backward.restype = C.c_int
     lib.bbb_philox_normal_fill.argtypes = [fp, u64, u64, u64, u64, vp]
     lib.bbb_philox_normal_fill.restype = C.c_int
     lib.bbb_lrt_noise_grad.argtypes = [dp, fp, fp, u64, u64, vp, fp, vp]

@@ -1,5 +1,6 @@
 // C-ABI entry points of libbbb_b200.so (declared in include/bbb_b200.h).
 #include <atomic>
+#include <cmath>
 #include <cstdarg>
 #include <cstdio>
 #include <cstring>
@@ -7,6 +8,7 @@
 #include "common.cuh"
 #include "fwd_simt.cuh"
 #include "misc_kernels.cuh"
+#include "kl_mc.cuh"
 #include "bwd_simt.cuh"
 #include "fwd_tc.cuh"
 #include "fused_tc.cuh"
@@ -168,6 +170,27 @@ bbb::PriorPtrs prior_ptrs(const bbb_prior* q, const float* kl_out) {
     bbb::PriorPtrs t = {nullptr, nullptr, nullptr, nullptr};
     if (q && kl_out) { t.w_mu = q->w_mu; t.w_sigma = q->w_sigma; t.b_mu = q->b_mu; t.b_sigma = q->b_sigma; }
     return t;
+}
+
+// Counters of a Monte-Carlo KL call (one per draw), padded so that the partial rows behind them stay aligned.
+size_t kl_mc_counter_bytes(size_t n_draws) { return (n_draws * sizeof(unsigned int) + 255) / 256 * 256; }
+
+// The scale-mixture prior of a Monte-Carlo KL call comes from outside the library: 0 < pi <= 1, sigma1, sigma2 > 0, all
+// finite, and sigma^2 within fp32 range (1 / (2 sigma^2) is what the kernels multiply by).
+int check_mixture(const bbb_mixture_prior* p, int32_t n_draws, bbb::MixPrior& q) {
+    if (!p) return fail(BBB_E_INVALID, "mixture prior is NULL");
+    if (!(p->pi > 0.0f && p->pi <= 1.0f)) return fail(BBB_E_INVALID, "mixture prior: pi must be in (0, 1] (got %g)", (double)p->pi);
+    if (!(p->sigma1 > 0.0f && std::isfinite(p->sigma1) && p->sigma2 > 0.0f && std::isfinite(p->sigma2)))
+        return fail(BBB_E_INVALID, "mixture prior: sigma1 and sigma2 must be finite and > 0 (got %g, %g)", (double)p->sigma1, (double)p->sigma2);
+    if (n_draws < 1) return fail(BBB_E_INVALID, "n_draws must be >= 1 (got %d)", n_draws);
+    const double s1 = p->sigma1, s2 = p->sigma2, pi = p->pi;
+    q.lc1 = (float)(std::log(pi) - std::log(s1));
+    q.lc2 = pi < 1.0 ? (float)(std::log1p(-pi) - std::log(s2)) : -INFINITY;
+    q.h1 = (float)(0.5 / (s1 * s1));
+    q.h2 = (float)(0.5 / (s2 * s2));
+    if (!std::isfinite(q.h1) || !std::isfinite(q.h2) || q.h1 == 0.0f || q.h2 == 0.0f)
+        return fail(BBB_E_INVALID, "mixture prior: sigma^2 outside fp32 range (got %g, %g)", s1, s2);
+    return BBB_OK;
 }
 
 int forward_impl(const bbb_layer_desc* d, bool linear, const void* x, const float* W_mu, const float* W_rho,
@@ -492,6 +515,64 @@ int bbb_kl_backward_prior(const float* mu, const float* rho, uint64_t n, float p
             mu, rho, n, prior_mu, prior_sigma, kl_convention, grad_kl, g_mu, g_rho);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return cuda_fail(e, "kl_backward launch");
+    g_launches += 1;
+    return BBB_OK;
+}
+
+size_t bbb_kl_mc_workspace_bytes(int32_t n_draws) {
+    const size_t d = n_draws > 0 ? (size_t)n_draws : 1;
+    return kl_mc_counter_bytes(d) + d * kMaxKlSlots * sizeof(double);
+}
+
+int bbb_kl_mc_forward(const float* W_mu, const float* W_rho, uint64_t n_w, const float* bias_mu, const float* bias_rho,
+                      uint64_t n_b, const bbb_mixture_prior* prior, uint64_t seed, uint64_t stream_id,
+                      const uint64_t* stream_base, int32_t n_draws, uint64_t draw_stride, float* kl_out, void* workspace,
+                      size_t workspace_bytes, void* cuda_stream) {
+    if (!W_mu || !W_rho || !kl_out) return fail(BBB_E_INVALID, "NULL tensor pointer");
+    if (n_b && (!bias_mu || !bias_rho)) return fail(BBB_E_INVALID, "n_b > 0 but bias pointers NULL");
+    bbb::MixPrior q;
+    if (int rc = check_mixture(prior, n_draws, q)) return rc;
+    const size_t need = bbb_kl_mc_workspace_bytes(n_draws);
+    if (!workspace || workspace_bytes < need) return fail(BBB_E_WORKSPACE, "workspace too small: need %zu bytes", need);
+    const uint64_t work = n_w / 4 + n_w % 4 + n_b;
+    uint64_t blocks = (work + bbb::KL_MC_THREADS - 1) / bbb::KL_MC_THREADS;
+    const uint64_t cap = (uint64_t)sm_count() * 8;
+    if (blocks > cap) blocks = cap;
+    if (blocks < 1) blocks = 1;
+    if (blocks > kMaxKlSlots) blocks = kMaxKlSlots;
+    unsigned int* counters = (unsigned int*)workspace;
+    double* partials = (double*)((char*)workspace + kl_mc_counter_bytes((size_t)n_draws));
+    // the draws go in launches of at most KL_MC_MAX_DRAWS, each draw with its own counter and partial row
+    for (int32_t d0 = 0; d0 < n_draws; d0 += bbb::KL_MC_MAX_DRAWS) {
+        const int nd = std::min<int32_t>(bbb::KL_MC_MAX_DRAWS, n_draws - d0);
+        bbb::kl_mc_forward_kernel<<<(unsigned)blocks, bbb::KL_MC_THREADS, (size_t)nd * bbb::KL_MC_THREADS * sizeof(double),
+                                    (cudaStream_t)cuda_stream>>>(
+            W_mu, W_rho, n_w, bias_mu, bias_rho, n_b, q, bbb::make_key(seed, stream_id + (uint64_t)d0 * draw_stride),
+            (const unsigned long long*)stream_base, nd, draw_stride, counters + d0, partials + (size_t)d0 * kMaxKlSlots,
+            kl_out + d0);
+        cudaError_t e = cudaGetLastError();
+        if (e != cudaSuccess) return cuda_fail(e, "kl_mc_forward launch");
+        g_launches += 1;
+    }
+    return BBB_OK;
+}
+
+int bbb_kl_mc_backward(const float* mu, const float* rho, uint64_t n, uint64_t first_element,
+                       const bbb_mixture_prior* prior, uint64_t seed, uint64_t stream_id, const uint64_t* stream_base,
+                       int32_t n_draws, uint64_t draw_stride, const float* grad_kl, float* g_mu, float* g_rho,
+                       void* cuda_stream) {
+    if (!mu || !rho || !grad_kl || !g_mu || !g_rho) return fail(BBB_E_INVALID, "NULL tensor pointer");
+    bbb::MixPrior q;
+    if (int rc = check_mixture(prior, n_draws, q)) return rc;
+    if (n == 0) return BBB_OK;
+    uint64_t blocks = ((n + 3) / 4 + bbb::KL_MC_THREADS - 1) / bbb::KL_MC_THREADS;
+    const uint64_t cap = (uint64_t)sm_count() * 8;
+    if (blocks > cap) blocks = cap;
+    bbb::kl_mc_backward_kernel<<<(unsigned)blocks, bbb::KL_MC_THREADS, 0, (cudaStream_t)cuda_stream>>>(
+        mu, rho, n, first_element, q, bbb::make_key(seed, stream_id), (const unsigned long long*)stream_base, n_draws,
+        draw_stride, grad_kl, g_mu, g_rho);
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return cuda_fail(e, "kl_mc_backward launch");
     g_launches += 1;
     return BBB_OK;
 }

@@ -289,20 +289,26 @@ def workspace_slot(k: int):
         _ws_slot = prev
 
 
-def workspace(device, desc=None, owner=None) -> torch.Tensor:
+def workspace(device, desc=None, owner=None, kl_mc_draws: int = 0) -> torch.Tensor:
     """Zero-initialised scratch.  Without `owner`: one per (device, stream) -- calls on
     one stream are ordered, so sharing is safe and the kernels leave the counters
     zeroed.  With `owner` (a layer module): a private buffer sized by bbb_workspace_bytes(desc),
     which on the tensor-core path also holds that layer's prepared bf16 operand tiles; it is held
-    through a weak reference to the layer, so it is freed with it and never re-bound to another one."""
-    n = int(L.lib().bbb_workspace_bytes(C.byref(desc) if desc is not None else None))
+    through a weak reference to the layer, so it is freed with it and never re-bound to another one.
+    ``kl_mc_draws`` > 0: the scratch of a Monte-Carlo KL call of that many draws instead
+    (bbb_kl_mc_workspace_bytes), a buffer of its own beside the layer call's."""
+    if kl_mc_draws:
+        n = int(L.lib().bbb_kl_mc_workspace_bytes(int(kl_mc_draws)))
+    else:
+        n = int(L.lib().bbb_workspace_bytes(C.byref(desc) if desc is not None else None))
+    kind = ("kl_mc",) if kl_mc_draws else ()
     if owner is None:
-        cache, key = _ws_cache, (device.index, torch.cuda.current_stream(device).cuda_stream)
+        cache, key = _ws_cache, (device.index, torch.cuda.current_stream(device).cuda_stream) + kind
     else:
         cache = _ws_layer.get(owner)
         if cache is None:
             cache = _ws_layer[owner] = {}
-        key = (device.index, _ws_slot)
+        key = (device.index, _ws_slot) + kind
     ws = cache.get(key)
     if ws is None or ws.numel() < n:
         if ws is not None:                        # a larger call (a BBB MC-sample fold) grows it: a graph captured on
@@ -551,7 +557,10 @@ class BayesLayerFn(torch.autograd.Function):
             oh, ow = out_hw(x.shape[2], x.shape[3], W_mu.shape[2], W_mu.shape[3], conv)
             yshape = (x.shape[0], W_mu.shape[0], oh, ow)
         y = torch.empty(yshape, dtype=x.dtype, device=dev)
+        # a mixture prior has no closed-form KL: the forward computes none (kl_out NULL) and the caller takes the layer's
+        # KL from KLMCFn; the `kl` returned here is then not a value
         kl = torch.empty((), dtype=torch.float32, device=dev)
+        no_kl = cfg.get("mixture") is not None
         eps_a = eps_b = None
         seed = stream_id = 0
         base = None
@@ -572,7 +581,7 @@ class BayesLayerFn(torch.autograd.Function):
         ws = workspace(dev, d, cfg.get("owner"))
         fn = lib.bbb_linear_forward_prior if conv is None else lib.bbb_conv2d_forward_prior
         rc = fn(C.byref(d), _ptr(x), _ptr(W_mu_c), _ptr(W_rho_c), _ptr(bias_mu), _ptr(bias_rho),
-                _ptr(y), _ptr(kl), _ptr(act_std), _ptr(eps_a), _ptr(eps_b),
+                _ptr(y), None if no_kl else _ptr(kl), _ptr(act_std), _ptr(eps_a), _ptr(eps_b),
                 C.c_uint64(seed), C.c_uint64(stream_id), _ptr(base), _ptr(ws), C.c_size_t(ws.numel()), _stream(dev),
                 prior_arg(cfg.get("prior")))
         L.check(rc, "bbb_linear_forward" if conv is None else "bbb_conv2d_forward")
@@ -587,6 +596,8 @@ class BayesLayerFn(torch.autograd.Function):
         ctx.fold = fold
         ctx.has_bias = has_bias
         ctx.save_for_backward(x, W_mu_c, W_rho_c, bias_mu, bias_rho, act_std, eps_a, eps_b)
+        if no_kl:
+            ctx.mark_non_differentiable(kl)
         return y, kl
 
     @staticmethod
@@ -635,7 +646,7 @@ class BayesLayerFn(torch.autograd.Function):
             L.check(rc, "bbb_*_backward")
         if gx is not None and gx.dtype != ctx.x_dtype:
             gx = gx.to(ctx.x_dtype)
-        if gkl is not None:
+        if gkl is not None and cfg.get("mixture") is None:
             gkl = gkl.contiguous().float()
             prior = cfg.get("prior")
             rc = lib.bbb_kl_backward_prior(_ptr(W_mu), _ptr(W_rho), C.c_uint64(W_mu.numel()),
@@ -766,6 +777,82 @@ class KLFn(torch.autograd.Function):
             L.check(rc, "bbb_kl_backward_prior")
             out += [g_mu, g_rho]
         return out[0], out[1], out[2], out[3], None, None, None, None
+
+
+def mixture_arg(mixture):
+    """The ``const bbb_mixture_prior*`` argument of the Monte-Carlo KL entry points, from (pi, sigma1, sigma2)."""
+    pi, sigma1, sigma2 = mixture
+    return C.byref(L.MixturePrior(float(pi), float(sigma1), float(sigma2)))
+
+
+def kl_draw_index(n_w: int, n: int, bias: bool = False) -> int:
+    """Which normal of the KL draw's Philox stream element `n` of W (or of the bias: |W| + n) takes."""
+    return int(n_w) + int(n) if bias else int(n)
+
+
+def fold_draws(rows_total: int):
+    """(n_draws, stream stride) of the Monte-Carlo KL of a layer call on `rows_total` rows: one draw per MC sample folded
+    into the batch (layer_fold), else None -- one draw, a 0-dim KL."""
+    if _noise.fold is None:
+        return None
+    rows, stride = _noise.fold
+    return int(rows_total) // rows, stride
+
+
+def kl_mc_forward(kl, W_mu, W_rho, bias_mu, bias_rho, mixture, seed, stream_id, base, stride=0, owner=None):
+    """bbb_kl_mc_forward into the fp32 device tensor ``kl``: kl.numel() draws, draw d from Philox stream stream_id
+    (+ the device scalar ``base``) + d * stride.  W_mu / W_rho contiguous."""
+    dev = W_mu.device
+    ws = workspace(dev, owner=owner, kl_mc_draws=kl.numel())
+    nb = 0 if bias_mu is None else bias_mu.numel()
+    rc = L.lib().bbb_kl_mc_forward(_ptr(W_mu), _ptr(W_rho), C.c_uint64(W_mu.numel()), _ptr(bias_mu), _ptr(bias_rho),
+                                   C.c_uint64(nb), mixture_arg(mixture), C.c_uint64(seed), C.c_uint64(stream_id),
+                                   _ptr(base), kl.numel(), C.c_uint64(stride & _MASK64), _ptr(kl), _ptr(ws),
+                                   C.c_size_t(ws.numel()), _stream(dev))
+    L.check(rc, "bbb_kl_mc_forward")
+
+
+class KLMCFn(torch.autograd.Function):
+    """Monte-Carlo KL(q || p) of a layer against the scale-mixture prior ``mixture`` = (pi, sigma1, sigma2)
+    (bbb_kl_mc_forward; Blundell et al. 2015, section 3.3).  Takes the next Philox stream id of the calling thread, as a
+    layer call takes its noise stream (next_stream, relative to the device base under stream_base), so the draw belongs
+    to the Monte-Carlo sample the call is made in.  ``draws`` = (n, stride): n estimates [n], draw d from stream id +
+    d * stride (the samples of an MC fold); None: one draw, 0-dim.  ``owner``: the layer whose private scratch the call
+    uses (calls that may run concurrently); None: the stream's shared scratch.  The backward draws the same eps again."""
+
+    @staticmethod
+    def forward(ctx, W_mu, W_rho, bias_mu, bias_rho, mixture, draws=None, owner=None):
+        _require_cuda(W_mu, "kl_loss (mixture prior)")
+        W_mu_c, W_rho_c = W_mu.contiguous(), W_rho.contiguous()
+        n_draws, stride = (1, 0) if draws is None else (int(draws[0]), int(draws[1]))
+        seed, stream_id = next_stream()
+        base = _noise.base
+        kl = torch.empty(n_draws, dtype=torch.float32, device=W_mu.device)
+        kl_mc_forward(kl, W_mu_c, W_rho_c, bias_mu, bias_rho, mixture, seed, stream_id, base, stride, owner)
+        ctx.save_for_backward(W_mu_c, W_rho_c, bias_mu, bias_rho)
+        ctx.call = (tuple(mixture), seed, stream_id, base, n_draws, stride)
+        return kl if draws is not None else kl.view(())
+
+    @staticmethod
+    def backward(ctx, gkl):
+        lib = L.lib()
+        W_mu, W_rho, bias_mu, bias_rho = ctx.saved_tensors
+        mixture, seed, stream_id, base, n_draws, stride = ctx.call
+        dev = W_mu.device
+        gkl = gkl.contiguous().float().reshape(-1)
+        out = []
+        for mu, rho, first in ((W_mu, W_rho, 0), (bias_mu, bias_rho, W_mu.numel())):
+            if mu is None:
+                out += [None, None]
+                continue
+            g_mu, g_rho = torch.zeros_like(mu), torch.zeros_like(rho)
+            rc = lib.bbb_kl_mc_backward(_ptr(mu), _ptr(rho), C.c_uint64(mu.numel()), C.c_uint64(first),
+                                        mixture_arg(mixture), C.c_uint64(seed), C.c_uint64(stream_id), _ptr(base),
+                                        n_draws, C.c_uint64(stride & _MASK64), _ptr(gkl), _ptr(g_mu), _ptr(g_rho),
+                                        _stream(dev))
+            L.check(rc, "bbb_kl_mc_backward")
+            out += [g_mu, g_rho]
+        return out[0], out[1], out[2], out[3], None, None, None
 
 
 # --------------------------------------------------------------------------- #

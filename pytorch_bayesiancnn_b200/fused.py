@@ -214,9 +214,20 @@ def _run(steps, x, overlap_prep, out, terms, owner, fold=None, kls_out=None):
     a few serial chains (default 3: layers 1,4 / 2,5 / 3) rather than all at once: six concurrent prep
     grids fill the machine and the first layer's prep -- the one the GEMM chain is waiting for -- was
     scheduled last (tools/timeline.py shows the start of each GEMM).  The KL sum
-    depends on the preps only and runs on the side as well."""
+    depends on the preps only and runs on the side as well.
+
+    A layer with a mixture prior (set_mixture_prior) computes no KL in its prep: its term is a Monte-Carlo draw per MC
+    sample (one, or the fold's samples), launched behind its prep on the prep's stream.  The chain then returns the
+    per-sample KL -- the layers' terms added in layer order, 0-dim or [samples] under a fold -- with ``terms`` as well."""
     dev = x.device
     kls = kls_out[:len(steps)] if kls_out is not None else torch.empty(len(steps), dtype=torch.float32, device=dev)
+    mixed = [i for i, st in enumerate(steps) if st.layer.mixture_values() is not None]
+    if mixed:
+        n_draws = 1 if fold is None else steps[0].batch // fold[0]
+        mix = torch.empty(len(mixed), n_draws, dtype=torch.float32, device=dev)
+        kl_of = [mix[mixed.index(i)] if i in mixed else kls[i] for i in range(len(steps))]
+    else:
+        kl_of = [kls[i] for i in range(len(steps))]
     snap = Fn.noise_snapshot()
     main = torch.cuda.current_stream(dev)
     chains = [_side_stream(dev, c) for c in range(min(_prep_chains(), len(steps)))] if overlap_prep else []
@@ -236,7 +247,7 @@ def _run(steps, x, overlap_prep, out, terms, owner, fold=None, kls_out=None):
             first_on_main = os.environ.get("BBB_B200_PREP0_MAIN", "1") == "1"
             ev0 = None
             if first_on_main:
-                run_step(steps[0], None, None, None, 0, kl=kls[0], noise=noise[0], phase=L.FUSED_PREP_ONLY, fold=fold)
+                run_step(steps[0], None, None, None, 0, kl=kl_of[0], noise=noise[0], phase=L.FUSED_PREP_ONLY, fold=fold)
                 ev0 = torch.cuda.Event()
                 ev0.record(main)
             for i, st in enumerate(steps):
@@ -244,13 +255,13 @@ def _run(steps, x, overlap_prep, out, terms, owner, fold=None, kls_out=None):
                     continue
                 side = chains[(i - 1) % len(chains)] if first_on_main else chains[i % len(chains)]
                 with torch.cuda.stream(side):
-                    run_step(st, None, None, None, 0, kl=kls[i], noise=noise[i], phase=L.FUSED_PREP_ONLY, fold=fold)
+                    run_step(st, None, None, None, 0, kl=kl_of[i], noise=noise[i], phase=L.FUSED_PREP_ONLY, fold=fold)
                     ev = torch.cuda.Event()
                     ev.record(side)
                     events[i] = ev
             for side in chains[1:]:
                 chains[0].wait_stream(side)
-            if not terms:
+            if not terms and not mixed:
                 with torch.cuda.stream(chains[0]):
                     if ev0 is not None:
                         chains[0].wait_event(ev0)
@@ -265,16 +276,24 @@ def _run(steps, x, overlap_prep, out, terms, owner, fold=None, kls_out=None):
             if overlap_prep:
                 if events[i] is not None:
                     main.wait_event(events[i])
-                cur, cur_sq, cur_pitch = run_step(st, nxt, cur, cur_sq, cur_pitch, kl=kls[i], noise=noise[i],
+                cur, cur_sq, cur_pitch = run_step(st, nxt, cur, cur_sq, cur_pitch, kl=kl_of[i], noise=noise[i],
                                                   phase=L.FUSED_SKIP_PREP, y_into=y_into, fold=fold)
             else:
-                cur, cur_sq, cur_pitch = run_step(st, nxt, cur, cur_sq, cur_pitch, kl=kls[i], noise=noise[i], y_into=y_into, fold=fold)
-        if terms:
+                cur, cur_sq, cur_pitch = run_step(st, nxt, cur, cur_sq, cur_pitch, kl=kl_of[i], noise=noise[i], y_into=y_into, fold=fold)
+        if mixed:
+            # element-wise adds in layer order (the main stream has waited for every prep): sample j's sum is the same
+            # whether the samples are folded or run one by one
+            kl_total = kl_of[0]
+            for t in kl_of[1:]:
+                kl_total = kl_total + t
+            if fold is None:
+                kl_total = kl_total.reshape(())
+        elif terms:
             kl_total = kls
-            if owner is not None:
-                owner.used = True
         elif not overlap_prep:
             kl_total = kls.sum()
+        if terms and owner is not None:
+            owner.used = True
     except BaseException:
         Fn.noise_restore(snap)                 # a retry / fallback sees the stream ids and eps queue it would have seen
         raise
@@ -287,8 +306,9 @@ def _run(steps, x, overlap_prep, out, terms, owner, fold=None, kls_out=None):
 
 
 def _draw_noise(st, B, dev):
-    """(eps_a, eps_b, seed, stream_id, base) for one layer call, consuming the external-eps
-    queue / the Philox stream counter exactly like the unfused layer would."""
+    """(eps_a, eps_b, seed, stream_id, base, kl_stream) for one layer call, consuming the external-eps
+    queue / the Philox stream counter exactly like the unfused layer would.  kl_stream: (seed, stream id) of the
+    Monte-Carlo KL draw of a layer with a mixture prior -- the next id behind the layer's own -- else None."""
     m = st.layer
     eps_a = eps_b = None
     seed = stream_id = 0
@@ -303,7 +323,8 @@ def _draw_noise(st, B, dev):
     else:
         seed, stream_id = Fn.next_stream()
         base = Fn._noise.base
-    return eps_a, eps_b, seed, stream_id, base
+    kl_stream = Fn.next_stream() if m.mixture_values() is not None else None
+    return eps_a, eps_b, seed, stream_id, base, kl_stream
 
 
 def run_step(st, nxt, cur, cur_sq, cur_pitch, kl=None, noise=None, phase=0, y_into=None, fold=None):
@@ -330,18 +351,26 @@ def run_step(st, nxt, cur, cur_sq, cur_pitch, kl=None, noise=None, phase=0, y_in
         else:
             pitch, y, y_sq = 0, torch.empty(B, cout, oh, ow, dtype=torch.float32, device=dev), None
         if kl is None:
-            kl = torch.empty((), dtype=torch.float32, device=dev)
+            kl = torch.empty(st.batch // fold[0] if (fold is not None and m.mixture_values() is not None) else (),
+                             dtype=torch.float32, device=dev)
         if noise is None:
             noise = _draw_noise(st, B, dev)
-        eps_a, eps_b, seed, stream_id, base = noise
+        eps_a, eps_b, seed, stream_id, base, kl_stream = noise
+        mixture = m.mixture_values()
         ws = Fn.workspace(dev, d, m)
         rc = lib.bbb_layer_forward_fused_prior(
             C.byref(d), Fn._ptr(cur), Fn._ptr(cur_sq), st.in_layout, in_pitch, st.prev_hw,
             Fn._ptr(m.W_mu), Fn._ptr(m.W_rho), Fn._ptr(m.bias_mu), Fn._ptr(m.bias_rho),
-            Fn._ptr(y), Fn._ptr(y_sq), st.out_layout, pitch, Fn._ptr(kl), Fn._ptr(eps_a), Fn._ptr(eps_b),
+            Fn._ptr(y), Fn._ptr(y_sq), st.out_layout, pitch, None if mixture is not None else Fn._ptr(kl),
+            Fn._ptr(eps_a), Fn._ptr(eps_b),
             C.c_uint64(seed), C.c_uint64(stream_id), Fn._ptr(base), Fn._ptr(ws), C.c_size_t(ws.numel()),
             Fn._stream(dev), Fn.prior_arg(m.prior_tensors()))
         L.check(rc, "bbb_layer_forward_fused_prior")
         if phase != L.FUSED_SKIP_PREP:
+            if mixture is not None:             # kl: one entry per folded MC sample, each from its own stream
+                Fn.kl_mc_forward(kl, m.W_mu, m.W_rho, m.bias_mu, m.bias_rho, mixture, kl_stream[0], kl_stream[1],
+                                 Fn._noise.base, fold[1] if fold is not None else 0, m)
+                if fold is None:
+                    kl = kl.reshape(())
             m._kl_cache = (kl, m._versions(), torch.is_grad_enabled())
         return y, y_sq, pitch

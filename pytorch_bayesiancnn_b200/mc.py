@@ -142,8 +142,9 @@ class MCForward:
     """``out = MCForward(net, example_x, num_ens, ...)(x, labels=None)`` -- the sharded MC step on the engine.
 
     Returns a dict of device tensors (the same objects every call; identical on all ranks):
-      log_outputs [B,C], kl (= sum_j kl_j / num_ens), and with ``want_uncertainty`` pred / epistemic / aleatoric [B,C]
-      and entropy [B]; with ``with_labels`` head = [loss, nll, accuracy, beta*kl] (metrics.py:12-14, 23-24); with
+      log_outputs [B,C], kl (= sum_j kl_j / num_ens; with mixture-prior layers kl_j is sample j's own Monte-Carlo
+      estimate, drawn on sample j's streams whatever the sharding or fold), and with ``want_uncertainty`` pred /
+      epistemic / aleatoric [B,C] and entropy [B]; with ``with_labels`` head = [loss, nll, accuracy, beta*kl] (metrics.py:12-14, 23-24); with
       ``want_information`` (needs ``want_uncertainty``) expected_entropy = mean_s H[p_hat_s] and mutual_info = entropy -
       expected_entropy [B] (include/bbb_b200.h, bbb_mc_exchange_info).
 
@@ -369,12 +370,24 @@ class MCForward:
         self._exchange(kl_ptr, n_kl)
         return self.out
 
+    def _mean_kl(self, kls, par=0):
+        """Nets with mixture-prior layers: every sample has its own KL estimate.  ``kls``: the local samples' KLs in
+        local order (0-dim tensors, or vectors of folded samples).  Their mean goes where the exchange reads one sample's
+        KL, which it multiplies by the local sample count.  The sum is taken over one [n_local] vector on every path, so
+        folded and sample-loop steps agree bit for bit."""
+        v = torch.cat([torch.as_tensor(k, dtype=torch.float32, device=self.dev).detach().reshape(-1) for k in kls])
+        one = self.kl_one_all[par:par + 1]
+        one.copy_((v.sum() / v.numel()).reshape(1))
+        return Fn._ptr(one), 1
+
     def _chain(self, x, base=None, advance=False, par=0):
         """This rank's samples through the engine into the sample buffer ``par``.  A fused chain writes its logits
         straight into it and hands over its per-layer KL scalars un-summed (fused.direct_output).  Returns the (pointer,
         count) of the floats whose sum is one sample's KL."""
         from . import fused
         from .graph import _STRIDE
+        from .modules import has_mixture
+        mixture, sample_kls = has_mixture(self.net), []
         logits_buf = self.logits_all[par]
         kl_buf = self.kl_terms_all[par] if self.overlap else None
         inc = _STRIDE * self.inflight
@@ -394,7 +407,7 @@ class MCForward:
                     _, kls = fused._run(self.fold_steps, x, True, logits_buf.view(len(self.ids) * nb, self.C), True, None,
                                         fold=self.fold, kls_out=kl_buf)
                 self._kl_terms = kls
-                kl_ptr, n_kl = Fn._ptr(kls), kls.numel()
+                kl_ptr, n_kl = self._mean_kl([kls], par) if mixture else (Fn._ptr(kls), kls.numel())
             if self._groups is not None:
                 # group (s0, n): local samples s0 .. s0+n-1 in one pass over n x nb rows; row block k is global sample
                 # ids[s0] + k * Rs (stream stride Rs << 40, as in the fused fold) and lands in logits_buf[s0 + k]
@@ -406,7 +419,9 @@ class MCForward:
                             Fn.layer_fold(nb, self.sample_shards << 40):
                         logits, kl = self.net(xr[:n * nb])
                     logits_buf[s0:s0 + n].view(n * nb, self.C).copy_(logits.reshape(n * nb, self.C))
-                    if gi == 0:                               # every sample has the same KL, computed once per pass
+                    if mixture:                               # [n] per-sample estimates of this pass
+                        sample_kls.append(kl)
+                    elif gi == 0:                               # every sample has the same KL, computed once per pass
                         one = self.kl_one_all[par:par + 1]
                         one.copy_(torch.as_tensor(kl, dtype=torch.float32, device=self.dev).reshape(1))
                         kl_ptr, n_kl = Fn._ptr(one), 1
@@ -416,7 +431,9 @@ class MCForward:
                     logits, kl = self.net(x)
                 if not hook.used:
                     logits_buf[k].copy_(logits.reshape(nb, self.C))
-                if k == 0:
+                if mixture:
+                    sample_kls.append(kl)
+                elif k == 0:
                     if hook.used:
                         self._kl_terms = kl                       # per-layer scalars of sample 0 (every sample has the same KL)
                         kl_ptr, n_kl = Fn._ptr(kl), kl.numel()
@@ -424,6 +441,8 @@ class MCForward:
                         one = self.kl_one_all[par:par + 1]
                         one.copy_(torch.as_tensor(kl, dtype=torch.float32, device=self.dev).reshape(1))
                         kl_ptr, n_kl = Fn._ptr(one), 1
+            if sample_kls:
+                kl_ptr, n_kl = self._mean_kl(sample_kls, par)
             if not self.ids and self.group_index == 0:
                 raise L.EngineError("MCForward: sample group 0 must own a sample")
         return kl_ptr, n_kl
@@ -975,8 +994,12 @@ class MCTrainStep(MCForward):
                 logits.append(lg)
                 kls.append(kl)
                 self.logits[k].copy_(lg.detach().reshape(self.nb, self.C))
+        from .modules import has_mixture
+        mixture = has_mixture(self.net)        # per-sample KL estimates: kls[i] is [n] for a folded group of n samples
         kl_ptr, n_kl = None, 0
-        if self.ids:
+        if self.ids and mixture:
+            kl_ptr, n_kl = self._mean_kl(kls)
+        elif self.ids:
             self.kl_one.copy_(kls[0].detach())
             kl_ptr, n_kl = Fn._ptr(self.kl_one), 1
         self._exchange(kl_ptr, n_kl)
@@ -1004,9 +1027,9 @@ class MCTrainStep(MCForward):
                 # bf16 logits (bf16 activations) take their gradient in bf16, as autograd would cast it
                 grads.append((blocks[0] if len(blocks) == 1 else torch.cat(blocks)).to(lg_dtype))
             # the KL does not depend on the rows: one block per sample group adds its gradient, n * beta / S for a
-            # folded group of n samples
-            wkl = train_fold_kl_weights(self._groups, self.beta, self.num_ens) if self._groups is not None else \
-                [self.beta / S] * len(kls)
+            # folded group of n samples (with mixture-prior layers its KL is the n samples' estimates: beta / S each)
+            wkl = train_fold_kl_weights(self._groups, self.beta, self.num_ens) \
+                if self._groups is not None and not mixture else [self.beta / S] * len(kls)
             kl_t = [(k_, w_) for k_, w_ in zip(kls, wkl) if torch.is_tensor(k_) and k_.requires_grad] \
                 if self.block == 0 else []
             kl_g = [torch.full_like(k_, w_) for k_, w_ in kl_t]

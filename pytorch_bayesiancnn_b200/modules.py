@@ -18,9 +18,17 @@ Per-weight Gaussian priors (``set_prior`` / ``posterior_as_prior``): the KL of e
 its own N(mu_p, sigma_p^2), e.g. the posterior of a previous task (variational continual learning) or a prior centred on
 pretrained weights.  The prior lives in four fp32 buffers (``W_prior_mu``, ``W_prior_sigma``, ``bias_prior_mu``,
 ``bias_prior_sigma``) that exist only after ``set_prior``: a layer that never had one keeps the reference's state_dict.
+
+Scale-mixture priors (``set_mixture_prior`` / ``mixture_prior``): the prior Bayes by Backprop was published with (Blundell
+et al. 2015, section 3.3), pi N(0, sigma1^2) + (1 - pi) N(0, sigma2^2).  It has no closed-form KL: the layer's KL is then
+a Monte-Carlo estimate of KL(q || p) from one weight draw per layer call (functional.KLMCFn), on a Philox stream of the
+call's own, so every Monte-Carlo sample has its own estimate.  ``kl_convention`` does not apply to it.  A layer has one
+prior: the scalar pair, the tensors or the mixture.  The mixture's three values live in the fp32 buffer
+``mixture_prior``, which exists only after ``set_mixture_prior``.
 """
 from __future__ import annotations
 
+import math
 import os
 
 import torch
@@ -37,6 +45,7 @@ _DEFAULT_PRIORS = {
     "posterior_rho_initial": (-3, 0.1),
 }
 _PRIOR_BUFFERS = ("W_prior_mu", "W_prior_sigma", "bias_prior_mu", "bias_prior_sigma")
+_MIXTURE_BUFFER = "mixture_prior"
 _prior_epoch = 0          # bumped whenever some layer's prior buffers are created, replaced, moved or removed (PriorGuard)
 
 
@@ -150,6 +159,7 @@ class _BayesLayer(ModuleWrapper):
         self.math = _default_math()
         self.kl_convention = "reference"
         self._kl_cache = None
+        self._mixture = None           # (pi, sigma1, sigma2) after set_mixture_prior: the host's copy of the buffer
         self.reset_parameters()
 
     def reset_parameters(self):
@@ -168,7 +178,7 @@ class _BayesLayer(ModuleWrapper):
         kl_convention or the prior -- scalar or tensor (set_prior) -- after a forward must not return the old value)."""
         ps = (self.W_mu, self.W_rho, self.bias_mu, self.bias_rho) + tuple(self._buffers.get(n) for n in _PRIOR_BUFFERS)
         return tuple((p._version, p.data_ptr()) if p is not None else None for p in ps) + (
-            self.kl_convention, float(self.prior_mu), float(self.prior_sigma))
+            self.kl_convention, float(self.prior_mu), float(self.prior_sigma), self.mixture_values())
 
     # -- per-weight priors ----------------------------------------------------
     def prior_tensors(self):
@@ -214,7 +224,35 @@ class _BayesLayer(ModuleWrapper):
             else:
                 self.register_buffer(name, torch.empty(shape, dtype=torch.float32, device=dev).copy_(t))
                 _prior_moved()
+        self._drop_mixture()
         return self
+
+    # -- scale-mixture prior --------------------------------------------------
+    def mixture_values(self):
+        """(pi, sigma1, sigma2) after set_mixture_prior, or None: the prior is a Gaussian (scalar or tensor)."""
+        return self.__dict__.get("_mixture")
+
+    def set_mixture_prior(self, pi=0.5, sigma1=1.0, sigma2=math.exp(-6)):
+        """Take the KL against the scale mixture pi N(0, sigma1^2) + (1 - pi) N(0, sigma2^2) from now on (Blundell et al.
+        2015, section 3.3; usually sigma1 > sigma2, a wide slab and a narrow spike).  The layer's KL becomes a Monte-Carlo
+        estimate of KL(q || p): every layer call draws one weight sample for it on a Philox stream id of its own, taken
+        after the layer's noise stream (the layer's outputs do not change), and under an MC-sample fold one per sample.
+        kl_convention does not apply.  0 < pi <= 1 and finite sigma1, sigma2 > 0 (ValueError).  Replaces a tensor prior
+        (set_prior); clear_prior goes back to the scalar prior.  The values are kept, rounded to fp32, in the 3-element
+        buffer ``mixture_prior`` -- saved in the state_dict, following .to() -- and passed to the kernels by value: a
+        captured engine (MCForward, GraphedForward) refuses its next replay once they changed (PriorGuard); mc_forward
+        and evaluate build new engines.  Change them through this method, not by writing to the buffer."""
+        vals = _check_mixture(pi, sigma1, sigma2)
+        self.clear_prior()
+        self.register_buffer(_MIXTURE_BUFFER, torch.tensor(vals, dtype=torch.float32, device=self.W_mu.device))
+        self._mixture = vals
+        _prior_moved()
+        return self
+
+    def _drop_mixture(self):
+        if self._buffers.pop(_MIXTURE_BUFFER, None) is not None or self.mixture_values() is not None:
+            self._mixture = None
+            _prior_moved()
 
     def clear_prior(self):
         """Back to the scalar prior_mu / prior_sigma: removes the prior buffers.  A captured engine that read them
@@ -222,6 +260,7 @@ class _BayesLayer(ModuleWrapper):
         removed = [self._buffers.pop(n, None) for n in _PRIOR_BUFFERS]
         if any(t is not None for t in removed):
             _prior_moved()
+        self._drop_mixture()
         return self
 
     def _apply(self, fn, *args, **kwargs):
@@ -242,8 +281,20 @@ class _BayesLayer(ModuleWrapper):
             if prefix + n in state_dict and self._buffers.get(n) is None:
                 self.register_buffer(n, torch.zeros(shape, dtype=torch.float32, device=self.W_mu.device))
                 _prior_moved()
+        # likewise the mixture prior; its values are read back to the host once, here
+        has_mix = prefix + _MIXTURE_BUFFER in state_dict
+        if has_mix and self._buffers.get(_MIXTURE_BUFFER) is None:
+            self.register_buffer(_MIXTURE_BUFFER, torch.zeros(3, dtype=torch.float32, device=self.W_mu.device))
         super()._load_from_state_dict(state_dict, prefix, local_metadata, strict, missing_keys, unexpected_keys,
                                       error_msgs)
+        if has_mix and tuple(self._buffers[_MIXTURE_BUFFER].shape) == (3,):
+            try:
+                self._mixture = _check_mixture(*self._buffers[_MIXTURE_BUFFER].tolist())
+            except ValueError as e:
+                error_msgs.append(f"{prefix}{_MIXTURE_BUFFER}: {e}")
+                self._buffers.pop(_MIXTURE_BUFFER)
+                self._mixture = None
+            _prior_moved()
 
     def _cfg(self, sample):
         return {
@@ -257,6 +308,7 @@ class _BayesLayer(ModuleWrapper):
             "act": L.ACT_NONE,
             "owner": self,
             "prior": self.prior_tensors(),
+            "mixture": self.mixture_values(),
         }
 
     def forward(self, x, sample=True):
@@ -264,6 +316,9 @@ class _BayesLayer(ModuleWrapper):
         cfg = self._cfg(stochastic)
         cfg["grad_enabled"] = torch.is_grad_enabled()  # grad mode is always off inside Function.forward
         y, kl = Fn.BayesLayerFn.apply(x, self.W_mu, self.W_rho, self.bias_mu, self.bias_rho, cfg)
+        if cfg["mixture"] is not None:                  # the forward computed no KL: one Monte-Carlo draw per MC sample
+            kl = Fn.KLMCFn.apply(self.W_mu, self.W_rho, self.bias_mu, self.bias_rho, cfg["mixture"],
+                                 Fn.fold_draws(x.shape[0]), self)
         self._kl_cache = (kl, self._versions(), torch.is_grad_enabled())
         return y
 
@@ -271,10 +326,14 @@ class _BayesLayer(ModuleWrapper):
         """0-dim tensor, differentiable w.r.t. mu and rho.  Normally the scalar the
         fused forward kernel just produced; recomputed by the stand-alone KL kernel
         if no forward preceded it or the parameters changed since (the reference
-        would raise AttributeError / use a stale sigma there -- SURVEY D7)."""
+        would raise AttributeError / use a stale sigma there -- SURVEY D7).  With a mixture prior the scalar is a
+        Monte-Carlo estimate: the preceding forward's draw (under an MC-sample fold, one per sample: a vector), or a new
+        draw on the next Philox stream id when there is none."""
         c = self._kl_cache
         if c is not None and c[1] == self._versions() and (c[2] or not torch.is_grad_enabled()):
             return c[0]
+        if self.mixture_values() is not None:
+            return Fn.KLMCFn.apply(self.W_mu, self.W_rho, self.bias_mu, self.bias_rho, self.mixture_values(), None, self)
         return Fn.KLFn.apply(self.W_mu, self.W_rho, self.bias_mu, self.bias_rho, float(self.prior_mu),
                              float(self.prior_sigma), L.KL_BY_NAME[self.kl_convention], self.prior_tensors())
 
@@ -359,10 +418,36 @@ class BBBLRTLinear(_LinearMixin, _BayesLayer):
         self._init_linear(in_features, out_features, bias, priors)
 
 
+def _check_mixture(pi, sigma1, sigma2):
+    """(pi, sigma1, sigma2) rounded to fp32, as the engine takes them; ValueError unless 0 < pi <= 1 and sigma1, sigma2
+    are finite, > 0 and have squares within fp32 range (what bbb_kl_mc_forward checks)."""
+    pi, sigma1, sigma2 = torch.tensor([float(pi), float(sigma1), float(sigma2)], dtype=torch.float32).tolist()
+    if not 0.0 < pi <= 1.0:
+        raise ValueError(f"mixture prior: pi must be in (0, 1], got {pi}")
+    for name, v in (("sigma1", sigma1), ("sigma2", sigma2)):
+        if not (math.isfinite(v) and v > 0.0):
+            raise ValueError(f"mixture prior: {name} must be finite and > 0, got {v}")
+        h = torch.tensor(0.5 / (v * v), dtype=torch.float32).item()
+        if not math.isfinite(h) or h == 0.0:
+            raise ValueError(f"mixture prior: {name}^2 is outside fp32 range, got {v}")
+    return pi, sigma1, sigma2
+
+
+def has_mixture(net: nn.Module) -> bool:
+    """Does a Bayesian layer of `net` take its KL against a mixture prior (a per-sample Monte-Carlo estimate)?"""
+    return any(isinstance(m, _BayesLayer) and m.mixture_values() is not None for m in net.modules())
+
+
 def prior_signature(net: nn.Module) -> tuple:
-    """Where every Bayesian layer of `net` keeps its prior: the buffers' addresses, or None for the scalar prior."""
-    return tuple(None if m.prior_tensors() is None else tuple(None if t is None else t.data_ptr() for t in m.prior_tensors())
-                 for m in net.modules() if isinstance(m, _BayesLayer))
+    """What a captured graph holds of every Bayesian layer's prior: the tensor prior's buffer addresses, the mixture
+    prior's values (kernel arguments), or None for the scalar prior."""
+    def one(m):
+        if m.mixture_values() is not None:
+            return ("mixture",) + m.mixture_values()
+        if m.prior_tensors() is None:
+            return None
+        return tuple(None if t is None else t.data_ptr() for t in m.prior_tensors())
+    return tuple(one(m) for m in net.modules() if isinstance(m, _BayesLayer))
 
 
 class PriorGuard:
@@ -389,7 +474,7 @@ class PriorGuard:
         if not self.ok():
             raise L.EngineError(f"{what}: a layer's prior was set, cleared, re-allocated or moved since this engine's "
                                 "CUDA graphs were captured; build a new engine (an in-place set_prior of the same shapes "
-                                "is read by the next replay)")
+                                "is read by the next replay; new set_mixture_prior values are not)")
 
 
 def posterior_as_prior(net: nn.Module) -> nn.Module:
@@ -403,4 +488,14 @@ def posterior_as_prior(net: nn.Module) -> nn.Module:
                 m.set_prior(m.W_mu.detach(), torch.log1p(torch.exp(m.W_rho.detach())),
                             m.bias_mu.detach() if m.use_bias else None,
                             torch.log1p(torch.exp(m.bias_rho.detach())) if m.use_bias else None)
+    return net
+
+
+def mixture_prior(net: nn.Module, pi=0.5, sigma1=1.0, sigma2=math.exp(-6)) -> nn.Module:
+    """Give every Bayesian layer of `net` the scale-mixture prior pi N(0, sigma1^2) + (1 - pi) N(0, sigma2^2) of Blundell
+    et al. 2015 (set_mixture_prior): the net's KL is from then on the sum of the layers' Monte-Carlo estimates, one draw
+    per layer and Monte-Carlo sample."""
+    for m in net.modules():
+        if isinstance(m, _BayesLayer):
+            m.set_mixture_prior(pi, sigma1, sigma2)
     return net
