@@ -203,8 +203,10 @@ enum { BBB_LAYOUT_NCHW_F32 = 0,      /* reference layout: [B, C, H, W] fp32     
  * desc->reserved[0] splits the call so the parameter-only half can run on a side stream, off
  * the activation critical path: BBB_FUSED_PREP_ONLY launches just the weight-prep kernel
  * (sigma, eps, bf16 operand tiles, KL -> kl_out; x/y unused), BBB_FUSED_SKIP_PREP just the GEMM
- * kernel (the caller orders it after the prep, e.g. with an event).  0 = both, in order.  Bits 8..30 of reserved[0]
- * carry the first image of a row block, as on bbb_conv2d_forward (the phase stays in bits 0..1).
+ * kernel (the caller orders it after the prep, e.g. with an event).  0 = both, in order.  BBB_FUSED_NO_TIMELINE
+ * (or'ed in): the call's kernels take no slot of the debug timeline (bbb_debug_set_timeline) -- for launches outside the
+ * step being traced, such as operand tiles prepared once per parameter version.  Bits 8..30 of reserved[0]
+ * carry the first image of a row block, as on bbb_conv2d_forward (the phase stays in bits 0..2).
  * desc->reserved[1] > 0 folds Monte-Carlo samples into the batch (in-kernel Philox noise only; what
  * uncertainty_estimation.py:38-41 does by repeating the input): row b of the batch is image b % reserved[1] of sample
  * s = b / reserved[1], whose noise comes from Philox stream stream_id + s * stride, stride = the uint64 in reserved[2]
@@ -214,7 +216,7 @@ enum { BBB_LAYOUT_NCHW_F32 = 0,      /* reference layout: [B, C, H, W] fp32     
  * times the operand workspace (bbb_workspace_bytes of the folding desc).  Either way the KL is computed once, as by an
  * unfolded call.  The gather path (an NCHW input the stride-4 kernel does not take) does not fold.  The NCHW input of
  * the first layer then holds reserved[1] images (it is not repeated). */
-enum { BBB_FUSED_PREP_ONLY = 1, BBB_FUSED_SKIP_PREP = 2 };
+enum { BBB_FUSED_PREP_ONLY = 1, BBB_FUSED_SKIP_PREP = 2, BBB_FUSED_NO_TIMELINE = 4 };
 int bbb_layer_forward_fused(const bbb_layer_desc* desc,
                             const void* x, const void* x_sq, int32_t in_layout, int32_t in_pitch, int32_t prev_hw,
                             const float* W_mu, const float* W_rho,
@@ -356,6 +358,17 @@ int bbb_lrt_noise_grad(const bbb_layer_desc* desc, const float* grad_y, const fl
 /* *base += inc on the device (one tiny kernel; put it at the head of a captured
  * graph so each replay moves every layer to a fresh Philox stream). */
 int bbb_noise_advance(uint64_t* base, uint64_t inc, void* cuda_stream);
+
+/* One step of a Monte-Carlo engine that keeps steps in flight, enqueued in one host call from the raw handles of its
+ * captured graphs (cudaGraphExec_t), streams (cudaStream_t) and events (cudaEvent_t):
+ *   run_stream != caller_stream: record in_ready on caller_stream, run_stream waits for it (the caller's work so far);
+ *   run_stream waits for wait_a and wait_b (each nullable: e.g. the last exchange that read this step's buffers);
+ *   chain_exec launched on run_stream, chain_done recorded there; result_stream waits for chain_done;
+ *   exch_exec launched on result_stream, exch_done recorded there.
+ * The same work as the runtime calls one by one, without a host round trip per call, so that the host keeps ahead of
+ * steps of ~0.1 ms.  Enqueues no kernel of its own. */
+int bbb_mc_graph_step(void* caller_stream, void* run_stream, void* in_ready, void* wait_a, void* wait_b,
+                      void* chain_exec, void* chain_done, void* result_stream, void* exch_exec, void* exch_done);
 
 /* Monte-Carlo combine that sits directly above the path (main_bayesian.py:46-53,
  * utils.py:14-22): logits [S, B, C] fp32 -> log_outputs [B, C] =

@@ -19,7 +19,7 @@ MATH_FP32, MATH_BF16_TC, MATH_AUTO, MATH_TF32_TC = 0, 1, 2, 3
 KL_REFERENCE, KL_TEXTBOOK = 0, 1
 ACT_NONE, ACT_SOFTPLUS, ACT_RELU = 0, 1, 2
 LAYOUT_NCHW_F32, LAYOUT_PACKED_BF16, LAYOUT_ROWMAJOR_F32 = 0, 1, 2
-FUSED_PREP_ONLY, FUSED_SKIP_PREP = 1, 2
+FUSED_PREP_ONLY, FUSED_SKIP_PREP, FUSED_NO_TIMELINE = 1, 2, 4
 
 MATH_BY_NAME = {"fp32": MATH_FP32, "bf16": MATH_BF16_TC, "auto": MATH_AUTO, "tf32": MATH_TF32_TC}
 KL_BY_NAME = {"reference": KL_REFERENCE, "textbook": KL_TEXTBOOK}
@@ -35,6 +35,7 @@ SYMBOLS = (
     "bbb_mc_metrics_bytes", "bbb_mc_exchange_metrics", "bbb_lrt_noise_grad",
     "bbb_conv2d_forward_prior", "bbb_linear_forward_prior", "bbb_layer_forward_fused_prior", "bbb_kl_forward_prior",
     "bbb_kl_backward_prior", "bbb_kl_mc_workspace_bytes", "bbb_kl_mc_forward", "bbb_kl_mc_backward",
+    "bbb_mc_graph_step",
 )
 MC_MOMENTS, MC_NORMALIZED, MC_INFO = 1, 2, 4
 MC_CAL_BINS = 15                 # BBB_MC_CAL_BINS: calibration bins of the evaluation accumulator
@@ -138,6 +139,8 @@ def _bind(lib):
         getattr(lib, name).restype = C.c_int
     lib.bbb_noise_advance.argtypes = [vp, u64, vp]
     lib.bbb_noise_advance.restype = C.c_int
+    lib.bbb_mc_graph_step.argtypes = [vp] * 10
+    lib.bbb_mc_graph_step.restype = C.c_int
     lib.bbb_last_error.argtypes = []
     lib.bbb_last_error.restype = C.c_char_p
     lib.bbb_abi_version.argtypes = []

@@ -410,6 +410,7 @@ int bbb_layer_forward_fused_prior(const bbb_layer_desc* d, const void* x, const 
     if (int rc = fused_check(d, g, in_layout, in_pitch, prev_hw, out_layout, out_pitch, s4)) return rc;
     const bool prep_only = (d->reserved[0] & BBB_FUSED_PREP_ONLY) != 0, skip_prep = (d->reserved[0] & BBB_FUSED_SKIP_PREP) != 0;
     if (prep_only && skip_prep) return fail(BBB_E_INVALID, "PREP_ONLY and SKIP_PREP are exclusive");
+    const bool timed = (d->reserved[0] & BBB_FUSED_NO_TIMELINE) == 0;
     if (!W_mu || !W_rho || (!prep_only && (!x || !y))) return fail(BBB_E_INVALID, "NULL tensor pointer");
     if (d->has_bias && (!bias_mu || !bias_rho)) return fail(BBB_E_INVALID, "has_bias set but bias pointers NULL");
     if (int rc = check_prior(prior, d->has_bias != 0)) return rc;
@@ -427,14 +428,14 @@ int bbb_layer_forward_fused_prior(const bbb_layer_desc* d, const void* x, const 
         // stride-4 first layer: the tensor core reads its A operand straight from the staged image (conv_s4_tc.cuh)
         bbb::S4Args a;
         layer_args(a, d, g, W_mu, W_rho, bias_mu, bias_rho, kl_out, eps_a, eps_b, seed, stream_id, stream_base, ws,
-                   bbb::conv_s4_bias_offset(g), fold, "conv_s4_prep", !skip_prep, "conv_s4", !prep_only);
+                   bbb::conv_s4_bias_offset(g), fold, "conv_s4_prep", timed && !skip_prep, "conv_s4", timed && !prep_only);
         a.x = (const float*)x; a.y = y; a.y_sq = y_sq; a.out_pitch = out_pitch;
         cudaError_t e = bbb::launch_conv_s4(a, st, !skip_prep, !prep_only, &nl, prior_ptrs(prior, kl_out));
         if (e != cudaSuccess) return cuda_fail(e, "conv_s4 launch");
     } else if (in_layout == BBB_LAYOUT_NCHW_F32) {
         bbb::TcArgs a;                  // fold.rows = 0: fused_check refuses a fold on the gather path
         layer_args(a, d, g, W_mu, W_rho, bias_mu, bias_rho, kl_out, eps_a, eps_b, seed, stream_id, stream_base, ws,
-                   bbb::tc_bias_offset(g, false), fold, "weight_prep", !skip_prep, "gemm_tc", !prep_only);
+                   bbb::tc_bias_offset(g, false), fold, "weight_prep", timed && !skip_prep, "gemm_tc", timed && !prep_only);
         a.x = x; a.y = y; a.act_std = nullptr; a.act_dtype = d->act_dtype; a.tf32 = 0;
         a.skip_prep = skip_prep; a.prep_only = prep_only; a.y_sq = y_sq; a.out_mode = out_mode == 1 ? 2 : out_mode; a.out_pitch = out_pitch; a.pool = pool;
         cudaError_t e = bbb::launch_fwd_tc(a, st, sm_count(), &nl, prior_ptrs(prior, kl_out));
@@ -442,7 +443,7 @@ int bbb_layer_forward_fused_prior(const bbb_layer_desc* d, const void* x, const 
     } else if (in_layout == BBB_LAYOUT_PACKED_BF16) {
         bbb::FusedArgs a;
         layer_args(a, d, g, W_mu, W_rho, bias_mu, bias_rho, kl_out, eps_a, eps_b, seed, stream_id, stream_base, ws,
-                   bbb::fused_bias_offset(g), fold, "tap_prep", !skip_prep, "tap_gemm", !prep_only);
+                   bbb::fused_bias_offset(g), fold, "tap_prep", timed && !skip_prep, "tap_gemm", timed && !prep_only);
         a.prev_hw = prev_hw; a.y = y; a.y_sq = y_sq; a.out_mode = out_mode; a.out_pitch = out_pitch; a.pool = pool;
         a.in_pitch = in_pitch;
         const char* why = "";
@@ -782,6 +783,26 @@ int bbb_noise_advance(uint64_t* base, uint64_t inc, void* cuda_stream) {
     if (e != cudaSuccess) return cuda_fail(e, "noise_advance launch");
     g_launches += 1;
     return BBB_OK;
+}
+
+int bbb_mc_graph_step(void* caller_stream, void* run_stream, void* in_ready, void* wait_a, void* wait_b,
+                      void* chain_exec, void* chain_done, void* result_stream, void* exch_exec, void* exch_done) {
+    if (!chain_exec || !chain_done || !exch_exec || !exch_done || (run_stream != caller_stream && !in_ready))
+        return fail(BBB_E_INVALID, "bbb_mc_graph_step: NULL graph or event");
+    const cudaStream_t cur = (cudaStream_t)caller_stream, run = (cudaStream_t)run_stream, rs = (cudaStream_t)result_stream;
+    cudaError_t e = cudaSuccess;
+    if (run != cur) {
+        e = cudaEventRecord((cudaEvent_t)in_ready, cur);
+        if (e == cudaSuccess) e = cudaStreamWaitEvent(run, (cudaEvent_t)in_ready, 0);
+    }
+    if (e == cudaSuccess && wait_a) e = cudaStreamWaitEvent(run, (cudaEvent_t)wait_a, 0);
+    if (e == cudaSuccess && wait_b) e = cudaStreamWaitEvent(run, (cudaEvent_t)wait_b, 0);
+    if (e == cudaSuccess) e = cudaGraphLaunch((cudaGraphExec_t)chain_exec, run);
+    if (e == cudaSuccess) e = cudaEventRecord((cudaEvent_t)chain_done, run);
+    if (e == cudaSuccess) e = cudaStreamWaitEvent(rs, (cudaEvent_t)chain_done, 0);
+    if (e == cudaSuccess) e = cudaGraphLaunch((cudaGraphExec_t)exch_exec, rs);
+    if (e == cudaSuccess) e = cudaEventRecord((cudaEvent_t)exch_done, rs);
+    return e == cudaSuccess ? BBB_OK : cuda_fail(e, "bbb_mc_graph_step");
 }
 
 /* debug only (not in the public header): per-CTA clock64 checkpoints of tap_gemm_kernel */

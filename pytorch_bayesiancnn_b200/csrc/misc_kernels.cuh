@@ -139,7 +139,13 @@ lrt_noise_grad_kernel(const float* __restrict__ gy, const float* __restrict__ ac
     }
 }
 
-__global__ void noise_advance_kernel(unsigned long long* base, unsigned long long inc) { *base += inc; }
+// The head of a captured Monte-Carlo step.  It lets its programmatic dependents start at once: the first GEMM kernel of
+// a chain whose operand tiles are prepared ahead of the step stages its input images meanwhile, and every reader of the
+// base waits (griddepcontrol.wait) for this kernel to complete.
+__global__ void noise_advance_kernel(unsigned long long* base, unsigned long long inc) {
+    asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+    *base += inc;
+}
 
 // main_bayesian.py:46-53 + utils.py:14-22 (+ uncertainty_estimation.py:70-96 moments).
 // One CTA per image; warps compute log-sum-exp per MC sample, then one thread per

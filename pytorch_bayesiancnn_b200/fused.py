@@ -165,6 +165,60 @@ def _step_desc(st, phase, fold=None):
 
 _side_streams: dict = {}
 _direct = {"out": None, "terms": False}
+_cached = {"prep": None}
+
+
+class PrepCache:
+    """The parameter-only half of a planned chain -- bf16 operand tiles, bias rows and the Gaussian KL of every layer --
+    in workspaces of its own, prepared ahead of the steps that read them (mc.MCForward: once per parameter version).
+
+    Only a chain of LRT layers is cached: an LRT prep is a pure function of the parameters and the prior (the LRT noise is
+    drawn on the activations, in the GEMM epilogue), so the tiles and KL of every step are the bits the step's own prep
+    would write.  A BBB prep draws the weights of its step and stays in the step.  A mixture-prior layer's tiles are
+    cached; its KL, a Monte-Carlo draw per sample, stays in the step.
+
+    ``fill()`` enqueues the preps on the current stream.  A chain entered under ``use_prep(cache)`` launches only its GEMM
+    kernels (and the mixture draws), reading the cache; ordering the fill against the steps is the caller's job."""
+
+    def __init__(self, steps, fold, dev):
+        self.steps, self.fold = steps, fold
+        self.layers = [st.layer for st in steps]
+        self.kl = torch.zeros(len(steps), dtype=torch.float32, device=dev)    # per-layer KL scalars (stable address)
+        self.ws = [None] * len(steps)
+
+    @staticmethod
+    def eligible(steps) -> bool:
+        return bool(steps) and all(st.layer._variant == L.VARIANT_LRT for st in steps)
+
+    def covers(self, steps) -> bool:
+        return len(steps) == len(self.layers) and all(st.layer is m for st, m in zip(steps, self.layers))
+
+    def fill(self):
+        """The preps of every layer, in layer order, on the current stream; they take no debug-timeline slot."""
+        lib = L.lib()
+        for i, st in enumerate(self.steps):
+            if self.ws[i] is None:
+                d = _step_desc(st, L.FUSED_PREP_ONLY, self.fold)
+                self.ws[i] = torch.zeros(int(lib.bbb_workspace_bytes(C.byref(d))), dtype=torch.uint8,
+                                         device=self.kl.device)
+            run_step(st, None, None, None, 0, kl=self.kl[i], noise=(None, None, 0, 0, None, None),
+                     phase=L.FUSED_PREP_ONLY, fold=self.fold, ws=self.ws[i], fill=True)
+
+
+class use_prep:
+    """``with fused.use_prep(cache): ...`` -- a chain run inside whose layers are those of ``cache`` (a PrepCache) reads
+    their operand tiles and KL from it instead of preparing them."""
+
+    def __init__(self, cache):
+        self.cache = cache
+
+    def __enter__(self):
+        self.prev, _cached["prep"] = _cached["prep"], self.cache
+        return self
+
+    def __exit__(self, *exc):
+        _cached["prep"] = self.prev
+        return False
 
 
 class direct_output:
@@ -218,7 +272,12 @@ def _run(steps, x, overlap_prep, out, terms, owner, fold=None, kls_out=None):
 
     A layer with a mixture prior (set_mixture_prior) computes no KL in its prep: its term is a Monte-Carlo draw per MC
     sample (one, or the fold's samples), launched behind its prep on the prep's stream.  The chain then returns the
-    per-sample KL -- the layers' terms added in layer order, 0-dim or [samples] under a fold -- with ``terms`` as well."""
+    per-sample KL -- the layers' terms added in layer order, 0-dim or [samples] under a fold -- with ``terms`` as well.
+
+    Under ``use_prep(cache)`` with a cache of this chain the preps are not launched (_run_cached)."""
+    cache = _cached["prep"]
+    if cache is not None and cache.covers(steps) and cache.fold == fold and steps[0].batch == cache.steps[0].batch:
+        return _run_cached(steps, x, cache, out, terms, owner, fold)
     dev = x.device
     kls = kls_out[:len(steps)] if kls_out is not None else torch.empty(len(steps), dtype=torch.float32, device=dev)
     mixed = [i for i, st in enumerate(steps) if st.layer.mixture_values() is not None]
@@ -305,6 +364,82 @@ def _run(steps, x, overlap_prep, out, terms, owner, fold=None, kls_out=None):
     return cur, kl_total
 
 
+def _run_cached(steps, x, cache, out, terms, owner, fold):
+    """_run with every layer's operand tiles, bias rows and Gaussian KL read from ``cache``: the GEMM kernels back to
+    back on the current stream -- the first one launched programmatically behind whatever heads the step -- and a
+    mixture-prior layer's Monte-Carlo KL draw on a side stream beside them.  Noise is drawn per layer exactly as _run
+    draws it, so every output is the same."""
+    dev = x.device
+    kls = cache.kl[:len(steps)]
+    mixed = [i for i, st in enumerate(steps) if st.layer.mixture_values() is not None]
+    kl_of = [kls[i] for i in range(len(steps))]
+    if mixed:
+        n_draws = 1 if fold is None else steps[0].batch // fold[0]
+        mix = torch.empty(len(mixed), n_draws, dtype=torch.float32, device=dev)
+        for k, i in enumerate(mixed):
+            kl_of[i] = mix[k]
+    snap = Fn.noise_snapshot()
+    main = torch.cuda.current_stream(dev)
+    side = _side_stream(dev) if mixed else None
+    forked = False
+    try:
+        if fold is not None and Fn.external_eps_active():
+            raise L.EngineError("MC-sample folding draws its noise in-kernel (no external eps)")
+        noise = [_draw_noise(st, x.shape[0], dev) for st in steps]
+        if mixed:
+            side.wait_stream(main)
+            forked = True
+            with torch.cuda.stream(side):
+                for i in mixed:
+                    kl_of[i] = _kl_mc(steps[i].layer, kl_of[i], noise[i], fold)
+        for i, st in enumerate(steps):
+            if i not in mixed:
+                st.layer._kl_cache = (kls[i], st.layer._versions(), torch.is_grad_enabled())
+        cur, cur_sq, cur_pitch = x.contiguous().float(), None, 0
+        last = steps[-1]
+        take = (out is not None and last.out_layout == L.LAYOUT_ROWMAJOR_F32 and out.is_contiguous()
+                and out.dtype == torch.float32 and tuple(out.shape) == (last.batch, last.out_chw[0]))
+        for i, st in enumerate(steps):
+            nxt = steps[i + 1].layer if i + 1 < len(steps) else None
+            y_into = out if (take and i == len(steps) - 1) else None
+            cur, cur_sq, cur_pitch = run_step(st, nxt, cur, cur_sq, cur_pitch, kl=kl_of[i], noise=noise[i],
+                                              phase=L.FUSED_SKIP_PREP, y_into=y_into, fold=fold, ws=cache.ws[i])
+        if forked:
+            main.wait_stream(side)
+            forked = False
+        if mixed:
+            kl_total = kl_of[0]                  # element-wise adds in layer order, as _run
+            for t in kl_of[1:]:
+                kl_total = kl_total + t
+            if fold is None:
+                kl_total = kl_total.reshape(())
+        elif terms:
+            kl_total = kls
+        else:
+            kl_total = kls.sum()
+        if terms and owner is not None:
+            owner.used = True
+    except BaseException:
+        Fn.noise_restore(snap)
+        raise
+    finally:
+        if forked:
+            main.wait_stream(side)
+    return cur, kl_total
+
+
+def _kl_mc(m, kl, noise, fold):
+    """A mixture-prior layer's Monte-Carlo KL of one layer call into ``kl`` (one entry per folded MC sample, each from
+    its own stream); returns it as the call returns it (0-dim unfolded) and keeps it as the layer's KL."""
+    kl_stream = noise[5]
+    Fn.kl_mc_forward(kl, m.W_mu, m.W_rho, m.bias_mu, m.bias_rho, m.mixture_values(), kl_stream[0], kl_stream[1],
+                     Fn._noise.base, fold[1] if fold is not None else 0, m)
+    if fold is None:
+        kl = kl.reshape(())
+    m._kl_cache = (kl, m._versions(), torch.is_grad_enabled())
+    return kl
+
+
 def _draw_noise(st, B, dev):
     """(eps_a, eps_b, seed, stream_id, base, kl_stream) for one layer call, consuming the external-eps
     queue / the Philox stream counter exactly like the unfused layer would.  kl_stream: (seed, stream id) of the
@@ -327,16 +462,19 @@ def _draw_noise(st, B, dev):
     return eps_a, eps_b, seed, stream_id, base, kl_stream
 
 
-def run_step(st, nxt, cur, cur_sq, cur_pitch, kl=None, noise=None, phase=0, y_into=None, fold=None):
+def run_step(st, nxt, cur, cur_sq, cur_pitch, kl=None, noise=None, phase=0, y_into=None, fold=None, ws=None,
+             fill=False):
     """One fused layer call: (y, y_sq, pitch) = step(cur, cur_sq).  phase: 0 = prep + GEMM,
-    FUSED_PREP_ONLY / FUSED_SKIP_PREP = one half (see include/bbb_b200.h)."""
+    FUSED_PREP_ONLY / FUSED_SKIP_PREP = one half (see include/bbb_b200.h).  ``ws``: the workspace of the operand tiles
+    (default: the layer's own, Fn.workspace).  ``fill``: a PREP_ONLY call filling a PrepCache -- off the debug timeline,
+    and a mixture prior's Monte-Carlo KL is left to the steps."""
     lib = L.lib()
     m = st.layer
     dev = m.W_mu.device
     B = st.batch                                    # (packed inputs carry rows padded to the 128-row tile)
     if True:
         cin, h, w = st.in_shape
-        d = _step_desc(st, phase, fold)
+        d = _step_desc(st, phase | (L.FUSED_NO_TIMELINE if fill else 0), fold)
         in_pitch = cur_pitch if st.in_layout == L.LAYOUT_NCHW_F32 else cin * h * w
         cout, oh, ow = st.out_chw
         if phase == L.FUSED_PREP_ONLY:
@@ -357,7 +495,8 @@ def run_step(st, nxt, cur, cur_sq, cur_pitch, kl=None, noise=None, phase=0, y_in
             noise = _draw_noise(st, B, dev)
         eps_a, eps_b, seed, stream_id, base, kl_stream = noise
         mixture = m.mixture_values()
-        ws = Fn.workspace(dev, d, m)
+        if ws is None:
+            ws = Fn.workspace(dev, d, m)
         rc = lib.bbb_layer_forward_fused_prior(
             C.byref(d), Fn._ptr(cur), Fn._ptr(cur_sq), st.in_layout, in_pitch, st.prev_hw,
             Fn._ptr(m.W_mu), Fn._ptr(m.W_rho), Fn._ptr(m.bias_mu), Fn._ptr(m.bias_rho),
@@ -366,11 +505,9 @@ def run_step(st, nxt, cur, cur_sq, cur_pitch, kl=None, noise=None, phase=0, y_in
             C.c_uint64(seed), C.c_uint64(stream_id), Fn._ptr(base), Fn._ptr(ws), C.c_size_t(ws.numel()),
             Fn._stream(dev), Fn.prior_arg(m.prior_tensors()))
         L.check(rc, "bbb_layer_forward_fused_prior")
-        if phase != L.FUSED_SKIP_PREP:
+        if phase != L.FUSED_SKIP_PREP and not fill:
             if mixture is not None:             # kl: one entry per folded MC sample, each from its own stream
-                Fn.kl_mc_forward(kl, m.W_mu, m.W_rho, m.bias_mu, m.bias_rho, mixture, kl_stream[0], kl_stream[1],
-                                 Fn._noise.base, fold[1] if fold is not None else 0, m)
-                if fold is None:
-                    kl = kl.reshape(())
-            m._kl_cache = (kl, m._versions(), torch.is_grad_enabled())
+                _kl_mc(m, kl, noise, fold)
+            else:
+                m._kl_cache = (kl, m._versions(), torch.is_grad_enabled())
         return y, y_sq, pitch

@@ -166,7 +166,7 @@ class MCForward:
                  seed: Optional[int] = None, graph: bool = True, num_classes: Optional[int] = None,
                  static_inputs=None, first_replay: int = 0, fold: bool = True, overlap: bool = False, inflight: int = 1,
                  fold_group: Optional[int] = None, fold_budget: int = LAYER_FOLD_BUDGET, want_information: bool = False,
-                 batch_shards: int = 1, metrics: Optional[torch.Tensor] = None):
+                 batch_shards: int = 1, metrics: Optional[torch.Tensor] = None, cache_prep: bool = True):
         """``static_inputs``: device tensors the caller fills in place (e.g. targets of its host->device copies, or a
         rotation of resident batches); one graph is captured per tensor and ``self(slot=k)`` runs the step on
         ``static_inputs[k]`` with no staging copy.  ``first_replay``: index of the first replay's noise block.
@@ -178,7 +178,14 @@ class MCForward:
         head of step t+1 (parameter preps, first layers) fills the SMs the tail of step t leaves idle.  Results are
         identical to the serial engine; ``wait()`` also covers the inputs (they may be rewritten afterwards).
         ``fold_group``: the largest number of samples one pass of the per-layer fold takes (nets the fused chain does not
-        take); None = as many as ``fold_budget`` bytes of activations allow (layer_fold_groups)."""
+        take); None = as many as ``fold_budget`` bytes of activations allow (layer_fold_groups).
+        ``cache_prep`` (captured engines whose fused chain is all LRT layers): the layers' bf16 operand tiles, bias rows
+        and Gaussian KL are prepared by a graph of their own once per parameter version, into one workspace the steps
+        read, instead of in every step (fused.PrepCache).  Before each step the host compares the version counters of
+        the layers' parameters and prior buffers with those of the last prep and, when one moved, replays the prep first -- after the work enqueued on the current stream so far and after every step still in
+        flight.  So an in-place update through an autograd-visible tensor (optimizer.step(), p.copy_() under no_grad,
+        set_prior, load_state_dict) is read by the next step; a write through p.data or a raw pointer is not.  False:
+        every step prepares its own operands, as a net with BBB layers always does."""
         if want_information and not want_uncertainty:
             raise L.EngineError("MCForward: want_information needs want_uncertainty")
         Fn._require_cuda(example_x, "MCForward")
@@ -286,6 +293,12 @@ class MCForward:
             self.xrep_all = [torch.empty((G * self.nb,) + tuple(example_x.shape[1:]), dtype=example_x.dtype, device=dev)
                              for _ in range(nbuf)]
         self.graph, self.graphs = None, []
+        self.cache_prep = bool(cache_prep)
+        self._prep, self._prep_graph, self._prep_key = None, None, None     # set by _capture (fused.PrepCache)
+        self._prep_watch = None
+        self._prep_pending = set()                # buffer parities whose next step must wait for the last re-prep
+        self.prep_replays = 0                     # replays of the prep graph (one per parameter version after the first)
+        self.prep_kernels = 0                     # kernels of the prep graph
         self._prior_guard = None                   # set by _capture (modules.PriorGuard)
         self.result_stream = None                 # overlap mode: the stream the results are complete on
         self.replays = 0
@@ -323,6 +336,55 @@ class MCForward:
                 if lib.bbb_forward_supported(C.byref(d)) != 0:
                     return None
         return groups
+
+    # -- operand tiles and KL prepared once per parameter version (cache_prep) ---------------------------------------
+    def _plan_prep(self, example_x):
+        """The PrepCache of this engine's fused chain -- the LRT fold's, or the chain a sample's net(x) runs -- or None
+        (no fused chain, or a layer that is not LRT)."""
+        from . import fused
+        from .modules import ModuleWrapper, _default_fuse
+        if self.fold_steps is not None:
+            steps, fold = self.fold_steps, self.fold
+        elif (self._groups is None and type(self.net).forward is ModuleWrapper.forward
+              and getattr(self.net, "fuse", _default_fuse())):
+            with Fn.first_image(self.rows[0]):
+                steps, fold = fused.plan(list(self.net.children()), (self.nb,) + tuple(example_x.shape[1:])), None
+        else:
+            return None
+        return fused.PrepCache(steps, fold, self.dev) if fused.PrepCache.eligible(steps) else None
+
+    def _prep_version(self):
+        """The version counters of the tensors the prep graph reads: the layers' parameters and prior buffers (the part of
+        _BayesLayer._versions a replay can see -- the KL settings and the addresses are baked into the graphs, and a
+        prior that is set anew is refused by PriorGuard).  About 2 us of host time for BBBAlexNet, where the whole
+        _versions() tuple takes ten times that."""
+        if self._prep_watch is None:
+            from .modules import _PRIOR_BUFFERS
+            self._prep_watch = [t for m in self._prep.layers for t in (m.W_mu, m.W_rho, m.bias_mu, m.bias_rho)
+                                + tuple(m._buffers.get(n) for n in _PRIOR_BUFFERS) if t is not None]
+        return [t._version for t in self._prep_watch]
+
+    def _fill_prep(self):
+        with torch.no_grad(), Fn.first_image(self.rows[0]):
+            self._prep.fill()
+
+    def _reprep(self):
+        """Replay the prep graph: after the current stream's work so far (in-place updates the caller enqueued) and after
+        every step that may still read the tiles or the KL; the steps enqueued from now on wait for it."""
+        cur = torch.cuda.current_stream(self.dev)
+        if self.overlap:
+            ps = self._prep_stream
+            ps.wait_stream(cur)
+            for ev, seen in zip(self._exch_done, self._exch_seen):     # the last step of each buffer parity: its
+                if seen:                                                 # exchange follows its chain
+                    ps.wait_event(ev)
+            with torch.cuda.stream(ps):
+                self._prep_graph.replay()
+            self._prep_done.record(ps)
+            self._prep_pending = set(range(self.nbuf))
+        else:
+            self._prep_graph.replay()              # stream order: behind the steps before, in front of this one
+        self.prep_replays += 1
 
     # -- peer-mapped receive buffers (CUDA IPC; handles travel over torch.distributed) -----------------------
     def _open_peers(self, nbytes):
@@ -394,11 +456,13 @@ class MCForward:
         b0, nb = self.rows[0], self.nb
         x = x[b0:b0 + nb]                                 # this rank's row block (a view: NCHW rows are contiguous)
         with torch.no_grad(), Fn.workspace_slot(par if self.inflight > 1 else Fn.current_workspace_slot()), \
-                Fn.first_image(b0):
+                Fn.first_image(b0), fused.use_prep(self._prep):
             # The Philox base moves at the HEAD of a captured step, BEFORE the prep streams fork: with this one-thread
             # kernel as the single root of the graph every GEMM kernel of the chain is launched programmatically behind
             # its predecessor; with the fork in front of it (prep kernels as further root nodes) or with no plain kernel
             # at the head, the programmatic edges of the whole chain are lost and every GEMM waits for its predecessor.
+            # With the operands prepared ahead (self._prep) there is no prep in the step: the first GEMM kernel follows
+            # this one directly.
             if advance:
                 Fn.noise_advance(base, inc)
             kl_ptr, n_kl = None, 0
@@ -497,7 +561,11 @@ class MCForward:
         live = self._metrics
         if live is not None:
             self._metrics = torch.zeros_like(live)      # the warm-up steps do not count
+        self._prep = self._plan_prep(self.x) if self.cache_prep else None
         with torch.cuda.stream(side):
+            if self._prep is not None:              # the first prep, which the warm-up steps already read
+                self._prep_key = self._prep_version()
+                self._fill_prep()
             for _ in range(warmup):                 # eager: creates plans / workspaces; every rank runs the same exchanges
                 self._step(self.x, self.base)
             for p_ in range(1, self.inflight):      # the other in-flight steps' own layer workspaces
@@ -519,6 +587,14 @@ class MCForward:
         def keep_pool(par, g):
             if self._groups is not None:
                 pools.setdefault(par, g.pool())
+        if self._prep is not None:
+            self._prep_graph = torch.cuda.CUDAGraph()
+            n0 = L.launch_count()
+            with torch.cuda.graph(self._prep_graph, stream=cap):
+                self._fill_prep()
+            self.prep_kernels = L.launch_count() - n0
+            self._prep_stream = torch.cuda.Stream(device=dev, priority=-1)
+            self._prep_done = torch.cuda.Event()
         if self.overlap:
             # two graphs per step: the layer chain (per resident input and buffer parity) and the exchange kernel (per
             # parity); __call__ replays the second on its own stream so that it runs beside the next step's chain
@@ -545,9 +621,24 @@ class MCForward:
             lo = getattr(torch.cuda.Stream, "priority_range", lambda: (-1, 0))()
             self.result_stream = torch.cuda.Stream(device=dev, priority=min(lo))
             self._chain_done = [torch.cuda.Event() for _ in range(nb)]
-            self._exch_done = [None] * nb
+            self._exch_done = [torch.cuda.Event() for _ in range(nb)]
+            self._exch_seen = [False] * nb          # has a step of buffer parity p been enqueued (its exchange event recorded)
             self._in_ready = [torch.cuda.Event() for _ in range(nb)]
             self.chain_streams = [torch.cuda.Stream(device=dev, priority=-1) for _ in range(nb)] if self.inflight > 1 else None
+            # torch creates an event at its first record: create them all now (nothing is pending), so that every step is
+            # enqueued by one native call on their raw handles (bbb_mc_graph_step) -- the host work of a step is then a
+            # small fraction of its ~0.1 ms on the device, where the runtime calls made one by one from Python were not
+            events = self._chain_done + self._exch_done + self._in_ready + \
+                ([self._prep_done] if self._prep is not None else [])
+            for ev in events:
+                ev.record(cap)
+            rs_raw = self.result_stream.cuda_stream
+            # per (parity, input slot): run stream (None = the caller's current stream), in_ready, chain graph, chain
+            # event, result stream, exchange graph, exchange event
+            self._step_handles = [[(self.chain_streams[p_].cuda_stream if self.chain_streams else None,
+                                    self._in_ready[p_].cuda_event, g_.raw_cuda_graph_exec(), self._chain_done[p_].cuda_event,
+                                    rs_raw, self.exch_graphs[p_].raw_cuda_graph_exec(), self._exch_done[p_].cuda_event)
+                                   for g_ in self.chain_graphs[p_]] for p_ in range(nb)]
             # replay r draws noise block first_replay + r: with k counters, counter p starts k blocks back and moves by k
             for p_ in range(nb):
                 self.base2[p_] = (self.first_replay + p_ - nb) * _STRIDE
@@ -567,29 +658,39 @@ class MCForward:
             raise L.EngineError("MCForward was built without with_labels=True")
         if self._prior_guard is not None:
             self._prior_guard.check("MCForward")
+        if self._prep_graph is not None:
+            key = self._prep_version()
+            if key != self._prep_key:
+                self._reprep()
+                self._prep_key = key
         if self.overlap:
-            cur = torch.cuda.current_stream(self.dev)
+            # Step `par` (even / odd / .. steps on their own streams when several are in flight) runs behind the caller's
+            # work so far, behind the exchange of the last step of the same parity (which read buffers `par`) and, for the
+            # first step of `par` since a re-prep, behind the prep.  Its exchange follows on result_stream.
             par = self.replays % self.nbuf
-            run = cur
-            if self.inflight > 1:                        # even / odd steps on their own streams, behind the caller's work so far
-                run = self.chain_streams[par]
-                self._in_ready[par].record(cur)
-                run.wait_event(self._in_ready[par])
-            if self._exch_done[par] is not None:          # buffers `par` were last read by the exchange of two steps ago
-                run.wait_event(self._exch_done[par])
-            with torch.cuda.stream(run):
-                if labels is not None:
-                    self.labels_all[par].copy_(labels, non_blocking=True)
-                if x is not None:
-                    self.inputs[slot].copy_(x, non_blocking=True)
-                self.chain_graphs[par][slot].replay()
-                self._chain_done[par].record(run)
-            rs = self.result_stream
-            rs.wait_event(self._chain_done[par])
-            with torch.cuda.stream(rs):
-                self.exch_graphs[par].replay()
-                ev = self._exch_done[par] = self._exch_done[par] or torch.cuda.Event()
-                ev.record(rs)
+            h = self._step_handles[par][slot]
+            wait_a = self._exch_done[par].cuda_event if self._exch_seen[par] else None
+            wait_b = self._prep_done.cuda_event if par in self._prep_pending else None
+            self._prep_pending.discard(par)
+            cur_raw = torch._C._cuda_getCurrentRawStream(self.dev.index)
+            if labels is not None or x is not None:       # the copies go on the step's stream, behind its waits
+                cur = torch.cuda.current_stream(self.dev)
+                run = self.chain_streams[par] if self.inflight > 1 else cur
+                if run is not cur:
+                    self._in_ready[par].record(cur)
+                    run.wait_event(self._in_ready[par])
+                for ev in (self._exch_done[par] if wait_a else None, self._prep_done if wait_b else None):
+                    if ev is not None:
+                        run.wait_event(ev)
+                with torch.cuda.stream(run):
+                    if labels is not None:
+                        self.labels_all[par].copy_(labels, non_blocking=True)
+                    if x is not None:
+                        self.inputs[slot].copy_(x, non_blocking=True)
+                cur_raw, wait_a, wait_b = run.cuda_stream, None, None
+            L.check(L.lib().bbb_mc_graph_step(cur_raw, h[0] if h[0] is not None else cur_raw, h[1], wait_a, wait_b,
+                                              h[2], h[3], h[4], h[5], h[6]), "bbb_mc_graph_step")
+            self._exch_seen[par] = True
             self._last = par
             self.replays += 1
             return self.out
@@ -605,7 +706,7 @@ class MCForward:
 
     def wait(self):
         """Make the current stream wait for the last step's results (a no-op unless built with ``overlap=True``)."""
-        if self.overlap and self.replays and self._exch_done[self._last] is not None:
+        if self.overlap and self.replays and self._exch_seen[self._last]:
             # exchanges run in step order on one stream and each follows its chain: the last one covers everything before
             torch.cuda.current_stream(self.dev).wait_event(self._exch_done[self._last])
         return self.out
