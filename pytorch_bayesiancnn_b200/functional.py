@@ -647,19 +647,8 @@ class BayesLayerFn(torch.autograd.Function):
         if gx is not None and gx.dtype != ctx.x_dtype:
             gx = gx.to(ctx.x_dtype)
         if gkl is not None and cfg.get("mixture") is None:
-            gkl = gkl.contiguous().float()
-            prior = cfg.get("prior")
-            rc = lib.bbb_kl_backward_prior(_ptr(W_mu), _ptr(W_rho), C.c_uint64(W_mu.numel()),
-                                           C.c_float(cfg["prior_mu"]), C.c_float(cfg["prior_sigma"]),
-                                           C.c_int32(cfg["kl_convention"]), _ptr(gkl), _ptr(g_W_mu), _ptr(g_W_rho),
-                                           _stream(dev), prior_arg(prior))
-            L.check(rc, "bbb_kl_backward_prior")
-            if ctx.has_bias:
-                rc = lib.bbb_kl_backward_prior(_ptr(bias_mu), _ptr(bias_rho), C.c_uint64(bias_mu.numel()),
-                                               C.c_float(cfg["prior_mu"]), C.c_float(cfg["prior_sigma"]),
-                                               C.c_int32(cfg["kl_convention"]), _ptr(gkl), _ptr(g_b_mu), _ptr(g_b_rho),
-                                               _stream(dev), prior_arg(prior, bias=True))
-                L.check(rc, "bbb_kl_backward_prior")
+            _kl_backward(gkl, (W_mu, W_rho, bias_mu, bias_rho), (g_W_mu, g_W_rho, g_b_mu, g_b_rho), cfg["prior_mu"],
+                         cfg["prior_sigma"], cfg["kl_convention"], cfg.get("prior"))
         return gx, g_W_mu, g_W_rho, g_b_mu, g_b_rho, None
 
 
@@ -760,23 +749,26 @@ class KLFn(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, gkl):
-        lib = L.lib()
-        W_mu, W_rho, bias_mu, bias_rho = ctx.saved_tensors
-        pm, ps, conv = ctx.cfg
-        dev = W_mu.device
-        gkl = gkl.contiguous().float()
-        out = []
-        for mu, rho, bias in ((W_mu, W_rho, False), (bias_mu, bias_rho, True)):
-            if mu is None:
-                out += [None, None]
-                continue
-            g_mu, g_rho = torch.zeros_like(mu), torch.zeros_like(rho)
-            rc = lib.bbb_kl_backward_prior(_ptr(mu), _ptr(rho), C.c_uint64(mu.numel()), C.c_float(pm), C.c_float(ps),
-                                           C.c_int32(conv), _ptr(gkl), _ptr(g_mu), _ptr(g_rho), _stream(dev),
-                                           prior_arg(ctx.prior, bias=bias))
-            L.check(rc, "bbb_kl_backward_prior")
-            out += [g_mu, g_rho]
-        return out[0], out[1], out[2], out[3], None, None, None, None
+        params = ctx.saved_tensors
+        grads = tuple(None if t is None else torch.zeros_like(t) for t in params)
+        _kl_backward(gkl, params, grads, *ctx.cfg, ctx.prior)
+        return grads + (None, None, None, None)
+
+
+def _kl_backward(gkl, params, grads, prior_mu, prior_sigma, kl_convention, prior):
+    """gkl * d kl / d (mu, rho) added into ``grads``, the weight's then the bias's (bbb_kl_backward_prior; no call for a
+    layer without a bias).  params = (W_mu, W_rho, bias_mu, bias_rho) and grads likewise; ``prior``: None or the layer's
+    tensor prior."""
+    lib = L.lib()
+    gkl = gkl.contiguous().float()
+    for k, bias in ((0, False), (2, True)):
+        mu, rho = params[k], params[k + 1]
+        if mu is None:
+            continue
+        rc = lib.bbb_kl_backward_prior(_ptr(mu), _ptr(rho), C.c_uint64(mu.numel()), C.c_float(prior_mu),
+                                       C.c_float(prior_sigma), C.c_int32(kl_convention), _ptr(gkl), _ptr(grads[k]),
+                                       _ptr(grads[k + 1]), _stream(mu.device), prior_arg(prior, bias=bias))
+        L.check(rc, "bbb_kl_backward_prior")
 
 
 def mixture_arg(mixture):

@@ -138,28 +138,13 @@ def _out_pitch(st):
 def _step_desc(st, phase, fold=None):
     m = st.layer
     cin, h, w = st.in_shape
-    d = L.LayerDesc()
-    d.batch, d.in_channels, d.in_h, d.in_w = st.batch, cin, h, w
-    if st.linear:
-        d.out_channels, d.kernel_h, d.kernel_w = m.out_features, 1, 1
-        d.stride_h = d.stride_w = d.dil_h = d.dil_w = 1
-        d.pad_h = d.pad_w = 0
-    else:
-        (sh, sw), (ph, pw), (dh, dw) = st.conv
-        d.out_channels, d.kernel_h, d.kernel_w = m.out_channels, m.kernel_size[0], m.kernel_size[1]
-        d.stride_h, d.stride_w, d.pad_h, d.pad_w, d.dil_h, d.dil_w = sh, sw, ph, pw, dh, dw
-    d.variant, d.sample, d.has_bias = m._variant, 1, int(m.use_bias)     # ModuleWrapper calls children with sample=True (SURVEY D6)
-    d.act_dtype, d.math = L.DTYPE_F32, L.MATH_BF16_TC
-    d.kl_convention = L.KL_BY_NAME[m.kl_convention]
-    d.epilogue_act = st.act
+    x_shape = (st.batch, cin) if st.linear else (st.batch, cin, h, w)
+    # ModuleWrapper calls children with sample=True (SURVEY D6)
+    d = Fn.make_desc(x_shape, tuple(m.W_mu.shape), st.conv, m._variant, True, m.use_bias, m.prior_mu, m.prior_sigma,
+                     L.MATH_BF16_TC, L.KL_BY_NAME[m.kl_convention], st.act, fold=fold,
+                     first_image=Fn.current_first_image())
     d.pool_k = d.pool_s = 2 if st.pool else 0
-    d.reserved[0] = phase | (Fn.first_image_word(Fn.current_first_image()) if Fn.current_first_image() else 0)
-    if fold is not None:                    # MC samples folded into the batch (include/bbb_b200.h)
-        rows, stride = fold
-        d.reserved[1] = int(rows)
-        d.reserved[2] = C.c_int32(stride & 0xFFFFFFFF).value
-        d.reserved[3] = C.c_int32((stride >> 32) & 0xFFFFFFFF).value
-    d.prior_mu, d.prior_sigma = float(m.prior_mu), float(m.prior_sigma)
+    d.reserved[0] |= phase
     return d
 
 
@@ -274,74 +259,94 @@ def _run(steps, x, overlap_prep, out, terms, owner, fold=None, kls_out=None):
     sample (one, or the fold's samples), launched behind its prep on the prep's stream.  The chain then returns the
     per-sample KL -- the layers' terms added in layer order, 0-dim or [samples] under a fold -- with ``terms`` as well.
 
-    Under ``use_prep(cache)`` with a cache of this chain the preps are not launched (_run_cached)."""
+    Under ``use_prep(cache)`` with a cache of this chain (same layers, fold and batch) the preps are not launched: every
+    layer's operand tiles, bias rows and Gaussian KL are read from the cache, the GEMM kernels run back to back on the
+    current stream -- the first one launched programmatically behind whatever heads the step -- and a mixture-prior
+    layer's Monte-Carlo KL draw runs on a side stream beside them.  Noise is drawn per layer either way, so every
+    output is the same."""
     cache = _cached["prep"]
-    if cache is not None and cache.covers(steps) and cache.fold == fold and steps[0].batch == cache.steps[0].batch:
-        return _run_cached(steps, x, cache, out, terms, owner, fold)
+    if not (cache is not None and cache.covers(steps) and cache.fold == fold and steps[0].batch == cache.steps[0].batch):
+        cache = None
     dev = x.device
-    kls = kls_out[:len(steps)] if kls_out is not None else torch.empty(len(steps), dtype=torch.float32, device=dev)
+    n = len(steps)
+    if cache is not None:
+        kls = cache.kl[:n]
+    else:
+        kls = kls_out[:n] if kls_out is not None else torch.empty(n, dtype=torch.float32, device=dev)
     mixed = [i for i, st in enumerate(steps) if st.layer.mixture_values() is not None]
     if mixed:
         n_draws = 1 if fold is None else steps[0].batch // fold[0]
         mix = torch.empty(len(mixed), n_draws, dtype=torch.float32, device=dev)
-        kl_of = [mix[mixed.index(i)] if i in mixed else kls[i] for i in range(len(steps))]
+        kl_of = [mix[mixed.index(i)] if i in mixed else kls[i] for i in range(n)]
     else:
-        kl_of = [kls[i] for i in range(len(steps))]
+        kl_of = [kls[i] for i in range(n)]
     snap = Fn.noise_snapshot()
     main = torch.cuda.current_stream(dev)
-    chains = [_side_stream(dev, c) for c in range(min(_prep_chains(), len(steps)))] if overlap_prep else []
+    # Where each layer's prep comes from: the cache; inline, in the launch of its GEMM kernel (phase 0); or a launch of
+    # its own on prep_on[i] (overlap).  The FIRST layer's prep then stays on the main stream, right in front of its GEMM
+    # kernel: launched with programmatic serialization the GEMM kernel's CTAs start while the prep runs and stage their
+    # input images meanwhile (conv_s4_tc.cuh); only its weight producer waits for the prep.  The other preps go to the
+    # side chains.
+    overlap = overlap_prep and cache is None
+    inline = not overlap_prep and cache is None
+    chains, prep_on = [], [None] * n
+    if overlap:
+        chains = [_side_stream(dev, c) for c in range(min(_prep_chains(), n))]
+        if os.environ.get("BBB_B200_PREP0_MAIN", "1") == "1":
+            prep_on = [main] + [chains[(i - 1) % len(chains)] for i in range(1, n)]
+        else:
+            prep_on = [chains[i % len(chains)] for i in range(n)]
+    elif cache is not None and mixed:
+        chains = [_side_stream(dev)]           # the mixture draws
     forked = False
     try:
         if fold is not None and Fn.external_eps_active():
             raise L.EngineError("MC-sample folding draws its noise in-kernel (no external eps)")
         noise = [_draw_noise(st, x.shape[0], dev) for st in steps]
-        if overlap_prep:
-            for side in chains:
-                side.wait_stream(main)
-            forked = True
-            # The FIRST layer's prep stays on the main stream, right in front of its GEMM kernel: launched with programmatic
-            # serialization the GEMM kernel's CTAs start while the prep runs and stage their input images meanwhile
-            # (conv_s4_tc.cuh); only its weight producer waits for the prep.  The other preps go to the side chains.
-            events = [None] * len(steps)
-            first_on_main = os.environ.get("BBB_B200_PREP0_MAIN", "1") == "1"
-            ev0 = None
-            if first_on_main:
-                run_step(steps[0], None, None, None, 0, kl=kl_of[0], noise=noise[0], phase=L.FUSED_PREP_ONLY, fold=fold)
-                ev0 = torch.cuda.Event()
-                ev0.record(main)
-            for i, st in enumerate(steps):
-                if i == 0 and first_on_main:
-                    continue
-                side = chains[(i - 1) % len(chains)] if first_on_main else chains[i % len(chains)]
-                with torch.cuda.stream(side):
+        for side in chains:
+            side.wait_stream(main)
+        forked = bool(chains)
+        events, ev0 = [None] * n, None         # the GEMM kernel of layer i waits for events[i]
+        for i, st in enumerate(steps):
+            if cache is not None and i in mixed:
+                with torch.cuda.stream(chains[0]):
+                    kl_of[i] = _kl_mc(st.layer, kl_of[i], noise[i], fold)
+            elif cache is not None:
+                st.layer._kl_cache = (kls[i], st.layer._versions(), torch.is_grad_enabled())
+            elif prep_on[i] is not None:
+                with torch.cuda.stream(prep_on[i]):
                     run_step(st, None, None, None, 0, kl=kl_of[i], noise=noise[i], phase=L.FUSED_PREP_ONLY, fold=fold)
                     ev = torch.cuda.Event()
-                    ev.record(side)
+                    ev.record(prep_on[i])
+                if prep_on[i] is main:
+                    ev0 = ev
+                else:
                     events[i] = ev
-            for side in chains[1:]:
-                chains[0].wait_stream(side)
-            if not terms and not mixed:
-                with torch.cuda.stream(chains[0]):
-                    if ev0 is not None:
-                        chains[0].wait_event(ev0)
-                    kl_total = kls.sum()
+        for side in chains[1:]:
+            chains[0].wait_stream(side)
+        if overlap and not terms and not mixed:
+            with torch.cuda.stream(chains[0]):
+                if ev0 is not None:
+                    chains[0].wait_event(ev0)
+                kl_total = kls.sum()
         cur, cur_sq, cur_pitch = x.contiguous().float(), None, 0
         last = steps[-1]
         take = (out is not None and last.out_layout == L.LAYOUT_ROWMAJOR_F32 and out.is_contiguous()
                 and out.dtype == torch.float32 and tuple(out.shape) == (last.batch, last.out_chw[0]))
         for i, st in enumerate(steps):
-            nxt = steps[i + 1].layer if i + 1 < len(steps) else None
-            y_into = out if (take and i == len(steps) - 1) else None
-            if overlap_prep:
-                if events[i] is not None:
-                    main.wait_event(events[i])
-                cur, cur_sq, cur_pitch = run_step(st, nxt, cur, cur_sq, cur_pitch, kl=kl_of[i], noise=noise[i],
-                                                  phase=L.FUSED_SKIP_PREP, y_into=y_into, fold=fold)
-            else:
-                cur, cur_sq, cur_pitch = run_step(st, nxt, cur, cur_sq, cur_pitch, kl=kl_of[i], noise=noise[i], y_into=y_into, fold=fold)
+            nxt = steps[i + 1].layer if i + 1 < n else None
+            y_into = out if (take and i == n - 1) else None
+            if events[i] is not None:
+                main.wait_event(events[i])
+            cur, cur_sq, cur_pitch = run_step(st, nxt, cur, cur_sq, cur_pitch, kl=kl_of[i], noise=noise[i],
+                                              phase=0 if inline else L.FUSED_SKIP_PREP, y_into=y_into,
+                                              fold=fold, ws=cache.ws[i] if cache is not None else None)
+        if cache is not None and forked:       # the cached chain's mixture draws: no event of theirs was waited for
+            main.wait_stream(chains[0])
+            forked = False
         if mixed:
-            # element-wise adds in layer order (the main stream has waited for every prep): sample j's sum is the same
-            # whether the samples are folded or run one by one
+            # element-wise adds in layer order (the main stream has waited for every prep and draw): sample j's sum is the
+            # same whether the samples are folded or run one by one
             kl_total = kl_of[0]
             for t in kl_of[1:]:
                 kl_total = kl_total + t
@@ -349,7 +354,7 @@ def _run(steps, x, overlap_prep, out, terms, owner, fold=None, kls_out=None):
                 kl_total = kl_total.reshape(())
         elif terms:
             kl_total = kls
-        elif not overlap_prep:
+        elif not overlap:
             kl_total = kls.sum()
         if terms and owner is not None:
             owner.used = True
@@ -361,70 +366,6 @@ def _run(steps, x, overlap_prep, out, terms, owner, fold=None, kls_out=None):
             for side in chains[1:]:            # written there, and an active graph capture must not be left with dangling forks
                 chains[0].wait_stream(side)
             main.wait_stream(chains[0])
-    return cur, kl_total
-
-
-def _run_cached(steps, x, cache, out, terms, owner, fold):
-    """_run with every layer's operand tiles, bias rows and Gaussian KL read from ``cache``: the GEMM kernels back to
-    back on the current stream -- the first one launched programmatically behind whatever heads the step -- and a
-    mixture-prior layer's Monte-Carlo KL draw on a side stream beside them.  Noise is drawn per layer exactly as _run
-    draws it, so every output is the same."""
-    dev = x.device
-    kls = cache.kl[:len(steps)]
-    mixed = [i for i, st in enumerate(steps) if st.layer.mixture_values() is not None]
-    kl_of = [kls[i] for i in range(len(steps))]
-    if mixed:
-        n_draws = 1 if fold is None else steps[0].batch // fold[0]
-        mix = torch.empty(len(mixed), n_draws, dtype=torch.float32, device=dev)
-        for k, i in enumerate(mixed):
-            kl_of[i] = mix[k]
-    snap = Fn.noise_snapshot()
-    main = torch.cuda.current_stream(dev)
-    side = _side_stream(dev) if mixed else None
-    forked = False
-    try:
-        if fold is not None and Fn.external_eps_active():
-            raise L.EngineError("MC-sample folding draws its noise in-kernel (no external eps)")
-        noise = [_draw_noise(st, x.shape[0], dev) for st in steps]
-        if mixed:
-            side.wait_stream(main)
-            forked = True
-            with torch.cuda.stream(side):
-                for i in mixed:
-                    kl_of[i] = _kl_mc(steps[i].layer, kl_of[i], noise[i], fold)
-        for i, st in enumerate(steps):
-            if i not in mixed:
-                st.layer._kl_cache = (kls[i], st.layer._versions(), torch.is_grad_enabled())
-        cur, cur_sq, cur_pitch = x.contiguous().float(), None, 0
-        last = steps[-1]
-        take = (out is not None and last.out_layout == L.LAYOUT_ROWMAJOR_F32 and out.is_contiguous()
-                and out.dtype == torch.float32 and tuple(out.shape) == (last.batch, last.out_chw[0]))
-        for i, st in enumerate(steps):
-            nxt = steps[i + 1].layer if i + 1 < len(steps) else None
-            y_into = out if (take and i == len(steps) - 1) else None
-            cur, cur_sq, cur_pitch = run_step(st, nxt, cur, cur_sq, cur_pitch, kl=kl_of[i], noise=noise[i],
-                                              phase=L.FUSED_SKIP_PREP, y_into=y_into, fold=fold, ws=cache.ws[i])
-        if forked:
-            main.wait_stream(side)
-            forked = False
-        if mixed:
-            kl_total = kl_of[0]                  # element-wise adds in layer order, as _run
-            for t in kl_of[1:]:
-                kl_total = kl_total + t
-            if fold is None:
-                kl_total = kl_total.reshape(())
-        elif terms:
-            kl_total = kls
-        else:
-            kl_total = kls.sum()
-        if terms and owner is not None:
-            owner.used = True
-    except BaseException:
-        Fn.noise_restore(snap)
-        raise
-    finally:
-        if forked:
-            main.wait_stream(side)
     return cur, kl_total
 
 
@@ -472,42 +413,41 @@ def run_step(st, nxt, cur, cur_sq, cur_pitch, kl=None, noise=None, phase=0, y_in
     m = st.layer
     dev = m.W_mu.device
     B = st.batch                                    # (packed inputs carry rows padded to the 128-row tile)
-    if True:
-        cin, h, w = st.in_shape
-        d = _step_desc(st, phase | (L.FUSED_NO_TIMELINE if fill else 0), fold)
-        in_pitch = cur_pitch if st.in_layout == L.LAYOUT_NCHW_F32 else cin * h * w
-        cout, oh, ow = st.out_chw
-        if phase == L.FUSED_PREP_ONLY:
-            pitch, y, y_sq = cout * oh * ow if st.out_layout == L.LAYOUT_PACKED_BF16 else 0, None, None
-        elif st.out_layout == L.LAYOUT_PACKED_BF16:
-            pitch = cout * oh * ow                   # tiled packed: [ceil(B/128)][F/64][planes][128 x 64] bf16
-            planes = 2 if (nxt is not None and nxt._variant == L.VARIANT_LRT) else 1
-            y = torch.empty((B + 127) // 128 * 128, pitch * planes, dtype=torch.bfloat16, device=dev)
-            y_sq = y.view(-1)[128 * 64:] if planes == 2 else None      # x^2 blocks interleaved behind the x blocks
-        elif st.out_layout == L.LAYOUT_ROWMAJOR_F32:
-            pitch, y, y_sq = 0, (y_into if y_into is not None else torch.empty(B, cout, dtype=torch.float32, device=dev)), None
+    cin, h, w = st.in_shape
+    d = _step_desc(st, phase | (L.FUSED_NO_TIMELINE if fill else 0), fold)
+    in_pitch = cur_pitch if st.in_layout == L.LAYOUT_NCHW_F32 else cin * h * w
+    cout, oh, ow = st.out_chw
+    if phase == L.FUSED_PREP_ONLY:
+        pitch, y, y_sq = cout * oh * ow if st.out_layout == L.LAYOUT_PACKED_BF16 else 0, None, None
+    elif st.out_layout == L.LAYOUT_PACKED_BF16:
+        pitch = cout * oh * ow                   # tiled packed: [ceil(B/128)][F/64][planes][128 x 64] bf16
+        planes = 2 if (nxt is not None and nxt._variant == L.VARIANT_LRT) else 1
+        y = torch.empty((B + 127) // 128 * 128, pitch * planes, dtype=torch.bfloat16, device=dev)
+        y_sq = y.view(-1)[128 * 64:] if planes == 2 else None      # x^2 blocks interleaved behind the x blocks
+    elif st.out_layout == L.LAYOUT_ROWMAJOR_F32:
+        pitch, y, y_sq = 0, (y_into if y_into is not None else torch.empty(B, cout, dtype=torch.float32, device=dev)), None
+    else:
+        pitch, y, y_sq = 0, torch.empty(B, cout, oh, ow, dtype=torch.float32, device=dev), None
+    if kl is None:
+        kl = torch.empty(st.batch // fold[0] if (fold is not None and m.mixture_values() is not None) else (),
+                         dtype=torch.float32, device=dev)
+    if noise is None:
+        noise = _draw_noise(st, B, dev)
+    eps_a, eps_b, seed, stream_id, base, kl_stream = noise
+    mixture = m.mixture_values()
+    if ws is None:
+        ws = Fn.workspace(dev, d, m)
+    rc = lib.bbb_layer_forward_fused_prior(
+        C.byref(d), Fn._ptr(cur), Fn._ptr(cur_sq), st.in_layout, in_pitch, st.prev_hw,
+        Fn._ptr(m.W_mu), Fn._ptr(m.W_rho), Fn._ptr(m.bias_mu), Fn._ptr(m.bias_rho),
+        Fn._ptr(y), Fn._ptr(y_sq), st.out_layout, pitch, None if mixture is not None else Fn._ptr(kl),
+        Fn._ptr(eps_a), Fn._ptr(eps_b),
+        C.c_uint64(seed), C.c_uint64(stream_id), Fn._ptr(base), Fn._ptr(ws), C.c_size_t(ws.numel()),
+        Fn._stream(dev), Fn.prior_arg(m.prior_tensors()))
+    L.check(rc, "bbb_layer_forward_fused_prior")
+    if phase != L.FUSED_SKIP_PREP and not fill:
+        if mixture is not None:             # kl: one entry per folded MC sample, each from its own stream
+            _kl_mc(m, kl, noise, fold)
         else:
-            pitch, y, y_sq = 0, torch.empty(B, cout, oh, ow, dtype=torch.float32, device=dev), None
-        if kl is None:
-            kl = torch.empty(st.batch // fold[0] if (fold is not None and m.mixture_values() is not None) else (),
-                             dtype=torch.float32, device=dev)
-        if noise is None:
-            noise = _draw_noise(st, B, dev)
-        eps_a, eps_b, seed, stream_id, base, kl_stream = noise
-        mixture = m.mixture_values()
-        if ws is None:
-            ws = Fn.workspace(dev, d, m)
-        rc = lib.bbb_layer_forward_fused_prior(
-            C.byref(d), Fn._ptr(cur), Fn._ptr(cur_sq), st.in_layout, in_pitch, st.prev_hw,
-            Fn._ptr(m.W_mu), Fn._ptr(m.W_rho), Fn._ptr(m.bias_mu), Fn._ptr(m.bias_rho),
-            Fn._ptr(y), Fn._ptr(y_sq), st.out_layout, pitch, None if mixture is not None else Fn._ptr(kl),
-            Fn._ptr(eps_a), Fn._ptr(eps_b),
-            C.c_uint64(seed), C.c_uint64(stream_id), Fn._ptr(base), Fn._ptr(ws), C.c_size_t(ws.numel()),
-            Fn._stream(dev), Fn.prior_arg(m.prior_tensors()))
-        L.check(rc, "bbb_layer_forward_fused_prior")
-        if phase != L.FUSED_SKIP_PREP and not fill:
-            if mixture is not None:             # kl: one entry per folded MC sample, each from its own stream
-                _kl_mc(m, kl, noise, fold)
-            else:
-                m._kl_cache = (kl, m._versions(), torch.is_grad_enabled())
-        return y, y_sq, pitch
+            m._kl_cache = (kl, m._versions(), torch.is_grad_enabled())
+    return y, y_sq, pitch

@@ -18,6 +18,7 @@ Two implementations of the same contract:
 """
 from __future__ import annotations
 
+import contextlib
 import ctypes as C
 import math
 from typing import Callable, Optional
@@ -282,16 +283,10 @@ class MCForward:
         # Nets the fused chain does not take (BBBLeNet, BBB3Conv3FC) fold on the per-layer path instead: groups of G
         # consecutive local samples, one pass of the tensor-core layer kernels over G x B rows each (Fn.layer_fold), with
         # the aten activations / pools between them -- per-image ops, so every output equals the sample loop's bit for bit.
-        # layer_fold = (G, number of groups) when it does.
-        self.layer_fold, self._groups = None, None
+        groups = None
         if self.fold_steps is None and fold and len(self.ids) > 1:
-            self._groups = self._plan_layer_fold(net, kids, example_x, fold_group, fold_budget)
-        if self._groups is not None:
-            G = max(n for _, n in self._groups)
-            self.layer_fold = (G, len(self._groups))
-            # the first layer's input: x repeated G times, one buffer per concurrently running step
-            self.xrep_all = [torch.empty((G * self.nb,) + tuple(example_x.shape[1:]), dtype=example_x.dtype, device=dev)
-                             for _ in range(nbuf)]
+            groups = self._plan_layer_fold(net, kids, example_x, fold_group, fold_budget)
+        self._set_passes(groups, example_x)
         self.graph, self.graphs = None, []
         self.cache_prep = bool(cache_prep)
         self._prep, self._prep_graph, self._prep_key = None, None, None     # set by _capture (fused.PrepCache)
@@ -325,17 +320,43 @@ class MCForward:
         groups = layer_fold_groups(len(self.ids), pass_bytes, big, budget, fold_group)
         if groups is None:
             return None
-        lib = L.lib()
+        fold = (self.nb, self.sample_shards << 40)
         for n in sorted({n for _, n in groups}):
             for m, xs in layers:
-                cfg = m._cfg(True)
-                d = Fn.make_desc((n * xs[0],) + tuple(xs[1:]), tuple(m.W_mu.shape), cfg["conv"], cfg["variant"], True,
-                                 m.bias_mu is not None, cfg["prior_mu"], cfg["prior_sigma"], cfg["math"],
-                                 cfg["kl_convention"], cfg["act"], fold=(self.nb, self.sample_shards << 40),
-                                 first_image=self.rows[0])
-                if lib.bbb_forward_supported(C.byref(d)) != 0:
+                if not _fold_forward_supported(m, xs, n, fold, self.rows[0]):
                     return None
         return groups
+
+    def _set_passes(self, groups, example_x):
+        """This rank's passes: (first local sample s0, sample count n) -- the fused fold's one pass over every local
+        sample, the per-layer fold's ``groups``, or one pass per sample.  ``layer_fold`` = (G, number of groups) when the
+        per-layer fold runs, else None."""
+        self._groups, self.layer_fold = groups, None
+        if self.fold_steps is not None:
+            self.passes = [(0, len(self.ids))]
+        elif groups is not None:
+            self.passes = list(groups)
+            G = max(n for _, n in groups)
+            self.layer_fold = (G, len(groups))
+            # the first layer's input: x repeated G times, one buffer per concurrently running step
+            self.xrep_all = [torch.empty((G * self.nb,) + tuple(example_x.shape[1:]), dtype=example_x.dtype,
+                                         device=self.dev) for _ in range(self.nbuf)]
+        else:
+            self.passes = [(k, 1) for k in range(len(self.ids))]
+
+    def _pass_inputs(self, x, par=0, grad=False):
+        """(s0, n, input, fold context) of every pass over this rank's row block ``x``.  Per-layer fold group (s0, n):
+        local samples s0 .. s0+n-1 in one pass over x repeated n times; row block k is global sample ids[s0] + k * Rs
+        (stream stride Rs << 40, as in the fused fold) and its logits are those of local sample s0 + k."""
+        if self._groups is not None:
+            xr, G = self.xrep_all[par], self.layer_fold[0]
+            with torch.no_grad():
+                xr.view((G,) + tuple(x.shape)).copy_(x.unsqueeze(0).expand((G,) + tuple(x.shape)))
+        for s0, n in self.passes:
+            if self._groups is None:
+                yield s0, n, x, contextlib.nullcontext()
+            else:
+                yield s0, n, xr[:n * self.nb], Fn.layer_fold(self.nb, self.sample_shards << 40, grad=grad)
 
     # -- operand tiles and KL prepared once per parameter version (cache_prep) ---------------------------------------
     def _plan_prep(self, example_x):
@@ -442,17 +463,29 @@ class MCForward:
         one.copy_((v.sum() / v.numel()).reshape(1))
         return Fn._ptr(one), 1
 
+    def _kl_arg(self, kls, terms=False, par=0):
+        """The (pointer, count) of the floats whose sum is one sample's KL, from the passes' KLs ``kls`` (local order):
+        with mixture-prior layers the mean of the per-sample estimates (_mean_kl).  Otherwise every sample has the same
+        KL, which a pass computes once: the first pass's per-layer scalars when a fused chain handed them over un-summed
+        (``terms``), else its scalar."""
+        from .modules import has_mixture
+        if has_mixture(self.net):
+            return self._mean_kl(kls, par)
+        if terms:
+            self._kl_terms = kls[0]                      # kept alive: a captured exchange reads it
+            return Fn._ptr(kls[0]), kls[0].numel()
+        one = self.kl_one_all[par:par + 1]
+        one.copy_(torch.as_tensor(kls[0], dtype=torch.float32, device=self.dev).detach().reshape(1))
+        return Fn._ptr(one), 1
+
     def _chain(self, x, base=None, advance=False, par=0):
         """This rank's samples through the engine into the sample buffer ``par``.  A fused chain writes its logits
         straight into it and hands over its per-layer KL scalars un-summed (fused.direct_output).  Returns the (pointer,
         count) of the floats whose sum is one sample's KL."""
         from . import fused
         from .graph import _STRIDE
-        from .modules import has_mixture
-        mixture, sample_kls = has_mixture(self.net), []
         logits_buf = self.logits_all[par]
         kl_buf = self.kl_terms_all[par] if self.overlap else None
-        inc = _STRIDE * self.inflight
         b0, nb = self.rows[0], self.nb
         x = x[b0:b0 + nb]                                 # this rank's row block (a view: NCHW rows are contiguous)
         with torch.no_grad(), Fn.workspace_slot(par if self.inflight > 1 else Fn.current_workspace_slot()), \
@@ -464,55 +497,30 @@ class MCForward:
             # With the operands prepared ahead (self._prep) there is no prep in the step: the first GEMM kernel follows
             # this one directly.
             if advance:
-                Fn.noise_advance(base, inc)
-            kl_ptr, n_kl = None, 0
-            if self.fold_steps is not None:
-                with Fn.stream_base(base), Fn.mc_sample(self.ids[0], self.seed):
-                    _, kls = fused._run(self.fold_steps, x, True, logits_buf.view(len(self.ids) * nb, self.C), True, None,
-                                        fold=self.fold, kls_out=kl_buf)
-                self._kl_terms = kls
-                kl_ptr, n_kl = self._mean_kl([kls], par) if mixture else (Fn._ptr(kls), kls.numel())
-            if self._groups is not None:
-                # group (s0, n): local samples s0 .. s0+n-1 in one pass over n x nb rows; row block k is global sample
-                # ids[s0] + k * Rs (stream stride Rs << 40, as in the fused fold) and lands in logits_buf[s0 + k]
-                xr = self.xrep_all[par]
-                G = self.layer_fold[0]
-                xr.view((G,) + tuple(x.shape)).copy_(x.unsqueeze(0).expand((G,) + tuple(x.shape)))
-                for gi, (s0, n) in enumerate(self._groups):
-                    with Fn.stream_base(base), Fn.mc_sample(self.ids[s0], self.seed), \
-                            Fn.layer_fold(nb, self.sample_shards << 40):
-                        logits, kl = self.net(xr[:n * nb])
-                    logits_buf[s0:s0 + n].view(n * nb, self.C).copy_(logits.reshape(n * nb, self.C))
-                    if mixture:                               # [n] per-sample estimates of this pass
-                        sample_kls.append(kl)
-                    elif gi == 0:                               # every sample has the same KL, computed once per pass
-                        one = self.kl_one_all[par:par + 1]
-                        one.copy_(torch.as_tensor(kl, dtype=torch.float32, device=self.dev).reshape(1))
-                        kl_ptr, n_kl = Fn._ptr(one), 1
-            for k, j in enumerate(self.ids if self.fold_steps is None and self._groups is None else ()):
-                with Fn.stream_base(base), Fn.mc_sample(j, self.seed), \
-                        fused.direct_output(logits_buf[k], kl_buf if k == 0 else None) as hook:
-                    logits, kl = self.net(x)
-                if not hook.used:
-                    logits_buf[k].copy_(logits.reshape(nb, self.C))
-                if mixture:
-                    sample_kls.append(kl)
-                elif k == 0:
-                    if hook.used:
-                        self._kl_terms = kl                       # per-layer scalars of sample 0 (every sample has the same KL)
-                        kl_ptr, n_kl = Fn._ptr(kl), kl.numel()
-                    else:
-                        one = self.kl_one_all[par:par + 1]
-                        one.copy_(torch.as_tensor(kl, dtype=torch.float32, device=self.dev).reshape(1))
-                        kl_ptr, n_kl = Fn._ptr(one), 1
-            if sample_kls:
-                kl_ptr, n_kl = self._mean_kl(sample_kls, par)
+                Fn.noise_advance(base, _STRIDE * self.inflight)
+            kls, terms = [], False
+            for s0, n, xin, fold_ctx in self._pass_inputs(x, par):
+                out = logits_buf[s0:s0 + n].view(n * nb, self.C)
+                with Fn.stream_base(base), Fn.mc_sample(self.ids[s0], self.seed), fold_ctx:
+                    if self.fold_steps is not None:
+                        _, kl = fused._run(self.fold_steps, xin, True, out, True, None, fold=self.fold, kls_out=kl_buf)
+                        taken = True
+                    else:                                 # (the fused chain never takes a per-layer fold's pass)
+                        with fused.direct_output(out, kl_buf if s0 == 0 else None) as hook:
+                            logits, kl = self.net(xin)
+                        taken = hook.used
+                if not taken:
+                    out.copy_(logits.reshape(n * nb, self.C))
+                if s0 == 0:
+                    terms = taken
+                kls.append(kl)
             if not self.ids and self.group_index == 0:
                 raise L.EngineError("MCForward: sample group 0 must own a sample")
-        return kl_ptr, n_kl
+            return self._kl_arg(kls, terms, par) if kls else (None, 0)
 
     def _exchange(self, kl_ptr, n_kl, advance_base=None, par=0):
-        """The one kernel behind the samples: combine + exchange + heads (bbb_mc_exchange_info)."""
+        """The one kernel behind the samples: combine + exchange + heads (bbb_mc_exchange_sharded; with an evaluation
+        accumulator bbb_mc_exchange_metrics)."""
         from .graph import _STRIDE
         o = self.out
         lib = L.lib()
@@ -526,8 +534,6 @@ class MCForward:
         if self._metrics is not None:
             L.check(lib.bbb_mc_exchange_metrics(*args, self.batch_shards, Fn._ptr(self._metrics), Fn._stream(self.dev)),
                     "bbb_mc_exchange_metrics")
-        elif self.batch_shards == 1:
-            L.check(lib.bbb_mc_exchange_info(*args, Fn._stream(self.dev)), "bbb_mc_exchange_info")
         else:
             L.check(lib.bbb_mc_exchange_sharded(*args, self.batch_shards, Fn._stream(self.dev)), "bbb_mc_exchange_sharded")
 
@@ -1002,19 +1008,23 @@ def train_fold_groups(net, x_shape, n_local: int, stride: int, first_image: int 
     return groups
 
 
+def _fold_forward_supported(m, xs, n, fold, first_image):
+    """Does the engine take Bayesian layer m's forward of n samples folded into the batch, one sample's input of shape
+    ``xs`` (bbb_forward_supported)?"""
+    cfg = m._cfg(True)
+    d = Fn.make_desc((n * xs[0],) + tuple(xs[1:]), tuple(m.W_mu.shape), cfg["conv"], cfg["variant"], True,
+                     m.bias_mu is not None, cfg["prior_mu"], cfg["prior_sigma"], cfg["math"], cfg["kl_convention"],
+                     cfg["act"], fold=fold, first_image=first_image)
+    return L.lib().bbb_forward_supported(C.byref(d)) == 0
+
+
 def _train_fold_accepted(layers, n, fold, first_image):
     """Does the engine take a training pass of n folded samples: every layer's forward and backward?"""
-    lib = L.lib()
     for i, (m, xs) in enumerate(layers):
-        cfg = m._cfg(True)
-        xs = (n * xs[0],) + tuple(xs[1:])
-        d = Fn.make_desc(xs, tuple(m.W_mu.shape), cfg["conv"], cfg["variant"], True, m.bias_mu is not None,
-                         cfg["prior_mu"], cfg["prior_sigma"], cfg["math"], cfg["kl_convention"], cfg["act"], fold=fold,
-                         first_image=first_image)
-        if lib.bbb_forward_supported(C.byref(d)) != 0:
+        if not _fold_forward_supported(m, xs, n, fold, first_image):
             return False
         # the first layer's input is data (no input gradient); a later layer's input comes out of a layer
-        if Fn._fold_grad_refusal(cfg, xs, tuple(m.W_mu.shape), i > 0) is not None:
+        if Fn._fold_grad_refusal(m._cfg(True), (n * xs[0],) + tuple(xs[1:]), tuple(m.W_mu.shape), i > 0) is not None:
             return False
     return True
 
@@ -1059,51 +1069,27 @@ class MCTrainStep(MCForward):
         self.params = [p for p in net.parameters() if p.requires_grad]
         self.steps = 0
         if fold and len(self.ids) > 1:
-            self._groups = train_fold_groups(net, (self.nb,) + tuple(example_x.shape[1:]), len(self.ids),
-                                             self.sample_shards << 40, self.rows[0], fold_group)
-        if self._groups is not None:
-            G = max(n for _, n in self._groups)
-            self.layer_fold = (G, len(self._groups))
-            self.xrep = torch.empty((G * self.nb,) + tuple(example_x.shape[1:]), dtype=example_x.dtype, device=self.dev)
+            self._set_passes(train_fold_groups(net, (self.nb,) + tuple(example_x.shape[1:]), len(self.ids),
+                                               self.sample_shards << 40, self.rows[0], fold_group), example_x)
 
     def __call__(self, x, labels, beta: float = 0.0):
         from .graph import _STRIDE
+        from .modules import has_mixture
         self.beta = float(beta)
         self.labels.copy_(labels, non_blocking=True)
         for p in self.params:
             p.grad = None
         logits, kls = [], []
         b0, b1 = self.rows
-        xb = x[b0:b1]                                                  # this rank's row block
-        if self._groups is not None:
-            # group (s0, n): local samples s0 .. s0+n-1 in one pass over n x nb rows (stream stride Rs << 40, as in
-            # MCForward's per-layer fold); logits[i] holds the n samples of group i, one nb-row block each
-            G, nb = self.layer_fold[0], self.nb
-            with torch.no_grad():
-                self.xrep.view((G,) + tuple(xb.shape)).copy_(xb.unsqueeze(0).expand((G,) + tuple(xb.shape)))
-            for s0, n in self._groups:
-                with Fn.mc_sample(self.ids[s0], self.seed, offset=self.steps * _STRIDE), Fn.first_image(b0), \
-                        Fn.layer_fold(nb, self.sample_shards << 40, grad=True):
-                    lg, kl = self.net(self.xrep[:n * nb])
-                logits.append(lg)
-                kls.append(kl)
-                self.logits[s0:s0 + n].view(n * nb, self.C).copy_(lg.detach().reshape(n * nb, self.C))
-        else:
-            for k, j in enumerate(self.ids):
-                with Fn.mc_sample(j, self.seed, offset=self.steps * _STRIDE), Fn.first_image(b0):
-                    lg, kl = self.net(xb)                              # autograd on: per-layer kernels (no fused chain)
-                logits.append(lg)
-                kls.append(kl)
-                self.logits[k].copy_(lg.detach().reshape(self.nb, self.C))
-        from .modules import has_mixture
+        # logits[i] holds the n samples of pass i, one nb-row block each; autograd on: per-layer kernels (no fused chain)
+        for s0, n, xin, fold_ctx in self._pass_inputs(x[b0:b1], grad=True):
+            with Fn.mc_sample(self.ids[s0], self.seed, offset=self.steps * _STRIDE), Fn.first_image(b0), fold_ctx:
+                lg, kl = self.net(xin)
+            logits.append(lg)
+            kls.append(kl)
+            self.logits[s0:s0 + n].view(n * self.nb, self.C).copy_(lg.detach().reshape(n * self.nb, self.C))
         mixture = has_mixture(self.net)        # per-sample KL estimates: kls[i] is [n] for a folded group of n samples
-        kl_ptr, n_kl = None, 0
-        if self.ids and mixture:
-            kl_ptr, n_kl = self._mean_kl(kls)
-        elif self.ids:
-            self.kl_one.copy_(kls[0].detach())
-            kl_ptr, n_kl = Fn._ptr(self.kl_one), 1
-        self._exchange(kl_ptr, n_kl)
+        self._exchange(*(self._kl_arg(kls) if kls else (None, 0)))
         o = self.out
         if self.ids:
             S = float(self.num_ens)
