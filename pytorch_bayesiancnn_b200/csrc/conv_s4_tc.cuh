@@ -146,7 +146,6 @@ conv_s4_kernel(const S4Args p) {
     long long* tr = p.trace ? p.trace + (size_t)blockIdx.x * 128 : nullptr;
     if (tr && threadIdx.x == 0) tr[0] = clock64();
     tl_enter(p.tl_gemm);
-    pdl_trigger();
     if (threadIdx.x == 0) {
         for (int s = 0; s < S4_STAGES; ++s) { mbar_init(smem_u32(&ctl->full[s]), 1); mbar_init(smem_u32(&ctl->empty[s]), 8); }
         mbar_init(smem_u32(&ctl->img_ready[0]), 256);
@@ -294,6 +293,7 @@ conv_s4_kernel(const S4Args p) {
         // accumulators -> shared memory over the ring and the images (both consumed), then one tile row per thread
         float* accs = reinterpret_cast<float*>(sm + (ring - base));
         bar_sync(1, 256);
+        pdl_trigger();                                                      // dependents start at the epilogue (tap_gemm_kernel)
 #pragma unroll
         for (int ohl = 0; ohl < 2; ++ohl) {
             acc_to_smem(acc[ohl][0], accs + ((ohl * p.planes) * 128 + half * 64) * S4_AP, S4_AP);

@@ -339,7 +339,6 @@ tap_gemm_kernel(const FusedArgs p, const int stages) {
     long long* tr = p.trace ? p.trace + (size_t)(blockIdx.y * gridDim.x + blockIdx.x) * 128 : nullptr;
     if (tr && threadIdx.x == 0) tr[0] = clock64();
     tl_enter(p.tl_gemm);
-    pdl_trigger();
     if (threadIdx.x == 0) {
         for (int s = 0; s < stages; ++s) {
             mbar_init(smem_u32(&ctl->full[s]), 1);
@@ -501,6 +500,10 @@ tap_gemm_kernel(const FusedArgs p, const int stages) {
         constexpr int AP = BN + 4;                       // row pitch in floats
         float* accs = reinterpret_cast<float*>(sm + tiles_off);
         bar_sync(1, 256);                                // both warpgroups' wgmma retired before the ring is overwritten
+        // Dependents start here, not at kernel entry: one CTA per SM, so a dependent CTA resident early holds a whole SM
+        // in griddepcontrol.wait, an SM another in-flight step could use.  The epilogue still hides the dependent's
+        // prologue.  Only these threads, past the main loop, trigger (the first thread of a CTA to do so counts for it).
+        pdl_trigger();
         acc_to_smem(acc, accs + h * 64 * AP, AP);
         if (two) acc_to_smem(acc2, accs + (TC_BM + h * 64) * AP, AP);
         bar_sync(1, 256);
