@@ -374,7 +374,10 @@ int bbb_mc_graph_step(void* caller_stream, void* run_stream, void* in_ready, voi
  * utils.py:14-22): logits [S, B, C] fp32 -> log_outputs [B, C] =
  * logmeanexp_s(log_softmax(logits[s])).  Also emits per-sample partials
  * (sum_s softmax, sum_s softmax^2, sum_s logits) [3, B, C] if `moments` != NULL
- * (uncertainty_estimation.py:70-96). */
+ * (uncertainty_estimation.py:70-96).  These are raw sums: sum p^2 / S - (sum p / S)^2
+ * cancels when the samples agree and is no way to get the epistemic variance (the
+ * exchange below returns it centred).  A class at -inf in some samples adds nothing
+ * to log_outputs for those samples. */
 int bbb_mc_combine(const float* logits, int32_t S, int32_t B, int32_t C,
                    float* log_outputs, float* moments, void* cuda_stream);
 
@@ -382,12 +385,14 @@ int bbb_mc_combine(const float* logits, int32_t S, int32_t B, int32_t C,
  * (main_bayesian.py:46-61, utils.py:14-22, metrics.py:12-14,23-24, uncertainty_estimation.py:70-96; SURVEY.md 8e, f3, f4).
  * The num_ens samples are sharded over `world` ranks (one process per GPU); this rank holds `S_local` of the
  * `S_total` samples' logits [S_local, B, C].  One kernel: per-(image, class) partials of the local samples
- * (the exact (max, sum-exp) pair of logmeanexp, + sum p / sum p^2 / sum logits with BBB_MC_MOMENTS) are stored straight
+ * (the exact (max, sum-exp) pair of logmeanexp, + mean p / M2 = sum (p - mean)^2 / sum logits and the sample count with
+ * BBB_MC_MOMENTS, the ranks' moments merged with Chan's update) are stored straight
  * into every rank's receive buffer over NVLink (peer-mapped memory, below) as 8-byte words {value, sequence number};
  * the receiver polls each word until its tag matches (no fence, no flag; a lost peer is a counted time-out, never a
  * hang) and the result is finished locally in fixed rank order (bitwise identical on all ranks):
  *   log_outputs [B,C] = logmeanexp_j log_softmax(logits_j)      kl_out = sum_j kl_j / S_total
  *   pred / epistemic / aleatoric [B,C], entropy [B]             (nullable; need BBB_MC_MOMENTS)
+ *     epistemic = mean_s (p_hat_s - p_bar)^2 >= 0 (centred), aleatoric = p_bar (1 - p_bar) - epistemic
  *   head [4] = {nll*train_size + beta*kl, nll, accuracy, beta*kl}   (nullable; needs labels [B] int64)
  * BBB_MC_NORMALIZED: p_hat = softplus(logits) / sum softplus (uncertainty_estimation.py:73-75) instead of softmax.
  * peer_buffers: HOST array of `world` device pointers, one receive buffer per rank (bbb_mc_buffer_bytes each, zero-

@@ -17,8 +17,11 @@
 // Receive buffer of one rank (all ranks use the same layout):
 //   [0, 4096)                       reserved
 //   [4096, ...)                     u64 data[2 slots][world][n_planes * B * C + 2 (+ B with INFO)]
-// Per sending rank: the n_planes [B, C] planes, the KL word at n_planes * B * C, a spare word, and -- only in the INFO
-// instantiation -- a plane of B words behind them: sum over the rank's samples of H[p_hat_s] per image.
+// Per sending rank: the n_planes [B, C] planes, the KL word at n_planes * B * C, the sender's sample count behind it,
+// and -- only in the INFO instantiation -- a plane of B words behind them: sum over the rank's samples of H[p_hat_s] per
+// image.  With moments the planes are (max, sum-exp, mean p, M2 = sum (p - mean)^2, sum logits) over the sender's
+// samples: the finish merges the senders' (count, mean, M2) with Chan's update, so the epistemic variance is a centred
+// sum that cannot go negative, never the one-pass E[p^2] - p_bar^2, which cancels when the samples agree.
 // Row blocks (bbb_mc_exchange_sharded, world = Rs sample groups x Rb row blocks): [2 slots][Rs][...] of the same layout,
 // one sender slot per sample group; rank (g, k) writes the words of its rows [b0, b1) into slot g, the group's block-0
 // rank also the KL word.  Every row of a slot then comes from exactly one rank of its group.
@@ -47,7 +50,7 @@ struct McxArgs {
     int n_kl;                     // every sample, SURVEY D11); nullable
     unsigned long long* noise_base; unsigned long long noise_inc;   // optional: *noise_base += noise_inc when the launch is done
     int S_local, S_total, B, C;
-    int want_moments, normalized; // moments: also exchange sum p, sum p^2, sum logits;  normalized: p_hat = softplus/sum softplus
+    int want_moments, normalized; // moments: also exchange mean p, M2 of p, sum logits;  normalized: p_hat = softplus/sum softplus
     const long long* labels;      // [B] int64, nullable
     float train_size, beta;
     int rank, world;
@@ -158,21 +161,32 @@ mc_exchange_kernel(const McxArgs p) {
 
     const unsigned long long* rx = reinterpret_cast<const unsigned long long*>(p.peer[p.rank] + MCX_CTRL_BYTES) + slot_off;
     const bool solo = p.world == 1;     // one rank: the partials never leave the registers (no buffer round trip, no handshake)
+    if (!solo && blockIdx.x == 0 && threadIdx.x < p.world && (!SHARD || p.block == 0)) {
+        // this rank's KL contribution S_local * kl and its sample count (row blocks: the group's block-0 rank, so each
+        // group counts once), pushed first: the finish of every CTA needs the counts of all senders
+        unsigned long long* dst = reinterpret_cast<unsigned long long*>(p.peer[threadIdx.x] + MCX_CTRL_BYTES) + slot_off + (size_t)src() * rank_floats
+                                  + (size_t)mcx_planes(p.want_moments) * BC;
+        float one = 0.0f;
+        for (int i = 0; p.kl && i < p.n_kl; ++i) one += __ldg(p.kl + i);
+        st_ll(dst, (float)p.S_local * one, seq);
+        st_ll(dst + 1, (float)p.S_local, seq);
+    }
     // nll and correct count of the head, on lane 0.  METRICS: lane l < MCM_PART / 2 of a warp sums parts 2l and 2l + 1 of
     // its rows in them (lane 0's are the head's two), so the partials need no registers or shared memory of their own
     double nll_acc = 0.0, hit_acc = 0.0;
     // per-row state of the finish (4): running argmax, entropy, the label's log-probability
     struct RowFin { float best; int best_c; float ent, lab_lp; long long lab; };
-    auto fin_elem = [&](RowFin& rf, size_t e, int c, float M, float tot, float sp, float sp2, float sl) {
+    // pbar: the mean of p_hat over all S_total samples; m2: sum over them of (p_hat - pbar)^2
+    auto fin_elem = [&](RowFin& rf, size_t e, int c, float M, float tot, float pbar, float m2, float sl) {
         const float lo = M + logf(tot * inv_S);                           // utils.py:14-22
         p.log_outputs[e] = lo;
         if (lo > rf.best) { rf.best = lo; rf.best_c = c; }
         if ((long long)c == rf.lab) rf.lab_lp = lo;
         if (p.want_moments) {
-            const float pbar = sp * inv_S, p2 = sp2 * inv_S;
+            const float epi = m2 * inv_S;
             if (p.pred) p.pred[e] = sl * inv_S;                           // uncertainty_estimation.py:82-83
-            if (p.epistemic) p.epistemic[e] = p2 - pbar * pbar;           // :89-91  (E[p^2] - p_bar^2)
-            if (p.aleatoric) p.aleatoric[e] = pbar - p2;                  // :94-95  (p_bar - E[p^2])
+            if (p.epistemic) p.epistemic[e] = epi;                        // :89-91  mean((p - p_bar)^2), >= 0
+            if (p.aleatoric) p.aleatoric[e] = pbar * (1.0f - pbar) - epi; // :94-95  p_bar - E[p^2] = p_bar (1 - p_bar) - epi
             rf.ent -= pbar > 0.0f ? pbar * logf(pbar) : 0.0f;             // H[p_bar] (no reference, SURVEY D3)
         }
     };
@@ -254,23 +268,29 @@ mc_exchange_kernel(const McxArgs p) {
         RowFin rf{-INFINITY, 0x7fffffff, 0.0f, 0.0f, (solo && p.labels) ? p.labels[b] : -1};
         float hl = 0.0f;                                         // INFO: sum over local samples and this lane's classes of -p log p
         for (int c = lane; c < C; c += 32) {
-            float mx = -INFINITY, acc = 0.0f, sp = 0.0f, sp2 = 0.0f, sl = 0.0f;
+            float mx = -INFINITY, acc = 0.0f, mean = 0.0f, m2 = 0.0f, sl = 0.0f;
             for (int s = 0; s < p.S_local; ++s) {
                 const float l = p.logits[((size_t)s * nrows + bl) * C + c];
                 float pr, lp;
-                if (p.normalized) { pr = softplus_f(l) / norm_dyn[warp * p.S_local + s]; lp = logf(pr); }
+                if (p.normalized) {
+                    const float spl = softplus_f(l), nrm = norm_dyn[warp * p.S_local + s];
+                    pr = spl / nrm;
+                    // below FLT_MIN p_hat is subnormal or 0: its log from the parts (softplus(l) = e^l there, so l)
+                    lp = pr >= 1.17549435e-38f ? logf(pr) : (l < -80.0f ? l : logf(spl)) - logf(nrm);
+                }
                 else { lp = l - norm_dyn[warp * p.S_local + s]; pr = expf(lp); }            // log_softmax (main_bayesian.py:49)
                 if (lp > mx) { acc = acc * expf(mx - lp) + 1.0f; mx = lp; }  // online logsumexp over the samples
                 else if (lp > -INFINITY) acc += expf(lp - mx);               // lp == -inf: a probability of exactly 0 adds nothing
-                sp += pr; sp2 += pr * pr; sl += l;
+                const float d = pr - mean;                                   // Welford: mean and centred M2 of p_hat
+                mean += __fdividef(d, (float)(s + 1)); m2 += d * (pr - mean); sl += l;   // (2 ulp, no slow-path call)
                 if constexpr (INFO) hl -= pr > 0.0f ? pr * lp : 0.0f;       // 0 log 0 = 0, not 0 * -inf
             }
             const size_t e = (size_t)b * C + c;
-            if (solo) { fin_elem(rf, e, c, mx, acc, sp, sp2, sl); continue; }
+            if (solo) { fin_elem(rf, e, c, mx, acc, mean, m2, sl); continue; }
             for (int q = 0; q < p.world; ++q) {
                 unsigned long long* dst = reinterpret_cast<unsigned long long*>(p.peer[q] + MCX_CTRL_BYTES) + slot_off + (size_t)src() * rank_floats;
                 st_ll(dst + e, mx, seq); st_ll(dst + BC + e, acc, seq);
-                if (p.want_moments) { st_ll(dst + 2 * (size_t)BC + e, sp, seq); st_ll(dst + 3 * (size_t)BC + e, sp2, seq); st_ll(dst + 4 * (size_t)BC + e, sl, seq); }
+                if (p.want_moments) { st_ll(dst + 2 * (size_t)BC + e, mean, seq); st_ll(dst + 3 * (size_t)BC + e, m2, seq); st_ll(dst + 4 * (size_t)BC + e, sl, seq); }
             }
         }
         float hloc = 0.0f;                                       // INFO: sum over the local samples of H[p_hat_s]
@@ -288,14 +308,16 @@ mc_exchange_kernel(const McxArgs p) {
         if (blockIdx.x == 0 && threadIdx.x == 0) for (int i = 0; p.kl && i < p.n_kl; ++i) kl_solo += __ldg(p.kl + i);
         kl_solo *= (float)p.S_local;
     } else {
-        // this rank's KL contribution: S_local * kl (row blocks: the group's block-0 rank, so each group counts once)
-        if (blockIdx.x == 0 && threadIdx.x < p.world && (!SHARD || p.block == 0)) {
-            unsigned long long* dst = reinterpret_cast<unsigned long long*>(p.peer[threadIdx.x] + MCX_CTRL_BYTES) + slot_off + (size_t)src() * rank_floats;
-            float one = 0.0f;
-            for (int i = 0; p.kl && i < p.n_kl; ++i) one += __ldg(p.kl + i);
-            st_ll(dst + (size_t)mcx_planes(p.want_moments) * BC, (float)p.S_local * one, seq);
-        }
         if (tracer) tr[1] = (long long)globaltimer_ns();
+        // the senders' sample counts, for the merge of their moments (red is free until the head's block sums)
+        float* cnt = reinterpret_cast<float*>(red);
+        if (p.want_moments) {
+            if (threadIdx.x < nsrc()) {
+                const unsigned long long* w = rx + (size_t)threadIdx.x * rank_floats + (size_t)mcx_planes(p.want_moments) * BC + 1;
+                cnt[threadIdx.x] = ll_value(ld_ll(w), w);
+            }
+            __syncthreads();
+        }
         // ---- (4) finish: fixed rank (row blocks: group) order => bitwise identical on every rank --------------
         for (int b = b0 + warp; b < b1; b += nwarp) {
             RowFin rf{-INFINITY, 0x7fffffff, 0.0f, 0.0f, p.labels ? p.labels[b] : -1};
@@ -303,9 +325,9 @@ mc_exchange_kernel(const McxArgs p) {
                 const size_t e = (size_t)b * C + c;
                 // the words of this element from up to 8 ranks in flight at once (one L2 round trip), stragglers polled;
                 // ranks merged in ascending order with the online logsumexp update: same operations on every rank
-                float M = -INFINITY, tot = 0.0f, mom[3] = {0.0f, 0.0f, 0.0f};
+                float M = -INFINITY, tot = 0.0f;
+                unsigned long long wm[8], wa[8];                         // one pair of 8-word batches for every plane
                 for (int q0 = 0; q0 < nsrc(); q0 += 8) {
-                    unsigned long long wm[8], wa[8];
 #pragma unroll
                     for (int j = 0; j < 8; ++j) {
                         if (q0 + j >= nsrc()) continue;
@@ -323,21 +345,40 @@ mc_exchange_kernel(const McxArgs p) {
                         }
                     }
                 }
+                // moments: (count, mean, M2) of the senders merged in ascending order with Chan's update
+                // M2 = M2a + M2b + d^2 na nb / (na + nb), d = mean_b - mean_a; the logit sums added in the same order
+                float n = 0.0f, pbar = 0.0f, m2 = 0.0f, sl = 0.0f;
                 if (p.want_moments) {
+                    for (int q0 = 0; q0 < nsrc(); q0 += 8) {
 #pragma unroll
-                    for (int pl = 0; pl < 3; ++pl)
-                        for (int q0 = 0; q0 < nsrc(); q0 += 8) {
-                            unsigned long long w[8];
-#pragma unroll
-                            for (int j = 0; j < 8; ++j)
-                                if (q0 + j < nsrc()) w[j] = ld_ll(rx + (size_t)(q0 + j) * rank_floats + (size_t)(2 + pl) * BC + e);
-#pragma unroll
-                            for (int j = 0; j < 8; ++j)
-                                if (q0 + j < nsrc()) mom[pl] += ll_value(w[j], rx + (size_t)(q0 + j) * rank_floats + (size_t)(2 + pl) * BC + e);
+                        for (int j = 0; j < 8; ++j) {
+                            if (q0 + j >= nsrc()) continue;
+                            const unsigned long long* r = rx + (size_t)(q0 + j) * rank_floats + 2 * (size_t)BC + e;
+                            wm[j] = ld_ll(r); wa[j] = ld_ll(r + BC);
                         }
+#pragma unroll
+                        for (int j = 0; j < 8; ++j) {
+                            if (q0 + j >= nsrc()) continue;
+                            const unsigned long long* r = rx + (size_t)(q0 + j) * rank_floats + 2 * (size_t)BC + e;
+                            const float mq = ll_value(wm[j], r), m2q = ll_value(wa[j], r + BC), nq = cnt[q0 + j];
+                            if (nq > 0.0f) {
+                                const float nn = n + nq, d = mq - pbar, wq = __fdividef(nq, nn);
+                                pbar += d * wq;
+                                m2 += m2q + d * d * (n * wq);
+                                n = nn;
+                            }
+                        }
+                    }
+                    for (int q0 = 0; q0 < nsrc(); q0 += 8) {
+#pragma unroll
+                        for (int j = 0; j < 8; ++j)
+                            if (q0 + j < nsrc()) wm[j] = ld_ll(rx + (size_t)(q0 + j) * rank_floats + 4 * (size_t)BC + e);
+#pragma unroll
+                        for (int j = 0; j < 8; ++j)
+                            if (q0 + j < nsrc()) sl += ll_value(wm[j], rx + (size_t)(q0 + j) * rank_floats + 4 * (size_t)BC + e);
+                    }
                 }
-                const float sp = mom[0], sp2 = mom[1], sl = mom[2];
-                fin_elem(rf, e, c, M, tot, sp, sp2, sl);
+                fin_elem(rf, e, c, M, tot, pbar, m2, sl);
             }
             float hsum = 0.0f;
             if constexpr (INFO) {       // lane q fetches rank q's word (one round trip); every lane adds them in rank order
@@ -365,6 +406,7 @@ mc_exchange_kernel(const McxArgs p) {
     const bool want_head = p.head && p.labels;
     double nll_cta = 0.0, hit_cta = 0.0;
     if (want_head) {
+        __syncthreads();                 // every warp's finish has read the sender counts kept in red
         nll_cta = block_sum(METRICS && lane ? 0.0 : nll_acc, red);     // the head: lane 0's only
         __syncthreads();
         hit_cta = block_sum(METRICS && lane ? 0.0 : hit_acc, red);

@@ -173,7 +173,7 @@ mc_combine_kernel(const float* __restrict__ logits, int S, int B, int C, float* 
             const float l = logits[((size_t)s * B + b) * C + c];
             const float v = l - lse[s];          // log_softmax
             if (v > mx) { acc = acc * expf(mx - v) + 1.0f; mx = v; }
-            else acc += expf(v - mx);
+            else if (v > -INFINITY) acc += expf(v - mx);   // v == -inf: a probability of 0 adds nothing (not exp(NaN))
             const float pr = expf(v);
             sp += pr; sp2 += pr * pr; sl += l;
         }

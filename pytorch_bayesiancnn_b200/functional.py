@@ -873,7 +873,9 @@ def lrt_noise_grad(desc: L.LayerDesc, gy: torch.Tensor, act_std: torch.Tensor, s
 
 def mc_combine(logits: torch.Tensor, want_moments: bool = False):
     """logits [S,B,C] -> log_outputs [B,C] (main_bayesian.py:46-53) and optionally the
-    [3,B,C] sums (softmax, softmax^2, logits) for uncertainty_estimation.py:70-96."""
+    [3,B,C] raw sums over the samples of (softmax, softmax^2, logits).  Do not form the epistemic variance as
+    sum(p^2)/S - (sum(p)/S)^2 from them: when the samples agree the two terms are nearly equal and the fp32 difference is
+    mostly rounding, often negative.  The exchange (mc_forward / MCForward) returns a centred epistemic variance."""
     _require_cuda(logits, "mc_combine")
     logits = logits.contiguous().float()
     S, B, Cc = logits.shape

@@ -723,6 +723,25 @@ class MCForward:
         return self._chain_done[self._last] if (self.overlap and self.replays) else None
 
 
+def chan_merge(counts, means, m2s):
+    """Merge per-group (count, mean, M2 = sum (x - mean)^2) in the order given with Chan's update
+    M2 = M2a + M2b + d^2 na nb / (na + nb), d = mean_b - mean_a; groups with count 0 are skipped.  Returns (mean, M2)
+    of all the samples.  The variance stays a centred sum: no E[x^2] - mean^2, which cancels when the samples agree."""
+    n, mean, m2 = 0, None, None
+    for nq, mq, m2q in zip(counts, means, m2s):
+        if nq == 0:
+            continue
+        if mean is None:
+            n, mean, m2 = nq, mq.clone(), m2q.clone()
+            continue
+        nn = n + nq
+        d = mq - mean
+        mean = mean + d * (nq / nn)
+        m2 = m2 + m2q + d * d * (n * nq / nn)
+        n = nn
+    return mean, m2
+
+
 def _generic_mc_forward(forward_fn: Callable, x: torch.Tensor, num_ens: int, group=None, want_uncertainty: bool = False,
                         information: bool = False, batch_shards: int = 1):
     """Backend-agnostic restatement (any device, any torch.distributed backend): the exact (max, sum-exp) partials of
@@ -750,15 +769,18 @@ def _generic_mc_forward(forward_fn: Callable, x: torch.Tensor, num_ens: int, gro
             klv = torch.as_tensor(kl, dtype=torch.float32, device=dev).reshape(1)
             if information:
                 h = -torch.where(p > 0, p * lsm, torch.zeros_like(p)).sum(1)   # H[p_hat_j], 0 log 0 = 0
-            if parts is None:
-                parts = [lsm.clone(), torch.ones_like(lsm), p.clone(), p * p, logits.clone(), klv.clone()]
+            if parts is None:                         # planes 2, 3: Welford mean and M2 = sum (p - mean)^2 of p_hat
+                parts = [lsm.clone(), torch.ones_like(lsm), p.clone(), torch.zeros_like(p), logits.clone(), klv.clone()]
                 if information:
                     parts.append(h)
+                n = 1
             else:
                 m = torch.maximum(parts[0], lsm)
                 parts[1] = parts[1] * (parts[0] - m).exp() + (lsm - m).exp()
                 parts[0] = m
-                parts[2] += p; parts[3] += p * p; parts[4] += logits; parts[5] += klv
+                n += 1
+                d = p - parts[2]
+                parts[2] += d / n; parts[3] += d * (p - parts[2]); parts[4] += logits; parts[5] += klv
                 if information:
                     parts[6] += h
     if world > 1:
@@ -802,11 +824,12 @@ def _generic_mc_forward(forward_fn: Callable, x: torch.Tensor, num_ens: int, gro
     kl = sum(v[5 * n] for r, v in enumerate(allv) if r // rs == 0) / S      # main_bayesian.py:51; one block per group
     if not want_uncertainty:
         return log_outputs, kl
-    p_bar = (sum(plane(2)) / S).view(full)
-    p2 = (sum(plane(3)) / S).view(full)
+    counts = [len(local_samples(num_ens, rs, q)) for q in range(rs)]
+    p_bar, m2 = chan_merge(counts, plane(2), plane(3))
+    p_bar, m2 = p_bar.view(full), m2.view(full)
     pred = (sum(plane(4)) / S).view(full)
-    epistemic = p2 - p_bar * p_bar                    # diag((p-pbar)^T (p-pbar))/T  (uncertainty_estimation.py:89-91)
-    aleatoric = p_bar - p2                            # diag(diag(pbar) - p^T p / T)  (:94-95)
+    epistemic = m2 / S                                # diag((p-pbar)^T (p-pbar))/T, centred (uncertainty_estimation.py:89-91)
+    aleatoric = p_bar * (1.0 - p_bar) - epistemic     # diag(diag(pbar) - p^T p / T) = pbar - E[p^2]  (:94-95)
     entropy = -(p_bar * torch.log(p_bar.clamp_min(1e-38))).sum(1)      # H[pbar]; no reference (SURVEY D3)
     if not information:
         return log_outputs, kl, (pred, epistemic, aleatoric, entropy)

@@ -179,8 +179,10 @@ def test_mc_combine_matches_oracle(dev):
         assert (out.cpu() - ref).abs().max() < 2e-5
         pred, epi, ale, ent = O.uncertainty(list(logits))
         p1, p2, sl = [m.double().cpu() / S for m in mom]
+        ph = torch.softmax(logits.double(), 2)
         assert (sl - pred).abs().max() < 1e-5
-        assert ((p2 - p1 * p1) - epi).abs().max() < 1e-6       # epistemic = E[p^2] - pbar^2
+        # raw means of p and p^2 (not an epistemic variance: E[p^2] - pbar^2 cancels when the samples agree)
+        assert (p1 - ph.mean(0)).abs().max() < 1e-6 and (p2 - (ph * ph).mean(0)).abs().max() < 1e-6
         assert ((p1 - p2) - ale).abs().max() < 1e-6            # aleatoric = pbar - E[p^2]
 
 
