@@ -90,6 +90,24 @@ typedef struct bbb_prior {
     const float* b_mu;  const float* b_sigma;   /* [out_channels]; required iff has_bias      */
 } bbb_prior;
 
+/* Pruning mask of one layer, for the same entry points: pass a bbb_masked_prior as their `prior` and OR
+ * BBB_PRIOR_MASKED into the call's kl_convention (desc->kl_convention, or the kl_convention argument of the KL calls);
+ * without the flag the entry points read a plain bbb_prior, as before.  w_mask / b_mask are one byte per element of
+ * W_mu / bias_mu (0 = pruned, 1 = kept; torch.bool storage), DEVICE pointers in the same layouts; b_mask NULL keeps
+ * every bias.  A pruned element is a deterministic 0: BBB weight 0 (not mu + eps sigma), LRT mean and variance
+ * operands 0; it adds +0.0 to the KL in its own place (every convention, the scalar or the tensor prior), and every
+ * backward gives it exactly 0 gradient in mu and rho.  The mask selects, so a pruned element's mu / rho (inf or NaN
+ * included) never reach an output.  Noise is drawn as without a mask: a kept element, and an all-ones mask, give the
+ * unmasked call's bits.  The mask is read on every call that gets it, not only where a KL is computed.  The four
+ * Gaussian pointers of `prior` all NULL (with w_mask set) = the desc's / call's scalar prior, masked.  The Monte-Carlo
+ * KL calls (bbb_kl_mc_*) take no mask. */
+#define BBB_PRIOR_MASKED 0x100
+typedef struct bbb_masked_prior {
+    bbb_prior prior;
+    const uint8_t* w_mask;                      /* layout of W_mu, 0/1; NULL: no mask          */
+    const uint8_t* b_mask;                      /* [out_channels], 0/1; NULL: every bias kept  */
+} bbb_masked_prior;
+
 /* Bytes of caller-allocated scratch a forward/KL call on `desc` needs.  The
  * scratch must be zero-filled ONCE when allocated; calls leave it zeroed where
  * that matters (self-resetting counters).  A desc that folds the MC samples of a BBB layer
@@ -157,7 +175,8 @@ int bbb_linear_forward(const bbb_layer_desc* desc, const void* x,
                        void* workspace, size_t workspace_bytes, void* cuda_stream);
 
 /* bbb_conv2d_forward / bbb_linear_forward with the layer's KL (kl_out) taken against the per-element prior `prior`
- * (bbb_prior; NULL = the scalar call).  y, act_std and every other output are those of the scalar call. */
+ * (bbb_prior; NULL = the scalar call).  y, act_std and every other output are those of the scalar call, unless a
+ * mask (bbb_masked_prior) prunes elements. */
 int bbb_conv2d_forward_prior(const bbb_layer_desc* desc, const void* x,
                              const float* W_mu, const float* W_rho,
                              const float* bias_mu, const float* bias_rho,
@@ -226,7 +245,8 @@ int bbb_layer_forward_fused(const bbb_layer_desc* desc,
                             uint64_t seed, uint64_t stream_id, const uint64_t* stream_base,
                             void* workspace, size_t workspace_bytes, void* cuda_stream);
 /* bbb_layer_forward_fused with the KL taken against the per-element prior `prior` (bbb_prior; NULL = the scalar call).
- * Only the weight-prep kernel reads it (a BBB_FUSED_SKIP_PREP call computes no KL and ignores it). */
+ * Only the weight-prep kernel reads it, a mask (bbb_masked_prior) included (a BBB_FUSED_SKIP_PREP call computes no KL
+ * and ignores it: the prepared operands already hold the mask of the prep that wrote them). */
 int bbb_layer_forward_fused_prior(const bbb_layer_desc* desc,
                                   const void* x, const void* x_sq, int32_t in_layout, int32_t in_pitch, int32_t prev_hw,
                                   const float* W_mu, const float* W_rho,
@@ -251,7 +271,8 @@ int bbb_kl_forward(const float* W_mu, const float* W_rho, uint64_t n_w,
                    float* kl_out, void* workspace, size_t workspace_bytes, void* cuda_stream);
 
 /* bbb_kl_forward against the per-element prior `prior` (bbb_prior over W_mu's n_w and bias_mu's n_b elements; the
- * bias pointers are required when n_b > 0).  prior_mu / prior_sigma are then not used; NULL = bbb_kl_forward. */
+ * bias pointers are required when n_b > 0).  prior_mu / prior_sigma are then not used (unless it is a mask only,
+ * bbb_masked_prior); NULL = bbb_kl_forward.  Pruned elements add +0.0 in their place of the same sum. */
 int bbb_kl_forward_prior(const float* W_mu, const float* W_rho, uint64_t n_w,
                          const float* bias_mu, const float* bias_rho, uint64_t n_b,
                          float prior_mu, float prior_sigma, int32_t kl_convention,
@@ -265,7 +286,8 @@ int bbb_kl_backward(const float* mu, const float* rho, uint64_t n,
                     const float* grad_kl, float* g_mu, float* g_rho, void* cuda_stream);
 /* bbb_kl_backward of n elements (a weight tensor, or a bias) against the per-element prior prior->w_mu / prior->w_sigma,
  * laid out like mu (b_mu / b_sigma are not read: for a bias, pass its prior in the w_ fields).  No gradient flows to
- * the prior.  NULL = bbb_kl_backward. */
+ * the prior.  NULL = bbb_kl_backward.  With a mask (bbb_masked_prior; w_mask is the n elements' mask, b_mask is not
+ * read) nothing is added to g_mu / g_rho at a pruned element. */
 int bbb_kl_backward_prior(const float* mu, const float* rho, uint64_t n,
                           float prior_mu, float prior_sigma, int32_t kl_convention,
                           const float* grad_kl, float* g_mu, float* g_rho, void* cuda_stream,
@@ -334,6 +356,28 @@ int bbb_linear_backward(const bbb_layer_desc* desc, const void* x, const void* g
                         void* grad_x, float* g_W_mu, float* g_W_rho,
                         float* g_bias_mu, float* g_bias_rho,
                         void* workspace, size_t workspace_bytes, void* cuda_stream);
+/* The same backwards for a layer with a pruning mask (a bbb_masked_prior with BBB_PRIOR_MASKED in desc->kl_convention;
+ * its Gaussian pointers are not read here, no KL is involved): a pruned weight is 0 in the input gradient, and nothing
+ * is added to g_* at a pruned element.  Two entry points of their own because the backwards above take no prior and
+ * their signatures cannot change without breaking their callers; NULL = the call above. */
+int bbb_conv2d_backward_prior(const bbb_layer_desc* desc, const void* x, const void* grad_y,
+                              const float* W_mu, const float* W_rho,
+                              const float* bias_mu, const float* bias_rho,
+                              const float* act_std,
+                              const float* eps_a, const float* eps_b,
+                              uint64_t seed, uint64_t stream_id, const uint64_t* stream_base,
+                              void* grad_x, float* g_W_mu, float* g_W_rho,
+                              float* g_bias_mu, float* g_bias_rho,
+                              void* workspace, size_t workspace_bytes, void* cuda_stream, const bbb_prior* prior);
+int bbb_linear_backward_prior(const bbb_layer_desc* desc, const void* x, const void* grad_y,
+                              const float* W_mu, const float* W_rho,
+                              const float* bias_mu, const float* bias_rho,
+                              const float* act_std,
+                              const float* eps_a, const float* eps_b,
+                              uint64_t seed, uint64_t stream_id, const uint64_t* stream_base,
+                              void* grad_x, float* g_W_mu, float* g_W_rho,
+                              float* g_bias_mu, float* g_bias_rho,
+                              void* workspace, size_t workspace_bytes, void* cuda_stream, const bbb_prior* prior);
 
 /* The engine's noise stream, exposed so the host side of the boundary can draw
  * exactly what a kernel draws: out[i] = N(0,1) lane ((offset+i)&3) of

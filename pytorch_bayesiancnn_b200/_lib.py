@@ -35,7 +35,7 @@ SYMBOLS = (
     "bbb_mc_metrics_bytes", "bbb_mc_exchange_metrics", "bbb_lrt_noise_grad",
     "bbb_conv2d_forward_prior", "bbb_linear_forward_prior", "bbb_layer_forward_fused_prior", "bbb_kl_forward_prior",
     "bbb_kl_backward_prior", "bbb_kl_mc_workspace_bytes", "bbb_kl_mc_forward", "bbb_kl_mc_backward",
-    "bbb_mc_graph_step",
+    "bbb_mc_graph_step", "bbb_conv2d_backward_prior", "bbb_linear_backward_prior",
 )
 MC_MOMENTS, MC_NORMALIZED, MC_INFO = 1, 2, 4
 MC_CAL_BINS = 15                 # BBB_MC_CAL_BINS: calibration bins of the evaluation accumulator
@@ -53,6 +53,15 @@ class LayerDesc(C.Structure):
 class Prior(C.Structure):
     """struct bbb_prior (include/bbb_b200.h): per-element Gaussian prior, fp32 device pointers."""
     _fields_ = [(n, C.c_void_p) for n in ("w_mu", "w_sigma", "b_mu", "b_sigma")]
+
+
+class MaskedPrior(Prior):
+    """struct bbb_masked_prior (include/bbb_b200.h): a bbb_prior followed by the pruning mask, one byte per element
+    (w_mask, b_mask; NULL: none).  Passed where a bbb_prior is, with PRIOR_MASKED in the call's kl_convention."""
+    _fields_ = [(n, C.c_void_p) for n in ("w_mask", "b_mask")]
+
+
+PRIOR_MASKED = 0x100             # BBB_PRIOR_MASKED
 
 
 class MixturePrior(C.Structure):
@@ -87,6 +96,9 @@ def _bind(lib):
     pp = C.POINTER(Prior)
     for name in ("bbb_conv2d_forward_prior", "bbb_linear_forward_prior"):
         getattr(lib, name).argtypes = fwd + [pp]
+        getattr(lib, name).restype = C.c_int
+    for name in ("bbb_conv2d_backward_prior", "bbb_linear_backward_prior"):
+        getattr(lib, name).argtypes = bwd + [pp]
         getattr(lib, name).restype = C.c_int
     lib.bbb_layer_forward_fused_prior.argtypes = lib.bbb_layer_forward_fused.argtypes + [pp]
     lib.bbb_layer_forward_fused_prior.restype = C.c_int

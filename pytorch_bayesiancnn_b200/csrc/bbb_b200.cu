@@ -157,17 +157,42 @@ void layer_args(bbb::LayerArgs& a, const bbb_layer_desc* d, const bbb::Geom& g, 
     a.tl_gemm = tl_slot(do_gemm, gemm_name, g);
 }
 
-// A tensor prior (bbb_prior) is all tensors: the weight part always, the bias part with a bias.
-int check_prior(const bbb_prior* q, bool has_bias) {
+// The pruning mask of a call (bbb_masked_prior): BBB_PRIOR_MASKED in its kl_convention says that `prior` points at a
+// bbb_masked_prior.  take_masks clears the flag and returns the masks (NULL without).
+struct Masks { const uint8_t* w; const uint8_t* b; };
+Masks take_masks(const bbb_prior* prior, int32_t& conv) {
+    Masks m = {nullptr, nullptr};
+    if (conv & BBB_PRIOR_MASKED) {
+        conv &= ~BBB_PRIOR_MASKED;
+        if (prior) {
+            const bbb_masked_prior* q = reinterpret_cast<const bbb_masked_prior*>(prior);
+            m.w = q->w_mask; m.b = q->w_mask ? q->b_mask : nullptr;
+        }
+    }
+    return m;
+}
+// The same for a call with a desc: the desc without the flag (a copy in `copy` when it had it)
+const bbb_layer_desc* desc_masks(const bbb_layer_desc* d, const bbb_prior* prior, bbb_layer_desc& copy, Masks& m) {
+    m = Masks{nullptr, nullptr};
+    if (!d || !(d->kl_convention & BBB_PRIOR_MASKED)) return d;
+    copy = *d;
+    m = take_masks(prior, copy.kl_convention);
+    return &copy;
+}
+
+// A tensor prior (bbb_prior) is all tensors: the weight part always, the bias part with a bias.  All four NULL is the
+// scalar prior of the desc / call, valid only beside a mask.
+int check_prior(const bbb_prior* q, bool has_bias, const Masks& mk = Masks{nullptr, nullptr}) {
     if (!q) return BBB_OK;
+    if (!q->w_mu && !q->w_sigma && !q->b_mu && !q->b_sigma && mk.w) return BBB_OK;
     if (!q->w_mu || !q->w_sigma) return fail(BBB_E_INVALID, "prior: w_mu / w_sigma NULL (a prior is all tensors)");
     if (has_bias && (!q->b_mu || !q->b_sigma)) return fail(BBB_E_INVALID, "prior: has_bias set but b_mu / b_sigma NULL");
     return BBB_OK;
 }
 // What the kernels get of a tensor prior: its pointers when the call computes a KL, else none (the scalar kernels run
-// and nothing of the prior is read)
-bbb::PriorPtrs prior_ptrs(const bbb_prior* q, const float* kl_out) {
-    bbb::PriorPtrs t = {nullptr, nullptr, nullptr, nullptr};
+// and nothing of the prior is read); and the mask, always (NULL: the unmasked kernels run)
+bbb::PriorPtrs prior_ptrs(const bbb_prior* q, const float* kl_out, const Masks& mk = Masks{nullptr, nullptr}) {
+    bbb::PriorPtrs t = {nullptr, nullptr, nullptr, nullptr, mk.w, mk.b};
     if (q && kl_out) { t.w_mu = q->w_mu; t.w_sigma = q->w_sigma; t.b_mu = q->b_mu; t.b_sigma = q->b_sigma; }
     return t;
 }
@@ -197,11 +222,14 @@ int forward_impl(const bbb_layer_desc* d, bool linear, const void* x, const floa
                  const float* bias_mu, const float* bias_rho, void* y, float* kl_out, float* act_std,
                  const float* eps_a, const float* eps_b, uint64_t seed, uint64_t stream_id, const uint64_t* stream_base, void* ws,
                  size_t ws_bytes, void* stream, const bbb_prior* prior) {
+    bbb_layer_desc dcopy;
+    Masks mk;
+    d = desc_masks(d, prior, dcopy, mk);
     bbb::Geom g;
     if (int rc = check_desc(d, g, linear)) return rc;
     if (!x || !W_mu || !W_rho || !y) return fail(BBB_E_INVALID, "NULL tensor pointer");
     if (d->has_bias && (!bias_mu || !bias_rho)) return fail(BBB_E_INVALID, "has_bias set but bias pointers NULL");
-    if (int rc = check_prior(prior, d->has_bias != 0)) return rc;
+    if (int rc = check_prior(prior, d->has_bias != 0, mk)) return rc;
     if (kl_out && (!ws || ws_bytes < bbb_workspace_bytes(d)))
         return fail(BBB_E_WORKSPACE, "workspace too small: need %zu bytes", bbb_workspace_bytes(d));
     cudaStream_t st = (cudaStream_t)stream;
@@ -222,7 +250,7 @@ int forward_impl(const bbb_layer_desc* d, bool linear, const void* x, const floa
         a.skip_prep = 0; a.prep_only = 0; a.y_sq = nullptr; a.out_mode = 2; a.out_pitch = 0; a.pool = 0;
         a.x = x; a.y = y; a.act_std = act_std; a.act_dtype = d->act_dtype;
         int nl = 0;
-        cudaError_t e = bbb::launch_fwd_tc(a, st, sm_count(), &nl, prior_ptrs(prior, kl_out));
+        cudaError_t e = bbb::launch_fwd_tc(a, st, sm_count(), &nl, prior_ptrs(prior, kl_out, mk));
         if (e != cudaSuccess) return cuda_fail(e, "fwd_tc launch");
         g_launches += nl;
         return BBB_OK;
@@ -236,7 +264,7 @@ int forward_impl(const bbb_layer_desc* d, bool linear, const void* x, const floa
     a.prior_mu = d->prior_mu; a.prior_sigma = d->prior_sigma;
     a.sample = d->sample; a.kl_convention = d->kl_convention; a.has_bias = d->has_bias; a.act = d->epilogue_act;
     a.first_image = first_image_of(*d);
-    a.prior = prior_ptrs(prior, kl_out);
+    a.prior = prior_ptrs(prior, kl_out, mk);
     cudaError_t e = d->variant == BBB_VARIANT_LRT ? bbb::launch_fwd_simt<BBB_VARIANT_LRT>(a, st)
                                                   : bbb::launch_fwd_simt<BBB_VARIANT_BBB>(a, st);
     if (e != cudaSuccess) return cuda_fail(e, "fwd_simt launch");
@@ -248,7 +276,10 @@ int backward_impl(const bbb_layer_desc* d, bool linear, const void* x, const voi
                   const float* W_rho, const float* bias_mu, const float* bias_rho, const float* act_std,
                   const float* eps_a, const float* eps_b, uint64_t seed, uint64_t stream_id, const uint64_t* stream_base, void* grad_x,
                   float* g_W_mu, float* g_W_rho, float* g_bias_mu, float* g_bias_rho, void* ws, size_t ws_bytes,
-                  void* stream) {
+                  void* stream, const bbb_prior* prior) {
+    bbb_layer_desc dcopy;
+    Masks mk;
+    d = desc_masks(d, prior, dcopy, mk);
     bbb::Geom g;
     if (int rc = check_desc(d, g, linear)) return rc;
     if (!x || !grad_y || !W_mu || !W_rho) return fail(BBB_E_INVALID, "NULL tensor pointer");
@@ -257,6 +288,7 @@ int backward_impl(const bbb_layer_desc* d, bool linear, const void* x, const voi
         return fail(BBB_E_UNSUPPORTED, "backward through a fused activation/pool epilogue is not available");
     if (d->variant == BBB_VARIANT_LRT && d->sample && !act_std)
         return fail(BBB_E_INVALID, "LRT backward needs the act_std tensor saved by the forward");
+    if (int rc = check_prior(prior, d->has_bias != 0, mk)) return rc;
     (void)ws; (void)ws_bytes;
     bbb::BwdArgs a;
     a.g = g; a.x = (const float*)x; a.gy = (const float*)grad_y; a.w_mu = W_mu; a.w_rho = W_rho;
@@ -265,6 +297,7 @@ int backward_impl(const bbb_layer_desc* d, bool linear, const void* x, const voi
     a.gx = (float*)grad_x; a.g_w_mu = g_W_mu; a.g_w_rho = g_W_rho; a.g_b_mu = g_bias_mu; a.g_b_rho = g_bias_rho;
     a.sample = d->sample; a.has_bias = d->has_bias; a.variant = d->variant;
     a.first_image = first_image_of(*d);
+    a.prior = prior_ptrs(prior, nullptr, mk);       // the backward reads the mask only
     int nl = 0;
     cudaError_t e = bbb::launch_bwd_simt(a, (cudaStream_t)stream, sm_count(), &nl);
     if (e != cudaSuccess) return cuda_fail(e, "bwd_simt launch");
@@ -325,7 +358,7 @@ int bbb_conv2d_backward(const bbb_layer_desc* desc, const void* x, const void* g
                         size_t workspace_bytes, void* cuda_stream) {
     return backward_impl(desc, false, x, grad_y, W_mu, W_rho, bias_mu, bias_rho, act_std, eps_a, eps_b, seed,
                          stream_id, stream_base, grad_x, g_W_mu, g_W_rho, g_bias_mu, g_bias_rho, workspace, workspace_bytes,
-                         cuda_stream);
+                         cuda_stream, nullptr);
 }
 
 int bbb_linear_backward(const bbb_layer_desc* desc, const void* x, const void* grad_y, const float* W_mu,
@@ -335,7 +368,28 @@ int bbb_linear_backward(const bbb_layer_desc* desc, const void* x, const void* g
                         size_t workspace_bytes, void* cuda_stream) {
     return backward_impl(desc, true, x, grad_y, W_mu, W_rho, bias_mu, bias_rho, act_std, eps_a, eps_b, seed,
                          stream_id, stream_base, grad_x, g_W_mu, g_W_rho, g_bias_mu, g_bias_rho, workspace, workspace_bytes,
-                         cuda_stream);
+                         cuda_stream, nullptr);
+}
+
+int bbb_conv2d_backward_prior(const bbb_layer_desc* desc, const void* x, const void* grad_y, const float* W_mu,
+                              const float* W_rho, const float* bias_mu, const float* bias_rho, const float* act_std,
+                              const float* eps_a, const float* eps_b, uint64_t seed, uint64_t stream_id,
+                              const uint64_t* stream_base, void* grad_x, float* g_W_mu, float* g_W_rho, float* g_bias_mu,
+                              float* g_bias_rho, void* workspace, size_t workspace_bytes, void* cuda_stream,
+                              const bbb_prior* prior) {
+    return backward_impl(desc, false, x, grad_y, W_mu, W_rho, bias_mu, bias_rho, act_std, eps_a, eps_b, seed,
+                         stream_id, stream_base, grad_x, g_W_mu, g_W_rho, g_bias_mu, g_bias_rho, workspace, workspace_bytes,
+                         cuda_stream, prior);
+}
+int bbb_linear_backward_prior(const bbb_layer_desc* desc, const void* x, const void* grad_y, const float* W_mu,
+                              const float* W_rho, const float* bias_mu, const float* bias_rho, const float* act_std,
+                              const float* eps_a, const float* eps_b, uint64_t seed, uint64_t stream_id,
+                              const uint64_t* stream_base, void* grad_x, float* g_W_mu, float* g_W_rho, float* g_bias_mu,
+                              float* g_bias_rho, void* workspace, size_t workspace_bytes, void* cuda_stream,
+                              const bbb_prior* prior) {
+    return backward_impl(desc, true, x, grad_y, W_mu, W_rho, bias_mu, bias_rho, act_std, eps_a, eps_b, seed,
+                         stream_id, stream_base, grad_x, g_W_mu, g_W_rho, g_bias_mu, g_bias_rho, workspace, workspace_bytes,
+                         cuda_stream, prior);
 }
 
 /* shape / layout / MC-fold checks of bbb_layer_forward_fused, callable without a GPU (host logic only); `s4` tells
@@ -405,6 +459,9 @@ int bbb_layer_forward_fused_prior(const bbb_layer_desc* d, const void* x, const 
                                   int32_t out_pitch, float* kl_out, const float* eps_a, const float* eps_b, uint64_t seed,
                                   uint64_t stream_id, const uint64_t* stream_base, void* ws, size_t ws_bytes, void* stream,
                                   const bbb_prior* prior) {
+    bbb_layer_desc dcopy;
+    Masks mk;
+    d = desc_masks(d, prior, dcopy, mk);
     bbb::Geom g;
     bool s4;
     if (int rc = fused_check(d, g, in_layout, in_pitch, prev_hw, out_layout, out_pitch, s4)) return rc;
@@ -413,7 +470,7 @@ int bbb_layer_forward_fused_prior(const bbb_layer_desc* d, const void* x, const 
     const bool timed = (d->reserved[0] & BBB_FUSED_NO_TIMELINE) == 0;
     if (!W_mu || !W_rho || (!prep_only && (!x || !y))) return fail(BBB_E_INVALID, "NULL tensor pointer");
     if (d->has_bias && (!bias_mu || !bias_rho)) return fail(BBB_E_INVALID, "has_bias set but bias pointers NULL");
-    if (int rc = check_prior(prior, d->has_bias != 0)) return rc;
+    if (int rc = check_prior(prior, d->has_bias != 0, mk)) return rc;
     const int pool = d->pool_k != 0;
     bbb::McFold fold;                   // rows, samples and path checked by fused_check
     if (int rc = layer_fold(d, g, eps_a, eps_b, fold)) return rc;
@@ -430,7 +487,7 @@ int bbb_layer_forward_fused_prior(const bbb_layer_desc* d, const void* x, const 
         layer_args(a, d, g, W_mu, W_rho, bias_mu, bias_rho, kl_out, eps_a, eps_b, seed, stream_id, stream_base, ws,
                    bbb::conv_s4_bias_offset(g), fold, "conv_s4_prep", timed && !skip_prep, "conv_s4", timed && !prep_only);
         a.x = (const float*)x; a.y = y; a.y_sq = y_sq; a.out_pitch = out_pitch;
-        cudaError_t e = bbb::launch_conv_s4(a, st, !skip_prep, !prep_only, &nl, prior_ptrs(prior, kl_out));
+        cudaError_t e = bbb::launch_conv_s4(a, st, !skip_prep, !prep_only, &nl, prior_ptrs(prior, kl_out, mk));
         if (e != cudaSuccess) return cuda_fail(e, "conv_s4 launch");
     } else if (in_layout == BBB_LAYOUT_NCHW_F32) {
         bbb::TcArgs a;                  // fold.rows = 0: fused_check refuses a fold on the gather path
@@ -438,7 +495,7 @@ int bbb_layer_forward_fused_prior(const bbb_layer_desc* d, const void* x, const 
                    bbb::tc_bias_offset(g, false), fold, "weight_prep", timed && !skip_prep, "gemm_tc", timed && !prep_only);
         a.x = x; a.y = y; a.act_std = nullptr; a.act_dtype = d->act_dtype; a.tf32 = 0;
         a.skip_prep = skip_prep; a.prep_only = prep_only; a.y_sq = y_sq; a.out_mode = out_mode == 1 ? 2 : out_mode; a.out_pitch = out_pitch; a.pool = pool;
-        cudaError_t e = bbb::launch_fwd_tc(a, st, sm_count(), &nl, prior_ptrs(prior, kl_out));
+        cudaError_t e = bbb::launch_fwd_tc(a, st, sm_count(), &nl, prior_ptrs(prior, kl_out, mk));
         if (e != cudaSuccess) return cuda_fail(e, "fused gather launch");
     } else if (in_layout == BBB_LAYOUT_PACKED_BF16) {
         bbb::FusedArgs a;
@@ -448,7 +505,7 @@ int bbb_layer_forward_fused_prior(const bbb_layer_desc* d, const void* x, const 
         a.in_pitch = in_pitch;
         const char* why = "";
         cudaError_t e = bbb::launch_fused(a, x, x_sq, st, &nl, &why, !skip_prep, !prep_only, sm_count(), g_wide_tiles.load() != 0,
-                                          prior_ptrs(prior, kl_out));
+                                          prior_ptrs(prior, kl_out, mk));
         if (e != cudaSuccess) return fail(BBB_E_CUDA, "fused tap-GEMM launch: %s %s", cudaGetErrorString(e), why);
     } else {
         return fail(BBB_E_INVALID, "bad in_layout %d", in_layout);
@@ -467,11 +524,13 @@ int bbb_kl_forward(const float* W_mu, const float* W_rho, uint64_t n_w, const fl
 int bbb_kl_forward_prior(const float* W_mu, const float* W_rho, uint64_t n_w, const float* bias_mu,
                          const float* bias_rho, uint64_t n_b, float prior_mu, float prior_sigma, int32_t kl_convention,
                          float* kl_out, void* workspace, size_t workspace_bytes, void* cuda_stream, const bbb_prior* prior) {
+    const Masks mk = take_masks(prior, kl_convention);
     if (!W_mu || !W_rho || !kl_out) return fail(BBB_E_INVALID, "NULL tensor pointer");
     if (n_b && (!bias_mu || !bias_rho)) return fail(BBB_E_INVALID, "n_b > 0 but bias pointers NULL");
-    if (int rc = check_prior(prior, n_b > 0)) return rc;
+    if (int rc = check_prior(prior, n_b > 0, mk)) return rc;
     if (!workspace || workspace_bytes < kBaseWorkspace) return fail(BBB_E_WORKSPACE, "workspace too small: need %zu bytes", kBaseWorkspace);
-    if (!prior && !(prior_sigma > 0.0f)) return fail(BBB_E_INVALID, "prior_sigma must be > 0");
+    const bool tensor_prior = prior && prior->w_mu, masked = mk.w != nullptr;
+    if (!tensor_prior && !(prior_sigma > 0.0f)) return fail(BBB_E_INVALID, "prior_sigma must be > 0");
     const uint64_t work = (n_w + 3) / 4 + n_b;
     uint64_t blocks = (work + 255) / 256;
     const uint64_t cap = (uint64_t)sm_count() * 8;
@@ -479,7 +538,15 @@ int bbb_kl_forward_prior(const float* W_mu, const float* W_rho, uint64_t n_w, co
     if (blocks < 1) blocks = 1;
     if (blocks > kMaxKlSlots) blocks = kMaxKlSlots;
     double* partials = (double*)((char*)workspace + kCounterBytes);
-    if (prior)
+    if (masked && tensor_prior)
+        bbb::kl_forward_masked_kernel<true><<<(unsigned)blocks, 256, 0, (cudaStream_t)cuda_stream>>>(
+            W_mu, W_rho, n_w, bias_mu, bias_rho, n_b, 0.0f, 1.0f, prior_ptrs(prior, kl_out, mk), kl_convention, partials,
+            (unsigned int*)workspace, kl_out);
+    else if (masked)
+        bbb::kl_forward_masked_kernel<false><<<(unsigned)blocks, 256, 0, (cudaStream_t)cuda_stream>>>(
+            W_mu, W_rho, n_w, bias_mu, bias_rho, n_b, prior_mu, prior_sigma, prior_ptrs(prior, kl_out, mk), kl_convention,
+            partials, (unsigned int*)workspace, kl_out);
+    else if (prior)
         bbb::kl_forward_prior_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)cuda_stream>>>(
             W_mu, W_rho, n_w, bias_mu, bias_rho, n_b, prior_ptrs(prior, kl_out), kl_convention, partials,
             (unsigned int*)workspace, kl_out);
@@ -502,13 +569,20 @@ int bbb_kl_backward(const float* mu, const float* rho, uint64_t n, float prior_m
 int bbb_kl_backward_prior(const float* mu, const float* rho, uint64_t n, float prior_mu, float prior_sigma,
                           int32_t kl_convention, const float* grad_kl, float* g_mu, float* g_rho, void* cuda_stream,
                           const bbb_prior* prior) {
+    const Masks mk = take_masks(prior, kl_convention);
     if (!mu || !rho || !grad_kl || !g_mu || !g_rho) return fail(BBB_E_INVALID, "NULL tensor pointer");
-    if (int rc = check_prior(prior, false)) return rc;       // the n elements' prior is prior->w_mu / w_sigma
+    if (int rc = check_prior(prior, false, mk)) return rc;   // the n elements' prior is prior->w_mu / w_sigma
     if (n == 0) return BBB_OK;
     uint64_t blocks = (n + 255) / 256;
     const uint64_t cap = (uint64_t)sm_count() * 8;
     if (blocks > cap) blocks = cap;
-    if (prior)
+    const bool tensor_prior = prior && prior->w_mu;
+    if (mk.w)
+        (tensor_prior ? bbb::kl_backward_masked_kernel<true> : bbb::kl_backward_masked_kernel<false>)
+            <<<(unsigned)blocks, 256, 0, (cudaStream_t)cuda_stream>>>(mu, rho, n, prior_mu, prior_sigma, prior->w_mu,
+                                                                      prior->w_sigma, mk.w, kl_convention,
+                                                                      grad_kl, g_mu, g_rho);
+    else if (prior)
         bbb::kl_backward_prior_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)cuda_stream>>>(
             mu, rho, n, prior->w_mu, prior->w_sigma, kl_convention, grad_kl, g_mu, g_rho);
     else

@@ -27,6 +27,7 @@ struct BwdArgs {
     int sample, has_bias, variant;
     int m_chunk;        // rows of M per wgrad split
     int first_image;    // as in the forward (FwdArgs): LRT noise of image b is drawn at image first_image + b
+    PriorPtrs prior;    // only the mask (w_mask, b_mask) is read, by the MK = true instantiations
 };
 
 __device__ __forceinline__ float sigmoidf_(float r) { return 1.0f / (1.0f + expf(-r)); }
@@ -39,7 +40,8 @@ __device__ __forceinline__ float lrt_gv(const BwdArgs& p, const NoiseKey& k, flo
 
 // --------------------------------------------------------------------- wgrad
 // grid = (k tiles, n tiles, M splits); 256 threads; tile 64(n) x 64(k), reduction chunk 16 rows of M.
-template <int VARIANT>
+// MK: nothing is added to the gradients of a pruned element (p.prior.w_mask / b_mask), which stay exactly zero.
+template <int VARIANT, bool MK = false>
 __global__ void __launch_bounds__(256)
 wgrad_simt_kernel(const BwdArgs p) {
     constexpr bool LRT = VARIANT == BBB_VARIANT_LRT;
@@ -129,6 +131,7 @@ wgrad_simt_kernel(const BwdArgs p) {
             const int k = k0 + tx * 4 + j;
             if (k >= g.K) continue;
             const size_t wi = (size_t)n * g.K + k;
+            if (!kept(w_keep<MK>(p.prior, wi))) continue;
             atomicAdd(p.g_w_mu + wi, acc[i][j]);
             if (stoch) {
                 const float rho = __ldg(p.w_rho + wi);
@@ -142,7 +145,7 @@ wgrad_simt_kernel(const BwdArgs p) {
             }
         }
     }
-    if (p.has_bias && blockIdx.x == 0 && t < 64 && n0 + t < g.N) {
+    if (p.has_bias && blockIdx.x == 0 && t < 64 && n0 + t < g.N && kept(b_keep<MK>(p.prior, n0 + t))) {
         const int n = n0 + t;
         atomicAdd(p.g_b_mu + n, bsum);
         if (stoch) {
@@ -160,7 +163,8 @@ wgrad_simt_kernel(const BwdArgs p) {
 // --------------------------------------------------------------------- dgrad
 // Implicit GEMM: rows m' = (b, ih, iw) input pixels, columns c = input channels,
 // reduction k' = (n, r, s).  grid = (m' tiles, c tiles); 256 threads; 64 x 64 x 16 tiles.
-template <int VARIANT>
+// MK: a pruned weight is a zero operand (p.prior.w_mask).
+template <int VARIANT, bool MK = false>
 __global__ void __launch_bounds__(256)
 dgrad_simt_kernel(const BwdArgs p) {
     constexpr bool LRT = VARIANT == BBB_VARIANT_LRT;
@@ -210,7 +214,7 @@ dgrad_simt_kernel(const BwdArgs p) {
                     }
                 }
                 const int c = c0 + lc;
-                if (c < g.Cin) {
+                if (c < g.Cin && kept(w_keep<MK>(p.prior, ((size_t)n * g.Cin + c) * g.KHW + rs))) {
                     const size_t wi = ((size_t)n * g.Cin + c) * g.KHW + rs;
                     const float mu = __ldg(p.w_mu + wi);
                     if (LRT) {
@@ -273,16 +277,26 @@ inline cudaError_t launch_bwd_simt(BwdArgs a, cudaStream_t st, int n_sm, int* n_
         a.m_chunk = ((g.M + splits - 1) / splits + 15) / 16 * 16;
         splits = (g.M + a.m_chunk - 1) / a.m_chunk;
         dim3 grid(kt, nt, splits);
-        if (lrt) wgrad_simt_kernel<BBB_VARIANT_LRT><<<grid, 256, 0, st>>>(a);
-        else     wgrad_simt_kernel<BBB_VARIANT_BBB><<<grid, 256, 0, st>>>(a);
+        if (a.prior.w_mask) {
+            if (lrt) wgrad_simt_kernel<BBB_VARIANT_LRT, true><<<grid, 256, 0, st>>>(a);
+            else     wgrad_simt_kernel<BBB_VARIANT_BBB, true><<<grid, 256, 0, st>>>(a);
+        } else {
+            if (lrt) wgrad_simt_kernel<BBB_VARIANT_LRT><<<grid, 256, 0, st>>>(a);
+            else     wgrad_simt_kernel<BBB_VARIANT_BBB><<<grid, 256, 0, st>>>(a);
+        }
         cudaError_t e = cudaGetLastError();
         if (e != cudaSuccess) return e;
         *n_launch += 1;
     }
     if (a.gx) {
         dim3 grid((g.B * g.HW + 63) / 64, (g.Cin + 63) / 64);
-        if (lrt) dgrad_simt_kernel<BBB_VARIANT_LRT><<<grid, 256, 0, st>>>(a);
-        else     dgrad_simt_kernel<BBB_VARIANT_BBB><<<grid, 256, 0, st>>>(a);
+        if (a.prior.w_mask) {
+            if (lrt) dgrad_simt_kernel<BBB_VARIANT_LRT, true><<<grid, 256, 0, st>>>(a);
+            else     dgrad_simt_kernel<BBB_VARIANT_BBB, true><<<grid, 256, 0, st>>>(a);
+        } else {
+            if (lrt) dgrad_simt_kernel<BBB_VARIANT_LRT><<<grid, 256, 0, st>>>(a);
+            else     dgrad_simt_kernel<BBB_VARIANT_BBB><<<grid, 256, 0, st>>>(a);
+        }
         cudaError_t e = cudaGetLastError();
         if (e != cudaSuccess) return e;
         *n_launch += 1;

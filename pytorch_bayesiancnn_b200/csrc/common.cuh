@@ -3,6 +3,7 @@
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
 #include <stdint.h>
+#include <type_traits>
 #include "../../include/bbb_b200.h"
 
 namespace bbb {
@@ -125,7 +126,39 @@ struct LayerArgs {
 // bias_mu.  The weight-prep kernels take it as a parameter of its own behind their argument struct, so the structs (and
 // the parameter offsets of the GEMM kernels that share them) stay as they were; only the tensor-prior instantiations
 // (template flag TP) read it, and only where they compute a KL.
-struct PriorPtrs { const float* w_mu; const float* w_sigma; const float* b_mu; const float* b_sigma; };
+// w_mask / b_mask: the layer's pruning mask (bbb_masked_prior: one byte per element of W_mu / bias_mu, 0 = pruned;
+// b_mask NULL: every bias kept), read by the masked instantiations (template flag MK) only, wherever mu / rho are read.
+struct PriorPtrs {
+    const float* w_mu; const float* w_sigma; const float* b_mu; const float* b_sigma;
+    const uint8_t* w_mask; const uint8_t* b_mask;
+};
+
+// Is element i of a masked tensor kept?  A compile-time source like the prior's: KeepAll (no mask: always, no load) or
+// element i of a mask (NULL: every element kept).  A pruned element is a deterministic zero in every operand and adds
+// nothing to the KL: the mask selects, so its mu / rho never reach an output, whatever they hold.
+struct KeepAll {};
+struct KeepAt { const uint8_t* m; size_t i; };
+__device__ __forceinline__ constexpr bool kept(const KeepAll&) { return true; }
+__device__ __forceinline__ bool kept(const KeepAt& k) { return !k.m || __ldg(k.m + k.i) != 0; }
+template <bool MK>
+__device__ __forceinline__ auto w_keep(const PriorPtrs& q, size_t i) {
+    if constexpr (MK) return KeepAt{q.w_mask, i};
+    else return KeepAll{};
+}
+template <bool MK>
+__device__ __forceinline__ auto b_keep(const PriorPtrs& q, size_t n) {
+    if constexpr (MK) return KeepAt{q.b_mask, n};
+    else return KeepAll{};
+}
+// The instantiation a call of the kernels above takes: f(TP, MK) with TP = a tensor prior (q.w_mu), MK = a mask
+// (q.w_mask), each a std::bool_constant
+template <class F>
+inline auto prior_dispatch(const PriorPtrs& q, F&& f) {
+    using Y = std::true_type;
+    using N = std::false_type;
+    if (q.w_mask) return q.w_mu ? f(Y{}, Y{}) : f(N{}, Y{});
+    return q.w_mu ? f(Y{}, N{}) : f(N{}, N{});
+}
 
 // The prior of one KL term, as a compile-time source: the scalar pair of the argument struct (desc->prior_mu /
 // prior_sigma) or element i of the tensors.  prior_of() is called only where the term is computed, so either is read

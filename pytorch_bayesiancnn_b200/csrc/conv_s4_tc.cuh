@@ -59,8 +59,8 @@ inline size_t conv_s4_workspace_bytes(const Geom& g) { return conv_s4_bias_offse
 // ------------------------------------------------------------------ (P) prep
 // item = (kernel row r, 8-wide K chunk, output channel): K' = chunk*8 + e -> window pixel j = K'/4 (s = j - 1), channel K'%4
 // FOLD: BBB fold, one operand set per weight sample (a separate instantiation keeps the other preps as they were)
-// TP: the KL is taken against the tensor prior q (bbb_prior), in the same order.
-template <int VARIANT, bool FOLD = false, bool TP = false>
+// TP: the KL is taken against the tensor prior q (bbb_prior), in the same order.  MK: q.w_mask / q.b_mask prune.
+template <int VARIANT, bool FOLD = false, bool TP = false, bool MK = false>
 __global__ void __launch_bounds__(256)
 conv_s4_prep_kernel(const S4Args p, const PriorPtrs q) {
     constexpr bool LRT = VARIANT == BBB_VARIANT_LRT;
@@ -88,8 +88,9 @@ conv_s4_prep_kernel(const S4Args p, const PriorPtrs q) {
             if (w_ok(e)) {
                 const size_t wi = w_index(e);
                 const float mu = __ldg(p.w_mu + wi);
-                const PrepElem o = prep_elem<LRT>(p, mu, RhoAt{p.w_rho, wi}, w_prior_now<TP>(p, q, wi), p.eps_a, wi, wi, nkey, kl_acc);
-                w[e] = o.w; s2[e] = o.s2; mu8[e] = mu; sg8[e] = o.sigma;
+                const PrepElem o = prep_elem<LRT>(p, mu, RhoAt{p.w_rho, wi}, w_prior_now<TP>(p, q, wi), w_keep<MK>(q, wi),
+                                                  p.eps_a, wi, wi, nkey, kl_acc);
+                w[e] = o.w; s2[e] = o.s2; mu8[e] = o.mu; sg8[e] = o.sigma;
             }
         }
         const size_t off = (size_t)r * p.planes * (S4_BPLANE / 2) + chunk * 512 + row * 8;   // canonical K-major, no swizzle
@@ -103,7 +104,7 @@ conv_s4_prep_kernel(const S4Args p, const PriorPtrs q) {
             *reinterpret_cast<uint4*>(fold_set(p.wtiles, p.fold, j) + off) = pack_chunk<false>(w);
         }
     }
-    prep_bias<LRT, FOLD, TP>(p, q, nkey, 64, kl_acc);
+    prep_bias<LRT, FOLD, TP, MK>(p, q, nkey, 64, kl_acc);
     prep_finish(p, kl_acc);
 }
 
@@ -386,7 +387,7 @@ conv_s4_kernel(const S4Args p) {
     tl_exit(p.tl_gemm, 256);
 }
 
-// q: the tensor prior of the weight-prep kernel (all NULL: the scalar prior of `a`)
+// q: the tensor prior and mask of the weight-prep kernel (all NULL: the scalar prior of `a`, no mask)
 inline cudaError_t launch_conv_s4(S4Args a, cudaStream_t st, bool do_prep, bool do_gemm, int* n_launch, const PriorPtrs& q = PriorPtrs{}) {
     const Geom& g = a.g;
     *n_launch = 0;
@@ -397,20 +398,15 @@ inline cudaError_t launch_conv_s4(S4Args a, cudaStream_t st, bool do_prep, bool 
     const bool lrt = a.variant == BBB_VARIANT_LRT;
     if (do_prep) {
         const int grid = (g.KH * 6 * 64 + 255) / 256;
-        cudaError_t e;
-        if (q.w_mu) {                // tensor prior (set only when the call computes a KL): same grid and work split
-            prep_carveout<conv_s4_prep_kernel<BBB_VARIANT_LRT, false, true>, conv_s4_prep_kernel<BBB_VARIANT_BBB, false, true>,
-                          conv_s4_prep_kernel<BBB_VARIANT_BBB, true, true>>();
-            e = lrt ? launch_pdl(conv_s4_prep_kernel<BBB_VARIANT_LRT, false, true>, dim3(grid), dim3(256), 0, st, a, q)
-                : a.fold.sets > 1 ? launch_pdl(conv_s4_prep_kernel<BBB_VARIANT_BBB, true, true>, dim3(grid), dim3(256), 0, st, a, q)
-                                  : launch_pdl(conv_s4_prep_kernel<BBB_VARIANT_BBB, false, true>, dim3(grid), dim3(256), 0, st, a, q);
-        } else {
-            prep_carveout<conv_s4_prep_kernel<BBB_VARIANT_LRT>, conv_s4_prep_kernel<BBB_VARIANT_BBB>,
-                          conv_s4_prep_kernel<BBB_VARIANT_BBB, true>>();
-            e = lrt ? launch_pdl(conv_s4_prep_kernel<BBB_VARIANT_LRT>, dim3(grid), dim3(256), 0, st, a, q)
-                : a.fold.sets > 1 ? launch_pdl(conv_s4_prep_kernel<BBB_VARIANT_BBB, true>, dim3(grid), dim3(256), 0, st, a, q)
-                                  : launch_pdl(conv_s4_prep_kernel<BBB_VARIANT_BBB>, dim3(grid), dim3(256), 0, st, a, q);
-        }
+        // a tensor prior (set only when the call computes a KL) or a mask: same grid and work split
+        cudaError_t e = prior_dispatch(q, [&](auto tp, auto mk) {
+            constexpr bool TP = decltype(tp)::value, MK = decltype(mk)::value;
+            prep_carveout<conv_s4_prep_kernel<BBB_VARIANT_LRT, false, TP, MK>, conv_s4_prep_kernel<BBB_VARIANT_BBB, false, TP, MK>,
+                          conv_s4_prep_kernel<BBB_VARIANT_BBB, true, TP, MK>>();
+            return lrt ? launch_pdl(conv_s4_prep_kernel<BBB_VARIANT_LRT, false, TP, MK>, dim3(grid), dim3(256), 0, st, a, q)
+                : a.fold.sets > 1 ? launch_pdl(conv_s4_prep_kernel<BBB_VARIANT_BBB, true, TP, MK>, dim3(grid), dim3(256), 0, st, a, q)
+                                  : launch_pdl(conv_s4_prep_kernel<BBB_VARIANT_BBB, false, TP, MK>, dim3(grid), dim3(256), 0, st, a, q);
+        });
         if (e == cudaSuccess) e = cudaGetLastError();
         if (e != cudaSuccess) return e;
         *n_launch += 1;

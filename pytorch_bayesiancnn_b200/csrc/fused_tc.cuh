@@ -51,7 +51,7 @@ inline size_t fused_workspace_bytes(const Geom& g) { return fused_bias_offset(g)
 // ------------------------------------------------------------- (P) tap prep
 // Tail of both tap preps, per operand set: one all-zero sub-tile behind the real ones (staged for pool-window pixels
 // whose tap is outside the kernel), then the bias rows and the KL publish.
-template <bool LRT, bool FOLD, bool TP>
+template <bool LRT, bool FOLD, bool TP, bool MK>
 __device__ __forceinline__ void tap_prep_tail(const FusedArgs& p, const PriorPtrs& q, const NoiseKey& nkey, double kl_acc) {
     const int sets = FOLD ? p.fold.sets : 1;
     const size_t sub = fused_wtile_elems(p);
@@ -60,7 +60,7 @@ __device__ __forceinline__ void tap_prep_tail(const FusedArgs& p, const PriorPtr
         for (long gi = (long)blockIdx.x * blockDim.x + threadIdx.x; gi < (long)(sub / 8); gi += (long)gridDim.x * blockDim.x)
             zero[gi] = make_uint4(0u, 0u, 0u, 0u);
     }
-    prep_bias<LRT, FOLD, TP>(p, q, nkey, p.n_cblk * p.ng, kl_acc);
+    prep_bias<LRT, FOLD, TP, MK>(p, q, nkey, p.n_cblk * p.ng, kl_acc);
     prep_finish(p, kl_acc);
 }
 
@@ -68,8 +68,9 @@ __device__ __forceinline__ void tap_prep_tail(const FusedArgs& p, const PriorPtr
 // Resident CTAs per SM: left to itself ptxas gives the LRT instantiation 54 registers (4 CTAs); the bound keeps it at 48
 // (5 CTAs).  The other two are given the occupancy they reach anyway (40 and 64 registers): any explicit bound changes
 // ptxas's register target for every instantiation of the template.
-// TP: the KL is taken against the tensor prior q (bbb_prior), in the same order (both tap preps).
-template <int VARIANT, bool FOLD = false, bool TP = false>
+// TP: the KL is taken against the tensor prior q (bbb_prior), in the same order (both tap preps).  MK: q.w_mask /
+// q.b_mask prune (both tap preps).
+template <int VARIANT, bool FOLD = false, bool TP = false, bool MK = false>
 __global__ void __launch_bounds__(256, VARIANT == BBB_VARIANT_LRT ? 5 : FOLD ? 4 : 6)
 tap_prep_kernel(const FusedArgs p, const PriorPtrs q) {
     constexpr bool LRT = VARIANT == BBB_VARIANT_LRT;
@@ -103,8 +104,9 @@ tap_prep_kernel(const FusedArgs p, const PriorPtrs q) {
             if (w_ok(e)) {
                 const size_t wi = w_index(e);
                 const float mu = __ldg(p.w_mu + wi);
-                const PrepElem o = prep_elem<LRT>(p, mu, RhoAt{p.w_rho, wi}, w_prior_now<TP>(p, q, wi), p.eps_a, wi, wi, nkey, kl_acc);
-                w[e] = o.w; s2[e] = o.s2; mu8[e] = mu; sg8[e] = o.sigma;
+                const PrepElem o = prep_elem<LRT>(p, mu, RhoAt{p.w_rho, wi}, w_prior_now<TP>(p, q, wi), w_keep<MK>(q, wi),
+                                                  p.eps_a, wi, wi, nkey, kl_acc);
+                w[e] = o.w; s2[e] = o.s2; mu8[e] = o.mu; sg8[e] = o.sigma;
             }
         }
         // K-major SWIZZLE_128B image: row r = 128 contiguous bytes, its 16-byte chunk c stored at chunk (c ^ (r & 7))
@@ -118,7 +120,7 @@ tap_prep_kernel(const FusedArgs p, const PriorPtrs q) {
             *reinterpret_cast<uint4*>(fold_set(dst, p.fold, j) + sw) = pack_chunk<false>(w);
         }
     }
-    tap_prep_tail<LRT, FOLD, TP>(p, q, nkey, kl_acc);
+    tap_prep_tail<LRT, FOLD, TP, MK>(p, q, nkey, kl_acc);
 }
 
 // ------------------------------------------------- (P2) tap prep, conv layers
@@ -136,7 +138,7 @@ tap_prep_kernel(const FusedArgs p, const PriorPtrs q) {
 constexpr int PREP2_BATCH = 4;                                     // loads in flight per thread
 __host__ __device__ inline int prep2_slab(int R) { return R * 64 + 8; }   // bf16 per (plane, tap) slab; +8 keeps 16 B alignment, skews banks
 
-template <int VARIANT, bool FOLD = false, bool TP = false>
+template <int VARIANT, bool FOLD = false, bool TP = false, bool MK = false>
 __global__ void __launch_bounds__(256)
 tap_prep_conv_kernel(const FusedArgs p, const int R, const PriorPtrs q) {
     extern __shared__ __align__(16) uint8_t prep2_smem[];
@@ -191,8 +193,9 @@ tap_prep_conv_kernel(const FusedArgs p, const int R, const PriorPtrs q) {
                 if (so[u] < 0) continue;
                 PrepElem o = {0.0f, 0.0f, 0.0f};
                 if (ok[u]) {
-                    o = prep_elem<LRT, !fold>(p, mu[u], rho[u], prior_u(u), p.eps_a, wi[u], wi[u], nkey, kl_acc);
-                    if (fold) smf[so[u]] = make_float2(mu[u], o.sigma);   // every sample's weight is drawn in phase 2
+                    o = prep_elem<LRT, !fold>(p, mu[u], rho[u], prior_u(u), w_keep<MK>(q, wi[u]), p.eps_a, wi[u], wi[u],
+                                              nkey, kl_acc);
+                    if (fold) smf[so[u]] = make_float2(o.mu, o.sigma);   // every sample's weight is drawn in phase 2
                 }
                 if (fold) continue;
                 sm[so[u]] = __float2bfloat16_rn(o.w);
@@ -236,7 +239,7 @@ tap_prep_conv_kernel(const FusedArgs p, const int R, const PriorPtrs q) {
         }
         __syncthreads();
     }
-    tap_prep_tail<LRT, FOLD, TP>(p, q, nkey, kl_acc);
+    tap_prep_tail<LRT, FOLD, TP, MK>(p, q, nkey, kl_acc);
 }
 
 // ------------------------------------------------------------ wgmma helpers
@@ -614,8 +617,9 @@ inline bool fused_supported(const Geom& g, int pool) {
     return true;
 }
 
-// The weight-prep launch of launch_fused (a.planes, ng, n_cblk, n_kblk and taps set); TP: the tensor-prior instantiations.
-template <bool TP>
+// The weight-prep launch of launch_fused (a.planes, ng, n_cblk, n_kblk and taps set); TP: the tensor-prior
+// instantiations, MK: the masked ones.
+template <bool TP, bool MK>
 inline cudaError_t launch_tap_prep(const FusedArgs& a, const PriorPtrs& q, cudaStream_t st, int n_sm) {
     const Geom& g = a.g;
     const bool lrt = a.variant == BBB_VARIANT_LRT;
@@ -624,7 +628,7 @@ inline cudaError_t launch_tap_prep(const FusedArgs& a, const PriorPtrs& q, cudaS
     int grid = (int)((items + 255) / 256);
     if (grid > 2048) grid = 2048;
     if (grid < 1) grid = 1;
-    prep_carveout<tap_prep_kernel<BBB_VARIANT_LRT, false, TP>, tap_prep_kernel<BBB_VARIANT_BBB, false, TP>, tap_prep_kernel<BBB_VARIANT_BBB, true, TP>>();
+    prep_carveout<tap_prep_kernel<BBB_VARIANT_LRT, false, TP, MK>, tap_prep_kernel<BBB_VARIANT_BBB, false, TP, MK>, tap_prep_kernel<BBB_VARIANT_BBB, true, TP, MK>>();
     // conv layers: the coalesced variant (rows x 64-channel block per CTA); R = rows per CTA, shrunk until the
     // grid covers the SMs and the staging tile fits 48 KB
     static const bool prep2_on = [] { const char* e = getenv("BBB_B200_PREP2"); return !(e && e[0] == '0'); }();
@@ -638,28 +642,28 @@ inline cudaError_t launch_tap_prep(const FusedArgs& a, const PriorPtrs& q, cudaS
     while (R > 2 && ((long)(npad / R) * a.n_kblk < n_sm || need(R) > kPrepSmem)) R >>= 1;
     const bool prep2 = prep2_on && g.KHW > 1 && a.prev_hw == 1 && g.Cin % 64 == 0 && a.taps == g.KHW && need(R) <= 48 * 1024;
     if (prep2) {
-        prep_carveout<tap_prep_conv_kernel<BBB_VARIANT_LRT, false, TP>, tap_prep_conv_kernel<BBB_VARIANT_BBB, false, TP>,
-                      tap_prep_conv_kernel<BBB_VARIANT_BBB, true, TP>>();
+        prep_carveout<tap_prep_conv_kernel<BBB_VARIANT_LRT, false, TP, MK>, tap_prep_conv_kernel<BBB_VARIANT_BBB, false, TP, MK>,
+                      tap_prep_conv_kernel<BBB_VARIANT_BBB, true, TP, MK>>();
         int grid2 = (npad / R) * a.n_kblk;
         if (grid2 > 2048) grid2 = 2048;
         // a BBB fold stages fp32 (mu, sigma) pairs: 4x the bf16 slab, same R and grid as the unfolded call
         if (fold) {
             const size_t smem2 = (size_t)g.KHW * prep2_slab(R) * 8;
-            const cudaError_t e2 = cudaFuncSetAttribute(tap_prep_conv_kernel<BBB_VARIANT_BBB, true, TP>,
+            const cudaError_t e2 = cudaFuncSetAttribute(tap_prep_conv_kernel<BBB_VARIANT_BBB, true, TP, MK>,
                                                         cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem2);
             if (e2 != cudaSuccess) return e2;
-            tap_prep_conv_kernel<BBB_VARIANT_BBB, true, TP><<<grid2, 256, smem2, st>>>(a, R, q);
+            tap_prep_conv_kernel<BBB_VARIANT_BBB, true, TP, MK><<<grid2, 256, smem2, st>>>(a, R, q);
         }
-        else if (lrt) tap_prep_conv_kernel<BBB_VARIANT_LRT, false, TP><<<grid2, 256, need(R), st>>>(a, R, q);
-        else          tap_prep_conv_kernel<BBB_VARIANT_BBB, false, TP><<<grid2, 256, need(R), st>>>(a, R, q);
+        else if (lrt) tap_prep_conv_kernel<BBB_VARIANT_LRT, false, TP, MK><<<grid2, 256, need(R), st>>>(a, R, q);
+        else          tap_prep_conv_kernel<BBB_VARIANT_BBB, false, TP, MK><<<grid2, 256, need(R), st>>>(a, R, q);
     }
-    else if (fold) tap_prep_kernel<BBB_VARIANT_BBB, true, TP><<<grid, 256, 0, st>>>(a, q);
-    else if (lrt)  tap_prep_kernel<BBB_VARIANT_LRT, false, TP><<<grid, 256, 0, st>>>(a, q);
-    else           tap_prep_kernel<BBB_VARIANT_BBB, false, TP><<<grid, 256, 0, st>>>(a, q);
+    else if (fold) tap_prep_kernel<BBB_VARIANT_BBB, true, TP, MK><<<grid, 256, 0, st>>>(a, q);
+    else if (lrt)  tap_prep_kernel<BBB_VARIANT_LRT, false, TP, MK><<<grid, 256, 0, st>>>(a, q);
+    else           tap_prep_kernel<BBB_VARIANT_BBB, false, TP, MK><<<grid, 256, 0, st>>>(a, q);
     return cudaGetLastError();
 }
 
-// q: the tensor prior of the weight-prep kernel (all NULL: the scalar prior of `a`)
+// q: the tensor prior and mask of the weight-prep kernel (all NULL: the scalar prior of `a`, no mask)
 inline cudaError_t launch_fused(FusedArgs a, const void* x, const void* x_sq, cudaStream_t st, int* n_launch, const char** why,
                                 bool do_prep = true, bool do_gemm = true, int n_sm = 132, bool prefer_wide = false,
                                 const PriorPtrs& q = PriorPtrs{}) {
@@ -687,8 +691,11 @@ inline cudaError_t launch_fused(FusedArgs a, const void* x, const void* x_sq, cu
         return cudaErrorInvalidValue;
     }
     if (do_prep) {
-        // a tensor prior (set only when the call computes a KL) takes the TP instantiations: same kernels' grids and work split
-        const cudaError_t e = q.w_mu ? launch_tap_prep<true>(a, q, st, n_sm) : launch_tap_prep<false>(a, q, st, n_sm);
+        // a tensor prior (set only when the call computes a KL) takes the TP instantiations, a mask the MK ones: same
+        // kernels' grids and work split
+        const cudaError_t e = prior_dispatch(q, [&](auto tp, auto mk) {
+            return launch_tap_prep<decltype(tp)::value, decltype(mk)::value>(a, q, st, n_sm);
+        });
         if (e != cudaSuccess) return e;
         *n_launch += 1;
     }

@@ -24,7 +24,7 @@ struct FwdArgs {
     float prior_mu, prior_sigma;
     int sample, kl_convention, has_bias, act;
     int first_image;    // global index of image 0: LRT noise of image b is drawn at image first_image + b (McFold)
-    PriorPtrs prior;    // tensor prior (TP = true instantiations only)
+    PriorPtrs prior;    // tensor prior (TP = true instantiations only) and mask (MK = true instantiations only)
 };
 
 __device__ __noinline__ float apply_act(float v, int act) {
@@ -34,7 +34,8 @@ __device__ __noinline__ float apply_act(float v, int act) {
 }
 
 // TP: the KL terms are taken against the tensor prior p.prior (bbb_prior) instead of (prior_mu, prior_sigma).
-template <int VARIANT, int BM, int BN, int TM, int TN, bool TP = false>
+// MK: p.prior.w_mask / b_mask prune: a pruned element is a zero operand (mean and variance) and adds no KL term.
+template <int VARIANT, int BM, int BN, int TM, int TN, bool TP = false, bool MK = false>
 __global__ void __launch_bounds__((BM / TM) * (BN / TN))
 fwd_simt_kernel(const FwdArgs p) {
     constexpr int BK = 16, NT = (BM / TM) * (BN / TN), PAD = 4;
@@ -105,7 +106,7 @@ fwd_simt_kernel(const FwdArgs p) {
         for (int i = 0; i < B_PER; ++i) {
             const int n = n0 + b_n + i * B_NSTEP, k = kt * BK + b_k;
             float w = 0.0f, s2 = 0.0f;
-            if (n < g.N && k < g.K) {
+            if (n < g.N && k < g.K && kept(w_keep<MK>(p.prior, (size_t)n * g.K + k))) {
                 const size_t wi = (size_t)n * g.K + k;
                 const float mu = __ldg(p.w_mu + wi);
                 float sigma = 0.0f;
@@ -180,7 +181,7 @@ fwd_simt_kernel(const FwdArgs p) {
     for (int j = 0; j < TN; ++j) {
         const int n = n0 + ty * TN + j;
         float bm = 0.0f, bv = 0.0f;
-        if (p.has_bias && n < g.N) {
+        if (p.has_bias && n < g.N && kept(b_keep<MK>(p.prior, n))) {
             const float mu = __ldg(p.b_mu + n);
             if (stoch) {
                 const float sigma = softplus_sigma(__ldg(p.b_rho + n));
@@ -197,7 +198,7 @@ fwd_simt_kernel(const FwdArgs p) {
         if (LRT) bias_v[j] = bv;
     }
     if (do_kl) {
-        if (p.has_bias && t < BN && n0 + t < g.N) {
+        if (p.has_bias && t < BN && n0 + t < g.N && kept(b_keep<MK>(p.prior, n0 + t))) {
             const float mu = __ldg(p.b_mu + n0 + t), sigma = softplus_sigma(__ldg(p.b_rho + n0 + t));
             const float2 q = prior_of(b_prior<TP>(p, p.prior, (size_t)(n0 + t)));
             kl_acc += (double)kl_term(mu, sigma, q.x, q.y, p.kl_convention);
@@ -232,27 +233,30 @@ fwd_simt_kernel(const FwdArgs p) {
     }
 }
 
-template <int VARIANT, int BM, int BN, int TM, int TN, bool TP>
+template <int VARIANT, int BM, int BN, int TM, int TN, bool TP, bool MK>
 inline cudaError_t launch_fwd_simt_cfg(const FwdArgs& a, cudaStream_t st) {
     dim3 grid((a.g.M + BM - 1) / BM, (a.g.N + BN - 1) / BN);
-    fwd_simt_kernel<VARIANT, BM, BN, TM, TN, TP><<<grid, (BM / TM) * (BN / TN), 0, st>>>(a);
+    fwd_simt_kernel<VARIANT, BM, BN, TM, TN, TP, MK><<<grid, (BM / TM) * (BN / TN), 0, st>>>(a);
     return cudaGetLastError();
 }
 
 inline int simt_n_tile(int N) { return N <= 16 ? 16 : (N <= 32 ? 32 : 64); }
 inline int simt_kl_slots(const Geom& g) { const int bn = simt_n_tile(g.N); return (g.N + bn - 1) / bn; }
 
-template <int VARIANT, bool TP>
+template <int VARIANT, bool TP, bool MK>
 inline cudaError_t launch_fwd_simt_tp(const FwdArgs& a, cudaStream_t st) {
     const int bn = simt_n_tile(a.g.N);
-    if (bn == 16) return launch_fwd_simt_cfg<VARIANT, 128, 16, 4, 2, TP>(a, st);
-    if (bn == 32) return launch_fwd_simt_cfg<VARIANT, 128, 32, 4, 4, TP>(a, st);
-    return launch_fwd_simt_cfg<VARIANT, 64, 64, 4, 4, TP>(a, st);
+    if (bn == 16) return launch_fwd_simt_cfg<VARIANT, 128, 16, 4, 2, TP, MK>(a, st);
+    if (bn == 32) return launch_fwd_simt_cfg<VARIANT, 128, 32, 4, 4, TP, MK>(a, st);
+    return launch_fwd_simt_cfg<VARIANT, 64, 64, 4, 4, TP, MK>(a, st);
 }
-// a tensor prior (a.prior.w_mu, set only when the call computes a KL) takes the TP instantiations
+// a tensor prior (a.prior.w_mu, set only when the call computes a KL) takes the TP instantiations, a mask
+// (a.prior.w_mask) the MK ones
 template <int VARIANT>
 inline cudaError_t launch_fwd_simt(const FwdArgs& a, cudaStream_t st) {
-    return a.prior.w_mu ? launch_fwd_simt_tp<VARIANT, true>(a, st) : launch_fwd_simt_tp<VARIANT, false>(a, st);
+    return prior_dispatch(a.prior, [&](auto tp, auto mk) {
+        return launch_fwd_simt_tp<VARIANT, decltype(tp)::value, decltype(mk)::value>(a, st);
+    });
 }
 
 }  // namespace bbb

@@ -302,12 +302,18 @@ __device__ __forceinline__ float rho_of(const RhoAt& r) { return __ldg(r.rho + r
 // else Philox element i), otherwise mu; plane 1 = LRT sigma^2; and its KL term against `prior` (PriorScalar / PriorAt,
 // read only here) added to `kl`.
 // DRAW = false leaves plane 0 at mu: a BBB fold that draws every sample later with fold_draw.
-struct PrepElem { float w, s2, sigma; };
-template <bool LRT, bool DRAW = true, class Rho, class Prior>
+// `keep` (KeepAll / KeepAt): a pruned element is all zeros (w, s2, sigma and the mu the fold draws from) and adds no KL
+// term; nothing of its mu / rho is used, and its Philox element is not drawn (every other element's is unchanged).
+struct PrepElem { float w, s2, sigma, mu; };
+template <bool LRT, bool DRAW = true, class Rho, class Prior, class Keep>
 __device__ __forceinline__ PrepElem prep_elem(const LayerArgs& p, float mu, const Rho& rho, const Prior& prior,
-                                              const float* eps, size_t ei, uint64_t i, const NoiseKey& nkey, double& kl) {
+                                              const Keep& keep, const float* eps, size_t ei, uint64_t i,
+                                              const NoiseKey& nkey, double& kl) {
+    if constexpr (!std::is_same_v<Keep, KeepAll>) {
+        if (!kept(keep)) return PrepElem{0.0f, 0.0f, 0.0f, 0.0f};
+    }
     const bool stoch = p.sample != 0, do_kl = p.kl_out != nullptr;
-    PrepElem o = {mu, 0.0f, 0.0f};
+    PrepElem o = {mu, 0.0f, 0.0f, mu};
     if (stoch || do_kl) o.sigma = softplus_sigma_fast(rho_of(rho));
     if (LRT) o.s2 = o.sigma * o.sigma;
     else if (DRAW && stoch) {
@@ -329,24 +335,25 @@ __device__ __forceinline__ float fold_draw(float mu, float sigma, uint64_t i, co
 // Bias rows of every operand set: bias_ws[n] (BBB: sampled, LRT: mu) and bias_ws[npad + n] (LRT: sigma_b^2) for all npad
 // padded columns, zero past N or without a bias; one thread per column, each bias KL term counted once.  Bias element n
 // is Philox element N*K + n, behind the weights.  TP: the KL terms take the bias part of the tensor prior q.
-template <bool LRT, bool FOLD, bool TP>
+// MK: q.b_mask (if any) prunes bias elements.
+template <bool LRT, bool FOLD, bool TP, bool MK>
 __device__ __forceinline__ void prep_bias(const LayerArgs& p, const PriorPtrs& q, const NoiseKey& nkey, int npad, double& kl) {
     const Geom& g = p.g;
     const uint64_t i0 = (uint64_t)g.N * g.K;
     for (int n = blockIdx.x * blockDim.x + threadIdx.x; n < npad; n += gridDim.x * blockDim.x) {
         const bool real = p.has_bias && n < g.N;
-        float mu = 0.0f;
-        PrepElem o = {0.0f, 0.0f, 0.0f};
+        PrepElem o = {0.0f, 0.0f, 0.0f, 0.0f};
         if (real) {
-            mu = __ldg(p.b_mu + n);
-            o = prep_elem<LRT>(p, mu, RhoAt{p.b_rho, (size_t)n}, b_prior<TP>(p, q, n), p.eps_b, n, i0 + n, nkey, kl);
+            const float mu = __ldg(p.b_mu + n);
+            o = prep_elem<LRT>(p, mu, RhoAt{p.b_rho, (size_t)n}, b_prior<TP>(p, q, n), b_keep<MK>(q, n), p.eps_b, n,
+                               i0 + n, nkey, kl);
         }
         p.bias_ws[n] = o.w;
         p.bias_ws[npad + n] = o.s2;
         if (FOLD) {
             for (int j = 1; j < p.fold.sets; ++j) {
                 float* bj = fold_set(p.bias_ws, p.fold, j);
-                bj[n] = real ? fold_draw(mu, o.sigma, i0 + n, sample_key(nkey, p.fold, j)) : 0.0f;
+                bj[n] = real ? fold_draw(o.mu, o.sigma, i0 + n, sample_key(nkey, p.fold, j)) : 0.0f;
                 bj[npad + n] = 0.0f;
             }
         }
@@ -383,8 +390,8 @@ inline void prep_carveout() {
 // K chunk); consecutive threads take consecutive rows so the 16-byte writes are contiguous.
 // FOLD: BBB fold, one operand set per weight sample, all drawn from the same (mu, sigma) in the same work split as an
 // unfolded call, so the KL sums in the same order (a separate instantiation keeps the unfolded prep as it was).
-// TP: the KL is taken against the tensor prior q (bbb_prior), in the same order.
-template <int VARIANT, bool TF32, bool FOLD = false, bool TP = false>
+// TP: the KL is taken against the tensor prior q (bbb_prior), in the same order.  MK: q.w_mask / q.b_mask prune.
+template <int VARIANT, bool TF32, bool FOLD = false, bool TP = false, bool MK = false>
 __global__ void __launch_bounds__(256)
 weight_prep_kernel(const TcArgs p, const PriorPtrs q) {
     constexpr bool LRT = VARIANT == BBB_VARIANT_LRT;
@@ -411,8 +418,9 @@ weight_prep_kernel(const TcArgs p, const PriorPtrs q) {
             if (n < g.N && k < g.K) {
                 const size_t wi = (size_t)n * g.K + k;
                 const float mu = __ldg(p.w_mu + wi);
-                const PrepElem o = prep_elem<LRT>(p, mu, RhoAt{p.w_rho, wi}, w_prior_now<TP>(p, q, wi), p.eps_a, wi, wi, nkey, kl_acc);
-                w[e] = o.w; s2[e] = o.s2; mu8[e] = mu; sg8[e] = o.sigma;
+                const PrepElem o = prep_elem<LRT>(p, mu, RhoAt{p.w_rho, wi}, w_prior_now<TP>(p, q, wi), w_keep<MK>(q, wi),
+                                                  p.eps_a, wi, wi, nkey, kl_acc);
+                w[e] = o.w; s2[e] = o.s2; mu8[e] = o.mu; sg8[e] = o.sigma;
             }
         }
         // canonical K-major core-matrix order inside the 8 KB tile: chunk*1024 + row*16 bytes
@@ -430,7 +438,7 @@ weight_prep_kernel(const TcArgs p, const PriorPtrs q) {
             }
         }
     }
-    prep_bias<LRT, FOLD, TP>(p, q, nkey, p.n_tiles * TC_BN, kl_acc);
+    prep_bias<LRT, FOLD, TP, MK>(p, q, nkey, p.n_tiles * TC_BN, kl_acc);
     prep_finish(p, kl_acc);
 }
 
@@ -747,16 +755,16 @@ inline cudaError_t launch_fwd_tc_t(TcArgs a, cudaStream_t st, int* n_launch, con
         if (grid > 2048) grid = 2048;
         // A BBB fold (one operand set per weight sample) keeps the grid, so its KL sums in the unfolded call's order.
         // (For LRT both names below are the unfolded prep: only BBB has a fold instantiation.)
-        // A tensor prior (set only when the call computes a KL) takes the TP instantiations: same grid, same work split.
+        // A tensor prior (set only when the call computes a KL) takes the TP instantiations, a mask the MK ones: same grid,
+        // same work split.
         constexpr bool BBB = VARIANT == BBB_VARIANT_BBB;
-        auto* prep = BBB && a.fold.sets > 1 ? weight_prep_kernel<VARIANT, TF32, BBB> : weight_prep_kernel<VARIANT, TF32, false>;
-        if (q.w_mu) {
-            prep_carveout<weight_prep_kernel<VARIANT, TF32, false, true>, weight_prep_kernel<VARIANT, TF32, BBB, true>>();
-            prep = BBB && a.fold.sets > 1 ? weight_prep_kernel<VARIANT, TF32, BBB, true> : weight_prep_kernel<VARIANT, TF32, false, true>;
-        } else {
-            prep_carveout<weight_prep_kernel<VARIANT, TF32, false>, weight_prep_kernel<VARIANT, TF32, BBB>>();
-        }
-        prep<<<grid, 256, 0, st>>>(a, q);
+        prior_dispatch(q, [&](auto tp, auto mk) {
+            constexpr bool TP = decltype(tp)::value, MK = decltype(mk)::value;
+            prep_carveout<weight_prep_kernel<VARIANT, TF32, false, TP, MK>, weight_prep_kernel<VARIANT, TF32, BBB, TP, MK>>();
+            auto* prep = BBB && a.fold.sets > 1 ? weight_prep_kernel<VARIANT, TF32, BBB, TP, MK>
+                                                : weight_prep_kernel<VARIANT, TF32, false, TP, MK>;
+            prep<<<grid, 256, 0, st>>>(a, q);
+        });
         cudaError_t e = cudaGetLastError();
         if (e != cudaSuccess) return e;
         *n_launch += 1;
@@ -800,7 +808,7 @@ inline cudaError_t launch_fwd_tc_t(TcArgs a, cudaStream_t st, int* n_launch, con
     return e;
 }
 
-// q: the tensor prior of the weight-prep kernel (all NULL: the scalar prior of `a`)
+// q: the tensor prior and mask of the weight-prep kernel (all NULL: the scalar prior of `a`, no mask)
 inline cudaError_t launch_fwd_tc(TcArgs a, cudaStream_t st, int n_sm, int* n_launch, const PriorPtrs& q = PriorPtrs{}) {
     const Geom& g = a.g;
     const bool tf32 = a.tf32 != 0;

@@ -7,8 +7,8 @@ namespace bbb {
 // kl_loss() without a preceding forward (SURVEY.md D7): sigma recomputed from rho.
 // HBM-bound: reads 8 B per weight once (16 B with a tensor prior), float4-vectorised when aligned.
 // TP: the prior of element i is (q.w_mu[i], q.w_sigma[i]) / (q.b_mu[i], q.b_sigma[i]) (bbb_prior) instead of (pm, ps);
-// same loops, so the same summation order.
-template <bool TP>
+// same loops, so the same summation order.  MK: a pruned element (q.w_mask / q.b_mask) adds +0.0 in its own place.
+template <bool TP, bool MK = false>
 __device__ __forceinline__ void kl_forward_body(const float* __restrict__ w_mu, const float* __restrict__ w_rho, uint64_t n_w,
                                                 const float* __restrict__ b_mu, const float* __restrict__ b_rho, uint64_t n_b,
                                                 float pm, float ps, const PriorPtrs& q, int conv, double* partials,
@@ -25,19 +25,22 @@ __device__ __forceinline__ void kl_forward_body(const float* __restrict__ w_mu, 
         const float4 r = __ldg(reinterpret_cast<const float4*>(w_rho) + i);
         float4 a = make_float4(pm, pm, pm, pm), b = make_float4(ps, ps, ps, ps);
         if (TP) { a = __ldg(reinterpret_cast<const float4*>(q.w_mu) + i); b = __ldg(reinterpret_cast<const float4*>(q.w_sigma) + i); }
-        float s = kl_term(m.x, softplus_sigma(r.x), a.x, b.x, conv);
-        s += kl_term(m.y, softplus_sigma(r.y), a.y, b.y, conv);
-        s += kl_term(m.z, softplus_sigma(r.z), a.z, b.z, conv);
-        s += kl_term(m.w, softplus_sigma(r.w), a.w, b.w, conv);
+        const auto w_in = [&](int j) { return kept(w_keep<MK>(q, 4 * i + j)); };
+        float s = w_in(0) ? kl_term(m.x, softplus_sigma(r.x), a.x, b.x, conv) : 0.0f;
+        s += w_in(1) ? kl_term(m.y, softplus_sigma(r.y), a.y, b.y, conv) : 0.0f;
+        s += w_in(2) ? kl_term(m.z, softplus_sigma(r.z), a.z, b.z, conv) : 0.0f;
+        s += w_in(3) ? kl_term(m.w, softplus_sigma(r.w), a.w, b.w, conv) : 0.0f;
         acc += (double)s;
     }
     for (uint64_t i = (n4 << 2) + tid; i < n_w; i += nth) {
         const float2 pr = TP ? make_float2(__ldg(q.w_mu + i), __ldg(q.w_sigma + i)) : make_float2(pm, ps);
-        acc += (double)kl_term(__ldg(w_mu + i), softplus_sigma(__ldg(w_rho + i)), pr.x, pr.y, conv);
+        acc += kept(w_keep<MK>(q, i)) ? (double)kl_term(__ldg(w_mu + i), softplus_sigma(__ldg(w_rho + i)), pr.x, pr.y, conv)
+                                      : 0.0;
     }
     for (uint64_t i = tid; i < n_b; i += nth) {
         const float2 pr = TP ? make_float2(__ldg(q.b_mu + i), __ldg(q.b_sigma + i)) : make_float2(pm, ps);
-        acc += (double)kl_term(__ldg(b_mu + i), softplus_sigma(__ldg(b_rho + i)), pr.x, pr.y, conv);
+        acc += kept(b_keep<MK>(q, i)) ? (double)kl_term(__ldg(b_mu + i), softplus_sigma(__ldg(b_rho + i)), pr.x, pr.y, conv)
+                                      : 0.0;
     }
     const double tot = block_sum(acc, red);
     if (threadIdx.x == 0) kl_publish(tot, blockIdx.x, gridDim.x, partials, counter, kl_out);
@@ -55,18 +58,29 @@ kl_forward_prior_kernel(const float* __restrict__ w_mu, const float* __restrict_
                         const PriorPtrs q, int conv, double* partials, unsigned int* counter, float* kl_out) {
     kl_forward_body<true>(w_mu, w_rho, n_w, b_mu, b_rho, n_b, 0.0f, 1.0f, q, conv, partials, counter, kl_out);
 }
+// a masked layer (q.w_mask set); TP: against q's tensor prior, else the scalar (pm, ps)
+template <bool TP>
+__global__ void __launch_bounds__(256)
+kl_forward_masked_kernel(const float* __restrict__ w_mu, const float* __restrict__ w_rho, uint64_t n_w,
+                         const float* __restrict__ b_mu, const float* __restrict__ b_rho, uint64_t n_b,
+                         float pm, float ps, const PriorPtrs q, int conv, double* partials, unsigned int* counter,
+                         float* kl_out) {
+    kl_forward_body<TP, true>(w_mu, w_rho, n_w, b_mu, b_rho, n_b, pm, ps, q, conv, partials, counter, kl_out);
+}
 
 // d kl / d mu = (mu - pm) / sigma^2 ; d kl / d sigma = 1/sigma - ps^2/sigma^3 - (mu-pm)^2/sigma^3 ;
 // d sigma / d rho = sigmoid(rho)   (SURVEY.md Appendix A; reference convention).
-// TP: element i's prior is (q_mu[i], q_sigma[i]) instead of (pm, ps).
-template <bool TP>
+// TP: element i's prior is (q_mu[i], q_sigma[i]) instead of (pm, ps).  MK: nothing is added for a pruned element
+// (mask[i] == 0).
+template <bool TP, bool MK = false>
 __device__ __forceinline__ void kl_backward_body(const float* __restrict__ mu, const float* __restrict__ rho, uint64_t n,
                                                  float pm_, float ps_, const float* __restrict__ q_mu,
                                                  const float* __restrict__ q_sigma, int conv,
                                                  const float* __restrict__ grad_kl, float* __restrict__ g_mu,
-                                                 float* __restrict__ g_rho) {
+                                                 float* __restrict__ g_rho, const uint8_t* __restrict__ mask = nullptr) {
     const float go = __ldg(grad_kl);
     for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
+        if (MK && !kept(KeepAt{mask, i})) continue;
         const float pm = TP ? __ldg(q_mu + i) : pm_, ps = TP ? __ldg(q_sigma + i) : ps_;
         const float m = mu[i], r = rho[i];
         const float s = softplus_sigma(r), d = m - pm;
@@ -95,6 +109,14 @@ kl_backward_prior_kernel(const float* __restrict__ mu, const float* __restrict__
                          const float* __restrict__ q_mu, const float* __restrict__ q_sigma, int conv,
                          const float* __restrict__ grad_kl, float* __restrict__ g_mu, float* __restrict__ g_rho) {
     kl_backward_body<true>(mu, rho, n, 0.0f, 1.0f, q_mu, q_sigma, conv, grad_kl, g_mu, g_rho);
+}
+// masked elements (mask non-NULL); TP: against (q_mu, q_sigma), else the scalar (pm, ps)
+template <bool TP>
+__global__ void __launch_bounds__(256)
+kl_backward_masked_kernel(const float* __restrict__ mu, const float* __restrict__ rho, uint64_t n, float pm, float ps,
+                          const float* __restrict__ q_mu, const float* __restrict__ q_sigma, const uint8_t* __restrict__ mask,
+                          int conv, const float* __restrict__ grad_kl, float* __restrict__ g_mu, float* __restrict__ g_rho) {
+    kl_backward_body<TP, true>(mu, rho, n, pm, ps, q_mu, q_sigma, conv, grad_kl, g_mu, g_rho, mask);
 }
 
 __global__ void __launch_bounds__(256)

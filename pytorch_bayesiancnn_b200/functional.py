@@ -256,6 +256,34 @@ def prior_arg(prior, bias: bool = False):
     return C.byref(L.Prior(p(w_mu), p(w_sigma), p(b_mu), p(b_sigma)))
 
 
+def masked_prior_arg(prior, mask, bias: bool = False):
+    """(the ``prior`` argument, the flag for kl_convention) of a *_prior entry point for a layer with the tensor prior
+    ``prior`` (or None) and the pruning mask ``mask`` = (w_mask, b_mask) (or None): without a mask, (prior_arg, 0);
+    with one, a reference to a bbb_masked_prior and PRIOR_MASKED.  ``bias=True`` as in prior_arg, b_mask in w_mask."""
+    w_mask, b_mask = mask if mask is not None else (None, None)
+    if bias:
+        w_mask, b_mask = b_mask, None
+    if w_mask is None:
+        return prior_arg(prior, bias), 0
+    w_mu, w_sigma, b_mu, b_sigma = prior if prior is not None else (None, None, None, None)
+    if bias:
+        w_mu, w_sigma, b_mu, b_sigma = b_mu, b_sigma, None, None
+    for t in (w_mu, w_sigma, b_mu, b_sigma, w_mask, b_mask):
+        if t is not None:
+            _require_cuda(t, "tensor prior / weight mask")
+    p = lambda t: None if t is None else t.data_ptr()
+    return C.byref(L.MaskedPrior(p(w_mu), p(w_sigma), p(b_mu), p(b_sigma), p(w_mask), p(b_mask))), L.PRIOR_MASKED
+
+
+def desc_with(d: L.LayerDesc, flag: int) -> L.LayerDesc:
+    """``d``, or a copy of it with ``flag`` (masked_prior_arg) in its kl_convention."""
+    if not flag:
+        return d
+    c = L.LayerDesc.from_buffer_copy(d)
+    c.kl_convention |= flag
+    return c
+
+
 def _stream(device):
     return C.c_void_p(torch.cuda.current_stream(device).cuda_stream)
 
@@ -580,10 +608,11 @@ class BayesLayerFn(torch.autograd.Function):
             act_std = torch.empty(yshape, dtype=torch.float32, device=dev)
         ws = workspace(dev, d, cfg.get("owner"))
         fn = lib.bbb_linear_forward_prior if conv is None else lib.bbb_conv2d_forward_prior
-        rc = fn(C.byref(d), _ptr(x), _ptr(W_mu_c), _ptr(W_rho_c), _ptr(bias_mu), _ptr(bias_rho),
+        parg, flag = masked_prior_arg(cfg.get("prior"), cfg.get("mask"))
+        rc = fn(C.byref(desc_with(d, flag)), _ptr(x), _ptr(W_mu_c), _ptr(W_rho_c), _ptr(bias_mu), _ptr(bias_rho),
                 _ptr(y), None if no_kl else _ptr(kl), _ptr(act_std), _ptr(eps_a), _ptr(eps_b),
                 C.c_uint64(seed), C.c_uint64(stream_id), _ptr(base), _ptr(ws), C.c_size_t(ws.numel()), _stream(dev),
-                prior_arg(cfg.get("prior")))
+                parg)
         L.check(rc, "bbb_linear_forward" if conv is None else "bbb_conv2d_forward")
         if y.dtype != y_dtype:                      # a bf16 input the engine took as fp32
             y = y.to(y_dtype)
@@ -637,18 +666,19 @@ class BayesLayerFn(torch.autograd.Function):
             if ctx.needs_input_grad[0]:
                 gx = torch.zeros_like(x)
             ws = workspace(dev)
-            fn = lib.bbb_linear_backward if cfg["conv"] is None else lib.bbb_conv2d_backward
+            fn = lib.bbb_linear_backward_prior if cfg["conv"] is None else lib.bbb_conv2d_backward_prior
             seed, stream_id, base = ctx.noise
-            rc = fn(C.byref(d), _ptr(x), _ptr(gy), _ptr(W_mu), _ptr(W_rho), _ptr(bias_mu), _ptr(bias_rho),
+            parg, flag = masked_prior_arg(None, cfg.get("mask"))
+            rc = fn(C.byref(desc_with(d, flag)), _ptr(x), _ptr(gy), _ptr(W_mu), _ptr(W_rho), _ptr(bias_mu), _ptr(bias_rho),
                     _ptr(act_std), _ptr(eps_a), _ptr(eps_b), C.c_uint64(seed), C.c_uint64(stream_id), _ptr(base),
                     _ptr(gx), _ptr(g_W_mu), _ptr(g_W_rho), _ptr(g_b_mu), _ptr(g_b_rho),
-                    _ptr(ws), C.c_size_t(ws.numel()), _stream(dev))
+                    _ptr(ws), C.c_size_t(ws.numel()), _stream(dev), parg)
             L.check(rc, "bbb_*_backward")
         if gx is not None and gx.dtype != ctx.x_dtype:
             gx = gx.to(ctx.x_dtype)
         if gkl is not None and cfg.get("mixture") is None:
             _kl_backward(gkl, (W_mu, W_rho, bias_mu, bias_rho), (g_W_mu, g_W_rho, g_b_mu, g_b_rho), cfg["prior_mu"],
-                         cfg["prior_sigma"], cfg["kl_convention"], cfg.get("prior"))
+                         cfg["prior_sigma"], cfg["kl_convention"], cfg.get("prior"), cfg.get("mask"))
         return gx, g_W_mu, g_W_rho, g_b_mu, g_b_rho, None
 
 
@@ -659,7 +689,9 @@ class BayesLayerFn(torch.autograd.Function):
         regenerated from the forward's Philox stream; the element-wise chain rule through sigma = softplus(rho) is
         parameter-sized glue.  Returns None when a shape does not fit (the caller then uses the CUDA-core kernels).
         LRT: the noise term's gradient gv = gy * eps / (2 act_std) is one kernel (bbb_lrt_noise_grad) on the forward's
-        desc, folded or not, which reads the stream base on the device."""
+        desc, folded or not, which reads the stream base on the device.
+        A weight mask selects, as in the forward: the dgrad operands are 0 at pruned elements and the parameter
+        gradients are set to exactly 0 there (torch.where, so a pruned element's mu / rho never reach a value)."""
         x, W_mu, W_rho, bias_mu, bias_rho, act_std, eps_a, eps_b = ctx.saved_tensors
         x = x.float()
         cfg = ctx.cfg
@@ -669,8 +701,11 @@ class BayesLayerFn(torch.autograd.Function):
         _tc_math = _tc_operand_math(cfg["math"])           # same operand type as the forward
         seed, stream_id, base = ctx.noise
         need_x = ctx.needs_input_grad[0]
+        w_keep, b_keep = cfg.get("mask") or (None, None)
         sig = torch.log1p(torch.exp(W_rho))
         dsig = torch.sigmoid(W_rho)
+        if w_keep is not None:
+            W_mu, sig = W_mu.where(w_keep, 0.0), sig.where(w_keep, 0.0)
         gb_mu = gb_rho = None
         red = (0,) if conv is None else (0, 2, 3)
         if variant == L.VARIANT_LRT:
@@ -721,6 +756,11 @@ class BayesLayerFn(torch.autograd.Function):
                     gb_rho = gb_mu * eb * torch.sigmoid(bias_rho)
                 else:
                     gb_rho = torch.zeros_like(bias_rho)
+        if w_keep is not None:
+            gw_mu = gw_mu.reshape(W_mu.shape).where(w_keep, 0.0)
+            gw_rho = gw_rho.reshape(W_mu.shape).where(w_keep, 0.0)
+        if b_keep is not None and ctx.has_bias:
+            gb_mu, gb_rho = gb_mu.where(b_keep, 0.0), gb_rho.where(b_keep, 0.0)
         return gx, gw_mu, gw_rho, gb_mu, gb_rho
 
 
@@ -729,7 +769,7 @@ class KLFn(torch.autograd.Function):
     prior_mu / prior_sigma) or the tensor prior (w_mu, w_sigma, b_mu, b_sigma) of the layer (no gradient flows to it)."""
 
     @staticmethod
-    def forward(ctx, W_mu, W_rho, bias_mu, bias_rho, prior_mu, prior_sigma, kl_convention, prior=None):
+    def forward(ctx, W_mu, W_rho, bias_mu, bias_rho, prior_mu, prior_sigma, kl_convention, prior=None, mask=None):
         lib = L.lib()
         _require_cuda(W_mu, "kl_loss")
         dev = W_mu.device
@@ -737,37 +777,39 @@ class KLFn(torch.autograd.Function):
         kl = torch.empty((), dtype=torch.float32, device=dev)
         ws = workspace(dev)
         nb = 0 if bias_mu is None else bias_mu.numel()
+        parg, flag = masked_prior_arg(prior, mask)
         rc = lib.bbb_kl_forward_prior(_ptr(W_mu_c), _ptr(W_rho_c), C.c_uint64(W_mu.numel()), _ptr(bias_mu),
                                       _ptr(bias_rho), C.c_uint64(nb), C.c_float(prior_mu), C.c_float(prior_sigma),
-                                      C.c_int32(kl_convention), _ptr(kl), _ptr(ws), C.c_size_t(ws.numel()), _stream(dev),
-                                      prior_arg(prior))
+                                      C.c_int32(kl_convention | flag), _ptr(kl), _ptr(ws), C.c_size_t(ws.numel()),
+                                      _stream(dev), parg)
         L.check(rc, "bbb_kl_forward_prior")
         ctx.save_for_backward(W_mu_c, W_rho_c, bias_mu, bias_rho)
         ctx.cfg = (float(prior_mu), float(prior_sigma), int(kl_convention))
-        ctx.prior = prior
+        ctx.prior, ctx.mask = prior, mask
         return kl
 
     @staticmethod
     def backward(ctx, gkl):
         params = ctx.saved_tensors
         grads = tuple(None if t is None else torch.zeros_like(t) for t in params)
-        _kl_backward(gkl, params, grads, *ctx.cfg, ctx.prior)
-        return grads + (None, None, None, None)
+        _kl_backward(gkl, params, grads, *ctx.cfg, ctx.prior, ctx.mask)
+        return grads + (None, None, None, None, None)
 
 
-def _kl_backward(gkl, params, grads, prior_mu, prior_sigma, kl_convention, prior):
+def _kl_backward(gkl, params, grads, prior_mu, prior_sigma, kl_convention, prior, mask=None):
     """gkl * d kl / d (mu, rho) added into ``grads``, the weight's then the bias's (bbb_kl_backward_prior; no call for a
     layer without a bias).  params = (W_mu, W_rho, bias_mu, bias_rho) and grads likewise; ``prior``: None or the layer's
-    tensor prior."""
+    tensor prior; ``mask``: None or the layer's (W_mask, bias_mask) (nothing is added at a pruned element)."""
     lib = L.lib()
     gkl = gkl.contiguous().float()
     for k, bias in ((0, False), (2, True)):
         mu, rho = params[k], params[k + 1]
         if mu is None:
             continue
+        parg, flag = masked_prior_arg(prior, mask, bias=bias)
         rc = lib.bbb_kl_backward_prior(_ptr(mu), _ptr(rho), C.c_uint64(mu.numel()), C.c_float(prior_mu),
-                                       C.c_float(prior_sigma), C.c_int32(kl_convention), _ptr(gkl), _ptr(grads[k]),
-                                       _ptr(grads[k + 1]), _stream(mu.device), prior_arg(prior, bias=bias))
+                                       C.c_float(prior_sigma), C.c_int32(kl_convention | flag), _ptr(gkl),
+                                       _ptr(grads[k]), _ptr(grads[k + 1]), _stream(mu.device), parg)
         L.check(rc, "bbb_kl_backward_prior")
 
 

@@ -437,13 +437,14 @@ def run_step(st, nxt, cur, cur_sq, cur_pitch, kl=None, noise=None, phase=0, y_in
     mixture = m.mixture_values()
     if ws is None:
         ws = Fn.workspace(dev, d, m)
+    parg, flag = Fn.masked_prior_arg(m.prior_tensors(), m.mask_tensors())
     rc = lib.bbb_layer_forward_fused_prior(
-        C.byref(d), Fn._ptr(cur), Fn._ptr(cur_sq), st.in_layout, in_pitch, st.prev_hw,
+        C.byref(Fn.desc_with(d, flag)), Fn._ptr(cur), Fn._ptr(cur_sq), st.in_layout, in_pitch, st.prev_hw,
         Fn._ptr(m.W_mu), Fn._ptr(m.W_rho), Fn._ptr(m.bias_mu), Fn._ptr(m.bias_rho),
         Fn._ptr(y), Fn._ptr(y_sq), st.out_layout, pitch, None if mixture is not None else Fn._ptr(kl),
         Fn._ptr(eps_a), Fn._ptr(eps_b),
         C.c_uint64(seed), C.c_uint64(stream_id), Fn._ptr(base), Fn._ptr(ws), C.c_size_t(ws.numel()),
-        Fn._stream(dev), Fn.prior_arg(m.prior_tensors()))
+        Fn._stream(dev), parg)
     L.check(rc, "bbb_layer_forward_fused_prior")
     if phase != L.FUSED_SKIP_PREP and not fill:
         if mixture is not None:             # kl: one entry per folded MC sample, each from its own stream

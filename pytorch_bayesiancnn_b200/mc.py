@@ -375,14 +375,14 @@ class MCForward:
         return fused.PrepCache(steps, fold, self.dev) if fused.PrepCache.eligible(steps) else None
 
     def _prep_version(self):
-        """The version counters of the tensors the prep graph reads: the layers' parameters and prior buffers (the part of
+        """The version counters of the tensors the prep graph reads: the layers' parameters, prior and mask buffers (the part of
         _BayesLayer._versions a replay can see -- the KL settings and the addresses are baked into the graphs, and a
         prior that is set anew is refused by PriorGuard).  About 2 us of host time for BBBAlexNet, where the whole
         _versions() tuple takes ten times that."""
         if self._prep_watch is None:
-            from .modules import _PRIOR_BUFFERS
+            from .modules import _MASK_BUFFERS, _PRIOR_BUFFERS
             self._prep_watch = [t for m in self._prep.layers for t in (m.W_mu, m.W_rho, m.bias_mu, m.bias_rho)
-                                + tuple(m._buffers.get(n) for n in _PRIOR_BUFFERS) if t is not None]
+                                + tuple(m._buffers.get(n) for n in _PRIOR_BUFFERS + _MASK_BUFFERS) if t is not None]
         return [t._version for t in self._prep_watch]
 
     def _fill_prep(self):

@@ -25,6 +25,12 @@ a Monte-Carlo estimate of KL(q || p) from one weight draw per layer call (functi
 call's own, so every Monte-Carlo sample has its own estimate.  ``kl_convention`` does not apply to it.  A layer has one
 prior: the scalar pair, the tensors or the mixture.  The mixture's three values live in the fp32 buffer
 ``mixture_prior``, which exists only after ``set_mixture_prior``.
+
+Pruning (``set_weight_mask`` / ``prune_by_snr``): a bool mask per layer removes weights (and optionally biases) from the
+model.  A pruned element is a deterministic zero in every forward, adds nothing to the KL and gets exactly zero gradient
+on every path of the engine; kept elements compute exactly what they compute without a mask.  The mask lives in the bool
+buffers ``W_mask`` / ``bias_mask``, which exist only after ``set_weight_mask``.  A pruned net is not faster: the kernels
+still multiply the zeros.
 """
 from __future__ import annotations
 
@@ -46,6 +52,7 @@ _DEFAULT_PRIORS = {
 }
 _PRIOR_BUFFERS = ("W_prior_mu", "W_prior_sigma", "bias_prior_mu", "bias_prior_sigma")
 _MIXTURE_BUFFER = "mixture_prior"
+_MASK_BUFFERS = ("W_mask", "bias_mask")
 _prior_epoch = 0          # bumped whenever some layer's prior buffers are created, replaced, moved or removed (PriorGuard)
 
 
@@ -176,7 +183,8 @@ class _BayesLayer(ModuleWrapper):
     def _versions(self):
         """What a cached KL scalar depends on: the parameters' versions AND the KL settings (changing
         kl_convention or the prior -- scalar or tensor (set_prior) -- after a forward must not return the old value)."""
-        ps = (self.W_mu, self.W_rho, self.bias_mu, self.bias_rho) + tuple(self._buffers.get(n) for n in _PRIOR_BUFFERS)
+        ps = (self.W_mu, self.W_rho, self.bias_mu, self.bias_rho) + tuple(
+            self._buffers.get(n) for n in _PRIOR_BUFFERS + _MASK_BUFFERS)
         return tuple((p._version, p.data_ptr()) if p is not None else None for p in ps) + (
             self.kl_convention, float(self.prior_mu), float(self.prior_sigma), self.mixture_values())
 
@@ -227,6 +235,57 @@ class _BayesLayer(ModuleWrapper):
         self._drop_mixture()
         return self
 
+    # -- pruning mask ---------------------------------------------------------
+    def mask_tensors(self):
+        """(W_mask, bias_mask) after set_weight_mask (bias_mask None when every bias is kept), or None: no mask."""
+        if self._buffers.get("W_mask") is None:
+            return None
+        return self._buffers.get("W_mask"), self._buffers.get("bias_mask")
+
+    def set_weight_mask(self, W_mask, bias_mask=None):
+        """Prune the layer: from now on a weight whose W_mask element is False (a bias, with ``bias_mask``; without one
+        every bias is kept) is a deterministic zero in the forward, adds nothing to the KL and gets exactly zero gradient
+        in mu and rho, on every path of the engine.  The kept elements are computed exactly as without a mask (same noise,
+        same bits).  Masks are bool tensors of exactly the shape of W_mu / bias_mu on the parameters' device (ValueError
+        otherwise); they are stored in the buffers ``W_mask`` / ``bias_mask``, follow .to() and are saved in the
+        state_dict.  Setting again with the same shapes copies in place: an engine captured after the first
+        set_weight_mask (MCForward, GraphedForward) reads the new mask on its next replay.  Not with a mixture prior
+        (ValueError): its Monte-Carlo KL takes no mask."""
+        if self.mixture_values() is not None:
+            raise ValueError("set_weight_mask: the layer has a mixture prior, whose Monte-Carlo KL takes no mask")
+        if bias_mask is not None and not self.use_bias:
+            raise ValueError("set_weight_mask: the layer has no bias")
+        parts = [("W_mask", W_mask, self.W_mu)]
+        if bias_mask is not None:
+            parts.append(("bias_mask", bias_mask, self.bias_mu))
+        for name, t, like in parts:
+            if not torch.is_tensor(t) or t.dtype != torch.bool:
+                raise ValueError(f"set_weight_mask: {name} must be a torch.bool tensor, got "
+                                 f"{t.dtype if torch.is_tensor(t) else type(t).__name__}")
+            if t.shape != like.shape:
+                raise ValueError(f"set_weight_mask: {name} of shape {tuple(t.shape)}, expected {tuple(like.shape)}")
+            if t.device != like.device:
+                raise ValueError(f"set_weight_mask: {name} is on device {t.device}, the parameters on {like.device}")
+        for name, t, like in parts:
+            buf = self._buffers.get(name)
+            if buf is not None and buf.shape == like.shape and buf.device == like.device and buf.is_contiguous():
+                with torch.no_grad():
+                    buf.copy_(t)
+            else:
+                self.register_buffer(name, t.detach().clone(memory_format=torch.contiguous_format))
+                _prior_moved()
+        if bias_mask is None and self._buffers.pop("bias_mask", None) is not None:
+            _prior_moved()
+        return self
+
+    def clear_weight_mask(self):
+        """Keep every element again: removes the mask buffers.  A captured engine that read them refuses its next replay
+        (PriorGuard); mc_forward / evaluate build new engines."""
+        removed = [self._buffers.pop(n, None) for n in _MASK_BUFFERS]
+        if any(t is not None for t in removed):
+            _prior_moved()
+        return self
+
     # -- scale-mixture prior --------------------------------------------------
     def mixture_values(self):
         """(pi, sigma1, sigma2) after set_mixture_prior, or None: the prior is a Gaussian (scalar or tensor)."""
@@ -243,6 +302,9 @@ class _BayesLayer(ModuleWrapper):
         captured engine (MCForward, GraphedForward) refuses its next replay once they changed (PriorGuard); mc_forward
         and evaluate build new engines.  Change them through this method, not by writing to the buffer."""
         vals = _check_mixture(pi, sigma1, sigma2)
+        if self.mask_tensors() is not None:
+            raise ValueError("set_mixture_prior: the layer has a weight mask; the mixture prior's Monte-Carlo KL takes "
+                             "no mask (clear_weight_mask first)")
         self.clear_prior()
         self.register_buffer(_MIXTURE_BUFFER, torch.tensor(vals, dtype=torch.float32, device=self.W_mu.device))
         self._mixture = vals
@@ -266,7 +328,7 @@ class _BayesLayer(ModuleWrapper):
     def _apply(self, fn, *args, **kwargs):
         # .to() / .cuda() / .float() replace the buffers: engines captured on the old ones must notice
         out = super()._apply(fn, *args, **kwargs)
-        if self._buffers.get("W_prior_mu") is not None:
+        if self._buffers.get("W_prior_mu") is not None or self._buffers.get("W_mask") is not None:
             _prior_moved()
         return out
 
@@ -280,6 +342,14 @@ class _BayesLayer(ModuleWrapper):
         for n, shape in shapes.items():
             if prefix + n in state_dict and self._buffers.get(n) is None:
                 self.register_buffer(n, torch.zeros(shape, dtype=torch.float32, device=self.W_mu.device))
+                _prior_moved()
+        # likewise a pruning mask (bool, the parameters' shapes)
+        masks = {"W_mask": self.W_mu.shape}
+        if self.use_bias:
+            masks["bias_mask"] = self.bias_mu.shape
+        for n, shape in masks.items():
+            if prefix + n in state_dict and self._buffers.get(n) is None:
+                self.register_buffer(n, torch.ones(shape, dtype=torch.bool, device=self.W_mu.device))
                 _prior_moved()
         # likewise the mixture prior; its values are read back to the host once, here
         has_mix = prefix + _MIXTURE_BUFFER in state_dict
@@ -309,6 +379,7 @@ class _BayesLayer(ModuleWrapper):
             "owner": self,
             "prior": self.prior_tensors(),
             "mixture": self.mixture_values(),
+            "mask": self.mask_tensors(),
         }
 
     def forward(self, x, sample=True):
@@ -335,7 +406,8 @@ class _BayesLayer(ModuleWrapper):
         if self.mixture_values() is not None:
             return Fn.KLMCFn.apply(self.W_mu, self.W_rho, self.bias_mu, self.bias_rho, self.mixture_values(), None, self)
         return Fn.KLFn.apply(self.W_mu, self.W_rho, self.bias_mu, self.bias_rho, float(self.prior_mu),
-                             float(self.prior_sigma), L.KL_BY_NAME[self.kl_convention], self.prior_tensors())
+                             float(self.prior_sigma), L.KL_BY_NAME[self.kl_convention], self.prior_tensors(),
+                             self.mask_tensors())
 
     @property
     def W_sigma(self):
@@ -450,31 +522,40 @@ def prior_signature(net: nn.Module) -> tuple:
     return tuple(one(m) for m in net.modules() if isinstance(m, _BayesLayer))
 
 
+def mask_signature(net: nn.Module) -> tuple:
+    """What a captured graph holds of every Bayesian layer's weight mask: the mask buffers' addresses, or None."""
+    def one(m):
+        ts = m.mask_tensors()
+        return None if ts is None else tuple(None if t is None else t.data_ptr() for t in ts)
+    return tuple(one(m) for m in net.modules() if isinstance(m, _BayesLayer))
+
+
 class PriorGuard:
-    """The layers' priors as a captured CUDA graph of `net` bakes them in: the buffers' addresses, or NULL for a scalar
-    prior.  It holds the buffers, so a replay never reads freed memory, and ``ok()`` tells whether a replay still reads
+    """The layers' priors and weight masks as a captured CUDA graph of `net` bakes them in: the buffers' addresses, or
+    NULL for a scalar prior / no mask.  It holds the buffers, so a replay never reads freed memory, and ``ok()`` tells whether a replay still reads
     what the layers hold: false once a prior was set for the first time, cleared, re-allocated or moved.  An in-place
     set_prior keeps the addresses (the next replay reads the new values).  While no layer anywhere changed its prior's
     identity, ``ok()`` is one integer compare."""
 
     def __init__(self, net: nn.Module):
-        self.net, self.epoch, self.sig = net, _prior_epoch, prior_signature(net)
-        self.keep = [t for m in net.modules() if isinstance(m, _BayesLayer) for t in (m.prior_tensors() or ())
-                     if t is not None]
+        self.net, self.epoch, self.sig = net, _prior_epoch, (prior_signature(net), mask_signature(net))
+        self.keep = [t for m in net.modules() if isinstance(m, _BayesLayer)
+                     for t in (m.prior_tensors() or ()) + (m.mask_tensors() or ()) if t is not None]
 
     def ok(self) -> bool:
         if self.epoch == _prior_epoch:
             return True
-        if prior_signature(self.net) != self.sig:
+        if (prior_signature(self.net), mask_signature(self.net)) != self.sig:
             return False
         self.epoch = _prior_epoch
         return True
 
     def check(self, what: str):
         if not self.ok():
-            raise L.EngineError(f"{what}: a layer's prior was set, cleared, re-allocated or moved since this engine's "
-                                "CUDA graphs were captured; build a new engine (an in-place set_prior of the same shapes "
-                                "is read by the next replay; new set_mixture_prior values are not)")
+            raise L.EngineError(f"{what}: a layer's prior or weight mask was set, cleared, re-allocated or moved since this "
+                                "engine's CUDA graphs were captured; build a new engine (an in-place set_prior or "
+                                "set_weight_mask of the same shapes is read by the next replay; new set_mixture_prior "
+                                "values are not)")
 
 
 def posterior_as_prior(net: nn.Module) -> nn.Module:
@@ -499,3 +580,64 @@ def mixture_prior(net: nn.Module, pi=0.5, sigma1=1.0, sigma2=math.exp(-6)) -> nn
         if isinstance(m, _BayesLayer):
             m.set_mixture_prior(pi, sigma1, sigma2)
     return net
+
+
+def snr(layer: _BayesLayer) -> torch.Tensor:
+    """Signal-to-noise ratio of every weight of a Bayesian layer, |W_mu| / sigma with sigma = log1p(exp(W_rho)) in fp32
+    as the reference computes it (Blundell et al. 2015, section 5.1): the shape of W_mu, on its device."""
+    return _snr(layer.W_mu, layer.W_rho)
+
+
+def _snr(mu, rho):
+    mu, rho = mu.detach().float(), rho.detach().float()
+    return mu.abs() / torch.log1p(torch.exp(rho))
+
+
+def prune_by_snr(net: nn.Module, fraction: float, biases: bool = False) -> dict:
+    """Prune the weights of every Bayesian layer of `net` with the lowest signal-to-noise ratio (snr), as Blundell et al.
+    2015 (section 5.1) do: one ranking over all layers' weights (and biases, with ``biases``), of which exactly
+    floor(fraction * N) are pruned, lowest SNR first, ties broken by (layer order in net.modules(), flat index).
+    Elements a layer's mask already prunes rank first, so ``fraction`` is the share pruned in total, and pruning again
+    never brings an element back (a fraction below the share already pruned leaves the masks as they are).  The masks
+    are set with set_weight_mask (without ``biases`` a layer's bias mask is left as it was).  Runs on the parameters'
+    device with torch ops.  Returns {"pruned", "total", "threshold" (the SNR of the last element pruned by this call;
+    None when it prunes nothing), "per_layer": {name: (pruned, total)}}."""
+    fraction = float(fraction)
+    if not 0.0 <= fraction <= 1.0:
+        raise ValueError(f"prune_by_snr: fraction must be in [0, 1], got {fraction}")
+    layers = [(name, m) for name, m in net.named_modules() if isinstance(m, _BayesLayer)]
+    keys, sizes = [], []
+    for _, m in layers:
+        parts = [(m.W_mu, m.W_rho, 0)] + ([(m.bias_mu, m.bias_rho, 1)] if biases and m.use_bias else [])
+        masks = m.mask_tensors() or (None, None)
+        for mu, rho, j in parts:
+            k = _snr(mu, rho).reshape(-1)
+            if masks[j] is not None:
+                k = k.masked_fill(~masks[j].reshape(-1), -math.inf)
+            keys.append(k)
+            sizes.append(k.numel())
+    if not keys:
+        return {"pruned": 0, "total": 0, "threshold": None, "per_layer": {}}
+    dev = keys[0].device
+    key = torch.cat([k.to(dev) for k in keys])
+    total = key.numel()
+    already = int((key == -math.inf).sum())
+    n = max(int(math.floor(fraction * total)), already)
+    order = torch.sort(key, stable=True).indices
+    pruned = torch.zeros(total, dtype=torch.bool, device=dev)
+    pruned[order[:n]] = True
+    threshold = None
+    if n > already:
+        threshold = float(key[order[n - 1]])
+    per_layer, off, it = {}, 0, iter(sizes)
+    for name, m in layers:
+        ranked = [m.W_mu] + ([m.bias_mu] if biases and m.use_bias else [])
+        cut = []
+        for t in ranked:
+            sz = next(it)
+            cut.append(pruned[off:off + sz].view(t.shape).to(t.device))
+            off += sz
+        bias_keep = ~cut[1] if len(cut) > 1 else (m.mask_tensors() or (None, None))[1]
+        m.set_weight_mask(~cut[0], bias_keep)
+        per_layer[name] = (int(sum(int(c.sum()) for c in cut)), sum(c.numel() for c in cut))
+    return {"pruned": n, "total": total, "threshold": threshold, "per_layer": per_layer}
