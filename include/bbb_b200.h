@@ -520,6 +520,31 @@ int bbb_mc_exchange_metrics(const float* logits, int32_t S_local, int32_t S_tota
                             uint64_t* noise_base, uint64_t noise_inc, float* expected_entropy, float* mutual_info,
                             int32_t batch_shards, double* metrics, void* cuda_stream);
 
+/* Appends one Monte-Carlo step's per-image scores to a data-set-long log, at a device-resident cursor
+ * (out-of-distribution detection and selective prediction over a whole data set: uncertainty_estimation.py:61-102).
+ * Inputs are the outputs of one exchange: log_outputs [B, C] (required); entropy, expected_entropy, mutual_info [B]
+ * and epistemic [B, C] (each nullable); labels [B] int64 (nullable).
+ * The log: BBB_MC_SCORE_PLANES fp32 planes planes[k * capacity + i] and one int32 plane pred[i]; image b of the launch
+ * goes to i = cursor[0] + b:
+ *   k = 0 confidence        expf(max_c log_outputs[b]), argmax = the first maximal class (as bbb_mc_exchange_metrics'
+ *                           conf; NaN is never maximal, a row of -inf gives class 0)
+ *   k = 1 entropy           entropy[b], bit for bit; NaN when entropy == NULL
+ *   k = 2 mutual_info       mutual_info[b]; NaN when NULL
+ *   k = 3 expected_entropy  expected_entropy[b]; NaN when NULL
+ *   k = 4 epistemic         sum_c epistemic[b, c], summed in double and rounded once; NaN when NULL
+ *   k = 5 correct           1 if pred == labels[b] else 0; NaN when labels == NULL
+ *   pred                    the argmax class
+ * Nothing is written at i >= capacity; those images are added to cursor[1] (dropped).  cursor[0] += B once per launch,
+ * after every CTA has read it, so launches that run one after another (one stream, or a replayed graph) append in
+ * launch order; launches on one cursor must not run concurrently.  The caller zeroes cursor[0..1] to start a log;
+ * cursor[0] must stay below 2^48 (its top 16 bits count the CTAs of a launch while it runs).
+ * B, C > 0, 0 <= capacity < 2^48 and non-NULL log_outputs, planes, pred, cursor, else BBB_E_INVALID. */
+enum { BBB_MC_SCORE_PLANES = 6 };
+int bbb_mc_score_log(const float* log_outputs, const float* entropy, const float* expected_entropy,
+                     const float* mutual_info, const float* epistemic, const int64_t* labels, int32_t B, int32_t C,
+                     float* planes, int32_t* pred, int64_t capacity, int64_t* cursor /* [2]: next index, images dropped */,
+                     void* cuda_stream);
+
 /* Peer-mapped receive buffers for bbb_mc_exchange (one process per GPU, same node): allocate locally, export a
  * 64-byte CUDA-IPC handle, ship it to the peers by any host channel (the Python side uses torch.distributed),
  * import theirs.  These five calls are the only ones in this library that allocate or synchronise. */

@@ -14,6 +14,7 @@
 #include "fused_tc.cuh"
 #include "conv_s4_tc.cuh"
 #include "mc_head.cuh"
+#include "score_log.cuh"
 
 namespace {
 
@@ -813,6 +814,26 @@ int bbb_mc_exchange(const float* logits, int32_t S_local, int32_t S_total, int32
     return bbb_mc_exchange_info(logits, S_local, S_total, B, C, kl, n_kl, flags, labels, train_size, beta, rank, world,
                                 peer_buffers, state, log_outputs, kl_out, pred, epistemic, aleatoric, entropy, head,
                                 noise_base, noise_inc, nullptr, nullptr, cuda_stream);
+}
+
+static_assert(BBB_MC_SCORE_PLANES == bbb::SL_PLANES, "score log planes: header and kernel disagree");
+int bbb_mc_score_log(const float* log_outputs, const float* entropy, const float* expected_entropy,
+                     const float* mutual_info, const float* epistemic, const int64_t* labels, int32_t B, int32_t C,
+                     float* planes, int32_t* pred, int64_t capacity, int64_t* cursor, void* cuda_stream) {
+    if (!log_outputs || !planes || !pred || !cursor) return fail(BBB_E_INVALID, "NULL pointer");
+    if (B <= 0 || C <= 0) return fail(BBB_E_INVALID, "bad B/C %d/%d", B, C);
+    if (capacity < 0 || (uint64_t)capacity > bbb::SL_INDEX_MASK) return fail(BBB_E_INVALID, "bad capacity %lld", (long long)capacity);
+    bbb::ScoreLogArgs a;
+    a.log_outputs = log_outputs; a.entropy = entropy; a.expected_entropy = expected_entropy; a.mutual_info = mutual_info;
+    a.epistemic = epistemic; a.labels = (const long long*)labels; a.B = B; a.C = C;
+    a.planes = planes; a.pred = pred; a.capacity = capacity; a.cursor = (unsigned long long*)cursor;
+    int grid = (B + bbb::SL_THREADS / 32 - 1) / (bbb::SL_THREADS / 32);
+    if (grid > bbb::SL_MAX_CTAS) grid = bbb::SL_MAX_CTAS;
+    bbb::mc_score_log_kernel<<<grid, bbb::SL_THREADS, 0, (cudaStream_t)cuda_stream>>>(a);
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return cuda_fail(e, "mc_score_log launch");
+    g_launches += 1;
+    return BBB_OK;
 }
 
 int bbb_comm_alloc(size_t bytes, void** dev_ptr) {

@@ -167,7 +167,8 @@ class MCForward:
                  seed: Optional[int] = None, graph: bool = True, num_classes: Optional[int] = None,
                  static_inputs=None, first_replay: int = 0, fold: bool = True, overlap: bool = False, inflight: int = 1,
                  fold_group: Optional[int] = None, fold_budget: int = LAYER_FOLD_BUDGET, want_information: bool = False,
-                 batch_shards: int = 1, metrics: Optional[torch.Tensor] = None, cache_prep: bool = True):
+                 batch_shards: int = 1, metrics: Optional[torch.Tensor] = None, cache_prep: bool = True,
+                 score_log: Optional["ScoreLog"] = None):
         """``static_inputs``: device tensors the caller fills in place (e.g. targets of its host->device copies, or a
         rotation of resident batches); one graph is captured per tensor and ``self(slot=k)`` runs the step on
         ``static_inputs[k]`` with no staging copy.  ``first_replay``: index of the first replay's noise block.
@@ -186,7 +187,11 @@ class MCForward:
         the layers' parameters and prior buffers with those of the last prep and, when one moved, replays the prep first -- after the work enqueued on the current stream so far and after every step still in
         flight.  So an in-place update through an autograd-visible tensor (optimizer.step(), p.copy_() under no_grad,
         set_prior, load_state_dict) is read by the next step; a write through p.data or a raw pointer is not.  False:
-        every step prepares its own operands, as a net with BBB layers always does."""
+        every step prepares its own operands, as a net with BBB layers always does.
+        ``score_log``: a ScoreLog every step appends its B images' scores to (bbb_mc_score_log, one more kernel behind
+        the exchange on the same stream): the outputs this engine computes, so ``want_uncertainty`` /
+        ``want_information`` decide which planes hold numbers, and ``with_labels`` whether ``correct`` does.  Steps
+        append in call order, in every mode; the warm-up steps the constructor runs do not."""
         if want_information and not want_uncertainty:
             raise L.EngineError("MCForward: want_information needs want_uncertainty")
         Fn._require_cuda(example_x, "MCForward")
@@ -200,6 +205,9 @@ class MCForward:
                 raise L.EngineError(f"MCForward: metrics must be a contiguous float64 tensor of >= {n} elements on "
                                     f"{example_x.device} (mc.new_metrics)")
         self.metrics = self._metrics = metrics      # _metrics: the accumulator the exchange adds to
+        if score_log is not None and score_log.device != example_x.device:
+            raise L.EngineError(f"MCForward: score_log is on {score_log.device}, the step on {example_x.device}")
+        self.score_log = self._score_log = score_log      # _score_log: the log the steps append to
         self.net, self.group = net, group
         self.dist, self.world, self.rank = _dist_info(group)
         if self.world > 16:
@@ -536,6 +544,9 @@ class MCForward:
                     "bbb_mc_exchange_metrics")
         else:
             L.check(lib.bbb_mc_exchange_sharded(*args, self.batch_shards, Fn._stream(self.dev)), "bbb_mc_exchange_sharded")
+        if self._score_log is not None:
+            self._score_log.append(o["log_outputs"], o.get("entropy"), o.get("expected_entropy"), o.get("mutual_info"),
+                                   o.get("epistemic"), self.labels_all[par] if self.labels_all is not None else None)
 
     def _capture(self, warmup: int = 2):
         from .graph import _STRIDE
@@ -564,9 +575,11 @@ class MCForward:
         dev = self.dev
         side = torch.cuda.Stream(device=dev)
         side.wait_stream(torch.cuda.current_stream(dev))
-        live = self._metrics
+        live, live_log = self._metrics, self._score_log
         if live is not None:
             self._metrics = torch.zeros_like(live)      # the warm-up steps do not count
+        if live_log is not None:
+            self._score_log = ScoreLog(dev, 0)          # nor are they logged (a log of no capacity drops them)
         self._prep = self._plan_prep(self.x) if self.cache_prep else None
         with torch.cuda.stream(side):
             if self._prep is not None:              # the first prep, which the warm-up steps already read
@@ -578,7 +591,7 @@ class MCForward:
                 self._exchange(*self._chain(self.x, self.base, par=p_), par=p_)
         torch.cuda.current_stream(dev).wait_stream(side)
         torch.cuda.synchronize(dev)
-        self._metrics = live
+        self._metrics, self._score_log = live, live_log
         # GEMM chain on a HIGH-priority stream, parameter preps on the (default-priority) side streams: when both have CTAs
         # pending, the chain's go first -- the preps of later layers no longer keep the first GEMM's CTAs off the SMs
         cap = torch.cuda.Stream(device=dev, priority=-1)
@@ -618,10 +631,12 @@ class MCForward:
                     n_chain = L.launch_count() - n0
                     self.chain_graphs[par].append(g)
                 g = torch.cuda.CUDAGraph()
+                n0 = L.launch_count()
                 with torch.cuda.graph(g, stream=cap):
                     self._exchange(kl_ptr, n_kl, par=par)
+                n_exch = L.launch_count() - n0
                 self.exch_graphs.append(g)
-            self.kernels_per_step = n_chain + 1
+            self.kernels_per_step = n_chain + n_exch
             self.graphs = self.chain_graphs[0]
             # the exchange kernel is tiny and latency-critical (peers wait for it): highest priority the device offers
             lo = getattr(torch.cuda.Stream, "priority_range", lambda: (-1, 0))()
@@ -908,8 +923,83 @@ def read_metrics(t: torch.Tensor) -> dict:
             "bin_accuracy": [div(cor[m], cnt[m]) for m in range(nb)]}
 
 
+class ScoreLog:
+    """A data-set-long log of per-image scores on the device, appended to by the Monte-Carlo step (bbb_mc_score_log):
+    ``MCForward(..., score_log=log)`` and ``evaluate(..., score_log=log)`` add one entry per image, in step order, with
+    no host read; ``read()`` returns the entries once the data set is done.
+
+    Entry i holds ``confidence`` = max_c p_bar (exp of the largest log_output; the first maximal class is ``pred``),
+    ``entropy`` = H[p_bar], ``mutual_info`` and ``expected_entropy`` (the BALD decomposition), ``epistemic`` = sum_c of
+    the epistemic variance, ``correct`` = 1.0 / 0.0 (pred == label), and ``pred`` (int32).  A score the step does not
+    compute (no ``want_uncertainty`` / ``want_information`` / labels) is NaN.  ``capacity`` entries fit; images past
+    them are counted, not written, and ``read()`` refuses a log that dropped any."""
+
+    PLANES = ("confidence", "entropy", "mutual_info", "expected_entropy", "epistemic", "correct")
+
+    def __init__(self, device, capacity: int):
+        capacity = int(capacity)
+        if capacity < 0:
+            raise ValueError(f"ScoreLog: capacity must be >= 0 (got {capacity})")
+        self.device = torch.device(device)
+        if self.device.type == "cuda" and self.device.index is None:
+            self.device = torch.device("cuda", torch.cuda.current_device())
+        self.capacity = capacity
+        assert len(self.PLANES) == L.MC_SCORE_PLANES
+        # (one column at least: an empty tensor has no address, and the kernel takes the log's pointers even when
+        # nothing fits)
+        self._planes = torch.zeros(L.MC_SCORE_PLANES, max(1, capacity), dtype=torch.float32, device=self.device)
+        self._pred = torch.zeros(max(1, capacity), dtype=torch.int32, device=self.device)
+        self._cursor = torch.zeros(2, dtype=torch.int64, device=self.device)     # next index, images dropped
+
+    def reset(self):
+        """Start the log again (stream-ordered: after the work enqueued on the current stream so far)."""
+        self._cursor.zero_()
+
+    def _counts(self):
+        nxt, dropped = self._cursor.tolist()
+        return min(nxt, self.capacity), dropped
+
+    def __len__(self):
+        """Entries held (a host read of the cursor)."""
+        return self._counts()[0]
+
+    @property
+    def dropped(self) -> int:
+        """Images that did not fit (a host read of the cursor)."""
+        return self._counts()[1]
+
+    def read(self) -> dict:
+        """The entries logged so far: {plane name: float32 [n], "pred": int32 [n]}, copies on the log's device.  Raises
+        EngineError if images were dropped.  Steps in flight must be complete first (``MCForward.wait()``)."""
+        n, dropped = self._counts()
+        if dropped:
+            raise L.EngineError(f"ScoreLog: {dropped} images did not fit (capacity {self.capacity}, "
+                                f"{n + dropped} logged)")
+        out = {k: self._planes[i, :n].clone() for i, k in enumerate(self.PLANES)}
+        out["pred"] = self._pred[:n].clone()
+        return out
+
+    def append(self, log_outputs, entropy=None, expected_entropy=None, mutual_info=None, epistemic=None, labels=None):
+        """Append one step's images (bbb_mc_score_log on the current stream): log_outputs [B, C] and the optional
+        [B] / [B, C] uncertainty outputs and int64 labels [B] of the same step, fp32 contiguous on the log's device."""
+        Fn._require_cuda(self._cursor, "ScoreLog.append")
+        B, Cc = log_outputs.shape
+        for t, shape, dt in ((log_outputs, (B, Cc), torch.float32), (entropy, (B,), torch.float32),
+                             (expected_entropy, (B,), torch.float32), (mutual_info, (B,), torch.float32),
+                             (epistemic, (B, Cc), torch.float32), (labels, (B,), torch.int64)):
+            if t is not None and not (t.device == self.device and tuple(t.shape) == shape and t.dtype == dt
+                                      and t.is_contiguous()):
+                raise L.EngineError(f"ScoreLog.append: expected a contiguous {dt} tensor of shape {shape} on "
+                                    f"{self.device}, got {t.dtype} {tuple(t.shape)} on {t.device}")
+        L.check(L.lib().bbb_mc_score_log(Fn._ptr(log_outputs), Fn._ptr(entropy), Fn._ptr(expected_entropy),
+                                         Fn._ptr(mutual_info), Fn._ptr(epistemic), Fn._ptr(labels), B, Cc,
+                                         Fn._ptr(self._planes), Fn._ptr(self._pred), self.capacity,
+                                         Fn._ptr(self._cursor), Fn._stream(self.device)), "bbb_mc_score_log")
+
+
 def evaluate(net, loader, num_ens: int, train_size: float, beta_type=0.1, epoch=None, num_epochs=None, group=None,
-             seed: Optional[int] = None, inflight: int = 4, batch_shards: int = 1) -> dict:
+             seed: Optional[int] = None, inflight: int = 4, batch_shards: int = 1, normalized: bool = False,
+             score_log: Optional[ScoreLog] = None) -> dict:
     """main_bayesian.validate_model over ``loader`` (batches of (inputs, labels)) on the engine, with calibration.
 
     Returns read_metrics' dict plus ``valid_loss`` and ``valid_acc`` as validate_model computes them: the mean over
@@ -922,12 +1012,19 @@ def evaluate(net, loader, num_ens: int, train_size: float, beta_type=0.1, epoch=
     not pinned are first copied into pinned slots, so the host can run up to ``max(2, inflight)`` batches ahead.  The
     engines and the accumulator are kept on the net, as mc_forward keeps its engines, for the next call with the same
     options (the next epoch); each call draws fresh noise.  Every rank must iterate the same loader (as MCForward
-    requires)."""
+    requires).
+
+    ``normalized``: p_hat_s is the softplus-normalised row (uncertainty_estimation.py:73-77), not the softmax.
+    ``score_log``: a ScoreLog every image is appended to, in loader order (after what it already holds: ``reset()`` it
+    to start over).  The engines then also compute the uncertainty and information outputs; the returned figures are
+    the same bits as without a log.  Engines are kept per log object: reuse a log from epoch to epoch."""
     dev = next(net.parameters()).device
-    key = (int(num_ens), float(train_size), seed, id(group), int(inflight), int(batch_shards))
+    log = score_log is not None
+    key = (int(num_ens), float(train_size), seed, id(group), int(inflight), int(batch_shards), bool(normalized),
+           id(score_log) if log else None)
     ev = _engine_cache(net, "_mc_eval").get(key)
     if ev is None:
-        ev = net.__dict__["_mc_eval"][key] = {"acc": new_metrics(dev), "engines": {}, "seed": seed}
+        ev = net.__dict__["_mc_eval"][key] = {"acc": new_metrics(dev), "engines": {}, "seed": seed, "log": score_log}
     acc, engines, nslots = ev["acc"], ev["engines"], max(2, int(inflight))
     cur = torch.cuda.current_stream(dev)
     acc.zero_()
@@ -940,7 +1037,8 @@ def evaluate(net, loader, num_ens: int, train_size: float, beta_type=0.1, epoch=
             # the k-th engine built draws noise blocks k * 2^16, k * 2^16 + 1, ...: engines do not share noise
             eng = MCForward(net, slots[0], num_ens, group, with_labels=True, train_size=train_size, seed=ev["seed"],
                             static_inputs=slots, first_replay=len(engines) << 16, overlap=True, inflight=inflight,
-                            batch_shards=batch_shards, metrics=acc)
+                            batch_shards=batch_shards, metrics=acc, normalized=normalized, want_uncertainty=log,
+                            want_information=log, score_log=score_log)
             ev["seed"] = eng.seed               # every engine draws from the same seed
             e = engines[shape] = {"eng": eng, "slots": slots, "consumed": [None] * nslots, "steps": 0,
                                   "labels": [torch.zeros(x.shape[0], dtype=torch.int64, device=dev) for _ in range(nslots)],
@@ -1086,7 +1184,9 @@ class MCTrainStep(MCForward):
     exchange, and the step holds as much as the sample loop does."""
 
     def __init__(self, net, example_x, num_ens, train_size, group=None, seed=None, batch_shards: int = 1,
-                 fold: bool = False, fold_group: Optional[int] = None):
+                 fold: bool = False, fold_group: Optional[int] = None, score_log=None):
+        if score_log is not None:
+            raise L.EngineError("MCTrainStep does not log scores: log them from MCForward or evaluate()")
         super().__init__(net, example_x, num_ens, group=group, with_labels=True, train_size=train_size, seed=seed,
                          graph=False, fold=False, batch_shards=batch_shards)
         self.params = [p for p in net.parameters() if p.requires_grad]
@@ -1158,3 +1258,154 @@ class MCTrainStep(MCForward):
                 off += n
         self.steps += 1
         return o
+
+
+# --------------------------------------------------------------------------------------------------------------------
+# Ranking metrics over a score log: out-of-distribution detection and selective prediction.  Larger score = more likely
+# out-of-distribution / wrong.  They run once per data set, in float64 torch ops on the scores' device.
+# --------------------------------------------------------------------------------------------------------------------
+OOD_SCORES = ("confidence", "entropy", "mutual_info", "expected_entropy", "epistemic")
+SELECTIVE_COVERAGES = (0.5, 0.8, 0.9, 0.95, 0.99)
+
+
+def _scores64(s, what):
+    s = torch.as_tensor(s).detach().reshape(-1).to(torch.float64)
+    if s.numel() == 0:
+        raise ValueError(f"{what}: empty score set")
+    if bool(torch.isnan(s).any()):
+        raise ValueError(f"{what}: NaN score")
+    return s
+
+
+def _auroc(neg, pos):
+    """P(pos > neg) + 1/2 P(pos = neg) over all pairs, from the midranks of the pooled scores (Mann-Whitney U)."""
+    v, order = torch.sort(torch.cat([neg, pos]))
+    _, inv, counts = torch.unique_consecutive(v, return_inverse=True, return_counts=True)
+    ends = counts.cumsum(0).to(torch.float64)
+    mid = ends - (counts.to(torch.float64) - 1.0) / 2.0          # mean of the 1-based ranks end - count + 1 .. end
+    n_neg, n_pos = neg.numel(), pos.numel()
+    r_pos = mid[inv][order >= n_neg].sum()
+    return float((r_pos - n_pos * (n_pos + 1) / 2.0) / (float(n_pos) * float(n_neg)))
+
+
+def _flagged(s, pos):
+    """At the distinct thresholds t_1 > t_2 > ... of s, flagging s >= t_k: (positives flagged, negatives flagged)."""
+    v, order = torch.sort(s, descending=True)
+    _, counts = torch.unique_consecutive(v, return_counts=True)
+    ends = counts.cumsum(0) - 1
+    p = pos[order].to(torch.float64)
+    return p.cumsum(0)[ends], (1.0 - p).cumsum(0)[ends]
+
+
+def _average_precision(s, pos):
+    """sum_k (R_k - R_{k-1}) P_k over the distinct thresholds, R_0 = 0 (sklearn's average_precision_score)."""
+    tp, fp = _flagged(s, pos)
+    recall = tp / tp[-1]
+    return float((torch.diff(recall, prepend=recall.new_zeros(1)) * (tp / (tp + fp))).sum())
+
+
+def ood_metrics(s_in, s_out) -> dict:
+    """Out-of-distribution detection from the scores of an in-distribution set ``s_in`` and an OOD set ``s_out``
+    (larger = more likely OOD; OOD is the positive class): ``auroc``, ``aupr_out`` (average precision, OOD positive),
+    ``aupr_in`` (the in-distribution set positive, scores negated) and ``fpr_at_95_tpr`` (the least false-positive
+    rate over thresholds whose true-positive rate is >= 0.95).  NaN scores or an empty set raise ValueError."""
+    s_in, s_out = _scores64(s_in, "ood_metrics: s_in"), _scores64(s_out, "ood_metrics: s_out")
+    s_out = s_out.to(s_in.device)
+    s = torch.cat([s_in, s_out])
+    out = torch.cat([torch.zeros_like(s_in, dtype=torch.bool), torch.ones_like(s_out, dtype=torch.bool)])
+    tp, fp = _flagged(s, out)
+    tpr, fpr = tp / s_out.numel(), fp / s_in.numel()
+    return {"auroc": _auroc(s_in, s_out), "aupr_out": _average_precision(s, out),
+            "aupr_in": _average_precision(-s, ~out), "fpr_at_95_tpr": float(fpr[tpr >= 0.95].min()),
+            "n_in": s_in.numel(), "n_out": s_out.numel()}
+
+
+def selective_metrics(score, correct) -> dict:
+    """Selective prediction (Geifman et al. 2019) and misclassification detection (Hendrycks & Gimpel 2017) from a
+    per-image ``score`` (larger = more likely wrong) and ``correct`` (1 / 0).
+
+    ``coverage`` / ``risk``: the risk-coverage curve at the distinct thresholds in ascending order, accepting score <= t
+    (float64 tensors); ``aurc`` = sum_k (cov_k - cov_{k-1}) risk_k; ``eaurc`` = aurc minus the AURC of the ideal order
+    (every correct image first, no ties: (1/n) sum_{k=1..n} max(0, k - n_correct) / k); ``auroc`` with the wrong
+    predictions positive (NaN when all or none are correct); ``accuracy``; ``accuracy_at`` {c: accuracy of the
+    ceil(c * n) lowest scores (ties by index)} for c in SELECTIVE_COVERAGES.  NaN or an empty set raise ValueError."""
+    from fractions import Fraction
+    s = _scores64(score, "selective_metrics: score")
+    ok = _scores64(correct, "selective_metrics: correct").to(s.device)
+    if ok.numel() != s.numel():
+        raise ValueError(f"selective_metrics: {s.numel()} scores but {ok.numel()} correct flags")
+    if not bool(((ok == 0) | (ok == 1)).all()):
+        raise ValueError("selective_metrics: correct must be 0 or 1")
+    n = s.numel()
+    v, order = torch.sort(s, stable=True)
+    _, counts = torch.unique_consecutive(v, return_counts=True)
+    ends = counts.cumsum(0) - 1
+    wrong = (1.0 - ok[order]).cumsum(0)[ends]
+    accepted = (ends + 1).to(torch.float64)
+    cov, risk = accepted / n, wrong / accepted
+    aurc = float((torch.diff(cov, prepend=cov.new_zeros(1)) * risk).sum())
+    n_ok = int(ok.sum())
+    k = torch.arange(1, n + 1, dtype=torch.float64, device=s.device)
+    ideal = float(((k - n_ok).clamp_min(0.0) / k).sum() / n)
+    bad = ok == 0
+    auroc = _auroc(s[~bad], s[bad]) if 0 < n_ok < n else float("nan")
+    at = {}
+    for c in SELECTIVE_COVERAGES:
+        m = max(1, math.ceil(Fraction(repr(c)) * n))
+        at[c] = float(ok[order[:m]].mean())
+    return {"coverage": cov, "risk": risk, "aurc": aurc, "eaurc": aurc - ideal, "auroc": auroc,
+            "accuracy": n_ok / n, "accuracy_at": at, "n": n}
+
+
+def _score(log: dict, name: str):
+    """The score ``name`` of a ScoreLog.read() dict, larger = more likely OOD / wrong: -confidence (not 1 - conf,
+    which loses the bits near 1), the others as logged."""
+    if name not in OOD_SCORES:
+        raise ValueError(f"unknown score {name!r}: one of {OOD_SCORES}")
+    return -log["confidence"] if name == "confidence" else log[name]
+
+
+def _loader_images(loader):
+    """Images a loader yields: len(loader.dataset), else the batches of a sized sequence counted."""
+    ds = getattr(loader, "dataset", None)
+    if ds is not None:
+        return len(ds)
+    if hasattr(loader, "__len__") and hasattr(loader, "__getitem__"):
+        return sum(int(b[0].shape[0]) for b in loader)
+    raise ValueError("detect_ood: a loader without .dataset must be a sequence of (x, y) batches")
+
+
+def detect_ood(net, in_loader, out_loader, num_ens: int, score: Optional[str] = "mutual_info", normalized: bool = False,
+               **evaluate_kwargs) -> dict:
+    """Out-of-distribution detection over whole data sets (uncertainty_estimation.py's MNIST vs notMNIST comparison):
+    ``evaluate`` over ``in_loader`` and ``out_loader`` (batches of (x, y); the OOD set's labels are not used), each
+    into a ScoreLog, and the ranking metrics of their scores.
+
+    Returns ``in`` (evaluate's dict on the in-distribution set), ``ood`` (ood_metrics of ``score``, or {name:
+    ood_metrics} for every name of OOD_SCORES with ``score=None``), ``selective`` (selective_metrics on the
+    in-distribution set, per score in the same way) and ``logs`` ({"in": ..., "out": ...}, ScoreLog.read() dicts).
+    ``evaluate_kwargs`` go to evaluate (``train_size`` defaults to 1.0).  The two logs are kept on the net, as evaluate
+    keeps its engines, and reused by the next call."""
+    names = OOD_SCORES if score is None else (score,)
+    if any(nm not in OOD_SCORES for nm in names):
+        raise ValueError(f"detect_ood: unknown score {score!r}: one of {OOD_SCORES}, or None for all")
+    dev = next(net.parameters()).device
+    kw = dict(evaluate_kwargs)
+    train_size = kw.pop("train_size", 1.0)
+    logs, res = net.__dict__.setdefault("_ood_logs", {}), {}
+    for role, loader in (("in", in_loader), ("out", out_loader)):
+        n = _loader_images(loader)
+        log = logs.get(role)
+        if log is None or log.capacity < n or log.device != dev:
+            if log is not None:                     # evaluate's engines that append to the old log go with it
+                cache = net.__dict__.get("_mc_eval", {})
+                for k in [k for k, e in cache.items() if e.get("log") is log]:
+                    del cache[k]
+            log = logs[role] = ScoreLog(dev, n)
+        log.reset()
+        res[role] = evaluate(net, loader, num_ens, train_size, normalized=normalized, score_log=log, **kw)
+    got = {role: logs[role].read() for role in ("in", "out")}
+    ood = {nm: ood_metrics(_score(got["in"], nm), _score(got["out"], nm)) for nm in names}
+    sel = {nm: selective_metrics(_score(got["in"], nm), got["in"]["correct"]) for nm in names}
+    return {"in": res["in"], "ood": ood if score is None else ood[score],
+            "selective": sel if score is None else sel[score], "logs": got}
