@@ -13,166 +13,15 @@ every map, kernel, channel count, batch, tile width, prep and output layout list
 then check the planner's wiring end to end, and the nets it must refuse run correctly unfused.
 Run with -s to see the worst normalised error per case family."""
 import collections
-import ctypes as C
 import sys
 
 import pytest
 import torch
 
 from tests import fused_ref as R
+from tests.fused_ref import CASES, GUARD, SENTINEL, _alloc_out, _layer, _out_hw, _prep, _step, _tile_bn
+from tests.fused_ref import fused_call as _call
 from tests.util import scale_err
-
-Case = collections.namedtuple("Case", "name why kind variant cin hw cout k s p pool act out sq wide B prev_hw")
-
-
-def _c(name, why, kind, variant, cin, hw, cout, k=1, s=1, p=0, pool=False, act="none", out="packed", sq=False,
-       wide=0, B=128, prev_hw=1):
-    return Case(name, why, kind, variant, cin, hw, cout, k, s, p, pool, act, out, sq, wide, B, prev_hw)
-
-
-CASES = [
-    # ---- tap-GEMM conv layers (tap_gemm_kernel; tap_prep_conv_kernel for k > 1, tap_prep_kernel for 1x1 taps)
-    _c("t8x8_c64_k3p1_pool_lrt", "8x8 map with exactly TAP_MAX_ITEMS = 64 schedule items; pooled packed + x^2; ragged "
-       "second row tile", "tap", "lrt", 64, (8, 8), 128, 3, 1, 1, True, "softplus", "packed", True, 0, 129),
-    _c("t8x8_k3s2p1_bbb", "stride-2 taps; unpooled bulk-copy store of one full row tile", "tap", "bbb",
-       64, (8, 8), 64, 3, 2, 1, False, "relu", "packed", False, 0, 128),
-    _c("t8x8_k3s2p1_wide_lrt", "stride-2 taps, BN = 128 unpooled: bulk copy of two tiles + direct store of the ragged "
-       "third", "tap", "lrt", 64, (8, 8), 128, 3, 2, 1, False, "none", "packed", True, 1, 300),
-    _c("t4x8_c128_items64_lrt", "non-square 4x8 map, Cin = 128 (64 items); one ragged tile: direct stores only",
-       "tap", "lrt", 128, (4, 8), 64, 3, 1, 1, False, "none", "packed", False, 0, 127),
-    _c("t4x8_pool_nchw72_bbb", "non-square pooled NCHW fp32 output, Cout = 72: partial 16-column pool group",
-       "tap", "bbb", 64, (4, 8), 72, 3, 1, 1, True, "relu", "f32", False, 0, 129),
-    _c("t4x8_pool_nchw72_lrt", "as above, LRT, one image", "tap", "lrt", 64, (4, 8), 72, 3, 1, 1, True, "softplus",
-       "f32", False, 0, 1),
-    _c("t4x4_c256_items64_wide_bbb", "Cin = 256 on 4x4 (64 items), BN = 128 unpooled, x^2 for an LRT consumer",
-       "tap", "bbb", 256, (4, 4), 256, 3, 1, 1, False, "relu", "packed", True, 1, 129),
-    _c("t4x4_c192_k1_lrt", "1x1 taps (tap_prep_kernel), Cin = Cout = 192", "tap", "lrt", 192, (4, 4), 192, 1, 1, 0,
-       False, "softplus", "packed", True, 0, 129),
-    _c("t4x4_k5p2_pool_bbb", "5x5 p2 taps, pooled BN = 64 (16-channel groups), Cout = 192", "tap", "bbb",
-       64, (4, 4), 192, 5, 1, 2, True, "softplus", "packed", False, 0, 128),
-    _c("t4x4_k5p2_pool_wide_lrt", "5x5 p2, pooled BN = 128 (32-channel groups) + x^2, three row tiles", "tap", "lrt",
-       64, (4, 4), 192, 5, 1, 2, True, "relu", "packed", True, 1, 300),
-    _c("t4x4_k3p0_b1_bbb", "3x3 p0 (4x4 -> 2x2), a single image", "tap", "bbb", 128, (4, 4), 128, 3, 1, 0, False,
-       "relu", "packed", False, 0, 1),
-    _c("t4x4_k3p0_nchw100_lrt", "unpooled NCHW fp32 map output, Cout = 100", "tap", "lrt", 64, (4, 4), 100, 3, 1, 0,
-       False, "softplus", "f32", False, 0, 127),
-    _c("t2x2_c256_lrt", "2x2 map, Cin = 256, 4 of 9 taps live per pixel", "tap", "lrt", 256, (2, 2), 256, 3, 1, 1,
-       False, "softplus", "packed", True, 0, 128),
-    _c("t2x2_pool320_bbb", "pool to 1x1, Cout = 320, pooled BN = 64", "tap", "bbb", 128, (2, 2), 320, 3, 1, 1, True,
-       "none", "packed", False, 0, 129),
-    _c("t2x2_pool320_wide_lrt", "Cin = 192, Cout = 320, pooled BN = 128 + x^2", "tap", "lrt", 192, (2, 2), 320, 3, 1, 1,
-       True, "relu", "packed", True, 1, 300),
-    _c("t2x2_k1_b300_bbb", "1x1 taps; two bulk-copied tiles and a ragged third", "tap", "bbb", 64, (2, 2), 64, 1, 1, 0,
-       False, "none", "packed", False, 0, 300),
-    _c("t8x8_k1_pool_b1_lrt", "1x1 taps pooled on 8x8, a single image", "tap", "lrt", 64, (8, 8), 64, 1, 1, 0, True,
-       "relu", "packed", True, 0, 1),
-    _c("t8x8_k5p2_pool_nchw_bbb", "5x5 p2 on 8x8, pooled NCHW fp32 4x4 output", "tap", "bbb", 64, (8, 8), 64, 5, 1, 2,
-       True, "softplus", "f32", False, 0, 127),
-    _c("t8x8_k3p0_c192_lrt", "3x3 p0 (8x8 -> 6x6), Cout = 192 (BN stays 64 with wide tiles on)", "tap", "lrt",
-       64, (8, 8), 192, 3, 1, 0, False, "relu", "packed", True, 1, 128),
-    _c("t4x4_c128_softplus_bbb", "BBB softplus unpooled, ragged tile", "tap", "bbb", 128, (4, 4), 64, 3, 1, 1, False,
-       "softplus", "packed", False, 0, 127),
-    _c("t2x2_nchw10_bbb", "NCHW fp32 output, Cout = 10", "tap", "bbb", 64, (2, 2), 10, 3, 1, 1, False, "none", "f32",
-       False, 0, 300),
-    _c("t4x4_nchw10_lrt", "Cout = 10 (N % 4 != 0: per-element Philox draws) on a 4x4 map", "tap", "lrt", 64, (4, 4), 10,
-       3, 1, 1, False, "relu", "f32", False, 0, 129),
-    # ---- linear layers on the tap-GEMM (a 1x1 map; prev_hw = H*W of the flattened map feeding it)
-    _c("l_prev1_n10_bbb", "classifier, fp32 logits, Cout = 10", "linear", "bbb", 256, (1, 1), 10, out="f32", B=129),
-    _c("l_prev4_n100_lrt", "prev_hw = 4 feature permutation, Cout = 100", "linear", "lrt", 512, (1, 1), 100, out="f32",
-       B=300, prev_hw=4),
-    _c("l_prev8_n10_lrt", "prev_hw = 8, N % 4 != 0 Philox", "linear", "lrt", 512, (1, 1), 10, out="f32", B=127,
-       prev_hw=8),
-    _c("l_prev6_n72_lrt", "prev_hw = 6 (a 3x2 map), Cin = 1920 (30 K blocks), fp32 N = 72", "linear", "lrt", 1920, (1, 1),
-       72, act="none", out="f32", B=128, prev_hw=6),
-    _c("l_prev4_packed_bbb", "hidden linear fed by a 2x2 map, packed output + x^2", "linear", "bbb", 1024, (1, 1), 128,
-       act="relu", out="packed", sq=True, B=129, prev_hw=4),
-    _c("l_prev1_packed_wide_lrt", "hidden linear, BN = 128 unpooled, Cin = 192", "linear", "lrt", 192, (1, 1), 256,
-       act="softplus", out="packed", sq=True, wide=1, B=300),
-    _c("l_prev6_n100_b1_bbb", "prev_hw = 6, a single image", "linear", "bbb", 384, (1, 1), 100, act="softplus",
-       out="f32", B=1, prev_hw=6),
-    _c("l_4096_items64_lrt", "Cin = 4096: 64 K blocks, the schedule limit", "linear", "lrt", 4096, (1, 1), 10, out="f32",
-       B=128),
-    # ---- gather first layer (gemm_tc_kernel with the fused epilogue) on an NCHW fp32 image
-    _c("g_c3_8x8_pool_packed_lrt", "gather, fused pool, packed output + x^2", "gather", "lrt", 3, (8, 8), 64, 3, 1, 1,
-       True, "softplus", "packed", True, 0, 129),
-    _c("g_c1_8x8_pool_packed_bbb", "gather, Cin = 1, Cout = 128", "gather", "bbb", 1, (8, 8), 128, 3, 1, 1, True, "relu",
-       "packed", False, 0, 128),
-    _c("g_c16_4x8_pool_packed_lrt", "gather, Cin = 16, non-square, three row tiles", "gather", "lrt", 16, (4, 8), 64,
-       3, 1, 1, True, "relu", "packed", False, 0, 300),
-    _c("g_c3_4x8_pool_nchw72_bbb", "gather, pooled NCHW fp32 output, Cout = 72", "gather", "bbb", 3, (4, 8), 72,
-       3, 1, 1, True, "relu", "f32", False, 0, 127),
-    _c("g_c16_8x8_pool_nchw100_lrt", "gather, pooled NCHW fp32, Cout = 100, one image", "gather", "lrt", 16, (8, 8), 100,
-       3, 1, 1, True, "softplus", "f32", False, 0, 1),
-    _c("g_c1_64x64_k11s4_lrt", "stride 4, k11 with OW = 16: not the stride-4 kernel, the gather one", "gather", "lrt",
-       1, (64, 64), 64, 11, 4, 5, True, "relu", "packed", True, 0, 37),
-    _c("g_c3_4x8_nopool_bbb", "gather, unpooled packed output", "gather", "bbb", 3, (4, 8), 64, 3, 1, 1, False, "relu",
-       "packed", False, 0, 5),
-    # ---- stride-4 first layer (conv_s4_kernel): 16-image row tiles, OW = 8, Cout = 64, pooled packed output
-    _c("s_c3_k11_32x32_b17_lrt", "AlexNet conv1 geometry, a ragged second 16-image tile", "s4", "lrt", 3, (32, 32), 64,
-       11, 4, 5, True, "relu", "packed", True, 0, 17),
-    _c("s_c1_k11_64x32_b16_bbb", "Cin = 1, OH = 16, one full 16-image tile", "s4", "bbb", 1, (64, 32), 64, 11, 4, 5, True,
-       "softplus", "packed", False, 0, 16),
-    _c("s_c4_k7_48x32_b200_lrt", "Cin = 4, k7 p3, OH = 12 != OW", "s4", "lrt", 4, (48, 32), 64, 7, 4, 3, True,
-       "softplus", "packed", True, 0, 200),
-    _c("s_c3_k7_32x32_b1_bbb", "k7 p3, a single image", "s4", "bbb", 3, (32, 32), 64, 7, 4, 3, True, "relu", "packed",
-       False, 0, 1),
-    _c("s_c1_k7_48x32_b15_lrt", "Cin = 1, k7, 15 images (one partial tile), no x^2", "s4", "lrt", 1, (48, 32), 64,
-       7, 4, 3, True, "none", "packed", False, 0, 15),
-    _c("s_c4_k11_48x32_b17_bbb", "Cin = 4, k11 on 48x32, x^2 for an LRT consumer", "s4", "bbb", 4, (48, 32), 64,
-       11, 4, 5, True, "relu", "packed", True, 0, 17),
-    _c("s_c3_k11_32x32_b200_bbb", "AlexNet conv1, 200 images (13 tiles, the last partial)", "s4", "bbb", 3, (32, 32),
-       64, 11, 4, 5, True, "softplus", "packed", False, 0, 200),
-    _c("s_c4_k7_64x32_b16_lrt", "Cin = 4, k7 on 64x32 (OH = 16)", "s4", "lrt", 4, (64, 32), 64, 7, 4, 3, True, "none",
-       "packed", True, 0, 16),
-]
-assert len({c.name for c in CASES}) == len(CASES)
-
-
-def _out_hw(cs):
-    h, w = cs.hw
-    return (h + 2 * cs.p - cs.k) // cs.s + 1, (w + 2 * cs.p - cs.k) // cs.s + 1
-
-
-def _tile_bn(cs):
-    """Column tile width launch_fused picks for a tap-GEMM case (132 SMs)."""
-    oh, ow = _out_hw(cs)
-    ng128 = 32 if cs.pool else 128
-    psets = (oh // 2) * (ow // 2) if cs.pool else oh * ow
-    row_tiles = (cs.B + 127) // 128
-    return 128 if cs.cout % ng128 == 0 and (cs.wide or psets * (cs.cout // ng128) * row_tiles >= 132 * 6 // 10) else 64
-
-
-def _prep(cs):
-    return "tap_prep_conv_kernel" if cs.k > 1 and cs.prev_hw == 1 else "tap_prep_kernel"
-
-
-def _layer(cs):
-    import pytorch_bayesiancnn_b200 as bbb
-    if cs.kind == "linear":
-        return (bbb.BBBLRTLinear if cs.variant == "lrt" else bbb.BBBLinear)(cs.cin, cs.cout)
-    cls = bbb.BBBLRTConv2d if cs.variant == "lrt" else bbb.BBBConv2d
-    return cls(cs.cin, cs.cout, cs.k, stride=cs.s, padding=cs.p)
-
-
-def _step(cs, m):
-    from pytorch_bayesiancnn_b200 import fused, _lib as L
-    st = fused._Step()
-    st.layer, st.batch, st.conv = m, cs.B, m._conv_geometry()
-    st.linear = st.conv is None
-    st.prev_hw = cs.prev_hw
-    st.in_shape = (cs.cin,) + tuple(cs.hw)
-    st.in_layout = L.LAYOUT_NCHW_F32 if cs.kind in ("gather", "s4") else L.LAYOUT_PACKED_BF16
-    oh, ow = _out_hw(cs)
-    st.eps_shape = (cs.cout, oh, ow)
-    st.act = L.ACT_BY_NAME[cs.act]
-    st.pool = cs.pool
-    st.out_chw = (cs.cout, oh // 2, ow // 2) if cs.pool else (cs.cout, oh, ow)
-    if cs.out == "packed":
-        st.out_layout = L.LAYOUT_PACKED_BF16
-    else:
-        st.out_layout = L.LAYOUT_ROWMAJOR_F32 if st.out_chw[1:] == (1, 1) else L.LAYOUT_NCHW_F32
-    return st
-
 
 def test_case_table_covers_every_branch():
     tap = [c for c in CASES if c.kind == "tap"]
@@ -203,8 +52,6 @@ def test_case_table_covers_every_branch():
 
 # --------------------------------------------------------------------------------------------- per-layer GPU tests
 _worst = collections.defaultdict(float)
-GUARD = 64
-SENTINEL = -1.25e37
 
 
 @pytest.fixture(scope="module")
@@ -215,36 +62,6 @@ def dev():
     if _worst:
         lines = [f"  {fam:8s} worst |y - ref| / (C (M + |ref|)) = {v:.3f}" for fam, v in sorted(_worst.items())]
         sys.__stdout__.write("\n[fused geometry]\n" + "\n".join(lines) + "\n")
-
-
-def _call(st, x, x_sq, y, y_sq, eps_a, eps_b, seed=0, stream=0):
-    """One bbb_layer_forward_fused call, arguments as fused.run_step passes them; returns the KL scalar."""
-    from pytorch_bayesiancnn_b200 import fused, functional as Fn, _lib as L
-    m = st.layer
-    dev = m.W_mu.device
-    d = fused._step_desc(st, 0)
-    kl = torch.empty((), dtype=torch.float32, device=dev)
-    ws = Fn.workspace(dev, d, m)
-    rc = L.lib().bbb_layer_forward_fused(
-        C.byref(d), Fn._ptr(x), Fn._ptr(x_sq), st.in_layout, fused._in_pitch(st), st.prev_hw,
-        Fn._ptr(m.W_mu), Fn._ptr(m.W_rho), Fn._ptr(m.bias_mu), Fn._ptr(m.bias_rho),
-        Fn._ptr(y), Fn._ptr(y_sq), st.out_layout, fused._out_pitch(st), Fn._ptr(kl), Fn._ptr(eps_a), Fn._ptr(eps_b),
-        C.c_uint64(seed), C.c_uint64(stream), None, Fn._ptr(ws), C.c_size_t(ws.numel()), Fn._stream(dev))
-    L.check(rc, "bbb_layer_forward_fused")
-    return kl
-
-
-def _alloc_out(cs, st, dev):
-    """(y, y_sq, n): a NaN-filled tiled buffer, or an fp32 buffer of n outputs + GUARD sentinel floats."""
-    cout, oh, ow = st.out_chw
-    if cs.out == "packed":
-        planes = 2 if cs.sq else 1
-        y = torch.full((R.tiled_rows(cs.B), cout * oh * ow * planes), float("nan"), dtype=torch.bfloat16, device=dev)
-        return y, (y.view(-1)[8192:] if cs.sq else None), 0
-    n = cs.B * cout * oh * ow
-    y = torch.full((n + GUARD,), float("nan"), dtype=torch.float32, device=dev)
-    y[n:] = SENTINEL
-    return y, None, n
 
 
 @pytest.mark.gpu
