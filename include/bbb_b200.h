@@ -545,6 +545,38 @@ int bbb_mc_score_log(const float* log_outputs, const float* entropy, const float
                      float* planes, int32_t* pred, int64_t capacity, int64_t* cursor /* [2]: next index, images dropped */,
                      void* cuda_stream);
 
+/* Appends every sample's probability row of one Monte-Carlo step to a pool-long probability bank, at a device-resident
+ * cursor (active learning: BatchBALD scores a candidate against the per-sample rows of the images already chosen, so
+ * the rows must outlive the step; the exchange reduces them to moments).  logits: the step's per-sample logits
+ * [S, B, C] (the exchange's input); p_hat_s is the row the exchange uses: softmax(logits_s), or with normalized != 0
+ * softplus(logits_s) / sum softplus.  Entry i = cursor[0] + b of image b:
+ *   bank[i][c][s]         p_hat_s[b, c] rounded to the nearest tf32 value (cvt.rna), fp32 words; S_pad = S rounded up
+ *                         to 8, C_pad = the next power of two >= C; bank is [capacity][C_pad][S_pad] and its padding
+ *                         (c >= C or s >= S) is never written: the caller zeroes it once
+ *   expected_entropy[i]   (1/S) sum_s H[p_hat_s], from the fp32 p_hat_s before rounding, summed in double
+ * The cursor is bbb_mc_score_log's: the same arrival bits, dropped count (cursor[1]) and ordering rules.
+ * 1 <= S <= BBB_BANK_MAX_SAMPLES, 2 <= C <= BBB_BANK_MAX_CLASSES, B > 0, 0 <= capacity < 2^48 and non-NULL pointers,
+ * else BBB_E_INVALID. */
+enum { BBB_BANK_MAX_SAMPLES = 256, BBB_BANK_MAX_CLASSES = 128 };
+int bbb_mc_prob_log(const float* logits, int32_t S, int32_t B, int32_t C, int32_t normalized, float* bank,
+                    double* expected_entropy, int64_t capacity, int64_t* cursor /* [2]: next index, images dropped */,
+                    void* cuda_stream);
+
+/* BatchBALD's joint-entropy scores of every candidate of a probability bank (bbb_mc_prob_log's layout, S_pad / C_pad
+ * from S / C as there) against M configurations of the labels already chosen:
+ *   out[i] = sum_{m < M} omega[m] * ( -sum_{c < C} Q[m,c] log Q[m,c] ),   Q[m,c] = sum_s pt[m][s] * bank[i][c][s]
+ * pt: [M_pad][S_pad] fp32 tf32 values, M_pad = M rounded up to 64, row m a distribution over the samples; rows m >= M
+ * are read and weigh nothing (keep them finite).  omega: [M] double.  mask: [N] bytes, nonzero = out[i] = -inf
+ * (nullable).  out: [N] double.  Q is formed by tf32 wgmma with fp32 accumulation and never stored; Q <= 0 adds 0;
+ * the sums over m and c are taken in double in a fixed order, so equal inputs give equal bits.  pt and bank 16-byte
+ * aligned.  1 <= S <= BBB_BANK_MAX_SAMPLES, 2 <= C <= BBB_BANK_MAX_CLASSES, 1 <= M <= 2^20, N >= 1, else
+ * BBB_E_INVALID.  workspace: bbb_joint_entropy_workspace_bytes() bytes (0 for every accepted shape: a CTA keeps its
+ * candidates' sums to the end; NULL is then fine). */
+size_t bbb_joint_entropy_workspace_bytes(int32_t N, int32_t S, int32_t C, int32_t M);
+int bbb_joint_entropy(const float* pt, const double* omega, const uint8_t* mask, const float* bank, int32_t N,
+                      int32_t S, int32_t C, int32_t M, double* out, void* workspace, size_t workspace_bytes,
+                      void* cuda_stream);
+
 /* Peer-mapped receive buffers for bbb_mc_exchange (one process per GPU, same node): allocate locally, export a
  * 64-byte CUDA-IPC handle, ship it to the peers by any host channel (the Python side uses torch.distributed),
  * import theirs.  These five calls are the only ones in this library that allocate or synchronise. */

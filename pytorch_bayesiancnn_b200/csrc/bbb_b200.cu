@@ -15,6 +15,7 @@
 #include "conv_s4_tc.cuh"
 #include "mc_head.cuh"
 #include "score_log.cuh"
+#include "batchbald.cuh"
 
 namespace {
 
@@ -832,6 +833,55 @@ int bbb_mc_score_log(const float* log_outputs, const float* entropy, const float
     bbb::mc_score_log_kernel<<<grid, bbb::SL_THREADS, 0, (cudaStream_t)cuda_stream>>>(a);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return cuda_fail(e, "mc_score_log launch");
+    g_launches += 1;
+    return BBB_OK;
+}
+
+static int pb_pad_s(int S) { return (S + 7) / 8 * 8; }
+static int pb_pad_c(int C) { int p = 1; while (p < C) p <<= 1; return p; }
+
+int bbb_mc_prob_log(const float* logits, int32_t S, int32_t B, int32_t C, int32_t normalized, float* bank,
+                    double* expected_entropy, int64_t capacity, int64_t* cursor, void* cuda_stream) {
+    if (!logits || !bank || !expected_entropy || !cursor) return fail(BBB_E_INVALID, "NULL pointer");
+    if (S < 1 || S > BBB_BANK_MAX_SAMPLES || C < 2 || C > BBB_BANK_MAX_CLASSES || B <= 0)
+        return fail(BBB_E_INVALID, "bad S/B/C %d/%d/%d", S, B, C);
+    if (capacity < 0 || (uint64_t)capacity > bbb::SL_INDEX_MASK) return fail(BBB_E_INVALID, "bad capacity %lld", (long long)capacity);
+    bbb::ProbLogArgs a;
+    a.logits = logits; a.S = S; a.B = B; a.C = C; a.S_pad = pb_pad_s(S); a.C_pad = pb_pad_c(C);
+    a.normalized = normalized != 0; a.bank = bank; a.expected_entropy = expected_entropy; a.capacity = capacity;
+    a.cursor = (unsigned long long*)cursor;
+    int grid = (B + bbb::PB_THREADS / 32 - 1) / (bbb::PB_THREADS / 32);
+    if (grid > bbb::PB_MAX_CTAS) grid = bbb::PB_MAX_CTAS;
+    bbb::mc_prob_log_kernel<<<grid, bbb::PB_THREADS, 0, (cudaStream_t)cuda_stream>>>(a);
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return cuda_fail(e, "mc_prob_log launch");
+    g_launches += 1;
+    return BBB_OK;
+}
+
+size_t bbb_joint_entropy_workspace_bytes(int32_t N, int32_t S, int32_t C, int32_t M) {
+    (void)N; (void)S; (void)C; (void)M;
+    return 0;
+}
+
+int bbb_joint_entropy(const float* pt, const double* omega, const uint8_t* mask, const float* bank, int32_t N,
+                      int32_t S, int32_t C, int32_t M, double* out, void* workspace, size_t workspace_bytes,
+                      void* cuda_stream) {
+    (void)workspace; (void)workspace_bytes;
+    if (!pt || !omega || !bank || !out) return fail(BBB_E_INVALID, "NULL pointer");
+    if (S < 1 || S > BBB_BANK_MAX_SAMPLES || C < 2 || C > BBB_BANK_MAX_CLASSES || M < 1 || M > (1 << 20) || N < 1)
+        return fail(BBB_E_INVALID, "bad N/S/C/M %d/%d/%d/%d", N, S, C, M);
+    if (((uintptr_t)pt | (uintptr_t)bank) & 15u) return fail(BBB_E_INVALID, "pt and bank must be 16-byte aligned");
+    bbb::JointArgs a;
+    a.pt = pt; a.omega = omega; a.mask = mask; a.bank = bank; a.N = N; a.S_pad = pb_pad_s(S); a.C = C;
+    a.C_pad = pb_pad_c(C); a.M = M; a.stages = bbb::je_stages(a.S_pad); a.out = out;
+    const size_t smem = bbb::je_smem_bytes(a.S_pad, a.stages);
+    const int cand = bbb::JE_BN / a.C_pad;
+    cudaError_t e = cudaFuncSetAttribute(bbb::joint_entropy_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return cuda_fail(e, "joint_entropy smem attribute");
+    bbb::joint_entropy_kernel<<<(N + cand - 1) / cand, bbb::JE_THREADS, smem, (cudaStream_t)cuda_stream>>>(a);
+    e = cudaGetLastError();
+    if (e != cudaSuccess) return cuda_fail(e, "joint_entropy launch");
     g_launches += 1;
     return BBB_OK;
 }

@@ -27,24 +27,29 @@ struct ScoreLogArgs {
     unsigned long long* cursor;                 // [2]: next index, images dropped
 };
 
-// One warp per image, grid-stride over the batch.  The cursor protocol needs no counter of its own: every CTA takes the
-// old index and counts itself in with ONE atomicAdd of 1 << 48 on cursor[0] (index in the low 48 bits, arrivals in
-// the high 16).  The CTA that arrives last has seen every other CTA's read, so it alone writes the advanced index (with
-// the arrival bits cleared) and the dropped count; a launch that follows in stream order sees both.
+// The cursor claim of one CTA of a log launch (thread 0 of each CTA; B entries per launch).  The protocol needs no
+// counter of its own: every CTA takes the old index into base_sh and counts itself in with ONE atomicAdd of 1 << 48 on
+// cursor[0] (index in the low 48 bits, arrivals in the high 16).  The CTA that arrives last has seen every other CTA's
+// read, so it alone writes the advanced index (with the arrival bits cleared) and the dropped count; a launch that
+// follows in stream order sees both.  Shared by the score log and the probability bank (batchbald.cuh).
+__device__ __forceinline__ void log_claim(unsigned long long* cursor, long long capacity, int B,
+                                          unsigned long long& base_sh) {
+    const unsigned long long old = atomicAdd(cursor, 1ull << SL_ARRIVE_SHIFT);
+    const unsigned long long base = old & SL_INDEX_MASK;
+    base_sh = base;
+    if ((old >> SL_ARRIVE_SHIFT) == gridDim.x - 1u) {
+        const unsigned long long cap = (unsigned long long)capacity;
+        const unsigned long long fit = base >= cap ? 0ull : min(cap - base, (unsigned long long)B);
+        atomicExch(cursor, base + (unsigned long long)B);
+        cursor[1] += (unsigned long long)B - fit;
+    }
+}
+
+// One warp per image, grid-stride over the batch; the cursor as log_claim says.
 __global__ void __launch_bounds__(SL_THREADS)
 mc_score_log_kernel(const ScoreLogArgs a) {
     __shared__ unsigned long long base_sh;
-    if (threadIdx.x == 0) {
-        const unsigned long long old = atomicAdd(a.cursor, 1ull << SL_ARRIVE_SHIFT);
-        const unsigned long long base = old & SL_INDEX_MASK;
-        base_sh = base;
-        if ((old >> SL_ARRIVE_SHIFT) == gridDim.x - 1u) {
-            const unsigned long long cap = (unsigned long long)a.capacity;
-            const unsigned long long fit = base >= cap ? 0ull : min(cap - base, (unsigned long long)a.B);
-            atomicExch(a.cursor, base + (unsigned long long)a.B);
-            a.cursor[1] += (unsigned long long)a.B - fit;
-        }
-    }
+    if (threadIdx.x == 0) log_claim(a.cursor, a.capacity, a.B, base_sh);
     __syncthreads();
     const unsigned long long base = base_sh;
     const int lane = threadIdx.x & 31, nwarp = SL_THREADS / 32;

@@ -168,7 +168,7 @@ class MCForward:
                  static_inputs=None, first_replay: int = 0, fold: bool = True, overlap: bool = False, inflight: int = 1,
                  fold_group: Optional[int] = None, fold_budget: int = LAYER_FOLD_BUDGET, want_information: bool = False,
                  batch_shards: int = 1, metrics: Optional[torch.Tensor] = None, cache_prep: bool = True,
-                 score_log: Optional["ScoreLog"] = None):
+                 score_log: Optional["ScoreLog"] = None, prob_bank: Optional["ProbBank"] = None):
         """``static_inputs``: device tensors the caller fills in place (e.g. targets of its host->device copies, or a
         rotation of resident batches); one graph is captured per tensor and ``self(slot=k)`` runs the step on
         ``static_inputs[k]`` with no staging copy.  ``first_replay``: index of the first replay's noise block.
@@ -191,7 +191,10 @@ class MCForward:
         ``score_log``: a ScoreLog every step appends its B images' scores to (bbb_mc_score_log, one more kernel behind
         the exchange on the same stream): the outputs this engine computes, so ``want_uncertainty`` /
         ``want_information`` decide which planes hold numbers, and ``with_labels`` whether ``correct`` does.  Steps
-        append in call order, in every mode; the warm-up steps the constructor runs do not."""
+        append in call order, in every mode; the warm-up steps the constructor runs do not.
+        ``prob_bank``: a ProbBank every step appends its B images' per-sample probability rows to (bbb_mc_prob_log,
+        behind the exchange on the same stream, as the score log), in call order, in every mode; the warm-up steps are
+        not logged, and every output keeps its bits.  One rank only: a rank holds only its own samples."""
         if want_information and not want_uncertainty:
             raise L.EngineError("MCForward: want_information needs want_uncertainty")
         Fn._require_cuda(example_x, "MCForward")
@@ -210,6 +213,14 @@ class MCForward:
         self.score_log = self._score_log = score_log      # _score_log: the log the steps append to
         self.net, self.group = net, group
         self.dist, self.world, self.rank = _dist_info(group)
+        if prob_bank is not None:
+            if self.world > 1:
+                raise L.EngineError(f"MCForward: a prob_bank needs one rank (the group has {self.world}): a rank holds "
+                                    "only its own samples")
+            if prob_bank.device != example_x.device:
+                raise L.EngineError(f"MCForward: prob_bank is on {prob_bank.device}, the step on {example_x.device}")
+            prob_bank._require(num_ens, num_classes if num_classes is not None else net.num_classes, "MCForward")
+        self.prob_bank = self._prob_bank = prob_bank      # _prob_bank: the bank the steps append to
         if self.world > 16:
             raise L.EngineError("MCForward: at most 16 ranks (one node)")
         dev = self.dev = example_x.device
@@ -547,6 +558,8 @@ class MCForward:
         if self._score_log is not None:
             self._score_log.append(o["log_outputs"], o.get("entropy"), o.get("expected_entropy"), o.get("mutual_info"),
                                    o.get("epistemic"), self.labels_all[par] if self.labels_all is not None else None)
+        if self._prob_bank is not None:
+            self._prob_bank._launch(self.logits_all[par], self.B, bool(self.flags & L.MC_NORMALIZED))
 
     def _capture(self, warmup: int = 2):
         from .graph import _STRIDE
@@ -575,11 +588,13 @@ class MCForward:
         dev = self.dev
         side = torch.cuda.Stream(device=dev)
         side.wait_stream(torch.cuda.current_stream(dev))
-        live, live_log = self._metrics, self._score_log
+        live, live_log, live_bank = self._metrics, self._score_log, self._prob_bank
         if live is not None:
             self._metrics = torch.zeros_like(live)      # the warm-up steps do not count
         if live_log is not None:
             self._score_log = ScoreLog(dev, 0)          # nor are they logged (a log of no capacity drops them)
+        if live_bank is not None:
+            self._prob_bank = ProbBank(dev, 0, live_bank.num_ens, live_bank.num_classes)
         self._prep = self._plan_prep(self.x) if self.cache_prep else None
         with torch.cuda.stream(side):
             if self._prep is not None:              # the first prep, which the warm-up steps already read
@@ -591,7 +606,7 @@ class MCForward:
                 self._exchange(*self._chain(self.x, self.base, par=p_), par=p_)
         torch.cuda.current_stream(dev).wait_stream(side)
         torch.cuda.synchronize(dev)
-        self._metrics, self._score_log = live, live_log
+        self._metrics, self._score_log, self._prob_bank = live, live_log, live_bank
         # GEMM chain on a HIGH-priority stream, parameter preps on the (default-priority) side streams: when both have CTAs
         # pending, the chain's go first -- the preps of later layers no longer keep the first GEMM's CTAs off the SMs
         cap = torch.cuda.Stream(device=dev, priority=-1)
@@ -923,32 +938,18 @@ def read_metrics(t: torch.Tensor) -> dict:
             "bin_accuracy": [div(cor[m], cnt[m]) for m in range(nb)]}
 
 
-class ScoreLog:
-    """A data-set-long log of per-image scores on the device, appended to by the Monte-Carlo step (bbb_mc_score_log):
-    ``MCForward(..., score_log=log)`` and ``evaluate(..., score_log=log)`` add one entry per image, in step order, with
-    no host read; ``read()`` returns the entries once the data set is done.
+class _CursorLog:
+    """What a data-set-long device log shares: the two-word cursor of bbb_mc_score_log / bbb_mc_prob_log (next index,
+    images dropped) and its host reads."""
 
-    Entry i holds ``confidence`` = max_c p_bar (exp of the largest log_output; the first maximal class is ``pred``),
-    ``entropy`` = H[p_bar], ``mutual_info`` and ``expected_entropy`` (the BALD decomposition), ``epistemic`` = sum_c of
-    the epistemic variance, ``correct`` = 1.0 / 0.0 (pred == label), and ``pred`` (int32).  A score the step does not
-    compute (no ``want_uncertainty`` / ``want_information`` / labels) is NaN.  ``capacity`` entries fit; images past
-    them are counted, not written, and ``read()`` refuses a log that dropped any."""
-
-    PLANES = ("confidence", "entropy", "mutual_info", "expected_entropy", "epistemic", "correct")
-
-    def __init__(self, device, capacity: int):
+    def _init_cursor(self, device, capacity: int, what: str):
         capacity = int(capacity)
         if capacity < 0:
-            raise ValueError(f"ScoreLog: capacity must be >= 0 (got {capacity})")
+            raise ValueError(f"{what}: capacity must be >= 0 (got {capacity})")
         self.device = torch.device(device)
         if self.device.type == "cuda" and self.device.index is None:
             self.device = torch.device("cuda", torch.cuda.current_device())
         self.capacity = capacity
-        assert len(self.PLANES) == L.MC_SCORE_PLANES
-        # (one column at least: an empty tensor has no address, and the kernel takes the log's pointers even when
-        # nothing fits)
-        self._planes = torch.zeros(L.MC_SCORE_PLANES, max(1, capacity), dtype=torch.float32, device=self.device)
-        self._pred = torch.zeros(max(1, capacity), dtype=torch.int32, device=self.device)
         self._cursor = torch.zeros(2, dtype=torch.int64, device=self.device)     # next index, images dropped
 
     def reset(self):
@@ -968,13 +969,40 @@ class ScoreLog:
         """Images that did not fit (a host read of the cursor)."""
         return self._counts()[1]
 
+    def _held(self, what: str) -> int:
+        """Entries held; raises EngineError if images were dropped."""
+        n, dropped = self._counts()
+        if dropped:
+            raise L.EngineError(f"{what}: {dropped} images did not fit (capacity {self.capacity}, "
+                                f"{n + dropped} logged)")
+        return n
+
+
+class ScoreLog(_CursorLog):
+    """A data-set-long log of per-image scores on the device, appended to by the Monte-Carlo step (bbb_mc_score_log):
+    ``MCForward(..., score_log=log)`` and ``evaluate(..., score_log=log)`` add one entry per image, in step order, with
+    no host read; ``read()`` returns the entries once the data set is done.
+
+    Entry i holds ``confidence`` = max_c p_bar (exp of the largest log_output; the first maximal class is ``pred``),
+    ``entropy`` = H[p_bar], ``mutual_info`` and ``expected_entropy`` (the BALD decomposition), ``epistemic`` = sum_c of
+    the epistemic variance, ``correct`` = 1.0 / 0.0 (pred == label), and ``pred`` (int32).  A score the step does not
+    compute (no ``want_uncertainty`` / ``want_information`` / labels) is NaN.  ``capacity`` entries fit; images past
+    them are counted, not written, and ``read()`` refuses a log that dropped any."""
+
+    PLANES = ("confidence", "entropy", "mutual_info", "expected_entropy", "epistemic", "correct")
+
+    def __init__(self, device, capacity: int):
+        self._init_cursor(device, capacity, "ScoreLog")
+        assert len(self.PLANES) == L.MC_SCORE_PLANES
+        # (one column at least: an empty tensor has no address, and the kernel takes the log's pointers even when
+        # nothing fits)
+        self._planes = torch.zeros(L.MC_SCORE_PLANES, max(1, capacity), dtype=torch.float32, device=self.device)
+        self._pred = torch.zeros(max(1, capacity), dtype=torch.int32, device=self.device)
+
     def read(self) -> dict:
         """The entries logged so far: {plane name: float32 [n], "pred": int32 [n]}, copies on the log's device.  Raises
         EngineError if images were dropped.  Steps in flight must be complete first (``MCForward.wait()``)."""
-        n, dropped = self._counts()
-        if dropped:
-            raise L.EngineError(f"ScoreLog: {dropped} images did not fit (capacity {self.capacity}, "
-                                f"{n + dropped} logged)")
+        n = self._held("ScoreLog")
         out = {k: self._planes[i, :n].clone() for i, k in enumerate(self.PLANES)}
         out["pred"] = self._pred[:n].clone()
         return out
@@ -999,7 +1027,7 @@ class ScoreLog:
 
 def evaluate(net, loader, num_ens: int, train_size: float, beta_type=0.1, epoch=None, num_epochs=None, group=None,
              seed: Optional[int] = None, inflight: int = 4, batch_shards: int = 1, normalized: bool = False,
-             score_log: Optional[ScoreLog] = None) -> dict:
+             score_log: Optional[ScoreLog] = None, prob_bank: Optional["ProbBank"] = None) -> dict:
     """main_bayesian.validate_model over ``loader`` (batches of (inputs, labels)) on the engine, with calibration.
 
     Returns read_metrics' dict plus ``valid_loss`` and ``valid_acc`` as validate_model computes them: the mean over
@@ -1017,14 +1045,17 @@ def evaluate(net, loader, num_ens: int, train_size: float, beta_type=0.1, epoch=
     ``normalized``: p_hat_s is the softplus-normalised row (uncertainty_estimation.py:73-77), not the softmax.
     ``score_log``: a ScoreLog every image is appended to, in loader order (after what it already holds: ``reset()`` it
     to start over).  The engines then also compute the uncertainty and information outputs; the returned figures are
-    the same bits as without a log.  Engines are kept per log object: reuse a log from epoch to epoch."""
+    the same bits as without a log.  Engines are kept per log object: reuse a log from epoch to epoch.
+    ``prob_bank``: a ProbBank every image's per-sample probability rows are appended to, in loader order, as the score
+    log is (one rank only); the returned figures keep their bits."""
     dev = next(net.parameters()).device
     log = score_log is not None
     key = (int(num_ens), float(train_size), seed, id(group), int(inflight), int(batch_shards), bool(normalized),
-           id(score_log) if log else None)
+           id(score_log) if log else None, id(prob_bank) if prob_bank is not None else None)
     ev = _engine_cache(net, "_mc_eval").get(key)
     if ev is None:
-        ev = net.__dict__["_mc_eval"][key] = {"acc": new_metrics(dev), "engines": {}, "seed": seed, "log": score_log}
+        ev = net.__dict__["_mc_eval"][key] = {"acc": new_metrics(dev), "engines": {}, "seed": seed, "log": score_log,
+                                              "bank": prob_bank}
     acc, engines, nslots = ev["acc"], ev["engines"], max(2, int(inflight))
     cur = torch.cuda.current_stream(dev)
     acc.zero_()
@@ -1038,7 +1069,7 @@ def evaluate(net, loader, num_ens: int, train_size: float, beta_type=0.1, epoch=
             eng = MCForward(net, slots[0], num_ens, group, with_labels=True, train_size=train_size, seed=ev["seed"],
                             static_inputs=slots, first_replay=len(engines) << 16, overlap=True, inflight=inflight,
                             batch_shards=batch_shards, metrics=acc, normalized=normalized, want_uncertainty=log,
-                            want_information=log, score_log=score_log)
+                            want_information=log, score_log=score_log, prob_bank=prob_bank)
             ev["seed"] = eng.seed               # every engine draws from the same seed
             e = engines[shape] = {"eng": eng, "slots": slots, "consumed": [None] * nslots, "steps": 0,
                                   "labels": [torch.zeros(x.shape[0], dtype=torch.int64, device=dev) for _ in range(nslots)],
@@ -1184,9 +1215,11 @@ class MCTrainStep(MCForward):
     exchange, and the step holds as much as the sample loop does."""
 
     def __init__(self, net, example_x, num_ens, train_size, group=None, seed=None, batch_shards: int = 1,
-                 fold: bool = False, fold_group: Optional[int] = None, score_log=None):
+                 fold: bool = False, fold_group: Optional[int] = None, score_log=None, prob_bank=None):
         if score_log is not None:
             raise L.EngineError("MCTrainStep does not log scores: log them from MCForward or evaluate()")
+        if prob_bank is not None:
+            raise L.EngineError("MCTrainStep does not fill a prob_bank: fill it from MCForward or evaluate()")
         super().__init__(net, example_x, num_ens, group=group, with_labels=True, train_size=train_size, seed=seed,
                          graph=False, fold=False, batch_shards=batch_shards)
         self.params = [p for p in net.parameters() if p.requires_grad]
@@ -1409,3 +1442,242 @@ def detect_ood(net, in_loader, out_loader, num_ens: int, score: Optional[str] = 
     sel = {nm: selective_metrics(_score(got["in"], nm), got["in"]["correct"]) for nm in names}
     return {"in": res["in"], "ood": ood if score is None else ood[score],
             "selective": sel if score is None else sel[score], "logs": got}
+
+
+# --------------------------------------------------------------------------------------------------------------------
+# Active learning: a pool-long bank of every sample's probabilities, and BALD / BatchBALD (Kirsch et al. 2019)
+# selection on the device.
+# --------------------------------------------------------------------------------------------------------------------
+def bank_pads(num_ens: int, num_classes: int):
+    """(S_pad, C_pad) of a probability bank: S rounded up to 8 (the tf32 wgmma K step), C to the next power of two."""
+    return -(-int(num_ens) // 8) * 8, 1 << (int(num_classes) - 1).bit_length()
+
+
+class ProbBank(_CursorLog):
+    """A device-resident bank of every Monte-Carlo sample's probability row for each image of a pool, appended to by the
+    step (bbb_mc_prob_log): ``MCForward(..., prob_bank=bank)`` and ``evaluate(..., prob_bank=bank)`` add one entry per
+    image, in step order, with no host read.  It is what BatchBALD scores (``batchbald``, ``bald``, ``acquire``).
+
+    Entry i holds the S rows p_hat_s (the exchange's softmax, or softplus-normalised row with ``normalized``), rounded to
+    tf32, in ``bank[i][c][s]`` order with S padded to S_pad and C to C_pad (bank_pads; the padding is zero), and
+    ``expected_entropy`` = (1/S) sum_s H[p_hat_s] in float64.  ``capacity`` entries fit; images past them are counted,
+    not written, and ``read()`` refuses a bank that dropped any."""
+
+    def __init__(self, device, capacity: int, num_ens: int, num_classes: int):
+        num_ens, num_classes = int(num_ens), int(num_classes)
+        if not 1 <= num_ens <= L.BANK_MAX_SAMPLES:
+            raise ValueError(f"ProbBank: num_ens must be in [1, {L.BANK_MAX_SAMPLES}] (got {num_ens})")
+        if not 2 <= num_classes <= L.BANK_MAX_CLASSES:
+            raise ValueError(f"ProbBank: num_classes must be in [2, {L.BANK_MAX_CLASSES}] (got {num_classes})")
+        self._init_cursor(device, capacity, "ProbBank")
+        self.num_ens, self.num_classes = num_ens, num_classes
+        self.S_pad, self.C_pad = bank_pads(num_ens, num_classes)
+        # (one entry at least: the kernel takes the bank's pointers even when nothing fits)
+        self._probs = torch.zeros(max(1, self.capacity), self.C_pad, self.S_pad, dtype=torch.float32, device=self.device)
+        self._ee = torch.zeros(max(1, self.capacity), dtype=torch.float64, device=self.device)
+
+    def _require(self, num_ens, num_classes, what):
+        if (int(num_ens), int(num_classes)) != (self.num_ens, self.num_classes):
+            raise L.EngineError(f"{what}: the prob_bank holds {self.num_ens} samples x {self.num_classes} classes, "
+                                f"the step makes {num_ens} x {num_classes}")
+
+    def _launch(self, logits, B, normalized):
+        L.check(L.lib().bbb_mc_prob_log(Fn._ptr(logits), self.num_ens, int(B), self.num_classes, int(bool(normalized)),
+                                        Fn._ptr(self._probs), Fn._ptr(self._ee), self.capacity, Fn._ptr(self._cursor),
+                                        Fn._stream(self.device)), "bbb_mc_prob_log")
+
+    def append(self, logits, normalized: bool = False):
+        """Append the images of per-sample logits [S, B, C] (fp32 contiguous on the bank's device; bbb_mc_prob_log on
+        the current stream): probabilities from anywhere else."""
+        Fn._require_cuda(self._cursor, "ProbBank.append")
+        if not (logits.dim() == 3 and logits.shape[0] == self.num_ens and logits.shape[2] == self.num_classes
+                and logits.shape[1] >= 1 and logits.dtype == torch.float32 and logits.is_contiguous()
+                and logits.device == self.device):
+            raise L.EngineError(f"ProbBank.append: expected contiguous float32 logits [{self.num_ens}, B, "
+                                f"{self.num_classes}] on {self.device}, got {logits.dtype} {tuple(logits.shape)} on "
+                                f"{logits.device}")
+        self._launch(logits, logits.shape[1], normalized)
+
+    def read(self) -> dict:
+        """The entries so far: {"probs": float32 [n, S, C], "expected_entropy": float64 [n]}, copies on the bank's
+        device.  Raises EngineError if images were dropped.  Steps in flight must be complete first."""
+        n = self._held("ProbBank")
+        return {"probs": self._probs[:n, :self.num_classes, :self.num_ens].transpose(1, 2).contiguous(),
+                "expected_entropy": self._ee[:n].clone()}
+
+
+def batchbald_plan(num_classes: int, k: int, num_configs: int):
+    """(M, exact) of each of the k greedy rounds: round n (n labels chosen) enumerates the C^n configurations of their
+    labels while C^n <= num_configs, and draws num_configs of them after that."""
+    out = []
+    for n in range(int(k)):
+        exact = int(num_classes) ** n <= int(num_configs)
+        out.append((int(num_classes) ** n if exact else int(num_configs), exact))
+    return out
+
+
+def _tf32(x64):
+    """float64 -> the nearest tf32 value (ties away from zero, as cvt.rna) in float32 words; x >= 0 and finite."""
+    b = x64.to(torch.float32).view(torch.int32)
+    return ((b + 0x1000) & ~0x1FFF).view(torch.float32)
+
+
+def _draw(w, gen, n=None):
+    """Inverse-CDF draws from non-negative weights: one index per row of w [R, K] ([R] int64), or with w [K] n indices
+    of the one distribution ([n] int64; one cumulative sum of K words, whatever n is)."""
+    cdf = w.cumsum(-1)
+    shape = (w.shape[0], 1) if w.dim() == 2 else (n,)
+    u = torch.rand(shape, dtype=torch.float64, device=w.device, generator=gen) * cdf[..., -1:]
+    idx = torch.searchsorted(cdf, u, right=True).clamp_(max=w.shape[-1] - 1)
+    return idx[:, 0] if w.dim() == 2 else idx
+
+
+def _check_selection(bank, k, num_configs=1):
+    n = bank._held("batch selection")
+    if not 1 <= int(k) <= n:
+        raise ValueError(f"select {k} of a pool of {n}: k must be in [1, {n}]")
+    if not 1 <= int(num_configs) <= 1 << 20:
+        raise ValueError(f"num_configs must be in [1, 2^20] (got {num_configs})")
+    Fn._require_cuda(bank._cursor, "batch selection")
+    return n
+
+
+class _Scorer:
+    """bbb_joint_entropy over the first n entries of a bank, with the Pt / omega / mask / output buffers of the rounds."""
+
+    def __init__(self, bank, n, m_max):
+        dev = bank.device
+        self.bank, self.n = bank, n
+        self.pt = torch.zeros(-(-m_max // 64) * 64, bank.S_pad, dtype=torch.float32, device=dev)
+        self.omega = torch.zeros(m_max, dtype=torch.float64, device=dev)
+        self.mask = torch.zeros(n, dtype=torch.uint8, device=dev)
+        self.out = torch.empty(n, dtype=torch.float64, device=dev)
+
+    def __call__(self, pt64, omega64):
+        """out[i] for the configurations pt64 [M, S] (normalised columns) and omega64 [M], both float64."""
+        b, M = self.bank, pt64.shape[0]
+        self.pt[:M, :b.num_ens].copy_(_tf32(pt64))
+        self.pt[M:].zero_()
+        self.omega[:M].copy_(omega64)
+        L.check(L.lib().bbb_joint_entropy(Fn._ptr(self.pt), Fn._ptr(self.omega), Fn._ptr(self.mask), Fn._ptr(b._probs),
+                                          self.n, b.num_ens, b.num_classes, M, Fn._ptr(self.out), None, 0,
+                                          Fn._stream(b.device)), "bbb_joint_entropy")
+        return self.out
+
+
+def bald(bank: ProbBank, k: int) -> dict:
+    """BALD top-k: the k candidates of largest mutual information, scored by round 0 of ``batchbald`` (the same kernel).
+    Returns ``indices`` (int64 [k], by decreasing score) and ``scores`` (float64 [k]) on the host."""
+    n = _check_selection(bank, k)
+    S = bank.num_ens
+    f64 = dict(dtype=torch.float64, device=bank.device)
+    mi = _Scorer(bank, n, 1)(torch.full((1, S), 1.0 / S, **f64), torch.ones(1, **f64)) - bank._ee[:n]
+    s, i = torch.topk(mi, int(k))
+    return {"indices": i.cpu(), "scores": s.cpu()}
+
+
+def batchbald(bank: ProbBank, k: int, num_configs: int = 10000, seed: Optional[int] = None, trace: bool = False) -> dict:
+    """Greedy BatchBALD (Kirsch et al. 2019) over the entries of ``bank``: round n picks the candidate i of largest
+        a(A u {i}) = H(y_A, y_i) - sum_{j in A} E_s H[p_hat_s(y_j)] - E_s H[p_hat_s(y_i)],
+    with H(y_A, y_i) = sum_m omega_m h_m(i) + const from bbb_joint_entropy over configurations m of the labels y_A:
+    enumerated while C^n <= num_configs (omega_m = P(y_A = m), const = -sum omega log omega), else num_configs of them
+    drawn -- the first time from the exact joint, then extended ancestrally, y_a(m) ~ Q_a[m, .] -- with omega = 1/M
+    and const = -(1/M) sum_m log P(y_A(m)).  Pt's column m is P(s | y_A = m); the update between rounds runs in float64
+    torch ops on the device and the k rounds are enqueued with no host read; ``seed`` seeds the draws (same seed, same
+    bits).
+
+    Returns ``indices`` (int64 [k]) and ``scores`` (float64 [k], a(A) after each pick) on the host, and ``exact`` (per
+    round: enumerated?).  ``trace=True`` adds ``trace``: per round a dict of the device tensors ``scores`` (every
+    candidate; chosen ones -inf), ``pt`` (the tf32 Pt the kernel read, [M, S]), ``omega``, ``const`` and ``configs`` (the
+    label configurations [M, n])."""
+    n = _check_selection(bank, k, num_configs)
+    picks, scores, plan, rounds = _batchbald_rounds(bank, n, int(k), int(num_configs), seed, trace)
+    res = {"indices": picks.cpu(), "scores": scores.cpu(), "exact": [e for _, e in plan]}
+    if trace:
+        res["trace"] = rounds
+    return res
+
+
+def _batchbald_rounds(bank, n, k, num_configs, seed, trace):
+    """The k rounds of batchbald over the first n entries, enqueued on the current stream with no host read: (picks,
+    scores) as device tensors, the plan and the trace."""
+    dev, S, Cc = bank.device, bank.num_ens, bank.num_classes
+    plan = batchbald_plan(Cc, k, num_configs)
+    score = _Scorer(bank, n, max(M for M, _ in plan))
+    f64 = dict(dtype=torch.float64, device=dev)
+    gen = torch.Generator(device=dev)
+    gen.manual_seed(int(seed) if seed is not None else int(torch.randint(1 << 62, (1,)).item()))
+    eh = bank._ee[:n]
+    pt, omega, const = torch.full((1, S), 1.0 / S, **f64), torch.ones(1, **f64), torch.zeros((), **f64)
+    configs = torch.zeros(1, 0, dtype=torch.int64, device=dev)
+    log_p = None
+    eh_sum = torch.zeros((), **f64)
+    picks = torch.zeros(k, dtype=torch.int64, device=dev)
+    scores = torch.zeros(k, **f64)
+    rounds, p_a = [], None
+    for r, (M, exact) in enumerate(plan):
+        if r > 0:
+            q_a = pt @ p_a.T                                         # [M_prev, C]: P(y_a = c | y_A = m)
+            M_prev = pt.shape[0]
+            if exact:
+                col = (pt[:, None, :] * p_a[None, :, :]).reshape(M_prev * Cc, S)
+                q = q_a.reshape(-1, 1)
+                pt = torch.where(q > 0, col / torch.where(q > 0, q, 1.0), 0.0)
+                omega = (omega[:, None] * q_a).reshape(-1)
+                const = -torch.special.xlogy(omega, omega).sum()
+                configs = torch.cat([configs.repeat_interleave(Cc, 0),
+                                     torch.arange(Cc, device=dev).repeat(M_prev)[:, None]], 1)
+            else:
+                if log_p is None:                                     # first sampled round: from the exact joint
+                    joint = (omega[:, None] * q_a).reshape(-1)       # [M_prev * C]
+                    idx = _draw(joint, gen, M)
+                    m_i, c_i = idx // Cc, idx % Cc
+                    log_p = torch.log(joint.gather(0, idx))
+                else:                                                 # ancestral: y_a(m) ~ Q_a[m, .]
+                    m_i, c_i = torch.arange(M, device=dev), _draw(q_a, gen)
+                    log_p = log_p + torch.log(q_a.gather(1, c_i[:, None])[:, 0])
+                q = q_a[m_i].gather(1, c_i[:, None])
+                pt = pt[m_i] * p_a.index_select(0, c_i) / q
+                configs = torch.cat([configs[m_i], c_i[:, None]], 1)
+                omega = torch.full((M,), 1.0 / M, **f64)
+                const = -log_p.sum() / M
+        out = score(pt, omega)
+        a = out + const - eh_sum - eh
+        pick = torch.argmax(a).view(1)
+        picks[r:r + 1].copy_(pick)
+        scores[r:r + 1].copy_(a.index_select(0, pick))
+        score.mask.index_fill_(0, pick, 1)
+        eh_sum = eh_sum + eh.index_select(0, pick)[0]
+        p_a = bank._probs.index_select(0, pick)[0, :Cc, :S].to(torch.float64)       # the stored (tf32) rows
+        if trace:
+            rounds.append({"scores": a.clone(), "pt": score.pt[:M, :S].clone(), "omega": omega.clone(),
+                           "const": const.clone(), "configs": configs.clone(), "exact": exact, "M": M})
+    return picks, scores, plan, rounds
+
+
+def acquire(net, pool_loader, k: int, num_ens: int, method: str = "batchbald", num_configs: int = 10000,
+            **evaluate_kwargs) -> dict:
+    """One active-learning acquisition (Gal et al. 2017, Kirsch et al. 2019): ``evaluate`` over ``pool_loader``
+    (batches of (x, y); the labels are not used) into a ProbBank sized from the loader, then ``batchbald`` or ``bald``
+    selects k pool images.  Returns the selection's dict (``indices`` are positions in loader order) plus
+    ``evaluate`` (evaluate's figures).  ``evaluate_kwargs`` go to evaluate (``train_size`` defaults to 1.0); its
+    ``seed`` also seeds the sampled configurations.  The bank is kept on the net, as detect_ood keeps its logs."""
+    if method not in ("batchbald", "bald"):
+        raise ValueError(f"acquire: method must be 'batchbald' or 'bald' (got {method!r})")
+    dev = next(net.parameters()).device
+    kw = dict(evaluate_kwargs)
+    train_size = kw.pop("train_size", 1.0)
+    n = _loader_images(pool_loader)
+    bank = net.__dict__.get("_al_bank")
+    if bank is None or bank.capacity < n or bank.device != dev or (bank.num_ens, bank.num_classes) != \
+            (int(num_ens), int(net.num_classes)):
+        if bank is not None:                    # evaluate's engines that append to the old bank go with it
+            cache = net.__dict__.get("_mc_eval", {})
+            for key in [key for key, e in cache.items() if e.get("bank") is bank]:
+                del cache[key]
+        bank = net.__dict__["_al_bank"] = ProbBank(dev, n, num_ens, net.num_classes)
+    bank.reset()
+    m = evaluate(net, pool_loader, num_ens, train_size, prob_bank=bank, **kw)
+    sel = batchbald(bank, k, num_configs, seed=kw.get("seed")) if method == "batchbald" else bald(bank, k)
+    sel["evaluate"] = m
+    return sel

@@ -21,7 +21,9 @@ def kernels(so):
             cur = m.group(1)
             fs[cur] = []
         elif cur is not None:
-            ins = re.sub(r"/\*[0-9a-f]{4,}\*/", "", line).strip()
+            # (runs of blanks collapsed: cuobjdump pads every line to the widest instruction of the whole library, so a
+            # kernel that gains a longer instruction would shift the columns of every other one)
+            ins = re.sub(r"\s+", " ", re.sub(r"/\*[0-9a-f]{4,}\*/", "", line)).strip()
             if ins:
                 fs[cur].append(ins)
     return fs
