@@ -562,6 +562,40 @@ int bbb_mc_prob_log(const float* logits, int32_t S, int32_t B, int32_t C, int32_
                     double* expected_entropy, int64_t capacity, int64_t* cursor /* [2]: next index, images dropped */,
                     void* cuda_stream);
 
+/* Split conformal prediction (Vovk et al. 2005; Romano et al. 2020; Angelopoulos et al. 2021) behind the Monte-Carlo
+ * step: appends each image's conformity score (calibration) and its prediction set at a threshold q_hat (prediction)
+ * to a data-set-long log, at a device-resident cursor.  log_outputs [B, C] is the exchange's log p_bar (softmax
+ * average, or softplus-normalised); labels [B] int64 (nullable; a label outside [0, C) counts as none).  Image b goes to
+ * i = cursor[0] + b.  In double precision, with p_c = exp((double) log_outputs[b, c]):
+ *   order   classes sorted by log_outputs descending, ties to the smaller class index, -inf last; o(c) = 0-based
+ *           position of c, S_c = sum_{c' before c} p_c'
+ *   u       (r.x + 0.5) * 2^-32, r = philox4x32_10(counter = (i_lo, i_hi, stream_lo, stream_hi), key = seed): a
+ *           function of (seed, stream, i) only, whatever the batch size, fold, sharding or in-flight mode
+ *   E_c     BBB_CONFORMAL_LAC   1 - p_c
+ *           BBB_CONFORMAL_APS   S_c + u p_c with randomized != 0, S_c + p_c otherwise
+ *           BBB_CONFORMAL_RAPS  the APS score + lam * max(0, o(c) + 1 - k_reg)
+ *           A row that holds a NaN has E_c = NaN for every c.
+ * Outputs of entry i:
+ *   score[i]    E_y (double); NaN without a label
+ *   sets[i]     [ceil(C/32)] uint32 words: bit c of word c/32 set iff E_c <= q_hat_c (q_hat_c = qhat[c] with
+ *               qhat_per_class != 0, the class-conditional threshold, else qhat[0])
+ *   size[i]     number of classes in the set;  covered[i] 1 / 0: y in the set, -1 without a label
+ *   label[i]    y, -1 without a label
+ * qhat (device float64, 1 or C words) is read at run time: a NaN in it means no threshold yet (size = covered = -1,
+ * every word 0), so a graph captured before calibration reads the threshold written in place later.  One device
+ * function forms E_c for both the score and the set: a calibration image re-scored against q_hat is in its set
+ * exactly when its score is <= q_hat, which is what the coverage guarantee rests on.
+ * Layout: score, size, covered, label [capacity]; sets [capacity][ceil(C/32)].  The cursor is bbb_mc_score_log's: the
+ * same arrival bits, dropped count (cursor[1]) and ordering rules.
+ * B > 0, 2 <= C <= BBB_CONFORMAL_MAX_CLASSES, method one of BBB_CONFORMAL_*, lam >= 0 and finite, k_reg >= 0,
+ * 0 <= capacity < 2^48 and non-NULL pointers (labels excepted), else BBB_E_INVALID. */
+enum { BBB_CONFORMAL_LAC = 0, BBB_CONFORMAL_APS = 1, BBB_CONFORMAL_RAPS = 2, BBB_CONFORMAL_MAX_CLASSES = 1024 };
+int bbb_mc_conformal_log(const float* log_outputs, const int64_t* labels, int32_t B, int32_t C, int32_t method,
+                         int32_t randomized, double lam, int32_t k_reg, uint64_t seed, uint64_t stream,
+                         const double* qhat, int32_t qhat_per_class, double* score, int32_t* size, int32_t* covered,
+                         int32_t* label, uint32_t* sets, int64_t capacity,
+                         int64_t* cursor /* [2]: next index, images dropped */, void* cuda_stream);
+
 /* BatchBALD's joint-entropy scores of every candidate of a probability bank (bbb_mc_prob_log's layout, S_pad / C_pad
  * from S / C as there) against M configurations of the labels already chosen:
  *   out[i] = sum_{m < M} omega[m] * ( -sum_{c < C} Q[m,c] log Q[m,c] ),   Q[m,c] = sum_s pt[m][s] * bank[i][c][s]

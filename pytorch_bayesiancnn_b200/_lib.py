@@ -36,12 +36,14 @@ SYMBOLS = (
     "bbb_conv2d_forward_prior", "bbb_linear_forward_prior", "bbb_layer_forward_fused_prior", "bbb_kl_forward_prior",
     "bbb_kl_backward_prior", "bbb_kl_mc_workspace_bytes", "bbb_kl_mc_forward", "bbb_kl_mc_backward",
     "bbb_mc_graph_step", "bbb_conv2d_backward_prior", "bbb_linear_backward_prior", "bbb_mc_score_log",
-    "bbb_mc_prob_log", "bbb_joint_entropy_workspace_bytes", "bbb_joint_entropy",
+    "bbb_mc_prob_log", "bbb_joint_entropy_workspace_bytes", "bbb_joint_entropy", "bbb_mc_conformal_log",
 )
 MC_MOMENTS, MC_NORMALIZED, MC_INFO = 1, 2, 4
 MC_CAL_BINS = 15                 # BBB_MC_CAL_BINS: calibration bins of the evaluation accumulator
 MC_SCORE_PLANES = 6              # BBB_MC_SCORE_PLANES: fp32 planes of a score log (bbb_mc_score_log)
 BANK_MAX_SAMPLES, BANK_MAX_CLASSES = 256, 128      # BBB_BANK_MAX_*: a probability bank's S and C (bbb_mc_prob_log)
+CONFORMAL_LAC, CONFORMAL_APS, CONFORMAL_RAPS = 0, 1, 2   # BBB_CONFORMAL_*: conformity scores (bbb_mc_conformal_log)
+CONFORMAL_MAX_CLASSES = 1024     # BBB_CONFORMAL_MAX_CLASSES
 
 
 class LayerDesc(C.Structure):
@@ -147,6 +149,9 @@ def _bind(lib):
     lib.bbb_mc_score_log.restype = C.c_int
     lib.bbb_mc_prob_log.argtypes = [fp, i32, i32, i32, i32, fp, vp, C.c_int64, vp, vp]
     lib.bbb_mc_prob_log.restype = C.c_int
+    lib.bbb_mc_conformal_log.argtypes = [fp, vp, i32, i32, i32, i32, C.c_double, i32, u64, u64, vp, i32, vp, vp, vp,
+                                         vp, vp, C.c_int64, vp, vp]
+    lib.bbb_mc_conformal_log.restype = C.c_int
     lib.bbb_joint_entropy_workspace_bytes.argtypes = [i32, i32, i32, i32]
     lib.bbb_joint_entropy_workspace_bytes.restype = sz
     lib.bbb_joint_entropy.argtypes = [fp, vp, vp, fp, i32, i32, i32, i32, vp, vp, sz, vp]

@@ -16,6 +16,7 @@
 #include "mc_head.cuh"
 #include "score_log.cuh"
 #include "batchbald.cuh"
+#include "conformal.cuh"
 
 namespace {
 
@@ -855,6 +856,39 @@ int bbb_mc_prob_log(const float* logits, int32_t S, int32_t B, int32_t C, int32_
     bbb::mc_prob_log_kernel<<<grid, bbb::PB_THREADS, 0, (cudaStream_t)cuda_stream>>>(a);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return cuda_fail(e, "mc_prob_log launch");
+    g_launches += 1;
+    return BBB_OK;
+}
+
+int bbb_mc_conformal_log(const float* log_outputs, const int64_t* labels, int32_t B, int32_t C, int32_t method,
+                         int32_t randomized, double lam, int32_t k_reg, uint64_t seed, uint64_t stream,
+                         const double* qhat, int32_t qhat_per_class, double* score, int32_t* size, int32_t* covered,
+                         int32_t* label, uint32_t* sets, int64_t capacity, int64_t* cursor, void* cuda_stream) {
+    if (!log_outputs || !qhat || !score || !size || !covered || !label || !sets || !cursor)
+        return fail(BBB_E_INVALID, "NULL pointer");
+    if (B <= 0 || C < 2 || C > BBB_CONFORMAL_MAX_CLASSES) return fail(BBB_E_INVALID, "bad B/C %d/%d", B, C);
+    if (method != BBB_CONFORMAL_LAC && method != BBB_CONFORMAL_APS && method != BBB_CONFORMAL_RAPS)
+        return fail(BBB_E_INVALID, "bad method %d", method);
+    if (!(lam >= 0.0) || !std::isfinite(lam) || k_reg < 0) return fail(BBB_E_INVALID, "bad lam/k_reg %g/%d", lam, k_reg);
+    if (capacity < 0 || (uint64_t)capacity > bbb::SL_INDEX_MASK) return fail(BBB_E_INVALID, "bad capacity %lld", (long long)capacity);
+    bbb::ConformalArgs a;
+    a.log_outputs = log_outputs; a.labels = (const long long*)labels; a.B = B; a.C = C;
+    a.n_sort = 32;
+    while (a.n_sort < C) a.n_sort <<= 1;
+    a.method = method; a.randomized = randomized != 0; a.k_reg = k_reg; a.per_class = qhat_per_class != 0; a.lam = lam;
+    a.seed_lo = (uint32_t)seed; a.seed_hi = (uint32_t)(seed >> 32);
+    a.stream_lo = (uint32_t)stream; a.stream_hi = (uint32_t)(stream >> 32);
+    a.qhat = qhat; a.score = score; a.size = size; a.covered = covered; a.label = label; a.sets = sets;
+    a.capacity = capacity; a.cursor = (unsigned long long*)cursor;
+    // as many warps as fit in the default 48 KB of shared memory, at most CF_MAX_WARPS
+    const int per_warp = a.n_sort * 8 + bbb::CF_WORDS * 4;
+    int nwarp = 48 * 1024 / per_warp;
+    if (nwarp > bbb::CF_MAX_WARPS) nwarp = bbb::CF_MAX_WARPS;
+    int grid = (B + nwarp - 1) / nwarp;
+    if (grid > bbb::CF_MAX_CTAS) grid = bbb::CF_MAX_CTAS;
+    bbb::conformal_log_kernel<<<grid, nwarp * 32, (size_t)nwarp * per_warp, (cudaStream_t)cuda_stream>>>(a);
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return cuda_fail(e, "mc_conformal_log launch");
     g_launches += 1;
     return BBB_OK;
 }

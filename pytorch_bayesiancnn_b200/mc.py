@@ -168,7 +168,8 @@ class MCForward:
                  static_inputs=None, first_replay: int = 0, fold: bool = True, overlap: bool = False, inflight: int = 1,
                  fold_group: Optional[int] = None, fold_budget: int = LAYER_FOLD_BUDGET, want_information: bool = False,
                  batch_shards: int = 1, metrics: Optional[torch.Tensor] = None, cache_prep: bool = True,
-                 score_log: Optional["ScoreLog"] = None, prob_bank: Optional["ProbBank"] = None):
+                 score_log: Optional["ScoreLog"] = None, prob_bank: Optional["ProbBank"] = None,
+                 conformal: Optional["ConformalLog"] = None):
         """``static_inputs``: device tensors the caller fills in place (e.g. targets of its host->device copies, or a
         rotation of resident batches); one graph is captured per tensor and ``self(slot=k)`` runs the step on
         ``static_inputs[k]`` with no staging copy.  ``first_replay``: index of the first replay's noise block.
@@ -194,7 +195,11 @@ class MCForward:
         append in call order, in every mode; the warm-up steps the constructor runs do not.
         ``prob_bank``: a ProbBank every step appends its B images' per-sample probability rows to (bbb_mc_prob_log,
         behind the exchange on the same stream, as the score log), in call order, in every mode; the warm-up steps are
-        not logged, and every output keeps its bits.  One rank only: a rank holds only its own samples."""
+        not logged, and every output keeps its bits.  One rank only: a rank holds only its own samples.
+        ``conformal``: a ConformalLog every step appends its B images' conformity scores and prediction sets to
+        (bbb_mc_conformal_log, behind the exchange on the same stream, as the score log), from log_outputs and, with
+        ``with_labels``, the labels; in call order, in every mode and with any sharding (every rank holds all B rows of
+        log_outputs); the warm-up steps are not logged, and every output keeps its bits."""
         if want_information and not want_uncertainty:
             raise L.EngineError("MCForward: want_information needs want_uncertainty")
         Fn._require_cuda(example_x, "MCForward")
@@ -211,6 +216,14 @@ class MCForward:
         if score_log is not None and score_log.device != example_x.device:
             raise L.EngineError(f"MCForward: score_log is on {score_log.device}, the step on {example_x.device}")
         self.score_log = self._score_log = score_log      # _score_log: the log the steps append to
+        if conformal is not None:
+            if conformal.device != example_x.device:
+                raise L.EngineError(f"MCForward: conformal is on {conformal.device}, the step on {example_x.device}")
+            ncls = int(num_classes if num_classes is not None else net.num_classes)
+            if ncls != conformal.num_classes:
+                raise L.EngineError(f"MCForward: the conformal log holds {conformal.num_classes} classes, the step "
+                                    f"makes {ncls}")
+        self.conformal = self._conformal = conformal     # _conformal: the log the steps append to
         self.net, self.group = net, group
         self.dist, self.world, self.rank = _dist_info(group)
         if prob_bank is not None:
@@ -560,6 +573,8 @@ class MCForward:
                                    o.get("epistemic"), self.labels_all[par] if self.labels_all is not None else None)
         if self._prob_bank is not None:
             self._prob_bank._launch(self.logits_all[par], self.B, bool(self.flags & L.MC_NORMALIZED))
+        if self._conformal is not None:
+            self._conformal._launch(o["log_outputs"], self.labels_all[par] if self.labels_all is not None else None)
 
     def _capture(self, warmup: int = 2):
         from .graph import _STRIDE
@@ -588,13 +603,15 @@ class MCForward:
         dev = self.dev
         side = torch.cuda.Stream(device=dev)
         side.wait_stream(torch.cuda.current_stream(dev))
-        live, live_log, live_bank = self._metrics, self._score_log, self._prob_bank
+        live, live_log, live_bank, live_cf = self._metrics, self._score_log, self._prob_bank, self._conformal
         if live is not None:
             self._metrics = torch.zeros_like(live)      # the warm-up steps do not count
         if live_log is not None:
             self._score_log = ScoreLog(dev, 0)          # nor are they logged (a log of no capacity drops them)
         if live_bank is not None:
             self._prob_bank = ProbBank(dev, 0, live_bank.num_ens, live_bank.num_classes)
+        if live_cf is not None:
+            self._conformal = live_cf._empty()
         self._prep = self._plan_prep(self.x) if self.cache_prep else None
         with torch.cuda.stream(side):
             if self._prep is not None:              # the first prep, which the warm-up steps already read
@@ -606,7 +623,7 @@ class MCForward:
                 self._exchange(*self._chain(self.x, self.base, par=p_), par=p_)
         torch.cuda.current_stream(dev).wait_stream(side)
         torch.cuda.synchronize(dev)
-        self._metrics, self._score_log, self._prob_bank = live, live_log, live_bank
+        self._metrics, self._score_log, self._prob_bank, self._conformal = live, live_log, live_bank, live_cf
         # GEMM chain on a HIGH-priority stream, parameter preps on the (default-priority) side streams: when both have CTAs
         # pending, the chain's go first -- the preps of later layers no longer keep the first GEMM's CTAs off the SMs
         cap = torch.cuda.Stream(device=dev, priority=-1)
@@ -1027,7 +1044,8 @@ class ScoreLog(_CursorLog):
 
 def evaluate(net, loader, num_ens: int, train_size: float, beta_type=0.1, epoch=None, num_epochs=None, group=None,
              seed: Optional[int] = None, inflight: int = 4, batch_shards: int = 1, normalized: bool = False,
-             score_log: Optional[ScoreLog] = None, prob_bank: Optional["ProbBank"] = None) -> dict:
+             score_log: Optional[ScoreLog] = None, prob_bank: Optional["ProbBank"] = None,
+             conformal: Optional["ConformalLog"] = None) -> dict:
     """main_bayesian.validate_model over ``loader`` (batches of (inputs, labels)) on the engine, with calibration.
 
     Returns read_metrics' dict plus ``valid_loss`` and ``valid_acc`` as validate_model computes them: the mean over
@@ -1047,15 +1065,18 @@ def evaluate(net, loader, num_ens: int, train_size: float, beta_type=0.1, epoch=
     to start over).  The engines then also compute the uncertainty and information outputs; the returned figures are
     the same bits as without a log.  Engines are kept per log object: reuse a log from epoch to epoch.
     ``prob_bank``: a ProbBank every image's per-sample probability rows are appended to, in loader order, as the score
-    log is (one rank only); the returned figures keep their bits."""
+    log is (one rank only); the returned figures keep their bits.
+    ``conformal``: a ConformalLog every image's conformity score and prediction set are appended to, in loader order,
+    as the score log is; the returned figures keep their bits.  Engines are kept per log object."""
     dev = next(net.parameters()).device
     log = score_log is not None
     key = (int(num_ens), float(train_size), seed, id(group), int(inflight), int(batch_shards), bool(normalized),
-           id(score_log) if log else None, id(prob_bank) if prob_bank is not None else None)
+           id(score_log) if log else None, id(prob_bank) if prob_bank is not None else None,
+           id(conformal) if conformal is not None else None)
     ev = _engine_cache(net, "_mc_eval").get(key)
     if ev is None:
         ev = net.__dict__["_mc_eval"][key] = {"acc": new_metrics(dev), "engines": {}, "seed": seed, "log": score_log,
-                                              "bank": prob_bank}
+                                              "bank": prob_bank, "conformal": conformal}
     acc, engines, nslots = ev["acc"], ev["engines"], max(2, int(inflight))
     cur = torch.cuda.current_stream(dev)
     acc.zero_()
@@ -1069,7 +1090,7 @@ def evaluate(net, loader, num_ens: int, train_size: float, beta_type=0.1, epoch=
             eng = MCForward(net, slots[0], num_ens, group, with_labels=True, train_size=train_size, seed=ev["seed"],
                             static_inputs=slots, first_replay=len(engines) << 16, overlap=True, inflight=inflight,
                             batch_shards=batch_shards, metrics=acc, normalized=normalized, want_uncertainty=log,
-                            want_information=log, score_log=score_log, prob_bank=prob_bank)
+                            want_information=log, score_log=score_log, prob_bank=prob_bank, conformal=conformal)
             ev["seed"] = eng.seed               # every engine draws from the same seed
             e = engines[shape] = {"eng": eng, "slots": slots, "consumed": [None] * nslots, "steps": 0,
                                   "labels": [torch.zeros(x.shape[0], dtype=torch.int64, device=dev) for _ in range(nslots)],
@@ -1215,7 +1236,9 @@ class MCTrainStep(MCForward):
     exchange, and the step holds as much as the sample loop does."""
 
     def __init__(self, net, example_x, num_ens, train_size, group=None, seed=None, batch_shards: int = 1,
-                 fold: bool = False, fold_group: Optional[int] = None, score_log=None, prob_bank=None):
+                 fold: bool = False, fold_group: Optional[int] = None, score_log=None, prob_bank=None, conformal=None):
+        if conformal is not None:
+            raise L.EngineError("MCTrainStep does not log conformal scores: log them from MCForward or evaluate()")
         if score_log is not None:
             raise L.EngineError("MCTrainStep does not log scores: log them from MCForward or evaluate()")
         if prob_bank is not None:
@@ -1681,3 +1704,236 @@ def acquire(net, pool_loader, k: int, num_ens: int, method: str = "batchbald", n
     sel = batchbald(bank, k, num_configs, seed=kw.get("seed")) if method == "batchbald" else bald(bank, k)
     sel["evaluate"] = m
     return sel
+
+
+# --------------------------------------------------------------------------------------------------------------------
+# Split conformal prediction (Vovk et al. 2005): a coverage threshold calibrated on held-out labelled images, and
+# prediction sets that hold the true label with probability >= 1 - alpha, on the device.
+# --------------------------------------------------------------------------------------------------------------------
+CONFORMAL_METHODS = {"lac": L.CONFORMAL_LAC, "aps": L.CONFORMAL_APS, "raps": L.CONFORMAL_RAPS}
+SIZE_BINS = (("0", 0, 0), ("1", 1, 1), ("2-3", 2, 3), ("4-10", 4, 10), ("11+", 11, None))
+
+
+class ConformalLog(_CursorLog):
+    """A data-set-long log of conformity scores and prediction sets on the device, appended to by the Monte-Carlo step
+    (bbb_mc_conformal_log): ``MCForward(..., conformal=log)`` and ``evaluate(..., conformal=log)`` add one entry per
+    image, in step order, with no host read.
+
+    Entry i holds ``score`` = E_y, the conformity score of the label (float64; NaN without a label), the prediction set
+    {c : E_c <= q_hat_c} at the log's threshold (``sets``, ``size``), ``covered`` (y in the set: 1 / 0, -1 without a
+    label) and ``label`` (-1 without one).  E_c is ``method``'s score: "lac" 1 - p_c, "aps" the probability mass of
+    the classes ranked above c plus ``u`` p_c (``randomized``; p_c otherwise), "raps" the APS score plus ``lam`` *
+    max(0, rank + 1 - ``k_reg``) (include/bbb_b200.h).  ``u`` is drawn from (``seed``, ``stream``, i): logs that must
+    be independent (a calibration set and a test set) take different streams.  Until ``set_threshold`` the log has no
+    threshold (size = covered = -1, empty sets): a calibration log needs none.  ``capacity`` entries fit; images past
+    them are counted, not written, and ``read()`` refuses a log that dropped any."""
+
+    def __init__(self, device, capacity: int, num_classes: int, method: str = "aps", randomized: bool = True,
+                 lam: float = 0.0, k_reg: int = 0, seed: Optional[int] = None, stream: int = 0):
+        num_classes, lam, k_reg = int(num_classes), float(lam), int(k_reg)
+        if method not in CONFORMAL_METHODS:
+            raise ValueError(f"ConformalLog: method must be one of {tuple(CONFORMAL_METHODS)} (got {method!r})")
+        if not 2 <= num_classes <= L.CONFORMAL_MAX_CLASSES:
+            raise ValueError(f"ConformalLog: num_classes must be in [2, {L.CONFORMAL_MAX_CLASSES}] (got {num_classes})")
+        if not (math.isfinite(lam) and lam >= 0.0):
+            raise ValueError(f"ConformalLog: lam must be finite and >= 0 (got {lam})")
+        if k_reg < 0:
+            raise ValueError(f"ConformalLog: k_reg must be >= 0 (got {k_reg})")
+        if not 0 <= int(stream) < 1 << 64:
+            raise ValueError(f"ConformalLog: stream must be in [0, 2^64) (got {stream})")
+        self._init_cursor(device, capacity, "ConformalLog")
+        self.num_classes, self.method, self.randomized, self.lam, self.k_reg = num_classes, method, bool(randomized), \
+            lam, k_reg
+        self.seed = int(Fn.current_seed() if seed is None else seed) & ((1 << 64) - 1)
+        self.stream = int(stream)
+        self.words = (num_classes + 31) // 32
+        # (one entry at least: the kernel takes the log's pointers even when nothing fits)
+        n = max(1, self.capacity)
+        self._score = torch.full((n,), float("nan"), dtype=torch.float64, device=self.device)
+        self._size, self._covered, self._label = (torch.zeros(n, dtype=torch.int32, device=self.device) for _ in range(3))
+        self._sets = torch.zeros(n, self.words, dtype=torch.int32, device=self.device)      # uint32 words
+        # the threshold, per class (a scalar is written to every class): NaN = none yet; read by the kernel at run time
+        self._qhat = torch.full((num_classes,), float("nan"), dtype=torch.float64, device=self.device)
+        self._threshold = None
+
+    def _options(self):
+        return dict(method=self.method, randomized=self.randomized, lam=self.lam, k_reg=self.k_reg, seed=self.seed,
+                    stream=self.stream)
+
+    def _empty(self):
+        """A log of no capacity with the same options (what an engine's warm-up steps append to)."""
+        return ConformalLog(self.device, 0, self.num_classes, **self._options())
+
+    def _launch(self, log_outputs, labels):
+        L.check(L.lib().bbb_mc_conformal_log(
+            Fn._ptr(log_outputs), Fn._ptr(labels), int(log_outputs.shape[0]), self.num_classes,
+            CONFORMAL_METHODS[self.method], int(self.randomized), C.c_double(self.lam), self.k_reg,
+            C.c_uint64(self.seed), C.c_uint64(self.stream), Fn._ptr(self._qhat), 1, Fn._ptr(self._score),
+            Fn._ptr(self._size), Fn._ptr(self._covered), Fn._ptr(self._label), Fn._ptr(self._sets), self.capacity,
+            Fn._ptr(self._cursor), Fn._stream(self.device)), "bbb_mc_conformal_log")
+
+    def append(self, log_outputs, labels=None):
+        """Append one step's images (bbb_mc_conformal_log on the current stream): log p_bar [B, C] fp32 and optional
+        int64 labels [B], contiguous on the log's device."""
+        Fn._require_cuda(self._cursor, "ConformalLog.append")
+        B = int(log_outputs.shape[0]) if log_outputs.dim() == 2 else 0
+        for t, shape, dt in ((log_outputs, (B, self.num_classes), torch.float32), (labels, (B,), torch.int64)):
+            if t is not None and not (B >= 1 and t.device == self.device and tuple(t.shape) == shape and t.dtype == dt
+                                      and t.is_contiguous()):
+                raise L.EngineError(f"ConformalLog.append: expected a contiguous {dt} tensor of shape {shape} on "
+                                    f"{self.device}, got {t.dtype} {tuple(t.shape)} on {t.device}")
+        self._launch(log_outputs, labels)
+
+    def read(self) -> dict:
+        """The entries logged so far: {"score": float64 [n], "size", "covered", "label": int32 [n], "sets": bool
+        [n, C]}, on the log's device.  Raises EngineError if images were dropped.  Steps in flight must be complete
+        first (``MCForward.wait()``)."""
+        n = self._held("ConformalLog")
+        bit = torch.arange(32, dtype=torch.int32, device=self.device)
+        sets = ((self._sets[:n, :, None] >> bit) & 1).reshape(n, self.words * 32)[:, :self.num_classes].bool()
+        return {"score": self._score[:n].clone(), "size": self._size[:n].clone(), "covered": self._covered[:n].clone(),
+                "label": self._label[:n].clone(), "sets": sets}
+
+    def set_threshold(self, q):
+        """Set q_hat, in place (stream-ordered on the current stream; engines captured with this log read it from the
+        next step on): a scalar, or [num_classes] class-conditional thresholds (``calibrate(mondrian=True)``).  NaN
+        clears it."""
+        q = torch.as_tensor(q, dtype=torch.float64).detach().reshape(-1)
+        if q.numel() not in (1, self.num_classes):
+            raise ValueError(f"ConformalLog.set_threshold: one value or {self.num_classes} (got {q.numel()})")
+        self._qhat.copy_(q.to(self.device).expand(self.num_classes))
+        self._threshold = q.to(self.device).clone().reshape(() if q.numel() == 1 else (self.num_classes,))
+
+    @property
+    def threshold(self):
+        """The threshold last set (float64 scalar or [num_classes] tensor on the log's device), or None."""
+        return self._threshold
+
+    def calibrate(self, alpha: float, mondrian: bool = False) -> torch.Tensor:
+        """q_hat from the scores logged so far (conformal_quantile; every entry needs a label): one value, or with
+        ``mondrian`` one per class from that class's images (class-conditional coverage).  The log is not changed."""
+        r = self.read()
+        if bool((r["label"] < 0).any()):
+            raise ValueError("ConformalLog.calibrate: every calibration image needs a label")
+        return conformal_quantile(r["score"], alpha, r["label"] if mondrian else None, num_classes=self.num_classes)
+
+
+def _conformal_rank(n: int, alpha) -> int:
+    """ceil((n + 1)(1 - alpha)), exactly (alpha as its shortest decimal)."""
+    from fractions import Fraction
+    a = Fraction(repr(float(alpha)))
+    return -(-(n + 1) * (a.denominator - a.numerator) // a.denominator)
+
+
+def conformal_quantile(scores, alpha: float, classes=None, num_classes: Optional[int] = None) -> torch.Tensor:
+    """The split-conformal threshold: the ceil((n + 1)(1 - alpha))-th smallest of the n ``scores``, +inf when that rank
+    exceeds n (too few calibration images for 1 - alpha).  Sets {c : E_c <= q_hat} then cover the label of a new
+    exchangeable image with probability >= 1 - alpha.  With ``classes`` (one label per score) the rule is applied to
+    each class's scores and the result is [num_classes] (default: the largest class + 1); a class without images gets
+    +inf.  float64 on the scores' device.  NaN scores or alpha outside (0, 1) raise ValueError."""
+    alpha = float(alpha)
+    if not 0.0 < alpha < 1.0:
+        raise ValueError(f"conformal_quantile: alpha must be in (0, 1) (got {alpha})")
+    s = torch.as_tensor(scores).detach().reshape(-1).to(torch.float64)
+    if bool(torch.isnan(s).any()):
+        raise ValueError("conformal_quantile: NaN score (an image without a label?)")
+    inf = float("inf")
+    if classes is None:
+        n, k = s.numel(), _conformal_rank(s.numel(), alpha)
+        return torch.sort(s).values[k - 1] if k <= n else torch.tensor(inf, dtype=torch.float64, device=s.device)
+    cls = torch.as_tensor(classes).detach().reshape(-1).to(device=s.device, dtype=torch.int64)
+    if cls.numel() != s.numel():
+        raise ValueError(f"conformal_quantile: {s.numel()} scores but {cls.numel()} classes")
+    if num_classes is None:
+        if cls.numel() == 0:
+            raise ValueError("conformal_quantile: num_classes is needed without scores")
+        num_classes = int(cls.max()) + 1
+    if cls.numel() and (int(cls.min()) < 0 or int(cls.max()) >= num_classes):
+        raise ValueError(f"conformal_quantile: classes must be in [0, {num_classes})")
+    counts = torch.bincount(cls, minlength=num_classes)
+    ks = torch.tensor([_conformal_rank(n, alpha) for n in counts.tolist()], dtype=torch.int64, device=s.device)
+    q = torch.full((num_classes,), inf, dtype=torch.float64, device=s.device)
+    if s.numel():
+        o = torch.argsort(s, stable=True)
+        ordered = s[o][torch.argsort(cls[o], stable=True)]         # by class, then by score
+        starts = counts.cumsum(0) - counts
+        ok = ks <= counts
+        q = torch.where(ok, ordered[(starts + ks - 1).clamp(0, s.numel() - 1)], q)
+    return q
+
+
+def conformal_metrics(log_or_read) -> dict:
+    """Figures of a thresholded ConformalLog (or its ``read()`` dict): ``coverage`` (the fraction of labelled images
+    whose label is in the set), ``mean_size``, ``size_histogram`` (int64 [C + 1]: images per set size),
+    ``empty_fraction``, ``class_coverage`` (float64 [C], NaN for a class without images), ``class_count``,
+    ``min_class_coverage`` and ``size_stratified`` ({bin: {"count", "coverage"}} over set sizes 0, 1, 2-3, 4-10, 11+;
+    coverage NaN for an empty bin).  Coverage figures are over the labelled images (NaN if there are none).  A log
+    without a threshold raises ValueError."""
+    r = log_or_read.read() if isinstance(log_or_read, ConformalLog) else log_or_read
+    size, covered, label = r["size"].long(), r["covered"].long(), r["label"].long()
+    n, ncls = size.numel(), int(r["sets"].shape[1])
+    if n == 0:
+        raise ValueError("conformal_metrics: no images")
+    if bool((size < 0).any()):
+        raise ValueError("conformal_metrics: the log had no threshold (set_threshold) when these images were logged")
+    lab = covered >= 0
+    cov = covered[lab].double()
+    nan = float("nan")
+    coverage = float(cov.mean()) if cov.numel() else nan
+    count = torch.bincount(label[lab], minlength=ncls)
+    hit = torch.bincount(label[lab], weights=cov, minlength=ncls)
+    per = torch.where(count > 0, hit / count.clamp_min(1).double(), torch.full_like(hit, nan))
+    strata = {}
+    for name, lo, hi in SIZE_BINS:
+        m = (size >= lo) & ((size <= hi) if hi is not None else True)
+        ml = m & lab
+        strata[name] = {"count": int(m.sum()),
+                        "coverage": float(covered[ml].double().mean()) if bool(ml.any()) else nan}
+    return {"n": n, "coverage": coverage, "mean_size": float(size.double().mean()),
+            "size_histogram": torch.bincount(size, minlength=ncls + 1), "empty_fraction": float((size == 0).double().mean()),
+            "class_coverage": per, "class_count": count,
+            "min_class_coverage": float(per[count > 0].min()) if bool((count > 0).any()) else nan,
+            "size_stratified": strata}
+
+
+def conformal(net, cal_loader, test_loader, num_ens: int, alpha: float = 0.1, method: str = "aps",
+              randomized: bool = True, lam: float = 0.0, k_reg: int = 0, mondrian: bool = False,
+              **evaluate_kwargs) -> dict:
+    """Split conformal prediction over whole data sets: ``evaluate`` over ``cal_loader`` (batches of (x, y)) into a
+    ConformalLog, q_hat = its ``calibrate(alpha, mondrian)``, then ``evaluate`` over ``test_loader`` into a second log
+    that holds q_hat, so every test image gets its prediction set on the device as its step runs.
+
+    Returns ``qhat``, ``test`` (conformal_metrics of the test log, plus ``evaluate``: evaluate's figures on the test
+    set), ``calibration`` ({"n", "alpha", "rank", "method", "mondrian"}; rank = ceil((n + 1)(1 - alpha))), ``in``
+    (evaluate's figures on the calibration set) and ``logs`` ({"calibration": ..., "test": ...}, read() dicts).  The
+    two logs draw APS's ``u`` from two streams of one seed (evaluate's ``seed`` when given).  ``evaluate_kwargs`` go to
+    evaluate (``train_size`` defaults to 1.0).  The logs are kept on the net, as detect_ood keeps its logs."""
+    dev = next(net.parameters()).device
+    kw = dict(evaluate_kwargs)
+    train_size = kw.pop("train_size", 1.0)
+    opts = dict(method=method, randomized=bool(randomized), lam=float(lam), k_reg=int(k_reg),
+                seed=int(kw["seed"] if kw.get("seed") is not None else Fn.current_seed()) & ((1 << 64) - 1))
+    logs, res = net.__dict__.setdefault("_conformal_logs", {}), {}
+    for stream, (role, loader) in enumerate((("calibration", cal_loader), ("test", test_loader))):
+        n = _loader_images(loader)
+        log = logs.get(role)
+        if log is None or log.capacity < n or log.device != dev or log.num_classes != int(net.num_classes) or \
+                log._options() != dict(opts, stream=stream):
+            if log is not None:                     # evaluate's engines that append to the old log go with it
+                cache = net.__dict__.get("_mc_eval", {})
+                for k in [k for k, e in cache.items() if e.get("conformal") is log]:
+                    del cache[k]
+            log = logs[role] = ConformalLog(dev, n, net.num_classes, stream=stream, **opts)
+        log.reset()
+        if role == "test":
+            log.set_threshold(qhat)
+        res[role] = evaluate(net, loader, num_ens, train_size, conformal=log, **kw)
+        if role == "calibration":
+            qhat = log.calibrate(alpha, mondrian)
+    got = {role: logs[role].read() for role in ("calibration", "test")}
+    test = conformal_metrics(got["test"])
+    test["evaluate"] = res["test"]
+    n_cal = got["calibration"]["score"].numel()
+    return {"qhat": qhat, "test": test, "in": res["calibration"], "logs": got,
+            "calibration": {"n": n_cal, "alpha": float(alpha), "rank": _conformal_rank(n_cal, alpha), "method": method,
+                            "mondrian": bool(mondrian)}}
