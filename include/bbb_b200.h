@@ -596,6 +596,53 @@ int bbb_mc_conformal_log(const float* log_outputs, const int64_t* labels, int32_
                          int32_t* label, uint32_t* sets, int64_t capacity,
                          int64_t* cursor /* [2]: next index, images dropped */, void* cuda_stream);
 
+/* Routes each image to the task expert least uncertain about it (the Split-MNIST mixture:
+ * Mixtures/utils_mixture.py:119-162, predict_using_uncertainty_separate_models, and :165-187, the confidence baseline),
+ * behind the K experts' Monte-Carlo exchanges, replacing get_uncertainty_per_batch's per-image numpy loop
+ * (uncertainty_estimation.py:61-102) for every expert.  experts: a host array of K pointer tables, each the planes of
+ * one exchange: pred, epistemic, aleatoric, log_outputs [B, C] and mutual_info [B] (mutual_info may be NULL unless
+ * score == BBB_ROUTE_MUTUAL_INFO); offsets: a host array of K class offsets (NULL = e * C).  In double from the fp32
+ * planes, per image b and expert e (smaller = preferred):
+ *   BBB_ROUTE_EPISTEMIC    sum_c epistemic[b, c]                      (utils_mixture.py:137-139)
+ *   BBB_ROUTE_ALEATORIC    sum_c aleatoric[b, c]                      (:140-142)
+ *   BBB_ROUTE_BOTH         sum_c epistemic[b, c] + sum_c aleatoric[b, c]   (:143-145)
+ *   BBB_ROUTE_MUTUAL_INFO  mutual_info[b]
+ *   BBB_ROUTE_CONFIDENCE   -exp(max_c log_outputs[b, c]), NaN when the row holds a NaN   (:178, applied to p_bar)
+ * The class sums run in class order.  The routed expert e* has the smallest score; ties go to the HIGHEST index, which
+ * for K = 2 is `u2 > u1` (:152) and `max1 > max2` (:178); a NaN score is never chosen while any expert's score is a
+ * number (all NaN: e* = K - 1).  Outputs per image (each nullable): expert[b] = e*; local[b] = argmax_c pred_e*[b, c],
+ * the first maximal class, NaN never maximal, a row of NaN gives 0 (:154); pred[b] = offsets[e*] + local[b];
+ * scores[b * K + e] = (float) score.
+ * labels [B] int64 (nullable) with task = -1 are global classes: the label's task is the first expert e with
+ * offsets[e] <= y < offsets[e] + C, its local class y - offsets[e]; with task = t >= 0 they are local classes of expert
+ * t (global offsets[t] + y, valid for 0 <= y < C).  A label outside every range is invalid: counted wrong, never an index.
+ * acc (nullable; needs labels): device float64 words, bbb_mc_route_bytes() in all, zeroed by the caller.  Each launch
+ * adds one step:
+ *   [0] steps  [1] images  [2] sum_steps (local correct / B): the reference's np.mean(accs) is [2] / [0], a wrong expert
+ *   counting as correct when its local class matches  [3] global correct  [4] routed to the label's task
+ *   [5] invalid labels  [6 + e] images sent to e (set*_selected, :156-157)  [22 + e] sum of e's score over every image,
+ *   routed to e or not (total_u*, :149-150)   (e < BBB_ROUTE_MAX_EXPERTS; the words behind [38] are per-launch scratch)
+ * Sums are taken per warp, per CTA and over the CTAs in a fixed order: equal inputs give equal bits.  Launches that share
+ * an accumulator must run one after another.
+ * Log (cursor non-NULL): image b also goes to entry i = cursor[0] + b of log_expert, log_local, log_pred [capacity] and
+ * log_scores [capacity][K]; the cursor is bbb_mc_score_log's: the same arrival bits, dropped count (cursor[1]) and
+ * ordering rules.
+ * 2 <= K <= BBB_ROUTE_MAX_EXPERTS, B > 0, C > 0, score one of BBB_ROUTE_*, -1 <= task < K, offsets >= 0 with
+ * offsets[e] + C < 2^31, the planes the score reads and pred non-NULL for every expert, a log with non-NULL planes and
+ * 0 <= capacity < 2^48, else BBB_E_INVALID. */
+enum { BBB_ROUTE_EPISTEMIC = 0, BBB_ROUTE_ALEATORIC = 1, BBB_ROUTE_BOTH = 2, BBB_ROUTE_MUTUAL_INFO = 3,
+       BBB_ROUTE_CONFIDENCE = 4, BBB_ROUTE_MAX_EXPERTS = 16 };
+typedef struct bbb_route_expert {
+    const float* pred; const float* epistemic; const float* aleatoric; const float* log_outputs;   /* [B, C] */
+    const float* mutual_info;                                                                       /* [B]    */
+} bbb_route_expert;
+size_t bbb_mc_route_bytes(void);
+int bbb_mc_route(const bbb_route_expert* experts, const int32_t* offsets, int32_t K, int32_t B, int32_t C,
+                 int32_t score, const int64_t* labels, int32_t task, int32_t* expert, int32_t* local, int32_t* pred,
+                 float* scores, double* acc, int32_t* log_expert, int32_t* log_local, int32_t* log_pred,
+                 float* log_scores, int64_t capacity, int64_t* cursor /* [2]: next index, images dropped; NULL = no log */,
+                 void* cuda_stream);
+
 /* BatchBALD's joint-entropy scores of every candidate of a probability bank (bbb_mc_prob_log's layout, S_pad / C_pad
  * from S / C as there) against M configurations of the labels already chosen:
  *   out[i] = sum_{m < M} omega[m] * ( -sum_{c < C} Q[m,c] log Q[m,c] ),   Q[m,c] = sum_s pt[m][s] * bank[i][c][s]

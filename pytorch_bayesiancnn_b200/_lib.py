@@ -37,6 +37,7 @@ SYMBOLS = (
     "bbb_kl_backward_prior", "bbb_kl_mc_workspace_bytes", "bbb_kl_mc_forward", "bbb_kl_mc_backward",
     "bbb_mc_graph_step", "bbb_conv2d_backward_prior", "bbb_linear_backward_prior", "bbb_mc_score_log",
     "bbb_mc_prob_log", "bbb_joint_entropy_workspace_bytes", "bbb_joint_entropy", "bbb_mc_conformal_log",
+    "bbb_mc_route_bytes", "bbb_mc_route",
 )
 MC_MOMENTS, MC_NORMALIZED, MC_INFO = 1, 2, 4
 MC_CAL_BINS = 15                 # BBB_MC_CAL_BINS: calibration bins of the evaluation accumulator
@@ -44,6 +45,9 @@ MC_SCORE_PLANES = 6              # BBB_MC_SCORE_PLANES: fp32 planes of a score l
 BANK_MAX_SAMPLES, BANK_MAX_CLASSES = 256, 128      # BBB_BANK_MAX_*: a probability bank's S and C (bbb_mc_prob_log)
 CONFORMAL_LAC, CONFORMAL_APS, CONFORMAL_RAPS = 0, 1, 2   # BBB_CONFORMAL_*: conformity scores (bbb_mc_conformal_log)
 CONFORMAL_MAX_CLASSES = 1024     # BBB_CONFORMAL_MAX_CLASSES
+# BBB_ROUTE_*: routing scores and the largest number of experts (bbb_mc_route)
+ROUTE_EPISTEMIC, ROUTE_ALEATORIC, ROUTE_BOTH, ROUTE_MUTUAL_INFO, ROUTE_CONFIDENCE = 0, 1, 2, 3, 4
+ROUTE_MAX_EXPERTS = 16
 
 
 class LayerDesc(C.Structure):
@@ -53,6 +57,11 @@ class LayerDesc(C.Structure):
         "stride_h", "stride_w", "pad_h", "pad_w", "dil_h", "dil_w", "variant", "sample",
         "has_bias", "act_dtype", "math", "kl_convention", "epilogue_act", "pool_k", "pool_s")]
     _fields_ += [("reserved", C.c_int32 * 4), ("prior_mu", C.c_float), ("prior_sigma", C.c_float)]
+
+
+class RouteExpert(C.Structure):
+    """struct bbb_route_expert (include/bbb_b200.h): one expert's exchange planes, fp32 device pointers."""
+    _fields_ = [(n, C.c_void_p) for n in ("pred", "epistemic", "aleatoric", "log_outputs", "mutual_info")]
 
 
 class Prior(C.Structure):
@@ -152,6 +161,11 @@ def _bind(lib):
     lib.bbb_mc_conformal_log.argtypes = [fp, vp, i32, i32, i32, i32, C.c_double, i32, u64, u64, vp, i32, vp, vp, vp,
                                          vp, vp, C.c_int64, vp, vp]
     lib.bbb_mc_conformal_log.restype = C.c_int
+    lib.bbb_mc_route_bytes.argtypes = []
+    lib.bbb_mc_route_bytes.restype = sz
+    lib.bbb_mc_route.argtypes = [C.POINTER(RouteExpert), vp, i32, i32, i32, i32, vp, i32, vp, vp, vp, vp, vp, vp, vp,
+                                 vp, vp, C.c_int64, vp, vp]
+    lib.bbb_mc_route.restype = C.c_int
     lib.bbb_joint_entropy_workspace_bytes.argtypes = [i32, i32, i32, i32]
     lib.bbb_joint_entropy_workspace_bytes.restype = sz
     lib.bbb_joint_entropy.argtypes = [fp, vp, vp, fp, i32, i32, i32, i32, vp, vp, sz, vp]

@@ -17,6 +17,7 @@
 #include "score_log.cuh"
 #include "batchbald.cuh"
 #include "conformal.cuh"
+#include "route.cuh"
 
 namespace {
 
@@ -889,6 +890,46 @@ int bbb_mc_conformal_log(const float* log_outputs, const int64_t* labels, int32_
     bbb::conformal_log_kernel<<<grid, nwarp * 32, (size_t)nwarp * per_warp, (cudaStream_t)cuda_stream>>>(a);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return cuda_fail(e, "mc_conformal_log launch");
+    g_launches += 1;
+    return BBB_OK;
+}
+
+size_t bbb_mc_route_bytes(void) { return bbb::rt_acc_bytes(); }
+
+int bbb_mc_route(const bbb_route_expert* experts, const int32_t* offsets, int32_t K, int32_t B, int32_t C,
+                 int32_t score, const int64_t* labels, int32_t task, int32_t* expert, int32_t* local, int32_t* pred,
+                 float* scores, double* acc, int32_t* log_expert, int32_t* log_local, int32_t* log_pred,
+                 float* log_scores, int64_t capacity, int64_t* cursor, void* cuda_stream) {
+    if (!experts) return fail(BBB_E_INVALID, "NULL expert table");
+    if (K < 2 || K > BBB_ROUTE_MAX_EXPERTS || B <= 0 || C <= 0) return fail(BBB_E_INVALID, "bad K/B/C %d/%d/%d", K, B, C);
+    if (score < BBB_ROUTE_EPISTEMIC || score > BBB_ROUTE_CONFIDENCE) return fail(BBB_E_INVALID, "bad score %d", score);
+    if (task < -1 || task >= K) return fail(BBB_E_INVALID, "bad task %d (K = %d)", task, K);
+    if (acc && !labels) return fail(BBB_E_INVALID, "an accumulator needs labels");
+    if (cursor && (!log_expert || !log_local || !log_pred || !log_scores || capacity < 0 ||
+                   (uint64_t)capacity > bbb::SL_INDEX_MASK))
+        return fail(BBB_E_INVALID, "bad log (capacity %lld)", (long long)capacity);
+    bbb::RouteArgs a = {};
+    for (int e = 0; e < K; ++e) {
+        const bbb_route_expert& x = experts[e];
+        const bool need_epi = score == BBB_ROUTE_EPISTEMIC || score == BBB_ROUTE_BOTH;
+        const bool need_ale = score == BBB_ROUTE_ALEATORIC || score == BBB_ROUTE_BOTH;
+        if (!x.pred || (need_epi && !x.epistemic) || (need_ale && !x.aleatoric) ||
+            (score == BBB_ROUTE_MUTUAL_INFO && !x.mutual_info) || (score == BBB_ROUTE_CONFIDENCE && !x.log_outputs))
+            return fail(BBB_E_INVALID, "expert %d: a plane the score reads is NULL", e);
+        const long long off = offsets ? (long long)offsets[e] : (long long)e * C;
+        if (off < 0 || off + C > 0x7fffffffll) return fail(BBB_E_INVALID, "expert %d: bad class offset %lld", e, off);
+        a.ex[e] = x;
+        a.offset[e] = (int)off;
+    }
+    a.K = K; a.B = B; a.C = C; a.score = score; a.task = task; a.labels = (const long long*)labels;
+    a.expert = expert; a.local = local; a.pred = pred; a.scores = scores; a.acc = acc;
+    a.log_expert = log_expert; a.log_local = log_local; a.log_pred = log_pred; a.log_scores = log_scores;
+    a.capacity = capacity; a.cursor = (unsigned long long*)cursor;
+    int grid = (B + bbb::RT_WARPS - 1) / bbb::RT_WARPS;          // a function of B alone (the accumulator's sum order)
+    if (grid > bbb::RT_MAX_CTAS) grid = bbb::RT_MAX_CTAS;
+    bbb::mc_route_kernel<<<grid, bbb::RT_THREADS, 0, (cudaStream_t)cuda_stream>>>(a);
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return cuda_fail(e, "mc_route launch");
     g_launches += 1;
     return BBB_OK;
 }

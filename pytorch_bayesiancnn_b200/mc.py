@@ -1141,10 +1141,11 @@ def _pinned(e, s, x, y):
     return x, y
 
 
-def engine_forward_fn(net) -> Callable:
-    """forward_fn for a net built on the engine: draws Monte-Carlo sample j (and leaves the training stream untouched)."""
+def engine_forward_fn(net, seed: Optional[int] = None, offset: int = 0) -> Callable:
+    """forward_fn for a net built on the engine: draws Monte-Carlo sample j (and leaves the training stream untouched).
+    ``seed`` / ``offset``: Fn.mc_sample's; an engine's replay r draws sample j at offset (first_replay + r) << 20."""
     def fn(x, j):
-        with Fn.mc_sample(j), torch.no_grad():
+        with Fn.mc_sample(j, seed, offset), torch.no_grad():
             return net(x)
     return fn
 
@@ -1937,3 +1938,365 @@ def conformal(net, cal_loader, test_loader, num_ens: int, alpha: float = 0.1, me
     return {"qhat": qhat, "test": test, "in": res["calibration"], "logs": got,
             "calibration": {"n": n_cal, "alpha": float(alpha), "rank": _conformal_rank(n_cal, alpha), "method": method,
                             "mondrian": bool(mondrian)}}
+
+
+# --------------------------------------------------------------------------------------------------------------------
+# Task experts: route each image to the expert least uncertain about it (the reference's Split-MNIST mixture,
+# Mixtures/utils_mixture.py:119-187), behind the experts' own Monte-Carlo steps.
+# --------------------------------------------------------------------------------------------------------------------
+ROUTE_SCORES = ("epistemic", "aleatoric", "both", "mutual_info", "confidence")     # BBB_ROUTE_*, in enum order
+_ROUTE_ACC_WORDS = 6 + 2 * L.ROUTE_MAX_EXPERTS
+
+
+def new_route_metrics(device) -> torch.Tensor:
+    """A zeroed routing accumulator for ``ExpertStep(metrics=...)`` (bbb_mc_route_bytes of float64 words)."""
+    return torch.zeros(int(L.lib().bbb_mc_route_bytes()) // 8, dtype=torch.float64, device=device)
+
+
+def read_route_metrics(t: torch.Tensor, num_experts: int) -> dict:
+    """One host read of a routing accumulator (layout: include/bbb_b200.h, bbb_mc_route).
+
+    ``steps``, ``images``; ``accuracy`` (routed global class == label), ``local_accuracy`` (the reference's figure: the
+    mean over batches of the batch's local accuracy, in which a wrong expert counts as correct when its local class
+    matches), ``routing_accuracy`` (routed to the label's task), ``selected`` (the fraction of images sent to each
+    expert), ``total_score`` (each expert's score summed over every image) and ``invalid`` (labels outside every
+    expert's class range, counted wrong)."""
+    K = int(num_experts)
+    a = t[:_ROUTE_ACC_WORDS].cpu().tolist()
+    steps, images = int(a[0]), int(a[1])
+    div = lambda x, n: x / n if n else float("nan")
+    sel = a[6:6 + K]
+    return {"steps": steps, "images": images, "local_accuracy": div(a[2], steps), "accuracy": div(a[3], images),
+            "routing_accuracy": div(a[4], images), "invalid": int(a[5]), "selected": [div(s, images) for s in sel],
+            "selected_count": [int(s) for s in sel],
+            "total_score": a[6 + L.ROUTE_MAX_EXPERTS:6 + L.ROUTE_MAX_EXPERTS + K]}
+
+
+class RouteLog(_CursorLog):
+    """A data-set-long log of routing decisions on the device, appended to by ``ExpertStep(log=...)`` / ``route`` at
+    the score log's device cursor: per image the routed ``expert``, its ``local`` class, the global class ``pred``
+    (int32) and every expert's ``scores`` (fp32 [K]).  ``capacity`` entries fit; images past them are counted, not
+    written, and ``read()`` refuses a log that dropped any."""
+
+    def __init__(self, device, capacity: int, num_experts: int):
+        self._init_cursor(device, capacity, "RouteLog")
+        K = int(num_experts)
+        if not 2 <= K <= L.ROUTE_MAX_EXPERTS:
+            raise ValueError(f"RouteLog: num_experts must be in [2, {L.ROUTE_MAX_EXPERTS}] (got {K})")
+        self.num_experts = K
+        n = max(1, self.capacity)           # an empty tensor has no address
+        self._ints = torch.zeros(3, n, dtype=torch.int32, device=self.device)
+        self._scores = torch.zeros(n, K, dtype=torch.float32, device=self.device)
+
+    def read(self) -> dict:
+        """The entries logged so far, copies on the log's device: ``expert``, ``local``, ``pred`` int32 [n] and
+        ``scores`` float32 [n, K].  Raises EngineError if images were dropped.  Steps in flight must be complete first
+        (``ExpertStep.wait()``)."""
+        n = self._held("RouteLog")
+        return {"expert": self._ints[0, :n].clone(), "local": self._ints[1, :n].clone(),
+                "pred": self._ints[2, :n].clone(), "scores": self._scores[:n].clone()}
+
+
+def _route_offsets(offsets, K, C):
+    if offsets is None:
+        return [e * C for e in range(K)]
+    offs = [int(o) for o in offsets]
+    if len(offs) != K or any(o < 0 or o + C > _INT32_MAX for o in offs):
+        raise ValueError(f"offsets: {K} class offsets >= 0 expected (got {list(offsets)})")
+    return offs
+
+
+def _route_score(score):
+    if score not in ROUTE_SCORES:
+        raise ValueError(f"unknown routing score {score!r}: one of {ROUTE_SCORES}")
+    return ROUTE_SCORES.index(score)
+
+
+def _route_launcher(outs, score, offsets, metrics, log, result):
+    """Checks the planes and buffers of a routing launch once; returns launch(labels, task), which enqueues
+    bbb_mc_route on the current stream (labels: int64 [B] or None; task: -1 or an expert)."""
+    kind = _route_score(score)
+    K = len(outs)
+    if not 2 <= K <= L.ROUTE_MAX_EXPERTS:
+        raise L.EngineError(f"route: {K} experts; 2 to {L.ROUTE_MAX_EXPERTS} are routed")
+    p0 = outs[0]["pred"]
+    B, Cc = p0.shape
+    dev = p0.device
+    need = {"pred", {L.ROUTE_EPISTEMIC: "epistemic", L.ROUTE_ALEATORIC: "aleatoric", L.ROUTE_BOTH: "epistemic",
+                     L.ROUTE_MUTUAL_INFO: "mutual_info", L.ROUTE_CONFIDENCE: "log_outputs"}[kind]}
+    if kind == L.ROUTE_BOTH:
+        need.add("aleatoric")
+    table = (L.RouteExpert * K)()
+    for e, o in enumerate(outs):
+        for name in ("pred", "epistemic", "aleatoric", "log_outputs", "mutual_info"):
+            t = o.get(name)
+            shape = (B,) if name == "mutual_info" else (B, Cc)
+            if t is None:
+                if name in need:
+                    raise L.EngineError(f"route: expert {e} has no {name!r} plane (score {score!r})")
+                continue
+            if not (t.device == dev and tuple(t.shape) == shape and t.dtype == torch.float32 and t.is_contiguous()):
+                raise L.EngineError(f"route: expert {e}'s {name!r} must be a contiguous float32 tensor of shape "
+                                    f"{shape} on {dev}, got {t.dtype} {tuple(t.shape)} on {t.device}")
+            setattr(table[e], name, t.data_ptr())
+    offs = (C.c_int32 * K)(*_route_offsets(offsets, K, Cc))
+    if metrics is not None and not (metrics.device == dev and metrics.dtype == torch.float64 and metrics.is_contiguous()
+                                    and metrics.numel() * 8 >= int(L.lib().bbb_mc_route_bytes())):
+        raise L.EngineError(f"route: metrics must be a contiguous float64 tensor from new_route_metrics on {dev}")
+    if log is not None and (log.device != dev or log.num_experts != K):
+        raise L.EngineError(f"route: the log holds {log.num_experts} experts on {log.device}, the step {K} on {dev}")
+    for k, shape in (("expert", (B,)), ("local", (B,)), ("pred", (B,)), ("scores", (B, K))):
+        t = result[k]
+        if not (t.device == dev and tuple(t.shape) == shape and t.is_contiguous() and
+                t.dtype == (torch.float32 if k == "scores" else torch.int32)):
+            raise L.EngineError(f"route: result {k!r} has the wrong shape, type or device")
+    lg = log is not None
+    fixed = (Fn._ptr(result["expert"]), Fn._ptr(result["local"]), Fn._ptr(result["pred"]), Fn._ptr(result["scores"]))
+    logs = (Fn._ptr(log._ints[0] if lg else None), Fn._ptr(log._ints[1] if lg else None),
+            Fn._ptr(log._ints[2] if lg else None), Fn._ptr(log._scores if lg else None), log.capacity if lg else 0,
+            Fn._ptr(log._cursor if lg else None))
+    fn = L.lib().bbb_mc_route
+
+    def launch(labels, task):
+        if labels is not None and not (labels.device == dev and tuple(labels.shape) == (B,) and
+                                       labels.dtype == torch.int64 and labels.is_contiguous()):
+            raise L.EngineError(f"route: labels must be a contiguous int64 tensor of shape ({B},) on {dev}")
+        L.check(fn(table, offs, K, B, Cc, kind, Fn._ptr(labels), task, *fixed,
+                   Fn._ptr(metrics if labels is not None else None), *logs, Fn._stream(dev)), "bbb_mc_route")
+    return launch
+
+
+def _route_result(B, K, dev):
+    i32 = dict(dtype=torch.int32, device=dev)
+    return {"expert": torch.empty(B, **i32), "local": torch.empty(B, **i32), "pred": torch.empty(B, **i32),
+            "scores": torch.empty(B, K, dtype=torch.float32, device=dev)}
+
+
+def _route_task(task, K):
+    t_ = -1 if task is None else int(task)
+    if not -1 <= t_ < K:
+        raise ValueError(f"route: task must be None or in [0, {K}) (got {task})")
+    return t_
+
+
+def route_batch(outs, score: str = "epistemic", offsets=None, labels: Optional[torch.Tensor] = None,
+                task: Optional[int] = None, metrics: Optional[torch.Tensor] = None,
+                log: Optional[RouteLog] = None) -> dict:
+    """Route one batch between K experts (bbb_mc_route, on the current stream): ``outs`` are the experts' exchange
+    outputs (``MCForward.out`` dicts with ``want_uncertainty``: pred, epistemic, aleatoric, log_outputs [B, C], and
+    mutual_info [B] for ``score="mutual_info"``).  Returns ``expert``, ``local``, ``pred`` (int32 [B]) and ``scores``
+    (fp32 [B, K]).  ``labels`` (int64 [B]): global classes, or with ``task=t`` the local classes of expert t; with
+    labels the step is added to ``metrics`` (new_route_metrics).  ``log``: a RouteLog the images are appended to.
+    ``offsets``: each expert's first global class (default e * C)."""
+    _route_score(score)
+    t_ = _route_task(task, len(outs))
+    B = int(outs[0]["pred"].shape[0])
+    result = _route_result(B, len(outs), outs[0]["pred"].device)
+    _route_launcher(outs, score, offsets, metrics, log, result)(labels, t_)
+    return result
+
+
+def _check_experts(experts, device, score, offsets, group):
+    """Host checks of ExpertStep / route: (K, C, offsets)."""
+    _route_score(score)
+    K = len(experts)
+    if not 2 <= K <= L.ROUTE_MAX_EXPERTS:
+        raise L.EngineError(f"ExpertStep: {K} experts; 2 to {L.ROUTE_MAX_EXPERTS} are routed")
+    ncls = {int(net.num_classes) for net in experts}
+    if len(ncls) != 1:
+        raise L.EngineError(f"ExpertStep: the experts make different numbers of classes {sorted(ncls)}")
+    Cc = ncls.pop()
+    offs = _route_offsets(offsets, K, Cc)
+    if _dist_info(group)[1] > 1:
+        raise L.EngineError("ExpertStep: one rank only (experts on several GPUs are not supported)")
+    devs = {next(net.parameters()).device for net in experts} | {torch.device(device)}
+    if len(devs) != 1:
+        raise L.EngineError(f"ExpertStep: the experts and the input must be on one device (got {sorted(map(str, devs))})")
+    return K, Cc, offs
+
+
+class ExpertStep:
+    """``res = ExpertStep(experts, example_x, num_ens, score=...)(x, labels=None, task=None, slot=k)`` -- one Monte-Carlo
+    step of every task expert and the routing between them (the reference's predict_using_uncertainty_separate_models,
+    Mixtures/utils_mixture.py:119-162, for K experts; ``score="confidence"`` is the baseline of :165-187 on p_bar).
+
+    Each expert gets its own in-flight MCForward (``overlap=True``, ``want_uncertainty=True``, ``want_information`` for
+    ``score="mutual_info"``, the same ``normalized``, ``seed``, ``first_replay`` and input slots), so it folds, caches
+    preps and runs on the fused chain or the per-layer path exactly as it would alone, with the same output bits.  The
+    K steps of a batch are independent and run concurrently; the routing kernel (bbb_mc_route) runs on a stream of its
+    own behind the K exchanges.  Before an expert's next step its exchange waits for the last routing, which reads the
+    expert's ``out``: the layer chains of batch t+1 overlap the routing of batch t, but no exchange of t+1 overwrites
+    planes the routing of t still reads.  No host synchronisation per batch.
+
+    Returns ``expert`` (the routed expert), ``pred`` (its global class offsets[e*] + local), ``local_pred`` (int32 [B])
+    and ``scores`` (fp32 [B, K]), the same tensors every call, complete on the routing stream (``wait()``), plus
+    ``experts``: the K experts' own ``out`` dicts.  ``labels`` (int64 [B]; global classes, or with ``task=t`` the local
+    classes of expert t) add the step to ``metrics`` (new_route_metrics); ``log``: a RouteLog every step appends to.
+    ``offsets``: each expert's first global class (default e * C).  Inference only, one rank only.  As with MCForward,
+    two engines over the same layers share the layers' workspaces: ``wait()`` for one before stepping the other."""
+
+    def __init__(self, experts, example_x: torch.Tensor, num_ens: int, score: str = "epistemic",
+                 normalized: bool = False, offsets=None, group=None, seed: Optional[int] = None, static_inputs=None,
+                 first_replay: int = 0, inflight: int = 1, metrics: Optional[torch.Tensor] = None,
+                 log: Optional[RouteLog] = None):
+        experts = list(experts)
+        self.K, self.C, self.offsets = _check_experts(experts, example_x.device, score, offsets, group)
+        Fn._require_cuda(example_x, "ExpertStep")
+        if log is not None and (log.device != example_x.device or log.num_experts != self.K):
+            raise L.EngineError(f"ExpertStep: the log holds {log.num_experts} experts on {log.device}, the step "
+                                f"{self.K} on {example_x.device}")
+        self.score, self.metrics, self.log = score, metrics, log
+        self.dev = example_x.device
+        self.B = int(example_x.shape[0])
+        self.seed = int(seed if seed is not None else Fn.current_seed())
+        self.inputs = list(static_inputs) if static_inputs else [example_x.clone()]
+        self.engines = [MCForward(net, self.inputs[0], num_ens, want_uncertainty=True, normalized=normalized,
+                                  seed=self.seed, static_inputs=self.inputs, first_replay=first_replay, overlap=True,
+                                  inflight=inflight, want_information=score == "mutual_info") for net in experts]
+        self.nbuf = self.engines[0].nbuf
+        res = _route_result(self.B, self.K, self.dev)
+        self._launch = _route_launcher([e.out for e in self.engines], score, self.offsets, metrics, log, res)
+        self.out = {"expert": res["expert"], "pred": res["pred"], "local_pred": res["local"],
+                    "scores": res["scores"], "experts": [e.out for e in self.engines]}
+        self._labels = torch.zeros(self.B, dtype=torch.int64, device=self.dev)
+        lo = getattr(torch.cuda.Stream, "priority_range", lambda: (-1, 0))()
+        self.route_stream = torch.cuda.Stream(device=self.dev, priority=min(lo))
+        self._join_stream = torch.cuda.Stream(device=self.dev)
+        # one stream per expert: the K layer chains of a batch run side by side (with inflight > 1 each engine also
+        # has its own chain streams behind this one)
+        self._streams = [torch.cuda.Stream(device=self.dev, priority=-1) for _ in self.engines]
+        self._in_ready, self._route_done, self._labels_read = torch.cuda.Event(), torch.cuda.Event(), torch.cuda.Event()
+        self._consumed = [torch.cuda.Event() for _ in range(self.nbuf)]
+        self.steps = 0
+
+    def __call__(self, x: Optional[torch.Tensor] = None, labels: Optional[torch.Tensor] = None,
+                 task: Optional[int] = None, slot: int = 0) -> dict:
+        t_ = _route_task(task, self.K)
+        if labels is not None and tuple(labels.shape) != (self.B,):
+            raise ValueError(f"ExpertStep: labels must have shape ({self.B},), got {tuple(labels.shape)}")
+        cur = torch.cuda.current_stream(self.dev)
+        if x is not None:
+            # the experts read the slot in place: the last step's chains must have read it first
+            for eng in self.engines:
+                ev = eng.input_consumed()
+                if ev is not None:
+                    cur.wait_event(ev)
+            self.inputs[slot].copy_(x, non_blocking=True)
+        self._in_ready.record(cur)
+        for eng, st in zip(self.engines, self._streams):
+            if self.steps:                  # the exchange overwrites the out planes the last routing reads
+                eng.result_stream.wait_event(self._route_done)
+            st.wait_event(self._in_ready)
+            with torch.cuda.stream(st):
+                eng(slot=slot)
+        rs = self.route_stream
+        rs.wait_event(self._in_ready)
+        with torch.cuda.stream(rs):
+            if labels is not None:          # copied before the routing waits: the caller may rewrite them once consumed
+                self._labels.copy_(labels, non_blocking=True)
+                if labels.is_cuda:
+                    labels.record_stream(rs)
+            self._labels_read.record(rs)
+            for eng in self.engines:
+                rs.wait_event(eng._exch_done[eng._last])
+            self._launch(self._labels if labels is not None else None, t_)
+        self._route_done.record(rs)
+        consumed = self._consumed[self.steps % self.nbuf]
+        for eng in self.engines:
+            self._join_stream.wait_event(eng.input_consumed())
+        self._join_stream.wait_event(self._labels_read)
+        consumed.record(self._join_stream)
+        self._last_consumed = consumed
+        self.steps += 1
+        return self.out
+
+    def wait(self):
+        """Make the current stream wait for the last step's routing (and so for every expert's outputs)."""
+        if self.steps:
+            torch.cuda.current_stream(self.dev).wait_event(self._route_done)
+        return self.out
+
+    def input_consumed(self):
+        """Event after which the input slot and labels of the LAST step may be rewritten: the join of the K experts'
+        chains (and of the routing stream's copy of the labels)."""
+        return self._last_consumed if self.steps else None
+
+
+def route(experts, loader, num_ens: int, score: str = "epistemic", normalized: bool = False,
+          task: Optional[int] = None, log: bool = True, inflight: int = 4, seed: Optional[int] = None,
+          offsets=None) -> dict:
+    """predict_using_uncertainty_separate_models (Mixtures/utils_mixture.py:119-162) over ``loader`` (batches of
+    (inputs, labels)) for K task experts, on the device: every batch through an ExpertStep, one per batch shape, all
+    adding to one routing accumulator that the host reads once, at the end.  Inputs and labels go into rotating device
+    slots (pinned host slots for host batches that are not pinned), as in ``evaluate``; the steps and the accumulator
+    are kept on the first expert per option key, so the next call rebuilds nothing and draws fresh noise.
+
+    ``labels``: global classes (expert e holds [offsets[e], offsets[e] + C), default e * C), or with ``task=t`` the
+    local classes of expert t (the reference's Split-MNIST loaders of task t).  Returns ``accuracy`` (global),
+    ``local_accuracy`` (the reference's figure), ``routing_accuracy``, ``selected`` (the fraction sent to each expert),
+    ``total_score`` (per expert), ``steps`` / ``images``, and with ``log`` ``per_image``: ``expert``, ``pred`` and
+    ``scores`` on the device, in loader order.  Raises ValueError at the end if a label was outside every range."""
+    experts = list(experts)
+    dev = next(experts[0].parameters()).device
+    K = _check_experts(experts, dev, score, offsets, None)[0]
+    _route_task(task, K)
+    if dev.type != "cuda":
+        raise L.EngineError(f"route: the experts are on {dev}; the engine runs on CUDA (sm_90a) only")
+    n_img = _loader_images(loader) if log else 0
+    key = (tuple(id(e) for e in experts), int(num_ens), score, bool(normalized), int(inflight), seed,
+           None if offsets is None else tuple(int(o) for o in offsets))
+    cache = _engine_cache(experts[0], "_mc_route")
+    ent = cache.get(key)
+    if ent is not None and not all(eng._prior_guard.ok() for e in ent["engines"].values()
+                                   for eng in e["eng"].engines):
+        ent = None                          # an expert's prior or mask changed since its graphs were captured
+    if ent is None:
+        ent = cache[key] = {"acc": new_route_metrics(dev), "engines": {}, "seed": seed, "log": None}
+    if log and (ent["log"] is None or ent["log"].capacity < n_img):
+        ent["log"] = RouteLog(dev, n_img, K)
+        ent["engines"].clear()              # the steps append to the log they were built with
+    rlog = ent["log"] if log else None
+    acc, engines, nslots = ent["acc"], ent["engines"], max(2, int(inflight))
+    cur = torch.cuda.current_stream(dev)
+    acc.zero_()
+    if rlog is not None:
+        rlog.reset()
+    last = None
+    for x, y in loader:
+        shape = (tuple(x.shape), x.dtype)
+        e = engines.get(shape)
+        if e is None:
+            slots = [torch.zeros(x.shape, dtype=x.dtype, device=dev) for _ in range(nslots)]
+            eng = ExpertStep(experts, slots[0], num_ens, score=score, normalized=normalized, offsets=offsets,
+                             seed=ent["seed"], static_inputs=slots, first_replay=len(engines) << 16,
+                             inflight=inflight, metrics=acc, log=rlog)
+            ent["seed"] = eng.seed
+            e = engines[shape] = {"eng": eng, "slots": slots, "consumed": [None] * nslots, "steps": 0,
+                                  "labels": [torch.zeros(x.shape[0], dtype=torch.int64, device=dev) for _ in range(nslots)],
+                                  "pinned": [None] * nslots}
+        eng = e["eng"]
+        if last is not None and last is not eng:
+            last.wait()                         # the accumulator and the log take the steps one after another
+        s = e["steps"] % nslots
+        x, y = _pinned(e, s, x, y)
+        if e["consumed"][s] is not None:
+            cur.wait_event(e["consumed"][s])
+        e["slots"][s].copy_(x, non_blocking=True)
+        e["labels"][s].copy_(y, non_blocking=True)
+        if e["pinned"][s] is not None:
+            e["pinned"][s][2].record(cur)
+        eng(labels=e["labels"][s], task=task, slot=s)
+        e["consumed"][s] = eng.input_consumed()
+        e["steps"] += 1
+        last = eng
+    if last is None:
+        raise ValueError("route: the loader yielded no batch")
+    last.wait()
+    m = read_route_metrics(acc, K)
+    if m["invalid"]:
+        raise ValueError(f"route: {m['invalid']} labels are outside every expert's class range"
+                         + (f" (task={task}: local classes 0..{experts[0].num_classes - 1})" if task is not None else ""))
+    if rlog is not None:
+        got = rlog.read()
+        m["per_image"] = {"expert": got["expert"], "pred": got["pred"], "scores": got["scores"]}
+    return m
