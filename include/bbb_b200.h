@@ -643,6 +643,56 @@ int bbb_mc_route(const bbb_route_expert* experts, const int32_t* offsets, int32_
                  float* log_scores, int64_t capacity, int64_t* cursor /* [2]: next index, images dropped; NULL = no log */,
                  void* cuda_stream);
 
+/* Temperature scaling of the Monte-Carlo predictive (Guo et al. 2017), per sample before the softmax and the average
+ * over samples (Laves et al. 2019): p_bar_T = mean_s softmax(z_s / T).
+ *
+ * bbb_mc_logit_log appends one step's raw per-sample logits [S, B, C] (the exchange's input) and labels [B] int64
+ * (nullable: -1 is logged) to a calibration bank: image b goes to entry i = cursor[0] + b, bank[i][s][c] = logits[s][b][c]
+ * bit for bit, bank_labels[i] = labels[b].  bank is [capacity][S][C] fp32, bank_labels [capacity].  The cursor is
+ * bbb_mc_score_log's: the same arrival bits, dropped count (cursor[1]) and ordering rules.
+ * 1 <= S <= BBB_LOGIT_BANK_MAX_SAMPLES, 2 <= C <= BBB_LOGIT_BANK_MAX_CLASSES, B > 0, 0 <= capacity < 2^48 and non-NULL
+ * pointers (labels excepted), else BBB_E_INVALID.
+ *
+ * bbb_temperature_nll evaluates, in one launch over a bank of n images (cursor non-NULL: the first min(cursor[0], n) of
+ * them, and every result is NaN when cursor[1] != 0, a bank that dropped images), the mean NLL of the tempered
+ * predictive at the K temperatures T_k = exp(tau[k]) (tau: device double [K]):
+ *   nll[k] = -(1/n) sum_i log( (1/S) sum_s softmax(z_is / T_k)[y_i] )      (device double [K])
+ * Per (i, s, k) in fp32: d_c = z_c - max_c z_c, log2 p = d_y a_k - log2 sum_c exp2(d_c a_k) with
+ * a_k = (float)(log2(e) / T_k), exp2 by ex2.approx.ftz (2 ulp, results below 2^-126 flushed to 0), accurate log2f; the
+ * logmeanexp over s as an online (max, sum) in fp32; the image's term and all sums after it in double.  One warp per
+ * image, one lane per sample row: a row is read 2 ceil(K / 11) times (a max and an exponential pass per sweep of 11
+ * temperatures), lanes s >= S idle.  Sums per warp, per CTA of BBB_TEMPERATURE_CTA_IMAGES consecutive images and over
+ * the CTAs in index order: the same bits on every run.  A label outside [0, C) makes every nll NaN.
+ * Search (K_search >= 2): k* = the first minimal nll[k], k < K_search (NaN never minimal; all NaN: 0).
+ *   next_tau (nullable, device double [K_search]): the next round's grid, K_search points equally spaced on
+ *            [tau[max(k*-1, 0)], tau[min(k*+1, K_search-1)]], point k = lo + ((hi - lo) * k) / (K_search - 1) in IEEE double
+ *   BBB_TEMPERATURE_FIRST: fit[0] = nll[K_search] (the caller puts tau = 0, T = 1, there; NaN when K == K_search),
+ *            fit[2] = 1.0 when k* is an end of the grid, else 0.0
+ *   BBB_TEMPERATURE_LAST: fit[1] = nll[k*], fit[3] = tau[k*], *temperature = (float) exp(tau[k*]); but when nll[k*] >
+ *            fit[0], fit[1] = fit[0], fit[3] = 0 and *temperature = 1 (never worse than T = 1).  When either is NaN
+ *            (no fit) fit[1] = fit[3] = NaN and *temperature is left as it was, so engines that read it keep tempering
+ *            with the last good value.
+ * workspace: bbb_temperature_workspace_bytes(n, K) bytes, zeroed once by the caller (a launch leaves it zeroed again);
+ * launches that share a workspace must run one after another.  1 <= n, 1 <= S <= BBB_LOGIT_BANK_MAX_SAMPLES,
+ * 2 <= C <= BBB_LOGIT_BANK_MAX_CLASSES, 1 <= K <= BBB_TEMPERATURE_MAX_POINTS, 0 <= K_search <= K, flags only with
+ * K_search >= 2 and fit (LAST: and temperature) non-NULL, else BBB_E_INVALID.
+ *
+ * bbb_mc_temper: logits[j] <- logits[j] / *temperature for j < n, in place, by IEEE division (the bits of fp32 z / T);
+ * the temperature (device fp32) is read at run time, so a graph captured once reads a value written in place later.
+ * Launched with programmatic stream serialization: it waits for the kernel before it (the logits' producer) and the
+ * next kernel's griddepcontrol.wait waits for it.  n > 0 and non-NULL pointers, else BBB_E_INVALID. */
+enum { BBB_LOGIT_BANK_MAX_SAMPLES = 256, BBB_LOGIT_BANK_MAX_CLASSES = 1024, BBB_TEMPERATURE_MAX_POINTS = 64,
+       BBB_TEMPERATURE_CTA_IMAGES = 32, BBB_TEMPERATURE_FIRST = 1, BBB_TEMPERATURE_LAST = 2 };
+int bbb_mc_logit_log(const float* logits, const int64_t* labels, int32_t S, int32_t B, int32_t C, float* bank,
+                     int64_t* bank_labels, int64_t capacity, int64_t* cursor /* [2]: next index, images dropped */,
+                     void* cuda_stream);
+size_t bbb_temperature_workspace_bytes(int32_t n, int32_t K);
+int bbb_temperature_nll(const float* logits, const int64_t* labels, const int64_t* cursor, int32_t n, int32_t S,
+                        int32_t C, const double* tau, int32_t K, int32_t K_search, int32_t flags, double* nll,
+                        double* next_tau, double* fit /* [4] */, float* temperature, void* workspace,
+                        size_t workspace_bytes, void* cuda_stream);
+int bbb_mc_temper(float* logits, int64_t n, const float* temperature, void* cuda_stream);
+
 /* BatchBALD's joint-entropy scores of every candidate of a probability bank (bbb_mc_prob_log's layout, S_pad / C_pad
  * from S / C as there) against M configurations of the labels already chosen:
  *   out[i] = sum_{m < M} omega[m] * ( -sum_{c < C} Q[m,c] log Q[m,c] ),   Q[m,c] = sum_s pt[m][s] * bank[i][c][s]

@@ -37,7 +37,8 @@ SYMBOLS = (
     "bbb_kl_backward_prior", "bbb_kl_mc_workspace_bytes", "bbb_kl_mc_forward", "bbb_kl_mc_backward",
     "bbb_mc_graph_step", "bbb_conv2d_backward_prior", "bbb_linear_backward_prior", "bbb_mc_score_log",
     "bbb_mc_prob_log", "bbb_joint_entropy_workspace_bytes", "bbb_joint_entropy", "bbb_mc_conformal_log",
-    "bbb_mc_route_bytes", "bbb_mc_route",
+    "bbb_mc_route_bytes", "bbb_mc_route", "bbb_mc_logit_log", "bbb_temperature_workspace_bytes", "bbb_temperature_nll",
+    "bbb_mc_temper",
 )
 MC_MOMENTS, MC_NORMALIZED, MC_INFO = 1, 2, 4
 MC_CAL_BINS = 15                 # BBB_MC_CAL_BINS: calibration bins of the evaluation accumulator
@@ -48,6 +49,11 @@ CONFORMAL_MAX_CLASSES = 1024     # BBB_CONFORMAL_MAX_CLASSES
 # BBB_ROUTE_*: routing scores and the largest number of experts (bbb_mc_route)
 ROUTE_EPISTEMIC, ROUTE_ALEATORIC, ROUTE_BOTH, ROUTE_MUTUAL_INFO, ROUTE_CONFIDENCE = 0, 1, 2, 3, 4
 ROUTE_MAX_EXPERTS = 16
+# BBB_LOGIT_BANK_MAX_* / BBB_TEMPERATURE_*: a logit bank's S and C (bbb_mc_logit_log), the temperatures of one pass and
+# the images per CTA of bbb_temperature_nll, and its search flags
+LOGIT_BANK_MAX_SAMPLES, LOGIT_BANK_MAX_CLASSES = 256, 1024
+TEMPERATURE_MAX_POINTS, TEMPERATURE_CTA_IMAGES = 64, 32
+TEMPERATURE_FIRST, TEMPERATURE_LAST = 1, 2
 
 
 class LayerDesc(C.Structure):
@@ -166,6 +172,14 @@ def _bind(lib):
     lib.bbb_mc_route.argtypes = [C.POINTER(RouteExpert), vp, i32, i32, i32, i32, vp, i32, vp, vp, vp, vp, vp, vp, vp,
                                  vp, vp, C.c_int64, vp, vp]
     lib.bbb_mc_route.restype = C.c_int
+    lib.bbb_mc_logit_log.argtypes = [fp, vp, i32, i32, i32, fp, vp, C.c_int64, vp, vp]
+    lib.bbb_mc_logit_log.restype = C.c_int
+    lib.bbb_temperature_workspace_bytes.argtypes = [i32, i32]
+    lib.bbb_temperature_workspace_bytes.restype = sz
+    lib.bbb_temperature_nll.argtypes = [fp, vp, vp, i32, i32, i32, vp, i32, i32, i32, vp, vp, vp, fp, vp, sz, vp]
+    lib.bbb_temperature_nll.restype = C.c_int
+    lib.bbb_mc_temper.argtypes = [fp, C.c_int64, fp, vp]
+    lib.bbb_mc_temper.restype = C.c_int
     lib.bbb_joint_entropy_workspace_bytes.argtypes = [i32, i32, i32, i32]
     lib.bbb_joint_entropy_workspace_bytes.restype = sz
     lib.bbb_joint_entropy.argtypes = [fp, vp, vp, fp, i32, i32, i32, i32, vp, vp, sz, vp]

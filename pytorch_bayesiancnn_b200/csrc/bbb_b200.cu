@@ -18,6 +18,7 @@
 #include "batchbald.cuh"
 #include "conformal.cuh"
 #include "route.cuh"
+#include "temperature.cuh"
 
 namespace {
 
@@ -930,6 +931,73 @@ int bbb_mc_route(const bbb_route_expert* experts, const int32_t* offsets, int32_
     bbb::mc_route_kernel<<<grid, bbb::RT_THREADS, 0, (cudaStream_t)cuda_stream>>>(a);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return cuda_fail(e, "mc_route launch");
+    g_launches += 1;
+    return BBB_OK;
+}
+
+int bbb_mc_logit_log(const float* logits, const int64_t* labels, int32_t S, int32_t B, int32_t C, float* bank,
+                     int64_t* bank_labels, int64_t capacity, int64_t* cursor, void* cuda_stream) {
+    if (!logits || !bank || !bank_labels || !cursor) return fail(BBB_E_INVALID, "NULL pointer");
+    if (S < 1 || S > BBB_LOGIT_BANK_MAX_SAMPLES || C < 2 || C > BBB_LOGIT_BANK_MAX_CLASSES || B <= 0)
+        return fail(BBB_E_INVALID, "bad S/B/C %d/%d/%d", S, B, C);
+    if (capacity < 0 || (uint64_t)capacity > bbb::SL_INDEX_MASK) return fail(BBB_E_INVALID, "bad capacity %lld", (long long)capacity);
+    bbb::LogitLogArgs a;
+    a.logits = logits; a.labels = (const long long*)labels; a.S = S; a.B = B; a.C = C; a.bank = bank;
+    a.bank_labels = (long long*)bank_labels; a.capacity = capacity; a.cursor = (unsigned long long*)cursor;
+    const int grid = B < bbb::LL_MAX_CTAS ? B : bbb::LL_MAX_CTAS;
+    bbb::mc_logit_log_kernel<<<grid, bbb::LL_THREADS, 0, (cudaStream_t)cuda_stream>>>(a);
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return cuda_fail(e, "mc_logit_log launch");
+    g_launches += 1;
+    return BBB_OK;
+}
+
+size_t bbb_temperature_workspace_bytes(int32_t n, int32_t K) {
+    if (n < 1 || K < 1 || K > BBB_TEMPERATURE_MAX_POINTS) return 0;
+    const size_t grid = ((size_t)n + bbb::TN_CTA_IMAGES - 1) / bbb::TN_CTA_IMAGES;
+    return 16 + grid * (size_t)K * sizeof(double);
+}
+
+int bbb_temperature_nll(const float* logits, const int64_t* labels, const int64_t* cursor, int32_t n, int32_t S,
+                        int32_t C, const double* tau, int32_t K, int32_t K_search, int32_t flags, double* nll,
+                        double* next_tau, double* fit, float* temperature, void* workspace, size_t workspace_bytes,
+                        void* cuda_stream) {
+    if (!logits || !labels || !tau || !nll || !workspace) return fail(BBB_E_INVALID, "NULL pointer");
+    if (n < 1 || S < 1 || S > BBB_LOGIT_BANK_MAX_SAMPLES || C < 2 || C > BBB_LOGIT_BANK_MAX_CLASSES)
+        return fail(BBB_E_INVALID, "bad n/S/C %d/%d/%d", n, S, C);
+    if (K < 1 || K > BBB_TEMPERATURE_MAX_POINTS || K_search < 0 || K_search > K)
+        return fail(BBB_E_INVALID, "bad K/K_search %d/%d", K, K_search);
+    if ((flags & ~(BBB_TEMPERATURE_FIRST | BBB_TEMPERATURE_LAST)) || (flags && K_search < 2))
+        return fail(BBB_E_INVALID, "bad flags %d (K_search %d)", flags, K_search);
+    if ((flags && !fit) || ((flags & BBB_TEMPERATURE_LAST) && !temperature))
+        return fail(BBB_E_INVALID, "a search pass needs fit (and the last one temperature)");
+    if (next_tau && K_search < 2) return fail(BBB_E_INVALID, "next_tau needs K_search >= 2");
+    if (workspace_bytes < bbb_temperature_workspace_bytes(n, K))
+        return fail(BBB_E_INVALID, "workspace of %zu bytes < %zu", workspace_bytes, bbb_temperature_workspace_bytes(n, K));
+    bbb::TempNllArgs a;
+    a.logits = logits; a.labels = (const long long*)labels; a.cursor = (const long long*)cursor;
+    a.n = n; a.S = S; a.C = C; a.K = K; a.K_search = K_search;
+    a.first = (flags & BBB_TEMPERATURE_FIRST) != 0; a.last = (flags & BBB_TEMPERATURE_LAST) != 0;
+    a.tau = tau; a.nll = nll; a.next_tau = next_tau; a.fit = fit; a.temperature = temperature;
+    a.arrive = (unsigned int*)workspace; a.partials = (double*)((char*)workspace + 16);
+    const int grid = (n + bbb::TN_CTA_IMAGES - 1) / bbb::TN_CTA_IMAGES;
+    bbb::temperature_nll_kernel<<<grid, bbb::TN_THREADS, 0, (cudaStream_t)cuda_stream>>>(a);
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return cuda_fail(e, "temperature_nll launch");
+    g_launches += 1;
+    return BBB_OK;
+}
+
+int bbb_mc_temper(float* logits, int64_t n, const float* temperature, void* cuda_stream) {
+    if (!logits || !temperature) return fail(BBB_E_INVALID, "NULL pointer");
+    if (n <= 0) return fail(BBB_E_INVALID, "bad n %lld", (long long)n);
+    long long grid = (n / 4 + bbb::TP_THREADS - 1) / bbb::TP_THREADS;
+    if (grid < 1) grid = 1;
+    if (grid > bbb::TP_MAX_CTAS) grid = bbb::TP_MAX_CTAS;
+    cudaError_t e = bbb::launch_pdl(bbb::mc_temper_kernel, dim3((unsigned)grid), dim3(bbb::TP_THREADS), 0,
+                                    (cudaStream_t)cuda_stream, logits, (long long)n, temperature);
+    if (e == cudaSuccess) e = cudaGetLastError();
+    if (e != cudaSuccess) return cuda_fail(e, "mc_temper launch");
     g_launches += 1;
     return BBB_OK;
 }

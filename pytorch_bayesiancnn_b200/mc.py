@@ -169,7 +169,8 @@ class MCForward:
                  fold_group: Optional[int] = None, fold_budget: int = LAYER_FOLD_BUDGET, want_information: bool = False,
                  batch_shards: int = 1, metrics: Optional[torch.Tensor] = None, cache_prep: bool = True,
                  score_log: Optional["ScoreLog"] = None, prob_bank: Optional["ProbBank"] = None,
-                 conformal: Optional["ConformalLog"] = None):
+                 conformal: Optional["ConformalLog"] = None, logit_bank: Optional["LogitBank"] = None,
+                 temperature=None):
         """``static_inputs``: device tensors the caller fills in place (e.g. targets of its host->device copies, or a
         rotation of resident batches); one graph is captured per tensor and ``self(slot=k)`` runs the step on
         ``static_inputs[k]`` with no staging copy.  ``first_replay``: index of the first replay's noise block.
@@ -199,7 +200,15 @@ class MCForward:
         ``conformal``: a ConformalLog every step appends its B images' conformity scores and prediction sets to
         (bbb_mc_conformal_log, behind the exchange on the same stream, as the score log), from log_outputs and, with
         ``with_labels``, the labels; in call order, in every mode and with any sharding (every rank holds all B rows of
-        log_outputs); the warm-up steps are not logged, and every output keeps its bits."""
+        log_outputs); the warm-up steps are not logged, and every output keeps its bits.
+        ``logit_bank``: a LogitBank every step appends its B images' raw per-sample logits and labels to (bbb_mc_logit_log,
+        in front of the temper and the exchange, on the same stream), in call order, in every mode; the warm-up steps are
+        not logged.  One rank only.
+        ``temperature``: temper every sample's logits, z <- z / T, before the exchange (bbb_mc_temper, one more kernel per
+        step): every output -- log_outputs, pred, the uncertainty and information planes, head, metrics and the logs behind
+        the exchange -- is then that of p_bar_T = mean_s softmax(z_s / T).  A float, or a one-element fp32 tensor on the
+        step's device that the step reads at run time: a value written into it in place is read by the next step, captured
+        or not (fit_temperature(out=...)).  Not with ``normalized``."""
         if want_information and not want_uncertainty:
             raise L.EngineError("MCForward: want_information needs want_uncertainty")
         Fn._require_cuda(example_x, "MCForward")
@@ -234,6 +243,15 @@ class MCForward:
                 raise L.EngineError(f"MCForward: prob_bank is on {prob_bank.device}, the step on {example_x.device}")
             prob_bank._require(num_ens, num_classes if num_classes is not None else net.num_classes, "MCForward")
         self.prob_bank = self._prob_bank = prob_bank      # _prob_bank: the bank the steps append to
+        if logit_bank is not None:
+            if self.world > 1:
+                raise L.EngineError(f"MCForward: a logit_bank needs one rank (the group has {self.world}): a rank holds "
+                                    "only its own samples")
+            if logit_bank.device != example_x.device:
+                raise L.EngineError(f"MCForward: logit_bank is on {logit_bank.device}, the step on {example_x.device}")
+            logit_bank._require(num_ens, num_classes if num_classes is not None else net.num_classes, "MCForward")
+        self.logit_bank = self._logit_bank = logit_bank   # _logit_bank: the bank the steps append to
+        self.temperature = _temperature_tensor(temperature, example_x.device, normalized, "MCForward")
         if self.world > 16:
             raise L.EngineError("MCForward: at most 16 ranks (one node)")
         dev = self.dev = example_x.device
@@ -556,6 +574,13 @@ class MCForward:
         from .graph import _STRIDE
         o = self.out
         lib = L.lib()
+        labels = self.labels_all[par] if self.labels_all is not None else None
+        if self._logit_bank is not None:
+            self._logit_bank._launch(self.logits_all[par], labels, self.B)
+        if self.temperature is not None and self.ids:
+            z = self.logits_all[par]
+            L.check(lib.bbb_mc_temper(Fn._ptr(z), z.numel(), Fn._ptr(self.temperature), Fn._stream(self.dev)),
+                    "bbb_mc_temper")
         args = (
             Fn._ptr(self.logits_all[par]), len(self.ids), self.num_ens, self.B, self.C, kl_ptr, n_kl, self.flags,
             Fn._ptr(self.labels_all[par] if self.labels_all is not None else None), C.c_float(self.train_size), C.c_float(self.beta), self.rank, self.world, self.peers,
@@ -604,6 +629,9 @@ class MCForward:
         side = torch.cuda.Stream(device=dev)
         side.wait_stream(torch.cuda.current_stream(dev))
         live, live_log, live_bank, live_cf = self._metrics, self._score_log, self._prob_bank, self._conformal
+        live_lb = self._logit_bank
+        if live_lb is not None:
+            self._logit_bank = LogitBank(dev, 0, live_lb.num_ens, live_lb.num_classes)
         if live is not None:
             self._metrics = torch.zeros_like(live)      # the warm-up steps do not count
         if live_log is not None:
@@ -624,6 +652,7 @@ class MCForward:
         torch.cuda.current_stream(dev).wait_stream(side)
         torch.cuda.synchronize(dev)
         self._metrics, self._score_log, self._prob_bank, self._conformal = live, live_log, live_bank, live_cf
+        self._logit_bank = live_lb
         # GEMM chain on a HIGH-priority stream, parameter preps on the (default-priority) side streams: when both have CTAs
         # pending, the chain's go first -- the preps of later layers no longer keep the first GEMM's CTAs off the SMs
         cap = torch.cuda.Stream(device=dev, priority=-1)
@@ -709,6 +738,8 @@ class MCForward:
     def __call__(self, x: Optional[torch.Tensor] = None, labels: Optional[torch.Tensor] = None, slot: int = 0):
         if labels is not None and self.labels is None:
             raise L.EngineError("MCForward was built without with_labels=True")
+        if self._logit_bank is not None and self.labels is None:
+            self._logit_bank._unlabelled = True   # this step logs label -1
         if self._prior_guard is not None:
             self._prior_guard.check("MCForward")
         if self._prep_graph is not None:
@@ -1045,7 +1076,8 @@ class ScoreLog(_CursorLog):
 def evaluate(net, loader, num_ens: int, train_size: float, beta_type=0.1, epoch=None, num_epochs=None, group=None,
              seed: Optional[int] = None, inflight: int = 4, batch_shards: int = 1, normalized: bool = False,
              score_log: Optional[ScoreLog] = None, prob_bank: Optional["ProbBank"] = None,
-             conformal: Optional["ConformalLog"] = None) -> dict:
+             conformal: Optional["ConformalLog"] = None, logit_bank: Optional["LogitBank"] = None,
+             temperature=None) -> dict:
     """main_bayesian.validate_model over ``loader`` (batches of (inputs, labels)) on the engine, with calibration.
 
     Returns read_metrics' dict plus ``valid_loss`` and ``valid_acc`` as validate_model computes them: the mean over
@@ -1067,16 +1099,23 @@ def evaluate(net, loader, num_ens: int, train_size: float, beta_type=0.1, epoch=
     ``prob_bank``: a ProbBank every image's per-sample probability rows are appended to, in loader order, as the score
     log is (one rank only); the returned figures keep their bits.
     ``conformal``: a ConformalLog every image's conformity score and prediction set are appended to, in loader order,
-    as the score log is; the returned figures keep their bits.  Engines are kept per log object."""
+    as the score log is; the returned figures keep their bits.  Engines are kept per log object.
+    ``logit_bank``: a LogitBank every image's raw per-sample logits and label are appended to, in loader order (one rank
+    only; calibrate_temperature fills one); the returned figures keep their bits.
+    ``temperature``: MCForward's -- every figure, log and bank behind the exchange is that of the tempered predictive.
+    Engines are kept per temperature tensor (a float: per value), and read a value written into the tensor in place."""
     dev = next(net.parameters()).device
     log = score_log is not None
+    tkey = None if temperature is None else \
+        ("tensor", id(temperature)) if isinstance(temperature, torch.Tensor) else float(temperature)
     key = (int(num_ens), float(train_size), seed, id(group), int(inflight), int(batch_shards), bool(normalized),
            id(score_log) if log else None, id(prob_bank) if prob_bank is not None else None,
-           id(conformal) if conformal is not None else None)
+           id(conformal) if conformal is not None else None, id(logit_bank) if logit_bank is not None else None, tkey)
     ev = _engine_cache(net, "_mc_eval").get(key)
     if ev is None:
         ev = net.__dict__["_mc_eval"][key] = {"acc": new_metrics(dev), "engines": {}, "seed": seed, "log": score_log,
-                                              "bank": prob_bank, "conformal": conformal}
+                                              "bank": prob_bank, "conformal": conformal, "logit_bank": logit_bank,
+                                              "temperature": temperature}
     acc, engines, nslots = ev["acc"], ev["engines"], max(2, int(inflight))
     cur = torch.cuda.current_stream(dev)
     acc.zero_()
@@ -1090,7 +1129,8 @@ def evaluate(net, loader, num_ens: int, train_size: float, beta_type=0.1, epoch=
             eng = MCForward(net, slots[0], num_ens, group, with_labels=True, train_size=train_size, seed=ev["seed"],
                             static_inputs=slots, first_replay=len(engines) << 16, overlap=True, inflight=inflight,
                             batch_shards=batch_shards, metrics=acc, normalized=normalized, want_uncertainty=log,
-                            want_information=log, score_log=score_log, prob_bank=prob_bank, conformal=conformal)
+                            want_information=log, score_log=score_log, prob_bank=prob_bank, conformal=conformal,
+                            logit_bank=logit_bank, temperature=temperature)
             ev["seed"] = eng.seed               # every engine draws from the same seed
             e = engines[shape] = {"eng": eng, "slots": slots, "consumed": [None] * nslots, "steps": 0,
                                   "labels": [torch.zeros(x.shape[0], dtype=torch.int64, device=dev) for _ in range(nslots)],
@@ -1237,7 +1277,13 @@ class MCTrainStep(MCForward):
     exchange, and the step holds as much as the sample loop does."""
 
     def __init__(self, net, example_x, num_ens, train_size, group=None, seed=None, batch_shards: int = 1,
-                 fold: bool = False, fold_group: Optional[int] = None, score_log=None, prob_bank=None, conformal=None):
+                 fold: bool = False, fold_group: Optional[int] = None, score_log=None, prob_bank=None, conformal=None,
+                 logit_bank=None, temperature=None):
+        if temperature is not None:
+            raise L.EngineError("MCTrainStep does not temper: a temperature is fitted after training "
+                                "(fit_temperature) and applied by MCForward or evaluate()")
+        if logit_bank is not None:
+            raise L.EngineError("MCTrainStep does not fill a logit_bank: fill it from MCForward or evaluate()")
         if conformal is not None:
             raise L.EngineError("MCTrainStep does not log conformal scores: log them from MCForward or evaluate()")
         if score_log is not None:
@@ -2132,15 +2178,18 @@ class ExpertStep:
     and ``scores`` (fp32 [B, K]), the same tensors every call, complete on the routing stream (``wait()``), plus
     ``experts``: the K experts' own ``out`` dicts.  ``labels`` (int64 [B]; global classes, or with ``task=t`` the local
     classes of expert t) add the step to ``metrics`` (new_route_metrics); ``log``: a RouteLog every step appends to.
+    ``temperatures``: one per expert (MCForward's ``temperature``; None: that expert is not tempered), so experts
+    calibrated one by one route on comparable uncertainty scores.
     ``offsets``: each expert's first global class (default e * C).  Inference only, one rank only.  As with MCForward,
     two engines over the same layers share the layers' workspaces: ``wait()`` for one before stepping the other."""
 
     def __init__(self, experts, example_x: torch.Tensor, num_ens: int, score: str = "epistemic",
                  normalized: bool = False, offsets=None, group=None, seed: Optional[int] = None, static_inputs=None,
                  first_replay: int = 0, inflight: int = 1, metrics: Optional[torch.Tensor] = None,
-                 log: Optional[RouteLog] = None):
+                 log: Optional[RouteLog] = None, temperatures=None):
         experts = list(experts)
         self.K, self.C, self.offsets = _check_experts(experts, example_x.device, score, offsets, group)
+        temps = _expert_temperatures(temperatures, self.K)
         Fn._require_cuda(example_x, "ExpertStep")
         if log is not None and (log.device != example_x.device or log.num_experts != self.K):
             raise L.EngineError(f"ExpertStep: the log holds {log.num_experts} experts on {log.device}, the step "
@@ -2152,7 +2201,8 @@ class ExpertStep:
         self.inputs = list(static_inputs) if static_inputs else [example_x.clone()]
         self.engines = [MCForward(net, self.inputs[0], num_ens, want_uncertainty=True, normalized=normalized,
                                   seed=self.seed, static_inputs=self.inputs, first_replay=first_replay, overlap=True,
-                                  inflight=inflight, want_information=score == "mutual_info") for net in experts]
+                                  inflight=inflight, want_information=score == "mutual_info", temperature=t)
+                        for net, t in zip(experts, temps)]
         self.nbuf = self.engines[0].nbuf
         res = _route_result(self.B, self.K, self.dev)
         self._launch = _route_launcher([e.out for e in self.engines], score, self.offsets, metrics, log, res)
@@ -2224,7 +2274,7 @@ class ExpertStep:
 
 def route(experts, loader, num_ens: int, score: str = "epistemic", normalized: bool = False,
           task: Optional[int] = None, log: bool = True, inflight: int = 4, seed: Optional[int] = None,
-          offsets=None) -> dict:
+          offsets=None, temperatures=None) -> dict:
     """predict_using_uncertainty_separate_models (Mixtures/utils_mixture.py:119-162) over ``loader`` (batches of
     (inputs, labels)) for K task experts, on the device: every batch through an ExpertStep, one per batch shape, all
     adding to one routing accumulator that the host reads once, at the end.  Inputs and labels go into rotating device
@@ -2235,7 +2285,8 @@ def route(experts, loader, num_ens: int, score: str = "epistemic", normalized: b
     local classes of expert t (the reference's Split-MNIST loaders of task t).  Returns ``accuracy`` (global),
     ``local_accuracy`` (the reference's figure), ``routing_accuracy``, ``selected`` (the fraction sent to each expert),
     ``total_score`` (per expert), ``steps`` / ``images``, and with ``log`` ``per_image``: ``expert``, ``pred`` and
-    ``scores`` on the device, in loader order.  Raises ValueError at the end if a label was outside every range."""
+    ``scores`` on the device, in loader order.  ``temperatures``: ExpertStep's, one per expert.  Raises ValueError at
+    the end if a label was outside every range."""
     experts = list(experts)
     dev = next(experts[0].parameters()).device
     K = _check_experts(experts, dev, score, offsets, None)[0]
@@ -2243,15 +2294,18 @@ def route(experts, loader, num_ens: int, score: str = "epistemic", normalized: b
     if dev.type != "cuda":
         raise L.EngineError(f"route: the experts are on {dev}; the engine runs on CUDA (sm_90a) only")
     n_img = _loader_images(loader) if log else 0
+    temps = _expert_temperatures(temperatures, K)
     key = (tuple(id(e) for e in experts), int(num_ens), score, bool(normalized), int(inflight), seed,
-           None if offsets is None else tuple(int(o) for o in offsets))
+           None if offsets is None else tuple(int(o) for o in offsets),
+           tuple(None if t is None else ("tensor", id(t)) if isinstance(t, torch.Tensor) else float(t) for t in temps))
     cache = _engine_cache(experts[0], "_mc_route")
     ent = cache.get(key)
     if ent is not None and not all(eng._prior_guard.ok() for e in ent["engines"].values()
                                    for eng in e["eng"].engines):
         ent = None                          # an expert's prior or mask changed since its graphs were captured
     if ent is None:
-        ent = cache[key] = {"acc": new_route_metrics(dev), "engines": {}, "seed": seed, "log": None}
+        ent = cache[key] = {"acc": new_route_metrics(dev), "engines": {}, "seed": seed, "log": None,
+                            "temperatures": temps}
     if log and (ent["log"] is None or ent["log"].capacity < n_img):
         ent["log"] = RouteLog(dev, n_img, K)
         ent["engines"].clear()              # the steps append to the log they were built with
@@ -2269,7 +2323,7 @@ def route(experts, loader, num_ens: int, score: str = "epistemic", normalized: b
             slots = [torch.zeros(x.shape, dtype=x.dtype, device=dev) for _ in range(nslots)]
             eng = ExpertStep(experts, slots[0], num_ens, score=score, normalized=normalized, offsets=offsets,
                              seed=ent["seed"], static_inputs=slots, first_replay=len(engines) << 16,
-                             inflight=inflight, metrics=acc, log=rlog)
+                             inflight=inflight, metrics=acc, log=rlog, temperatures=temps)
             ent["seed"] = eng.seed
             e = engines[shape] = {"eng": eng, "slots": slots, "consumed": [None] * nslots, "steps": 0,
                                   "labels": [torch.zeros(x.shape[0], dtype=torch.int64, device=dev) for _ in range(nslots)],
@@ -2300,3 +2354,252 @@ def route(experts, loader, num_ens: int, score: str = "epistemic", normalized: b
         got = rlog.read()
         m["per_image"] = {"expert": got["expert"], "pred": got["pred"], "scores": got["scores"]}
     return m
+
+
+# --------------------------------------------------------------------------------------------------------------------
+# Temperature scaling (Guo et al. 2017) of the Monte-Carlo predictive, on each sample's logits before the softmax and
+# the average over samples (Laves et al. 2019): p_bar_T = mean_s softmax(z_s / T).  A calibration bank of raw
+# per-sample logits, a grid search for T on the device, and the temper in front of the exchange.
+# --------------------------------------------------------------------------------------------------------------------
+def _temperature_tensor(t, device, normalized, what):
+    """MCForward's ``temperature`` as the one-element fp32 device tensor the temper reads (a tensor is used as given)."""
+    if t is None:
+        return None
+    if normalized:
+        raise ValueError(f"{what}: a temperature tempers the softmax predictive; the softplus-normalised one "
+                         "(normalized=True) takes none")
+    device = torch.device(device)
+    if isinstance(t, torch.Tensor):
+        if not (t.dtype == torch.float32 and t.numel() == 1 and t.device == device and t.is_contiguous()):
+            raise L.EngineError(f"{what}: temperature must be a contiguous one-element float32 tensor on {device}, got "
+                                f"{t.dtype} {tuple(t.shape)} on {t.device}")
+        return t
+    v = float(t)
+    if not (math.isfinite(v) and v > 0.0):
+        raise ValueError(f"{what}: temperature must be finite and > 0 (got {v})")
+    return torch.full((1,), v, dtype=torch.float32, device=device)
+
+
+def _expert_temperatures(temperatures, K):
+    if temperatures is None:
+        return [None] * K
+    temperatures = list(temperatures)
+    if len(temperatures) != K:
+        raise ValueError(f"ExpertStep: {len(temperatures)} temperatures for {K} experts (one per expert, None: none)")
+    return temperatures
+
+
+class LogitBank(_CursorLog):
+    """A device-resident bank of every Monte-Carlo sample's raw logits and the label of each image of a calibration set,
+    appended to by the step (bbb_mc_logit_log): ``MCForward(..., logit_bank=bank)`` and ``evaluate(..., logit_bank=bank)``
+    add one entry per image, in step order, with no host read.  It is what ``fit_temperature`` fits T on.
+
+    Entry i holds the S logit rows z_s [S, C] of its image as the net produced them, fp32 bit for bit -- before any
+    temperature, so a bank filled under any temperature fits the same T -- and its int64 label (-1 for a step without
+    labels, which the fit refuses).  Unlike ProbBank (tf32 probabilities, which lose the small ones a temperature > 1
+    raises) it keeps the logits themselves.  ``capacity`` entries fit; images past them are counted, not written, and
+    ``read()`` and the fit refuse a bank that dropped any."""
+
+    def __init__(self, device, capacity: int, num_ens: int, num_classes: int):
+        num_ens, num_classes = int(num_ens), int(num_classes)
+        if not 1 <= num_ens <= L.LOGIT_BANK_MAX_SAMPLES:
+            raise ValueError(f"LogitBank: num_ens must be in [1, {L.LOGIT_BANK_MAX_SAMPLES}] (got {num_ens})")
+        if not 2 <= num_classes <= L.LOGIT_BANK_MAX_CLASSES:
+            raise ValueError(f"LogitBank: num_classes must be in [2, {L.LOGIT_BANK_MAX_CLASSES}] (got {num_classes})")
+        if int(capacity) >= 1 << 31:
+            raise ValueError(f"LogitBank: capacity must be < 2^31 (got {capacity})")
+        self._init_cursor(device, capacity, "LogitBank")
+        self.num_ens, self.num_classes = num_ens, num_classes
+        # (one entry at least: the kernel takes the bank's pointers even when nothing fits)
+        self._logits = torch.zeros(max(1, self.capacity), num_ens, num_classes, dtype=torch.float32, device=self.device)
+        self._labels = torch.full((max(1, self.capacity),), -1, dtype=torch.int64, device=self.device)
+        # a step without labels has been appended since the last reset: append() and MCForward's steps say so (a
+        # captured step's kernel runs without the host seeing it)
+        self._unlabelled = False
+
+    def reset(self):
+        super().reset()
+        self._unlabelled = False
+
+    def _require(self, num_ens, num_classes, what):
+        if (int(num_ens), int(num_classes)) != (self.num_ens, self.num_classes):
+            raise L.EngineError(f"{what}: the logit_bank holds {self.num_ens} samples x {self.num_classes} classes, "
+                                f"the step makes {num_ens} x {num_classes}")
+
+    def _launch(self, logits, labels, B):
+        L.check(L.lib().bbb_mc_logit_log(Fn._ptr(logits), Fn._ptr(labels), self.num_ens, int(B), self.num_classes,
+                                         Fn._ptr(self._logits), Fn._ptr(self._labels), self.capacity,
+                                         Fn._ptr(self._cursor), Fn._stream(self.device)), "bbb_mc_logit_log")
+
+    def append(self, logits, labels=None):
+        """Append the images of per-sample logits [S, B, C] (fp32 contiguous on the bank's device) and their int64 labels
+        [B] (bbb_mc_logit_log on the current stream): logits from anywhere else."""
+        Fn._require_cuda(self._cursor, "LogitBank.append")
+        if not (logits.dim() == 3 and logits.shape[0] == self.num_ens and logits.shape[2] == self.num_classes
+                and logits.shape[1] >= 1 and logits.dtype == torch.float32 and logits.is_contiguous()
+                and logits.device == self.device):
+            raise L.EngineError(f"LogitBank.append: expected contiguous float32 logits [{self.num_ens}, B, "
+                                f"{self.num_classes}] on {self.device}, got {logits.dtype} {tuple(logits.shape)} on "
+                                f"{logits.device}")
+        B = logits.shape[1]
+        if labels is not None and not (labels.dtype == torch.int64 and tuple(labels.shape) == (B,)
+                                       and labels.is_contiguous() and labels.device == self.device):
+            raise L.EngineError(f"LogitBank.append: expected contiguous int64 labels [{B}] on {self.device}, got "
+                                f"{labels.dtype} {tuple(labels.shape)} on {labels.device}")
+        self._unlabelled |= labels is None
+        self._launch(logits, labels, B)
+
+    def read(self) -> dict:
+        """The entries so far: {"logits": float32 [n, S, C], "labels": int64 [n]}, copies on the bank's device.  Raises
+        EngineError if images were dropped.  Steps in flight must be complete first."""
+        n = self._held("LogitBank")
+        return {"logits": self._logits[:n].clone(), "labels": self._labels[:n].clone()}
+
+
+def _check_search(t_min, t_max, grid, rounds):
+    t_min, t_max = float(t_min), float(t_max)
+    if not (0.0 < t_min < t_max and math.isfinite(t_max)):
+        raise ValueError(f"temperature search: need 0 < t_min < t_max < inf (got {t_min}, {t_max})")
+    if int(grid) != grid or not 3 <= int(grid) <= L.TEMPERATURE_MAX_POINTS - 1:
+        raise ValueError(f"temperature search: grid must be an integer in [3, {L.TEMPERATURE_MAX_POINTS - 1}] "
+                         f"(got {grid})")
+    if int(rounds) != rounds or int(rounds) < 1:
+        raise ValueError(f"temperature search: rounds must be an integer >= 1 (got {rounds})")
+    return t_min, t_max, int(grid), int(rounds)
+
+
+def temperature_grid(t_min: float = 0.05, t_max: float = 20.0, grid: int = 32, prev=None, argmin=None) -> list:
+    """One round of the temperature search on tau = ln T (pure host): round 0 (``prev`` None) is ``grid`` points
+    equally spaced on [ln t_min, ln t_max]; the round after a grid ``prev`` whose first minimal NLL is point ``argmin``
+    spans [prev[max(argmin - 1, 0)], prev[min(argmin + 1, grid - 1)]] with ``grid`` points.  Point k is
+    lo + ((hi - lo) * k) / (grid - 1) in IEEE double, as bbb_temperature_nll forms the next round on the device, so
+    both plan the same bits.  Every round narrows the spacing by 2 / (grid - 1)."""
+    _, _, grid, _ = _check_search(t_min, t_max, grid, 1)
+    if prev is None:
+        lo, hi = math.log(float(t_min)), math.log(float(t_max))
+    else:
+        prev = [float(v) for v in prev]
+        if len(prev) != grid:
+            raise ValueError(f"temperature_grid: prev holds {len(prev)} points, grid is {grid}")
+        if argmin is None or int(argmin) != argmin or not 0 <= int(argmin) < grid:
+            raise ValueError(f"temperature_grid: argmin must be an index into prev (got {argmin})")
+        a = int(argmin)
+        lo, hi = prev[max(a - 1, 0)], prev[min(a + 1, grid - 1)]
+    return [lo + (hi - lo) * k / (grid - 1) for k in range(grid)]
+
+
+class TemperatureFit:
+    """What fit_temperature enqueued: ``temperature`` (one-element fp32 device tensor, the fitted T), and on ``read()``
+    -- the one host synchronisation -- the floats."""
+
+    def __init__(self, bank, temperature, fit, taus, nlls, grid, trace):
+        self.temperature, self._fit, self._taus, self._nlls = temperature, fit, taus, nlls
+        self._bank, self._grid, self._trace = bank, grid, trace
+
+    def read(self) -> dict:
+        """{"temperature", "nll" (the bank's NLL at it), "nll_at_one" (at T = 1), "at_bound" (round 0's minimum was an
+        end of [t_min, t_max]: widen the range), "tau" (ln T)}, and with ``trace`` "trace": one {"tau", "nll"} per round
+        (round 0 with T = 1 last).  Raises ValueError when there is no fit -- an empty bank, one that dropped images, or
+        one that holds an image logged without a label or with a label outside [0, C) -- and ``temperature`` then keeps
+        the value it had before the fit.  Read after the fit, not after later appends to the bank."""
+        v = torch.cat([self._fit, self.temperature.to(torch.float64)]).tolist()
+        if any(math.isnan(x) for x in v[:4]):
+            raise ValueError(f"fit_temperature: no fit -- {self._why()}")
+        out = {"temperature": v[4], "nll": v[1], "nll_at_one": v[0], "at_bound": bool(v[2]), "tau": v[3]}
+        if self._trace:
+            taus, nlls = self._taus.tolist(), self._nlls.tolist()
+            out["trace"] = [{"tau": taus[r][:self._grid + (r == 0)], "nll": nlls[r][:self._grid + (r == 0)]}
+                            for r in range(len(taus))]
+        return out
+
+    def _why(self):
+        """Why the device found no fit (host reads of the bank)."""
+        n, dropped = self._bank._counts()
+        if dropped:
+            return f"the bank dropped {dropped} images (capacity {self._bank.capacity})"
+        if n == 0:
+            return "the bank is empty"
+        y = self._bank._labels[:n]
+        if bool((y < 0).any()):
+            return f"{int((y < 0).sum())} images were logged without a label (a step with_labels=False)"
+        if bool((y >= self._bank.num_classes).any()):
+            return f"a label is outside [0, {self._bank.num_classes})"
+        return "the bank's logits give no finite NLL (NaN or infinite logits?)"
+
+
+def fit_temperature(bank: LogitBank, t_min: float = 0.05, t_max: float = 20.0, grid: int = 32, rounds: int = 4,
+                    out: Optional[torch.Tensor] = None, trace: bool = False) -> TemperatureFit:
+    """The temperature that minimises the bank's NLL of the tempered predictive,
+        l(T) = -(1/n) sum_i log( (1/S) sum_s softmax(z_is / T)[y_i] ),
+    by a grid search on tau = ln T, enqueued on the current stream with no host read: ``rounds`` passes of
+    bbb_temperature_nll over the bank, each evaluating ``grid`` points (temperature_grid; round 0 also T = 1) and
+    writing the next round's grid on the device.  The result is never worse than T = 1 on the bank.
+
+    Returns a TemperatureFit: ``.temperature`` is the fitted T as a one-element fp32 device tensor -- written in place
+    into ``out`` when given, so engines that temper with ``out`` (MCForward / evaluate ``temperature=out``) read the new
+    value at their next step; without ``out`` it starts at 1 -- and ``.read()`` gives the floats.  A fit the device
+    cannot make (an empty bank, one that dropped images, or one that holds an image without a valid label) leaves
+    ``.temperature`` as it was, and ``.read()`` raises.  A bank known on the host to hold images without labels (appended
+    without them, or by a step with_labels=False) is refused here already."""
+    t_min, t_max, grid, rounds = _check_search(t_min, t_max, grid, rounds)
+    if not isinstance(bank, LogitBank):
+        raise TypeError(f"fit_temperature: expected a LogitBank, got {type(bank).__name__}")
+    Fn._require_cuda(bank._cursor, "fit_temperature")
+    if bank.capacity < 1:
+        raise ValueError("fit_temperature: the bank has no capacity")
+    if bank._unlabelled:
+        raise ValueError("fit_temperature: the bank holds images logged without labels (a step with_labels=False)")
+    dev = bank.device
+    if out is None:
+        out = torch.ones(1, dtype=torch.float32, device=dev)
+    _temperature_tensor(out, dev, False, "fit_temperature(out=...)")
+    f64 = dict(dtype=torch.float64, device=dev)
+    taus = torch.zeros(rounds, grid + 1, **f64)               # round 0's point `grid` is tau = 0 (T = 1)
+    plan = torch.tensor(temperature_grid(t_min, t_max, grid), dtype=torch.float64).pin_memory()
+    taus[0, :grid].copy_(plan, non_blocking=True)
+    nlls = torch.full((rounds, grid + 1), float("nan"), **f64)
+    fit = torch.full((4,), float("nan"), **f64)
+    lib = L.lib()
+    nbytes = int(lib.bbb_temperature_workspace_bytes(bank.capacity, grid + 1))
+    ws = torch.zeros(nbytes, dtype=torch.uint8, device=dev)
+    for r in range(rounds):
+        flags = (L.TEMPERATURE_FIRST if r == 0 else 0) | (L.TEMPERATURE_LAST if r == rounds - 1 else 0)
+        L.check(lib.bbb_temperature_nll(
+            Fn._ptr(bank._logits), Fn._ptr(bank._labels), Fn._ptr(bank._cursor), bank.capacity, bank.num_ens,
+            bank.num_classes, Fn._ptr(taus[r]), grid + (r == 0), grid, flags, Fn._ptr(nlls[r]),
+            Fn._ptr(taus[r + 1]) if r + 1 < rounds else None, Fn._ptr(fit), Fn._ptr(out), Fn._ptr(ws), nbytes,
+            Fn._stream(dev)), "bbb_temperature_nll")
+    return TemperatureFit(bank, out, fit, taus, nlls, grid, trace)
+
+
+def calibrate_temperature(net, cal_loader, num_ens: int, t_min: float = 0.05, t_max: float = 20.0, grid: int = 32,
+                          rounds: int = 4, out: Optional[torch.Tensor] = None, trace: bool = False,
+                          **evaluate_kwargs) -> dict:
+    """Temperature scaling over a whole calibration set: ``evaluate`` over ``cal_loader`` (batches of (x, y), held out
+    from training) into a LogitBank, then fit_temperature on it.  Returns ``temperature`` (the one-element fp32 device
+    tensor; ``out`` when given), ``fit`` (TemperatureFit.read()) and ``evaluate`` (evaluate's figures on the calibration
+    set, untempered unless ``temperature`` is among ``evaluate_kwargs``).  The intended use:
+
+        cal = mc.calibrate_temperature(net, cal_loader, num_ens)
+        test = mc.evaluate(net, test_loader, num_ens, train_size, temperature=cal["temperature"])   # test ECE, NLL
+
+    and the same ``temperature=`` to detect_ood, conformal or acquire (through their evaluate keywords), MCForward, or
+    ExpertStep / route (one per expert).  ``evaluate_kwargs`` go to evaluate (``train_size`` defaults to 1.0).  The
+    bank is kept on the net, as detect_ood keeps its logs, and reused by the next call."""
+    dev = next(net.parameters()).device
+    kw = dict(evaluate_kwargs)
+    train_size = kw.pop("train_size", 1.0)
+    n = _loader_images(cal_loader)
+    S, Cc = int(num_ens), int(net.num_classes)
+    banks = net.__dict__.setdefault("_temperature_banks", {})
+    bank = banks.get("calibration")
+    if bank is None or bank.capacity < n or bank.device != dev or (bank.num_ens, bank.num_classes) != (S, Cc):
+        if bank is not None:                        # evaluate's engines that append to the old bank go with it
+            cache = net.__dict__.get("_mc_eval", {})
+            for k in [k for k, e in cache.items() if e.get("logit_bank") is bank]:
+                del cache[k]
+        bank = banks["calibration"] = LogitBank(dev, n, S, Cc)
+    bank.reset()
+    m = evaluate(net, cal_loader, num_ens, train_size, logit_bank=bank, **kw)
+    fit = fit_temperature(bank, t_min, t_max, grid, rounds, out=out, trace=trace)
+    return {"temperature": fit.temperature, "fit": fit.read(), "evaluate": m}
