@@ -222,40 +222,20 @@ class MCForward:
                 raise L.EngineError(f"MCForward: metrics must be a contiguous float64 tensor of >= {n} elements on "
                                     f"{example_x.device} (mc.new_metrics)")
         self.metrics = self._metrics = metrics      # _metrics: the accumulator the exchange adds to
-        if score_log is not None and score_log.device != example_x.device:
-            raise L.EngineError(f"MCForward: score_log is on {score_log.device}, the step on {example_x.device}")
-        self.score_log = self._score_log = score_log      # _score_log: the log the steps append to
-        if conformal is not None:
-            if conformal.device != example_x.device:
-                raise L.EngineError(f"MCForward: conformal is on {conformal.device}, the step on {example_x.device}")
-            ncls = int(num_classes if num_classes is not None else net.num_classes)
-            if ncls != conformal.num_classes:
-                raise L.EngineError(f"MCForward: the conformal log holds {conformal.num_classes} classes, the step "
-                                    f"makes {ncls}")
-        self.conformal = self._conformal = conformal     # _conformal: the log the steps append to
         self.net, self.group = net, group
         self.dist, self.world, self.rank = _dist_info(group)
-        if prob_bank is not None:
-            if self.world > 1:
-                raise L.EngineError(f"MCForward: a prob_bank needs one rank (the group has {self.world}): a rank holds "
-                                    "only its own samples")
-            if prob_bank.device != example_x.device:
-                raise L.EngineError(f"MCForward: prob_bank is on {prob_bank.device}, the step on {example_x.device}")
-            prob_bank._require(num_ens, num_classes if num_classes is not None else net.num_classes, "MCForward")
-        self.prob_bank = self._prob_bank = prob_bank      # _prob_bank: the bank the steps append to
-        if logit_bank is not None:
-            if self.world > 1:
-                raise L.EngineError(f"MCForward: a logit_bank needs one rank (the group has {self.world}): a rank holds "
-                                    "only its own samples")
-            if logit_bank.device != example_x.device:
-                raise L.EngineError(f"MCForward: logit_bank is on {logit_bank.device}, the step on {example_x.device}")
-            logit_bank._require(num_ens, num_classes if num_classes is not None else net.num_classes, "MCForward")
-        self.logit_bank = self._logit_bank = logit_bank   # _logit_bank: the bank the steps append to
+        dev = self.dev = example_x.device
+        self.num_ens = int(num_ens)
+        self.C = int(num_classes if num_classes is not None else net.num_classes)
+        # the logs the steps append to (_CursorLog._log), in the order their kernels are enqueued
+        self._logs = [lg for lg in (logit_bank, score_log, prob_bank, conformal) if lg is not None]
+        for lg in self._logs:
+            lg._bind(self)
+        # a step without labels logs label -1 into a logit bank, which the host must know of (LogitBank._unlabelled)
+        self._unlabelled_bank = logit_bank if not with_labels else None
         self.temperature = _temperature_tensor(temperature, example_x.device, normalized, "MCForward")
         if self.world > 16:
             raise L.EngineError("MCForward: at most 16 ranks (one node)")
-        dev = self.dev = example_x.device
-        self.num_ens = int(num_ens)
         self.sample_shards, self.group_index, self.block = shard_layout(self.world, self.rank, batch_shards)
         self.batch_shards = int(batch_shards)
         self.ids = local_samples(self.num_ens, self.sample_shards, self.group_index)
@@ -264,7 +244,6 @@ class MCForward:
             raise L.EngineError(f"MCForward: batch_shards={self.batch_shards} > batch {self.B} (a row block would be empty)")
         self.rows = row_block(self.B, self.batch_shards, self.block)     # this rank's images [b0, b1)
         self.nb = self.rows[1] - self.rows[0]
-        self.C = int(num_classes if num_classes is not None else net.num_classes)
         self.flags = (L.MC_MOMENTS if want_uncertainty else 0) | (L.MC_NORMALIZED if normalized else 0) | \
             (L.MC_INFO if want_information else 0)
         self.want_uncertainty, self.with_labels = want_uncertainty, with_labels
@@ -574,16 +553,16 @@ class MCForward:
         from .graph import _STRIDE
         o = self.out
         lib = L.lib()
-        labels = self.labels_all[par] if self.labels_all is not None else None
-        if self._logit_bank is not None:
-            self._logit_bank._launch(self.logits_all[par], labels, self.B)
+        for lg in self._logs:
+            if lg.before_temper:
+                lg._log(self, par)
         if self.temperature is not None and self.ids:
             z = self.logits_all[par]
             L.check(lib.bbb_mc_temper(Fn._ptr(z), z.numel(), Fn._ptr(self.temperature), Fn._stream(self.dev)),
                     "bbb_mc_temper")
         args = (
             Fn._ptr(self.logits_all[par]), len(self.ids), self.num_ens, self.B, self.C, kl_ptr, n_kl, self.flags,
-            Fn._ptr(self.labels_all[par] if self.labels_all is not None else None), C.c_float(self.train_size), C.c_float(self.beta), self.rank, self.world, self.peers,
+            Fn._ptr(self._labels_of(par)), C.c_float(self.train_size), C.c_float(self.beta), self.rank, self.world, self.peers,
             Fn._ptr(self.state), Fn._ptr(o["log_outputs"]), Fn._ptr(o["kl"]), Fn._ptr(o.get("pred")),
             Fn._ptr(o.get("epistemic")), Fn._ptr(o.get("aleatoric")), Fn._ptr(o.get("entropy")), Fn._ptr(o.get("head")),
             Fn._ptr(advance_base), C.c_uint64(_STRIDE if advance_base is not None else 0),
@@ -593,13 +572,13 @@ class MCForward:
                     "bbb_mc_exchange_metrics")
         else:
             L.check(lib.bbb_mc_exchange_sharded(*args, self.batch_shards, Fn._stream(self.dev)), "bbb_mc_exchange_sharded")
-        if self._score_log is not None:
-            self._score_log.append(o["log_outputs"], o.get("entropy"), o.get("expected_entropy"), o.get("mutual_info"),
-                                   o.get("epistemic"), self.labels_all[par] if self.labels_all is not None else None)
-        if self._prob_bank is not None:
-            self._prob_bank._launch(self.logits_all[par], self.B, bool(self.flags & L.MC_NORMALIZED))
-        if self._conformal is not None:
-            self._conformal._launch(o["log_outputs"], self.labels_all[par] if self.labels_all is not None else None)
+        for lg in self._logs:
+            if not lg.before_temper:
+                lg._log(self, par)
+
+    def _labels_of(self, par):
+        """The labels of buffer parity ``par``, or None without ``with_labels``."""
+        return self.labels_all[par] if self.labels_all is not None else None
 
     def _capture(self, warmup: int = 2):
         from .graph import _STRIDE
@@ -628,18 +607,10 @@ class MCForward:
         dev = self.dev
         side = torch.cuda.Stream(device=dev)
         side.wait_stream(torch.cuda.current_stream(dev))
-        live, live_log, live_bank, live_cf = self._metrics, self._score_log, self._prob_bank, self._conformal
-        live_lb = self._logit_bank
-        if live_lb is not None:
-            self._logit_bank = LogitBank(dev, 0, live_lb.num_ens, live_lb.num_classes)
+        live, live_logs = self._metrics, self._logs
         if live is not None:
             self._metrics = torch.zeros_like(live)      # the warm-up steps do not count
-        if live_log is not None:
-            self._score_log = ScoreLog(dev, 0)          # nor are they logged (a log of no capacity drops them)
-        if live_bank is not None:
-            self._prob_bank = ProbBank(dev, 0, live_bank.num_ens, live_bank.num_classes)
-        if live_cf is not None:
-            self._conformal = live_cf._empty()
+        self._logs = [lg._empty() for lg in live_logs]   # nor are they logged (a log of no capacity drops them)
         self._prep = self._plan_prep(self.x) if self.cache_prep else None
         with torch.cuda.stream(side):
             if self._prep is not None:              # the first prep, which the warm-up steps already read
@@ -651,8 +622,7 @@ class MCForward:
                 self._exchange(*self._chain(self.x, self.base, par=p_), par=p_)
         torch.cuda.current_stream(dev).wait_stream(side)
         torch.cuda.synchronize(dev)
-        self._metrics, self._score_log, self._prob_bank, self._conformal = live, live_log, live_bank, live_cf
-        self._logit_bank = live_lb
+        self._metrics, self._logs = live, live_logs
         # GEMM chain on a HIGH-priority stream, parameter preps on the (default-priority) side streams: when both have CTAs
         # pending, the chain's go first -- the preps of later layers no longer keep the first GEMM's CTAs off the SMs
         cap = torch.cuda.Stream(device=dev, priority=-1)
@@ -738,8 +708,8 @@ class MCForward:
     def __call__(self, x: Optional[torch.Tensor] = None, labels: Optional[torch.Tensor] = None, slot: int = 0):
         if labels is not None and self.labels is None:
             raise L.EngineError("MCForward was built without with_labels=True")
-        if self._logit_bank is not None and self.labels is None:
-            self._logit_bank._unlabelled = True   # this step logs label -1
+        if self._unlabelled_bank is not None:
+            self._unlabelled_bank._unlabelled = True   # this step logs label -1
         if self._prior_guard is not None:
             self._prior_guard.check("MCForward")
         if self._prep_graph is not None:
@@ -988,7 +958,20 @@ def read_metrics(t: torch.Tensor) -> dict:
 
 class _CursorLog:
     """What a data-set-long device log shares: the two-word cursor of bbb_mc_score_log / bbb_mc_prob_log (next index,
-    images dropped) and its host reads."""
+    images dropped) and its host reads.
+
+    A log the Monte-Carlo step appends to -- MCForward's keyword ``_keyword`` -- also implements the step's hooks:
+    ``_bind(step)`` refuses an engine being built that it cannot log, ``_empty()`` is a log of no capacity with the same
+    options (what the engine's warm-up steps append to), and ``_log(step, par)`` enqueues the append from the step's
+    buffers of parity ``par``: in front of the temper when ``before_temper`` (the log holds the raw logits), else
+    behind the exchange."""
+
+    _keyword = None
+    before_temper = False
+
+    def _bind(self, step):
+        if self.device != step.dev:
+            raise L.EngineError(f"MCForward: {self._keyword} is on {self.device}, the step on {step.dev}")
 
     def _init_cursor(self, device, capacity: int, what: str):
         capacity = int(capacity)
@@ -1038,6 +1021,7 @@ class ScoreLog(_CursorLog):
     them are counted, not written, and ``read()`` refuses a log that dropped any."""
 
     PLANES = ("confidence", "entropy", "mutual_info", "expected_entropy", "epistemic", "correct")
+    _keyword = "score_log"
 
     def __init__(self, device, capacity: int):
         self._init_cursor(device, capacity, "ScoreLog")
@@ -1046,6 +1030,14 @@ class ScoreLog(_CursorLog):
         # nothing fits)
         self._planes = torch.zeros(L.MC_SCORE_PLANES, max(1, capacity), dtype=torch.float32, device=self.device)
         self._pred = torch.zeros(max(1, capacity), dtype=torch.int32, device=self.device)
+
+    def _empty(self):
+        return ScoreLog(self.device, 0)
+
+    def _log(self, step, par):
+        o = step.out
+        self.append(o["log_outputs"], o.get("entropy"), o.get("expected_entropy"), o.get("mutual_info"),
+                    o.get("epistemic"), step._labels_of(par))
 
     def read(self) -> dict:
         """The entries logged so far: {plane name: float32 [n], "pred": int32 [n]}, copies on the log's device.  Raises
@@ -1105,39 +1097,56 @@ def evaluate(net, loader, num_ens: int, train_size: float, beta_type=0.1, epoch=
     ``temperature``: MCForward's -- every figure, log and bank behind the exchange is that of the tempered predictive.
     Engines are kept per temperature tensor (a float: per value), and read a value written into the tensor in place."""
     dev = next(net.parameters()).device
-    log = score_log is not None
+    logs = dict(score_log=score_log, prob_bank=prob_bank, conformal=conformal, logit_bank=logit_bank)
     tkey = None if temperature is None else \
         ("tensor", id(temperature)) if isinstance(temperature, torch.Tensor) else float(temperature)
     key = (int(num_ens), float(train_size), seed, id(group), int(inflight), int(batch_shards), bool(normalized),
-           id(score_log) if log else None, id(prob_bank) if prob_bank is not None else None,
-           id(conformal) if conformal is not None else None, id(logit_bank) if logit_bank is not None else None, tkey)
+           *(None if lg is None else id(lg) for lg in logs.values()), tkey)
     ev = _engine_cache(net, "_mc_eval").get(key)
     if ev is None:
-        ev = net.__dict__["_mc_eval"][key] = {"acc": new_metrics(dev), "engines": {}, "seed": seed, "log": score_log,
-                                              "bank": prob_bank, "conformal": conformal, "logit_bank": logit_bank,
+        # (the entry holds the logs and the temperature its key names by id, so that no other object takes their id)
+        ev = net.__dict__["_mc_eval"][key] = {"acc": new_metrics(dev), "engines": {}, "seed": seed,
+                                              "logs": [lg for lg in logs.values() if lg is not None],
                                               "temperature": temperature}
-    acc, engines, nslots = ev["acc"], ev["engines"], max(2, int(inflight))
-    cur = torch.cuda.current_stream(dev)
-    acc.zero_()
+    ev["acc"].zero_()
+
+    def build(slots, first_replay):
+        return MCForward(net, slots[0], num_ens, group, with_labels=True, train_size=train_size, seed=ev["seed"],
+                         static_inputs=slots, first_replay=first_replay, overlap=True, inflight=inflight,
+                         batch_shards=batch_shards, metrics=ev["acc"], normalized=normalized,
+                         want_uncertainty=score_log is not None, want_information=score_log is not None,
+                         temperature=temperature, **logs)
+    n = _run_loader(ev, loader, dev, max(2, int(inflight)), build)
+    if not n:
+        raise ValueError("evaluate: the loader yielded no batch")
+    m = read_metrics(ev["acc"])
+    beta_sum = sum(get_beta(i - 1, n, beta_type, epoch, num_epochs) for i in range(n))
+    m["valid_loss"] = (float(train_size) * m["sum_nll_step"] + beta_sum * m["klsum"]) / n
+    m["valid_acc"] = m["sum_acc_step"] / n
+    return m
+
+
+def _run_loader(entry, loader, dev, nslots, build, **call_kw):
+    """The loader loop of evaluate and route: every batch (x, y) through the in-flight step of its shape in the cache
+    ``entry`` (an MCForward or ExpertStep, made by ``build(slots, first_replay)`` over ``nslots`` rotating input slots
+    when the shape first comes), as ``step(labels=, slot=, **call_kw)``.  Returns the number of batches, with the
+    current stream behind the last step."""
+    engines, cur = entry["engines"], torch.cuda.current_stream(dev)
     last, n = None, 0
     for x, y in loader:
         shape = (tuple(x.shape), x.dtype)
         e = engines.get(shape)
         if e is None:
             slots = [torch.zeros(x.shape, dtype=x.dtype, device=dev) for _ in range(nslots)]
-            # the k-th engine built draws noise blocks k * 2^16, k * 2^16 + 1, ...: engines do not share noise
-            eng = MCForward(net, slots[0], num_ens, group, with_labels=True, train_size=train_size, seed=ev["seed"],
-                            static_inputs=slots, first_replay=len(engines) << 16, overlap=True, inflight=inflight,
-                            batch_shards=batch_shards, metrics=acc, normalized=normalized, want_uncertainty=log,
-                            want_information=log, score_log=score_log, prob_bank=prob_bank, conformal=conformal,
-                            logit_bank=logit_bank, temperature=temperature)
-            ev["seed"] = eng.seed               # every engine draws from the same seed
+            # the k-th step built draws noise blocks k * 2^16, k * 2^16 + 1, ...: steps do not share noise
+            eng = build(slots, len(engines) << 16)
+            entry["seed"] = eng.seed            # every step draws from the same seed
             e = engines[shape] = {"eng": eng, "slots": slots, "consumed": [None] * nslots, "steps": 0,
                                   "labels": [torch.zeros(x.shape[0], dtype=torch.int64, device=dev) for _ in range(nslots)],
                                   "pinned": [None] * nslots}
         eng = e["eng"]
         if last is not None and last is not eng:
-            last.wait()                         # the accumulator takes the steps one after another
+            last.wait()                         # the accumulator and the logs take the steps one after another
         s = e["steps"] % nslots
         x, y = _pinned(e, s, x, y)
         if e["consumed"][s] is not None:
@@ -1148,18 +1157,31 @@ def evaluate(net, loader, num_ens: int, train_size: float, beta_type=0.1, epoch=
         e["labels"][s].copy_(y, non_blocking=True)  # the step copies them on its own stream: they must outlive the call
         if e["pinned"][s] is not None:
             e["pinned"][s][2].record(cur)       # the pinned slot may be refilled once these copies are done
-        eng(labels=e["labels"][s], slot=s)
+        eng(labels=e["labels"][s], slot=s, **call_kw)
         e["consumed"][s] = eng.input_consumed()
         e["steps"] += 1
         last, n = eng, n + 1
-    if last is None:
-        raise ValueError("evaluate: the loader yielded no batch")
-    last.wait()
-    m = read_metrics(acc)
-    beta_sum = sum(get_beta(i - 1, n, beta_type, epoch, num_epochs) for i in range(n))
-    m["valid_loss"] = (float(train_size) * m["sum_nll_step"] + beta_sum * m["klsum"]) / n
-    m["valid_acc"] = m["sum_acc_step"] / n
-    return m
+    if last is not None:
+        last.wait()
+    return n
+
+
+def _kept_log(net, store: dict, key, loader, make, fits=lambda log: True):
+    """The log that detect_ood, acquire, conformal or calibrate_temperature keeps for the net in ``store[key]``, reset
+    and sized for ``loader``: ``make(capacity)`` makes a new one when there is none yet, or the one kept holds fewer
+    entries than the loader has images, is on another device than the net or does not pass ``fits``.  evaluate's
+    engines that append to the old log go with it."""
+    dev = next(net.parameters()).device
+    n = _loader_images(loader)
+    log = store.get(key)
+    if log is None or log.capacity < n or log.device != dev or not fits(log):
+        if log is not None:
+            cache = net.__dict__.get("_mc_eval", {})
+            for k in [k for k, e in cache.items() if any(lg is log for lg in e["logs"])]:
+                del cache[k]
+        log = store[key] = make(n)
+    log.reset()
+    return log
 
 
 def _pinned(e, s, x, y):
@@ -1279,17 +1301,14 @@ class MCTrainStep(MCForward):
     def __init__(self, net, example_x, num_ens, train_size, group=None, seed=None, batch_shards: int = 1,
                  fold: bool = False, fold_group: Optional[int] = None, score_log=None, prob_bank=None, conformal=None,
                  logit_bank=None, temperature=None):
-        if temperature is not None:
-            raise L.EngineError("MCTrainStep does not temper: a temperature is fitted after training "
-                                "(fit_temperature) and applied by MCForward or evaluate()")
-        if logit_bank is not None:
-            raise L.EngineError("MCTrainStep does not fill a logit_bank: fill it from MCForward or evaluate()")
-        if conformal is not None:
-            raise L.EngineError("MCTrainStep does not log conformal scores: log them from MCForward or evaluate()")
-        if score_log is not None:
-            raise L.EngineError("MCTrainStep does not log scores: log them from MCForward or evaluate()")
-        if prob_bank is not None:
-            raise L.EngineError("MCTrainStep does not fill a prob_bank: fill it from MCForward or evaluate()")
+        for given, why in ((temperature, "temper: a temperature is fitted after training (fit_temperature) and "
+                                         "applied by MCForward or evaluate()"),
+                           (logit_bank, "fill a logit_bank: fill it from MCForward or evaluate()"),
+                           (conformal, "log conformal scores: log them from MCForward or evaluate()"),
+                           (score_log, "log scores: log them from MCForward or evaluate()"),
+                           (prob_bank, "fill a prob_bank: fill it from MCForward or evaluate()")):
+            if given is not None:
+                raise L.EngineError(f"MCTrainStep does not {why}")
         super().__init__(net, example_x, num_ens, group=group, with_labels=True, train_size=train_size, seed=seed,
                          graph=False, fold=False, batch_shards=batch_shards)
         self.params = [p for p in net.parameters() if p.requires_grad]
@@ -1497,15 +1516,7 @@ def detect_ood(net, in_loader, out_loader, num_ens: int, score: Optional[str] = 
     train_size = kw.pop("train_size", 1.0)
     logs, res = net.__dict__.setdefault("_ood_logs", {}), {}
     for role, loader in (("in", in_loader), ("out", out_loader)):
-        n = _loader_images(loader)
-        log = logs.get(role)
-        if log is None or log.capacity < n or log.device != dev:
-            if log is not None:                     # evaluate's engines that append to the old log go with it
-                cache = net.__dict__.get("_mc_eval", {})
-                for k in [k for k, e in cache.items() if e.get("log") is log]:
-                    del cache[k]
-            log = logs[role] = ScoreLog(dev, n)
-        log.reset()
+        log = _kept_log(net, logs, role, loader, lambda n: ScoreLog(dev, n))
         res[role] = evaluate(net, loader, num_ens, train_size, normalized=normalized, score_log=log, **kw)
     got = {role: logs[role].read() for role in ("in", "out")}
     ood = {nm: ood_metrics(_score(got["in"], nm), _score(got["out"], nm)) for nm in names}
@@ -1523,7 +1534,37 @@ def bank_pads(num_ens: int, num_classes: int):
     return -(-int(num_ens) // 8) * 8, 1 << (int(num_classes) - 1).bit_length()
 
 
-class ProbBank(_CursorLog):
+class _SampleBank(_CursorLog):
+    """What ProbBank and LogitBank share: entries of all S samples x C classes of an image, taken from the step's
+    per-sample logits -- so one rank only, which holds only its own samples."""
+
+    def _bind(self, step):
+        if step.world > 1:
+            raise L.EngineError(f"MCForward: a {self._keyword} needs one rank (the group has {step.world}): a rank "
+                                "holds only its own samples")
+        super()._bind(step)
+        self._require(step.num_ens, step.C, "MCForward")
+
+    def _empty(self):
+        return type(self)(self.device, 0, self.num_ens, self.num_classes)
+
+    def _require(self, num_ens, num_classes, what):
+        if (int(num_ens), int(num_classes)) != (self.num_ens, self.num_classes):
+            raise L.EngineError(f"{what}: the {self._keyword} holds {self.num_ens} samples x {self.num_classes} "
+                                f"classes, the step makes {num_ens} x {num_classes}")
+
+    def _check_logits(self, logits):
+        """Refuse anything but per-sample logits [S, B, C] of this bank: fp32, contiguous, on its device."""
+        what = f"{type(self).__name__}.append"
+        Fn._require_cuda(self._cursor, what)
+        if not (logits.dim() == 3 and logits.shape[0] == self.num_ens and logits.shape[2] == self.num_classes
+                and logits.shape[1] >= 1 and logits.dtype == torch.float32 and logits.is_contiguous()
+                and logits.device == self.device):
+            raise L.EngineError(f"{what}: expected contiguous float32 logits [{self.num_ens}, B, {self.num_classes}] "
+                                f"on {self.device}, got {logits.dtype} {tuple(logits.shape)} on {logits.device}")
+
+
+class ProbBank(_SampleBank):
     """A device-resident bank of every Monte-Carlo sample's probability row for each image of a pool, appended to by the
     step (bbb_mc_prob_log): ``MCForward(..., prob_bank=bank)`` and ``evaluate(..., prob_bank=bank)`` add one entry per
     image, in step order, with no host read.  It is what BatchBALD scores (``batchbald``, ``bald``, ``acquire``).
@@ -1532,6 +1573,8 @@ class ProbBank(_CursorLog):
     tf32, in ``bank[i][c][s]`` order with S padded to S_pad and C to C_pad (bank_pads; the padding is zero), and
     ``expected_entropy`` = (1/S) sum_s H[p_hat_s] in float64.  ``capacity`` entries fit; images past them are counted,
     not written, and ``read()`` refuses a bank that dropped any."""
+
+    _keyword = "prob_bank"
 
     def __init__(self, device, capacity: int, num_ens: int, num_classes: int):
         num_ens, num_classes = int(num_ens), int(num_classes)
@@ -1546,26 +1589,18 @@ class ProbBank(_CursorLog):
         self._probs = torch.zeros(max(1, self.capacity), self.C_pad, self.S_pad, dtype=torch.float32, device=self.device)
         self._ee = torch.zeros(max(1, self.capacity), dtype=torch.float64, device=self.device)
 
-    def _require(self, num_ens, num_classes, what):
-        if (int(num_ens), int(num_classes)) != (self.num_ens, self.num_classes):
-            raise L.EngineError(f"{what}: the prob_bank holds {self.num_ens} samples x {self.num_classes} classes, "
-                                f"the step makes {num_ens} x {num_classes}")
-
     def _launch(self, logits, B, normalized):
         L.check(L.lib().bbb_mc_prob_log(Fn._ptr(logits), self.num_ens, int(B), self.num_classes, int(bool(normalized)),
                                         Fn._ptr(self._probs), Fn._ptr(self._ee), self.capacity, Fn._ptr(self._cursor),
                                         Fn._stream(self.device)), "bbb_mc_prob_log")
 
+    def _log(self, step, par):
+        self._launch(step.logits_all[par], step.B, bool(step.flags & L.MC_NORMALIZED))
+
     def append(self, logits, normalized: bool = False):
         """Append the images of per-sample logits [S, B, C] (fp32 contiguous on the bank's device; bbb_mc_prob_log on
         the current stream): probabilities from anywhere else."""
-        Fn._require_cuda(self._cursor, "ProbBank.append")
-        if not (logits.dim() == 3 and logits.shape[0] == self.num_ens and logits.shape[2] == self.num_classes
-                and logits.shape[1] >= 1 and logits.dtype == torch.float32 and logits.is_contiguous()
-                and logits.device == self.device):
-            raise L.EngineError(f"ProbBank.append: expected contiguous float32 logits [{self.num_ens}, B, "
-                                f"{self.num_classes}] on {self.device}, got {logits.dtype} {tuple(logits.shape)} on "
-                                f"{logits.device}")
+        self._check_logits(logits)
         self._launch(logits, logits.shape[1], normalized)
 
     def read(self) -> dict:
@@ -1737,16 +1772,8 @@ def acquire(net, pool_loader, k: int, num_ens: int, method: str = "batchbald", n
     dev = next(net.parameters()).device
     kw = dict(evaluate_kwargs)
     train_size = kw.pop("train_size", 1.0)
-    n = _loader_images(pool_loader)
-    bank = net.__dict__.get("_al_bank")
-    if bank is None or bank.capacity < n or bank.device != dev or (bank.num_ens, bank.num_classes) != \
-            (int(num_ens), int(net.num_classes)):
-        if bank is not None:                    # evaluate's engines that append to the old bank go with it
-            cache = net.__dict__.get("_mc_eval", {})
-            for key in [key for key, e in cache.items() if e.get("bank") is bank]:
-                del cache[key]
-        bank = net.__dict__["_al_bank"] = ProbBank(dev, n, num_ens, net.num_classes)
-    bank.reset()
+    bank = _kept_log(net, net.__dict__, "_al_bank", pool_loader, lambda n: ProbBank(dev, n, num_ens, net.num_classes),
+                     lambda b: (b.num_ens, b.num_classes) == (int(num_ens), int(net.num_classes)))
     m = evaluate(net, pool_loader, num_ens, train_size, prob_bank=bank, **kw)
     sel = batchbald(bank, k, num_configs, seed=kw.get("seed")) if method == "batchbald" else bald(bank, k)
     sel["evaluate"] = m
@@ -1774,6 +1801,8 @@ class ConformalLog(_CursorLog):
     be independent (a calibration set and a test set) take different streams.  Until ``set_threshold`` the log has no
     threshold (size = covered = -1, empty sets): a calibration log needs none.  ``capacity`` entries fit; images past
     them are counted, not written, and ``read()`` refuses a log that dropped any."""
+
+    _keyword = "conformal"
 
     def __init__(self, device, capacity: int, num_classes: int, method: str = "aps", randomized: bool = True,
                  lam: float = 0.0, k_reg: int = 0, seed: Optional[int] = None, stream: int = 0):
@@ -1810,6 +1839,15 @@ class ConformalLog(_CursorLog):
     def _empty(self):
         """A log of no capacity with the same options (what an engine's warm-up steps append to)."""
         return ConformalLog(self.device, 0, self.num_classes, **self._options())
+
+    def _bind(self, step):
+        super()._bind(step)
+        if step.C != self.num_classes:
+            raise L.EngineError(f"MCForward: the conformal log holds {self.num_classes} classes, the step makes "
+                                f"{step.C}")
+
+    def _log(self, step, par):
+        self._launch(step.out["log_outputs"], step._labels_of(par))
 
     def _launch(self, log_outputs, labels):
         L.check(L.lib().bbb_mc_conformal_log(
@@ -1962,16 +2000,9 @@ def conformal(net, cal_loader, test_loader, num_ens: int, alpha: float = 0.1, me
                 seed=int(kw["seed"] if kw.get("seed") is not None else Fn.current_seed()) & ((1 << 64) - 1))
     logs, res = net.__dict__.setdefault("_conformal_logs", {}), {}
     for stream, (role, loader) in enumerate((("calibration", cal_loader), ("test", test_loader))):
-        n = _loader_images(loader)
-        log = logs.get(role)
-        if log is None or log.capacity < n or log.device != dev or log.num_classes != int(net.num_classes) or \
-                log._options() != dict(opts, stream=stream):
-            if log is not None:                     # evaluate's engines that append to the old log go with it
-                cache = net.__dict__.get("_mc_eval", {})
-                for k in [k for k, e in cache.items() if e.get("conformal") is log]:
-                    del cache[k]
-            log = logs[role] = ConformalLog(dev, n, net.num_classes, stream=stream, **opts)
-        log.reset()
+        log = _kept_log(
+            net, logs, role, loader, lambda n: ConformalLog(dev, n, net.num_classes, stream=stream, **opts),
+            lambda lg: lg.num_classes == int(net.num_classes) and lg._options() == dict(opts, stream=stream))
         if role == "test":
             log.set_threshold(qhat)
         res[role] = evaluate(net, loader, num_ens, train_size, conformal=log, **kw)
@@ -2310,43 +2341,17 @@ def route(experts, loader, num_ens: int, score: str = "epistemic", normalized: b
         ent["log"] = RouteLog(dev, n_img, K)
         ent["engines"].clear()              # the steps append to the log they were built with
     rlog = ent["log"] if log else None
-    acc, engines, nslots = ent["acc"], ent["engines"], max(2, int(inflight))
-    cur = torch.cuda.current_stream(dev)
-    acc.zero_()
+    ent["acc"].zero_()
     if rlog is not None:
         rlog.reset()
-    last = None
-    for x, y in loader:
-        shape = (tuple(x.shape), x.dtype)
-        e = engines.get(shape)
-        if e is None:
-            slots = [torch.zeros(x.shape, dtype=x.dtype, device=dev) for _ in range(nslots)]
-            eng = ExpertStep(experts, slots[0], num_ens, score=score, normalized=normalized, offsets=offsets,
-                             seed=ent["seed"], static_inputs=slots, first_replay=len(engines) << 16,
-                             inflight=inflight, metrics=acc, log=rlog, temperatures=temps)
-            ent["seed"] = eng.seed
-            e = engines[shape] = {"eng": eng, "slots": slots, "consumed": [None] * nslots, "steps": 0,
-                                  "labels": [torch.zeros(x.shape[0], dtype=torch.int64, device=dev) for _ in range(nslots)],
-                                  "pinned": [None] * nslots}
-        eng = e["eng"]
-        if last is not None and last is not eng:
-            last.wait()                         # the accumulator and the log take the steps one after another
-        s = e["steps"] % nslots
-        x, y = _pinned(e, s, x, y)
-        if e["consumed"][s] is not None:
-            cur.wait_event(e["consumed"][s])
-        e["slots"][s].copy_(x, non_blocking=True)
-        e["labels"][s].copy_(y, non_blocking=True)
-        if e["pinned"][s] is not None:
-            e["pinned"][s][2].record(cur)
-        eng(labels=e["labels"][s], task=task, slot=s)
-        e["consumed"][s] = eng.input_consumed()
-        e["steps"] += 1
-        last = eng
-    if last is None:
+
+    def build(slots, first_replay):
+        return ExpertStep(experts, slots[0], num_ens, score=score, normalized=normalized, offsets=offsets,
+                          seed=ent["seed"], static_inputs=slots, first_replay=first_replay, inflight=inflight,
+                          metrics=ent["acc"], log=rlog, temperatures=temps)
+    if not _run_loader(ent, loader, dev, max(2, int(inflight)), build, task=task):
         raise ValueError("route: the loader yielded no batch")
-    last.wait()
-    m = read_route_metrics(acc, K)
+    m = read_route_metrics(ent["acc"], K)
     if m["invalid"]:
         raise ValueError(f"route: {m['invalid']} labels are outside every expert's class range"
                          + (f" (task={task}: local classes 0..{experts[0].num_classes - 1})" if task is not None else ""))
@@ -2389,7 +2394,7 @@ def _expert_temperatures(temperatures, K):
     return temperatures
 
 
-class LogitBank(_CursorLog):
+class LogitBank(_SampleBank):
     """A device-resident bank of every Monte-Carlo sample's raw logits and the label of each image of a calibration set,
     appended to by the step (bbb_mc_logit_log): ``MCForward(..., logit_bank=bank)`` and ``evaluate(..., logit_bank=bank)``
     add one entry per image, in step order, with no host read.  It is what ``fit_temperature`` fits T on.
@@ -2399,6 +2404,9 @@ class LogitBank(_CursorLog):
     labels, which the fit refuses).  Unlike ProbBank (tf32 probabilities, which lose the small ones a temperature > 1
     raises) it keeps the logits themselves.  ``capacity`` entries fit; images past them are counted, not written, and
     ``read()`` and the fit refuse a bank that dropped any."""
+
+    _keyword = "logit_bank"
+    before_temper = True
 
     def __init__(self, device, capacity: int, num_ens: int, num_classes: int):
         num_ens, num_classes = int(num_ens), int(num_classes)
@@ -2421,26 +2429,18 @@ class LogitBank(_CursorLog):
         super().reset()
         self._unlabelled = False
 
-    def _require(self, num_ens, num_classes, what):
-        if (int(num_ens), int(num_classes)) != (self.num_ens, self.num_classes):
-            raise L.EngineError(f"{what}: the logit_bank holds {self.num_ens} samples x {self.num_classes} classes, "
-                                f"the step makes {num_ens} x {num_classes}")
-
     def _launch(self, logits, labels, B):
         L.check(L.lib().bbb_mc_logit_log(Fn._ptr(logits), Fn._ptr(labels), self.num_ens, int(B), self.num_classes,
                                          Fn._ptr(self._logits), Fn._ptr(self._labels), self.capacity,
                                          Fn._ptr(self._cursor), Fn._stream(self.device)), "bbb_mc_logit_log")
 
+    def _log(self, step, par):
+        self._launch(step.logits_all[par], step._labels_of(par), step.B)
+
     def append(self, logits, labels=None):
         """Append the images of per-sample logits [S, B, C] (fp32 contiguous on the bank's device) and their int64 labels
         [B] (bbb_mc_logit_log on the current stream): logits from anywhere else."""
-        Fn._require_cuda(self._cursor, "LogitBank.append")
-        if not (logits.dim() == 3 and logits.shape[0] == self.num_ens and logits.shape[2] == self.num_classes
-                and logits.shape[1] >= 1 and logits.dtype == torch.float32 and logits.is_contiguous()
-                and logits.device == self.device):
-            raise L.EngineError(f"LogitBank.append: expected contiguous float32 logits [{self.num_ens}, B, "
-                                f"{self.num_classes}] on {self.device}, got {logits.dtype} {tuple(logits.shape)} on "
-                                f"{logits.device}")
+        self._check_logits(logits)
         B = logits.shape[1]
         if labels is not None and not (labels.dtype == torch.int64 and tuple(labels.shape) == (B,)
                                        and labels.is_contiguous() and labels.device == self.device):
@@ -2589,17 +2589,9 @@ def calibrate_temperature(net, cal_loader, num_ens: int, t_min: float = 0.05, t_
     dev = next(net.parameters()).device
     kw = dict(evaluate_kwargs)
     train_size = kw.pop("train_size", 1.0)
-    n = _loader_images(cal_loader)
     S, Cc = int(num_ens), int(net.num_classes)
-    banks = net.__dict__.setdefault("_temperature_banks", {})
-    bank = banks.get("calibration")
-    if bank is None or bank.capacity < n or bank.device != dev or (bank.num_ens, bank.num_classes) != (S, Cc):
-        if bank is not None:                        # evaluate's engines that append to the old bank go with it
-            cache = net.__dict__.get("_mc_eval", {})
-            for k in [k for k, e in cache.items() if e.get("logit_bank") is bank]:
-                del cache[k]
-        bank = banks["calibration"] = LogitBank(dev, n, S, Cc)
-    bank.reset()
+    bank = _kept_log(net, net.__dict__.setdefault("_temperature_banks", {}), "calibration", cal_loader,
+                     lambda n: LogitBank(dev, n, S, Cc), lambda b: (b.num_ens, b.num_classes) == (S, Cc))
     m = evaluate(net, cal_loader, num_ens, train_size, logit_bank=bank, **kw)
     fit = fit_temperature(bank, t_min, t_max, grid, rounds, out=out, trace=trace)
     return {"temperature": fit.temperature, "fit": fit.read(), "evaluate": m}
