@@ -60,6 +60,28 @@ int sm_count() {
     return n;
 }
 
+// The end of every launch: the launcher's error, else the last error the launch left (a <<<>>> launch passes
+// cudaSuccess); on success `n` kernels are counted.
+int launched(cudaError_t e, const char* what, int n = 1) {
+    if (e == cudaSuccess) e = cudaGetLastError();
+    if (e != cudaSuccess) return cuda_fail(e, what);
+    g_launches += n;
+    return BBB_OK;
+}
+
+// Blocks of a grid-stride kernel over `work` items: one per `threads` items, at least 1, at most 8 per SM and `limit`.
+// The KL forward kernels reduce one partial per block, so their result's bits depend on this number.
+unsigned grid_blocks(uint64_t work, unsigned threads, uint64_t limit = UINT64_MAX) {
+    const uint64_t cap = std::min<uint64_t>((uint64_t)sm_count() * 8, limit);
+    return (unsigned)std::max<uint64_t>(1, std::min<uint64_t>((work + threads - 1) / threads, cap));
+}
+
+// The capacity of a cursor log: entry indices live in the cursor word's bits below its arrival count (score_log.cuh).
+int check_log(int64_t capacity) {
+    if (capacity < 0 || (uint64_t)capacity > bbb::SL_INDEX_MASK) return fail(BBB_E_INVALID, "bad capacity %lld", (long long)capacity);
+    return BBB_OK;
+}
+
 // Bytes of one set of prepared operands (tiles, zero sub-tile, bias rows) of whichever tensor-core path takes the layer.
 size_t tc_set_bytes(const bbb::Geom& g) {
     return std::max({bbb::tc_workspace_bytes(g), bbb::fused_workspace_bytes(g), bbb::conv_s4_workspace_bytes(g)});
@@ -256,9 +278,7 @@ int forward_impl(const bbb_layer_desc* d, bool linear, const void* x, const floa
         a.x = x; a.y = y; a.act_std = act_std; a.act_dtype = d->act_dtype;
         int nl = 0;
         cudaError_t e = bbb::launch_fwd_tc(a, st, sm_count(), &nl, prior_ptrs(prior, kl_out, mk));
-        if (e != cudaSuccess) return cuda_fail(e, "fwd_tc launch");
-        g_launches += nl;
-        return BBB_OK;
+        return launched(e, "fwd_tc launch", nl);
     }
 
     bbb::FwdArgs a;
@@ -272,9 +292,7 @@ int forward_impl(const bbb_layer_desc* d, bool linear, const void* x, const floa
     a.prior = prior_ptrs(prior, kl_out, mk);
     cudaError_t e = d->variant == BBB_VARIANT_LRT ? bbb::launch_fwd_simt<BBB_VARIANT_LRT>(a, st)
                                                   : bbb::launch_fwd_simt<BBB_VARIANT_BBB>(a, st);
-    if (e != cudaSuccess) return cuda_fail(e, "fwd_simt launch");
-    g_launches += 1;
-    return BBB_OK;
+    return launched(e, "fwd_simt launch");
 }
 
 int backward_impl(const bbb_layer_desc* d, bool linear, const void* x, const void* grad_y, const float* W_mu,
@@ -305,9 +323,7 @@ int backward_impl(const bbb_layer_desc* d, bool linear, const void* x, const voi
     a.prior = prior_ptrs(prior, nullptr, mk);       // the backward reads the mask only
     int nl = 0;
     cudaError_t e = bbb::launch_bwd_simt(a, (cudaStream_t)stream, sm_count(), &nl);
-    if (e != cudaSuccess) return cuda_fail(e, "bwd_simt launch");
-    g_launches += nl;
-    return BBB_OK;
+    return launched(e, "bwd_simt launch", nl);
 }
 
 }  // namespace
@@ -493,7 +509,7 @@ int bbb_layer_forward_fused_prior(const bbb_layer_desc* d, const void* x, const 
                    bbb::conv_s4_bias_offset(g), fold, "conv_s4_prep", timed && !skip_prep, "conv_s4", timed && !prep_only);
         a.x = (const float*)x; a.y = y; a.y_sq = y_sq; a.out_pitch = out_pitch;
         cudaError_t e = bbb::launch_conv_s4(a, st, !skip_prep, !prep_only, &nl, prior_ptrs(prior, kl_out, mk));
-        if (e != cudaSuccess) return cuda_fail(e, "conv_s4 launch");
+        return launched(e, "conv_s4 launch", nl);
     } else if (in_layout == BBB_LAYOUT_NCHW_F32) {
         bbb::TcArgs a;                  // fold.rows = 0: fused_check refuses a fold on the gather path
         layer_args(a, d, g, W_mu, W_rho, bias_mu, bias_rho, kl_out, eps_a, eps_b, seed, stream_id, stream_base, ws,
@@ -501,7 +517,7 @@ int bbb_layer_forward_fused_prior(const bbb_layer_desc* d, const void* x, const 
         a.x = x; a.y = y; a.act_std = nullptr; a.act_dtype = d->act_dtype; a.tf32 = 0;
         a.skip_prep = skip_prep; a.prep_only = prep_only; a.y_sq = y_sq; a.out_mode = out_mode == 1 ? 2 : out_mode; a.out_pitch = out_pitch; a.pool = pool;
         cudaError_t e = bbb::launch_fwd_tc(a, st, sm_count(), &nl, prior_ptrs(prior, kl_out, mk));
-        if (e != cudaSuccess) return cuda_fail(e, "fused gather launch");
+        return launched(e, "fused gather launch", nl);
     } else if (in_layout == BBB_LAYOUT_PACKED_BF16) {
         bbb::FusedArgs a;
         layer_args(a, d, g, W_mu, W_rho, bias_mu, bias_rho, kl_out, eps_a, eps_b, seed, stream_id, stream_base, ws,
@@ -512,11 +528,10 @@ int bbb_layer_forward_fused_prior(const bbb_layer_desc* d, const void* x, const 
         cudaError_t e = bbb::launch_fused(a, x, x_sq, st, &nl, &why, !skip_prep, !prep_only, sm_count(), g_wide_tiles.load() != 0,
                                           prior_ptrs(prior, kl_out, mk));
         if (e != cudaSuccess) return fail(BBB_E_CUDA, "fused tap-GEMM launch: %s %s", cudaGetErrorString(e), why);
+        return launched(e, "fused tap-GEMM launch", nl);
     } else {
         return fail(BBB_E_INVALID, "bad in_layout %d", in_layout);
     }
-    g_launches += nl;
-    return BBB_OK;
 }
 
 int bbb_kl_forward(const float* W_mu, const float* W_rho, uint64_t n_w, const float* bias_mu,
@@ -536,33 +551,25 @@ int bbb_kl_forward_prior(const float* W_mu, const float* W_rho, uint64_t n_w, co
     if (!workspace || workspace_bytes < kBaseWorkspace) return fail(BBB_E_WORKSPACE, "workspace too small: need %zu bytes", kBaseWorkspace);
     const bool tensor_prior = prior && prior->w_mu, masked = mk.w != nullptr;
     if (!tensor_prior && !(prior_sigma > 0.0f)) return fail(BBB_E_INVALID, "prior_sigma must be > 0");
-    const uint64_t work = (n_w + 3) / 4 + n_b;
-    uint64_t blocks = (work + 255) / 256;
-    const uint64_t cap = (uint64_t)sm_count() * 8;
-    if (blocks > cap) blocks = cap;
-    if (blocks < 1) blocks = 1;
-    if (blocks > kMaxKlSlots) blocks = kMaxKlSlots;
+    const unsigned blocks = grid_blocks((n_w + 3) / 4 + n_b, 256, kMaxKlSlots);
     double* partials = (double*)((char*)workspace + kCounterBytes);
     if (masked && tensor_prior)
-        bbb::kl_forward_masked_kernel<true><<<(unsigned)blocks, 256, 0, (cudaStream_t)cuda_stream>>>(
+        bbb::kl_forward_masked_kernel<true><<<blocks, 256, 0, (cudaStream_t)cuda_stream>>>(
             W_mu, W_rho, n_w, bias_mu, bias_rho, n_b, 0.0f, 1.0f, prior_ptrs(prior, kl_out, mk), kl_convention, partials,
             (unsigned int*)workspace, kl_out);
     else if (masked)
-        bbb::kl_forward_masked_kernel<false><<<(unsigned)blocks, 256, 0, (cudaStream_t)cuda_stream>>>(
+        bbb::kl_forward_masked_kernel<false><<<blocks, 256, 0, (cudaStream_t)cuda_stream>>>(
             W_mu, W_rho, n_w, bias_mu, bias_rho, n_b, prior_mu, prior_sigma, prior_ptrs(prior, kl_out, mk), kl_convention,
             partials, (unsigned int*)workspace, kl_out);
     else if (prior)
-        bbb::kl_forward_prior_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)cuda_stream>>>(
+        bbb::kl_forward_prior_kernel<<<blocks, 256, 0, (cudaStream_t)cuda_stream>>>(
             W_mu, W_rho, n_w, bias_mu, bias_rho, n_b, prior_ptrs(prior, kl_out), kl_convention, partials,
             (unsigned int*)workspace, kl_out);
     else
-        bbb::kl_forward_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)cuda_stream>>>(
+        bbb::kl_forward_kernel<<<blocks, 256, 0, (cudaStream_t)cuda_stream>>>(
             W_mu, W_rho, n_w, bias_mu, bias_rho, n_b, prior_mu, prior_sigma, kl_convention, partials,
             (unsigned int*)workspace, kl_out);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return cuda_fail(e, "kl_forward launch");
-    g_launches += 1;
-    return BBB_OK;
+    return launched(cudaSuccess, "kl_forward launch");
 }
 
 int bbb_kl_backward(const float* mu, const float* rho, uint64_t n, float prior_mu, float prior_sigma,
@@ -578,25 +585,19 @@ int bbb_kl_backward_prior(const float* mu, const float* rho, uint64_t n, float p
     if (!mu || !rho || !grad_kl || !g_mu || !g_rho) return fail(BBB_E_INVALID, "NULL tensor pointer");
     if (int rc = check_prior(prior, false, mk)) return rc;   // the n elements' prior is prior->w_mu / w_sigma
     if (n == 0) return BBB_OK;
-    uint64_t blocks = (n + 255) / 256;
-    const uint64_t cap = (uint64_t)sm_count() * 8;
-    if (blocks > cap) blocks = cap;
+    const unsigned blocks = grid_blocks(n, 256);
     const bool tensor_prior = prior && prior->w_mu;
     if (mk.w)
         (tensor_prior ? bbb::kl_backward_masked_kernel<true> : bbb::kl_backward_masked_kernel<false>)
-            <<<(unsigned)blocks, 256, 0, (cudaStream_t)cuda_stream>>>(mu, rho, n, prior_mu, prior_sigma, prior->w_mu,
-                                                                      prior->w_sigma, mk.w, kl_convention,
-                                                                      grad_kl, g_mu, g_rho);
+            <<<blocks, 256, 0, (cudaStream_t)cuda_stream>>>(mu, rho, n, prior_mu, prior_sigma, prior->w_mu,
+                                                            prior->w_sigma, mk.w, kl_convention, grad_kl, g_mu, g_rho);
     else if (prior)
-        bbb::kl_backward_prior_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)cuda_stream>>>(
+        bbb::kl_backward_prior_kernel<<<blocks, 256, 0, (cudaStream_t)cuda_stream>>>(
             mu, rho, n, prior->w_mu, prior->w_sigma, kl_convention, grad_kl, g_mu, g_rho);
     else
-        bbb::kl_backward_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)cuda_stream>>>(
+        bbb::kl_backward_kernel<<<blocks, 256, 0, (cudaStream_t)cuda_stream>>>(
             mu, rho, n, prior_mu, prior_sigma, kl_convention, grad_kl, g_mu, g_rho);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return cuda_fail(e, "kl_backward launch");
-    g_launches += 1;
-    return BBB_OK;
+    return launched(cudaSuccess, "kl_backward launch");
 }
 
 size_t bbb_kl_mc_workspace_bytes(int32_t n_draws) {
@@ -614,25 +615,18 @@ int bbb_kl_mc_forward(const float* W_mu, const float* W_rho, uint64_t n_w, const
     if (int rc = check_mixture(prior, n_draws, q)) return rc;
     const size_t need = bbb_kl_mc_workspace_bytes(n_draws);
     if (!workspace || workspace_bytes < need) return fail(BBB_E_WORKSPACE, "workspace too small: need %zu bytes", need);
-    const uint64_t work = n_w / 4 + n_w % 4 + n_b;
-    uint64_t blocks = (work + bbb::KL_MC_THREADS - 1) / bbb::KL_MC_THREADS;
-    const uint64_t cap = (uint64_t)sm_count() * 8;
-    if (blocks > cap) blocks = cap;
-    if (blocks < 1) blocks = 1;
-    if (blocks > kMaxKlSlots) blocks = kMaxKlSlots;
+    const unsigned blocks = grid_blocks(n_w / 4 + n_w % 4 + n_b, bbb::KL_MC_THREADS, kMaxKlSlots);
     unsigned int* counters = (unsigned int*)workspace;
     double* partials = (double*)((char*)workspace + kl_mc_counter_bytes((size_t)n_draws));
     // the draws go in launches of at most KL_MC_MAX_DRAWS, each draw with its own counter and partial row
     for (int32_t d0 = 0; d0 < n_draws; d0 += bbb::KL_MC_MAX_DRAWS) {
         const int nd = std::min<int32_t>(bbb::KL_MC_MAX_DRAWS, n_draws - d0);
-        bbb::kl_mc_forward_kernel<<<(unsigned)blocks, bbb::KL_MC_THREADS, (size_t)nd * bbb::KL_MC_THREADS * sizeof(double),
+        bbb::kl_mc_forward_kernel<<<blocks, bbb::KL_MC_THREADS, (size_t)nd * bbb::KL_MC_THREADS * sizeof(double),
                                     (cudaStream_t)cuda_stream>>>(
             W_mu, W_rho, n_w, bias_mu, bias_rho, n_b, q, bbb::make_key(seed, stream_id + (uint64_t)d0 * draw_stride),
             (const unsigned long long*)stream_base, nd, draw_stride, counters + d0, partials + (size_t)d0 * kMaxKlSlots,
             kl_out + d0);
-        cudaError_t e = cudaGetLastError();
-        if (e != cudaSuccess) return cuda_fail(e, "kl_mc_forward launch");
-        g_launches += 1;
+        if (int rc = launched(cudaSuccess, "kl_mc_forward launch")) return rc;
     }
     return BBB_OK;
 }
@@ -645,30 +639,20 @@ int bbb_kl_mc_backward(const float* mu, const float* rho, uint64_t n, uint64_t f
     bbb::MixPrior q;
     if (int rc = check_mixture(prior, n_draws, q)) return rc;
     if (n == 0) return BBB_OK;
-    uint64_t blocks = ((n + 3) / 4 + bbb::KL_MC_THREADS - 1) / bbb::KL_MC_THREADS;
-    const uint64_t cap = (uint64_t)sm_count() * 8;
-    if (blocks > cap) blocks = cap;
-    bbb::kl_mc_backward_kernel<<<(unsigned)blocks, bbb::KL_MC_THREADS, 0, (cudaStream_t)cuda_stream>>>(
+    bbb::kl_mc_backward_kernel<<<grid_blocks((n + 3) / 4, bbb::KL_MC_THREADS), bbb::KL_MC_THREADS, 0,
+                                 (cudaStream_t)cuda_stream>>>(
         mu, rho, n, first_element, q, bbb::make_key(seed, stream_id), (const unsigned long long*)stream_base, n_draws,
         draw_stride, grad_kl, g_mu, g_rho);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return cuda_fail(e, "kl_mc_backward launch");
-    g_launches += 1;
-    return BBB_OK;
+    return launched(cudaSuccess, "kl_mc_backward launch");
 }
 
 int bbb_philox_normal_fill(float* out, uint64_t n, uint64_t seed, uint64_t stream_id, uint64_t offset,
                            void* cuda_stream) {
     if (!out) return fail(BBB_E_INVALID, "NULL output pointer");
     if (n == 0) return BBB_OK;
-    uint64_t blocks = (n + 255) / 256;
-    const uint64_t cap = (uint64_t)sm_count() * 8;
-    if (blocks > cap) blocks = cap;
-    bbb::philox_fill_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)cuda_stream>>>(out, n, bbb::make_key(seed, stream_id), offset);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return cuda_fail(e, "philox_fill launch");
-    g_launches += 1;
-    return BBB_OK;
+    bbb::philox_fill_kernel<<<grid_blocks(n, 256), 256, 0, (cudaStream_t)cuda_stream>>>(
+        out, n, bbb::make_key(seed, stream_id), offset);
+    return launched(cudaSuccess, "philox_fill launch");
 }
 
 int bbb_lrt_noise_grad(const bbb_layer_desc* d, const float* grad_y, const float* act_std, uint64_t seed,
@@ -683,22 +667,16 @@ int bbb_lrt_noise_grad(const bbb_layer_desc* d, const float* grad_y, const float
     bbb::McFold fold;
     if (int rc = layer_fold(d, g, nullptr, nullptr, fold)) return rc;
     const bool vec4 = g.N % 4 == 0;
-    const uint64_t work = (uint64_t)g.B * (vec4 ? g.N / 4 : g.N) * g.OHW;
-    uint64_t blocks = (work + 255) / 256;
-    const uint64_t cap = (uint64_t)sm_count() * 8;
-    if (blocks > cap) blocks = cap;
+    const unsigned blocks = grid_blocks((uint64_t)g.B * (vec4 ? g.N / 4 : g.N) * g.OHW, 256);
     const bbb::NoiseKey key = bbb::make_key(seed, stream_id);
     const auto* base = (const unsigned long long*)stream_base;
     if (vec4)
-        bbb::lrt_noise_grad_kernel<true><<<(unsigned)blocks, 256, 0, (cudaStream_t)cuda_stream>>>(
+        bbb::lrt_noise_grad_kernel<true><<<blocks, 256, 0, (cudaStream_t)cuda_stream>>>(
             grad_y, act_std, gv, g.B, g.N, g.OHW, key, base, fold);
     else
-        bbb::lrt_noise_grad_kernel<false><<<(unsigned)blocks, 256, 0, (cudaStream_t)cuda_stream>>>(
+        bbb::lrt_noise_grad_kernel<false><<<blocks, 256, 0, (cudaStream_t)cuda_stream>>>(
             grad_y, act_std, gv, g.B, g.N, g.OHW, key, base, fold);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return cuda_fail(e, "lrt_noise_grad launch");
-    g_launches += 1;
-    return BBB_OK;
+    return launched(cudaSuccess, "lrt_noise_grad launch");
 }
 
 int bbb_mc_combine(const float* logits, int32_t S, int32_t B, int32_t C, float* log_outputs, float* moments,
@@ -707,10 +685,7 @@ int bbb_mc_combine(const float* logits, int32_t S, int32_t B, int32_t C, float* 
     if (S <= 0 || B <= 0 || C <= 0) return fail(BBB_E_INVALID, "bad S/B/C");
     if ((size_t)S * sizeof(float) > 40000) return fail(BBB_E_UNSUPPORTED, "S too large");
     bbb::mc_combine_kernel<<<B, 128, S * sizeof(float), (cudaStream_t)cuda_stream>>>(logits, S, B, C, log_outputs, moments);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return cuda_fail(e, "mc_combine launch");
-    g_launches += 1;
-    return BBB_OK;
+    return launched(cudaSuccess, "mc_combine launch");
 }
 
 size_t bbb_mc_buffer_bytes(int32_t B, int32_t C, int32_t flags, int32_t world) {
@@ -772,10 +747,7 @@ static int mc_exchange_impl(const float* logits, int32_t S_local, int32_t S_tota
     cudaError_t e = bbb::launch_pdl(kern,
                                      dim3(grid), dim3(bbb::MCX_THREADS), bbb::mcx_smem_bytes(S_local, metrics != nullptr),
                                      (cudaStream_t)cuda_stream, a);
-    if (e == cudaSuccess) e = cudaGetLastError();
-    if (e != cudaSuccess) return cuda_fail(e, "mc_exchange launch");
-    g_launches += 1;
-    return BBB_OK;
+    return launched(e, "mc_exchange launch");
 }
 int bbb_mc_exchange_info(const float* logits, int32_t S_local, int32_t S_total, int32_t B, int32_t C, const float* kl,
                          int32_t n_kl, int32_t flags, const int64_t* labels, float train_size, float beta, int32_t rank,
@@ -826,7 +798,7 @@ int bbb_mc_score_log(const float* log_outputs, const float* entropy, const float
                      float* planes, int32_t* pred, int64_t capacity, int64_t* cursor, void* cuda_stream) {
     if (!log_outputs || !planes || !pred || !cursor) return fail(BBB_E_INVALID, "NULL pointer");
     if (B <= 0 || C <= 0) return fail(BBB_E_INVALID, "bad B/C %d/%d", B, C);
-    if (capacity < 0 || (uint64_t)capacity > bbb::SL_INDEX_MASK) return fail(BBB_E_INVALID, "bad capacity %lld", (long long)capacity);
+    if (int rc = check_log(capacity)) return rc;
     bbb::ScoreLogArgs a;
     a.log_outputs = log_outputs; a.entropy = entropy; a.expected_entropy = expected_entropy; a.mutual_info = mutual_info;
     a.epistemic = epistemic; a.labels = (const long long*)labels; a.B = B; a.C = C;
@@ -834,10 +806,7 @@ int bbb_mc_score_log(const float* log_outputs, const float* entropy, const float
     int grid = (B + bbb::SL_THREADS / 32 - 1) / (bbb::SL_THREADS / 32);
     if (grid > bbb::SL_MAX_CTAS) grid = bbb::SL_MAX_CTAS;
     bbb::mc_score_log_kernel<<<grid, bbb::SL_THREADS, 0, (cudaStream_t)cuda_stream>>>(a);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return cuda_fail(e, "mc_score_log launch");
-    g_launches += 1;
-    return BBB_OK;
+    return launched(cudaSuccess, "mc_score_log launch");
 }
 
 static int pb_pad_s(int S) { return (S + 7) / 8 * 8; }
@@ -848,7 +817,7 @@ int bbb_mc_prob_log(const float* logits, int32_t S, int32_t B, int32_t C, int32_
     if (!logits || !bank || !expected_entropy || !cursor) return fail(BBB_E_INVALID, "NULL pointer");
     if (S < 1 || S > BBB_BANK_MAX_SAMPLES || C < 2 || C > BBB_BANK_MAX_CLASSES || B <= 0)
         return fail(BBB_E_INVALID, "bad S/B/C %d/%d/%d", S, B, C);
-    if (capacity < 0 || (uint64_t)capacity > bbb::SL_INDEX_MASK) return fail(BBB_E_INVALID, "bad capacity %lld", (long long)capacity);
+    if (int rc = check_log(capacity)) return rc;
     bbb::ProbLogArgs a;
     a.logits = logits; a.S = S; a.B = B; a.C = C; a.S_pad = pb_pad_s(S); a.C_pad = pb_pad_c(C);
     a.normalized = normalized != 0; a.bank = bank; a.expected_entropy = expected_entropy; a.capacity = capacity;
@@ -856,10 +825,7 @@ int bbb_mc_prob_log(const float* logits, int32_t S, int32_t B, int32_t C, int32_
     int grid = (B + bbb::PB_THREADS / 32 - 1) / (bbb::PB_THREADS / 32);
     if (grid > bbb::PB_MAX_CTAS) grid = bbb::PB_MAX_CTAS;
     bbb::mc_prob_log_kernel<<<grid, bbb::PB_THREADS, 0, (cudaStream_t)cuda_stream>>>(a);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return cuda_fail(e, "mc_prob_log launch");
-    g_launches += 1;
-    return BBB_OK;
+    return launched(cudaSuccess, "mc_prob_log launch");
 }
 
 int bbb_mc_conformal_log(const float* log_outputs, const int64_t* labels, int32_t B, int32_t C, int32_t method,
@@ -872,7 +838,7 @@ int bbb_mc_conformal_log(const float* log_outputs, const int64_t* labels, int32_
     if (method != BBB_CONFORMAL_LAC && method != BBB_CONFORMAL_APS && method != BBB_CONFORMAL_RAPS)
         return fail(BBB_E_INVALID, "bad method %d", method);
     if (!(lam >= 0.0) || !std::isfinite(lam) || k_reg < 0) return fail(BBB_E_INVALID, "bad lam/k_reg %g/%d", lam, k_reg);
-    if (capacity < 0 || (uint64_t)capacity > bbb::SL_INDEX_MASK) return fail(BBB_E_INVALID, "bad capacity %lld", (long long)capacity);
+    if (int rc = check_log(capacity)) return rc;
     bbb::ConformalArgs a;
     a.log_outputs = log_outputs; a.labels = (const long long*)labels; a.B = B; a.C = C;
     a.n_sort = 32;
@@ -889,10 +855,7 @@ int bbb_mc_conformal_log(const float* log_outputs, const int64_t* labels, int32_
     int grid = (B + nwarp - 1) / nwarp;
     if (grid > bbb::CF_MAX_CTAS) grid = bbb::CF_MAX_CTAS;
     bbb::conformal_log_kernel<<<grid, nwarp * 32, (size_t)nwarp * per_warp, (cudaStream_t)cuda_stream>>>(a);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return cuda_fail(e, "mc_conformal_log launch");
-    g_launches += 1;
-    return BBB_OK;
+    return launched(cudaSuccess, "mc_conformal_log launch");
 }
 
 size_t bbb_mc_route_bytes(void) { return bbb::rt_acc_bytes(); }
@@ -906,9 +869,10 @@ int bbb_mc_route(const bbb_route_expert* experts, const int32_t* offsets, int32_
     if (score < BBB_ROUTE_EPISTEMIC || score > BBB_ROUTE_CONFIDENCE) return fail(BBB_E_INVALID, "bad score %d", score);
     if (task < -1 || task >= K) return fail(BBB_E_INVALID, "bad task %d (K = %d)", task, K);
     if (acc && !labels) return fail(BBB_E_INVALID, "an accumulator needs labels");
-    if (cursor && (!log_expert || !log_local || !log_pred || !log_scores || capacity < 0 ||
-                   (uint64_t)capacity > bbb::SL_INDEX_MASK))
-        return fail(BBB_E_INVALID, "bad log (capacity %lld)", (long long)capacity);
+    if (cursor) {
+        if (!log_expert || !log_local || !log_pred || !log_scores) return fail(BBB_E_INVALID, "bad log: NULL plane");
+        if (int rc = check_log(capacity)) return rc;
+    }
     bbb::RouteArgs a = {};
     for (int e = 0; e < K; ++e) {
         const bbb_route_expert& x = experts[e];
@@ -929,10 +893,7 @@ int bbb_mc_route(const bbb_route_expert* experts, const int32_t* offsets, int32_
     int grid = (B + bbb::RT_WARPS - 1) / bbb::RT_WARPS;          // a function of B alone (the accumulator's sum order)
     if (grid > bbb::RT_MAX_CTAS) grid = bbb::RT_MAX_CTAS;
     bbb::mc_route_kernel<<<grid, bbb::RT_THREADS, 0, (cudaStream_t)cuda_stream>>>(a);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return cuda_fail(e, "mc_route launch");
-    g_launches += 1;
-    return BBB_OK;
+    return launched(cudaSuccess, "mc_route launch");
 }
 
 int bbb_mc_logit_log(const float* logits, const int64_t* labels, int32_t S, int32_t B, int32_t C, float* bank,
@@ -940,16 +901,13 @@ int bbb_mc_logit_log(const float* logits, const int64_t* labels, int32_t S, int3
     if (!logits || !bank || !bank_labels || !cursor) return fail(BBB_E_INVALID, "NULL pointer");
     if (S < 1 || S > BBB_LOGIT_BANK_MAX_SAMPLES || C < 2 || C > BBB_LOGIT_BANK_MAX_CLASSES || B <= 0)
         return fail(BBB_E_INVALID, "bad S/B/C %d/%d/%d", S, B, C);
-    if (capacity < 0 || (uint64_t)capacity > bbb::SL_INDEX_MASK) return fail(BBB_E_INVALID, "bad capacity %lld", (long long)capacity);
+    if (int rc = check_log(capacity)) return rc;
     bbb::LogitLogArgs a;
     a.logits = logits; a.labels = (const long long*)labels; a.S = S; a.B = B; a.C = C; a.bank = bank;
     a.bank_labels = (long long*)bank_labels; a.capacity = capacity; a.cursor = (unsigned long long*)cursor;
     const int grid = B < bbb::LL_MAX_CTAS ? B : bbb::LL_MAX_CTAS;
     bbb::mc_logit_log_kernel<<<grid, bbb::LL_THREADS, 0, (cudaStream_t)cuda_stream>>>(a);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return cuda_fail(e, "mc_logit_log launch");
-    g_launches += 1;
-    return BBB_OK;
+    return launched(cudaSuccess, "mc_logit_log launch");
 }
 
 size_t bbb_temperature_workspace_bytes(int32_t n, int32_t K) {
@@ -982,10 +940,7 @@ int bbb_temperature_nll(const float* logits, const int64_t* labels, const int64_
     a.arrive = (unsigned int*)workspace; a.partials = (double*)((char*)workspace + 16);
     const int grid = (n + bbb::TN_CTA_IMAGES - 1) / bbb::TN_CTA_IMAGES;
     bbb::temperature_nll_kernel<<<grid, bbb::TN_THREADS, 0, (cudaStream_t)cuda_stream>>>(a);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return cuda_fail(e, "temperature_nll launch");
-    g_launches += 1;
-    return BBB_OK;
+    return launched(cudaSuccess, "temperature_nll launch");
 }
 
 int bbb_mc_temper(float* logits, int64_t n, const float* temperature, void* cuda_stream) {
@@ -996,10 +951,7 @@ int bbb_mc_temper(float* logits, int64_t n, const float* temperature, void* cuda
     if (grid > bbb::TP_MAX_CTAS) grid = bbb::TP_MAX_CTAS;
     cudaError_t e = bbb::launch_pdl(bbb::mc_temper_kernel, dim3((unsigned)grid), dim3(bbb::TP_THREADS), 0,
                                     (cudaStream_t)cuda_stream, logits, (long long)n, temperature);
-    if (e == cudaSuccess) e = cudaGetLastError();
-    if (e != cudaSuccess) return cuda_fail(e, "mc_temper launch");
-    g_launches += 1;
-    return BBB_OK;
+    return launched(e, "mc_temper launch");
 }
 
 size_t bbb_joint_entropy_workspace_bytes(int32_t N, int32_t S, int32_t C, int32_t M) {
@@ -1023,10 +975,7 @@ int bbb_joint_entropy(const float* pt, const double* omega, const uint8_t* mask,
     cudaError_t e = cudaFuncSetAttribute(bbb::joint_entropy_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return cuda_fail(e, "joint_entropy smem attribute");
     bbb::joint_entropy_kernel<<<(N + cand - 1) / cand, bbb::JE_THREADS, smem, (cudaStream_t)cuda_stream>>>(a);
-    e = cudaGetLastError();
-    if (e != cudaSuccess) return cuda_fail(e, "joint_entropy launch");
-    g_launches += 1;
-    return BBB_OK;
+    return launched(cudaSuccess, "joint_entropy launch");
 }
 
 int bbb_comm_alloc(size_t bytes, void** dev_ptr) {
@@ -1067,10 +1016,7 @@ int bbb_comm_unimport(void* peer_ptr) {
 int bbb_noise_advance(uint64_t* base, uint64_t inc, void* cuda_stream) {
     if (!base) return fail(BBB_E_INVALID, "NULL base pointer");
     bbb::noise_advance_kernel<<<1, 1, 0, (cudaStream_t)cuda_stream>>>((unsigned long long*)base, (unsigned long long)inc);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return cuda_fail(e, "noise_advance launch");
-    g_launches += 1;
-    return BBB_OK;
+    return launched(cudaSuccess, "noise_advance launch");
 }
 
 int bbb_mc_graph_step(void* caller_stream, void* run_stream, void* in_ready, void* wait_a, void* wait_b,

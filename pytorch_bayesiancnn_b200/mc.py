@@ -53,6 +53,17 @@ def shard_layout(world: int, rank: int, batch_shards: int = 1):
     return rs, rank % rs, rank // rs
 
 
+def _check_tensor(t, what, shape=None, dtype=None, device=None):
+    """Raise EngineError unless ``t`` is contiguous and has the ``shape``, ``dtype`` and ``device`` given (None: any)."""
+    shape = None if shape is None else tuple(shape)
+    if t.is_contiguous() and all(w is None or w == g for w, g in ((shape, tuple(t.shape)), (dtype, t.dtype),
+                                                                    (device, t.device))):
+        return
+    want = "".join((f" {dtype}" if dtype else "", " tensor", "" if shape is None else f" of shape {shape}",
+                    f" on {device}" if device else ""))
+    raise L.EngineError(f"{what}: expected a contiguous{want}, got {t.dtype} {tuple(t.shape)} on {t.device}")
+
+
 def get_beta(batch_idx, m, beta_type, epoch=None, num_epochs=None):
     """metrics.py:32-46 (host scalar; it only feeds the `beta` argument of the ELBO head)."""
     if isinstance(beta_type, (int, float)):
@@ -216,11 +227,10 @@ class MCForward:
         if metrics is not None:
             if not with_labels:
                 raise L.EngineError("MCForward: metrics needs with_labels")
+            _check_tensor(metrics, "MCForward: metrics", dtype=torch.float64, device=example_x.device)
             n = int(lib.bbb_mc_metrics_bytes()) // 8
-            if not (metrics.device == example_x.device and metrics.dtype == torch.float64 and metrics.is_contiguous()
-                    and metrics.numel() >= n):
-                raise L.EngineError(f"MCForward: metrics must be a contiguous float64 tensor of >= {n} elements on "
-                                    f"{example_x.device} (mc.new_metrics)")
+            if metrics.numel() < n:
+                raise L.EngineError(f"MCForward: metrics holds {metrics.numel()} float64 elements, < {n} (mc.new_metrics)")
         self.metrics = self._metrics = metrics      # _metrics: the accumulator the exchange adds to
         self.net, self.group = net, group
         self.dist, self.world, self.rank = _dist_info(group)
@@ -1055,10 +1065,8 @@ class ScoreLog(_CursorLog):
         for t, shape, dt in ((log_outputs, (B, Cc), torch.float32), (entropy, (B,), torch.float32),
                              (expected_entropy, (B,), torch.float32), (mutual_info, (B,), torch.float32),
                              (epistemic, (B, Cc), torch.float32), (labels, (B,), torch.int64)):
-            if t is not None and not (t.device == self.device and tuple(t.shape) == shape and t.dtype == dt
-                                      and t.is_contiguous()):
-                raise L.EngineError(f"ScoreLog.append: expected a contiguous {dt} tensor of shape {shape} on "
-                                    f"{self.device}, got {t.dtype} {tuple(t.shape)} on {t.device}")
+            if t is not None:
+                _check_tensor(t, "ScoreLog.append", shape, dt, self.device)
         L.check(L.lib().bbb_mc_score_log(Fn._ptr(log_outputs), Fn._ptr(entropy), Fn._ptr(expected_entropy),
                                          Fn._ptr(mutual_info), Fn._ptr(epistemic), Fn._ptr(labels), B, Cc,
                                          Fn._ptr(self._planes), Fn._ptr(self._pred), self.capacity,
@@ -1557,11 +1565,9 @@ class _SampleBank(_CursorLog):
         """Refuse anything but per-sample logits [S, B, C] of this bank: fp32, contiguous, on its device."""
         what = f"{type(self).__name__}.append"
         Fn._require_cuda(self._cursor, what)
-        if not (logits.dim() == 3 and logits.shape[0] == self.num_ens and logits.shape[2] == self.num_classes
-                and logits.shape[1] >= 1 and logits.dtype == torch.float32 and logits.is_contiguous()
-                and logits.device == self.device):
-            raise L.EngineError(f"{what}: expected contiguous float32 logits [{self.num_ens}, B, {self.num_classes}] "
-                                f"on {self.device}, got {logits.dtype} {tuple(logits.shape)} on {logits.device}")
+        B = max(1, logits.shape[1]) if logits.dim() == 3 else 1        # an empty batch is refused
+        _check_tensor(logits, f"{what}: expected contiguous float32 logits [S, B, C]",
+                      (self.num_ens, B, self.num_classes), torch.float32, self.device)
 
 
 class ProbBank(_SampleBank):
@@ -1861,12 +1867,10 @@ class ConformalLog(_CursorLog):
         """Append one step's images (bbb_mc_conformal_log on the current stream): log p_bar [B, C] fp32 and optional
         int64 labels [B], contiguous on the log's device."""
         Fn._require_cuda(self._cursor, "ConformalLog.append")
-        B = int(log_outputs.shape[0]) if log_outputs.dim() == 2 else 0
+        B = max(1, int(log_outputs.shape[0])) if log_outputs.dim() == 2 else 1     # an empty batch is refused
         for t, shape, dt in ((log_outputs, (B, self.num_classes), torch.float32), (labels, (B,), torch.int64)):
-            if t is not None and not (B >= 1 and t.device == self.device and tuple(t.shape) == shape and t.dtype == dt
-                                      and t.is_contiguous()):
-                raise L.EngineError(f"ConformalLog.append: expected a contiguous {dt} tensor of shape {shape} on "
-                                    f"{self.device}, got {t.dtype} {tuple(t.shape)} on {t.device}")
+            if t is not None:
+                _check_tensor(t, "ConformalLog.append", shape, dt, self.device)
         self._launch(log_outputs, labels)
 
     def read(self) -> dict:
@@ -2112,21 +2116,17 @@ def _route_launcher(outs, score, offsets, metrics, log, result):
                 if name in need:
                     raise L.EngineError(f"route: expert {e} has no {name!r} plane (score {score!r})")
                 continue
-            if not (t.device == dev and tuple(t.shape) == shape and t.dtype == torch.float32 and t.is_contiguous()):
-                raise L.EngineError(f"route: expert {e}'s {name!r} must be a contiguous float32 tensor of shape "
-                                    f"{shape} on {dev}, got {t.dtype} {tuple(t.shape)} on {t.device}")
+            _check_tensor(t, f"route: expert {e}'s {name!r}", shape, torch.float32, dev)
             setattr(table[e], name, t.data_ptr())
     offs = (C.c_int32 * K)(*_route_offsets(offsets, K, Cc))
-    if metrics is not None and not (metrics.device == dev and metrics.dtype == torch.float64 and metrics.is_contiguous()
-                                    and metrics.numel() * 8 >= int(L.lib().bbb_mc_route_bytes())):
-        raise L.EngineError(f"route: metrics must be a contiguous float64 tensor from new_route_metrics on {dev}")
+    if metrics is not None:
+        _check_tensor(metrics, "route: metrics", dtype=torch.float64, device=dev)
+        if metrics.numel() * 8 < int(L.lib().bbb_mc_route_bytes()):
+            raise L.EngineError(f"route: metrics holds {metrics.numel()} float64 elements, fewer than new_route_metrics")
     if log is not None and (log.device != dev or log.num_experts != K):
         raise L.EngineError(f"route: the log holds {log.num_experts} experts on {log.device}, the step {K} on {dev}")
     for k, shape in (("expert", (B,)), ("local", (B,)), ("pred", (B,)), ("scores", (B, K))):
-        t = result[k]
-        if not (t.device == dev and tuple(t.shape) == shape and t.is_contiguous() and
-                t.dtype == (torch.float32 if k == "scores" else torch.int32)):
-            raise L.EngineError(f"route: result {k!r} has the wrong shape, type or device")
+        _check_tensor(result[k], f"route: result {k!r}", shape, torch.float32 if k == "scores" else torch.int32, dev)
     lg = log is not None
     fixed = (Fn._ptr(result["expert"]), Fn._ptr(result["local"]), Fn._ptr(result["pred"]), Fn._ptr(result["scores"]))
     logs = (Fn._ptr(log._ints[0] if lg else None), Fn._ptr(log._ints[1] if lg else None),
@@ -2135,9 +2135,8 @@ def _route_launcher(outs, score, offsets, metrics, log, result):
     fn = L.lib().bbb_mc_route
 
     def launch(labels, task):
-        if labels is not None and not (labels.device == dev and tuple(labels.shape) == (B,) and
-                                       labels.dtype == torch.int64 and labels.is_contiguous()):
-            raise L.EngineError(f"route: labels must be a contiguous int64 tensor of shape ({B},) on {dev}")
+        if labels is not None:
+            _check_tensor(labels, "route: labels", (B,), torch.int64, dev)
         L.check(fn(table, offs, K, B, Cc, kind, Fn._ptr(labels), task, *fixed,
                    Fn._ptr(metrics if labels is not None else None), *logs, Fn._stream(dev)), "bbb_mc_route")
     return launch
@@ -2375,9 +2374,9 @@ def _temperature_tensor(t, device, normalized, what):
                          "(normalized=True) takes none")
     device = torch.device(device)
     if isinstance(t, torch.Tensor):
-        if not (t.dtype == torch.float32 and t.numel() == 1 and t.device == device and t.is_contiguous()):
-            raise L.EngineError(f"{what}: temperature must be a contiguous one-element float32 tensor on {device}, got "
-                                f"{t.dtype} {tuple(t.shape)} on {t.device}")
+        _check_tensor(t, f"{what}: temperature", dtype=torch.float32, device=device)
+        if t.numel() != 1:
+            raise L.EngineError(f"{what}: temperature must be a one-element float32 tensor, got shape {tuple(t.shape)}")
         return t
     v = float(t)
     if not (math.isfinite(v) and v > 0.0):
@@ -2442,10 +2441,8 @@ class LogitBank(_SampleBank):
         [B] (bbb_mc_logit_log on the current stream): logits from anywhere else."""
         self._check_logits(logits)
         B = logits.shape[1]
-        if labels is not None and not (labels.dtype == torch.int64 and tuple(labels.shape) == (B,)
-                                       and labels.is_contiguous() and labels.device == self.device):
-            raise L.EngineError(f"LogitBank.append: expected contiguous int64 labels [{B}] on {self.device}, got "
-                                f"{labels.dtype} {tuple(labels.shape)} on {labels.device}")
+        if labels is not None:
+            _check_tensor(labels, "LogitBank.append: labels", (B,), torch.int64, self.device)
         self._unlabelled |= labels is None
         self._launch(logits, labels, B)
 
