@@ -693,6 +693,50 @@ int bbb_temperature_nll(const float* logits, const int64_t* labels, const int64_
                         size_t workspace_bytes, void* cuda_stream);
 int bbb_mc_temper(float* logits, int64_t n, const float* temperature, void* cuda_stream);
 
+/* Vector and matrix scaling of the Monte-Carlo predictive (Guo et al. 2017), per sample before the softmax and the
+ * average over samples, as the temperature above: p_bar = mean_s softmax(f(z_s)) with
+ *   BBB_SCALING_VECTOR  f(z) = a . z + b, params = [a | b] (device fp32, 2C floats);
+ *   BBB_SCALING_MATRIX  f(z) = W z + b,   params = [W row by row | b] (C^2 + C floats), C <= BBB_SCALING_MATRIX_MAX_CLASSES.
+ * The identity (a = 1 or W = I, b = 0) gives the untransformed predictive.
+ *
+ * bbb_mc_logit_scale: logits[r] <- f(logits[r]) for r < rows, in place; params are read at run time, so a graph
+ * captured once reads values written in place later.  Vector: __fmul_rn then __fadd_rn (never an FMA: the bits of
+ * torch's fp32 z * a + b).  Matrix: the row is staged, then output j = (sum_k W[j][k] z[k] by fmaf in k = 0, 1, ..,
+ * C - 1 order from 0) + b[j].  Launched with programmatic stream serialization, as bbb_mc_temper.  rows > 0,
+ * 1 <= C <= BBB_LOGIT_BANK_MAX_CLASSES (matrix: BBB_SCALING_MATRIX_MAX_CLASSES) and non-NULL pointers, else
+ * BBB_E_INVALID.
+ *
+ * bbb_scaling_nll_grad: one full-batch pass over a logit bank (bbb_mc_logit_log's layout; the cursor, its poison and
+ * the label rules of bbb_temperature_nll) at the iterate theta = params (device fp32 [P], P = 2C or C^2 + C):
+ *   J = -(1/n) sum_i log( (1/S) sum_s softmax(f(z_is))[y_i] )
+ *       + l2_offdiag sum_{j != k} W_jk^2 / (C (C - 1)) (matrix; ODIR, Kull et al. 2019) + l2_bias sum_c b_c^2 / C
+ * and its gradient, and with BBB_SCALING_UPDATE one Adam step (beta 0.9 / 0.999, eps 1e-8, step lr, bias corrections
+ * bias1 = 1 - 0.9^t and bias2 = 1 - 0.999^t) of state = [x | m | v] (device double [3][P]: the double iterate and the
+ * moments), writing theta = (float) x.  Vector: the map in fp32 as the apply forms it, one warp per image, CTAs of
+ * BBB_SCALING_CTA_IMAGES consecutive images.  Matrix: the forward Z W^T and the gradient G^T Z on tf32 wgmma with fp32
+ * accumulation (operands rounded to tf32), the softmax, the logmeanexp over samples and dJ/dz' in the epilogue, CTAs
+ * of max(1, 2048 / S) consecutive images.  Per row the softmax in fp32 (ex2.approx.ftz, accurate log2f); the
+ * logmeanexp over samples and every sum after a CTA's in double, over the CTAs in index order: the same bits on every
+ * run and for any bank capacity.  A non-finite J (a poisoned or empty bank, a label outside [0, C)) takes no step.
+ *   fit [3]: fit[0] = J at the start (BBB_SCALING_FIRST), fit[1] = the least J so far, fit[2] = this pass's J;
+ *   best [P]: the iterate of fit[1] (FIRST: this pass's theta, else replaced only by a strictly smaller J);
+ *   result [1 + P] (nullable): J and dJ/dtheta of this pass;
+ *   BBB_SCALING_LAST: out = best when fit[0] and fit[1] are finite, else out is left as it was.
+ * workspace: bbb_scaling_workspace_bytes(n, S, C, kind) bytes, zeroed once by the caller (a launch leaves its arrival
+ * counter zeroed again); launches that share a workspace or a state must run one after another.  1 <= n,
+ * 1 <= S <= BBB_LOGIT_BANK_MAX_SAMPLES, 2 <= C <= BBB_LOGIT_BANK_MAX_CLASSES (matrix: BBB_SCALING_MATRIX_MAX_CLASSES),
+ * l2_bias >= 0, l2_offdiag >= 0 (0 for vector), an UPDATE with finite lr >= 0 and bias corrections in (0, 1], LAST
+ * with out non-NULL, else BBB_E_INVALID. */
+enum { BBB_SCALING_VECTOR = 1, BBB_SCALING_MATRIX = 2, BBB_SCALING_MATRIX_MAX_CLASSES = 128,
+       BBB_SCALING_CTA_IMAGES = 32, BBB_SCALING_FIRST = 1, BBB_SCALING_LAST = 2, BBB_SCALING_UPDATE = 4 };
+int bbb_mc_logit_scale(float* logits, int64_t rows, int32_t C, int32_t kind, const float* params, void* cuda_stream);
+size_t bbb_scaling_workspace_bytes(int32_t n, int32_t S, int32_t C, int32_t kind);
+int bbb_scaling_nll_grad(const float* logits, const int64_t* labels, const int64_t* cursor, int32_t n, int32_t S,
+                         int32_t C, int32_t kind, int32_t flags, float* theta, double* state, float* best,
+                         double* fit /* [3] */, double* result, float* out, double l2_offdiag, double l2_bias,
+                         double lr, double bias1, double bias2, void* workspace, size_t workspace_bytes,
+                         void* cuda_stream);
+
 /* BatchBALD's joint-entropy scores of every candidate of a probability bank (bbb_mc_prob_log's layout, S_pad / C_pad
  * from S / C as there) against M configurations of the labels already chosen:
  *   out[i] = sum_{m < M} omega[m] * ( -sum_{c < C} Q[m,c] log Q[m,c] ),   Q[m,c] = sum_s pt[m][s] * bank[i][c][s]

@@ -38,7 +38,7 @@ SYMBOLS = (
     "bbb_mc_graph_step", "bbb_conv2d_backward_prior", "bbb_linear_backward_prior", "bbb_mc_score_log",
     "bbb_mc_prob_log", "bbb_joint_entropy_workspace_bytes", "bbb_joint_entropy", "bbb_mc_conformal_log",
     "bbb_mc_route_bytes", "bbb_mc_route", "bbb_mc_logit_log", "bbb_temperature_workspace_bytes", "bbb_temperature_nll",
-    "bbb_mc_temper",
+    "bbb_mc_temper", "bbb_mc_logit_scale", "bbb_scaling_workspace_bytes", "bbb_scaling_nll_grad",
 )
 MC_MOMENTS, MC_NORMALIZED, MC_INFO = 1, 2, 4
 MC_CAL_BINS = 15                 # BBB_MC_CAL_BINS: calibration bins of the evaluation accumulator
@@ -54,6 +54,9 @@ ROUTE_MAX_EXPERTS = 16
 LOGIT_BANK_MAX_SAMPLES, LOGIT_BANK_MAX_CLASSES = 256, 1024
 TEMPERATURE_MAX_POINTS, TEMPERATURE_CTA_IMAGES = 64, 32
 TEMPERATURE_FIRST, TEMPERATURE_LAST = 1, 2
+# BBB_SCALING_*: the map of bbb_mc_logit_scale / bbb_scaling_nll_grad, the images per CTA of the fit pass and its flags
+SCALING_VECTOR, SCALING_MATRIX, SCALING_MATRIX_MAX_CLASSES, SCALING_CTA_IMAGES = 1, 2, 128, 32
+SCALING_FIRST, SCALING_LAST, SCALING_UPDATE = 1, 2, 4
 
 
 class LayerDesc(C.Structure):
@@ -180,6 +183,13 @@ def _bind(lib):
     lib.bbb_temperature_nll.restype = C.c_int
     lib.bbb_mc_temper.argtypes = [fp, C.c_int64, fp, vp]
     lib.bbb_mc_temper.restype = C.c_int
+    lib.bbb_mc_logit_scale.argtypes = [fp, C.c_int64, i32, i32, fp, vp]
+    lib.bbb_mc_logit_scale.restype = C.c_int
+    lib.bbb_scaling_workspace_bytes.argtypes = [i32, i32, i32, i32]
+    lib.bbb_scaling_workspace_bytes.restype = sz
+    lib.bbb_scaling_nll_grad.argtypes = [fp, vp, vp, i32, i32, i32, i32, i32, fp, vp, fp, vp, vp, fp, C.c_double,
+                                         C.c_double, C.c_double, C.c_double, C.c_double, vp, sz, vp]
+    lib.bbb_scaling_nll_grad.restype = C.c_int
     lib.bbb_joint_entropy_workspace_bytes.argtypes = [i32, i32, i32, i32]
     lib.bbb_joint_entropy_workspace_bytes.restype = sz
     lib.bbb_joint_entropy.argtypes = [fp, vp, vp, fp, i32, i32, i32, i32, vp, vp, sz, vp]

@@ -19,6 +19,7 @@
 #include "conformal.cuh"
 #include "route.cuh"
 #include "temperature.cuh"
+#include "logit_scaling.cuh"
 
 namespace {
 
@@ -952,6 +953,85 @@ int bbb_mc_temper(float* logits, int64_t n, const float* temperature, void* cuda
     cudaError_t e = bbb::launch_pdl(bbb::mc_temper_kernel, dim3((unsigned)grid), dim3(bbb::TP_THREADS), 0,
                                     (cudaStream_t)cuda_stream, logits, (long long)n, temperature);
     return launched(e, "mc_temper launch");
+}
+
+int bbb_mc_logit_scale(float* logits, int64_t rows, int32_t C, int32_t kind, const float* params, void* cuda_stream) {
+    if (!logits || !params) return fail(BBB_E_INVALID, "NULL pointer");
+    if (kind != BBB_SCALING_VECTOR && kind != BBB_SCALING_MATRIX) return fail(BBB_E_INVALID, "bad kind %d", kind);
+    const int max_c = kind == BBB_SCALING_MATRIX ? (int)BBB_SCALING_MATRIX_MAX_CLASSES : (int)BBB_LOGIT_BANK_MAX_CLASSES;
+    if (rows <= 0 || C < 1 || C > max_c) return fail(BBB_E_INVALID, "bad rows/C %lld/%d", (long long)rows, C);
+    const long long n = (long long)rows * C;
+    cudaError_t e;
+    if (kind == BBB_SCALING_VECTOR) {
+        const unsigned grid = grid_blocks((uint64_t)n, bbb::LS_THREADS, bbb::LS_MAX_CTAS);
+        e = bbb::launch_pdl(bbb::mc_logit_scale_kernel, dim3(grid), dim3(bbb::LS_THREADS), 0,
+                            (cudaStream_t)cuda_stream, logits, n, (int)C, params);
+    } else {
+        const size_t smem = ((size_t)C * C + (size_t)bbb::MA_ROWS * C) * sizeof(float);
+        e = cudaFuncSetAttribute(bbb::mc_logit_scale_matrix_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                 (int)smem);
+        if (e != cudaSuccess) return cuda_fail(e, "mc_logit_scale_matrix smem attribute");
+        const unsigned grid = grid_blocks((uint64_t)rows, bbb::MA_ROWS, 4ull * (uint64_t)sm_count());
+        e = bbb::launch_pdl(bbb::mc_logit_scale_matrix_kernel, dim3(grid), dim3(bbb::MA_THREADS), smem,
+                            (cudaStream_t)cuda_stream, logits, (long long)rows, (int)C, params);
+    }
+    return launched(e, "mc_logit_scale launch");
+}
+
+// CTAs of a fit pass over n images, and the parameters of one kind
+static size_t scaling_grid(int32_t n, int32_t S, int32_t kind) {
+    const size_t per = kind == BBB_SCALING_MATRIX ? (size_t)bbb::mx_images(S) : (size_t)bbb::SC_CTA_IMAGES;
+    return ((size_t)n + per - 1) / per;
+}
+static size_t scaling_params(int32_t C, int32_t kind) {
+    return kind == BBB_SCALING_MATRIX ? (size_t)C * C + C : 2 * (size_t)C;
+}
+
+size_t bbb_scaling_workspace_bytes(int32_t n, int32_t S, int32_t C, int32_t kind) {
+    if (n < 1 || S < 1 || S > BBB_LOGIT_BANK_MAX_SAMPLES || C < 2 || C > BBB_LOGIT_BANK_MAX_CLASSES) return 0;
+    if (kind != BBB_SCALING_VECTOR && (kind != BBB_SCALING_MATRIX || C > BBB_SCALING_MATRIX_MAX_CLASSES)) return 0;
+    return 16 + scaling_grid(n, S, kind) * (scaling_params(C, kind) + 1) * sizeof(double);
+}
+
+int bbb_scaling_nll_grad(const float* logits, const int64_t* labels, const int64_t* cursor, int32_t n, int32_t S,
+                         int32_t C, int32_t kind, int32_t flags, float* theta, double* state, float* best, double* fit,
+                         double* result, float* out, double l2_offdiag, double l2_bias, double lr, double bias1,
+                         double bias2, void* workspace, size_t workspace_bytes, void* cuda_stream) {
+    if (!logits || !labels || !theta || !state || !best || !fit || !workspace)
+        return fail(BBB_E_INVALID, "NULL pointer");
+    if (kind != BBB_SCALING_VECTOR && kind != BBB_SCALING_MATRIX) return fail(BBB_E_INVALID, "bad kind %d", kind);
+    const int max_c = kind == BBB_SCALING_MATRIX ? (int)BBB_SCALING_MATRIX_MAX_CLASSES : (int)BBB_LOGIT_BANK_MAX_CLASSES;
+    if (n < 1 || S < 1 || S > BBB_LOGIT_BANK_MAX_SAMPLES || C < 2 || C > max_c)
+        return fail(BBB_E_INVALID, "bad n/S/C %d/%d/%d", n, S, C);
+    if (flags & ~(BBB_SCALING_FIRST | BBB_SCALING_LAST | BBB_SCALING_UPDATE))
+        return fail(BBB_E_INVALID, "bad flags %d", flags);
+    if ((flags & BBB_SCALING_LAST) && !out) return fail(BBB_E_INVALID, "the last pass needs out");
+    if (!(l2_bias >= 0.0) || !std::isfinite(l2_bias)) return fail(BBB_E_INVALID, "bad l2_bias %g", l2_bias);
+    if (!(l2_offdiag >= 0.0) || !std::isfinite(l2_offdiag) || (kind == BBB_SCALING_VECTOR && l2_offdiag != 0.0))
+        return fail(BBB_E_INVALID, "bad l2_offdiag %g", l2_offdiag);
+    if ((flags & BBB_SCALING_UPDATE) &&
+        !(lr >= 0.0 && std::isfinite(lr) && bias1 > 0.0 && bias1 <= 1.0 && bias2 > 0.0 && bias2 <= 1.0))
+        return fail(BBB_E_INVALID, "bad Adam step lr %g, bias corrections %g/%g", lr, bias1, bias2);
+    const size_t need = bbb_scaling_workspace_bytes(n, S, C, kind);
+    if (workspace_bytes < need) return fail(BBB_E_INVALID, "workspace of %zu bytes < %zu", workspace_bytes, need);
+    bbb::ScalingNllArgs a;
+    a.logits = logits; a.labels = (const long long*)labels; a.cursor = (const long long*)cursor;
+    a.n = n; a.S = S; a.C = C;
+    a.first = (flags & BBB_SCALING_FIRST) != 0; a.last = (flags & BBB_SCALING_LAST) != 0;
+    a.update = (flags & BBB_SCALING_UPDATE) != 0; a.matrix = kind == BBB_SCALING_MATRIX;
+    a.theta = theta; a.state = state; a.best = best; a.fit = fit; a.result = result; a.out = out;
+    a.l2_offdiag = l2_offdiag; a.l2_bias = l2_bias; a.lr = lr; a.bias1 = bias1; a.bias2 = bias2;
+    a.arrive = (unsigned int*)workspace; a.partials = (double*)((char*)workspace + 16);
+    const unsigned grid = (unsigned)scaling_grid(n, S, kind);
+    auto kern = a.matrix ? bbb::scaling_nll_grad_matrix_kernel : bbb::scaling_nll_grad_kernel;
+    const size_t smem = a.matrix ? bbb::mx_smem_bytes(C) : bbb::sc_smem_bytes(C);
+    const unsigned threads = a.matrix ? bbb::MX_THREADS : bbb::SC_THREADS;
+    if (smem > 48 * 1024) {
+        cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        if (e != cudaSuccess) return cuda_fail(e, "scaling_nll_grad smem attribute");
+    }
+    kern<<<grid, threads, smem, (cudaStream_t)cuda_stream>>>(a);
+    return launched(cudaSuccess, "scaling_nll_grad launch");
 }
 
 size_t bbb_joint_entropy_workspace_bytes(int32_t N, int32_t S, int32_t C, int32_t M) {

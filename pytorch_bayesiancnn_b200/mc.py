@@ -181,7 +181,7 @@ class MCForward:
                  batch_shards: int = 1, metrics: Optional[torch.Tensor] = None, cache_prep: bool = True,
                  score_log: Optional["ScoreLog"] = None, prob_bank: Optional["ProbBank"] = None,
                  conformal: Optional["ConformalLog"] = None, logit_bank: Optional["LogitBank"] = None,
-                 temperature=None):
+                 temperature=None, scaling: Optional["LogitScaling"] = None):
         """``static_inputs``: device tensors the caller fills in place (e.g. targets of its host->device copies, or a
         rotation of resident batches); one graph is captured per tensor and ``self(slot=k)`` runs the step on
         ``static_inputs[k]`` with no staging copy.  ``first_replay``: index of the first replay's noise block.
@@ -219,7 +219,11 @@ class MCForward:
         step): every output -- log_outputs, pred, the uncertainty and information planes, head, metrics and the logs behind
         the exchange -- is then that of p_bar_T = mean_s softmax(z_s / T).  A float, or a one-element fp32 tensor on the
         step's device that the step reads at run time: a value written into it in place is read by the next step, captured
-        or not (fit_temperature(out=...)).  Not with ``normalized``."""
+        or not (fit_temperature(out=...)).  Not with ``normalized``.
+        ``scaling``: a LogitScaling that maps every sample's logits, z <- a * z + b, before the exchange, in the
+        temperature's place (bbb_mc_logit_scale, one more kernel per step): every output is then that of
+        p_bar = mean_s softmax(a * z_s + b).  Its parameters are read at run time (fit_scaling(out=...) writes them in
+        place).  Not with ``temperature`` or ``normalized``."""
         if want_information and not want_uncertainty:
             raise L.EngineError("MCForward: want_information needs want_uncertainty")
         Fn._require_cuda(example_x, "MCForward")
@@ -243,7 +247,8 @@ class MCForward:
             lg._bind(self)
         # a step without labels logs label -1 into a logit bank, which the host must know of (LogitBank._unlabelled)
         self._unlabelled_bank = logit_bank if not with_labels else None
-        self.temperature = _temperature_tensor(temperature, example_x.device, normalized, "MCForward")
+        self.temperature, self.scaling = _logit_map(temperature, scaling, example_x.device, normalized, self.C,
+                                                    "MCForward")
         if self.world > 16:
             raise L.EngineError("MCForward: at most 16 ranks (one node)")
         self.sample_shards, self.group_index, self.block = shard_layout(self.world, self.rank, batch_shards)
@@ -566,7 +571,9 @@ class MCForward:
         for lg in self._logs:
             if lg.before_temper:
                 lg._log(self, par)
-        if self.temperature is not None and self.ids:
+        if self.ids and self.scaling is not None:
+            self.scaling._launch(self.logits_all[par], Fn._stream(self.dev))
+        elif self.ids and self.temperature is not None:
             z = self.logits_all[par]
             L.check(lib.bbb_mc_temper(Fn._ptr(z), z.numel(), Fn._ptr(self.temperature), Fn._stream(self.dev)),
                     "bbb_mc_temper")
@@ -1077,7 +1084,7 @@ def evaluate(net, loader, num_ens: int, train_size: float, beta_type=0.1, epoch=
              seed: Optional[int] = None, inflight: int = 4, batch_shards: int = 1, normalized: bool = False,
              score_log: Optional[ScoreLog] = None, prob_bank: Optional["ProbBank"] = None,
              conformal: Optional["ConformalLog"] = None, logit_bank: Optional["LogitBank"] = None,
-             temperature=None) -> dict:
+             temperature=None, scaling: Optional["LogitScaling"] = None) -> dict:
     """main_bayesian.validate_model over ``loader`` (batches of (inputs, labels)) on the engine, with calibration.
 
     Returns read_metrics' dict plus ``valid_loss`` and ``valid_acc`` as validate_model computes them: the mean over
@@ -1103,19 +1110,18 @@ def evaluate(net, loader, num_ens: int, train_size: float, beta_type=0.1, epoch=
     ``logit_bank``: a LogitBank every image's raw per-sample logits and label are appended to, in loader order (one rank
     only; calibrate_temperature fills one); the returned figures keep their bits.
     ``temperature``: MCForward's -- every figure, log and bank behind the exchange is that of the tempered predictive.
-    Engines are kept per temperature tensor (a float: per value), and read a value written into the tensor in place."""
+    Engines are kept per temperature tensor (a float: per value), and read a value written into the tensor in place.
+    ``scaling``: MCForward's, kept and read in place as a temperature tensor is."""
     dev = next(net.parameters()).device
     logs = dict(score_log=score_log, prob_bank=prob_bank, conformal=conformal, logit_bank=logit_bank)
-    tkey = None if temperature is None else \
-        ("tensor", id(temperature)) if isinstance(temperature, torch.Tensor) else float(temperature)
     key = (int(num_ens), float(train_size), seed, id(group), int(inflight), int(batch_shards), bool(normalized),
-           *(None if lg is None else id(lg) for lg in logs.values()), tkey)
+           *(None if lg is None else id(lg) for lg in logs.values()), _map_key(temperature), _map_key(scaling))
     ev = _engine_cache(net, "_mc_eval").get(key)
     if ev is None:
-        # (the entry holds the logs and the temperature its key names by id, so that no other object takes their id)
+        # (the entry holds the logs and the maps its key names by id, so that no other object takes their id)
         ev = net.__dict__["_mc_eval"][key] = {"acc": new_metrics(dev), "engines": {}, "seed": seed,
                                               "logs": [lg for lg in logs.values() if lg is not None],
-                                              "temperature": temperature}
+                                              "maps": (temperature, scaling)}
     ev["acc"].zero_()
 
     def build(slots, first_replay):
@@ -1123,7 +1129,7 @@ def evaluate(net, loader, num_ens: int, train_size: float, beta_type=0.1, epoch=
                          static_inputs=slots, first_replay=first_replay, overlap=True, inflight=inflight,
                          batch_shards=batch_shards, metrics=ev["acc"], normalized=normalized,
                          want_uncertainty=score_log is not None, want_information=score_log is not None,
-                         temperature=temperature, **logs)
+                         temperature=temperature, scaling=scaling, **logs)
     n = _run_loader(ev, loader, dev, max(2, int(inflight)), build)
     if not n:
         raise ValueError("evaluate: the loader yielded no batch")
@@ -1308,9 +1314,11 @@ class MCTrainStep(MCForward):
 
     def __init__(self, net, example_x, num_ens, train_size, group=None, seed=None, batch_shards: int = 1,
                  fold: bool = False, fold_group: Optional[int] = None, score_log=None, prob_bank=None, conformal=None,
-                 logit_bank=None, temperature=None):
+                 logit_bank=None, temperature=None, scaling=None):
         for given, why in ((temperature, "temper: a temperature is fitted after training (fit_temperature) and "
                                          "applied by MCForward or evaluate()"),
+                           (scaling, "scale logits: a scaling is fitted after training (fit_scaling) and applied by "
+                                     "MCForward or evaluate()"),
                            (logit_bank, "fill a logit_bank: fill it from MCForward or evaluate()"),
                            (conformal, "log conformal scores: log them from MCForward or evaluate()"),
                            (score_log, "log scores: log them from MCForward or evaluate()"),
@@ -2209,17 +2217,19 @@ class ExpertStep:
     ``experts``: the K experts' own ``out`` dicts.  ``labels`` (int64 [B]; global classes, or with ``task=t`` the local
     classes of expert t) add the step to ``metrics`` (new_route_metrics); ``log``: a RouteLog every step appends to.
     ``temperatures``: one per expert (MCForward's ``temperature``; None: that expert is not tempered), so experts
-    calibrated one by one route on comparable uncertainty scores.
+    calibrated one by one route on comparable uncertainty scores.  ``scalings``: one LogitScaling (or None) per expert,
+    as ``temperatures``; an expert takes a temperature or a scaling, not both.
     ``offsets``: each expert's first global class (default e * C).  Inference only, one rank only.  As with MCForward,
     two engines over the same layers share the layers' workspaces: ``wait()`` for one before stepping the other."""
 
     def __init__(self, experts, example_x: torch.Tensor, num_ens: int, score: str = "epistemic",
                  normalized: bool = False, offsets=None, group=None, seed: Optional[int] = None, static_inputs=None,
                  first_replay: int = 0, inflight: int = 1, metrics: Optional[torch.Tensor] = None,
-                 log: Optional[RouteLog] = None, temperatures=None):
+                 log: Optional[RouteLog] = None, temperatures=None, scalings=None):
         experts = list(experts)
         self.K, self.C, self.offsets = _check_experts(experts, example_x.device, score, offsets, group)
-        temps = _expert_temperatures(temperatures, self.K)
+        temps = _expert_temperatures(temperatures, self.K, "temperatures")
+        scals = _expert_temperatures(scalings, self.K, "scalings")
         Fn._require_cuda(example_x, "ExpertStep")
         if log is not None and (log.device != example_x.device or log.num_experts != self.K):
             raise L.EngineError(f"ExpertStep: the log holds {log.num_experts} experts on {log.device}, the step "
@@ -2231,8 +2241,9 @@ class ExpertStep:
         self.inputs = list(static_inputs) if static_inputs else [example_x.clone()]
         self.engines = [MCForward(net, self.inputs[0], num_ens, want_uncertainty=True, normalized=normalized,
                                   seed=self.seed, static_inputs=self.inputs, first_replay=first_replay, overlap=True,
-                                  inflight=inflight, want_information=score == "mutual_info", temperature=t)
-                        for net, t in zip(experts, temps)]
+                                  inflight=inflight, want_information=score == "mutual_info", temperature=t,
+                                  scaling=sc)
+                        for net, t, sc in zip(experts, temps, scals)]
         self.nbuf = self.engines[0].nbuf
         res = _route_result(self.B, self.K, self.dev)
         self._launch = _route_launcher([e.out for e in self.engines], score, self.offsets, metrics, log, res)
@@ -2304,7 +2315,7 @@ class ExpertStep:
 
 def route(experts, loader, num_ens: int, score: str = "epistemic", normalized: bool = False,
           task: Optional[int] = None, log: bool = True, inflight: int = 4, seed: Optional[int] = None,
-          offsets=None, temperatures=None) -> dict:
+          offsets=None, temperatures=None, scalings=None) -> dict:
     """predict_using_uncertainty_separate_models (Mixtures/utils_mixture.py:119-162) over ``loader`` (batches of
     (inputs, labels)) for K task experts, on the device: every batch through an ExpertStep, one per batch shape, all
     adding to one routing accumulator that the host reads once, at the end.  Inputs and labels go into rotating device
@@ -2315,8 +2326,8 @@ def route(experts, loader, num_ens: int, score: str = "epistemic", normalized: b
     local classes of expert t (the reference's Split-MNIST loaders of task t).  Returns ``accuracy`` (global),
     ``local_accuracy`` (the reference's figure), ``routing_accuracy``, ``selected`` (the fraction sent to each expert),
     ``total_score`` (per expert), ``steps`` / ``images``, and with ``log`` ``per_image``: ``expert``, ``pred`` and
-    ``scores`` on the device, in loader order.  ``temperatures``: ExpertStep's, one per expert.  Raises ValueError at
-    the end if a label was outside every range."""
+    ``scores`` on the device, in loader order.  ``temperatures`` / ``scalings``: ExpertStep's, one per expert.  Raises
+    ValueError at the end if a label was outside every range."""
     experts = list(experts)
     dev = next(experts[0].parameters()).device
     K = _check_experts(experts, dev, score, offsets, None)[0]
@@ -2324,10 +2335,11 @@ def route(experts, loader, num_ens: int, score: str = "epistemic", normalized: b
     if dev.type != "cuda":
         raise L.EngineError(f"route: the experts are on {dev}; the engine runs on CUDA (sm_90a) only")
     n_img = _loader_images(loader) if log else 0
-    temps = _expert_temperatures(temperatures, K)
+    temps = _expert_temperatures(temperatures, K, "temperatures")
+    scals = _expert_temperatures(scalings, K, "scalings")
     key = (tuple(id(e) for e in experts), int(num_ens), score, bool(normalized), int(inflight), seed,
            None if offsets is None else tuple(int(o) for o in offsets),
-           tuple(None if t is None else ("tensor", id(t)) if isinstance(t, torch.Tensor) else float(t) for t in temps))
+           tuple(_map_key(t) for t in temps), tuple(_map_key(sc) for sc in scals))
     cache = _engine_cache(experts[0], "_mc_route")
     ent = cache.get(key)
     if ent is not None and not all(eng._prior_guard.ok() for e in ent["engines"].values()
@@ -2335,7 +2347,7 @@ def route(experts, loader, num_ens: int, score: str = "epistemic", normalized: b
         ent = None                          # an expert's prior or mask changed since its graphs were captured
     if ent is None:
         ent = cache[key] = {"acc": new_route_metrics(dev), "engines": {}, "seed": seed, "log": None,
-                            "temperatures": temps}
+                            "maps": (temps, scals)}
     if log and (ent["log"] is None or ent["log"].capacity < n_img):
         ent["log"] = RouteLog(dev, n_img, K)
         ent["engines"].clear()              # the steps append to the log they were built with
@@ -2347,7 +2359,7 @@ def route(experts, loader, num_ens: int, score: str = "epistemic", normalized: b
     def build(slots, first_replay):
         return ExpertStep(experts, slots[0], num_ens, score=score, normalized=normalized, offsets=offsets,
                           seed=ent["seed"], static_inputs=slots, first_replay=first_replay, inflight=inflight,
-                          metrics=ent["acc"], log=rlog, temperatures=temps)
+                          metrics=ent["acc"], log=rlog, temperatures=temps, scalings=scals)
     if not _run_loader(ent, loader, dev, max(2, int(inflight)), build, task=task):
         raise ValueError("route: the loader yielded no batch")
     m = read_route_metrics(ent["acc"], K)
@@ -2365,6 +2377,35 @@ def route(experts, loader, num_ens: int, score: str = "epistemic", normalized: b
 # the average over samples (Laves et al. 2019): p_bar_T = mean_s softmax(z_s / T).  A calibration bank of raw
 # per-sample logits, a grid search for T on the device, and the temper in front of the exchange.
 # --------------------------------------------------------------------------------------------------------------------
+def _logit_map(temperature, scaling, device, normalized, num_classes, what):
+    """MCForward's ``temperature`` and ``scaling``, the two maps of the one slot in front of the exchange: (the
+    one-element fp32 device tensor the temper reads or None, the LogitScaling or None), at most one of them given."""
+    if scaling is None:
+        return _temperature_tensor(temperature, device, normalized, what), None
+    if normalized:
+        raise ValueError(f"{what}: a scaling maps the logits of the softmax predictive; the softplus-normalised one "
+                         "(normalized=True) takes none")
+    if temperature is not None:
+        raise ValueError(f"{what}: a temperature or a scaling, not both (fit_scaling(init_temperature=T) starts a "
+                         "scaling from T)")
+    if not isinstance(scaling, LogitScaling):
+        raise TypeError(f"{what}: scaling must be a LogitScaling, got {type(scaling).__name__}")
+    if scaling.device != torch.device(device) or scaling.num_classes != int(num_classes):
+        raise L.EngineError(f"{what}: the scaling holds {scaling.num_classes} classes on {scaling.device}, the step "
+                            f"{num_classes} on {device}")
+    return None, scaling
+
+
+def _map_key(v):
+    """The engine-cache key of a temperature or a scaling: by object for a tensor or a LogitScaling (the engines read
+    it at run time), by value for a float."""
+    if v is None:
+        return None
+    if isinstance(v, (torch.Tensor, LogitScaling)):
+        return (type(v).__name__, id(v))
+    return float(v)
+
+
 def _temperature_tensor(t, device, normalized, what):
     """MCForward's ``temperature`` as the one-element fp32 device tensor the temper reads (a tensor is used as given)."""
     if t is None:
@@ -2384,13 +2425,13 @@ def _temperature_tensor(t, device, normalized, what):
     return torch.full((1,), v, dtype=torch.float32, device=device)
 
 
-def _expert_temperatures(temperatures, K):
-    if temperatures is None:
+def _expert_temperatures(values, K, what="temperatures"):
+    if values is None:
         return [None] * K
-    temperatures = list(temperatures)
-    if len(temperatures) != K:
-        raise ValueError(f"ExpertStep: {len(temperatures)} temperatures for {K} experts (one per expert, None: none)")
-    return temperatures
+    values = list(values)
+    if len(values) != K:
+        raise ValueError(f"ExpertStep: {len(values)} {what} for {K} experts (one per expert, None: none)")
+    return values
 
 
 class LogitBank(_SampleBank):
@@ -2510,18 +2551,22 @@ class TemperatureFit:
         return out
 
     def _why(self):
-        """Why the device found no fit (host reads of the bank)."""
-        n, dropped = self._bank._counts()
-        if dropped:
-            return f"the bank dropped {dropped} images (capacity {self._bank.capacity})"
-        if n == 0:
-            return "the bank is empty"
-        y = self._bank._labels[:n]
-        if bool((y < 0).any()):
-            return f"{int((y < 0).sum())} images were logged without a label (a step with_labels=False)"
-        if bool((y >= self._bank.num_classes).any()):
-            return f"a label is outside [0, {self._bank.num_classes})"
-        return "the bank's logits give no finite NLL (NaN or infinite logits?)"
+        return _no_fit_reason(self._bank)
+
+
+def _no_fit_reason(bank):
+    """Why the device found no fit on a LogitBank (host reads of the bank)."""
+    n, dropped = bank._counts()
+    if dropped:
+        return f"the bank dropped {dropped} images (capacity {bank.capacity})"
+    if n == 0:
+        return "the bank is empty"
+    y = bank._labels[:n]
+    if bool((y < 0).any()):
+        return f"{int((y < 0).sum())} images were logged without a label (a step with_labels=False)"
+    if bool((y >= bank.num_classes).any()):
+        return f"a label is outside [0, {bank.num_classes})"
+    return "the bank's logits give no finite NLL (NaN or infinite logits?)"
 
 
 def fit_temperature(bank: LogitBank, t_min: float = 0.05, t_max: float = 20.0, grid: int = 32, rounds: int = 4,
@@ -2592,3 +2637,210 @@ def calibrate_temperature(net, cal_loader, num_ens: int, t_min: float = 0.05, t_
     m = evaluate(net, cal_loader, num_ens, train_size, logit_bank=bank, **kw)
     fit = fit_temperature(bank, t_min, t_max, grid, rounds, out=out, trace=trace)
     return {"temperature": fit.temperature, "fit": fit.read(), "evaluate": m}
+
+
+# --------------------------------------------------------------------------------------------------------------------
+# Vector and matrix scaling (Guo et al. 2017) of the Monte-Carlo predictive, in the temperature's place:
+# p_bar = mean_s softmax(f(z_s)), f(z) = a * z + b or W z + b, fitted by full-batch Adam on a LogitBank on the device.
+# --------------------------------------------------------------------------------------------------------------------
+SCALING_KINDS = {"vector": L.SCALING_VECTOR, "matrix": L.SCALING_MATRIX}
+
+
+def _check_kind(kind, what, num_classes=None):
+    if kind not in SCALING_KINDS:
+        raise ValueError(f"{what}: kind must be 'vector' or 'matrix' (got {kind!r})")
+    if kind == "matrix" and num_classes is not None and int(num_classes) > L.SCALING_MATRIX_MAX_CLASSES:
+        raise ValueError(f"{what}: matrix scaling takes at most {L.SCALING_MATRIX_MAX_CLASSES} classes "
+                         f"(got {num_classes})")
+    return SCALING_KINDS[kind]
+
+
+class LogitScaling:
+    """The parameters of vector or matrix scaling on the device.  ``params`` is fp32: vector [2, C], ``a = params[0]``
+    (the per-class scales) and ``b = params[1]``; matrix [C + 1, C], ``W = params[:C]`` (row j maps to class j, C <= 128)
+    and ``b = params[C]``.  It starts at the identity (a = 1 or W = I, b = 0), which gives the untransformed predictive
+    bit for bit.  Engines given it (MCForward / evaluate ``scaling=``, ExpertStep / route ``scalings=``) read the
+    parameters at run time, so a fit written in place (fit_scaling(out=...)) or parameters set in place under no_grad
+    are read by their next step."""
+
+    def __init__(self, device, num_classes: int, kind: str = "vector"):
+        self._kind = _check_kind(kind, "LogitScaling", num_classes)
+        num_classes = int(num_classes)
+        if not 2 <= num_classes <= L.LOGIT_BANK_MAX_CLASSES:
+            raise ValueError(f"LogitScaling: num_classes must be in [2, {L.LOGIT_BANK_MAX_CLASSES}] (got {num_classes})")
+        self.kind, self.num_classes = kind, num_classes
+        rows = num_classes + 1 if kind == "matrix" else 2
+        self.params = torch.zeros(rows, num_classes, dtype=torch.float32, device=device)
+        self.device = self.params.device
+        self.reset()
+
+    @property
+    def a(self):
+        if self.kind != "vector":
+            raise AttributeError("LogitScaling.a: a matrix scaling has W")
+        return self.params[0]
+
+    @property
+    def W(self):
+        if self.kind != "matrix":
+            raise AttributeError("LogitScaling.W: a vector scaling has a")
+        return self.params[:self.num_classes]
+
+    @property
+    def b(self):
+        return self.params[-1]
+
+    def reset(self):
+        """Back to the identity, in place."""
+        self.params.zero_()
+        if self.kind == "matrix":
+            self.W.fill_diagonal_(1.0)
+        else:
+            self.a.fill_(1.0)
+        return self
+
+    def _launch(self, z, stream):
+        L.check(L.lib().bbb_mc_logit_scale(Fn._ptr(z), z.numel() // self.num_classes, self.num_classes, self._kind,
+                                           Fn._ptr(self.params), stream), "bbb_mc_logit_scale")
+
+    def apply_(self, z):
+        """z <- f(z) in place on fp32 logits [..., C] (contiguous, on the device; bbb_mc_logit_scale on the current
+        stream): vector, the bits of torch's ``z * a + b``; matrix, each output an fmaf chain over the classes in order,
+        then + b."""
+        _check_tensor(z, "LogitScaling.apply_: logits", dtype=torch.float32, device=self.device)
+        if z.dim() < 1 or z.shape[-1] != self.num_classes or z.numel() == 0:
+            raise L.EngineError(f"LogitScaling.apply_: expected non-empty logits [..., {self.num_classes}], got "
+                                f"{tuple(z.shape)}")
+        self._launch(z, Fn._stream(self.device))
+        return z
+
+
+class ScalingFit:
+    """What fit_scaling enqueued: ``scaling`` (the LogitScaling holding the fitted parameters), and on ``read()`` --
+    the one host synchronisation -- the floats."""
+
+    def __init__(self, bank, scaling, fit, iters):
+        self.scaling, self._bank, self._fit, self._iters = scaling, bank, fit, iters
+
+    def read(self) -> dict:
+        """{"nll" (the bank's objective at the fitted parameters: its NLL, plus the penalties when l2_offdiag or l2_bias
+        > 0), "nll_start" (at the starting point), "nll_last" (at the last iterate), "iters", and "a" or "W" (lists; W
+        row by row) and "b"}.  The result is the best iterate, never worse than the start.  Raises ValueError when
+        there is no fit -- an empty bank, one that dropped images, one that holds an image without a valid label, or
+        a non-finite objective -- and ``scaling`` then keeps the parameters it had before the fit."""
+        v = torch.cat([self._fit, self.scaling.params.flatten().to(torch.float64)]).tolist()
+        if not (math.isfinite(v[0]) and math.isfinite(v[1])):
+            raise ValueError(f"fit_scaling: no fit -- {_no_fit_reason(self._bank)}")
+        C = self.scaling.num_classes
+        p = v[3:]
+        out = {"nll": v[1], "nll_start": v[0], "nll_last": v[2], "iters": self._iters, "b": p[-C:]}
+        if self.scaling.kind == "matrix":
+            out["W"] = [p[j * C:(j + 1) * C] for j in range(C)]
+        else:
+            out["a"] = p[:C]
+        return out
+
+
+def scaling_schedule(lr: float, iters: int) -> list:
+    """The step sizes of fit_scaling's Adam passes (pure host): a cosine decay from ``lr`` to 0 over ``iters`` steps,
+    lr_t = lr (1 + cos(pi t / iters)) / 2 for t = 0 .. iters - 1."""
+    return [float(lr) * 0.5 * (1.0 + math.cos(math.pi * t / iters)) for t in range(int(iters))]
+
+
+def fit_scaling(bank: LogitBank, kind: str = "vector", *, iters: int = 300, lr: float = 0.1, l2_offdiag: float = 0.0,
+                l2_bias: float = 0.0, init_temperature=None, out: Optional[LogitScaling] = None) -> ScalingFit:
+    """The map f -- vector a * z + b, or matrix W z + b (C <= 128) -- that minimises the bank's objective
+        J = -(1/n) sum_i log( (1/S) sum_s softmax(f(z_is))[y_i] )
+            + l2_offdiag * sum_{j != k} W_jk^2 / (C (C - 1)) + l2_bias * sum_c b_c^2 / C
+    (the matrix penalties are ODIR, Kull et al. 2019; l2_offdiag is for matrix scaling only), by ``iters`` full-batch
+    Adam steps (scaling_schedule's step sizes; beta 0.9 / 0.999) from the identity -- or from a = 1 / T or W = I / T,
+    b = 0 with ``init_temperature`` T (a float or a one-element fp32 device tensor, e.g. a TemperatureFit's, read on
+    the device) -- enqueued on the current stream with no host read: ``iters + 1`` passes of bbb_scaling_nll_grad over
+    the bank, each the objective, its gradient and the step (matrix: both contractions on tf32 wgmma); the last pass
+    evaluates the last iterate.  The best iterate is kept on the device, so the result is never worse on the bank than
+    the start.
+
+    Returns a ScalingFit: ``.scaling`` holds the result -- ``out`` when given, written in place, so engines that scale
+    with it read the new parameters at their next step; a new LogitScaling otherwise -- and ``.read()`` gives the
+    floats.  A fit the device cannot make (an empty bank, one that dropped images, an image without a valid label, a
+    non-finite objective) leaves ``.scaling`` as it was, and ``.read()`` raises.  One rank's bank.  The arguments after
+    ``kind`` are keyword-only."""
+    if not isinstance(bank, LogitBank):
+        raise TypeError(f"fit_scaling: expected a LogitBank, got {type(bank).__name__}")
+    k = _check_kind(kind, "fit_scaling", bank.num_classes)
+    if int(iters) != iters or int(iters) < 0:
+        raise ValueError(f"fit_scaling: iters must be an integer >= 0 (got {iters})")
+    lr, l2_offdiag, l2_bias = float(lr), float(l2_offdiag), float(l2_bias)
+    if not (math.isfinite(lr) and lr >= 0.0):
+        raise ValueError(f"fit_scaling: lr must be finite and >= 0 (got {lr})")
+    if not (math.isfinite(l2_bias) and l2_bias >= 0.0):
+        raise ValueError(f"fit_scaling: l2_bias must be finite and >= 0 (got {l2_bias})")
+    if not (math.isfinite(l2_offdiag) and l2_offdiag >= 0.0) or (kind == "vector" and l2_offdiag != 0.0):
+        raise ValueError(f"fit_scaling: l2_offdiag must be finite and >= 0, and 0 for vector scaling (got {l2_offdiag})")
+    Fn._require_cuda(bank._cursor, "fit_scaling")
+    if bank.capacity < 1:
+        raise ValueError("fit_scaling: the bank has no capacity")
+    if bank._unlabelled:
+        raise ValueError("fit_scaling: the bank holds images logged without labels (a step with_labels=False)")
+    dev, C, S, iters = bank.device, bank.num_classes, bank.num_ens, int(iters)
+    if out is None:
+        out = LogitScaling(dev, C, kind)
+    elif not isinstance(out, LogitScaling) or out.device != dev or out.num_classes != C or out.kind != kind:
+        raise L.EngineError(f"fit_scaling(out=...): expected a {kind} LogitScaling of {C} classes on {dev}")
+    P = out.params.numel()
+    state = torch.zeros(3, P, dtype=torch.float64, device=dev)          # Adam's double iterate and moments
+    start = state[0, :P - C].view(C, C).diagonal() if kind == "matrix" else state[0, :C]
+    start.fill_(1.0)
+    if init_temperature is not None:
+        T = _temperature_tensor(init_temperature, dev, False, "fit_scaling(init_temperature=...)")
+        start.copy_((1.0 / T.to(torch.float64)).expand_as(start))
+    theta = state[0].to(torch.float32)
+    best = theta.clone()
+    fit = torch.full((3,), float("nan"), dtype=torch.float64, device=dev)
+    lib = L.lib()
+    nbytes = int(lib.bbb_scaling_workspace_bytes(bank.capacity, S, C, k))
+    ws = torch.zeros(nbytes, dtype=torch.uint8, device=dev)
+    steps = scaling_schedule(lr, iters)
+    for t in range(iters + 1):
+        flags = (L.SCALING_FIRST if t == 0 else 0) | (L.SCALING_LAST if t == iters else 0) | \
+            (L.SCALING_UPDATE if t < iters else 0)
+        lr_t = steps[t] if t < iters else 0.0
+        L.check(lib.bbb_scaling_nll_grad(
+            Fn._ptr(bank._logits), Fn._ptr(bank._labels), Fn._ptr(bank._cursor), bank.capacity, S, C, k,
+            flags, Fn._ptr(theta), Fn._ptr(state), Fn._ptr(best), Fn._ptr(fit), None, Fn._ptr(out.params), l2_offdiag,
+            l2_bias, lr_t, 1.0 - 0.9 ** (t + 1), 1.0 - 0.999 ** (t + 1), Fn._ptr(ws), nbytes, Fn._stream(dev)),
+            "bbb_scaling_nll_grad")
+    return ScalingFit(bank, out, fit, iters)
+
+
+def calibrate_scaling(net, cal_loader, num_ens: int, kind: str = "vector", *, init: Optional[str] = None,
+                      iters: int = 300, lr: float = 0.1, l2_offdiag: float = 0.0, l2_bias: float = 0.0,
+                      out: Optional[LogitScaling] = None, **evaluate_kwargs) -> dict:
+    """Vector or matrix scaling over a whole calibration set, as calibrate_temperature: ``evaluate`` over
+    ``cal_loader`` into the LogitBank kept on the net (the one calibrate_temperature keeps), then fit_scaling on it.
+    ``init="temperature"`` fits T first (fit_temperature's defaults) and starts from a = 1 / T or W = I / T.  Returns ``scaling`` (the LogitScaling;
+    ``out`` when given), ``fit`` (ScalingFit.read()), ``evaluate`` (evaluate's figures on the calibration set) and,
+    with ``init="temperature"``, ``temperature_fit`` (TemperatureFit.read()).  The intended use:
+
+        cal = mc.calibrate_scaling(net, cal_loader, num_ens, init="temperature")
+        test = mc.evaluate(net, test_loader, num_ens, train_size, scaling=cal["scaling"])"""
+    _check_kind(kind, "calibrate_scaling", net.num_classes if net is not None else None)
+    if init not in (None, "temperature"):
+        raise ValueError(f"calibrate_scaling: init must be None or 'temperature' (got {init!r})")
+    dev = next(net.parameters()).device
+    kw = dict(evaluate_kwargs)
+    train_size = kw.pop("train_size", 1.0)
+    S, Cc = int(num_ens), int(net.num_classes)
+    bank = _kept_log(net, net.__dict__.setdefault("_temperature_banks", {}), "calibration", cal_loader,
+                     lambda n: LogitBank(dev, n, S, Cc), lambda b: (b.num_ens, b.num_classes) == (S, Cc))
+    m = evaluate(net, cal_loader, num_ens, train_size, logit_bank=bank, **kw)
+    res = {"evaluate": m}
+    T = None
+    if init == "temperature":
+        tf = fit_temperature(bank)
+        res["temperature_fit"] = tf.read()
+        T = tf.temperature
+    fit = fit_scaling(bank, kind, iters=iters, lr=lr, l2_offdiag=l2_offdiag, l2_bias=l2_bias, init_temperature=T,
+                      out=out)
+    res.update(scaling=fit.scaling, fit=fit.read())
+    return res
