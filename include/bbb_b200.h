@@ -520,6 +520,30 @@ int bbb_mc_exchange_metrics(const float* logits, int32_t S_local, int32_t S_tota
                             uint64_t* noise_base, uint64_t noise_inc, float* expected_entropy, float* mutual_info,
                             int32_t batch_shards, double* metrics, void* cuda_stream);
 
+/* Gathers the per-sample logits of a sharded Monte-Carlo step onto every rank, for the sample banks (bbb_mc_prob_log,
+ * bbb_mc_logit_log), which need all S samples of every image; the exchange reduces them to moments.  The ranks are laid
+ * out as in bbb_mc_exchange_sharded: world = Rs x Rb, Rb = batch_shards; rank r is sample group g = r % Rs (global
+ * samples g, g + Rs, ..) and row block k = r / Rs (images [b0, b1)).  logits: [S_local, b1 - b0, C], its samples and
+ * rows only (S_local = the number of samples of group g, which may be 0: then logits may be NULL).  Every rank pushes
+ * its elements into every rank's receive buffer at their global position [sample j][image b][class c], as one 8-byte
+ * {value bits, sequence number} word per float (the exchange's transport: no fence, no flag; a lost peer is a counted
+ * time-out in state, never a hang; BBB_B200_MC_TIMEOUT_MS as for the exchange), then polls its own buffer until all
+ * S * B * C words carry this launch's sequence number and writes out [S, B, C] fp32: on every rank the bits of the
+ * one-rank step's logits of all S samples (NaN, inf and -0.0 included).
+ * peer_buffers: HOST array of `world` device pointers, one receive buffer per rank of bbb_mc_gather_bytes(S, B, C)
+ *   (zero-filled once; [rank] is the local one).
+ * state: local device scratch of bbb_mc_state_bytes(), zero-filled once, of this gather alone (not the exchange's):
+ *   word 0 counts its launches and word 2 its time-outs.  The time-out bounds a launch, not each word: once one wait
+ *   of a launch has given up, the launch takes the words still missing as they are.  Every rank must make the same
+ *   calls.
+ * bbb_mc_gather_bytes returns 0 unless S, B, C > 0.  Bad arguments (NULL out / peer_buffers / state / peer buffer,
+ * rank / world out of range or world > 16, world % batch_shards != 0, batch_shards > B, S_local not group g's sample
+ * count, S_local > 0 with NULL logits): BBB_E_INVALID. */
+size_t bbb_mc_gather_bytes(int32_t S, int32_t B, int32_t C);
+int bbb_mc_logit_gather(const float* logits, int32_t S_local, int32_t S, int32_t B, int32_t C, int32_t rank,
+                        int32_t world, int32_t batch_shards, void* const* peer_buffers, void* state, float* out,
+                        void* cuda_stream);
+
 /* Appends one Monte-Carlo step's per-image scores to a data-set-long log, at a device-resident cursor
  * (out-of-distribution detection and selective prediction over a whole data set: uncertainty_estimation.py:61-102).
  * Inputs are the outputs of one exchange: log_outputs [B, C] (required); entropy, expected_entropy, mutual_info [B]

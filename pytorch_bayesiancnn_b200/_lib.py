@@ -39,6 +39,7 @@ SYMBOLS = (
     "bbb_mc_prob_log", "bbb_joint_entropy_workspace_bytes", "bbb_joint_entropy", "bbb_mc_conformal_log",
     "bbb_mc_route_bytes", "bbb_mc_route", "bbb_mc_logit_log", "bbb_temperature_workspace_bytes", "bbb_temperature_nll",
     "bbb_mc_temper", "bbb_mc_logit_scale", "bbb_scaling_workspace_bytes", "bbb_scaling_nll_grad",
+    "bbb_mc_gather_bytes", "bbb_mc_logit_gather",
 )
 MC_MOMENTS, MC_NORMALIZED, MC_INFO = 1, 2, 4
 MC_CAL_BINS = 15                 # BBB_MC_CAL_BINS: calibration bins of the evaluation accumulator
@@ -163,6 +164,10 @@ def _bind(lib):
     lib.bbb_mc_exchange_sharded.restype = C.c_int
     lib.bbb_mc_exchange_metrics.argtypes = lib.bbb_mc_exchange_sharded.argtypes[:-1] + [vp, vp]
     lib.bbb_mc_exchange_metrics.restype = C.c_int
+    lib.bbb_mc_gather_bytes.argtypes = [i32, i32, i32]
+    lib.bbb_mc_gather_bytes.restype = sz
+    lib.bbb_mc_logit_gather.argtypes = [fp, i32, i32, i32, i32, i32, i32, i32, C.POINTER(C.c_void_p), vp, fp, vp]
+    lib.bbb_mc_logit_gather.restype = C.c_int
     lib.bbb_mc_score_log.argtypes = [fp, fp, fp, fp, fp, vp, i32, i32, fp, vp, C.c_int64, vp, vp]
     lib.bbb_mc_score_log.restype = C.c_int
     lib.bbb_mc_prob_log.argtypes = [fp, i32, i32, i32, i32, fp, vp, C.c_int64, vp, vp]

@@ -14,6 +14,7 @@
 #include "fused_tc.cuh"
 #include "conv_s4_tc.cuh"
 #include "mc_head.cuh"
+#include "mc_gather.cuh"
 #include "score_log.cuh"
 #include "batchbald.cuh"
 #include "conformal.cuh"
@@ -791,6 +792,41 @@ int bbb_mc_exchange(const float* logits, int32_t S_local, int32_t S_total, int32
     return bbb_mc_exchange_info(logits, S_local, S_total, B, C, kl, n_kl, flags, labels, train_size, beta, rank, world,
                                 peer_buffers, state, log_outputs, kl_out, pred, epistemic, aleatoric, entropy, head,
                                 noise_base, noise_inc, nullptr, nullptr, cuda_stream);
+}
+
+size_t bbb_mc_gather_bytes(int32_t S, int32_t B, int32_t C) {
+    if (S <= 0 || B <= 0 || C <= 0) return 0;
+    return 2 * bbb::mcg_words(S, B, C) * sizeof(unsigned long long);
+}
+
+int bbb_mc_logit_gather(const float* logits, int32_t S_local, int32_t S, int32_t B, int32_t C, int32_t rank,
+                        int32_t world, int32_t batch_shards, void* const* peer_buffers, void* state, float* out,
+                        void* cuda_stream) {
+    if (!out || !peer_buffers || !state) return fail(BBB_E_INVALID, "NULL pointer");
+    if (S <= 0 || B <= 0 || C <= 0) return fail(BBB_E_INVALID, "bad S/B/C %d/%d/%d", S, B, C);
+    if (world < 1 || world > bbb::MCX_MAX_RANKS || rank < 0 || rank >= world) return fail(BBB_E_INVALID, "bad rank/world %d/%d", rank, world);
+    if (batch_shards < 1 || world % batch_shards) return fail(BBB_E_INVALID, "world %d is not a multiple of batch_shards %d", world, batch_shards);
+    if (batch_shards > B) return fail(BBB_E_INVALID, "batch_shards %d > B %d: a row block would be empty", batch_shards, B);
+    // row blocks as bbb_mc_exchange_sharded: rank r = sample group r % Rs, row block r / Rs
+    const int Rs = world / batch_shards, g = rank % Rs, blk = rank / Rs, per = B / batch_shards, rem = B % batch_shards;
+    const int own = g < S ? (S - g + Rs - 1) / Rs : 0;
+    if (S_local != own) return fail(BBB_E_INVALID, "S_local %d: sample group %d of %d holds %d of %d samples", S_local, g, Rs, own, S);
+    if (S_local > 0 && !logits) return fail(BBB_E_INVALID, "S_local > 0 but logits is NULL");
+    bbb::McgArgs a;
+    a.logits = logits; a.S_local = S_local; a.S = S; a.B = B; a.C = C;
+    a.groups = Rs; a.group = g; a.row0 = blk * per + (blk < rem ? blk : rem); a.rows = per + (blk < rem ? 1 : 0);
+    a.rank = rank; a.world = world;
+    for (int q = 0; q < bbb::MCX_MAX_RANKS; ++q) a.peer[q] = q < world ? (unsigned char*)peer_buffers[q] : nullptr;
+    for (int q = 0; q < world; ++q) if (!a.peer[q]) return fail(BBB_E_INVALID, "peer buffer %d is NULL", q);
+    a.seq = (unsigned int*)state; a.done = (unsigned int*)state + 1; a.timeouts = (unsigned int*)state + 2;
+    a.timeouts_before = (unsigned int*)state + 3;
+    a.timeout_ns = 10ull * 1000 * 1000 * 1000;       // the exchange's time-out
+    if (const char* e = getenv("BBB_B200_MC_TIMEOUT_MS")) a.timeout_ns = (unsigned long long)atoll(e) * 1000000ull;
+    a.out = out;
+    const unsigned grid = grid_blocks(bbb::mcg_words(S, B, C), bbb::MCG_THREADS * bbb::MCG_BATCH, bbb::MCG_MAX_CTAS);
+    cudaError_t e = bbb::launch_pdl(bbb::mc_logit_gather_kernel, dim3(grid), dim3(bbb::MCG_THREADS), 0,
+                                    (cudaStream_t)cuda_stream, a);
+    return launched(e, "mc_logit_gather launch");
 }
 
 static_assert(BBB_MC_SCORE_PLANES == bbb::SL_PLANES, "score log planes: header and kernel disagree");

@@ -31,14 +31,13 @@
 //   expected_entropy[b]    = (1/S_total) sum_{s over all ranks} H[p_hat_s[b]]      (aleatoric)
 //   mutual_info[b]         = entropy[b] - expected_entropy[b]  in fp32, not clamped: rounding may leave it slightly < 0
 // p_hat_s is the same softmax (or softplus-normalised) row the moments use.
-// Every float travels as ONE 8-byte store {value bits, sequence number} (the "LL" idea of NCCL's low-latency protocol):
-// 8-byte stores are single-copy atomic over NVLink, so the receiver simply polls each word until its tag equals the
-// launch's sequence number -- no fence, no separate flag, no CTA barrier between the push and the finish.  (A fence.sys +
-// st.release.sys flag per CTA instead would put two system-scope fences per step on the critical path.)
-// Tags make the buffer reusable without a reset: launch k of a rank uses slot k & 1; a peer can be at most one launch
-// ahead (it cannot finish launch k+1 before it has OUR launch k+1 words, which we send after we finished reading k).
+// Every float travels as ONE 8-byte store {value bits, sequence number} (the "LL" idea of NCCL's low-latency protocol,
+// ll.cuh): the receiver simply polls each word until its tag equals the launch's sequence number -- no fence, no separate
+// flag, no CTA barrier between the push and the finish.  (A fence.sys + st.release.sys flag per CTA instead would put two
+// system-scope fences per step on the critical path.)  Tags make the buffer reusable without a reset (two slots).
 #pragma once
 #include "common.cuh"
+#include "ll.cuh"
 
 namespace bbb {
 
@@ -99,15 +98,6 @@ __host__ inline size_t mcx_buffer_bytes(int B, int C, int want_moments, int worl
     return MCX_CTRL_BYTES + 2 * (size_t)world * mcx_rank_floats(B, C, want_moments, info) * sizeof(unsigned long long);
 }
 
-__device__ __forceinline__ void st_ll(unsigned long long* p, float v, unsigned int seq) {
-    const unsigned long long w = ((unsigned long long)seq << 32) | (unsigned long long)__float_as_uint(v);
-    asm volatile("st.relaxed.sys.global.u64 [%0], %1;" ::"l"(p), "l"(w) : "memory");
-}
-__device__ __forceinline__ unsigned long long ld_ll(const unsigned long long* p) {
-    unsigned long long v;
-    asm volatile("ld.relaxed.sys.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
-    return v;
-}
 __device__ __forceinline__ float softplus_f(float v) { return v > 20.0f ? v : log1pf(expf(v)); }   // F.softplus(beta=1, threshold=20)
 
 // <= 51 registers: an exchange CTA has to fit beside a GEMM CTA (320 x ~120 registers) and a prep CTA of the next step.
@@ -232,15 +222,7 @@ mc_exchange_kernel(const McxArgs p) {
 
     // a word of the receive buffer, once its tag says it belongs to this launch (never hangs: a lost peer = a counted timeout)
     auto ll_value = [&](unsigned long long v, const unsigned long long* w) -> float {
-        if ((unsigned int)(v >> 32) != seq) {
-            const unsigned long long t0 = globaltimer_ns();
-            unsigned int spins = 0;
-            while ((unsigned int)((v = ld_ll(w)) >> 32) != seq) {
-                __nanosleep(64);          // the SM is shared with the next step's kernels (overlap mode): do not hammer the LSU
-                if ((++spins & 63u) == 0u && globaltimer_ns() - t0 > p.timeout_ns) { atomicAdd(p.timeouts, 1u); break; }
-            }
-        }
-        return __uint_as_float((unsigned int)v);
+        return ll_wait(v, w, seq, p.timeout_ns, p.timeouts);
     };
 
     // ---- (1) local partials of this CTA's images, pushed to every rank's receive buffer ---------------------

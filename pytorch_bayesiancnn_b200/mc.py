@@ -150,6 +150,17 @@ def _dist_info(group):
     return (dist if on else None), (dist.get_world_size(group) if on else 1), (dist.get_rank(group) if on else 0)
 
 
+def _from_rank0(value, group):
+    """Rank 0's ``value`` on every rank of ``group`` (torch.distributed's default group when None); on one rank
+    ``value`` itself."""
+    dist, world, _ = _dist_info(group)
+    if world > 1:
+        box = [value]
+        dist.broadcast_object_list(box, src=dist.get_global_rank(group, 0) if group is not None else 0, group=group)
+        value = box[0]
+    return value
+
+
 class MCForward:
     """``out = MCForward(net, example_x, num_ens, ...)(x, labels=None)`` -- the sharded MC step on the engine.
 
@@ -207,14 +218,17 @@ class MCForward:
         append in call order, in every mode; the warm-up steps the constructor runs do not.
         ``prob_bank``: a ProbBank every step appends its B images' per-sample probability rows to (bbb_mc_prob_log,
         behind the exchange on the same stream, as the score log), in call order, in every mode; the warm-up steps are
-        not logged, and every output keeps its bits.  One rank only: a rank holds only its own samples.
+        not logged, and every output keeps its bits.  On several ranks the bank must have been made with this step's
+        ``group``: every rank then gathers the step's per-sample logits of all S samples and B images (one more kernel
+        per step, bbb_mc_logit_gather, in front of the temper) and fills its bank with the one-rank bank's bits.
         ``conformal``: a ConformalLog every step appends its B images' conformity scores and prediction sets to
         (bbb_mc_conformal_log, behind the exchange on the same stream, as the score log), from log_outputs and, with
         ``with_labels``, the labels; in call order, in every mode and with any sharding (every rank holds all B rows of
         log_outputs); the warm-up steps are not logged, and every output keeps its bits.
         ``logit_bank``: a LogitBank every step appends its B images' raw per-sample logits and labels to (bbb_mc_logit_log,
         in front of the temper and the exchange, on the same stream), in call order, in every mode; the warm-up steps are
-        not logged.  One rank only.
+        not logged.  On several ranks, as ``prob_bank``: made with this step's ``group``, filled from the gathered
+        logits.
         ``temperature``: temper every sample's logits, z <- z / T, before the exchange (bbb_mc_temper, one more kernel per
         step): every output -- log_outputs, pred, the uncertainty and information planes, head, metrics and the logs behind
         the exchange -- is then that of p_bar_T = mean_s softmax(z_s / T).  A float, or a one-element fp32 tensor on the
@@ -264,12 +278,7 @@ class MCForward:
         self.want_uncertainty, self.with_labels = want_uncertainty, with_labels
         self.train_size, self.beta = float(train_size), float(beta)
         # every rank must draw sample j from the same (seed, stream): share rank 0's seed unless one is given
-        if seed is None:
-            box = [Fn.current_seed()]
-            if self.world > 1:
-                self.dist.broadcast_object_list(box, src=self.dist.get_global_rank(group, 0) if group is not None else 0, group=group)
-            seed = box[0]
-        self.seed = int(seed)
+        self.seed = int(seed if seed is not None else _from_rank0(Fn.current_seed(), group))
         B, Cc = self.B, self.C
         f32 = dict(dtype=torch.float32, device=dev)
         self.inputs = list(static_inputs) if static_inputs else [example_x.clone()]
@@ -299,13 +308,22 @@ class MCForward:
             self.out["head"] = torch.empty(4, **f32)
         self.state = torch.zeros(int(lib.bbb_mc_state_bytes()), dtype=torch.uint8, device=dev)
         nbytes = int(lib.bbb_mc_buffer_bytes(B, Cc, self.flags, self.sample_shards))   # one slot per sample group
-        self._imported, self._own = [], None
+        # a sample bank on several ranks: every step gathers the logits of all S samples onto every rank, with a receive
+        # buffer, a state and an [S, B, C] array per buffer parity of its own (None on one rank: nothing is gathered)
+        gather = self.world > 1 and any(isinstance(lg, _SampleBank) for lg in self._logs)
+        self._gather_state = self.gathered_all = None
+        self._imported, self._own = [], []
         if self.world == 1:
             self._buf = torch.zeros(nbytes, dtype=torch.uint8, device=dev)
             ptrs = [self._buf.data_ptr()]
         else:
-            ptrs = self._open_peers(nbytes)
+            ptrs, *gptrs = self._open_peers(nbytes, *([int(lib.bbb_mc_gather_bytes(self.num_ens, B, Cc))] if gather
+                                                       else []))
         self.peers = (C.c_void_p * self.world)(*ptrs)
+        if gather:
+            self._gather_peers = (C.c_void_p * self.world)(*gptrs[0])
+            self._gather_state = torch.zeros(int(lib.bbb_mc_state_bytes()), dtype=torch.uint8, device=dev)
+            self.gathered_all = torch.zeros(nbuf, self.num_ens, B, Cc, **f32)
         self.base = torch.zeros(1, dtype=torch.int64, device=dev)
         # The local samples FOLD into the batch -- one pass of the fused chain over S_local*B rows (what
         # uncertainty_estimation.py:38-41 does by repeating the input), each row drawing from its own sample's Philox
@@ -452,43 +470,54 @@ class MCForward:
         self.prep_replays += 1
 
     # -- peer-mapped receive buffers (CUDA IPC; handles travel over torch.distributed) -----------------------
-    def _open_peers(self, nbytes):
+    def _open_peers(self, *sizes):
+        """One receive buffer of each size in ``sizes`` on every rank, mapped into every peer: per buffer, the list of
+        every rank's pointer (the local one at [rank])."""
         lib = L.lib()
         torch.cuda.synchronize(self.dev)
-        own = C.c_void_p()
         with torch.cuda.device(self.dev):
-            L.check(lib.bbb_comm_alloc(C.c_size_t(nbytes), C.byref(own)), "bbb_comm_alloc")
-            self._own = own.value
-            handle = (C.c_ubyte * 64)()
-            L.check(lib.bbb_comm_export(C.c_void_p(self._own), handle), "bbb_comm_export")
+            mine = []
+            for nbytes in sizes:
+                own = C.c_void_p()
+                L.check(lib.bbb_comm_alloc(C.c_size_t(nbytes), C.byref(own)), "bbb_comm_alloc")
+                self._own.append(own.value)
+                handle = (C.c_ubyte * 64)()
+                L.check(lib.bbb_comm_export(C.c_void_p(own.value), handle), "bbb_comm_export")
+                mine.append(bytes(handle))
             handles = [None] * self.world
-            self.dist.all_gather_object(handles, bytes(handle), group=self.group)
-            ptrs = []
-            for q, h in enumerate(handles):
-                if q == self.rank:
-                    ptrs.append(self._own)
-                    continue
-                peer = C.c_void_p()
-                L.check(lib.bbb_comm_import((C.c_ubyte * 64).from_buffer_copy(h), C.byref(peer)), f"bbb_comm_import (rank {q})")
-                self._imported.append(peer.value)
-                ptrs.append(peer.value)
+            self.dist.all_gather_object(handles, mine, group=self.group)
+            bufs = []
+            for i, own in enumerate(self._own):
+                ptrs = []
+                for q, h in enumerate(handles):
+                    if q == self.rank:
+                        ptrs.append(own)
+                        continue
+                    peer = C.c_void_p()
+                    L.check(lib.bbb_comm_import((C.c_ubyte * 64).from_buffer_copy(h[i]), C.byref(peer)),
+                            f"bbb_comm_import (rank {q})")
+                    self._imported.append(peer.value)
+                    ptrs.append(peer.value)
+                bufs.append(ptrs)
         self.dist.barrier(group=self.group)
-        return ptrs
+        return bufs
 
     def timeouts(self) -> int:
-        """Exchange waits that gave up because a peer never delivered (results of those steps are invalid)."""
-        return int(self.state[8:12].view(torch.int32).item())
+        """Exchange and gather waits that gave up because a peer never delivered (results of those steps are invalid)."""
+        states = [self.state] + ([self._gather_state] if self._gather_state is not None else [])
+        return sum(int(st[8:12].view(torch.int32).item()) for st in states)
 
     def close(self):
-        """Unmap the peers' buffers and free the local one (after every rank is done with them)."""
+        """Unmap the peers' buffers and free the local ones (after every rank is done with them)."""
         lib = L.lib()
-        if self.world > 1 and self._own is not None:
+        if self.world > 1 and self._own:
             torch.cuda.synchronize(self.dev)
             self.dist.barrier(group=self.group)
             for p in self._imported:
                 lib.bbb_comm_unimport(C.c_void_p(p))
-            lib.bbb_comm_free(C.c_void_p(self._own))
-            self._imported, self._own = [], None
+            for p in self._own:
+                lib.bbb_comm_free(C.c_void_p(p))
+            self._imported, self._own = [], []
 
     # -- one step ----------------------------------------------------------------------------------------------
     def _step(self, x, base=None, advance=False):
@@ -568,15 +597,16 @@ class MCForward:
         from .graph import _STRIDE
         o = self.out
         lib = L.lib()
+        if self._gather_state is not None:
+            L.check(lib.bbb_mc_logit_gather(Fn._ptr(self.logits_all[par]) if self.ids else None, len(self.ids),
+                                            self.num_ens, self.B, self.C, self.rank, self.world, self.batch_shards,
+                                            self._gather_peers, Fn._ptr(self._gather_state),
+                                            Fn._ptr(self.gathered_all[par]), Fn._stream(self.dev)), "bbb_mc_logit_gather")
         for lg in self._logs:
             if lg.before_temper:
                 lg._log(self, par)
-        if self.ids and self.scaling is not None:
-            self.scaling._launch(self.logits_all[par], Fn._stream(self.dev))
-        elif self.ids and self.temperature is not None:
-            z = self.logits_all[par]
-            L.check(lib.bbb_mc_temper(Fn._ptr(z), z.numel(), Fn._ptr(self.temperature), Fn._stream(self.dev)),
-                    "bbb_mc_temper")
+        if self.ids:
+            self._map(self.logits_all[par])
         args = (
             Fn._ptr(self.logits_all[par]), len(self.ids), self.num_ens, self.B, self.C, kl_ptr, n_kl, self.flags,
             Fn._ptr(self._labels_of(par)), C.c_float(self.train_size), C.c_float(self.beta), self.rank, self.world, self.peers,
@@ -596,6 +626,27 @@ class MCForward:
     def _labels_of(self, par):
         """The labels of buffer parity ``par``, or None without ``with_labels``."""
         return self.labels_all[par] if self.labels_all is not None else None
+
+    def _map(self, z):
+        """The temperature or the scaling, in place on per-sample logits ``z`` (bbb_mc_temper / bbb_mc_logit_scale on
+        the step's stream); nothing without either."""
+        if self.scaling is not None:
+            self.scaling._launch(z, Fn._stream(self.dev))
+        elif self.temperature is not None:
+            L.check(L.lib().bbb_mc_temper(Fn._ptr(z), z.numel(), Fn._ptr(self.temperature), Fn._stream(self.dev)),
+                    "bbb_mc_temper")
+
+    def _bank_logits(self, par, mapped=False):
+        """The per-sample logits [S, B, C] of buffer parity ``par`` a sample bank logs: on one rank the step's own (the
+        map has run on them once the temper slot is passed), on several the gathered ones, raw -- or, with ``mapped``,
+        after the step's map, applied here.  The map works element by element or row by row, so mapping the gathered
+        logits gives the bits of gathering the mapped ones."""
+        if self._gather_state is None:
+            return self.logits_all[par]
+        z = self.gathered_all[par]
+        if mapped:
+            self._map(z)
+        return z
 
     def _capture(self, warmup: int = 2):
         from .graph import _STRIDE
@@ -1104,11 +1155,12 @@ def evaluate(net, loader, num_ens: int, train_size: float, beta_type=0.1, epoch=
     to start over).  The engines then also compute the uncertainty and information outputs; the returned figures are
     the same bits as without a log.  Engines are kept per log object: reuse a log from epoch to epoch.
     ``prob_bank``: a ProbBank every image's per-sample probability rows are appended to, in loader order, as the score
-    log is (one rank only); the returned figures keep their bits.
+    log is (on several ranks the bank's ``group`` must be ``group``: every rank then holds all of it); the returned figures
+    keep their bits.
     ``conformal``: a ConformalLog every image's conformity score and prediction set are appended to, in loader order,
     as the score log is; the returned figures keep their bits.  Engines are kept per log object.
-    ``logit_bank``: a LogitBank every image's raw per-sample logits and label are appended to, in loader order (one rank
-    only; calibrate_temperature fills one); the returned figures keep their bits.
+    ``logit_bank``: a LogitBank every image's raw per-sample logits and label are appended to, in loader order (as
+    ``prob_bank`` on several ranks; calibrate_temperature fills one); the returned figures keep their bits.
     ``temperature``: MCForward's -- every figure, log and bank behind the exchange is that of the tempered predictive.
     Engines are kept per temperature tensor (a float: per value), and read a value written into the tensor in place.
     ``scaling``: MCForward's, kept and read in place as a temperature tensor is."""
@@ -1552,17 +1604,30 @@ def bank_pads(num_ens: int, num_classes: int):
 
 class _SampleBank(_CursorLog):
     """What ProbBank and LogitBank share: entries of all S samples x C classes of an image, taken from the step's
-    per-sample logits -- so one rank only, which holds only its own samples."""
+    per-sample logits.  A rank of a sharded step holds only its own samples, so a bank binds to a step on several ranks
+    only when it was made with that step's ``group``: the step then gathers every rank's logits onto every rank
+    (bbb_mc_logit_gather), and each rank's bank holds all of them.  The group also carries the bank's collectives
+    (batchbald's seed)."""
+
+    def _init_bank(self, device, capacity, num_ens, num_classes, group):
+        self._init_cursor(device, capacity, type(self).__name__)
+        self.num_ens, self.num_classes, self.group = num_ens, num_classes, group
 
     def _bind(self, step):
         if step.world > 1:
-            raise L.EngineError(f"MCForward: a {self._keyword} needs one rank (the group has {step.world}): a rank "
-                                "holds only its own samples")
+            dist, n, _ = _dist_info(self.group) if self.group is not None else (None, 1, 0)
+            if n == 1:
+                raise L.EngineError(f"MCForward: a {self._keyword} needs one rank (the group has {step.world}): a rank "
+                                    "holds only its own samples")
+            world = dist.group.WORLD if dist is not None else None      # the step's group=None
+            if self.group is not (step.group if step.group is not None else world):
+                raise L.EngineError(f"MCForward: the {self._keyword} was made with another group than the step's: every "
+                                    "step that fills a bank must run over the bank's ranks")
         super()._bind(step)
         self._require(step.num_ens, step.C, "MCForward")
 
     def _empty(self):
-        return type(self)(self.device, 0, self.num_ens, self.num_classes)
+        return type(self)(self.device, 0, self.num_ens, self.num_classes, group=self.group)
 
     def _require(self, num_ens, num_classes, what):
         if (int(num_ens), int(num_classes)) != (self.num_ens, self.num_classes):
@@ -1586,18 +1651,20 @@ class ProbBank(_SampleBank):
     Entry i holds the S rows p_hat_s (the exchange's softmax, or softplus-normalised row with ``normalized``), rounded to
     tf32, in ``bank[i][c][s]`` order with S padded to S_pad and C to C_pad (bank_pads; the padding is zero), and
     ``expected_entropy`` = (1/S) sum_s H[p_hat_s] in float64.  ``capacity`` entries fit; images past them are counted,
-    not written, and ``read()`` refuses a bank that dropped any."""
+    not written, and ``read()`` refuses a bank that dropped any.
+
+    ``group``: the torch.distributed group of the steps that fill it (None: one rank).  Every rank then receives every
+    step's full [S, B, C] logits and holds the whole bank, with the one-rank bank's bits."""
 
     _keyword = "prob_bank"
 
-    def __init__(self, device, capacity: int, num_ens: int, num_classes: int):
+    def __init__(self, device, capacity: int, num_ens: int, num_classes: int, group=None):
         num_ens, num_classes = int(num_ens), int(num_classes)
         if not 1 <= num_ens <= L.BANK_MAX_SAMPLES:
             raise ValueError(f"ProbBank: num_ens must be in [1, {L.BANK_MAX_SAMPLES}] (got {num_ens})")
         if not 2 <= num_classes <= L.BANK_MAX_CLASSES:
             raise ValueError(f"ProbBank: num_classes must be in [2, {L.BANK_MAX_CLASSES}] (got {num_classes})")
-        self._init_cursor(device, capacity, "ProbBank")
-        self.num_ens, self.num_classes = num_ens, num_classes
+        self._init_bank(device, capacity, num_ens, num_classes, group)
         self.S_pad, self.C_pad = bank_pads(num_ens, num_classes)
         # (one entry at least: the kernel takes the bank's pointers even when nothing fits)
         self._probs = torch.zeros(max(1, self.capacity), self.C_pad, self.S_pad, dtype=torch.float32, device=self.device)
@@ -1609,7 +1676,7 @@ class ProbBank(_SampleBank):
                                         Fn._stream(self.device)), "bbb_mc_prob_log")
 
     def _log(self, step, par):
-        self._launch(step.logits_all[par], step.B, bool(step.flags & L.MC_NORMALIZED))
+        self._launch(step._bank_logits(par, mapped=True), step.B, bool(step.flags & L.MC_NORMALIZED))
 
     def append(self, logits, normalized: bool = False):
         """Append the images of per-sample logits [S, B, C] (fp32 contiguous on the bank's device; bbb_mc_prob_log on
@@ -1703,7 +1770,8 @@ def batchbald(bank: ProbBank, k: int, num_configs: int = 10000, seed: Optional[i
     drawn -- the first time from the exact joint, then extended ancestrally, y_a(m) ~ Q_a[m, .] -- with omega = 1/M
     and const = -(1/M) sum_m log P(y_A(m)).  Pt's column m is P(s | y_A = m); the update between rounds runs in float64
     torch ops on the device and the k rounds are enqueued with no host read; ``seed`` seeds the draws (same seed, same
-    bits).
+    bits).  ``seed=None`` draws one; on a bank made with a group of several ranks, rank 0's draw, so that every rank
+    selects the same images.
 
     Returns ``indices`` (int64 [k]) and ``scores`` (float64 [k], a(A) after each pick) on the host, and ``exact`` (per
     round: enumerated?).  ``trace=True`` adds ``trace``: per round a dict of the device tensors ``scores`` (every
@@ -1717,6 +1785,15 @@ def batchbald(bank: ProbBank, k: int, num_configs: int = 10000, seed: Optional[i
     return res
 
 
+def _selection_seed(bank, seed):
+    """The seed of batchbald's draws: ``seed``, or a fresh draw -- rank 0's on a bank made with a group, so that every
+    rank of it selects the same images."""
+    if seed is not None:
+        return int(seed)
+    seed = int(torch.randint(1 << 62, (1,)).item())
+    return int(_from_rank0(seed, bank.group)) if bank.group is not None else seed
+
+
 def _batchbald_rounds(bank, n, k, num_configs, seed, trace):
     """The k rounds of batchbald over the first n entries, enqueued on the current stream with no host read: (picks,
     scores) as device tensors, the plan and the trace."""
@@ -1725,7 +1802,7 @@ def _batchbald_rounds(bank, n, k, num_configs, seed, trace):
     score = _Scorer(bank, n, max(M for M, _ in plan))
     f64 = dict(dtype=torch.float64, device=dev)
     gen = torch.Generator(device=dev)
-    gen.manual_seed(int(seed) if seed is not None else int(torch.randint(1 << 62, (1,)).item()))
+    gen.manual_seed(_selection_seed(bank, seed))
     eh = bank._ee[:n]
     pt, omega, const = torch.full((1, S), 1.0 / S, **f64), torch.ones(1, **f64), torch.zeros((), **f64)
     configs = torch.zeros(1, 0, dtype=torch.int64, device=dev)
@@ -1780,14 +1857,18 @@ def acquire(net, pool_loader, k: int, num_ens: int, method: str = "batchbald", n
     (batches of (x, y); the labels are not used) into a ProbBank sized from the loader, then ``batchbald`` or ``bald``
     selects k pool images.  Returns the selection's dict (``indices`` are positions in loader order) plus
     ``evaluate`` (evaluate's figures).  ``evaluate_kwargs`` go to evaluate (``train_size`` defaults to 1.0); its
-    ``seed`` also seeds the sampled configurations.  The bank is kept on the net, as detect_ood keeps its logs."""
+    ``seed`` also seeds the sampled configurations.  The bank is kept on the net, as detect_ood keeps its logs; it is
+    made with evaluate's ``group``, so on several ranks every rank holds the whole pool's bank and selects the same
+    images (with ``seed=None``, rank 0's draw)."""
     if method not in ("batchbald", "bald"):
         raise ValueError(f"acquire: method must be 'batchbald' or 'bald' (got {method!r})")
     dev = next(net.parameters()).device
     kw = dict(evaluate_kwargs)
     train_size = kw.pop("train_size", 1.0)
-    bank = _kept_log(net, net.__dict__, "_al_bank", pool_loader, lambda n: ProbBank(dev, n, num_ens, net.num_classes),
-                     lambda b: (b.num_ens, b.num_classes) == (int(num_ens), int(net.num_classes)))
+    group = kw.get("group")
+    bank = _kept_log(net, net.__dict__, "_al_bank", pool_loader,
+                     lambda n: ProbBank(dev, n, num_ens, net.num_classes, group=group),
+                     lambda b: (b.num_ens, b.num_classes) == (int(num_ens), int(net.num_classes)) and b.group is group)
     m = evaluate(net, pool_loader, num_ens, train_size, prob_bank=bank, **kw)
     sel = batchbald(bank, k, num_configs, seed=kw.get("seed")) if method == "batchbald" else bald(bank, k)
     sel["evaluate"] = m
@@ -2443,12 +2524,12 @@ class LogitBank(_SampleBank):
     temperature, so a bank filled under any temperature fits the same T -- and its int64 label (-1 for a step without
     labels, which the fit refuses).  Unlike ProbBank (tf32 probabilities, which lose the small ones a temperature > 1
     raises) it keeps the logits themselves.  ``capacity`` entries fit; images past them are counted, not written, and
-    ``read()`` and the fit refuse a bank that dropped any."""
+    ``read()`` and the fit refuse a bank that dropped any.  ``group``: as ProbBank's."""
 
     _keyword = "logit_bank"
     before_temper = True
 
-    def __init__(self, device, capacity: int, num_ens: int, num_classes: int):
+    def __init__(self, device, capacity: int, num_ens: int, num_classes: int, group=None):
         num_ens, num_classes = int(num_ens), int(num_classes)
         if not 1 <= num_ens <= L.LOGIT_BANK_MAX_SAMPLES:
             raise ValueError(f"LogitBank: num_ens must be in [1, {L.LOGIT_BANK_MAX_SAMPLES}] (got {num_ens})")
@@ -2456,8 +2537,7 @@ class LogitBank(_SampleBank):
             raise ValueError(f"LogitBank: num_classes must be in [2, {L.LOGIT_BANK_MAX_CLASSES}] (got {num_classes})")
         if int(capacity) >= 1 << 31:
             raise ValueError(f"LogitBank: capacity must be < 2^31 (got {capacity})")
-        self._init_cursor(device, capacity, "LogitBank")
-        self.num_ens, self.num_classes = num_ens, num_classes
+        self._init_bank(device, capacity, num_ens, num_classes, group)
         # (one entry at least: the kernel takes the bank's pointers even when nothing fits)
         self._logits = torch.zeros(max(1, self.capacity), num_ens, num_classes, dtype=torch.float32, device=self.device)
         self._labels = torch.full((max(1, self.capacity),), -1, dtype=torch.int64, device=self.device)
@@ -2475,7 +2555,7 @@ class LogitBank(_SampleBank):
                                          Fn._ptr(self._cursor), Fn._stream(self.device)), "bbb_mc_logit_log")
 
     def _log(self, step, par):
-        self._launch(step.logits_all[par], step._labels_of(par), step.B)
+        self._launch(step._bank_logits(par), step._labels_of(par), step.B)
 
     def append(self, logits, labels=None):
         """Append the images of per-sample logits [S, B, C] (fp32 contiguous on the bank's device) and their int64 labels
@@ -2627,13 +2707,16 @@ def calibrate_temperature(net, cal_loader, num_ens: int, t_min: float = 0.05, t_
 
     and the same ``temperature=`` to detect_ood, conformal or acquire (through their evaluate keywords), MCForward, or
     ExpertStep / route (one per expert).  ``evaluate_kwargs`` go to evaluate (``train_size`` defaults to 1.0).  The
-    bank is kept on the net, as detect_ood keeps its logs, and reused by the next call."""
+    bank is kept on the net, as detect_ood keeps its logs, and reused by the next call; it is made with evaluate's
+    ``group``, so on several ranks every rank fits the same T on the whole calibration set."""
     dev = next(net.parameters()).device
     kw = dict(evaluate_kwargs)
     train_size = kw.pop("train_size", 1.0)
     S, Cc = int(num_ens), int(net.num_classes)
+    group = kw.get("group")
     bank = _kept_log(net, net.__dict__.setdefault("_temperature_banks", {}), "calibration", cal_loader,
-                     lambda n: LogitBank(dev, n, S, Cc), lambda b: (b.num_ens, b.num_classes) == (S, Cc))
+                     lambda n: LogitBank(dev, n, S, Cc, group=group),
+                     lambda b: (b.num_ens, b.num_classes) == (S, Cc) and b.group is group)
     m = evaluate(net, cal_loader, num_ens, train_size, logit_bank=bank, **kw)
     fit = fit_temperature(bank, t_min, t_max, grid, rounds, out=out, trace=trace)
     return {"temperature": fit.temperature, "fit": fit.read(), "evaluate": m}
@@ -2763,7 +2846,8 @@ def fit_scaling(bank: LogitBank, kind: str = "vector", *, iters: int = 300, lr: 
     Returns a ScalingFit: ``.scaling`` holds the result -- ``out`` when given, written in place, so engines that scale
     with it read the new parameters at their next step; a new LogitScaling otherwise -- and ``.read()`` gives the
     floats.  A fit the device cannot make (an empty bank, one that dropped images, an image without a valid label, a
-    non-finite objective) leaves ``.scaling`` as it was, and ``.read()`` raises.  One rank's bank.  The arguments after
+    non-finite objective) leaves ``.scaling`` as it was, and ``.read()`` raises.  A bank on several ranks (``group``) holds
+    every sample on every rank, so every rank fits the same bits.  The arguments after
     ``kind`` are keyword-only."""
     if not isinstance(bank, LogitBank):
         raise TypeError(f"fit_scaling: expected a LogitBank, got {type(bank).__name__}")
@@ -2831,8 +2915,10 @@ def calibrate_scaling(net, cal_loader, num_ens: int, kind: str = "vector", *, in
     kw = dict(evaluate_kwargs)
     train_size = kw.pop("train_size", 1.0)
     S, Cc = int(num_ens), int(net.num_classes)
+    group = kw.get("group")
     bank = _kept_log(net, net.__dict__.setdefault("_temperature_banks", {}), "calibration", cal_loader,
-                     lambda n: LogitBank(dev, n, S, Cc), lambda b: (b.num_ens, b.num_classes) == (S, Cc))
+                     lambda n: LogitBank(dev, n, S, Cc, group=group),
+                     lambda b: (b.num_ens, b.num_classes) == (S, Cc) and b.group is group)
     m = evaluate(net, cal_loader, num_ens, train_size, logit_bank=bank, **kw)
     res = {"evaluate": m}
     T = None
